@@ -1,16 +1,18 @@
 #!/usr/bin/env python
-"""bench.py — KMeans.fit() Lloyd-loop throughput on B200 (BASELINE.json metric), one process per GPU.
+"""bench.py — KMeans.fit() Lloyd-loop throughput on H100 (BASELINE.json metric), one process per GPU.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W]            # our arm (sm_100a kernels via the C ABI)
+  python bench.py [--gpus N] [--steps K] [--warmup W]            # our arm (sm_90a kernels via the C ABI)
+  python bench.py ... --dump-outputs DIR                         # + the timed loop's final centres as DIR/*.npy
   python bench.py --impl reference [--gpus N] [--steps K] ...    # CPU arm: the oracle port on host cores
 
 A "step" is ONE Lloyd iteration over this rank's resident partition: fused assign+partial-sum pass over X,
 fixed-order partial reduce, NCCL allreduce of the [k*d sums | k counts | cost] buffer (N>1), finalize.
 
-Headline line (every N, so that the driver's 1/2/4/8 series is one workload): BASELINE.json configs[1] PER GPU
+Headline line (every N, so that a 1/2/4/8 series is one workload): BASELINE.json configs[1] PER GPU
 (k=64, n=10M rows/GPU, d=128, float32; weak scaling).  The same run also measures BASELINE configs[2]'s shape
 (k=256, d=256, 12.5M rows/GPU — the 8-GPU config of the north star) and reports it under "cfg3" in the same JSON
-line, with its own roofline (HBM and tf32 tensor bounds) — see DESIGN.md "Measurement".
+line, with its own roofline (HBM and tf32 tensor bounds) — see DESIGN.md "Measurement".  The headline timed region is
+exactly --steps Lloyd iterations (the cfg3 region: --cfg3-steps).
 Prints ONE JSON line (rank 0).
 """
 from __future__ import annotations
@@ -59,9 +61,10 @@ CONFIGS = {
 }
 METRIC = "kmeans_fit_samples_per_sec"
 UNIT = "samples/s"
-# tcgen05 kind::tf32 peak measured with tools/microbench/mma_rate.cu on this pool's B200 (N = 256: 143 cycles per
-# 128 x 256 x 8 MMA per SM = 3666 flop/cycle/SM; x 148 SMs x 1.965 GHz), DESIGN.md 4.1 item 3
-TF32_PEAK_TFLOPS = 3666.0 * 148 * 1.965e9 / 1e12
+# NVIDIA's H100 SXM data sheet (700 W card): dense TF32 and HBM3 bandwidth.  Ceilings for the roofline fractions, not
+# measured rates.
+TF32_PEAK_TFLOPS = 495.0
+HBM_PEAK_GBS = 3350.0
 
 
 def parse_args():
@@ -72,7 +75,8 @@ def parse_args():
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--config", default="cfg2", choices=sorted(CONFIGS))
     ap.add_argument("--n-per-gpu", type=int, default=0, help="override rows per GPU")
-    ap.add_argument("--kernel-path", default="auto", choices=["auto", "generic", "tcgen05"])
+    ap.add_argument("--kernel-path", default="auto", choices=["auto", "generic", "fused", "tcgen05"],
+                    help="tcgen05: the earlier spelling of fused")
     ap.add_argument("--init", default="auto", choices=["auto", "first_k", "near_true", "kmeans||"],
                     help="initial centres of the timed Lloyd loop: the first k rows of rank 0 (cfg2 default), the "
                          "generating centres + 0.25 sigma noise, or the library's own k-means|| initialiser — the "
@@ -84,37 +88,11 @@ def parse_args():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-cfg3", action="store_true", help="skip the cfg3-shape sub-record")
     ap.add_argument("--cfg3-steps", type=int, default=20)
-    ap.add_argument("--long-steps", type=int, default=200, help="second timed loop for the power-capped regime (0 = skip)")
+    ap.add_argument("--long-steps", type=int, default=0, help="optional second timed loop for the power-capped regime")
     ap.add_argument("--cpu-sample-rows", type=int, default=1_000_000)
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the centres the timed Lloyd loop computed (headline and cfg3) as DIR/<name>.npy")
     return ap.parse_args()
-
-
-def measured_peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        try:
-            j = json.load(open(p))
-            return float(j["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-        except Exception:
-            pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
-
-
-def ncu_traffic_per_launch(tag: str, workload_rows: int, d: int):
-    """dram bytes per launch of the fused kernel from the committed ncu summary (profiles/), scaled to this n.
-    NOT measured in this run: the source file is named beside the number."""
-    for name in (f"r02_{tag}_ncu_summary.json", "fused_kernel_ncu_summary.json"):
-        p = os.path.join(ROOT, "profiles", name)
-        if not os.path.exists(p):
-            continue
-        try:
-            j = json.load(open(p))
-            if int(j.get("d", d)) != d:
-                continue
-            return float(j["dram_bytes_per_row"]) * workload_rows, f"profiles/{name} (ncu --set full, scaled by n)"
-        except Exception:
-            continue
-    return None, None
 
 
 class ClockSampler:
@@ -360,26 +338,17 @@ def timed_lloyd(torch, dist, ctx, X, C0, steps, dev, world, local_rank, sample_c
     return float(ms.item()), ctx.stats(), clocks, shift, C
 
 
-def timed_lloyd_median(torch, dist, ctx, X, C0, steps, dev, world, local_rank, repeats=3):
-    """`repeats` back-to-back timed regions of exactly K steps each (every one bracketed by barrier + synchronize, device
-    timed, max over ranks); the MEDIAN region is reported and all of them are listed.  A single region on a shared host
-    occasionally absorbs a multi-millisecond scheduling hiccup of one rank's process (seen at N=2: 1.19 / 1.63 / 1.19)."""
-    runs = [timed_lloyd(torch, dist, ctx, X, C0, steps, dev, world, local_rank) for _ in range(max(1, repeats))]
-    order = sorted(range(len(runs)), key=lambda i: runs[i][0])
-    mid = order[len(order) // 2]
-    return runs[mid], [r[0] / steps for r in runs]
-
-
-def roofline_record(st, n_local, d, k, kernel, peak, peak_src, tag):
-    """Roofline of the dominant kernel from the live per-launch CUDA-event times of the timed loop itself."""
+def roofline_record(st, n_local, d, k, kernel, peak, peak_src, passes=1):
+    """Roofline of the fused pass from the live per-launch CUDA-event times of the timed loop itself.  The events bracket
+    everything b2k_launch_fused enqueues (centre prep, the wgmma pass with its update and, for k or d > 128, the fix-up
+    of the near-tie rows): `passes` = full reads of X inside that span."""
     if st["last_fused_ms"] <= 0:
         return None
-    alg_bytes = 4.0 * n_local * d  # X read once (SURVEY.md 8d); partial flush and row norms are < 1 %
+    alg_bytes = 4.0 * n_local * d * passes  # X read `passes` times (SURVEY.md 8d); partial flush and row norms are < 1 %
     t = st["last_fused_ms"] / 1e3
     hbm = alg_bytes / t / 1e9
     flops = 2.0 * n_local * d * k
     tf = flops / t / 1e12
-    traffic, traffic_src = ncu_traffic_per_launch(tag, n_local, d)
     hbm_frac, tf_frac = hbm / peak, tf / TF32_PEAK_TFLOPS
     bound = "hbm" if hbm_frac >= tf_frac else "tensor"
     return {"bound": bound, "kernel": kernel, "achieved": hbm if bound == "hbm" else tf,
@@ -387,13 +356,13 @@ def roofline_record(st, n_local, d, k, kernel, peak, peak_src, tag):
             "frac": max(hbm_frac, tf_frac),
             "bounds": {"hbm": {"achieved_gbs": hbm, "peak_gbs": peak, "frac": hbm_frac},
                        "tf32": {"achieved_tflops_1x": tf, "peak_tflops": TF32_PEAK_TFLOPS, "frac": tf_frac,
-                                "peak_source": "tools/microbench/mma_rate.cu (tcgen05 kind::tf32, N=256), DESIGN.md 4.1"},
+                                "peak_source": "H100 SXM data sheet, dense TF32 (700 W)"},
                        "rule": "the kernel's floor is max(t_hbm, t_tf32): frac = max of the two fractions"},
-            "traffic": traffic, "traffic_source": traffic_src, "peak_source": peak_src,
+            "peak_source": peak_src,
             "kernel_ms": st["last_fused_ms"], "loop_ms_per_iter": st["last_loop_ms"] / max(1, st["last_n_iter"]),
             "step_breakdown_ms": {"fused_pass(+centre prep)": st["last_fused_ms"], "partial_fold": st["last_reduce_ms"],
                                   "allreduce": st["last_allreduce_ms"], "finalize": st["last_finalize_ms"]},
-            "algorithmic_bytes_per_launch": alg_bytes, "tensor_flops_per_launch": flops,
+            "algorithmic_bytes_per_launch": alg_bytes, "passes_over_x": passes, "tensor_flops_per_launch": flops,
             "recheck_rows_per_iter": st["recheck_rows"] / max(1, st["last_n_iter"]),
             "recheck_candidates_per_iter": st["recheck_candidates"] / max(1, st["last_n_iter"])}
 
@@ -499,10 +468,10 @@ def main():
                      device=local_rank)
     cc.__enter__()
     ctx = cc.handle
-    ctx.set_option("kernel_path", {"auto": 0, "generic": 1, "tcgen05": 2}[args.kernel_path])
+    ctx.set_option("kernel_path", {"auto": 0, "generic": 1, "fused": 2, "tcgen05": 2}[args.kernel_path])
     if args.probe:
         ctx.set_option("probe", args.probe)
-    peak, peak_src = measured_peaks()
+    peak, peak_src = HBM_PEAK_GBS, "H100 SXM data sheet, 3.35 TB/s HBM3 (700 W)"
 
     def pick_init(name, cfg, X, centers_true, kk, dd):
         mode = name if name != "auto" else ("kmeans||" if cfg == "cfg3" else "first_k")
@@ -523,20 +492,23 @@ def main():
     X, centers_true = make_blobs_device(torch, dev, n_local, d, k, rank)
     C0, init_mode = pick_init(args.init, args.config, X, centers_true, k, d)
     ctx.kmeans_lloyd(X, C0.clone(), max(args.warmup, 3), -1.0)          # warm-up
-    (ms, st, clocks, shift, _), rep_ms = timed_lloyd_median(torch, dist, ctx, X, C0, args.steps, dev, world, local_rank)
+    ms, st, clocks, shift, C_out = timed_lloyd(torch, dist, ctx, X, C0, args.steps, dev, world, local_rank)
+    dumps = {"centers": C_out}
     launches = int(st["kernel_launches"])
-    path = {1: "generic", 2: "tcgen05"}.get(st["last_path"], "?")
+    path = {1: "generic", 2: "wgmma"}.get(st["last_path"], "?")
     value = n_total * args.steps / (ms / 1e3)
-    kernel_name = "k_fused_t (1xTF32 + recheck)" if (k > 128 or d > 128) else "k_fused_assign_update (3xTF32)"
-    roofline = roofline_record(st, n_local, d, k, kernel_name, peak, peak_src, args.config)
+    big = k > 128 or d > 128
+    kernel_name = ("centre prep + k_wg_assign (1xTF32 + recheck, clustered update) + fix-up" if big
+                   else "centre prep + k_wg_assign (3xTF32, fused update)")
+    roofline = roofline_record(st, n_local, d, k, kernel_name, peak, peak_src)
     if roofline is None:  # generic path: time one assign+update iteration as a whole
         ach = 4.0 * n_local * d / (ms / args.steps / 1e3) / 1e9
         roofline = {"bound": "hbm", "kernel": "generic assign+update (2 passes over X)", "achieved": ach, "peak": peak,
                     "unit": "GB/s", "frac": ach / peak, "traffic": None, "peak_source": peak_src}
     if args.long_steps and args.long_steps > args.steps:
-        # the power-capped regime: a run long enough to sit at the 1 kW cap (sw_power_cap), same kernel
+        # the power-capped regime: a run long enough to sit at the card's power cap, same kernel
         ms_l, st_l, clocks_l, _, _ = timed_lloyd(torch, dist, ctx, X, C0, args.long_steps, dev, world, local_rank)
-        rl = roofline_record(st_l, n_local, d, k, kernel_name, peak, peak_src, args.config)
+        rl = roofline_record(st_l, n_local, d, k, kernel_name, peak, peak_src)
         roofline["long_run"] = {"steps": args.long_steps, "ms_per_step": ms_l / args.long_steps,
                                 "kernel_ms": rl["kernel_ms"] if rl else None, "frac": rl["frac"] if rl else None,
                                 "clocks": clocks_l}
@@ -670,15 +642,16 @@ def main():
             torch.cuda.synchronize(dev)
             t_init = time.perf_counter() - t_init0
             ctx.kmeans_lloyd(X3, C03.clone(), 3, -1.0)
-            (ms3, st3, clocks3, shift3, _), rep3 = timed_lloyd_median(torch, dist, ctx, X3, C03, args.cfg3_steps, dev, world,
-                                                                      local_rank)
+            ms3, st3, clocks3, shift3, C3_out = timed_lloyd(torch, dist, ctx, X3, C03, args.cfg3_steps, dev, world,
+                                                            local_rank)
+            dumps["cfg3_centers"] = C3_out
             cfg3 = {"value": n3 * world * args.cfg3_steps / (ms3 / 1e3), "unit": UNIT, "n_gpus": world,
                     "steps": args.cfg3_steps, "warmup": 3, "ms_per_step": ms3 / args.cfg3_steps,
-                    "repeat_ms_per_step": rep3,
                     "config": {"workload": f"cfg3 shape: k={k3}, d={d3}, n={n3}/GPU x {world} GPU, float32 blobs resident in HBM",
-                               "k": k3, "d": d3, "n_per_gpu": n3, "kernel_path": {1: "generic", 2: "tcgen05"}.get(st3["last_path"]),
+                               "k": k3, "d": d3, "n_per_gpu": n3, "kernel_path": {1: "generic", 2: "wgmma"}.get(st3["last_path"]),
                                "init": mode3, "init_seconds": t_init},
-                    "roofline": roofline_record(st3, n3, d3, k3, "k_fused_t (1xTF32 + recheck)", peak, peak_src, "cfg3"),
+                    "roofline": roofline_record(st3, n3, d3, k3, "centre prep + k_wg_assign (1xTF32 + recheck, clustered "
+                                                "update) + fix-up", peak, peak_src),
                     "clocks": clocks3, "gpu_launches": int(st3["kernel_launches"]), "final_shift": shift3}
             del X3
             torch.cuda.empty_cache()
@@ -697,17 +670,23 @@ def main():
                                   f"parallel first touch, best of 3: {dt:.2f} s",
                         "other_legs": cpu_sklearn_legs(min(rows, 500_000), d, k, 5)}
 
+    if rank == 0 and args.dump_outputs:
+        # seeded inputs (make_blobs_device, first-k / seeded init): two builds given the same arguments compare output for
+        # output; float32, k x d each (<= 256 KB)
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, t in dumps.items():
+            np.save(os.path.join(args.dump_outputs, name + ".npy"), t.detach().float().cpu().numpy())
+
     if rank == 0:
         line = {
             "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": args.steps,
-            "warmup": max(args.warmup, 3), "ms_per_step": ms / args.steps, "repeat_ms_per_step": rep_ms,
-            "repeats": "3 timed regions of exactly K steps each; the median region is the one reported",
+            "warmup": max(args.warmup, 3), "ms_per_step": ms / args.steps,
             "higher_is_better": True,
             "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
             "config": {"workload": f"{args.config}: KMeans Lloyd iteration, k={k}, n={n_local}/GPU x {world} GPU, d={d}, "
                                    "float32 blobs resident in HBM; fixed 'array' init; tol<0 so every step does full work",
                        "k": k, "d": d, "n_per_gpu": n_local, "n_total": n_total, "kernel_path": path, "init": init_mode,
-                       "l2": f"inputs ({n_local * d * 4 / 1e9:.2f} GB/GPU) are larger than the 126 MB L2: no flush needed",
+                       "l2": f"inputs ({n_local * d * 4 / 1e9:.2f} GB/GPU) are larger than the 50 MB L2: no flush needed",
                        "parallelism": f"dp{world} (rows sharded; one f64 allreduce of k*d+k+1 values per step)",
                        "comm_bootstrap": "CumlContext (NCCL uid from rank 0 over the barrier allGather)" if world > 1 else None},
             "roofline": roofline, "cpu_baseline": cpu_baseline, "e2e": e2e, "e2e_cabi_pinned": e2e_cabi, "ingest": ingest,

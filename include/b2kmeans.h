@@ -1,5 +1,5 @@
 /*
- * b2kmeans.h — C ABI of libb2kmeans.so: the B200-native (sm_100a) KMeans Lloyd-loop backend that
+ * b2kmeans.h — C ABI of libb2kmeans.so: the H100-native (sm_90a) KMeans Lloyd-loop backend that
  * replaces the cuML calls on spark-rapids-ml's distributed KMeans.fit() path.
  *
  * Reference interfaces each entry point stands in for (paths relative to the reference repo
@@ -78,18 +78,18 @@ typedef enum b2k_dtype {
  *   COLUMNS : d separate scalar columns; `values` is a const void* const[d] array of column buffers. */
 typedef enum b2k_layout { B2K_LAYOUT_ROWS = 0, B2K_LAYOUT_COLUMNS = 1 } b2k_layout;
 
-/* Values for the "kernel_path" option. AUTO picks the tcgen05 fused kernel when the shape fits it. */
+/* Values for the "kernel_path" option. AUTO picks the wgmma fused kernel when the shape fits it. */
 typedef enum b2k_kernel_path {
   B2K_PATH_AUTO = 0,
   B2K_PATH_GENERIC = 1, /* SIMT fp32 tiles: any (k, d) */
-  B2K_PATH_TCGEN05 = 2  /* TMA + tcgen05 fused assign+update (3xTF32 for k, d <= 128; 1xTF32 screening + exact
+  B2K_PATH_TCGEN05 = 2  /* TMA + wgmma fused assign (+ deterministic update pass) (3xTF32 for k, d <= 128; 1xTF32 screening + exact
                            recheck for k, d <= 256); fails with UNSUPPORTED otherwise */
 } b2k_kernel_path;
 
 /* Per-fit statistics (b2k_get_stats): what ran, for tests and bench.py's gpu_launches claim. */
 typedef struct b2k_stats {
   int64_t kernel_launches;     /* kernels of this library launched since ctx creation / last reset */
-  int64_t fused_tc_launches;   /* ... of which the tcgen05 fused assign+update kernel */
+  int64_t fused_tc_launches;   /* ... of which the wgmma fused assign kernel */
   int64_t generic_launches;    /* ... of which generic assign/update kernels */
   int64_t nccl_allreduces;     /* collectives issued */
   int32_t last_path;           /* b2k_kernel_path actually used by the last fit/lloyd/assign */
@@ -104,7 +104,7 @@ typedef struct b2k_stats {
                                   whose approximate margin was below the proven error bound and were re-decided
                                   exactly (summed over its passes; 0 unless option "collect_recheck" is 1) */
   int64_t recheck_candidates;  /* ... exact candidate distances evaluated for them */
-  int64_t path_switch_iter;    /* iteration from which the last Lloyd loop left the large-shape tcgen05 kernel for the
+  int64_t path_switch_iter;    /* iteration from which the last Lloyd loop left the large-shape wgmma kernel for the
                                   generic kernels because most rows needed the exact fix-up (option "adaptive_path",
                                   default 1; only with kernel_path = auto); -1 = it did not */
 } b2k_stats;
@@ -119,15 +119,11 @@ int b2k_ctx_destroy(b2k_ctx* ctx);
  * convergence polls, default 4), "grid_limit" (cap on persistent CTAs, 0 = #SMs), "variant_t" (1 = route every shape with k, d <= 256 through the
  * large-shape kernel b2k_fused_t.cu; default 0 = only shapes the 3xTF32 kernel does not cover), "collect_recheck"
  * (1 = lloyd/assign synchronise and fill b2k_stats.recheck_*), "adaptive_path" (see b2k_stats.path_switch_iter), "ingest_threads" (host threads of the pageable -> pinned
- * staging copy of b2k_ingest_append; 0 = default: 4, capped by half of the CPUs the process may use), "pair" (1 = use the
- * CTA-pair tcgen05 cta_group::2 kernel where instantiated, default 1); diagnostic builds only (`make trace` ->
- * libb2kmeans_trace.so, `-DB2K_PROBE=1`): "profile_fused" (0/1; the product build rejects it with
- * B2K_ERR_UNSUPPORTED at the next fused launch), "probe" (timing experiments that skip work). */
+ * staging copy of b2k_ingest_append; 0 = default: 4, capped by half of the CPUs the process may use), "profile_fused" (0/1; this build
+ * records no per-role profile and rejects it with B2K_ERR_UNSUPPORTED at the next fused launch), "probe" (unused). */
 int b2k_ctx_set_option(b2k_ctx* ctx, const char* key, int64_t value);
 int b2k_get_stats(const b2k_ctx* ctx, b2k_stats* out);
-/* Diagnostics (diagnostic build + option "profile_fused"=1): per-CTA, per-warp-role cycle counters of the last fused
- * launch, layout [grid (+4 trace pseudo-CTAs)][warps][8] = {role cycles, 3 blocked-cycle counters, 2 stage timers, 0, 0}.
- * Synchronises the device. */
+/* Diagnostics: per-role cycle counters of the last fused launch.  This build records none and returns B2K_ERR_STATE. */
 int b2k_get_fused_profile(b2k_ctx* ctx, long long* out, int64_t cap, int* grid_out, int* warps_out);
 int b2k_reset_stats(b2k_ctx* ctx);
 /* Diagnostics: one pass of X[n, d] (d % 32 == 0) through an nslot x 16 KB TMA ring whose slots are released

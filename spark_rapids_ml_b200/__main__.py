@@ -8,7 +8,7 @@ import sys
 
 def main(argv=None) -> int:
     ap = argparse.ArgumentParser(prog="python -m spark_rapids_ml_b200",
-                                 description="Run a program with pyspark.ml.clustering.KMeans replaced by the B200 build.")
+                                 description="Run a program with pyspark.ml.clustering.KMeans replaced by this package.")
     ap.add_argument("-m", dest="module", default=None, help="run a module as __main__ (like python -m)")
     ap.add_argument("rest", nargs=argparse.REMAINDER, help="script path (unless -m) followed by its arguments")
     ns = ap.parse_args(argv)

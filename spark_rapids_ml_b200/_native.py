@@ -81,7 +81,7 @@ class Stats(ctypes.Structure):
 
 
 def build(verbose: bool = False) -> str:
-    """Compile libb2kmeans.so for sm_100a with nvcc (cross-compiles without a GPU)."""
+    """Compile libb2kmeans.so for sm_90a with nvcc (cross-compiles without a GPU)."""
     cmd = ["make", "-C", CSRC_DIR, "-j", "8"]
     res = subprocess.run(cmd, capture_output=True, text=True)
     if res.returncode != 0:

@@ -1,6 +1,6 @@
 """KMeans / KMeansModel — the reference's PySpark-ML Estimator/Model surface for the distributed KMeans.fit()
 path (python/src/spark_rapids_ml/clustering.py:84-604), with the cuML calls replaced by libb2kmeans
-(hand-written sm_100a CUDA behind include/b2kmeans.h).
+(hand-written sm_90a CUDA behind include/b2kmeans.h).
 
 Same names, argument meaning and error behaviour as the reference:
   KMeansClass._param_mapping / _param_value_mapping / _get_cuml_params_default      clustering.py:84-141
@@ -107,8 +107,8 @@ class _KMeansCumlParams(_CumlParams, _KMeansParams, HasFeaturesCols):
 
 
 class KMeans(KMeansClass, _CumlEstimator, _KMeansCumlParams):
-    """KMeans on B200: one barrier task per GPU; each iteration is ONE fused pass over the device-resident
-    partition (TMA -> tcgen05 3xTF32 distance tile -> argmin -> per-cluster partial sums) followed by one NCCL
+    """KMeans on H100: one barrier task per GPU; each iteration is ONE fused pass over the device-resident
+    partition (TMA -> wgmma 3xTF32 distance tile -> argmin, then per-cluster partial sums) followed by one NCCL
     allreduce of the [k*d sums | k counts] buffer.  Parameters as in the reference (clustering.py:197-236):
 
     k (default 2), initMode ("k-means||" | "random"), maxIter (20), tol (1e-4), seed, featuresCol (str for an

@@ -13,7 +13,7 @@ Mirrors the reference's contract (python/src/spark_rapids_ml/core.py):
   * _CumlModel(WithColumns)._transform core.py:1797-1941 per-batch predict appended as predictionCol
   * persistence                        core.py:268-355   metadata JSON + model-attribute JSON under path/data
 
-What is re-designed (B200-first): the executor never stacks Python objects or concatenates on the host —
+What is re-designed (GPU-first): the executor never stacks Python objects or concatenates on the host —
 each Arrow batch goes host -> pinned -> HBM once through b2k_ingest_append into a device-resident matrix
 (utils.DeviceRowAppender), and `inputs` handed to the fit function are device tensors.  The internal hook keeps
 the reference's signature: cuml_fit_func(inputs: List[Tuple[X, None, None]], params: Dict) -> Dict[str, list].

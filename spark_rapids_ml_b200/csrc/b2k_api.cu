@@ -51,10 +51,10 @@ extern "C" int b2k_ctx_create(int device, b2k_ctx** out) {
     delete ctx;
     return b2k_fail(nullptr, B2K_ERR_CUDA, std::string("cudaGetDeviceProperties: ") + cudaGetErrorString(e));
   }
-  if (prop.major != 10) {
+  if (prop.major != 9 || prop.minor != 0) {
     delete ctx;
     return b2k_fail(nullptr, B2K_ERR_UNSUPPORTED,
-                    "libb2kmeans is built for sm_100a (B200) only; device is sm_" + std::to_string(prop.major) +
+                    "libb2kmeans is built for sm_90a (H100) only; device is sm_" + std::to_string(prop.major) +
                         std::to_string(prop.minor));
   }
   ctx->sm_count = prop.multiProcessorCount;
@@ -90,7 +90,7 @@ extern "C" int b2k_ctx_set_option(b2k_ctx* ctx, const char* key, int64_t value) 
   std::string k(key);
   if (k == "kernel_path") {
     if (value < B2K_PATH_AUTO || value > B2K_PATH_TCGEN05)
-      return b2k_fail(ctx, B2K_ERR_INVALID, "kernel_path must be 0 (auto), 1 (generic) or 2 (tcgen05)");
+      return b2k_fail(ctx, B2K_ERR_INVALID, "kernel_path must be 0 (auto), 1 (generic) or 2 (fused wgmma)");
     ctx->kernel_path = (int)value;
   } else if (k == "time_kernels") {
     ctx->time_kernels = value < 0 ? 0 : (value > 2 ? 2 : (int)value);
@@ -99,10 +99,11 @@ extern "C" int b2k_ctx_set_option(b2k_ctx* ctx, const char* key, int64_t value) 
     ctx->check_every = (int)value;
   } else if (k == "probe") {
     ctx->probe = (int)value;
-  } else if (k == "pair") {
-    ctx->pair = value ? 1 : 0;
   } else if (k == "adaptive_path") {
     ctx->adaptive_path = value ? 1 : 0;
+  } else if (k == "pair") {
+    // CTA-pair (cta_group::2) kernels do not exist on sm_90a: accepted for compatibility, no effect
+    (void)value;
   } else if (k == "variant_t") {
     ctx->force_variant_t = value ? 1 : 0;
   } else if (k == "ingest_threads") {
@@ -184,7 +185,7 @@ bool want_fused(b2k_ctx* ctx, int64_t n, int d, int k, const float* X, int* stat
   if (ctx->kernel_path == B2K_PATH_GENERIC) return false;
   if (ctx->kernel_path == B2K_PATH_TCGEN05 && !ok) {
     *status = b2k_fail(ctx, B2K_ERR_UNSUPPORTED,
-                       "kernel_path=tcgen05 requested but shape (n=" + std::to_string(n) + ", d=" +
+                       "kernel_path=2 (fused) requested but shape (n=" + std::to_string(n) + ", d=" +
                            std::to_string(d) + ", k=" + std::to_string(k) +
                            ") is outside the fused kernel's instantiations");
     return false;
@@ -376,7 +377,6 @@ static int lloyd_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, int k, flo
       cudaEvent_t* e = ctx->time_kernels ? &ev[(size_t)launched * nev_per_it] : nullptr;
       if (fused_now) {
         if (e) B2K_CUDA_OK(ctx, cudaEventRecord(e[0], s));
-        // cluster sizes of the previous iteration (R = [k*d sums | k counts | cost]) drive the update-warp balancing
         B2K_TRY(b2k_launch_fused(ctx, B.plan, B.plan_scratch, X, n, d, C, k, nullptr, nullptr, true, B.st, s,
                                  launched > 0 ? B.R + (size_t)k * d : nullptr));
         if (e) B2K_CUDA_OK(ctx, cudaEventRecord(e[1], s));
@@ -413,8 +413,9 @@ static int lloyd_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, int k, flo
       const B2kLoopState& m = mirror[slot ^ 1];
       done = m.done != 0;
       if (can_switch && fused_now && burst_iters[slot ^ 1] > 0 && n > 0) {
-        // measured on B200 (tools/fix_split.py, k = d = 256): the fix-up costs ~0.14 ns per candidate distance + ~0.85 ns
-        // per deferred row; the generic kernels ~6.4 ns per row more than the fused pass (scaled here by k d)
+        // cost model (k = d = 256): the fix-up costs ~0.14 ns per candidate distance + ~0.85 ns per deferred row; the
+        // generic kernels ~6.4 ns per row more than the fused pass (scaled here by k d).  These constants were fitted on
+        // the earlier B200 kernels and have not been re-measured on H100: the switch point is unvalidated there.
         const double it = (double)burst_iters[slot ^ 1];
         const double rows_per_row = (double)(m.fix_rows_cum - seen_rows) / it / (double)n;
         const double cands_per_row = (double)(m.fix_cands_cum - seen_cands) / it / (double)n;

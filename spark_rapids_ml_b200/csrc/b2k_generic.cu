@@ -1,7 +1,7 @@
 // Generic (any k, d) SIMT kernels of the Lloyd loop: exact-fp32 tiled assign, ownership-based
 // (atomic-free, deterministic) per-cluster partial sums, fixed-order reductions, finalize.
-// These serve every shape the tcgen05 fused kernel (b2k_fused_tc.cu) does not cover, the k-means||
-// initialiser, and KMeansModel.transform for odd shapes.  sm_100a only; no CPU fallback.
+// These serve every shape the wgmma fused kernels (b2k_fused_tc.cu, b2k_fused_t.cu) does not cover, the k-means||
+// initialiser, and KMeansModel.transform for odd shapes.  sm_90a only; no CPU fallback.
 //
 // Semantics restated from the reference's backend (EXTERNAL cuML 25.12, called at
 // spark_rapids_ml/clustering.py:383-415): argmin over ||c||^2 - 2 x.c with lowest index on ties,

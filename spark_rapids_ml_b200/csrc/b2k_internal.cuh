@@ -1,4 +1,4 @@
-// Internal declarations shared by the translation units of libb2kmeans.so (sm_100a only).
+// Internal declarations shared by the translation units of libb2kmeans.so (sm_90a only).
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -42,7 +42,6 @@ struct b2k_ctx {
   int check_every = 4;
   int grid_limit = 0;
   int probe = 0;                 // debug/experiment switch for the fused kernel (0 = normal)
-  int pair = 1;                  // option "pair": use the cta_group::2 instantiation where available (default on)
   int adaptive_path = 1;         // option "adaptive_path": a Lloyd loop on the large-shape kernel falls back to the generic
                                  // kernels for its remaining iterations when most rows need the exact fix-up
   int lloyd_switched = 0;
@@ -146,14 +145,13 @@ int b2k_launch_weighted_update(b2k_ctx* ctx, const float* P, const double* w, co
 int b2k_launch_pairwise_sqdist(b2k_ctx* ctx, const float* P, int M, int d, float* D2, cudaStream_t s);
 
 // ------------------------------------------------------------------------------------------------
-// tcgen05 fused kernel — b2k_fused_tc.cu
+// wgmma fused assign kernel — b2k_fused_tc.cu / b2k_fused_t.cu (b2k_wg.cuh)
 // ------------------------------------------------------------------------------------------------
 struct B2kFusedPlan {
   int KP = 0, DP = 0;        // padded cluster count / dimension of the instantiation, 0 = unsupported
   int grid = 0;              // persistent CTAs
-  int pair = 0;              // 1: CTA-pair (tcgen05 cta_group::2) instantiation, grid is even
   int variant = 0;           // 0: b2k_fused_tc.cu (k <= 128, d <= 128, 3xTF32); 1: b2k_fused_t.cu (k, d <= 256, 1xTF32 + recheck)
-  int P = 0;                 // partial-sum slots the pass writes (variant 0: grid; variant 1: CTA pairs + 1 for the deferred rows)
+  int P = 0;                 // partial-sum slots of the update pass (b2k_update_generic_scratch)
   int Pc = 0;                // cost partials the pass writes (variant 0: grid; variant 1: grid + fix-up CTAs)
   size_t scratch_bytes = 0;  // centre operands/cnorm + partials/counts/cost (+ row norms, variant 1)
 };

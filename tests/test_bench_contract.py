@@ -1,5 +1,5 @@
 """bench.py contract on CPU: the reference arm (oracle C/OpenMP port on host cores) prints ONE JSON line with the keys the
-driver reads; the B200 arm refuses to run without a GPU instead of falling back to the CPU."""
+driver reads; the GPU arm refuses to run without a GPU instead of falling back to the CPU."""
 import json
 import os
 import subprocess

@@ -1,5 +1,5 @@
 """GPU parity tests of the large-shape fused kernel (csrc/b2k_fused_t.cu: k <= 256, d <= 256 — BASELINE cfg3's shape):
-tcgen05 1xTF32 screening + proven-bound exact recheck, through the C ABI, against the fp64 oracle.
+wgmma 1xTF32 screening + proven-bound exact recheck, through the C ABI, against the fp64 oracle.
 
 Parity rule as in test_gpu_parity.py: labels bit-exact except rows whose fp64 margin is below 1e-6;
 centroids within 1e-4 relative.  Shapes the 3xTF32 kernel covers are pushed through this kernel with option
@@ -20,7 +20,7 @@ def ctx():
     from spark_rapids_ml_b200 import _native
 
     c = _native.Context(0)
-    c.set_option("kernel_path", 2)       # tcgen05 or fail: never a silent generic fallback
+    c.set_option("kernel_path", 2)       # fused kernel or fail: never a silent generic fallback
     c.set_option("collect_recheck", 1)
     yield c
     c.close()

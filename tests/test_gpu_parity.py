@@ -286,7 +286,7 @@ def test_errors_are_loud(ctx):
 
 def test_baseline_config_shapes(ctx):
     """BASELINE.json configs[0] (k=8, n=100k, d=32: full size) and configs[2] (k=256, d=256: a 20k-row slice of the
-    per-GPU partition) against the oracle from an injected init; 'auto' path selection: both take a tcgen05 kernel
+    per-GPU partition) against the oracle from an injected init; 'auto' path selection: both take a wgmma kernel
     (cfg1 the 3xTF32 one, cfg3 the large-shape 1xTF32 + recheck one, tests/test_gpu_large.py)."""
     ctx.set_option("kernel_path", 0)
     for (n, d, k, iters, want_path) in [(100_000, 32, 8, 6, 2), (20_000, 256, 256, 3, 2)]:
