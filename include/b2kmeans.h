@@ -119,11 +119,16 @@ int b2k_ctx_destroy(b2k_ctx* ctx);
  * convergence polls, default 4), "grid_limit" (cap on persistent CTAs, 0 = #SMs), "variant_t" (1 = route every shape with k, d <= 256 through the
  * large-shape kernel b2k_fused_t.cu; default 0 = only shapes the 3xTF32 kernel does not cover), "collect_recheck"
  * (1 = lloyd/assign synchronise and fill b2k_stats.recheck_*), "adaptive_path" (see b2k_stats.path_switch_iter), "ingest_threads" (host threads of the pageable -> pinned
- * staging copy of b2k_ingest_append; 0 = default: 4, capped by half of the CPUs the process may use), "profile_fused" (0/1; this build
- * records no per-role profile and rejects it with B2K_ERR_UNSUPPORTED at the next fused launch), "probe" (unused). */
+ * staging copy of b2k_ingest_append; 0 = default: 4, capped by half of the CPUs the process may use), "profile_fused" (0/1; the k, d <= 128
+ * fused kernel runs a separately compiled instantiation that records per-warp phase cycle counters, read back with
+ * b2k_get_fused_profile; the large-shape kernel rejects it with B2K_ERR_UNSUPPORTED), "probe" (unused). */
 int b2k_ctx_set_option(b2k_ctx* ctx, const char* key, int64_t value);
 int b2k_get_stats(const b2k_ctx* ctx, b2k_stats* out);
-/* Diagnostics: per-role cycle counters of the last fused launch.  This build records none and returns B2K_ERR_STATE. */
+/* Diagnostics: per-warp phase cycle counters of the last fused launch made with option profile_fused (k, d <= 128
+ * kernel): out[grid][warps][8] int64 (cap = capacity of out in elements), *grid_out and *warps_out (= 12) set.
+ * Consumer warps 0-7: X wait, centre wait, hand-off wait, A load + split, MMA issue + drain, epilogue, sort, column
+ * sums; producer warp 8: X slot wait, centre stage wait, issue.  A warp's counters sum to its whole run.
+ * B2K_ERR_STATE when no profiled launch was made. */
 int b2k_get_fused_profile(b2k_ctx* ctx, long long* out, int64_t cap, int* grid_out, int* warps_out);
 int b2k_reset_stats(b2k_ctx* ctx);
 /* Diagnostics: one pass of X[n, d] (d % 32 == 0) through an nslot x 16 KB TMA ring whose slots are released

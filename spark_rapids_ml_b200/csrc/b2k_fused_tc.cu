@@ -194,8 +194,6 @@ int b2k_launch_fused(b2k_ctx* ctx, const B2kFusedPlan& plan, void* plan_scratch,
   if (plan.variant == 1)
     return b2k_launch_fused_t(ctx, plan, plan_scratch, X, n, d, C, k, labels_out, mindist_out, do_update,
                               !do_update && (mindist_out != nullptr || ctx->want_cost), st, s, prev_counts);
-  if (ctx->profile_fused)
-    return b2k_fail(ctx, B2K_ERR_UNSUPPORTED, "profile_fused: this build records no per-role profile");
   PlanLayout L = plan_layout(plan, n, k, d);
   char* b = static_cast<char*>(plan_scratch);
   float* Chi = reinterpret_cast<float*>(b + L.off_chi);
@@ -226,6 +224,13 @@ int b2k_launch_fused(b2k_ctx* ctx, const B2kFusedPlan& plan, void* plan_scratch,
   a.partials = reinterpret_cast<float*>(b + L.off_partials);
   a.counts = reinterpret_cast<int32_t*>(b + L.off_counts);
   a.st = st;
+  if (ctx->profile_fused) {
+    const size_t pbytes = (size_t)plan.grid * (WG_NTHREADS / 32) * WG_NPROF * sizeof(long long);
+    if (ctx->prof_dev == nullptr) B2K_CUDA_OK(ctx, cudaMalloc(&ctx->prof_dev, (size_t)ctx->sm_count * (WG_NTHREADS / 32) * WG_NPROF * sizeof(long long)));
+    B2K_CUDA_OK(ctx, cudaMemsetAsync(ctx->prof_dev, 0, pbytes, s));
+    ctx->prof_grid = plan.grid;
+    a.prof = ctx->prof_dev;
+  }
   // a Lloyd pass computes labels + sums (its callers pass no min distance); the other passes compute labels + cost
   if (do_update && mindist_out != nullptr)
     return b2k_fail(ctx, B2K_ERR_INVALID, "fused kernel: a Lloyd pass does not produce min distances");
@@ -254,13 +259,19 @@ int b2k_launch_fused(b2k_ctx* ctx, const B2kFusedPlan& plan, void* plan_scratch,
   return B2K_OK;
 }
 
-// diagnostics: per-role blocked-cycle counters of the last fused launch (this build records none)
+// diagnostics: per-warp phase cycle counters of the last profiled launch of the k, d <= 128 kernel (option
+// profile_fused): [grid][WG_NTHREADS / 32][WG_NPROF], phases as in b2k_wg.cuh (WG_P_*)
 extern "C" int b2k_get_fused_profile(b2k_ctx* ctx, long long* out, int64_t cap, int* grid_out, int* warps_out) {
-  (void)cap;
-  (void)grid_out;
-  (void)warps_out;
-  if (!ctx || !out) return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_get_fused_profile: NULL argument");
-  return b2k_fail(ctx, B2K_ERR_STATE, "no fused profile recorded");
+  if (!ctx || !out || !grid_out || !warps_out) return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_get_fused_profile: NULL argument");
+  if (ctx->prof_dev == nullptr || ctx->prof_grid == 0) return b2k_fail(ctx, B2K_ERR_STATE, "no fused profile recorded");
+  const int64_t len = (int64_t)ctx->prof_grid * (WG_NTHREADS / 32) * WG_NPROF;
+  if (cap < len) return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_get_fused_profile: output buffer too small");
+  B2K_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  B2K_CUDA_OK(ctx, cudaDeviceSynchronize());
+  B2K_CUDA_OK(ctx, cudaMemcpy(out, ctx->prof_dev, (size_t)len * sizeof(long long), cudaMemcpyDeviceToHost));
+  *grid_out = ctx->prof_grid;
+  *warps_out = WG_NTHREADS / 32;
+  return B2K_OK;
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -59,7 +59,7 @@ struct b2k_ctx {
   void* xnorm_cache = nullptr;            // float2 [xnorm_cache_rows]
   int64_t xnorm_cache_rows = 0;
   int xnorm_cache_valid = 0;
-  long long* prof_dev = nullptr;  // [grid][18 warps][8]
+  long long* prof_dev = nullptr;  // [grid][12 warps][8] phase cycle counters (option profile_fused)
   int prof_grid = 0;
   // comm
   B2kNccl* nccl = nullptr;

@@ -1,9 +1,10 @@
 // Fused assign kernel for sm_90a (H100): wgmma (tf32) distances + argmin, ONE pass over X per launch.  Shared by the two
 // shape families (included inside the anonymous namespace of b2k_fused_tc.cu and b2k_fused_t.cu after b2k_ptx.cuh):
 //
-//   THREE = true  (k <= 128, d <= 128): "3xTF32".  Each consumer warpgroup splits its 64 rows of an X chunk in shared
-//                 memory into x = hi + lo (both round-to-nearest tf32, in split buffers) and accumulates
-//                 lo.Chi^T + hi.Clo^T + hi.Chi^T: fp32-class dot products.  argmin in index order with strict '<'
+//   THREE = true  (k <= 128, d <= 128): "3xTF32".  Each consumer thread loads its wgmma A fragments from the X slot,
+//                 splits them in registers into x = hi + lo (both round-to-nearest tf32) and accumulates
+//                 lo.Chi^T + hi.Clo^T + hi.Chi^T (A from registers): fp32-class dot products.  The centres stay
+//                 resident in shared memory when WgCfg::CRES.  argmin in index order with strict '<'
 //                 (lowest index wins ties) -> labels (+ min distance ||x||^2 + min_j (||c_j||^2 - 2 x.c_j), cost).
 //   THREE = false (k <= 256, d <= 256): 1xTF32 screening + exact recheck (b2k_fused_t.cu "Bound"): dist' of every
 //                 centre is packed with its index into an ordered 32-bit key; rows whose two best keys are closer than
@@ -12,9 +13,9 @@
 //                 label (+ exact min distance sum (x - c)^2 in assign / inertia passes).
 //
 // UPD (THREE only, Lloyd passes): the same pass also forms the per-cluster sums.  The tile's X chunks stay in shared
-// memory until its labels are known (the A operands are copies: the hi / lo split buffers); the 128 rows are then
-// ordered by (label, row), and the thread that owns column c adds each label's run of rows in registers and then into
-// the CTA's shared-memory sums S[KP][DP].  Every sum is formed in a fixed order (deterministic, no atomics); the CTA
+// memory until its sums are formed (the A operands are register copies); the warpgroups take turns: one orders the
+// 128 rows by (label, row), and its thread that owns column c adds each label's run of rows in registers and then into
+// the CTA's shared-memory sums S[KP][DP], while the other goes on to the next tile.  Every sum is formed in a fixed order (deterministic, no atomics); the CTA
 // writes S to its partial slot when it ends.  For k or d > 128 (THREE = false) the sums ([256][256] f32 = 256 KB) do
 // not fit beside a tile in one CTA, so the kernel runs in clusters of WG_CL = 8 CTAs: after each step every CTA sums
 // the centres [32 r, 32 r + 32) over the 8 tiles of the cluster, reading the peers' labels and X rows through
@@ -33,7 +34,16 @@ constexpr int WG_SMEM_LIMIT = 227 * 1024;
 constexpr int WG_MISC = 7680;   // barriers, ||c||^2, ||x||^2, labels, flag counts, cost, row order, cluster row list
 constexpr int WG_M_CNORM = 256, WG_M_XN = 1280, WG_M_LAB = 1792, WG_M_FLAG = 2816, WG_M_COST = 2880, WG_M_SRT = 2944,
               WG_M_LIST = 3584;
-constexpr int WG_CL = 8;        // THREE = false, UPD: CTAs per cluster; CTA r sums centres [r KP / 8, (r + 1) KP / 8)
+// THREE: barriers, ||c||^2 [KP], ||x||^2 [128] (NC) or the row order [128] (UPD) in one area, labels [2][128], cost
+constexpr int WG_MISC3 = 2368;
+constexpr int WG_M3_XN = 768, WG_M3_SRT = 768, WG_M3_LAB = 1280, WG_M3_COST = 2304;
+constexpr int WG_CL = 8;
+// PROF builds: per-warp cycle counters [grid][WG_NTHREADS / 32][WG_NPROF].  Each mark charges the cycles since the
+// previous mark to one phase, so a warp's counters sum to its whole run.  Consumer warps: X wait, centre wait, hand-off
+// wait, A load + split, MMA issue + drain, epilogue, sort, column sums.  Producer warp: X slot wait, centre stage wait,
+// issue (slot 2).
+constexpr int WG_NPROF = 8;
+enum { WG_P_WX, WG_P_WC, WG_P_HAND, WG_P_SPLIT, WG_P_MMA, WG_P_EPI, WG_P_SORT, WG_P_SUMS };        // THREE = false, UPD: CTAs per cluster; CTA r sums centres [r KP / 8, (r + 1) KP / 8)
 
 template <int KP, int NCH, bool THREE, bool UPD>
 struct WgCfg {
@@ -44,22 +54,27 @@ struct WgCfg {
   static constexpr int NB = THREE ? 2 : 1;                  // centre operands per chunk: (hi, lo) or tf32
   static constexpr int CBYTES = KP * WG_CHUNK * 4;          // one centre chunk (multiple of 1 KB)
   static constexpr int CSTAGE = NB * CBYTES;
-  static constexpr int HL_BYTES = THREE ? 2 * WG_XBYTES : 0;            // hi and lo split of one chunk (both warpgroups)
+  static constexpr int MISC = THREE ? WG_MISC3 : WG_MISC;
   static constexpr int SUM_BYTES = UPD ? SROWS * DP * 4 + SROWS * 4 : 0;   // S[SROWS][DP] f32 + counts[SROWS]
-  static constexpr int FIXED = HL_BYTES + SUM_BYTES + WG_MISC;
+  static constexpr int FIXED = SUM_BYTES + MISC;
   static constexpr int XMIN = UPD ? NCH : 2;                            // UPD holds a whole tile until its update
-  // two centre stages when the X ring still holds XMIN slots, else one
-  static constexpr int SC = (WG_SMEM_LIMIT - FIXED - 2 * CSTAGE) / WG_XBYTES >= XMIN ? 2 : 1;
-  static constexpr int SX_RAW = (WG_SMEM_LIMIT - FIXED - SC * CSTAGE) / WG_XBYTES;
+  // THREE: the centres stay resident (all NCH chunks, loaded once per CTA) when the X ring still holds XRES slots: a
+  // Lloyd pass sums tile t while the next tile is multiplied, so it wants two tiles of slots
+  static constexpr int XRES = UPD ? 2 * NCH : 2;
+  static constexpr bool CRES = THREE && (WG_SMEM_LIMIT - FIXED - NCH * CSTAGE) / WG_XBYTES >= XRES;
+  // else a ring of centre stages: two when the X ring still holds XMIN slots, else one
+  static constexpr int SC = CRES ? 1 : (WG_SMEM_LIMIT - FIXED - 2 * CSTAGE) / WG_XBYTES >= XMIN ? 2 : 1;
+  static constexpr int C_BYTES = CRES ? NCH * CSTAGE : SC * CSTAGE;
+  static constexpr int SX_RAW = (WG_SMEM_LIMIT - FIXED - C_BYTES) / WG_XBYTES;
   static constexpr int SX = SX_RAW > 12 ? 12 : SX_RAW;
   static_assert(SX >= XMIN && 2 * (SX + SC) * 8 + 16 <= WG_M_CNORM, "ring");
   static constexpr int OFF_X = 0;
   static constexpr int OFF_C = SX * WG_XBYTES;
-  static constexpr int OFF_HL = OFF_C + SC * CSTAGE;
-  static constexpr int OFF_SUM = OFF_HL + HL_BYTES;
-  static constexpr int OFF_MISC = OFF_SUM + ((SUM_BYTES + 1023) & ~1023);
-  static constexpr int SMEM_BYTES = OFF_MISC + WG_MISC;
+  static constexpr int OFF_SUM = OFF_C + C_BYTES;
+  static constexpr int OFF_MISC = OFF_SUM + (THREE ? (SUM_BYTES + 7) & ~7 : (SUM_BYTES + 1023) & ~1023);
+  static constexpr int SMEM_BYTES = OFF_MISC + MISC;
   static_assert(SMEM_BYTES <= WG_SMEM_LIMIT, "smem");
+  static_assert(!THREE || WG_M_CNORM + KP * 4 <= WG_M3_XN, "misc");
 };
 
 struct WgArgs {
@@ -85,6 +100,7 @@ struct WgArgs {
   int seg_cap;
   int mask_cap;
   unsigned long long* rstat;    // [2] deferred rows (this kernel), candidates evaluated (k_fix_labels_t) or NULL
+  long long* prof;              // PROF: [grid][WG_NTHREADS / 32][WG_NPROF] cycles
 };
 
 // merge two (smallest, second smallest) pairs of disjoint key sets
@@ -94,7 +110,7 @@ __device__ __forceinline__ void wg_merge2(uint32_t& a1, uint32_t& a2, uint32_t b
   a1 = lo;
 }
 
-template <int KP, int NCH, bool THREE, bool NC, bool UPD>
+template <int KP, int NCH, bool THREE, bool NC, bool UPD, bool PROF = false>
 __global__ void __launch_bounds__(WG_NTHREADS, 1)
 k_wg_assign(const __grid_constant__ CUtensorMap mapX, const __grid_constant__ CUtensorMap mapC0,
             const __grid_constant__ CUtensorMap mapC1, const WgArgs args) {
@@ -112,11 +128,11 @@ k_wg_assign(const __grid_constant__ CUtensorMap mapX, const __grid_constant__ CU
   uint8_t* misc = smem_raw + G::OFF_MISC;
   const uint32_t bars = base + G::OFF_MISC;
   float* cnorm_s = reinterpret_cast<float*>(misc + WG_M_CNORM);
-  float* xn_s = reinterpret_cast<float*>(misc + WG_M_XN);         // [128] ||x||^2 (THREE)
-  int32_t* lab_s = reinterpret_cast<int32_t*>(misc + WG_M_LAB);   // [2][128] labels, -1 = deferred / invalid
-  int32_t* flag_s = reinterpret_cast<int32_t*>(misc + WG_M_FLAG); // [2][8] deferred rows per warp
-  double* cost_s = reinterpret_cast<double*>(misc + WG_M_COST);   // [8]
-  uint32_t* srt_s = reinterpret_cast<uint32_t*>(misc + WG_M_SRT); // [128] (label << 16 | row) in (label, row) order
+  float* xn_s = reinterpret_cast<float*>(misc + WG_M3_XN);                             // [128] ||x||^2 (THREE, NC)
+  int32_t* lab_s = reinterpret_cast<int32_t*>(misc + (THREE ? WG_M3_LAB : WG_M_LAB));   // [2][128] labels, -1 = deferred / invalid
+  int32_t* flag_s = reinterpret_cast<int32_t*>(misc + WG_M_FLAG);                      // [2][8] deferred rows per warp
+  double* cost_s = reinterpret_cast<double*>(misc + (THREE ? WG_M3_COST : WG_M_COST)); // [8]
+  uint32_t* srt_s = reinterpret_cast<uint32_t*>(misc + (THREE ? WG_M3_SRT : WG_M_SRT)); // [128] (label << 16 | row) in (label, row) order
   float* sum_s = reinterpret_cast<float*>(smem_raw + G::OFF_SUM); // UPD: [KP][DP] sums, then [KP] counts
   int32_t* cnt_s = reinterpret_cast<int32_t*>(sum_s + G::SROWS * DP);
   uint32_t* list_s = reinterpret_cast<uint32_t*>(misc + WG_M_LIST);  // [8 * 128] cluster rows (centre, CTA, row)
@@ -127,13 +143,31 @@ k_wg_assign(const __grid_constant__ CUtensorMap mapX, const __grid_constant__ CU
   constexpr bool CLU = UPD && !THREE;   // cluster update through distributed shared memory
   const uint32_t ready_bar = bars + 8u * (uint32_t)(2 * G::SX + 2 * G::SC);   // CLU: the cluster's labels of a step
   const uint32_t done_bar = ready_bar + 8u;                                     // CLU: the cluster has read my step
+  // THREE && UPD: labels of the tiles with parity p are written (by the warpgroup that does not sum them)
+  auto labfull = [&](int p) -> uint32_t { return bars + 8u * (uint32_t)(2 * G::SX + 2 * G::SC + p); };
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
+  long long pc[WG_NPROF] = {};
+  long long tp = PROF ? clock64() : 0;
+  auto mark = [&](int ph) {
+    if constexpr (PROF) {
+      const long long t = clock64();
+      pc[ph] += t - tp;
+      tp = t;
+    }
+  };
+  auto prof_store = [&]() {
+    if constexpr (PROF) {
+      long long* o = args.prof + ((size_t)blockIdx.x * (WG_NTHREADS / 32) + warp) * WG_NPROF;
+      for (int i = 0; i < WG_NPROF; ++i) o[i] = pc[i];
+    }
+  };
   if (threadIdx.x == 0) {
     for (int s = 0; s < G::SX; ++s) {
       mbar_init(xfull(s), 1);
-      mbar_init(xempty(s), 8);   // every consumer warp releases the slot
+      // every consumer warp releases the slot; THREE && UPD: the one warp that summed its 32 columns
+      mbar_init(xempty(s), THREE && UPD ? 1 : 8);
     }
     for (int s = 0; s < G::SC; ++s) {
       mbar_init(cfull(s), 1);
@@ -142,6 +176,10 @@ k_wg_assign(const __grid_constant__ CUtensorMap mapX, const __grid_constant__ CU
     if constexpr (CLU) {
       mbar_init(ready_bar, WG_CL);
       mbar_init(done_bar, WG_CL);
+    }
+    if constexpr (THREE && UPD) {
+      mbar_init(labfull(0), 4);   // the 4 warps of the other warpgroup
+      mbar_init(labfull(1), 4);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
@@ -169,22 +207,38 @@ k_wg_assign(const __grid_constant__ CUtensorMap mapX, const __grid_constant__ CU
       tma_prefetch_desc(&mapX);
       tma_prefetch_desc(&mapC0);
       if constexpr (THREE) tma_prefetch_desc(&mapC1);
+      if constexpr (G::CRES) {   // every centre chunk, once
+        mbar_expect_tx(cfull(0), (uint32_t)(NCH * G::CSTAGE));
+        for (int c = 0; c < NCH; ++c) {
+          const uint32_t cst = base + (uint32_t)(G::OFF_C + c * G::CSTAGE);
+          tma_load_2d(cst, &mapC0, cfull(0), c * WG_CHUNK, 0);
+          tma_load_2d(cst + G::CBYTES, &mapC1, cfull(0), c * WG_CHUNK, 0);
+        }
+      }
       for (int it = 0; it < nit; ++it) {
         const int tile = (int)blockIdx.x + it * (int)gridDim.x;
 #pragma unroll 1
         for (int c = 0; c < NCH; ++c) {
           const int q = it * NCH + c;
           const int xs = q % G::SX, cs = q % G::SC;
+          mark(WG_P_HAND);
           mbar_wait_nocall(xempty(xs), (uint32_t)((q / G::SX) & 1) ^ 1u);
+          mark(WG_P_WX);
           mbar_expect_tx(xfull(xs), (uint32_t)WG_XBYTES);
           tma_load_2d(base + (uint32_t)(G::OFF_X + xs * WG_XBYTES), &mapX, xfull(xs), c * WG_CHUNK, tile * WG_TM);
-          mbar_wait_nocall(cempty(cs), (uint32_t)((q / G::SC) & 1) ^ 1u);
-          const uint32_t cst = base + (uint32_t)(G::OFF_C + cs * G::CSTAGE);
-          mbar_expect_tx(cfull(cs), (uint32_t)G::CSTAGE);
-          tma_load_2d(cst, &mapC0, cfull(cs), c * WG_CHUNK, 0);
-          if constexpr (THREE) tma_load_2d(cst + G::CBYTES, &mapC1, cfull(cs), c * WG_CHUNK, 0);
+          if constexpr (!G::CRES) {
+            mark(WG_P_HAND);
+            mbar_wait_nocall(cempty(cs), (uint32_t)((q / G::SC) & 1) ^ 1u);
+            mark(WG_P_WC);
+            const uint32_t cst = base + (uint32_t)(G::OFF_C + cs * G::CSTAGE);
+            mbar_expect_tx(cfull(cs), (uint32_t)G::CSTAGE);
+            tma_load_2d(cst, &mapC0, cfull(cs), c * WG_CHUNK, 0);
+            if constexpr (THREE) tma_load_2d(cst + G::CBYTES, &mapC1, cfull(cs), c * WG_CHUNK, 0);
+          }
         }
       }
+      mark(WG_P_HAND);
+      prof_store();
     }
     __syncwarp();
   } else {
@@ -204,101 +258,105 @@ k_wg_assign(const __grid_constant__ CUtensorMap mapX, const __grid_constant__ CU
       thr2 = args.thr[2];
       thr3 = args.thr[3];
     }
-    const uint32_t hi_s = base + (uint32_t)(G::OFF_HL + g * (WG_XBYTES / 2));
-    const uint32_t lo_s = hi_s + (uint32_t)WG_XBYTES;
-    for (int it = 0; it < nit; ++it) {
-      const int tile = (int)blockIdx.x + it * (int)gridDim.x;
-      float xnp[4] = {0.f, 0.f, 0.f, 0.f};   // THREE && NC: partial ||x||^2 of rows (tw >> 3) + 16 i
-      int prev_q = -1;                         // THREE = false: chunk whose wgmma group may still be in flight
-#pragma unroll 1
-      for (int c = 0; c < NCH; ++c) {
-        const int q = it * NCH + c;
-        const int xsl = q % G::SX, csl = q % G::SC;
-        const uint32_t xs = base + (uint32_t)(G::OFF_X + xsl * WG_XBYTES + g * (WG_XBYTES / 2));   // my 64 rows
-        const uint32_t cs = base + (uint32_t)(G::OFF_C + csl * G::CSTAGE);
-        mbar_wait_nocall(xfull(xsl), (uint32_t)((q / G::SX) & 1));
-        uint32_t a_hi = xs, a_lo = xs;
-        if constexpr (THREE) {
-          // elementwise split (the swizzled layout is preserved): hi = RN_tf32(x), lo = RN_tf32(x - hi); X stays intact
+    if constexpr (THREE) {
+      // A fragments straight from the swizzled X slot: this thread holds rows ar and ar + 8 of the tile (ar = 64 g +
+      // 16 wi + lane / 4, so both rows are lane / 4 modulo 8, which selects the 16-byte unit swizzle) and columns
+      // lane % 4 and lane % 4 + 4 of each k step of 8
+      const uint32_t arow = (uint32_t)(g * 64 + wi * 16 + (lane >> 2)) * 128u + (uint32_t)(lane & 3) * 4u;
+      const uint32_t asw = (uint32_t)(lane >> 2);
+      // one wgmma group in flight across chunks needs two chunks' A fragments (32 registers each) and a second centre
+      // stage; at KP = 128 the accumulators take 64 registers and two chunks' fragments no longer fit
+      constexpr bool PIPE = (G::CRES || G::SC > 1) && KP < 128;
+      if constexpr (G::CRES) {
+        mark(WG_P_EPI);
+        if (nit > 0) mbar_wait_nocall(cfull(0), 0u);
+        mark(WG_P_WC);
+      }
+      for (int it = 0; it < nit; ++it) {
+        const int tile = (int)blockIdx.x + it * (int)gridDim.x;
+        float xnp[4] = {0.f, 0.f, 0.f, 0.f};   // NC: partial ||x||^2 of rows (tw >> 3) + 16 i
 #pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const uint32_t off = (uint32_t)(tw + 128 * i) * 16u;
-            const float4 v = lds128(xs + off);
-            if constexpr (NC) xnp[i] = fmaf(v.w, v.w, fmaf(v.z, v.z, fmaf(v.y, v.y, fmaf(v.x, v.x, xnp[i]))));
-            float4 h, l;
-            h.x = __uint_as_float(rn_tf32_bits(v.x));
-            h.y = __uint_as_float(rn_tf32_bits(v.y));
-            h.z = __uint_as_float(rn_tf32_bits(v.z));
-            h.w = __uint_as_float(rn_tf32_bits(v.w));
-            l.x = __uint_as_float(rn_tf32_bits(v.x - h.x));
-            l.y = __uint_as_float(rn_tf32_bits(v.y - h.y));
-            l.z = __uint_as_float(rn_tf32_bits(v.z - h.z));
-            l.w = __uint_as_float(rn_tf32_bits(v.w - h.w));
-            sts128(hi_s + off, h);
-            sts128(lo_s + off, l);
-          }
-          fence_proxy_async();
-          asm volatile("bar.sync %0, 128;" ::"r"(1 + g) : "memory");
-          if constexpr (!UPD) {
-            __syncwarp();
-            if (lane == 0) mbar_arrive(xempty(xsl));   // the split buffers are the operands: X is no longer read
-          }
-          a_hi = hi_s;
-          a_lo = lo_s;
-        }
-        mbar_wait_nocall(cfull(csl), (uint32_t)((q / G::SC) & 1));
-        wgmma_fence();
+        for (int c = 0; c < NCH; ++c) {
+          const int q = it * NCH + c;
+          const int xsl = q % G::SX, csl = q % G::SC;
+          const uint32_t xs = base + (uint32_t)(G::OFF_X + xsl * WG_XBYTES);
+          const uint32_t cs = base + (uint32_t)(G::OFF_C + (G::CRES ? c : csl) * G::CSTAGE);
+          const uint8_t* xp = smem_raw + G::OFF_X + xsl * WG_XBYTES;
+          mark(WG_P_EPI);
+          mbar_wait_nocall(xfull(xsl), (uint32_t)((q / G::SX) & 1));
+          mark(WG_P_WX);
+          if constexpr (NC) {
 #pragma unroll
-        for (int ks = 0; ks < WG_CHUNK / 8; ++ks) {
-          const uint64_t da = make_kmajor_sw128_desc(a_hi + ks * 32);
-          const uint64_t db = make_kmajor_sw128_desc(cs + ks * 32);
-          const uint32_t sd = (c | ks) != 0 ? 1u : 0u;
-          if constexpr (THREE) {
-            const uint64_t dal = make_kmajor_sw128_desc(a_lo + ks * 32);
-            const uint64_t dbl = make_kmajor_sw128_desc(cs + G::CBYTES + ks * 32);
-            wgmma_tf32<KP>(acc, dal, db, sd);   // small terms first
-            wgmma_tf32<KP>(acc, da, dbl, 1u);
-            wgmma_tf32<KP>(acc, da, db, 1u);
-          } else {
-            wgmma_tf32<KP>(acc, da, db, sd);
-          }
-        }
-        wgmma_commit();
-        // X slots of an updating pass stay until the tile's sums are formed
-        if constexpr (THREE || G::SC == 1) {
-          // the split buffers / the only centre stage are needed by the next chunk: this chunk's group must complete
-          wgmma_wait0();
-          __syncwarp();
-          if (lane == 0) {
-            mbar_arrive(cempty(csl));
-            if constexpr (!THREE && !UPD) mbar_arrive(xempty(xsl));
-          }
-        } else {
-          // one group stays in flight: the previous chunk's operands are released while this one runs
-          wgmma_wait1();
-          if (prev_q >= 0) {
-            __syncwarp();
-            if (lane == 0) {
-              if constexpr (!UPD) mbar_arrive(xempty(prev_q % G::SX));
-              mbar_arrive(cempty(prev_q % G::SC));
+            for (int i = 0; i < 4; ++i) {
+              const float4 v = lds128(xs + (uint32_t)(g * (WG_XBYTES / 2) + (tw + 128 * i) * 16));
+              xnp[i] = fmaf(v.w, v.w, fmaf(v.z, v.z, fmaf(v.y, v.y, fmaf(v.x, v.x, xnp[i]))));
             }
           }
-          prev_q = q;
+          // x = hi + lo, hi = RN_tf32(x), lo = RN_tf32(x - hi), in registers
+          uint32_t ah[WG_CHUNK / 8][4], al[WG_CHUNK / 8][4];
+#pragma unroll
+          for (int ks = 0; ks < WG_CHUNK / 8; ++ks) {
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {   // row ar + 8 (e & 1), column 8 ks + lane % 4 + 4 (e >> 1)
+              const uint32_t unit = (uint32_t)(2 * ks + (e >> 1));
+              const float v = *reinterpret_cast<const float*>(xp + arow + (uint32_t)(e & 1) * 1024u + ((unit ^ asw) << 4));
+              ah[ks][e] = rn_tf32_bits(v);
+              al[ks][e] = rn_tf32_bits(v - __uint_as_float(ah[ks][e]));
+            }
+          }
+#pragma unroll
+          for (int ks = 0; ks < WG_CHUNK / 8; ++ks) {   // every fragment is formed before the wgmma fence
+            reg_fence(ah[ks]);
+            reg_fence(al[ks]);
+          }
+          if constexpr (!UPD) {
+            __syncwarp();
+            if (lane == 0) mbar_arrive(xempty(xsl));   // the operands are in registers: X is no longer read
+          }
+          mark(WG_P_SPLIT);
+          if constexpr (!G::CRES) {
+            mbar_wait_nocall(cfull(csl), (uint32_t)((q / G::SC) & 1));
+            mark(WG_P_WC);
+          }
+          wgmma_fence();
+#pragma unroll
+          for (int ks = 0; ks < WG_CHUNK / 8; ++ks) {
+            const uint64_t db = make_kmajor_sw128_desc(cs + ks * 32);
+            const uint64_t dbl = make_kmajor_sw128_desc(cs + G::CBYTES + ks * 32);
+            wgmma_tf32_rs<KP>(acc, al[ks], db, (c | ks) != 0 ? 1u : 0u);   // small terms first
+            wgmma_tf32_rs<KP>(acc, ah[ks], dbl, 1u);
+            wgmma_tf32_rs<KP>(acc, ah[ks], db, 1u);
+          }
+          wgmma_commit();
+          if constexpr (PIPE) {
+            // one group stays in flight: loading and splitting the next chunk overlaps this chunk's MMAs
+            wgmma_wait1();
+            if constexpr (!G::CRES) {
+              if (c > 0) {
+                __syncwarp();
+                if (lane == 0) mbar_arrive(cempty((q - 1) % G::SC));
+              }
+            }
+          } else {
+            wgmma_wait0();
+            if constexpr (!G::CRES) {
+              __syncwarp();
+              if (lane == 0) mbar_arrive(cempty(csl));
+            }
+          }
+          mark(WG_P_MMA);
         }
-      }
-      if constexpr (!THREE && G::SC > 1) {
         wgmma_wait0();
-        __syncwarp();
-        if (lane == 0) {
-          if constexpr (!UPD) mbar_arrive(xempty(prev_q % G::SX));
-          mbar_arrive(cempty(prev_q % G::SC));
+        if constexpr (PIPE && !G::CRES) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(cempty((it * NCH + NCH - 1) % G::SC));
         }
-      }
-      reg_fence(acc);
+        reg_fence(acc);
+        mark(WG_P_MMA);
 
-      // ---- epilogue: thread holds rows rr0 and rr0 + 8 of the tile, columns 8 a + 2 (lane & 3) + e ----
-      const int rr0 = g * 64 + wi * 16 + (lane >> 2);
-      if constexpr (THREE) {
+        // ---- epilogue: thread holds rows rr0 and rr0 + 8 of the tile, columns 8 a + 2 (lane & 3) + e ----
+        const int rr0 = g * 64 + wi * 16 + (lane >> 2);
+        int32_t* lab = lab_s + (it & 1) * WG_TM;   // UPD: the tile's labels (two tiles may be in use, see below)
         if constexpr (NC) {
 #pragma unroll
           for (int i = 0; i < 4; ++i) {   // the 8 lanes of a row group hold one row's 8 float4 units
@@ -329,7 +387,7 @@ k_wg_assign(const __grid_constant__ CUtensorMap mapX, const __grid_constant__ CU
           }
           const int64_t grow = (int64_t)tile * WG_TM + rr0 + 8 * h;
           if ((lane & 3) == 0) {
-            if constexpr (UPD) lab_s[rr0 + 8 * h] = grow < args.n ? bj[h] : -1;
+            if constexpr (UPD) lab[rr0 + 8 * h] = grow < args.n ? bj[h] : -1;
             if (grow < args.n) {
               if (args.labels_out != nullptr) args.labels_out[grow] = bj[h];
               if constexpr (NC) {
@@ -340,69 +398,137 @@ k_wg_assign(const __grid_constant__ CUtensorMap mapX, const __grid_constant__ CU
             }
           }
         }
+        mark(WG_P_EPI);
         if constexpr (UPD) {
-          // ---- per-cluster sums of the tile, from the X chunks still in shared memory ----
-          asm volatile("bar.sync 3, 256;" ::: "memory");   // labels of all 128 rows
-          if (threadIdx.x < WG_TM) {   // rank of row t in (label, row) order; rows past n sort last
-            const int t = threadIdx.x;
-            const int mine = lab_s[t] < 0 ? KP : lab_s[t];
-            int rank = 0;
+          // ---- per-cluster sums of the tile, from its X chunks still in shared memory.  The warpgroups take turns:
+          // warpgroup u = it & 1 waits for the other one's labels and forms the sums, while the other goes straight on
+          // to the next tile's MMAs.  The sums of tile it + 1 are formed by the other warpgroup after it has the
+          // labels of tile it + 1, which u writes only after this update: the updates (and the row order buffer)
+          // stay in tile order, and labels of at most two tiles are in use. ----
+          const int u = it & 1;
+          if (g != u) {
+            __syncwarp();
+            if (lane == 0) mbar_arrive(labfull(u));   // this warp's labels of the tile are written
+          } else {
+            mbar_wait_nocall(labfull(u), (uint32_t)((it >> 1) & 1));   // the other warpgroup's labels
+            asm volatile("bar.sync %0, 128;" ::"r"(1 + g) : "memory");    // ... and this one's
+            mark(WG_P_HAND);
+            {   // rank of row t in (label, row) order; rows past n sort last
+              const int t = tw;
+              const int mine = lab[t] < 0 ? KP : lab[t];
+              int rank = 0;
 #pragma unroll 8
-            for (int r = 0; r < WG_TM; ++r) {
-              const int o = lab_s[r] < 0 ? KP : lab_s[r];
-              rank += (o < mine || (o == mine && r < t)) ? 1 : 0;
-            }
-            srt_s[rank] = ((uint32_t)(mine < KP ? mine : 0xffff) << 16) | (uint32_t)t;
-          }
-          asm volatile("bar.sync 3, 256;" ::: "memory");   // row order complete
-          if (threadIdx.x < DP) {
-            const int col = threadIdx.x;
-            // column col of row r: X slot of chunk col / 32, 16-B unit (col % 32) / 4 swizzled by r % 8
-            const uint8_t* cbase = smem_raw + G::OFF_X + ((it * NCH + col / WG_CHUNK) % G::SX) * WG_XBYTES + (col % 4) * 4;
-            const uint32_t unit = (uint32_t)((col % WG_CHUNK) / 4);
-            int cur = -1, run = 0;
-            float a = 0.f;
-#pragma unroll 1
-            for (int i0 = 0; i0 < WG_TM; i0 += 8) {   // 8 rows' loads in flight, then the adds in order
-              uint32_t e[8];
-              float x[8];
-#pragma unroll
-              for (int u = 0; u < 8; ++u) e[u] = srt_s[i0 + u];
-#pragma unroll
-              for (int u = 0; u < 8; ++u) {
-                const uint32_t r = e[u] & 0xffffu;
-                x[u] = *reinterpret_cast<const float*>(cbase + r * 128u + ((unit ^ (r & 7u)) << 4));
+              for (int r = 0; r < WG_TM; ++r) {
+                const int o = lab[r] < 0 ? KP : lab[r];
+                rank += (o < mine || (o == mine && r < t)) ? 1 : 0;
               }
+              srt_s[rank] = ((uint32_t)(mine < KP ? mine : 0xffff) << 16) | (uint32_t)t;
+            }
+            mark(WG_P_SORT);
+            asm volatile("bar.sync %0, 128;" ::"r"(1 + g) : "memory");   // row order complete
+            mark(WG_P_HAND);
+            if (tw < DP) {
+              const int col = tw;
+              // column col of row r: X slot of chunk col / 32, 16-B unit (col % 32) / 4 swizzled by r % 8
+              const uint8_t* cbase = smem_raw + G::OFF_X + ((it * NCH + col / WG_CHUNK) % G::SX) * WG_XBYTES + (col % 4) * 4;
+              const uint32_t unit = (uint32_t)((col % WG_CHUNK) / 4);
+              int cur = -1, run = 0;
+              float a = 0.f;
+#pragma unroll 1
+              for (int i0 = 0; i0 < WG_TM; i0 += 8) {   // 8 rows' loads in flight, then the adds in order
+                uint32_t e[8];
+                float x[8];
 #pragma unroll
-              for (int u = 0; u < 8; ++u) {
-                const int l = (int)(e[u] >> 16);
-                if (l == 0xffff) continue;   // rows past n sort last
-                if (l != cur) {
-                  if (cur >= 0) {
-                    sum_s[cur * DP + col] += a;
-                    if (col == 0) cnt_s[cur] += run;
-                  }
-                  cur = l;
-                  a = 0.f;
-                  run = 0;
+                for (int v = 0; v < 8; ++v) e[v] = srt_s[i0 + v];
+#pragma unroll
+                for (int v = 0; v < 8; ++v) {
+                  const uint32_t r = e[v] & 0xffffu;
+                  x[v] = *reinterpret_cast<const float*>(cbase + r * 128u + ((unit ^ (r & 7u)) << 4));
                 }
-                a += x[u];
-                ++run;
+#pragma unroll
+                for (int v = 0; v < 8; ++v) {
+                  const int l = (int)(e[v] >> 16);
+                  if (l == 0xffff) continue;   // rows past n sort last
+                  if (l != cur) {
+                    if (cur >= 0) {
+                      sum_s[cur * DP + col] += a;
+                      if (col == 0) cnt_s[cur] += run;
+                    }
+                    cur = l;
+                    a = 0.f;
+                    run = 0;
+                  }
+                  a += x[v];
+                  ++run;
+                }
+              }
+              if (cur >= 0) {
+                sum_s[cur * DP + col] += a;
+                if (col == 0) cnt_s[cur] += run;
               }
             }
-            if (cur >= 0) {
-              sum_s[cur * DP + col] += a;
-              if (col == 0) cnt_s[cur] += run;
-            }
-          }
-          asm volatile("bar.sync 3, 256;" ::: "memory");   // the tile's X slots and labels are consumed
-          __syncwarp();
-          if (lane == 0) {
-#pragma unroll 1
-            for (int c = 0; c < NCH; ++c) mbar_arrive(xempty((it * NCH + c) % G::SX));
+            __syncwarp();
+            // warp wi summed columns [32 wi, 32 wi + 32): chunk wi of the tile is consumed
+            if (lane == 0 && wi < NCH) mbar_arrive(xempty((it * NCH + wi) % G::SX));
+            mark(WG_P_SUMS);
           }
         }
-      } else {
+      }
+    } else {
+      for (int it = 0; it < nit; ++it) {
+        const int tile = (int)blockIdx.x + it * (int)gridDim.x;
+        int prev_q = -1;                         // chunk whose wgmma group may still be in flight
+#pragma unroll 1
+        for (int c = 0; c < NCH; ++c) {
+          const int q = it * NCH + c;
+          const int xsl = q % G::SX, csl = q % G::SC;
+          const uint32_t xs = base + (uint32_t)(G::OFF_X + xsl * WG_XBYTES + g * (WG_XBYTES / 2));   // my 64 rows
+          const uint32_t cs = base + (uint32_t)(G::OFF_C + csl * G::CSTAGE);
+          mbar_wait_nocall(xfull(xsl), (uint32_t)((q / G::SX) & 1));
+          mbar_wait_nocall(cfull(csl), (uint32_t)((q / G::SC) & 1));
+          wgmma_fence();
+#pragma unroll
+          for (int ks = 0; ks < WG_CHUNK / 8; ++ks) {
+            const uint64_t da = make_kmajor_sw128_desc(xs + ks * 32);
+            const uint64_t db = make_kmajor_sw128_desc(cs + ks * 32);
+            const uint32_t sd = (c | ks) != 0 ? 1u : 0u;
+            wgmma_tf32<KP>(acc, da, db, sd);
+          }
+          wgmma_commit();
+          // X slots of an updating pass stay until the tile's sums are formed
+          if constexpr (G::SC == 1) {
+            // the only centre stage is needed by the next chunk: this chunk's group must complete
+            wgmma_wait0();
+            __syncwarp();
+            if (lane == 0) {
+              mbar_arrive(cempty(csl));
+              if constexpr (!UPD) mbar_arrive(xempty(xsl));
+            }
+          } else {
+            // one group stays in flight: the previous chunk's operands are released while this one runs
+            wgmma_wait1();
+            if (prev_q >= 0) {
+              __syncwarp();
+              if (lane == 0) {
+                if constexpr (!UPD) mbar_arrive(xempty(prev_q % G::SX));
+                mbar_arrive(cempty(prev_q % G::SC));
+              }
+            }
+            prev_q = q;
+          }
+        }
+        if constexpr (G::SC > 1) {
+          wgmma_wait0();
+          __syncwarp();
+          if (lane == 0) {
+            if constexpr (!UPD) mbar_arrive(xempty(prev_q % G::SX));
+            mbar_arrive(cempty(prev_q % G::SC));
+          }
+        }
+        reg_fence(acc);
+
+        // ---- epilogue: thread holds rows rr0 and rr0 + 8 of the tile, columns 8 a + 2 (lane & 3) + e ----
+        const int rr0 = g * 64 + wi * 16 + (lane >> 2);
         // keys: (dist' + ||x||^2 + thr) is a positive float, so its bits order like an unsigned integer; the low 8 bits
         // carry the centre index
         float thr[2], xoff[2];
@@ -604,6 +730,8 @@ k_wg_assign(const __grid_constant__ CUtensorMap mapX, const __grid_constant__ CU
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) cost += __shfl_xor_sync(0xffffffffu, cost, o);
     if (lane == 0) cost_s[warp] = cost;
+    mark(WG_P_EPI);
+    if (lane == 0) prof_store();
     if constexpr (!THREE) {
       if (threadIdx.x == 0) args.fix_count[blockIdx.x] = seg_cnt;
       if (args.rstat != nullptr) {
@@ -636,6 +764,7 @@ k_wg_assign(const __grid_constant__ CUtensorMap mapX, const __grid_constant__ CU
   }
 }
 
+// a.prof != NULL selects the PROF instantiation (THREE only)
 template <int KP, int NCH, bool THREE>
 int b2k_launch_wg(b2k_ctx* ctx, int grid, const CUtensorMap& mx, const CUtensorMap& m0, const CUtensorMap& m1,
                   const WgArgs& a, bool need_cost, bool do_update, cudaStream_t s) {
@@ -647,6 +776,13 @@ int b2k_launch_wg(b2k_ctx* ctx, int grid, const CUtensorMap& mx, const CUtensorM
   } else {
     kern = need_cost ? k_wg_assign<KP, NCH, THREE, true, false> : k_wg_assign<KP, NCH, THREE, false, false>;
     smem = WgCfg<KP, NCH, THREE, false>::SMEM_BYTES;
+  }
+  if constexpr (THREE) {
+    if (a.prof != nullptr) {
+      kern = do_update ? k_wg_assign<KP, NCH, THREE, false, true, true>
+             : need_cost ? k_wg_assign<KP, NCH, THREE, true, false, true>
+                         : k_wg_assign<KP, NCH, THREE, false, false, true>;
+    }
   }
   B2K_CUDA_OK(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   if (!THREE && do_update) {   // the update of the 1xTF32 family runs in clusters of WG_CL CTAs
