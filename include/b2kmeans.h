@@ -82,7 +82,7 @@ typedef enum b2k_layout { B2K_LAYOUT_ROWS = 0, B2K_LAYOUT_COLUMNS = 1 } b2k_layo
 typedef enum b2k_kernel_path {
   B2K_PATH_AUTO = 0,
   B2K_PATH_GENERIC = 1, /* SIMT fp32 tiles: any (k, d) */
-  B2K_PATH_TCGEN05 = 2  /* TMA + wgmma fused assign (+ deterministic update pass) (3xTF32 for k, d <= 128; 1xTF32 screening + exact
+  B2K_PATH_FUSED = 2    /* TMA + wgmma fused assign (+ deterministic update pass) (3xTF32 for k, d <= 128; 1xTF32 screening + exact
                            recheck for k, d <= 256); fails with UNSUPPORTED otherwise */
 } b2k_kernel_path;
 
@@ -114,14 +114,22 @@ const char* b2k_last_error(const b2k_ctx* ctx);
 
 int b2k_ctx_create(int device, b2k_ctx** out);
 int b2k_ctx_destroy(b2k_ctx* ctx);
-/* Options: "kernel_path" (b2k_kernel_path), "time_kernels" (0/1/2: CUDA events around every fused launch; 2 = also
- * around the partial fold, the allreduce and finalize), "check_every" (iterations between host
- * convergence polls, default 4), "grid_limit" (cap on persistent CTAs, 0 = #SMs), "variant_t" (1 = route every shape with k, d <= 256 through the
- * large-shape kernel b2k_fused_t.cu; default 0 = only shapes the 3xTF32 kernel does not cover), "collect_recheck"
- * (1 = lloyd/assign synchronise and fill b2k_stats.recheck_*), "adaptive_path" (see b2k_stats.path_switch_iter), "ingest_threads" (host threads of the pageable -> pinned
- * staging copy of b2k_ingest_append; 0 = default: 4, capped by half of the CPUs the process may use), "profile_fused" (0/1; the k, d <= 128
- * fused kernel runs a separately compiled instantiation that records per-warp phase cycle counters, read back with
- * b2k_get_fused_profile; the large-shape kernel rejects it with B2K_ERR_UNSUPPORTED), "probe" (unused). */
+/* Options:
+ *   "kernel_path"      b2k_kernel_path
+ *   "time_kernels"     0/1/2: CUDA events around every fused launch; 2 = also around the partial fold, the allreduce and
+ *                      finalize
+ *   "check_every"      iterations between host convergence polls, default 4
+ *   "grid_limit"       cap on persistent CTAs, 0 = #SMs
+ *   "variant_t"        1 = route every shape with k, d <= 256 through the large-shape kernel b2k_fused_t.cu; default 0 =
+ *                      only shapes the 3xTF32 kernel does not cover
+ *   "collect_recheck"  1 = lloyd/assign synchronise and fill b2k_stats.recheck_*
+ *   "adaptive_path"    see b2k_stats.path_switch_iter
+ *   "ingest_threads"   host threads of the pageable -> pinned staging copy of b2k_ingest_append; 0 = default: 4, capped
+ *                      by half of the CPUs the process may use
+ *   "profile_fused"    0/1; the k, d <= 128 fused kernel runs a separately compiled instantiation that records per-warp
+ *                      phase cycle counters, read back with b2k_get_fused_profile; the large-shape kernel rejects it
+ *                      with B2K_ERR_UNSUPPORTED
+ *   "probe", "pair"    accepted and ignored (switches of earlier builds) */
 int b2k_ctx_set_option(b2k_ctx* ctx, const char* key, int64_t value);
 int b2k_get_stats(const b2k_ctx* ctx, b2k_stats* out);
 /* Diagnostics: per-warp phase cycle counters of the last fused launch made with option profile_fused (k, d <= 128
@@ -131,9 +139,6 @@ int b2k_get_stats(const b2k_ctx* ctx, b2k_stats* out);
  * B2K_ERR_STATE when no profiled launch was made. */
 int b2k_get_fused_profile(b2k_ctx* ctx, long long* out, int64_t cap, int* grid_out, int* warps_out);
 int b2k_reset_stats(b2k_ctx* ctx);
-/* Diagnostics: one pass of X[n, d] (d % 32 == 0) through an nslot x 16 KB TMA ring whose slots are released
- * `hold_cycles` after landing; *out_ms = device time.  Maps the bandwidth ceiling of the fused kernel's ring. */
-int b2k_debug_tma_stream(b2k_ctx* ctx, const float* X, int64_t n, int d, int nslot, int hold_cycles, float* out_ms);
 
 /* ---- communicator (NCCL over NVLink; one rank per process per GPU) ---- */
 int b2k_comm_unique_id(char out[B2K_UNIQUE_ID_BYTES]); /* rank 0 only */

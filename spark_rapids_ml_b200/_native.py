@@ -14,13 +14,13 @@ from typing import Any, Dict, Optional, Sequence, Tuple
 import numpy as np
 
 _PKG_DIR = os.path.dirname(os.path.abspath(__file__))
-# B2K_LIB selects another build of the same library (e.g. the diagnostic libb2kmeans_trace.so from `make trace`)
+# B2K_LIB loads another build of the same library instead of the in-tree one
 LIB_PATH = os.environ.get("B2K_LIB") or os.path.join(_PKG_DIR, "libb2kmeans.so")
 CSRC_DIR = os.path.join(_PKG_DIR, "csrc")
 
 B2K_OK = 0
 INIT_ARRAY, INIT_RANDOM, INIT_KMEANS_PARALLEL = 0, 1, 2
-PATH_AUTO, PATH_GENERIC, PATH_TCGEN05 = 0, 1, 2
+PATH_AUTO, PATH_GENERIC, PATH_FUSED = 0, 1, 2
 LAYOUT_ROWS, LAYOUT_COLUMNS = 0, 1
 UNIQUE_ID_BYTES = 128
 
@@ -43,7 +43,6 @@ EXPORTED_SYMBOLS = (
     "b2k_get_stats",
     "b2k_get_fused_profile",
     "b2k_reset_stats",
-    "b2k_debug_tma_stream",
     "b2k_comm_unique_id",
     "b2k_comm_init",
     "b2k_comm_destroy",
@@ -115,7 +114,6 @@ def load_library() -> ctypes.CDLL:
     L.b2k_get_stats.argtypes = [vp, ctypes.POINTER(Stats)]
     L.b2k_reset_stats.argtypes = [vp]
     L.b2k_get_fused_profile.argtypes = [vp, vp, i64, ctypes.POINTER(i32), ctypes.POINTER(i32)]
-    L.b2k_debug_tma_stream.argtypes = [vp, vp, i64, i32, i32, i32, ctypes.POINTER(ctypes.c_float)]
     L.b2k_comm_unique_id.argtypes = [ctypes.c_char_p]
     L.b2k_comm_init.argtypes = [vp, i32, i32, ctypes.c_char_p]
     L.b2k_comm_destroy.argtypes = [vp]
@@ -205,13 +203,6 @@ class Context:
         g, w = ctypes.c_int(0), ctypes.c_int(0)
         self._check(self._L.b2k_get_fused_profile(self._h, buf.ctypes.data, buf.size, ctypes.byref(g), ctypes.byref(w)))
         return buf[: g.value * w.value * 8].reshape(g.value, w.value, 8)
-
-    def debug_tma_stream(self, X: Any, nslot: int, hold_cycles: int = 0) -> float:
-        """ms for one TMA pass over X through an nslot x 16 KB ring (diagnostic)."""
-        ms = ctypes.c_float(0.0)
-        self._check(self._L.b2k_debug_tma_stream(self._h, X.data_ptr(), int(X.shape[0]), int(X.shape[1]), int(nslot),
-                                                 int(hold_cycles), ctypes.byref(ms)))
-        return float(ms.value)
 
     def reset_stats(self) -> None:
         self._check(self._L.b2k_reset_stats(self._h))

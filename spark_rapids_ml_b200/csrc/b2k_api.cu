@@ -89,20 +89,18 @@ extern "C" int b2k_ctx_set_option(b2k_ctx* ctx, const char* key, int64_t value) 
   if (!ctx || !key) return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_ctx_set_option: NULL argument");
   std::string k(key);
   if (k == "kernel_path") {
-    if (value < B2K_PATH_AUTO || value > B2K_PATH_TCGEN05)
-      return b2k_fail(ctx, B2K_ERR_INVALID, "kernel_path must be 0 (auto), 1 (generic) or 2 (fused wgmma)");
+    if (value < B2K_PATH_AUTO || value > B2K_PATH_FUSED)
+      return b2k_fail(ctx, B2K_ERR_INVALID, "kernel_path must be 0 (auto), 1 (generic) or 2 (fused)");
     ctx->kernel_path = (int)value;
   } else if (k == "time_kernels") {
     ctx->time_kernels = value < 0 ? 0 : (value > 2 ? 2 : (int)value);
   } else if (k == "check_every") {
     if (value < 1) return b2k_fail(ctx, B2K_ERR_INVALID, "check_every must be >= 1");
     ctx->check_every = (int)value;
-  } else if (k == "probe") {
-    ctx->probe = (int)value;
   } else if (k == "adaptive_path") {
     ctx->adaptive_path = value ? 1 : 0;
-  } else if (k == "pair") {
-    // CTA-pair (cta_group::2) kernels do not exist on sm_90a: accepted for compatibility, no effect
+  } else if (k == "probe" || k == "pair") {
+    // switches of the earlier sm_100a kernels (diagnostic builds, CTA pairs): accepted for compatibility, no effect
     (void)value;
   } else if (k == "variant_t") {
     ctx->force_variant_t = value ? 1 : 0;
@@ -110,8 +108,6 @@ extern "C" int b2k_ctx_set_option(b2k_ctx* ctx, const char* key, int64_t value) 
     if (value < 0 || value > 64) return b2k_fail(ctx, B2K_ERR_INVALID, "ingest_threads must be in [0, 64]");
     b2k_copy_pool_destroy(ctx);
     ctx->ingest_threads = (int)value;
-  } else if (k == "tma_box_rows") {
-    ctx->tma_box_rows = (int)value;
   } else if (k == "collect_recheck") {
     ctx->collect_recheck = value ? 1 : 0;
   } else if (k == "profile_fused") {
@@ -181,9 +177,9 @@ int check_shape(b2k_ctx* ctx, const char* who, const void* X, int64_t n, int d, 
 
 bool want_fused(b2k_ctx* ctx, int64_t n, int d, int k, const float* X, int* status) {
   *status = B2K_OK;
-  bool ok = b2k_fused_supported(ctx, n, d, k, X);
+  bool ok = b2k_fused_supported(n, d, k, X);
   if (ctx->kernel_path == B2K_PATH_GENERIC) return false;
-  if (ctx->kernel_path == B2K_PATH_TCGEN05 && !ok) {
+  if (ctx->kernel_path == B2K_PATH_FUSED && !ok) {
     *status = b2k_fail(ctx, B2K_ERR_UNSUPPORTED,
                        "kernel_path=2 (fused) requested but shape (n=" + std::to_string(n) + ", d=" +
                            std::to_string(d) + ", k=" + std::to_string(k) +
@@ -191,6 +187,19 @@ bool want_fused(b2k_ctx* ctx, int64_t n, int d, int k, const float* X, int* stat
     return false;
   }
   return ok;
+}
+
+// stats.recheck_*: the rows the large-shape kernel re-decided exactly since b2k_fused_prepare and the candidate distances
+// it evaluated for them (zero for the 3xTF32 kernel, which defers none).  Synchronises the stream.
+int fill_recheck_stats(b2k_ctx* ctx, const B2kFusedPlan& plan, void* plan_scratch, cudaStream_t s) {
+  unsigned long long rs[2] = {0ull, 0ull};
+  if (const unsigned long long* dev = plan.rstat(plan_scratch)) {
+    B2K_CUDA_OK(ctx, cudaMemcpyAsync(rs, dev, sizeof(rs), cudaMemcpyDeviceToHost, s));
+    B2K_CUDA_OK(ctx, cudaStreamSynchronize(s));
+  }
+  ctx->stats.recheck_rows = (int64_t)rs[0];
+  ctx->stats.recheck_candidates = (int64_t)rs[1];
+  return B2K_OK;
 }
 
 // Scratch footprint of one assign/lloyd call.
@@ -236,7 +245,7 @@ int chunked_assign_ch(const b2k_ctx* ctx, int64_t n, int d, int k, const float* 
   if (ctx->kernel_path == B2K_PATH_GENERIC || n <= 0 || d > 256) return 0;
   const int ch = (d <= 128 && !ctx->force_variant_t) ? 128 : 256;
   const bool want = k > 256 || (ch == 128 && k > 128 && ctx->near_tie_hint);
-  if (!want || !b2k_fused_supported(ctx, n, d, ch, X)) return 0;
+  if (!want || !b2k_fused_supported(n, d, ch, X)) return 0;
   return ch;
 }
 size_t chunked_assign_bytes(b2k_ctx* ctx, int64_t n, int d, int ch) {
@@ -265,7 +274,7 @@ int chunked_assign_run(b2k_ctx* ctx, const ChunkedAssign& ca, const float* X, in
     const int base = std::min(c0, k - ca.ch);
     const bool first = c0 == 0;
     B2K_TRY(b2k_launch_fused(ctx, ca.plan, ca.ps, X, n, d, C + (size_t)base * d, ca.ch, first ? lab : ca.tmp_lab,
-                             first ? md : ca.tmp_md, false, st, s));
+                             first ? md : ca.tmp_md, false, false, st, s));
     if (!first) B2K_TRY(b2k_launch_merge_chunk(ctx, md, lab, ca.tmp_md, ca.tmp_lab, base, n, st, s));
   }
   return B2K_OK;
@@ -289,7 +298,7 @@ static int lloyd_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, int k, flo
   int st_rc = B2K_OK;
   const bool fused = chunked ? false : want_fused(ctx, n, d, k, X, &st_rc);
   B2K_TRY(st_rc);
-  ctx->stats.last_path = (fused || chunked) ? B2K_PATH_TCGEN05 : B2K_PATH_GENERIC;
+  ctx->stats.last_path = (fused || chunked) ? B2K_PATH_FUSED : B2K_PATH_GENERIC;
 
   LoopBuffers B{};
   size_t gen_bytes = 0;
@@ -377,14 +386,10 @@ static int lloyd_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, int k, flo
       cudaEvent_t* e = ctx->time_kernels ? &ev[(size_t)launched * nev_per_it] : nullptr;
       if (fused_now) {
         if (e) B2K_CUDA_OK(ctx, cudaEventRecord(e[0], s));
-        B2K_TRY(b2k_launch_fused(ctx, B.plan, B.plan_scratch, X, n, d, C, k, nullptr, nullptr, true, B.st, s,
-                                 launched > 0 ? B.R + (size_t)k * d : nullptr));
+        B2K_TRY(b2k_launch_fused(ctx, B.plan, B.plan_scratch, X, n, d, C, k, nullptr, nullptr, true, false, B.st, s));
         if (e) B2K_CUDA_OK(ctx, cudaEventRecord(e[1], s));
-        float* partials;
-        int32_t* counts;
-        double* cost_partials;
-        b2k_fused_views(B.plan, B.plan_scratch, n, k, d, &partials, &counts, &cost_partials);
-        B2K_TRY(b2k_launch_reduce_partials(ctx, partials, counts, cost_partials, B.plan.P, B.plan.Pc, k, d, B.R, B.st, s));
+        B2K_TRY(b2k_launch_reduce_partials(ctx, B.plan.partials(B.plan_scratch), B.plan.counts(B.plan_scratch),
+                                           B.plan.cost_partials(B.plan_scratch), B.plan.P, B.plan.Pc, k, d, B.R, B.st, s));
       } else {
         if (e) B2K_CUDA_OK(ctx, cudaEventRecord(e[0], s));
         if (chunked) {
@@ -471,12 +476,7 @@ static int lloyd_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, int k, flo
   ctx->stats.last_n_iter = ctx->h_state->iter;
   ctx->lloyd_switched = (fused && !fused_now) ? 1 : 0;
   if (ctx->lloyd_switched) ctx->stats.last_path = B2K_PATH_GENERIC;
-  if (fused && ctx->collect_recheck && max_iter > 0) {
-    unsigned long long rs[2];
-    B2K_TRY(b2k_fused_recheck_stats(ctx, B.plan, B.plan_scratch, n, k, d, rs, s));
-    ctx->stats.recheck_rows = (int64_t)rs[0];
-    ctx->stats.recheck_candidates = (int64_t)rs[1];
-  }
+  if (fused && ctx->collect_recheck && max_iter > 0) B2K_TRY(fill_recheck_stats(ctx, B.plan, B.plan_scratch, s));
   if (n_iter_out) *n_iter_out = ctx->h_state->iter;
   if (shift_out) *shift_out = ctx->h_state->shift;
   return B2K_OK;
@@ -512,19 +512,14 @@ static int assign_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, const flo
     B2K_TRY(b2k_fused_prepare(ctx, ca.plan, ca.ps, X, n, d, ch, s));
     B2K_TRY(chunked_assign_run(ctx, ca, X, n, d, C, k, labels, mindist, nullptr, s));
     if (cost_dev) B2K_TRY(b2k_launch_sum_f32_to_f64(ctx, mindist ? mindist : ca.md_acc, n, cost_dev, blocks, nblocks, s));
-    ctx->stats.last_path = B2K_PATH_TCGEN05;
-    if (ctx->collect_recheck) {
-      unsigned long long rs[2];
-      B2K_TRY(b2k_fused_recheck_stats(ctx, ca.plan, ca.ps, n, ch, d, rs, s));
-      ctx->stats.recheck_rows = (int64_t)rs[0];
-      ctx->stats.recheck_candidates = (int64_t)rs[1];
-    }
+    ctx->stats.last_path = B2K_PATH_FUSED;
+    if (ctx->collect_recheck) B2K_TRY(fill_recheck_stats(ctx, ca.plan, ca.ps, s));
     return B2K_OK;
   }
   int st_rc;
   const bool fused = want_fused(ctx, n, d, k, X, &st_rc);
   B2K_TRY(st_rc);
-  ctx->stats.last_path = fused ? B2K_PATH_TCGEN05 : B2K_PATH_GENERIC;
+  ctx->stats.last_path = fused ? B2K_PATH_FUSED : B2K_PATH_GENERIC;
   if (fused) {
     B2kFusedPlan plan;
     B2K_TRY(b2k_fused_plan(ctx, n, d, k, &plan));
@@ -534,22 +529,10 @@ static int assign_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, const flo
     B2K_TRY(b2k_scratch_reserve(ctx, need));
     void* ps = static_cast<char*>(ctx->scratch) + align_up(scratch_off, 1024);
     B2K_TRY(b2k_fused_prepare(ctx, plan, ps, X, n, d, k, s));
-    ctx->want_cost = cost_dev != nullptr ? 1 : 0;
-    B2K_TRY(b2k_launch_fused(ctx, plan, ps, X, n, d, C, k, labels, mindist, false, nullptr, s));
-    if (cost_dev) {
-      float* partials;
-      int32_t* counts;
-      double* cost_partials;
-      b2k_fused_views(plan, ps, n, k, d, &partials, &counts, &cost_partials);
-      // fold the per-CTA cost partials in index order
-      B2K_TRY(b2k_launch_fold_f64(ctx, cost_partials, plan.Pc, cost_dev, s));
-    }
-    if (ctx->collect_recheck) {
-      unsigned long long rs[2];
-      B2K_TRY(b2k_fused_recheck_stats(ctx, plan, ps, n, k, d, rs, s));
-      ctx->stats.recheck_rows = (int64_t)rs[0];
-      ctx->stats.recheck_candidates = (int64_t)rs[1];
-    }
+    B2K_TRY(b2k_launch_fused(ctx, plan, ps, X, n, d, C, k, labels, mindist, false, cost_dev != nullptr, nullptr, s));
+    // fold the per-CTA cost partials in index order
+    if (cost_dev) B2K_TRY(b2k_launch_fold_f64(ctx, plan.cost_partials(ps), plan.Pc, cost_dev, s));
+    if (ctx->collect_recheck) B2K_TRY(fill_recheck_stats(ctx, plan, ps, s));
   } else {
     const int nblocks = 1024;
     size_t need = align_up(scratch_off, 256) + align_up((size_t)k * 4, 256) +
@@ -575,7 +558,7 @@ static int assign_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, const flo
 static size_t assign_scratch_bound(b2k_ctx* ctx, int64_t n, int d, int k, const float* X) {
   size_t b = align_up((size_t)k * 4, 256) + align_up((size_t)(n > 0 ? n : 1) * 4, 256) + 1024 * 8 + 4096;
   if (const int ch = chunked_assign_ch(ctx, n, d, k, X)) b = std::max(b, chunked_assign_bytes(ctx, n, d, ch) + 1024 * 8 + 8192);
-  if (b2k_fused_supported(ctx, n, d, k, X) && ctx->kernel_path != B2K_PATH_GENERIC) {
+  if (b2k_fused_supported(n, d, k, X) && ctx->kernel_path != B2K_PATH_GENERIC) {
     B2kFusedPlan plan;
     if (b2k_fused_plan(ctx, n, d, k, &plan) == B2K_OK) b = std::max(b, align_up(plan.scratch_bytes, 1024) + 4096);
   }

@@ -1,7 +1,10 @@
 // Fused assign for LARGE (k, d) on sm_90a — k <= 256, d <= 256 (BASELINE cfg3: k = 256, d = 256) — 1xTF32 screening
-// + exact recheck, ONE pass over X per launch.  At k = d = 256 the tf32 centres (256 KB) do not fit in shared memory,
-// so every TMA stage carries the X chunk [128 rows x 32 f32] together with the matching centre chunk [256 x 32 f32]
-// (L2-resident); the wgmma kernel is shared with b2k_fused_tc.cu (b2k_wg.cuh, THREE = false):
+// + exact recheck, ONE pass over X per launch: variant 1 of the fused kernel, whose shape rules, plan and dispatch are in
+// b2k_fused.cu.  This file holds its prep, row-norm and fix-up kernels, scratch layout and launch.
+//
+// At k = d = 256 the tf32 centres (256 KB) do not fit in shared memory, so every TMA stage carries the X chunk
+// [128 rows x 32 f32] together with the matching centre chunk [256 x 32 f32] (L2-resident); the wgmma kernel is shared
+// with b2k_fused_tc.cu (b2k_wg.cuh, THREE = false):
 //
 //   * 1xTF32 screening: D = x~.c~ (x~: the fp32 words cut to tf32 by the tensor core, c~ = RN_tf32(c)); the epilogue
 //     packs (dist' + ||x||^2 + thr, centre) into one ordered 32-bit key per centre and finds the smallest AND second
@@ -385,40 +388,20 @@ TLayout t_layout(const B2kFusedPlan& p, int64_t n, int k, int d) {
 }
 }  // namespace
 
-bool b2k_fused_t_supported(const b2k_ctx* ctx, int64_t n, int d, int k, const float* X) {
-  (void)ctx;
-  if (n < 1 || n > (int64_t)0x7fffff00 * 1LL) return false;
-  if (d % 4 != 0 || d > 256 || k > 256) return false;
-  if ((reinterpret_cast<uintptr_t>(X) & 15u) != 0) return false;
-  return true;
-}
-
-int b2k_fused_t_plan(b2k_ctx* ctx, int64_t n, int d, int k, B2kFusedPlan* plan) {
+void b2k_fused_t_plan(const b2k_ctx* ctx, int64_t n, int d, int k, B2kFusedPlan* plan) {
   plan->variant = 1;
   plan->KP = 256;
   plan->DP = d <= 128 ? 128 : 256;
-  const int64_t ntiles = (n + TN - 1) / TN;
   // whole clusters of WG_CL CTAs (the Lloyd pass sums in clusters); CTAs past the last tile run empty steps
-  int grid = ctx->sm_count;
-  if (ctx->grid_limit > 0 && ctx->grid_limit < grid) grid = ctx->grid_limit;
-  if (ntiles < grid) grid = (int)ntiles;
-  grid = grid / WG_CL * WG_CL;
-  if (grid < WG_CL) grid = WG_CL;
-  plan->grid = grid;
-  plan->P = grid / WG_CL + FIX_SLOTS;   // one slot per cluster + the deferred rows' slots (k_fix_accum_t)
-  plan->Pc = grid + 8 * ctx->sm_count;        // cost partials: one per CTA + one per k_fix_labels_t CTA
-  plan->scratch_bytes = t_layout(*plan, n, k, d).total;
-  return B2K_OK;
-}
-
-void b2k_fused_t_views(const B2kFusedPlan& plan, void* plan_scratch, int64_t n, int k, int d, float** partials,
-                       int32_t** counts, double** cost_partials, unsigned long long** rstat) {
-  TLayout L = t_layout(plan, n, k, d);
-  char* b = static_cast<char*>(plan_scratch);
-  *partials = reinterpret_cast<float*>(b + L.off_partials);
-  *counts = reinterpret_cast<int32_t*>(b + L.off_counts);
-  *cost_partials = reinterpret_cast<double*>(b + L.off_cost);
-  if (rstat) *rstat = reinterpret_cast<unsigned long long*>(b + L.off_rstat);
+  plan->grid = std::max(plan->grid / WG_CL * WG_CL, WG_CL);
+  plan->P = plan->grid / WG_CL + FIX_SLOTS;   // one slot per cluster + the deferred rows' slots (k_fix_accum_t)
+  plan->Pc = plan->grid + 8 * ctx->sm_count;  // cost partials: one per CTA + one per k_fix_labels_t CTA
+  const TLayout L = t_layout(*plan, n, k, d);
+  plan->off_partials = L.off_partials;
+  plan->off_counts = L.off_counts;
+  plan->off_cost = L.off_cost;
+  plan->off_rstat = L.off_rstat;
+  plan->scratch_bytes = L.total;
 }
 
 static bool xnorm_in_scope(const b2k_ctx* ctx, const float* X, int64_t n, int d) {
@@ -455,8 +438,7 @@ int b2k_fused_t_prepare(b2k_ctx* ctx, const B2kFusedPlan& plan, void* plan_scrat
 
 int b2k_launch_fused_t(b2k_ctx* ctx, const B2kFusedPlan& plan, void* plan_scratch, const float* X, int64_t n, int d,
                        const float* C, int k, int32_t* labels_out, float* mindist_out, bool do_update, bool need_cost,
-                       const B2kLoopState* st, cudaStream_t s, const double* prev_counts) {
-  (void)prev_counts;
+                       const B2kLoopState* st, cudaStream_t s) {
   if (ctx->profile_fused)
     return b2k_fail(ctx, B2K_ERR_UNSUPPORTED, "profile_fused: this build records no per-role profile");
   TLayout L = t_layout(plan, n, k, d);
@@ -466,6 +448,8 @@ int b2k_launch_fused_t(b2k_ctx* ctx, const B2kFusedPlan& plan, void* plan_scratc
   float* cnorm = reinterpret_cast<float*>(b + L.off_cnorm);
   float* thr = reinterpret_cast<float*>(b + L.off_thr);
   int32_t* labels = labels_out;
+  // an assign pass forms the exact min distances (and cost partials) only when the caller takes either
+  const bool cost = !do_update && (mindist_out != nullptr || need_cost);
 
   k_prep_centers_t<<<32, 256, 0, s>>>(C, k, d, plan.DP, Ct, cnorm, st);
   k_tables_t<<<1, 256, 0, s>>>(k, cnorm, thr, st);
@@ -473,8 +457,10 @@ int b2k_launch_fused_t(b2k_ctx* ctx, const B2kFusedPlan& plan, void* plan_scratc
   B2K_CUDA_OK(ctx, cudaGetLastError());
 
   CUtensorMap mx, mc;
-  B2K_TRY(b2k_fused_encode_2d(ctx, &mx, X, (uint64_t)d, (uint64_t)n, (uint64_t)d * 4, CHUNK, TN, 1));
-  B2K_TRY(b2k_fused_encode_2d(ctx, &mc, Ct, (uint64_t)plan.DP, 256, (uint64_t)plan.DP * 4, CHUNK, 256, 0));
+  B2K_TRY(b2k_encode_2d(ctx, &mx, X, (uint64_t)d, (uint64_t)n, (uint64_t)d * 4, CHUNK, TN,
+                        CU_TENSOR_MAP_L2_PROMOTION_L2_256B));
+  B2K_TRY(b2k_encode_2d(ctx, &mc, Ct, (uint64_t)plan.DP, 256, (uint64_t)plan.DP * 4, CHUNK, 256,
+                        CU_TENSOR_MAP_L2_PROMOTION_L2_128B));
 
   WgArgs a{};
   a.n = n;
@@ -500,8 +486,8 @@ int b2k_launch_fused_t(b2k_ctx* ctx, const B2kFusedPlan& plan, void* plan_scratc
   a.partials = reinterpret_cast<float*>(b + L.off_partials);
   a.counts = reinterpret_cast<int32_t*>(b + L.off_counts);
 
-  const int rc = plan.DP == 128 ? b2k_launch_wg<256, 4, false>(ctx, plan.grid, mx, mc, mc, a, need_cost, do_update, s)
-                                : b2k_launch_wg<256, 8, false>(ctx, plan.grid, mx, mc, mc, a, need_cost, do_update, s);
+  const int rc = plan.DP == 128 ? b2k_launch_wg<256, 4, false>(ctx, plan.grid, mx, mc, mc, a, cost, do_update, s)
+                                : b2k_launch_wg<256, 8, false>(ctx, plan.grid, mx, mc, mc, a, cost, do_update, s);
   B2K_TRY(rc);
   ctx->stats.kernel_launches++;
   ctx->stats.fused_tc_launches++;
@@ -522,7 +508,7 @@ int b2k_launch_fused_t(b2k_ctx* ctx, const B2kFusedPlan& plan, void* plan_scratc
   f.mask_cap = L.mask_cap;
   f.labels_out = labels;
   f.mind_out = mindist_out;
-  f.need_cost = need_cost ? 1 : 0;
+  f.need_cost = cost ? 1 : 0;
   f.cost_out = a.cost_partials + plan.grid;
   f.rstat = a.rstat;
   f.partial = a.partials + (size_t)(plan.P - FIX_SLOTS) * k * d;

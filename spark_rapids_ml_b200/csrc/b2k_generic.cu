@@ -462,21 +462,6 @@ int b2k_launch_gather_rows(b2k_ctx* ctx, const float* X, int d, const int64_t* r
   return B2K_OK;
 }
 
-__global__ void k_min_inplace(float* __restrict__ a, const float* __restrict__ b, int64_t n) {
-  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  int64_t stride = (int64_t)gridDim.x * blockDim.x;
-  for (; i < n; i += stride) a[i] = fminf(a[i], b[i]);
-}
-int b2k_launch_min_inplace(b2k_ctx* ctx, float* a, const float* b, int64_t n, cudaStream_t s) {
-  if (n <= 0) return B2K_OK;
-  int64_t blocks = (n + 255) / 256;
-  if (blocks > ctx->sm_count * 16) blocks = ctx->sm_count * 16;
-  k_min_inplace<<<(unsigned)blocks, 256, 0, s>>>(a, b, n);
-  ctx->stats.kernel_launches++;
-  B2K_CUDA_OK(ctx, cudaGetLastError());
-  return B2K_OK;
-}
-
 // chunked assign (k > 256): fold one chunk's (min distance, local label) into the running (min distance, global label);
 // strict '<' keeps the earlier chunk (= the lower cluster index) on ties
 __global__ void k_merge_chunk(float* __restrict__ md_acc, int32_t* __restrict__ lab_acc, const float* __restrict__ md,

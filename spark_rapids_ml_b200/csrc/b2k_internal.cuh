@@ -41,15 +41,12 @@ struct b2k_ctx {
   int time_kernels = 0;
   int check_every = 4;
   int grid_limit = 0;
-  int probe = 0;                 // debug/experiment switch for the fused kernel (0 = normal)
   int adaptive_path = 1;         // option "adaptive_path": a Lloyd loop on the large-shape kernel falls back to the generic
                                  // kernels for its remaining iterations when most rows need the exact fix-up
-  int lloyd_switched = 0;
-  int near_tie_hint = 0;         // set around the k-means|| candidate passes: prefer exact 128-centre chunks (d <= 128)        // the last lloyd_impl call did so (the fit's inertia pass follows it)
+  int lloyd_switched = 0;        // the last lloyd_impl call did so (the fit's inertia pass follows it)
+  int near_tie_hint = 0;         // set around the k-means|| candidate passes: prefer exact 128-centre chunks (d <= 128)
   int force_variant_t = 0;       // option "variant_t": route every supported shape through b2k_fused_t.cu (tests)
-  int tma_box_rows = 0;          // option "tma_box_rows": rows per TMA box of b2k_debug_tma_stream (diagnostic; 0 = 128)
   int collect_recheck = 0;       // option "collect_recheck": fill stats.recheck_* (costs a stream sync per call)
-  int want_cost = 1;             // assign passes: compute the cost partial (set by assign_impl)
   int profile_fused = 0;         // record per-role blocked-cycle counters of the fused kernel
   // Row norms of the large-shape kernel, shared by every pass of ONE b2k_kmeans_fit call (k-means|| candidate passes,
   // the Lloyd loop, the inertia pass all see the same immutable X): computed by the first pass, reused by the rest.
@@ -133,8 +130,10 @@ int b2k_launch_sum_f32_to_f64(b2k_ctx* ctx, const float* v, int64_t n, double* o
 int b2k_launch_fold_f64(b2k_ctx* ctx, const double* in, int m, double* out /*1*/, cudaStream_t s);
 int b2k_launch_gather_rows(b2k_ctx* ctx, const float* X, int d, const int64_t* rows_local, int m,
                            float* out, int64_t out_row0, cudaStream_t s);
+// chunked assign: md_acc/lab_acc <- (md, lab + base) where md < md_acc
+int b2k_launch_merge_chunk(b2k_ctx* ctx, float* md_acc, int32_t* lab_acc, const float* md, const int32_t* lab, int base,
+                           int64_t n, const B2kLoopState* st, cudaStream_t s);
 // k-means|| helpers
-int b2k_launch_min_inplace(b2k_ctx* ctx, float* a, const float* b, int64_t n, cudaStream_t s);
 int b2k_launch_bernoulli_pick(b2k_ctx* ctx, const float* mind, int64_t n, int64_t row_offset,
                               double scale /* l/phi */, uint64_t seed, int round, int64_t* picked,
                               int* n_picked, int cap, cudaStream_t s);
@@ -145,47 +144,58 @@ int b2k_launch_weighted_update(b2k_ctx* ctx, const float* P, const double* w, co
 int b2k_launch_pairwise_sqdist(b2k_ctx* ctx, const float* P, int M, int d, float* D2, cudaStream_t s);
 
 // ------------------------------------------------------------------------------------------------
-// wgmma fused assign kernel — b2k_fused_tc.cu / b2k_fused_t.cu (b2k_wg.cuh)
+// wgmma fused assign kernel (b2k_wg.cuh) in two families:
+//   variant 0 — b2k_fused_tc.cu: k <= 128, d <= 128 (its compiled instantiations), 3xTF32
+//   variant 1 — b2k_fused_t.cu:  k, d <= 256, 1xTF32 screening + exact fix-up of the near-tie rows
+// b2k_fused.cu holds what does not depend on the family: the shape rules, the plan, dispatch and the TMA encoder.
 // ------------------------------------------------------------------------------------------------
+constexpr int B2K_FUSED_TILE_ROWS = 128;   // X rows per tile of the fused kernel (WG_TM)
+
 struct B2kFusedPlan {
-  int KP = 0, DP = 0;        // padded cluster count / dimension of the instantiation, 0 = unsupported
-  int grid = 0;              // persistent CTAs
-  int variant = 0;           // 0: b2k_fused_tc.cu (k <= 128, d <= 128, 3xTF32); 1: b2k_fused_t.cu (k, d <= 256, 1xTF32 + recheck)
-  int P = 0;                 // partial-sum slots of the update pass (b2k_update_generic_scratch)
+  int KP = 0, DP = 0;        // padded cluster count / dimension of the instantiation
+  int grid = 0;              // persistent CTAs (variant 1: whole clusters of WG_CL CTAs)
+  int variant = 0;           // family, see above
+  int P = 0;                 // partial-sum slots a Lloyd pass writes (variant 0: one per CTA; 1: one per cluster + fix-up)
   int Pc = 0;                // cost partials the pass writes (variant 0: grid; variant 1: grid + fix-up CTAs)
-  size_t scratch_bytes = 0;  // centre operands/cnorm + partials/counts/cost (+ row norms, variant 1)
+  size_t scratch_bytes = 0;  // centre operands/cnorm + partials/counts/cost (+ row norms, fix-up list, variant 1)
+  // byte offsets into the plan scratch of what a pass leaves for its caller
+  size_t off_partials = 0;   // f32 [P][k][d]
+  size_t off_counts = 0;     // i32 [P][k]
+  size_t off_cost = 0;       // f64 [Pc]
+  size_t off_rstat = 0;      // variant 1: u64 {rows re-decided exactly, candidate distances} since b2k_fused_prepare
+  float* partials(void* ps) const { return reinterpret_cast<float*>(static_cast<char*>(ps) + off_partials); }
+  int32_t* counts(void* ps) const { return reinterpret_cast<int32_t*>(static_cast<char*>(ps) + off_counts); }
+  double* cost_partials(void* ps) const { return reinterpret_cast<double*>(static_cast<char*>(ps) + off_cost); }
+  unsigned long long* rstat(void* ps) const {
+    return variant == 1 ? reinterpret_cast<unsigned long long*>(static_cast<char*>(ps) + off_rstat) : nullptr;
+  }
 };
-bool b2k_fused_supported(const b2k_ctx* ctx, int64_t n, int d, int k, const float* X);
+bool b2k_fused_supported(int64_t n, int d, int k, const float* X);
 int b2k_fused_plan(b2k_ctx* ctx, int64_t n, int d, int k, B2kFusedPlan* plan);
 // Once per fit / lloyd / assign call, before the first b2k_launch_fused on this X (variant 1: row norms; variant 0: no-op)
 int b2k_fused_prepare(b2k_ctx* ctx, const B2kFusedPlan& plan, void* plan_scratch, const float* X, int64_t n, int d, int k,
                       cudaStream_t s);
-// One fused pass: (labels_out, mindist_out optional) + partial sums/counts/cost into plan scratch.
-// `do_update` = accumulate partial sums (Lloyd iteration) or labels only (assign/inertia pass).
-int b2k_launch_fused(b2k_ctx* ctx, const B2kFusedPlan& plan, void* plan_scratch, const float* X,
-                     int64_t n, int d, const float* C, int k, int32_t* labels_out, float* mindist_out,
-                     bool do_update, const B2kLoopState* st, cudaStream_t s, const double* prev_counts = nullptr);
-// Views into the plan scratch after a fused pass (to feed b2k_launch_reduce_partials)
-void b2k_fused_views(const B2kFusedPlan& plan, void* plan_scratch, int64_t n, int k, int d, float** partials,
-                     int32_t** counts, double** cost_partials);
-// variant 1 diagnostics: {rows re-decided exactly, candidate distances evaluated} since the last b2k_fused_prepare
-int b2k_fused_recheck_stats(b2k_ctx* ctx, const B2kFusedPlan& plan, void* plan_scratch, int64_t n, int k, int d,
-                            unsigned long long out[2], cudaStream_t s);
+// One fused pass: labels_out and mindist_out (either may be NULL) + partial sums/counts/cost into the plan scratch.
+// `do_update` = accumulate partial sums (Lloyd iteration, no min distances) or not (assign/inertia pass); `need_cost` =
+// the caller reads the cost partials of an assign pass (variant 0 forms them on every assign pass).
+int b2k_launch_fused(b2k_ctx* ctx, const B2kFusedPlan& plan, void* plan_scratch, const float* X, int64_t n, int d,
+                     const float* C, int k, int32_t* labels_out, float* mindist_out, bool do_update, bool need_cost,
+                     const B2kLoopState* st, cudaStream_t s);
+int b2k_encode_2d(b2k_ctx* ctx, CUtensorMap* map, const void* base, uint64_t inner, uint64_t outer,
+                  uint64_t row_stride_bytes, uint32_t box_inner, uint32_t box_outer, CUtensorMapL2promotion l2);
 
-// b2k_fused_t.cu (variant 1)
-bool b2k_fused_t_supported(const b2k_ctx* ctx, int64_t n, int d, int k, const float* X);
-int b2k_fused_t_plan(b2k_ctx* ctx, int64_t n, int d, int k, B2kFusedPlan* plan);
-void b2k_fused_t_views(const B2kFusedPlan& plan, void* plan_scratch, int64_t n, int k, int d, float** partials,
-                       int32_t** counts, double** cost_partials, unsigned long long** rstat);
+// the families (called by b2k_fused.cu only).  *_plan fill the rest of a plan whose grid b2k_fused_plan has set
+// (variant 1 rounds it down to whole clusters).
+bool b2k_fused_tc_plan(int64_t n, int d, int k, B2kFusedPlan* plan);   // false: no instantiation for (k, d)
+int b2k_launch_fused_tc(b2k_ctx* ctx, const B2kFusedPlan& plan, void* plan_scratch, const float* X, int64_t n, int d,
+                        const float* C, int k, int32_t* labels_out, float* mindist_out, bool do_update,
+                        const B2kLoopState* st, cudaStream_t s);
+void b2k_fused_t_plan(const b2k_ctx* ctx, int64_t n, int d, int k, B2kFusedPlan* plan);
 int b2k_fused_t_prepare(b2k_ctx* ctx, const B2kFusedPlan& plan, void* plan_scratch, const float* X, int64_t n, int d,
                         int k, cudaStream_t s);
 int b2k_launch_fused_t(b2k_ctx* ctx, const B2kFusedPlan& plan, void* plan_scratch, const float* X, int64_t n, int d,
                        const float* C, int k, int32_t* labels_out, float* mindist_out, bool do_update, bool need_cost,
-                       const B2kLoopState* st, cudaStream_t s, const double* prev_counts);
-int b2k_launch_merge_chunk(b2k_ctx* ctx, float* md_acc, int32_t* lab_acc, const float* md, const int32_t* lab, int base,
-                           int64_t n, const B2kLoopState* st, cudaStream_t s);
-int b2k_fused_encode_2d(b2k_ctx* ctx, CUtensorMap* map, const void* base, uint64_t inner, uint64_t outer,
-                        uint64_t row_stride_bytes, uint32_t box_inner, uint32_t box_outer, int l2_256);
+                       const B2kLoopState* st, cudaStream_t s);
 
 // ------------------------------------------------------------------------------------------------
 // comm — b2k_comm.cu

@@ -27,25 +27,9 @@ __device__ __forceinline__ uint32_t mbar_try_wait(uint32_t bar, uint32_t parity)
       : "memory");
   return ok;
 }
-// Bounded wait: a protocol bug traps (sticky launch failure the host reports) instead of hanging the GPU.
-__device__ __noinline__ void mbar_timeout(uint32_t bar, uint32_t parity) {
-  printf("b2k fused: mbarrier timeout block %d warp %d bar_off %u parity %u\n", blockIdx.x, threadIdx.x >> 5, bar,
-         parity);
-  __trap();
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  uint32_t spins = 0;
-  for (;;) {   // 4 polls per bookkeeping step: the poll loop is 2 instructions per try
-    if (mbar_try_wait(bar, parity)) return;
-    if (mbar_try_wait(bar, parity)) return;
-    if (mbar_try_wait(bar, parity)) return;
-    if (mbar_try_wait(bar, parity)) return;
-    if (++spins == (1u << 20)) mbar_timeout(bar, parity);
-  }
-}
-
-// Bounded wait without a call: a function call between wgmma instructions makes ptxas serialize the whole wgmma pipeline
-// of the kernel (C7510), so the wgmma kernels trap without reporting.
+// Bounded wait: a protocol bug traps (sticky launch failure the host reports) instead of hanging the GPU.  It traps
+// without a printf: a function call between wgmma instructions makes ptxas serialize the whole wgmma pipeline of the
+// kernel (C7510).
 __device__ __forceinline__ void mbar_wait_nocall(uint32_t bar, uint32_t parity) {
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {

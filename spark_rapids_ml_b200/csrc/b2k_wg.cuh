@@ -1,5 +1,6 @@
 // Fused assign kernel for sm_90a (H100): wgmma (tf32) distances + argmin, ONE pass over X per launch.  Shared by the two
-// shape families (included inside the anonymous namespace of b2k_fused_tc.cu and b2k_fused_t.cu after b2k_ptx.cuh):
+// shape families (included inside the anonymous namespace of b2k_fused_tc.cu and b2k_fused_t.cu after b2k_ptx.cuh; their
+// common host side — shape rules, plan, dispatch, TMA descriptors — is b2k_fused.cu):
 //
 //   THREE = true  (k <= 128, d <= 128): "3xTF32".  Each consumer thread loads its wgmma A fragments from the X slot,
 //                 splits them in registers into x = hi + lo (both round-to-nearest tf32) and accumulates
@@ -26,7 +27,7 @@
 // centre chunk(s) [KP x 32 f32] (SC stages), all with 128-byte swizzle = K-major GMMA operands.  Warps 0-7 are two
 // consumer warpgroups; warpgroup g owns rows [64 g, 64 g + 64) of every 128-row tile and keeps D[64 x KP] in registers
 // (KP / 2 per thread).  Persistent grid, static round-robin over tiles: every output is a fixed function of the data.
-constexpr int WG_TM = 128;                          // rows per tile (two warpgroups x wgmma M = 64)
+constexpr int WG_TM = B2K_FUSED_TILE_ROWS;          // rows per tile (two warpgroups x wgmma M = 64)
 constexpr int WG_CHUNK = 32;                        // f32 per 128-byte swizzle row = one TMA box / 4 wgmma K steps
 constexpr int WG_XBYTES = WG_TM * WG_CHUNK * 4;     // 16 KB: one X slot
 constexpr int WG_NTHREADS = 384;                    // 8 consumer warps + a producer warpgroup (one warp issues)
@@ -37,13 +38,13 @@ constexpr int WG_M_CNORM = 256, WG_M_XN = 1280, WG_M_LAB = 1792, WG_M_FLAG = 281
 // THREE: barriers, ||c||^2 [KP], ||x||^2 [128] (NC) or the row order [128] (UPD) in one area, labels [2][128], cost
 constexpr int WG_MISC3 = 2368;
 constexpr int WG_M3_XN = 768, WG_M3_SRT = 768, WG_M3_LAB = 1280, WG_M3_COST = 2304;
-constexpr int WG_CL = 8;
+constexpr int WG_CL = 8;   // THREE = false, UPD: CTAs per cluster; CTA r sums centres [r KP / 8, (r + 1) KP / 8)
 // PROF builds: per-warp cycle counters [grid][WG_NTHREADS / 32][WG_NPROF].  Each mark charges the cycles since the
 // previous mark to one phase, so a warp's counters sum to its whole run.  Consumer warps: X wait, centre wait, hand-off
 // wait, A load + split, MMA issue + drain, epilogue, sort, column sums.  Producer warp: X slot wait, centre stage wait,
 // issue (slot 2).
 constexpr int WG_NPROF = 8;
-enum { WG_P_WX, WG_P_WC, WG_P_HAND, WG_P_SPLIT, WG_P_MMA, WG_P_EPI, WG_P_SORT, WG_P_SUMS };        // THREE = false, UPD: CTAs per cluster; CTA r sums centres [r KP / 8, (r + 1) KP / 8)
+enum { WG_P_WX, WG_P_WC, WG_P_HAND, WG_P_SPLIT, WG_P_MMA, WG_P_EPI, WG_P_SORT, WG_P_SUMS };
 
 template <int KP, int NCH, bool THREE, bool UPD>
 struct WgCfg {
