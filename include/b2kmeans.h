@@ -1,6 +1,6 @@
 /*
- * b2kmeans.h — C ABI of libb2kmeans.so: the H100-native (sm_90a) KMeans Lloyd-loop backend that
- * replaces the cuML calls on spark-rapids-ml's distributed KMeans.fit() path.
+ * b2kmeans.h — C ABI of libb2kmeans.so: the H100-native (sm_90a) KMeans Lloyd-loop and PCA backend that
+ * replaces the cuML calls on spark-rapids-ml's distributed KMeans.fit() and PCA.fit() paths.
  *
  * Reference interfaces each entry point stands in for (paths relative to the reference repo
  * NVIDIA/spark-rapids-ml @ c51743bb, python/src/spark_rapids_ml/):
@@ -17,6 +17,11 @@
  *                               reduce_rows_by_key, allreduce x2, divide, convergence) — also the unit
  *                               bench.py times as one "step" per iteration
  *   b2k_kmeans_assign           clustering.py:582-602 (KMeans.predict with injected cluster_centers_)
+ *   b2k_pca_fit                 feature.py:196-242 (PCAMG(handle, **cuml_init).fit(...) and the mean_/components_/
+ *                               explained_variance_ratio_/singular_values_ attribute reads)
+ *   b2k_pca_finalize            the eigen step inside the above (EXTERNAL cuML: eigendecomposition of the covariance,
+ *                               sign flip, explained variance ratio, singular values)
+ *   b2k_pca_transform           feature.py:398-451 (PCAMG.transform with injected components_, mean added back)
  *
  * Conventions
  *   - Plain C, no exceptions across the boundary: every call returns a b2k_status; the message for the
@@ -25,7 +30,7 @@
  *   - All device pointers are BORROWED from the caller (torch tensors on the Python side); the library owns
  *     only its scratch, TMA descriptors, pinned staging and the NCCL communicator, all inside the ctx.
  *   - `stream` is a cudaStream_t passed as uintptr_t (0 = legacy default stream).  All device work is
- *     enqueued on it.  Calls that return host values (fit, lloyd) synchronise that stream before returning.
+ *     enqueued on it.  Calls that return host values (fit, lloyd, pca_fit) synchronise that stream before returning.
  *   - One context per process per GPU; NOT thread-safe (callers are single-threaded Spark Python workers).
  *   - There is no CPU fallback: without a CUDA device every compute entry point fails with B2K_ERR_CUDA.
  */
@@ -108,6 +113,10 @@ typedef struct b2k_stats {
                                   generic kernels because most rows needed the exact fix-up (option "adaptive_path",
                                   default 1; only with kernel_path = auto); -1 = it did not */
 } b2k_stats;
+/* b2k_pca_fit reuses the fields: last_path = the Gram pass that ran (B2K_PATH_FUSED = wgmma, B2K_PATH_GENERIC = SIMT);
+ * with option "time_kernels" != 0, last_reduce_ms = the column-sum pass, last_fused_ms = the Gram pass, last_allreduce_ms
+ * = both allreduces (device times, CUDA events), last_finalize_ms = the host eigen step and last_loop_ms = the whole call
+ * (host clock). */
 
 int b2k_version(void);
 const char* b2k_last_error(const b2k_ctx* ctx);
@@ -177,6 +186,31 @@ int b2k_kmeans_lloyd(b2k_ctx* ctx, const float* X, int64_t n_local, int d, int k
  * or NULL.  Ties -> lowest center index. Asynchronous on `stream`. ---- */
 int b2k_kmeans_assign(b2k_ctx* ctx, const float* X, int64_t n, int d, const float* centers, int k,
                       int32_t* labels_out, float* mindist_out, uintptr_t stream);
+
+/* ---- PCA ----
+ * Shapes: 1 <= k <= d <= 1024.  The Gram pass runs on wgmma (3xTF32, fp64 partials every 4096 rows) when d % 4 == 0 and X is
+ * 16-byte aligned, else on the generic SIMT kernel (fp64 products and sums); option "kernel_path" = B2K_PATH_GENERIC
+ * forces the generic kernel, B2K_PATH_FUSED fails with B2K_ERR_UNSUPPORTED where the wgmma pass cannot run.  d > 1024:
+ * B2K_ERR_UNSUPPORTED.
+ *
+ * fit: X device f32 [n_local, d] row-major.  Host f64 outputs: mean_out [d] = sum x / n_total (fp64), components_out
+ * [k][d] = eigenvectors of the covariance (x - mean)^T (x - mean) / (n_total - 1) by descending eigenvalue, each signed
+ * so that its largest-|value| element (lowest index on a tie) is positive; explained_variance_ratio_out [k] = lambda_i /
+ * trace(covariance); singular_values_out [k] = sqrt(lambda_i (n_total - 1)).  Eigenvalues below 0 (rounding) count as 0.
+ * Zero total variance (constant features) is not an error: the ratios and singular values are 0 and the components are
+ * the first k unit vectors.  Errors: k < 1, k > d ("source vector size d must be no less than k"), n_total < 2, an
+ * empty partition on any rank.  Collective across the communicator when one is initialised; synchronises `stream`
+ * before returning.  Bitwise reproducible for the same input, rank count and device. */
+int b2k_pca_fit(b2k_ctx* ctx, const float* X, int64_t n_local, int d, int k, double* mean_out, double* components_out,
+                double* explained_variance_ratio_out, double* singular_values_out, uintptr_t stream);
+/* The eigen step of b2k_pca_fit alone, on the host (no context, no device): cov [d][d] f64 (only the upper triangle is
+ * read), outputs as above.  Errors through b2k_last_error(NULL). */
+int b2k_pca_finalize(const double* cov, int d, int64_t n_total, int k, double* components_out,
+                     double* explained_variance_ratio_out, double* singular_values_out);
+/* out [n][k] f32 = X [n][d] . components^T (components device f32 [k][d]); no mean is subtracted, as in Spark's
+ * PCAModel.  fp32 accumulation in feature order.  Asynchronous on `stream`. */
+int b2k_pca_transform(b2k_ctx* ctx, const float* X, int64_t n, int d, const float* components, int k, float* out,
+                      uintptr_t stream);
 
 #ifdef __cplusplus
 }

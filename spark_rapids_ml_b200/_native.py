@@ -51,6 +51,9 @@ EXPORTED_SYMBOLS = (
     "b2k_kmeans_fit",
     "b2k_kmeans_lloyd",
     "b2k_kmeans_assign",
+    "b2k_pca_fit",
+    "b2k_pca_finalize",
+    "b2k_pca_transform",
 )
 
 
@@ -125,6 +128,9 @@ def load_library() -> ctypes.CDLL:
     L.b2k_kmeans_lloyd.argtypes = [vp, vp, i64, i32, i32, vp, i32, f64, ctypes.POINTER(i32),
                                    ctypes.POINTER(f64), ctypes.c_size_t]
     L.b2k_kmeans_assign.argtypes = [vp, vp, i64, i32, vp, i32, vp, vp, ctypes.c_size_t]
+    L.b2k_pca_fit.argtypes = [vp, vp, i64, i32, i32, vp, vp, vp, vp, ctypes.c_size_t]
+    L.b2k_pca_finalize.argtypes = [vp, i32, i64, i32, vp, vp, vp]
+    L.b2k_pca_transform.argtypes = [vp, vp, i64, i32, vp, i32, vp, ctypes.c_size_t]
     for name in EXPORTED_SYMBOLS:
         if name not in ("b2k_last_error",):
             getattr(L, name).restype = i32
@@ -140,6 +146,24 @@ def comm_unique_id() -> bytes:
     if rc != B2K_OK:
         raise B2KError(rc, (L.b2k_last_error(None) or b"").decode())
     return buf.raw
+
+
+def pca_finalize(cov: np.ndarray, n_total: int, k: int) -> Dict[str, np.ndarray]:
+    """The host eigen step of b2k_pca_fit alone (no device): cov [d, d] float64 -> components_ [k, d],
+    explained_variance_ratio_ [k], singular_values_ [k] (float64)."""
+    L = load_library()
+    cov = np.ascontiguousarray(cov, dtype=np.float64)
+    if cov.ndim != 2 or cov.shape[0] != cov.shape[1]:
+        raise ValueError("cov must be a square matrix")
+    d = int(cov.shape[0])
+    kk = max(int(k), 0)
+    comp = np.zeros((kk, d), dtype=np.float64)
+    evr = np.zeros(kk, dtype=np.float64)
+    sv = np.zeros(kk, dtype=np.float64)
+    rc = L.b2k_pca_finalize(cov.ctypes.data, d, int(n_total), int(k), comp.ctypes.data, evr.ctypes.data, sv.ctypes.data)
+    if rc != B2K_OK:
+        raise B2KError(rc, (L.b2k_last_error(None) or b"").decode())
+    return {"components_": comp, "explained_variance_ratio_": evr, "singular_values_": sv}
 
 
 def _stream_handle(torch_mod: Any, device: Any) -> int:
@@ -347,3 +371,32 @@ class Context:
                 md.data_ptr() if md is not None else None, self._stream()))
         t.cuda.current_stream(self.device).synchronize()  # C (a temporary) must outlive the kernels
         return labels, md
+
+    def pca_fit(self, X: Any, k: int) -> Dict[str, np.ndarray]:
+        """PCAMG(n_components=k).fit(X) equivalent (collective when a communicator is initialised).  Returns host float64
+        arrays: mean_ [d], components_ [k, d], explained_variance_ratio_ [k], singular_values_ [k]."""
+        n, d = self._check_X(X)
+        kk = max(int(k), 0)
+        mean = np.zeros(d, dtype=np.float64)
+        comp = np.zeros((kk, d), dtype=np.float64)
+        evr = np.zeros(kk, dtype=np.float64)
+        sv = np.zeros(kk, dtype=np.float64)
+        with self._torch.cuda.device(self.device):
+            self._check(self._L.b2k_pca_fit(self._h, X.data_ptr(), n, d, int(k), mean.ctypes.data, comp.ctypes.data,
+                                            evr.ctypes.data, sv.ctypes.data, self._stream()))
+        return {"mean_": mean, "components_": comp, "explained_variance_ratio_": evr, "singular_values_": sv}
+
+    def pca_transform(self, X: Any, components: Any) -> Any:
+        """PCAModel.transform equivalent: X [n, d] . components^T -> float32 CUDA tensor [n, k] (no mean subtracted)."""
+        t = self._torch
+        n, d = self._check_X(X)
+        C = t.as_tensor(components, dtype=t.float32, device=self.device).contiguous()
+        if C.dim() != 2 or C.shape[1] != d:
+            raise ValueError(f"components must be [k, {d}]")
+        k = int(C.shape[0])
+        out = t.empty((n, k), dtype=t.float32, device=self.device)
+        with t.cuda.device(self.device):
+            self._check(self._L.b2k_pca_transform(self._h, X.data_ptr(), n, d, C.data_ptr(), k, out.data_ptr(),
+                                                  self._stream()))
+        t.cuda.current_stream(self.device).synchronize()  # C (possibly a temporary) must outlive the kernel
+        return out

@@ -19,10 +19,11 @@ from typing import Any, Callable, Dict, List, Optional, Sequence, Tuple, Union
 import numpy as np
 import pandas as pd
 
-from .core import (FitInputType, _CumlEstimator, _CumlModelWithPredictionCol, alias, param_alias)
+from .core import (FitInputType, _append_transform_features, _CumlEstimator, _CumlModelWithPredictionCol,
+                   _transform_context, param_alias)
 from .params import HasFeaturesCols, P, _CumlClass, _CumlParams, _KMeansParams
 from .sparkshim import Row, keyword_only
-from .utils import arrow_list_column_buffers, get_logger
+from .utils import get_logger
 
 
 class KMeansClass(_CumlClass):
@@ -223,38 +224,6 @@ class KMeans(KMeansClass, _CumlEstimator, _KMeansCumlParams):
         return [_one_model_row([r]) for r in rows]
 
 
-_TRANSFORM_CONTEXTS: Dict[int, Any] = {}
-_TRANSFORM_CONTEXTS_LOCK = __import__("threading").Lock()
-
-
-def _transform_context(gpu: int) -> Any:
-    """One library context per (process, GPU) for transform tasks: a Spark Python worker is reused across tasks, and a
-    context's set-up (stream, pinned staging buffers, scratch, copy threads) costs more than labelling a small
-    partition.  Released at interpreter exit."""
-    from . import _native
-
-    with _TRANSFORM_CONTEXTS_LOCK:
-        ctx = _TRANSFORM_CONTEXTS.get(gpu)
-        if ctx is None:
-            ctx = _native.Context(gpu)
-            _TRANSFORM_CONTEXTS[gpu] = ctx
-            if len(_TRANSFORM_CONTEXTS) == 1:
-                import atexit
-
-                atexit.register(_close_transform_contexts)
-        return ctx
-
-
-def _close_transform_contexts() -> None:
-    with _TRANSFORM_CONTEXTS_LOCK:
-        for ctx in _TRANSFORM_CONTEXTS.values():
-            try:
-                ctx.close()
-            except Exception:
-                pass
-        _TRANSFORM_CONTEXTS.clear()
-
-
 class KMeansModel(KMeansClass, _CumlModelWithPredictionCol, _KMeansCumlParams):
     """reference: clustering.py:505-604."""
 
@@ -308,30 +277,6 @@ class KMeansModel(KMeansClass, _CumlModelWithPredictionCol, _KMeansCumlParams):
         def _construct_kmeans(gpu: int = 0) -> Any:
             return _DeviceKMeans(gpu)
 
-        def _append_features(app: Any, df: Union[pd.DataFrame, np.ndarray]) -> None:
-            n_b = len(df)
-            if isinstance(df, pd.DataFrame) and alias.data in df.columns:
-                col = df[alias.data]
-                bufs = arrow_list_column_buffers(col, n_cols)
-                if bufs is not None:
-                    app.append_values(bufs[0], bufs[1], bufs[2])
-                else:
-                    stacked = np.ascontiguousarray(np.array(list(col), order="C"), dtype=np.float32)
-                    if stacked.ndim != 2 or stacked.shape[1] != n_cols:
-                        raise ValueError(f"feature rows do not match the model's {n_cols} columns")
-                    app.append_values(stacked.reshape(-1), None, n_b)
-            elif isinstance(df, pd.DataFrame):
-                if len(df.columns) != n_cols:
-                    raise ValueError(f"{len(df.columns)} feature columns do not match the model's {n_cols}")
-                cols = [np.ascontiguousarray(df[c].to_numpy()) for c in df.columns]
-                dt = cols[0].dtype
-                app.append_columns([c if c.dtype == dt else c.astype(dt) for c in cols])
-            else:
-                arr = np.ascontiguousarray(df, dtype=np.float32)
-                if arr.ndim != 2 or arr.shape[1] != n_cols:
-                    raise ValueError(f"feature rows do not match the model's {n_cols} columns")
-                app.append_values(arr.reshape(-1), None, n_b)
-
         def _transform_many(kmeans: Any, dfs: List[Union[pd.DataFrame, np.ndarray]]) -> List[pd.Series]:
             """Several input batches in ONE device pass: every batch is ingested into the same device matrix, one
             b2k_kmeans_assign labels all rows, one read-back, one Series per input batch (same order, same lengths).
@@ -346,7 +291,7 @@ class KMeansModel(KMeansClass, _CumlModelWithPredictionCol, _KMeansCumlParams):
             app = DeviceRowAppender(kmeans.ctx, n_cols, first_capacity=total)
             for df, n_b in zip(dfs, sizes):
                 if n_b:
-                    _append_features(app, df)
+                    _append_transform_features(app, df, n_cols)
             X = app.finish()
             labels, _ = kmeans.ctx.kmeans_assign(X, kmeans.C)
             host = labels.cpu().numpy()

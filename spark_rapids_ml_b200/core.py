@@ -115,6 +115,82 @@ def _features_from_pdf(pdf: pd.DataFrame, multi_col_names: Optional[List[str]], 
     return n_b
 
 
+def _append_transform_features(app: DeviceRowAppender, df: Union[pd.DataFrame, np.ndarray], n_cols: int) -> None:
+    """One transform input batch -> rows of the device matrix: the Arrow child buffer of the feature column (zero-copy),
+    an object column of ndarrays (stacked on the host), scalar feature columns, or a plain array."""
+    n_b = len(df)
+    if isinstance(df, pd.DataFrame) and alias.data in df.columns:
+        col = df[alias.data]
+        bufs = arrow_list_column_buffers(col, n_cols)
+        if bufs is not None:
+            app.append_values(bufs[0], bufs[1], bufs[2])
+        else:
+            stacked = np.ascontiguousarray(np.array(list(col), order="C"), dtype=np.float32)
+            if stacked.ndim != 2 or stacked.shape[1] != n_cols:
+                raise ValueError(f"feature rows do not match the model's {n_cols} columns")
+            app.append_values(stacked.reshape(-1), None, n_b)
+    elif isinstance(df, pd.DataFrame):
+        if len(df.columns) != n_cols:
+            raise ValueError(f"{len(df.columns)} feature columns do not match the model's {n_cols}")
+        cols = [np.ascontiguousarray(df[c].to_numpy()) for c in df.columns]
+        dt = cols[0].dtype
+        app.append_columns([c if c.dtype == dt else c.astype(dt) for c in cols])
+    else:
+        arr = np.ascontiguousarray(df, dtype=np.float32)
+        if arr.ndim != 2 or arr.shape[1] != n_cols:
+            raise ValueError(f"feature rows do not match the model's {n_cols} columns")
+        app.append_values(arr.reshape(-1), None, n_b)
+
+
+_TRANSFORM_CONTEXTS: Dict[int, Any] = {}
+_TRANSFORM_CONTEXTS_LOCK = __import__("threading").Lock()
+
+
+def _transform_context(gpu: int) -> Any:
+    """One library context per (process, GPU) for transform tasks: a Spark Python worker is reused across tasks, and a
+    context's set-up (stream, pinned staging buffers, scratch, copy threads) costs more than labelling a small
+    partition.  Released at interpreter exit."""
+    from . import _native
+
+    with _TRANSFORM_CONTEXTS_LOCK:
+        ctx = _TRANSFORM_CONTEXTS.get(gpu)
+        if ctx is None:
+            ctx = _native.Context(gpu)
+            _TRANSFORM_CONTEXTS[gpu] = ctx
+            if len(_TRANSFORM_CONTEXTS) == 1:
+                import atexit
+
+                atexit.register(_close_transform_contexts)
+        return ctx
+
+
+def _close_transform_contexts() -> None:
+    with _TRANSFORM_CONTEXTS_LOCK:
+        for ctx in _TRANSFORM_CONTEXTS.values():
+            try:
+                ctx.close()
+            except Exception:
+                pass
+        _TRANSFORM_CONTEXTS.clear()
+
+
+_ARROW_SCALARS = {"int": pa.int32(), "float": pa.float32(), "double": pa.float64()}
+
+
+def _transform_result_array(res: Any, out_type: str) -> pa.Array:
+    """One transform result (a pandas Series) as the Arrow array of the model's output type: "int" or "array<float>" /
+    "array<double>" (one fixed-width vector per row)."""
+    if out_type.startswith("array<"):
+        elem = _ARROW_SCALARS[out_type[len("array<"):-1]]
+        rows = list(res)
+        width = len(rows[0]) if rows else 0
+        vals = np.asarray(rows, dtype=elem.to_pandas_dtype()).reshape(-1) if rows else np.zeros(0, elem.to_pandas_dtype())
+        offsets = np.arange(0, len(rows) * width + 1, max(width, 1), dtype=np.int32)[: len(rows) + 1]
+        return pa.ListArray.from_arrays(pa.array(offsets), pa.array(vals, type=elem))
+    return pa.array(np.asarray(res), type=_ARROW_SCALARS[out_type])
+
+
+
 class _CumlCaller(_CumlParams, _CumlCommon):
     """reference: core.py:435-1019."""
 
@@ -617,7 +693,11 @@ class _CumlModel(ModelBase, _CumlParams, _CumlCommon):
 
 
 class _CumlModelWithColumns(_CumlModel):
-    """reference: core.py:1797-1941 — keeps the input columns and appends the prediction column."""
+    """reference: core.py:1797-1941 — keeps the input columns and appends the output column."""
+
+    def _output_col_name(self) -> str:
+        """The column transform() appends: predictionCol here, outputCol for a feature transformer."""
+        return self.getOrDefault("predictionCol")
 
     def _transform(self, dataset: Any) -> Any:
         if HAVE_PYSPARK:
@@ -628,8 +708,8 @@ class _CumlModelWithColumns(_CumlModel):
                     self, dataset, alias.data, lambda ctx, local: _CumlCommon._set_gpu_device(ctx, local, True))
         input_col, input_cols = self._get_input_columns()
         construct, transform_internal, _ = self._get_cuml_transform_func(dataset)
-        pred_name = self.getOrDefault("predictionCol")
-        types = dict(dataset.dtypes)
+        pred_name = self._output_col_name()
+        out_type = self._out_schema(dataset.schema)
         n_cols = self.n_cols
         out_parts: List[List[pa.Array]] = []
         state: Dict[str, Any] = {}
@@ -649,7 +729,7 @@ class _CumlModelWithColumns(_CumlModel):
 
                 return _batches_to_pdf_iter(selected(), dataset.arrow_backed_pandas)
 
-            out_parts.append([pa.array(np.asarray(res), type=pa.int32())
+            out_parts.append([_transform_result_array(res, out_type)
                               for res in _iter_transform(transform_internal, lambda: state["model"], frames())])
         if "model" in state and hasattr(state["model"], "close"):
             state["model"].close()

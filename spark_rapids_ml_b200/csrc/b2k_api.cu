@@ -949,3 +949,41 @@ extern "C" int b2k_kmeans_fit(b2k_ctx* ctx, const float* X, int64_t n_local, int
   }
   return B2K_OK;
 }
+
+// ------------------------------------------------------------------------------------------------
+// PCA (b2k_pca.cu)
+// ------------------------------------------------------------------------------------------------
+extern "C" int b2k_pca_fit(b2k_ctx* ctx, const float* X, int64_t n_local, int d, int k, double* mean_out,
+                           double* components_out, double* explained_variance_ratio_out, double* singular_values_out,
+                           uintptr_t stream) {
+  if (!ctx) return b2k_fail(nullptr, B2K_ERR_INVALID, "b2k_pca_fit: ctx is NULL");
+  if (!X || n_local < 0 || d <= 0) return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_pca_fit: bad X/n/d");
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  B2K_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  {
+    // as b2k_kmeans_fit: every rank fails together on an empty partition (core.py:959-962)
+    Rows rows;
+    B2K_TRY(gather_sizes(ctx, n_local, &rows, s));
+    for (int r = 0; r < ctx->nranks; ++r)
+      if (rows.sizes[r] == 0)
+        return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_pca_fit: empty partition (rank " + std::to_string(r) +
+                                                  " has n_local == 0)");
+  }
+  return b2k_pca_fit_impl(ctx, X, n_local, d, k, mean_out, components_out, explained_variance_ratio_out,
+                          singular_values_out, s);
+}
+
+extern "C" int b2k_pca_finalize(const double* cov, int d, int64_t n_total, int k, double* components_out,
+                                double* explained_variance_ratio_out, double* singular_values_out) {
+  return b2k_pca_finalize_impl(nullptr, cov, d, n_total, k, components_out, explained_variance_ratio_out,
+                               singular_values_out);
+}
+
+extern "C" int b2k_pca_transform(b2k_ctx* ctx, const float* X, int64_t n, int d, const float* components, int k,
+                                 float* out, uintptr_t stream) {
+  if (!ctx) return b2k_fail(nullptr, B2K_ERR_INVALID, "b2k_pca_transform: ctx is NULL");
+  if (!X || !components || !out || n < 0 || d <= 0 || k <= 0)
+    return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_pca_transform: bad X/components/out/n/d/k");
+  B2K_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  return b2k_pca_transform_impl(ctx, X, n, d, components, k, out, reinterpret_cast<cudaStream_t>(stream));
+}

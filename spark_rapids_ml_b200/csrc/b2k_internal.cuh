@@ -206,3 +206,15 @@ int b2k_comm_allgather_i64(b2k_ctx* ctx, const int64_t* send_dev, int64_t* recv_
 int b2k_comm_allreduce_f32(b2k_ctx* ctx, float* buf, size_t count, cudaStream_t s);
 
 // ingest — b2k_ingest.cu (entry point is the C ABI itself)
+
+// ------------------------------------------------------------------------------------------------
+// PCA — b2k_pca.cu (the C ABI entry points in b2k_api.cu check their arguments and the partitions, then call these)
+// ------------------------------------------------------------------------------------------------
+constexpr int B2K_PCA_MAX_D = 1024;   // both Gram paths, the projection kernel and the host eigen step
+int b2k_pca_fit_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, int k, double* mean_out, double* components_out,
+                     double* evr_out, double* sv_out, cudaStream_t s);
+// ctx may be NULL (b2k_pca_finalize): errors then go to b2k_last_error(NULL)
+int b2k_pca_finalize_impl(b2k_ctx* ctx, const double* cov, int d, int64_t n_total, int k, double* components_out,
+                          double* evr_out, double* sv_out);
+int b2k_pca_transform_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, const float* C, int k, float* Y,
+                           cudaStream_t s);

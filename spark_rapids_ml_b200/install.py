@@ -1,9 +1,9 @@
 """No-import-change mode: after `import spark_rapids_ml_b200.install`, user code that says
-`from pyspark.ml.clustering import KMeans` (or KMeansModel) receives this package's accelerated classes; every other
-attribute of `pyspark.ml.clustering`, and every access made from inside pyspark.ml or from this package itself, still
-resolves to pyspark's own module.  Reference behaviour: python/src/spark_rapids_ml/install.py:21-81 (a proxy module per
-pyspark.ml sub-module whose __getattr__ looks at the calling file); only the clustering entry exists here because KMeans
-is the one path this package accelerates (SURVEY.md 8 f-4).
+`from pyspark.ml.clustering import KMeans` (or KMeansModel, or `from pyspark.ml.feature import PCA` / PCAModel) receives
+this package's accelerated classes; every other attribute of those modules, and every access made from inside pyspark.ml
+or from this package itself, still resolves to pyspark's own module.  Reference behaviour:
+python/src/spark_rapids_ml/install.py:21-81 (a proxy module per pyspark.ml sub-module whose __getattr__ looks at the
+calling file); only the sub-modules of the paths this package accelerates have an entry (SURVEY.md 8 f-4, f-1).
 
 `python -m spark_rapids_ml_b200 script.py [args]` / `-m module [args]` runs a script with this mode on
 (reference: python/src/spark_rapids_ml/__main__.py).
@@ -16,7 +16,7 @@ import sys
 import types
 from typing import Any, Dict, Tuple
 
-ACCELERATED: Dict[str, Tuple[str, ...]] = {"clustering": ("KMeans", "KMeansModel")}
+ACCELERATED: Dict[str, Tuple[str, ...]] = {"clustering": ("KMeans", "KMeansModel"), "feature": ("PCA", "PCAModel")}
 
 _PKG_DIR = os.path.dirname(os.path.abspath(__file__))
 

@@ -101,6 +101,39 @@ class _KMeansParams(HasFeaturesCol, HasPredictionCol):
         return self.getOrDefault(self.distanceMeasure)
 
 
+class HasInputCol(Params):
+    inputCol = Param("parent", "inputCol", "input column name.", TypeConverters.toString)
+
+
+class HasInputCols(Params):
+    """reference: params.py:91-107 — multi-column (scalar) input of a feature transformer."""
+
+    inputCols = Param("parent", "inputCols", "input column names.", TypeConverters.toListString)
+
+    def getInputCols(self) -> List[str]:
+        return self.getOrDefault(self.inputCols)
+
+
+class HasOutputCol(Params):
+    outputCol = Param("parent", "outputCol", "output column name.", TypeConverters.toString)
+
+    def __init__(self) -> None:
+        super().__init__()
+        self._setDefault(outputCol=self.uid + "__output")   # pyspark's HasOutputCol default
+
+    def getOutputCol(self) -> str:
+        return self.getOrDefault(self.outputCol)
+
+
+class _PCAParams(HasInputCol, HasOutputCol):
+    """pyspark.ml.feature._PCAParams stand-in: k (no default), inputCol, outputCol."""
+
+    k = Param("parent", "k", "the number of principal components (> 0).", TypeConverters.toInt)
+
+    def getK(self) -> int:
+        return self.getOrDefault(self.k)
+
+
 class _CumlClass(object):
     """reference: params.py:162-257."""
 
@@ -188,11 +221,11 @@ class _CumlParams(_CumlClass, HasVerboseParam, Params):
             if spark_param != cuml_param and spark_param in kwargs and cuml_param in kwargs:
                 raise ValueError(f"'{cuml_param}' is an alias of '{spark_param}', set one or the other.")
         for k, v in kwargs.items():
-            if k == "featuresCol":
+            if k in ("featuresCol", "inputCol") and self.hasParam(k):   # a list selects the multi-column param
                 if isinstance(v, str):
-                    self._set(featuresCol=v)
+                    self._set(**{k: v})
                 elif isinstance(v, list):
-                    self._set(featuresCols=v)
+                    self._set(**{k + "s": v})
             elif self.hasParam(k):
                 self._set(**{k: v})
                 self._set_cuml_param(k, v, silent=self._fallback_enabled)
@@ -226,10 +259,11 @@ class _CumlParams(_CumlClass, HasVerboseParam, Params):
 
     def _get_input_columns(self) -> Tuple[Optional[str], Optional[List[str]]]:
         """reference: params.py:521-554."""
-        if self.hasParam("featuresCols") and self.isDefined("featuresCols"):
-            return None, self.getOrDefault("featuresCols")
-        if self.hasParam("featuresCol") and self.isDefined("featuresCol"):
-            return self.getOrDefault("featuresCol"), None
+        for multi, single in (("featuresCols", "featuresCol"), ("inputCols", "inputCol")):
+            if self.hasParam(multi) and self.isDefined(multi):
+                return None, self.getOrDefault(multi)
+            if self.hasParam(single) and self.isDefined(single):
+                return self.getOrDefault(single), None
         raise ValueError("Please set inputCol(s) or featuresCol(s)")
 
     def _get_cuml_param(self, spark_param: str, silent: bool = True) -> Optional[str]:

@@ -149,7 +149,7 @@ def current_barrier_context() -> Any:
 
 
 def transform_with_pandas_udf(model: Any, dataset: Any, data_alias: str, set_gpu: Callable[[Any, bool], int]) -> Any:
-    """reference core.py:1797-1941 for a single prediction column: pandas_udf over struct(features) + withColumn."""
+    """reference core.py:1797-1941 for a single output column: pandas_udf over struct(features) + withColumn."""
     from pyspark.ml.functions import vector_to_array
     from pyspark.ml.linalg import VectorUDT
     from pyspark.sql.functions import col, pandas_udf, struct
@@ -166,7 +166,7 @@ def transform_with_pandas_udf(model: Any, dataset: Any, data_alias: str, set_gpu
     else:
         select_cols = [col(c) for c in (input_cols or [])]
 
-    @pandas_udf(model._out_schema(dataset.schema))   # "int"
+    @pandas_udf(model._out_schema(dataset.schema))   # "int" (KMeans), "array<float>" (PCA)
     def predict_udf(iterator: Iterator[pd.DataFrame]) -> Iterator[pd.Series]:
         from pyspark import TaskContext
 
@@ -180,8 +180,7 @@ def transform_with_pandas_udf(model: Any, dataset: Any, data_alias: str, set_gpu
             if hasattr(device_model, "close"):
                 device_model.close()
 
-    pred_name = model.getOrDefault("predictionCol")
-    return dataset.withColumn(pred_name, predict_udf(struct(*select_cols)))
+    return dataset.withColumn(model._output_col_name(), predict_udf(struct(*select_cols)))
 
 
 def _extra_metadata(inst: Any) -> dict:
