@@ -152,22 +152,6 @@ int b2k_scratch_reserve(b2k_ctx* ctx, size_t bytes) {
 }
 
 namespace {
-inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
-
-// Bump allocator over ctx->scratch.
-struct Arena {
-  char* base;
-  size_t off = 0;
-  explicit Arena(void* b) : base(static_cast<char*>(b)) {}
-  template <typename T>
-  T* take(size_t count) {
-    off = align_up(off, 256);
-    T* p = reinterpret_cast<T*>(base + off);
-    off += count * sizeof(T);
-    return p;
-  }
-};
-
 int check_shape(b2k_ctx* ctx, const char* who, const void* X, int64_t n, int d, int k) {
   if (!ctx) return b2k_fail(nullptr, B2K_ERR_INVALID, std::string(who) + ": ctx is NULL");
   if (!X || n < 0 || d <= 0 || k <= 0)
@@ -175,18 +159,16 @@ int check_shape(b2k_ctx* ctx, const char* who, const void* X, int64_t n, int d, 
   return B2K_OK;
 }
 
-bool want_fused(b2k_ctx* ctx, int64_t n, int d, int k, const float* X, int* status) {
-  *status = B2K_OK;
-  bool ok = b2k_fused_supported(n, d, k, X);
-  if (ctx->kernel_path == B2K_PATH_GENERIC) return false;
-  if (ctx->kernel_path == B2K_PATH_FUSED && !ok) {
-    *status = b2k_fail(ctx, B2K_ERR_UNSUPPORTED,
-                       "kernel_path=2 (fused) requested but shape (n=" + std::to_string(n) + ", d=" +
-                           std::to_string(d) + ", k=" + std::to_string(k) +
-                           ") is outside the fused kernel's instantiations");
-    return false;
-  }
-  return ok;
+bool use_fused(const b2k_ctx* ctx, int64_t n, int d, int k, const float* X) {
+  return ctx->kernel_path != B2K_PATH_GENERIC && b2k_fused_supported(n, d, k, X);
+}
+
+// kernel_path = 2 on a shape the fused kernel does not take is an error, not a fall-back to the generic kernels
+int check_forced_fused(b2k_ctx* ctx, int64_t n, int d, int k, const float* X) {
+  if (ctx->kernel_path != B2K_PATH_FUSED || b2k_fused_supported(n, d, k, X)) return B2K_OK;
+  return b2k_fail(ctx, B2K_ERR_UNSUPPORTED,
+                  "kernel_path=2 (fused) requested but shape (n=" + std::to_string(n) + ", d=" + std::to_string(d) +
+                      ", k=" + std::to_string(k) + ") is outside the fused kernel's instantiations");
 }
 
 // stats.recheck_*: the rows the large-shape kernel re-decided exactly since b2k_fused_prepare and the candidate distances
@@ -231,14 +213,18 @@ struct LoopBuffers {
 // the screening kernel and free for the 3xTF32 one).  Replaces the SIMT assign of the generic path for d % 4 == 0.
 // ------------------------------------------------------------------------------------------------
 namespace {
-struct ChunkedAssign {
-  B2kFusedPlan plan;
-  int ch = 0;                // chunk size
-  void* ps = nullptr;        // plan scratch
-  int32_t* tmp_lab = nullptr;
+// The path of one assign pass and where it keeps its scratch (assign_layout)
+struct AssignScratch {
+  int ch = 0;                   // chunk size, 0 = not chunked
+  bool fused = false;           // not chunked: one fused pass over every centre, else the generic kernels
+  B2kFusedPlan plan;            // chunked, fused
+  void* ps = nullptr;           // plan scratch
+  int32_t* tmp_lab = nullptr;   // chunked
   float* tmp_md = nullptr;
   int32_t* lab_acc = nullptr;   // used when the caller passes no labels / mindist buffer
   float* md_acc = nullptr;
+  float* cnorm = nullptr;       // generic
+  double* blocks = nullptr;     // chunked, generic: block sums of the cost
 };
 // chunk size, 0 = this (d, k) is not chunked
 int chunked_assign_ch(const b2k_ctx* ctx, int64_t n, int d, int k, const float* X) {
@@ -248,25 +234,37 @@ int chunked_assign_ch(const b2k_ctx* ctx, int64_t n, int d, int k, const float* 
   if (!want || !b2k_fused_supported(n, d, ch, X)) return 0;
   return ch;
 }
-size_t chunked_assign_bytes(b2k_ctx* ctx, int64_t n, int d, int ch) {
-  B2kFusedPlan plan;
-  if (b2k_fused_plan(ctx, n, d, ch, &plan) != B2K_OK) return 0;
-  return align_up(plan.scratch_bytes, 1024) + 4 * align_up((size_t)n * 4, 256) + 4096;
-}
-// `base`: 1 KB aligned scratch of chunked_assign_bytes(); the caller runs b2k_fused_prepare(ca.plan, ca.ps, ..., ca.ch)
-int chunked_assign_setup(b2k_ctx* ctx, int64_t n, int d, int ch, void* base, ChunkedAssign* ca) {
-  ca->ch = ch;
-  B2K_TRY(b2k_fused_plan(ctx, n, d, ch, &ca->plan));
-  Arena A(base);
-  ca->tmp_lab = A.take<int32_t>(n);
-  ca->tmp_md = A.take<float>(n);
-  ca->lab_acc = A.take<int32_t>(n);
-  ca->md_acc = A.take<float>(n);
-  A.off = align_up(A.off, 1024);
-  ca->ps = A.base + A.off;
+constexpr int kCostBlocks = 1024;   // block sums of the two-level cost reduction
+// Lays out the scratch of one assign pass in L and chooses its path.  own_md: the caller wants the cost and passes no
+// mindist buffer (the generic path then keeps its own in md_acc).  A fused or chunked pass starts with b2k_fused_prepare.
+int assign_layout(b2k_ctx* ctx, int64_t n, int d, int k, const float* X, bool own_md, B2kLayout& L, AssignScratch* a) {
+  if ((a->ch = chunked_assign_ch(ctx, n, d, k, X))) {
+    B2K_TRY(b2k_fused_plan(ctx, n, d, a->ch, &a->plan));
+    a->tmp_lab = L.take<int32_t>(n);
+    a->tmp_md = L.take<float>(n);
+    a->lab_acc = L.take<int32_t>(n);
+    a->md_acc = L.take<float>(n);
+    a->ps = L.take<char>(a->plan.scratch_bytes, 1024);
+    a->blocks = L.take<double>(kCostBlocks);
+  } else if ((a->fused = use_fused(ctx, n, d, k, X))) {
+    B2K_TRY(b2k_fused_plan(ctx, n, d, k, &a->plan));
+    a->ps = L.take<char>(a->plan.scratch_bytes, 1024);
+  } else {
+    a->cnorm = L.take<float>(k);
+    if (own_md) a->md_acc = L.take<float>(n > 0 ? n : 1);
+    a->blocks = L.take<double>(kCostBlocks);
+  }
   return B2K_OK;
 }
-int chunked_assign_run(b2k_ctx* ctx, const ChunkedAssign& ca, const float* X, int64_t n, int d, const float* C, int k,
+// raises *bytes to what assign_impl lays out for these arguments (a caller sizes its nested region with the largest)
+int assign_need(b2k_ctx* ctx, int64_t n, int d, int k, const float* X, bool own_md, size_t* bytes) {
+  B2kLayout measure;
+  AssignScratch a;
+  B2K_TRY(assign_layout(ctx, n, d, k, X, own_md, measure, &a));
+  *bytes = std::max(*bytes, measure.off);
+  return B2K_OK;
+}
+int chunked_assign_run(b2k_ctx* ctx, const AssignScratch& ca, const float* X, int64_t n, int d, const float* C, int k,
                        int32_t* labels, float* mindist, const B2kLoopState* st, cudaStream_t s) {
   int32_t* lab = labels ? labels : ca.lab_acc;
   float* md = mindist ? mindist : ca.md_acc;
@@ -295,45 +293,34 @@ static int lloyd_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, int k, flo
   // k > 256 (d <= 256): the assignment runs in 256-centre chunks on the large-shape kernel, the update stays generic
   const int chunk_ch = k > 256 ? chunked_assign_ch(ctx, n, d, k, X) : 0;
   const bool chunked = chunk_ch != 0;
-  int st_rc = B2K_OK;
-  const bool fused = chunked ? false : want_fused(ctx, n, d, k, X, &st_rc);
-  B2K_TRY(st_rc);
+  if (!chunked) B2K_TRY(check_forced_fused(ctx, n, d, k, X));
+  const bool fused = !chunked && use_fused(ctx, n, d, k, X);
   ctx->stats.last_path = (fused || chunked) ? B2K_PATH_FUSED : B2K_PATH_GENERIC;
 
   LoopBuffers B{};
-  size_t gen_bytes = 0;
   if (fused) B2K_TRY(b2k_fused_plan(ctx, n, d, k, &B.plan));
   // The large-shape kernel (1xTF32 screening) hands near-tie rows to an exact fix-up; on data where most rows are
   // near-ties (e.g. uniform noise in 256 dimensions) the generic kernels are several times faster, so the loop may
   // switch to them between bursts.  The choice is local to the rank: both paths fill the same R buffer.
   const bool can_switch = fused && B.plan.variant == 1 && ctx->adaptive_path && ctx->kernel_path == B2K_PATH_AUTO;
   const bool need_generic = !fused || can_switch;
-  if (need_generic) gen_bytes = b2k_update_generic_scratch(ctx, n, d, k, &B.P);
+  if (need_generic) B.P = b2k_update_generic_slots(ctx, n, d, k);
   const size_t rlen = b2k_reduced_len(k, d);
-  size_t total = 4096 + align_up(rlen * 8, 256) + align_up((size_t)k * 8, 256) + align_up((size_t)k * 4, 256) +
-                 (fused ? align_up(B.plan.scratch_bytes, 1024) + 2048 : 0) +
-                 (need_generic ? align_up((size_t)n * 4, 256) + align_up(gen_bytes, 256) + 4096 : 0) +
-                 (chunked ? chunked_assign_bytes(ctx, n, d, chunk_ch) + 2048 : 0);
-  B2K_TRY(b2k_scratch_reserve(ctx, total));
-  Arena A(ctx->scratch);
-  B.st = A.take<B2kLoopState>(1);
-  B.R = A.take<double>(rlen);
-  B.shift_scratch = A.take<double>(k);
-  B.cnorm = A.take<float>(k);
-  if (need_generic) {
-    B.labels = A.take<int32_t>(n > 0 ? n : 1);
-    B.partials = A.take<float>((size_t)B.P * k * d);
-    B.counts = A.take<int32_t>((size_t)B.P * k);
-  }
-  if (fused) {
-    A.off = align_up(A.off, 1024);
-    B.plan_scratch = A.base + A.off;
-  }
-  ChunkedAssign ca;
-  if (chunked) {
-    A.off = align_up(A.off, 1024);
-    B2K_TRY(chunked_assign_setup(ctx, n, d, chunk_ch, A.base + A.off, &ca));
-  }
+  AssignScratch ca;
+  B2K_TRY(b2k_scratch_layout(ctx, "lloyd", [&](B2kLayout& L) -> int {
+    B.st = L.take<B2kLoopState>(1);
+    B.R = L.take<double>(rlen);
+    B.shift_scratch = L.take<double>(k);
+    B.cnorm = L.take<float>(k);
+    if (need_generic) {
+      B.labels = L.take<int32_t>(n > 0 ? n : 1);
+      B.partials = L.take<float>((size_t)B.P * k * d);
+      B.counts = L.take<int32_t>((size_t)B.P * k);
+    }
+    if (fused) B.plan_scratch = L.take<char>(B.plan.scratch_bytes, 1024);
+    if (chunked) B2K_TRY(assign_layout(ctx, n, d, k, X, false, L, &ca));   // takes the chunked path, as chunk_ch says
+    return B2K_OK;
+  }));
 
   B2kLoopState init{};
   init.iter = 0;
@@ -492,77 +479,34 @@ extern "C" int b2k_kmeans_lloyd(b2k_ctx* ctx, const float* X, int64_t n_local, i
 }
 
 // ------------------------------------------------------------------------------------------------
-// assign (+ optional total cost): labels/mindist may be NULL.  Scratch beyond `scratch_off` is used.
+// assign (+ optional total cost): labels/mindist may be NULL.  assign_impl lays out its scratch in the region its caller
+// sized with assign_need; it never grows ctx->scratch, which would move memory the caller still holds there.
 // ------------------------------------------------------------------------------------------------
 static int assign_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, const float* C, int k, int32_t* labels,
-                       float* mindist, double* cost_dev /* device, 1 double, may be NULL */, size_t scratch_off,
+                       float* mindist, double* cost_dev /* device, 1 double, may be NULL */, B2kLayout region,
                        cudaStream_t s) {
-  if (const int ch = chunked_assign_ch(ctx, n, d, k, X)) {   // chunks of ch centres through a fused assign pass each
-    const int nblocks = 1024;
-    const size_t off = align_up(scratch_off, 1024);
-    const size_t cbytes = chunked_assign_bytes(ctx, n, d, ch);
-    size_t need = off + cbytes + align_up((size_t)nblocks * 8, 256) + 1024;
-    if (need > ctx->scratch_bytes && scratch_off != 0)
-      return b2k_fail(ctx, B2K_ERR_STATE, "assign_impl: scratch must be pre-reserved by the caller");
-    B2K_TRY(b2k_scratch_reserve(ctx, need));
-    char* base = static_cast<char*>(ctx->scratch) + off;
-    ChunkedAssign ca;
-    B2K_TRY(chunked_assign_setup(ctx, n, d, ch, base, &ca));
-    double* blocks = reinterpret_cast<double*>(base + cbytes);
-    B2K_TRY(b2k_fused_prepare(ctx, ca.plan, ca.ps, X, n, d, ch, s));
-    B2K_TRY(chunked_assign_run(ctx, ca, X, n, d, C, k, labels, mindist, nullptr, s));
-    if (cost_dev) B2K_TRY(b2k_launch_sum_f32_to_f64(ctx, mindist ? mindist : ca.md_acc, n, cost_dev, blocks, nblocks, s));
-    ctx->stats.last_path = B2K_PATH_FUSED;
-    if (ctx->collect_recheck) B2K_TRY(fill_recheck_stats(ctx, ca.plan, ca.ps, s));
-    return B2K_OK;
-  }
-  int st_rc;
-  const bool fused = want_fused(ctx, n, d, k, X, &st_rc);
-  B2K_TRY(st_rc);
-  ctx->stats.last_path = fused ? B2K_PATH_FUSED : B2K_PATH_GENERIC;
-  if (fused) {
-    B2kFusedPlan plan;
-    B2K_TRY(b2k_fused_plan(ctx, n, d, k, &plan));
-    size_t need = align_up(scratch_off, 1024) + align_up(plan.scratch_bytes, 1024) + 1024;
-    if (need > ctx->scratch_bytes && scratch_off != 0)
-      return b2k_fail(ctx, B2K_ERR_STATE, "assign_impl: scratch must be pre-reserved by the caller");
-    B2K_TRY(b2k_scratch_reserve(ctx, need));
-    void* ps = static_cast<char*>(ctx->scratch) + align_up(scratch_off, 1024);
-    B2K_TRY(b2k_fused_prepare(ctx, plan, ps, X, n, d, k, s));
-    B2K_TRY(b2k_launch_fused(ctx, plan, ps, X, n, d, C, k, labels, mindist, false, cost_dev != nullptr, nullptr, s));
+  AssignScratch a;
+  B2K_TRY(assign_layout(ctx, n, d, k, X, cost_dev && !mindist, region, &a));
+  if (!a.ch) B2K_TRY(check_forced_fused(ctx, n, d, k, X));
+  B2K_TRY(region.check(ctx, "assign"));
+  const bool any_fused = a.ch || a.fused;
+  ctx->stats.last_path = any_fused ? B2K_PATH_FUSED : B2K_PATH_GENERIC;
+  if (any_fused) B2K_TRY(b2k_fused_prepare(ctx, a.plan, a.ps, X, n, d, a.ch ? a.ch : k, s));
+  float* md = mindist ? mindist : a.md_acc;
+  if (a.ch) {   // chunks of ch centres through a fused assign pass each
+    B2K_TRY(chunked_assign_run(ctx, a, X, n, d, C, k, labels, mindist, nullptr, s));
+    if (cost_dev) B2K_TRY(b2k_launch_sum_f32_to_f64(ctx, md, n, cost_dev, a.blocks, kCostBlocks, s));
+  } else if (a.fused) {
+    B2K_TRY(b2k_launch_fused(ctx, a.plan, a.ps, X, n, d, C, k, labels, mindist, false, cost_dev != nullptr, nullptr, s));
     // fold the per-CTA cost partials in index order
-    if (cost_dev) B2K_TRY(b2k_launch_fold_f64(ctx, plan.cost_partials(ps), plan.Pc, cost_dev, s));
-    if (ctx->collect_recheck) B2K_TRY(fill_recheck_stats(ctx, plan, ps, s));
+    if (cost_dev) B2K_TRY(b2k_launch_fold_f64(ctx, a.plan.cost_partials(a.ps), a.plan.Pc, cost_dev, s));
   } else {
-    const int nblocks = 1024;
-    size_t need = align_up(scratch_off, 256) + align_up((size_t)k * 4, 256) +
-                  (cost_dev && !mindist ? align_up((size_t)(n > 0 ? n : 1) * 4, 256) : 0) +
-                  align_up((size_t)nblocks * 8, 256) + 1024;
-    if (need > ctx->scratch_bytes && scratch_off != 0)
-      return b2k_fail(ctx, B2K_ERR_STATE, "assign_impl: scratch must be pre-reserved by the caller");
-    B2K_TRY(b2k_scratch_reserve(ctx, need));
-    Arena A(ctx->scratch);
-    A.off = scratch_off;
-    float* cnorm = A.take<float>(k);
-    float* md = mindist;
-    if (cost_dev && !md) md = A.take<float>(n > 0 ? n : 1);
-    double* blocks = A.take<double>(nblocks);
-    B2K_TRY(b2k_launch_center_norms(ctx, C, k, d, cnorm, nullptr, s));
-    B2K_TRY(b2k_launch_assign_generic(ctx, X, n, d, C, cnorm, k, labels, md, nullptr, s));
-    if (cost_dev) B2K_TRY(b2k_launch_sum_f32_to_f64(ctx, md, n, cost_dev, blocks, nblocks, s));
+    B2K_TRY(b2k_launch_center_norms(ctx, C, k, d, a.cnorm, nullptr, s));
+    B2K_TRY(b2k_launch_assign_generic(ctx, X, n, d, C, a.cnorm, k, labels, md, nullptr, s));
+    if (cost_dev) B2K_TRY(b2k_launch_sum_f32_to_f64(ctx, md, n, cost_dev, a.blocks, kCostBlocks, s));
   }
+  if (any_fused && ctx->collect_recheck) B2K_TRY(fill_recheck_stats(ctx, a.plan, a.ps, s));
   return B2K_OK;
-}
-
-// upper bound of what assign_impl needs past scratch_off
-static size_t assign_scratch_bound(b2k_ctx* ctx, int64_t n, int d, int k, const float* X) {
-  size_t b = align_up((size_t)k * 4, 256) + align_up((size_t)(n > 0 ? n : 1) * 4, 256) + 1024 * 8 + 4096;
-  if (const int ch = chunked_assign_ch(ctx, n, d, k, X)) b = std::max(b, chunked_assign_bytes(ctx, n, d, ch) + 1024 * 8 + 8192);
-  if (b2k_fused_supported(n, d, k, X) && ctx->kernel_path != B2K_PATH_GENERIC) {
-    B2kFusedPlan plan;
-    if (b2k_fused_plan(ctx, n, d, k, &plan) == B2K_OK) b = std::max(b, align_up(plan.scratch_bytes, 1024) + 4096);
-  }
-  return b;
 }
 
 extern "C" int b2k_kmeans_assign(b2k_ctx* ctx, const float* X, int64_t n, int d, const float* centers, int k,
@@ -571,8 +515,11 @@ extern "C" int b2k_kmeans_assign(b2k_ctx* ctx, const float* X, int64_t n, int d,
   if (!centers) return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_kmeans_assign: centers is NULL");
   if (n == 0) return B2K_OK;
   B2K_CUDA_OK(ctx, cudaSetDevice(ctx->device));
-  return assign_impl(ctx, X, n, d, centers, k, labels_out, mindist_out, nullptr, 0,
-                     reinterpret_cast<cudaStream_t>(stream));
+  size_t need = 0;
+  B2K_TRY(assign_need(ctx, n, d, k, X, false, &need));
+  B2K_TRY(b2k_scratch_reserve(ctx, need));
+  return assign_impl(ctx, X, n, d, centers, k, labels_out, mindist_out, nullptr,
+                     B2kLayout(ctx->scratch, ctx->scratch_bytes), reinterpret_cast<cudaStream_t>(stream));
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -591,9 +538,12 @@ int gather_sizes(b2k_ctx* ctx, int64_t n_local, Rows* rows, cudaStream_t s) {
   if (ctx->nranks == 1) {
     rows->sizes[0] = n_local;
   } else {
-    B2K_TRY(b2k_scratch_reserve(ctx, 4096 + 16 * (size_t)ctx->nranks));
-    int64_t* send = reinterpret_cast<int64_t*>(ctx->scratch);
-    int64_t* recv = send + 32;
+    int64_t *send = nullptr, *recv = nullptr;
+    B2K_TRY(b2k_scratch_layout(ctx, "gather_sizes", [&](B2kLayout& L) -> int {
+      send = L.take<int64_t>(1);
+      recv = L.take<int64_t>(ctx->nranks);
+      return B2K_OK;
+    }));
     B2K_CUDA_OK(ctx, cudaMemcpyAsync(send, &n_local, 8, cudaMemcpyHostToDevice, s));
     B2K_TRY(b2k_comm_allgather_i64(ctx, send, recv, 1, s));
     B2K_CUDA_OK(ctx, cudaMemcpyAsync(rows->sizes.data(), recv, 8 * (size_t)ctx->nranks, cudaMemcpyDeviceToHost, s));
@@ -605,6 +555,18 @@ int gather_sizes(b2k_ctx* ctx, int64_t n_local, Rows* rows, cudaStream_t s) {
     if (r < ctx->rank) rows->offset += rows->sizes[r];
     rows->total += rows->sizes[r];
   }
+  return B2K_OK;
+}
+
+// Reference: core.py:959-962 "A python worker received no data".  With a communicator the decision is taken on the
+// allgathered sizes, so that every rank fails together instead of one rank leaving its peers in a collective.
+int check_no_empty_partition(b2k_ctx* ctx, const char* who, int64_t n_local, cudaStream_t s) {
+  Rows rows;
+  B2K_TRY(gather_sizes(ctx, n_local, &rows, s));
+  for (int r = 0; r < ctx->nranks; ++r)
+    if (rows.sizes[r] == 0)
+      return b2k_fail(ctx, B2K_ERR_INVALID, std::string(who) + ": empty partition (rank " + std::to_string(r) +
+                                                " has n_local == 0)");
   return B2K_OK;
 }
 
@@ -706,8 +668,11 @@ static int init_random(b2k_ctx* ctx, const float* X, int64_t n, int d, int k, ui
     return b2k_fail(ctx, B2K_ERR_INVALID, "init=random: fewer rows (" + std::to_string(rows.total) + ") than k");
   std::mt19937_64 rng(seed);
   std::vector<int64_t> gidx = sample_distinct(rng, rows.total, k);
-  B2K_TRY(b2k_scratch_reserve(ctx, 4096 + (size_t)k * 8));
-  int64_t* idx_dev = reinterpret_cast<int64_t*>(static_cast<char*>(ctx->scratch) + 1024);
+  int64_t* idx_dev = nullptr;
+  B2K_TRY(b2k_scratch_layout(ctx, "init=random", [&](B2kLayout& L) -> int {
+    idx_dev = L.take<int64_t>(k);
+    return B2K_OK;
+  }));
   return fetch_global_rows(ctx, X, n, d, rows, gidx, C, idx_dev, s);
 }
 
@@ -728,35 +693,37 @@ static int init_kmeans_parallel(b2k_ctx* ctx, const float* X, int64_t n, int d, 
   const double ell = oversampling * k;
   const int cap = (int)std::min<int64_t>(rows.total, (int64_t)(4 * ell) + 64);  // per-round candidate cap
   const int Mmax = 1 + rounds * cap + k;
-  // scratch (all taken from one arena sized from cap / nranks: no fixed-offset control region):
-  //   idx[cap+8] | n_picked | phi | blocks[1024] | exchange[(cap+1)*(nranks+1)] | mind[n] | dn[n] | labels[n] | lab_new[n] |
-  //   cand[Mmax*d] | newc[cap*d] | hist[Mmax] | assign scratch
   size_t nn = (size_t)(n > 0 ? n : 1);
   const size_t per = (size_t)cap + 1;   // [count | cap indices] per rank in the candidate exchange
-  size_t fixed = align_up((size_t)(cap + 8) * 8, 256) + 256 + 256 + align_up(1024 * 8, 256) +
-                 align_up(per * (size_t)(ctx->nranks + 1) * 8, 256) + 4 * align_up(nn * 4, 256) +
-                 align_up((size_t)Mmax * d * 4, 256) + align_up((size_t)cap * d * 4, 256) +
-                 align_up((size_t)Mmax * 8, 256) + 8192;
-  // the assign passes below run with 1 .. Mmax centres: small counts take a fused kernel (its scratch holds per-CTA
-  // partial slots and, for the large-shape kernel, the row norms), large ones the generic path
-  size_t abound = 0;
+  // The assign passes below run with 1, m <= cap (a round) or M <= Mmax (the top-up) centres.  Within one path each need
+  // grows with the count: the generic path's (taken for every count or none) with k, a fused plan's up to the 128 or 256
+  // where the path changes; a chunked pass needs one full chunk's plan, which covers the fused need of any smaller
+  // count.  These counts include every point where the path changes, so their needs bound every pass.
+  size_t assign_bytes = 0;
   for (int kk : {1, std::min(cap, 128), std::min(cap, 256), cap, Mmax})
-    abound = std::max(abound, assign_scratch_bound(ctx, n, d, kk, X));
-  B2K_TRY(b2k_scratch_reserve(ctx, fixed + abound + 4096));
-  Arena A(ctx->scratch);
-  int64_t* idx_dev = A.take<int64_t>(cap + 8);
-  int* n_picked_dev = A.take<int>(8);
-  double* phi_dev = A.take<double>(4);
-  double* blocks = A.take<double>(1024);
-  int64_t* xchg = A.take<int64_t>(per * (size_t)(ctx->nranks + 1));
-  float* mind = A.take<float>(nn);
-  float* dn = A.take<float>(nn);
-  int32_t* labels = A.take<int32_t>(nn);    // running nearest candidate of every row (global candidate index)
-  int32_t* lab_new = A.take<int32_t>(nn);   // nearest among one round's new candidates
-  float* cand = A.take<float>((size_t)Mmax * d);
-  float* newc = A.take<float>((size_t)cap * d);
-  double* hist = A.take<double>(Mmax);
-  const size_t assign_off = align_up(A.off, 1024);
+    B2K_TRY(assign_need(ctx, n, d, kk, X, false, &assign_bytes));
+  int64_t *idx_dev, *xchg;
+  int* n_picked_dev;
+  double *phi_dev, *blocks, *hist;
+  float *mind, *dn, *cand, *newc;
+  int32_t *labels, *lab_new;
+  B2kLayout assign_region;
+  B2K_TRY(b2k_scratch_layout(ctx, "init=k-means||", [&](B2kLayout& L) -> int {
+    idx_dev = L.take<int64_t>(cap + 8);
+    n_picked_dev = L.take<int>(8);
+    phi_dev = L.take<double>(4);
+    blocks = L.take<double>(kCostBlocks);
+    xchg = L.take<int64_t>(per * (size_t)(ctx->nranks + 1));
+    mind = L.take<float>(nn);
+    dn = L.take<float>(nn);
+    labels = L.take<int32_t>(nn);    // running nearest candidate of every row (global candidate index)
+    lab_new = L.take<int32_t>(nn);   // nearest among one round's new candidates
+    cand = L.take<float>((size_t)Mmax * d);
+    newc = L.take<float>((size_t)cap * d);
+    hist = L.take<double>(Mmax);
+    assign_region = L.tail(assign_bytes);
+    return B2K_OK;
+  }));
 
   std::mt19937_64 rng(seed);
   int M = 0;
@@ -765,7 +732,7 @@ static int init_kmeans_parallel(b2k_ctx* ctx, const float* X, int64_t n, int d, 
     std::vector<int64_t> g{U(rng)};
     B2K_TRY(fetch_global_rows(ctx, X, n, d, rows, g, cand, idx_dev, s));
     M = 1;
-    B2K_TRY(assign_impl(ctx, X, n, d, cand, 1, nullptr, mind, phi_dev, assign_off, s));
+    B2K_TRY(assign_impl(ctx, X, n, d, cand, 1, nullptr, mind, phi_dev, assign_region, s));
     B2K_CUDA_OK(ctx, cudaMemsetAsync(labels, 0, nn * 4, s));   // every row is nearest to candidate 0 so far
   }
   std::vector<int64_t> picked_host(cap);
@@ -774,7 +741,7 @@ static int init_kmeans_parallel(b2k_ctx* ctx, const float* X, int64_t n, int d, 
     double phi = 0;
     if (r > 0) {
       // phi = sum(mind) (deterministic two-level sum)
-      B2K_TRY(b2k_launch_sum_f32_to_f64(ctx, mind, n, phi_dev, blocks, 1024, s));
+      B2K_TRY(b2k_launch_sum_f32_to_f64(ctx, mind, n, phi_dev, blocks, kCostBlocks, s));
     }
     if (ctx->nranks > 1) B2K_TRY(b2k_comm_allreduce_f64(ctx, phi_dev, 1, s));
     B2K_CUDA_OK(ctx, cudaMemcpyAsync(&phi, phi_dev, 8, cudaMemcpyDeviceToHost, s));
@@ -827,7 +794,7 @@ static int init_kmeans_parallel(b2k_ctx* ctx, const float* X, int64_t n, int d, 
     // nearest among the new candidates, folded into the running (min distance, nearest candidate): strict '<' keeps the
     // earlier candidate on ties, so after the last round `labels` IS the argmin over all candidates — the k-means||
     // weights need no extra pass over X
-    B2K_TRY(assign_impl(ctx, X, n, d, newc, m, lab_new, dn, nullptr, assign_off, s));
+    B2K_TRY(assign_impl(ctx, X, n, d, newc, m, lab_new, dn, nullptr, assign_region, s));
     B2K_TRY(b2k_launch_merge_chunk(ctx, mind, labels, dn, lab_new, M, n, nullptr, s));
     M += m;
   }
@@ -835,7 +802,7 @@ static int init_kmeans_parallel(b2k_ctx* ctx, const float* X, int64_t n, int d, 
     std::vector<int64_t> extra = sample_distinct(rng, rows.total, k - M + 1);
     B2K_TRY(fetch_global_rows(ctx, X, n, d, rows, extra, cand + (size_t)M * d, idx_dev, s));
     M += (int)extra.size();
-    B2K_TRY(assign_impl(ctx, X, n, d, cand, M, labels, nullptr, nullptr, assign_off, s));
+    B2K_TRY(assign_impl(ctx, X, n, d, cand, M, labels, nullptr, nullptr, assign_region, s));
   }
   // weights = #points closest to each candidate (the running argmin of the rounds)
   B2K_TRY(b2k_launch_histogram(ctx, labels, n, M, hist, s));
@@ -850,18 +817,26 @@ static int init_kmeans_parallel(b2k_ctx* ctx, const float* X, int64_t n, int d, 
   // greedy weighted k-means++ on the host (table look-ups), then 10 weighted Lloyd steps on the device: the assignment
   // of the M candidates through the same kernels as any other assign pass, the weighted update in fixed order (fp64)
   std::vector<float> D2h((size_t)M * M);
-  const size_t reg = align_up((size_t)M * d * 4, 256) + align_up((size_t)M * M * 4, 256) + align_up((size_t)M * 8, 256) +
-                     align_up((size_t)k * d * 4, 256) + align_up((size_t)M * 4, 256) + align_up((size_t)k * 8, 256) + 4096;
-  B2K_TRY(b2k_scratch_reserve(ctx, reg + assign_scratch_bound(ctx, M, d, k, static_cast<const float*>(ctx->scratch)) + 4096));
-  // the scratch may have moved: only `cand` is needed from here on, and it was copied to P above
-  Arena R(ctx->scratch);
-  float* candd = R.take<float>((size_t)M * d);
-  float* D2d = R.take<float>((size_t)M * M);
-  double* wts_dev = R.take<double>(M);
-  float* Ck_dev = R.take<float>((size_t)k * d);
-  int32_t* lab_dev = R.take<int32_t>(M);
-  int64_t* chosen_dev = R.take<int64_t>(k);
-  const size_t refine_off = align_up(R.off, 1024);
+  float *candd, *D2d, *Ck_dev;
+  double* wts_dev;
+  int32_t* lab_dev;
+  int64_t* chosen_dev;
+  B2kLayout refine_region;
+  // the scratch may move here: only `cand` is needed from here on, and it was copied to P above
+  B2K_TRY(b2k_scratch_layout(ctx, "init=k-means|| refinement", [&](B2kLayout& L) -> int {
+    candd = L.take<float>((size_t)M * d);
+    D2d = L.take<float>((size_t)M * M);
+    wts_dev = L.take<double>(M);
+    Ck_dev = L.take<float>((size_t)k * d);
+    lab_dev = L.take<int32_t>(M);
+    chosen_dev = L.take<int64_t>(k);
+    // the refinement assigns the candidates candd: null when measuring, 256-byte aligned when placed, so the fused
+    // path's 16-byte alignment rule sees the same in both runs
+    size_t need = 0;
+    B2K_TRY(assign_need(ctx, M, d, k, candd, false, &need));
+    refine_region = L.tail(need);
+    return B2K_OK;
+  }));
   B2K_CUDA_OK(ctx, cudaMemcpyAsync(candd, P.data(), P.size() * 4, cudaMemcpyHostToDevice, s));
   B2K_CUDA_OK(ctx, cudaMemcpyAsync(wts_dev, wts.data(), (size_t)M * 8, cudaMemcpyHostToDevice, s));
   B2K_TRY(b2k_launch_pairwise_sqdist(ctx, candd, M, d, D2d, s));
@@ -873,7 +848,7 @@ static int init_kmeans_parallel(b2k_ctx* ctx, const float* X, int64_t n, int d, 
   B2K_CUDA_OK(ctx, cudaStreamSynchronize(s));  // `chosen` is pageable
   B2K_TRY(b2k_launch_gather_rows(ctx, candd, d, chosen_dev, k, Ck_dev, 0, s));
   for (int it = 0; it < 10; ++it) {
-    B2K_TRY(assign_impl(ctx, candd, M, d, Ck_dev, k, lab_dev, nullptr, nullptr, refine_off, s));
+    B2K_TRY(assign_impl(ctx, candd, M, d, Ck_dev, k, lab_dev, nullptr, nullptr, refine_region, s));
     B2K_TRY(b2k_launch_weighted_update(ctx, candd, wts_dev, lab_dev, M, d, k, Ck_dev, s));
   }
   B2K_CUDA_OK(ctx, cudaMemcpyAsync(C, Ck_dev, (size_t)k * d * 4, cudaMemcpyDeviceToDevice, s));
@@ -894,16 +869,7 @@ extern "C" int b2k_kmeans_fit(b2k_ctx* ctx, const float* X, int64_t n_local, int
     return b2k_fail(ctx, B2K_ERR_UNSUPPORTED, "b2k_kmeans_fit: n_init must be 1 (the reference forces n_init=1)");
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   B2K_CUDA_OK(ctx, cudaSetDevice(ctx->device));
-  {
-    // reference: core.py:959-962 "A python worker received no data".  With a communicator the decision is taken on the
-    // allgathered sizes, so that every rank fails together instead of one rank leaving its peers in a collective.
-    Rows rows;
-    B2K_TRY(gather_sizes(ctx, n_local, &rows, s));
-    for (int r = 0; r < ctx->nranks; ++r)
-      if (rows.sizes[r] == 0)
-        return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_kmeans_fit: empty partition (rank " + std::to_string(r) +
-                                                  " has n_local == 0)");
-  }
+  B2K_TRY(check_no_empty_partition(ctx, "b2k_kmeans_fit", n_local, s));
   struct NormScope {   // see b2k_ctx::xnorm_scope_X
     b2k_ctx* c;
     NormScope(b2k_ctx* c_, const float* X_, int64_t n_, int d_) : c(c_) {
@@ -938,9 +904,16 @@ extern "C" int b2k_kmeans_fit(b2k_ctx* ctx, const float* X, int64_t n_local, int
     // the inertia pass follows the Lloyd loop's choice of path (see lloyd_impl: adaptive_path)
     const int saved_path = ctx->kernel_path;
     if (ctx->lloyd_switched) ctx->kernel_path = B2K_PATH_GENERIC;
-    int rc = b2k_scratch_reserve(ctx, 4096 + assign_scratch_bound(ctx, n_local, d, k, X));
-    double* cost_dev = reinterpret_cast<double*>(ctx->scratch);
-    if (rc == B2K_OK) rc = assign_impl(ctx, X, n_local, d, centers_out, k, nullptr, nullptr, cost_dev, 1024, s);
+    double* cost_dev = nullptr;
+    B2kLayout assign_region;
+    int rc = b2k_scratch_layout(ctx, "inertia", [&](B2kLayout& L) -> int {
+      cost_dev = L.take<double>(1);
+      size_t need = 0;
+      B2K_TRY(assign_need(ctx, n_local, d, k, X, true, &need));
+      assign_region = L.tail(need);
+      return B2K_OK;
+    });
+    if (rc == B2K_OK) rc = assign_impl(ctx, X, n_local, d, centers_out, k, nullptr, nullptr, cost_dev, assign_region, s);
     ctx->kernel_path = saved_path;
     B2K_TRY(rc);
     if (ctx->nranks > 1) B2K_TRY(b2k_comm_allreduce_f64(ctx, cost_dev, 1, s));
@@ -960,15 +933,7 @@ extern "C" int b2k_pca_fit(b2k_ctx* ctx, const float* X, int64_t n_local, int d,
   if (!X || n_local < 0 || d <= 0) return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_pca_fit: bad X/n/d");
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   B2K_CUDA_OK(ctx, cudaSetDevice(ctx->device));
-  {
-    // as b2k_kmeans_fit: every rank fails together on an empty partition (core.py:959-962)
-    Rows rows;
-    B2K_TRY(gather_sizes(ctx, n_local, &rows, s));
-    for (int r = 0; r < ctx->nranks; ++r)
-      if (rows.sizes[r] == 0)
-        return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_pca_fit: empty partition (rank " + std::to_string(r) +
-                                                  " has n_local == 0)");
-  }
+  B2K_TRY(check_no_empty_partition(ctx, "b2k_pca_fit", n_local, s));
   return b2k_pca_fit_impl(ctx, X, n_local, d, k, mean_out, components_out, explained_variance_ratio_out,
                           singular_values_out, s);
 }

@@ -263,11 +263,7 @@ UpdatePlan plan_update(const b2k_ctx* ctx, int64_t n, int d, int k) {
 }
 }  // namespace
 
-size_t b2k_update_generic_scratch(b2k_ctx* ctx, int64_t n, int d, int k, int* P_out) {
-  UpdatePlan u = plan_update(ctx, n, d, k);
-  if (P_out) *P_out = u.P;
-  return (size_t)u.P * k * d * sizeof(float) + (size_t)u.P * k * sizeof(int32_t);
-}
+int b2k_update_generic_slots(b2k_ctx* ctx, int64_t n, int d, int k) { return plan_update(ctx, n, d, k).P; }
 
 int b2k_launch_update_generic(b2k_ctx* ctx, const float* X, int64_t n, int d, const int32_t* labels, int k,
                               int P, float* partials, int32_t* counts, const B2kLoopState* st,

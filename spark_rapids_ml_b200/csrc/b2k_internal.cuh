@@ -102,6 +102,44 @@ int b2k_fail(b2k_ctx* ctx, int code, const std::string& msg);
 int b2k_scratch_reserve(b2k_ctx* ctx, size_t bytes);
 void b2k_copy_pool_destroy(b2k_ctx* ctx);
 
+// Scratch layout: a bump allocator over a device region {base, cap}.  A driver states its takes once and runs them twice:
+// with no base to measure (`off` is then the bytes they need), then over the region to place its arrays.  Offsets are
+// aligned relative to base: ctx->scratch comes from cudaMalloc (256 B), a nested region starts at a 1 KB boundary.
+struct B2kLayout {
+  char* base = nullptr;   // nullptr: measure only, no pointer is formed
+  size_t cap = 0, off = 0;
+  explicit B2kLayout(void* b = nullptr, size_t c = 0) : base(static_cast<char*>(b)), cap(c) {}
+  template <typename T>
+  T* take(size_t count, size_t align = 256) {
+    off = (off + align - 1) / align * align;
+    T* p = base ? reinterpret_cast<T*>(base + off) : nullptr;
+    off += count * sizeof(T);
+    return p;
+  }
+  // the unused tail from the next `align` boundary on, as the region of a nested call that measured `need` bytes
+  B2kLayout tail(size_t need, size_t align = 1024) {
+    char* p = take<char>(need, align);
+    const size_t start = off - need;
+    return base ? B2kLayout(p, start < cap ? cap - start : 0) : B2kLayout();
+  }
+  int check(b2k_ctx* ctx, const char* who) const {   // after placing: every take stayed inside the region
+    if (off <= cap) return B2K_OK;
+    return b2k_fail(ctx, B2K_ERR_STATE, std::string(who) + ": scratch layout of " + std::to_string(off) +
+                                            " bytes overruns its region of " + std::to_string(cap));
+  }
+};
+
+// Runs `layout` (int(B2kLayout&)) to measure, grows ctx->scratch to that size, then runs it over the scratch to place.
+template <typename F>
+int b2k_scratch_layout(b2k_ctx* ctx, const char* who, F&& layout) {
+  B2kLayout measure;
+  B2K_TRY(layout(measure));
+  B2K_TRY(b2k_scratch_reserve(ctx, measure.off));
+  B2kLayout place(ctx->scratch, ctx->scratch_bytes);
+  B2K_TRY(layout(place));
+  return place.check(ctx, who);
+}
+
 // ------------------------------------------------------------------------------------------------
 // generic (any k, d) kernels — b2k_generic.cu
 // ------------------------------------------------------------------------------------------------
@@ -112,8 +150,8 @@ int b2k_launch_center_norms(b2k_ctx* ctx, const float* C, int k, int d, float* c
 int b2k_launch_assign_generic(b2k_ctx* ctx, const float* X, int64_t n, int d, const float* C,
                               const float* cnorm, int k, int32_t* labels, float* mindist,
                               const B2kLoopState* st, cudaStream_t s);
-// per-cluster partial sums from labels: partials [P][k*d] f32, counts [P][k] i32; returns P via *P_out.
-size_t b2k_update_generic_scratch(b2k_ctx* ctx, int64_t n, int d, int k, int* P_out);
+// per-cluster partial sums from labels: partials [P][k*d] f32, counts [P][k] i32; returns P, the partial slots.
+int b2k_update_generic_slots(b2k_ctx* ctx, int64_t n, int d, int k);
 int b2k_launch_update_generic(b2k_ctx* ctx, const float* X, int64_t n, int d, const int32_t* labels, int k,
                               int P, float* partials, int32_t* counts, const B2kLoopState* st,
                               cudaStream_t s);

@@ -187,8 +187,6 @@ k_project(const float* __restrict__ X, int64_t n, int d, const float* __restrict
   }
 }
 
-inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
-
 struct Timer {   // CUDA events around the device phases when option time_kernels is set
   cudaEvent_t ev[8] = {};
   bool on = false;
@@ -400,19 +398,17 @@ int b2k_pca_fit_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, int k, doub
   const size_t dd = (size_t)d * d;
   const int S = (int)std::max<int64_t>(1, std::min<int64_t>({64, (int64_t)((64u << 20) / (dd * 8)), (n + GG_T - 1) / GG_T}));
   const int64_t gspan = std::max<int64_t>(1, (n + S - 1) / S);
-  const size_t o_colp = 0;
-  const size_t o_sums = align_up(o_colp + (size_t)nspan * d * 8, 256);
-  const size_t o_mu = align_up(o_sums + (size_t)(d + 1) * 8, 256);
-  const size_t o_G = align_up(o_mu + (size_t)nblk * GW_BLK * 4, 256);
-  const size_t o_part = align_up(o_G + dd * 8, 1024);
-  const size_t part_bytes = wg ? (size_t)P * ntile * GW_BLK * GW_BLK * 8 : (size_t)S * dd * 8;
-  B2K_TRY(b2k_scratch_reserve(ctx, o_part + part_bytes));
-  char* sc = static_cast<char*>(ctx->scratch);
-  double* colp = reinterpret_cast<double*>(sc + o_colp);
-  double* sums = reinterpret_cast<double*>(sc + o_sums);
-  float* mu32_dev = reinterpret_cast<float*>(sc + o_mu);
-  double* G = reinterpret_cast<double*>(sc + o_G);
-  double* part = reinterpret_cast<double*>(sc + o_part);
+  const size_t part_len = wg ? (size_t)P * ntile * GW_BLK * GW_BLK : (size_t)S * dd;   // fp64 partials
+  double *colp, *sums, *G, *part;
+  float* mu32_dev;
+  B2K_TRY(b2k_scratch_layout(ctx, "PCA", [&](B2kLayout& L) -> int {
+    colp = L.take<double>((size_t)nspan * d);
+    sums = L.take<double>((size_t)d + 1);
+    mu32_dev = L.take<float>((size_t)nblk * GW_BLK);
+    G = L.take<double>(dd);
+    part = L.take<double>(part_len, 1024);
+    return B2K_OK;
+  }));
 
   // ---- pass 1: column sums, allreduce of [d sums | n] ----
   tm.mark(0, s);
@@ -464,7 +460,7 @@ int b2k_pca_fit_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, int k, doub
       B2K_CUDA_OK(ctx, cudaGetLastError());
       ctx->stats.kernel_launches++;
     } else {
-      B2K_CUDA_OK(ctx, cudaMemsetAsync(part, 0, part_bytes, s));
+      B2K_CUDA_OK(ctx, cudaMemsetAsync(part, 0, part_len * 8, s));
     }
     k_gram_fold_wg<<<fold_blocks, 256, 0, s>>>(part, P, ntile, nblk, d, G);
   } else {
@@ -475,7 +471,7 @@ int b2k_pca_fit_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, int k, doub
       ctx->stats.kernel_launches++;
       ctx->stats.generic_launches++;
     } else {
-      B2K_CUDA_OK(ctx, cudaMemsetAsync(part, 0, part_bytes, s));
+      B2K_CUDA_OK(ctx, cudaMemsetAsync(part, 0, part_len * 8, s));
     }
     k_gram_fold_generic<<<fold_blocks, 256, 0, s>>>(part, S, d, G);
   }
