@@ -14,9 +14,10 @@
 //                 label (+ exact min distance sum (x - c)^2 in assign / inertia passes).
 //
 // UPD (THREE only, Lloyd passes): the same pass also forms the per-cluster sums.  The tile's X chunks stay in shared
-// memory until its sums are formed (the A operands are register copies); the warpgroups take turns: one orders the
-// 128 rows by (label, row), and its thread that owns column c adds each label's run of rows in registers and then into
-// the CTA's shared-memory sums S[KP][DP], while the other goes on to the next tile.  Every sum is formed in a fixed order (deterministic, no atomics); the CTA
+// memory until its sums are formed (the A operands are register copies) while the producer fills the next tile's
+// slots.  All 8 consumer warps update every tile together: a counting sort orders the 128 rows by (label, row), and
+// each warp adds whole runs of equal labels (lane = 4 columns, one 16-byte unit of a row) in registers and then into
+// the CTA's shared-memory sums S[KP][DP].  Every sum is formed in a fixed order (deterministic, no atomics); the CTA
 // writes S to its partial slot when it ends.  For k or d > 128 (THREE = false) the sums ([256][256] f32 = 256 KB) do
 // not fit beside a tile in one CTA, so the kernel runs in clusters of WG_CL = 8 CTAs: after each step every CTA sums
 // the centres [32 r, 32 r + 32) over the 8 tiles of the cluster, reading the peers' labels and X rows through
@@ -35,9 +36,10 @@ constexpr int WG_SMEM_LIMIT = 227 * 1024;
 constexpr int WG_MISC = 7680;   // barriers, ||c||^2, ||x||^2, labels, flag counts, cost, row order, cluster row list
 constexpr int WG_M_CNORM = 256, WG_M_XN = 1280, WG_M_LAB = 1792, WG_M_FLAG = 2816, WG_M_COST = 2880, WG_M_SRT = 2944,
               WG_M_LIST = 3584;
-// THREE: barriers, ||c||^2 [KP], ||x||^2 [128] (NC) or the row order [128] (UPD) in one area, labels [2][128], cost
+// THREE: barriers, ||c||^2 [KP], ||x||^2 [128] (NC) or the row order [128] (UPD) in one area, per-warp label counts
+// [8][KP] u8 (UPD), cost
 constexpr int WG_MISC3 = 2368;
-constexpr int WG_M3_XN = 768, WG_M3_SRT = 768, WG_M3_LAB = 1280, WG_M3_COST = 2304;
+constexpr int WG_M3_XN = 768, WG_M3_SRT = 768, WG_M3_HIST = 1280, WG_M3_COST = 2304;
 constexpr int WG_CL = 8;   // THREE = false, UPD: CTAs per cluster; CTA r sums centres [r KP / 8, (r + 1) KP / 8)
 // PROF builds: per-warp cycle counters [grid][WG_NTHREADS / 32][WG_NPROF].  Each mark charges the cycles since the
 // previous mark to one phase, so a warp's counters sum to its whole run.  Consumer warps: X wait, centre wait, hand-off
@@ -60,7 +62,7 @@ struct WgCfg {
   static constexpr int FIXED = SUM_BYTES + MISC;
   static constexpr int XMIN = UPD ? NCH : 2;                            // UPD holds a whole tile until its update
   // THREE: the centres stay resident (all NCH chunks, loaded once per CTA) when the X ring still holds XRES slots: a
-  // Lloyd pass sums tile t while the next tile is multiplied, so it wants two tiles of slots
+  // Lloyd pass sums tile t while the next tile's slots fill, so it wants two tiles of slots
   static constexpr int XRES = UPD ? 2 * NCH : 2;
   static constexpr bool CRES = THREE && (WG_SMEM_LIMIT - FIXED - NCH * CSTAGE) / WG_XBYTES >= XRES;
   // else a ring of centre stages: two when the X ring still holds XMIN slots, else one
@@ -76,7 +78,10 @@ struct WgCfg {
   static constexpr int SMEM_BYTES = OFF_MISC + MISC;
   static_assert(SMEM_BYTES <= WG_SMEM_LIMIT, "smem");
   static_assert(!THREE || WG_M_CNORM + KP * 4 <= WG_M3_XN, "misc");
+  static_assert(!THREE || WG_M3_HIST + 8 * KP <= WG_M3_COST, "misc");
 };
+// BASELINE cfg2's Lloyd pass (k = 64, d = 128) keeps its centres resident: the fixed areas must leave it 8 X slots
+static_assert(WgCfg<64, 4, true, true>::CRES, "cfg2 centres no longer resident");
 
 struct WgArgs {
   int64_t n;
@@ -130,7 +135,8 @@ k_wg_assign(const __grid_constant__ CUtensorMap mapX, const __grid_constant__ CU
   const uint32_t bars = base + G::OFF_MISC;
   float* cnorm_s = reinterpret_cast<float*>(misc + WG_M_CNORM);
   float* xn_s = reinterpret_cast<float*>(misc + WG_M3_XN);                             // [128] ||x||^2 (THREE, NC)
-  int32_t* lab_s = reinterpret_cast<int32_t*>(misc + (THREE ? WG_M3_LAB : WG_M_LAB));   // [2][128] labels, -1 = deferred / invalid
+  int32_t* lab_s = reinterpret_cast<int32_t*>(misc + WG_M_LAB);   // THREE = false: [2][128] labels, -1 = deferred / invalid
+  uint8_t* hist_s = misc + WG_M3_HIST;                             // THREE && UPD: [8][KP] rows of each label per warp
   int32_t* flag_s = reinterpret_cast<int32_t*>(misc + WG_M_FLAG);                      // [2][8] deferred rows per warp
   double* cost_s = reinterpret_cast<double*>(misc + (THREE ? WG_M3_COST : WG_M_COST)); // [8]
   uint32_t* srt_s = reinterpret_cast<uint32_t*>(misc + (THREE ? WG_M3_SRT : WG_M_SRT)); // [128] (label << 16 | row) in (label, row) order
@@ -144,8 +150,6 @@ k_wg_assign(const __grid_constant__ CUtensorMap mapX, const __grid_constant__ CU
   constexpr bool CLU = UPD && !THREE;   // cluster update through distributed shared memory
   const uint32_t ready_bar = bars + 8u * (uint32_t)(2 * G::SX + 2 * G::SC);   // CLU: the cluster's labels of a step
   const uint32_t done_bar = ready_bar + 8u;                                     // CLU: the cluster has read my step
-  // THREE && UPD: labels of the tiles with parity p are written (by the warpgroup that does not sum them)
-  auto labfull = [&](int p) -> uint32_t { return bars + 8u * (uint32_t)(2 * G::SX + 2 * G::SC + p); };
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -167,8 +171,7 @@ k_wg_assign(const __grid_constant__ CUtensorMap mapX, const __grid_constant__ CU
   if (threadIdx.x == 0) {
     for (int s = 0; s < G::SX; ++s) {
       mbar_init(xfull(s), 1);
-      // every consumer warp releases the slot; THREE && UPD: the one warp that summed its 32 columns
-      mbar_init(xempty(s), THREE && UPD ? 1 : 8);
+      mbar_init(xempty(s), 8);   // every consumer warp releases the slot
     }
     for (int s = 0; s < G::SC; ++s) {
       mbar_init(cfull(s), 1);
@@ -177,10 +180,6 @@ k_wg_assign(const __grid_constant__ CUtensorMap mapX, const __grid_constant__ CU
     if constexpr (CLU) {
       mbar_init(ready_bar, WG_CL);
       mbar_init(done_bar, WG_CL);
-    }
-    if constexpr (THREE && UPD) {
-      mbar_init(labfull(0), 4);   // the 4 warps of the other warpgroup
-      mbar_init(labfull(1), 4);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
@@ -357,7 +356,6 @@ k_wg_assign(const __grid_constant__ CUtensorMap mapX, const __grid_constant__ CU
 
         // ---- epilogue: thread holds rows rr0 and rr0 + 8 of the tile, columns 8 a + 2 (lane & 3) + e ----
         const int rr0 = g * 64 + wi * 16 + (lane >> 2);
-        int32_t* lab = lab_s + (it & 1) * WG_TM;   // UPD: the tile's labels (two tiles may be in use, see below)
         if constexpr (NC) {
 #pragma unroll
           for (int i = 0; i < 4; ++i) {   // the 8 lanes of a row group hold one row's 8 float4 units
@@ -388,7 +386,6 @@ k_wg_assign(const __grid_constant__ CUtensorMap mapX, const __grid_constant__ CU
           }
           const int64_t grow = (int64_t)tile * WG_TM + rr0 + 8 * h;
           if ((lane & 3) == 0) {
-            if constexpr (UPD) lab[rr0 + 8 * h] = grow < args.n ? bj[h] : -1;
             if (grow < args.n) {
               if (args.labels_out != nullptr) args.labels_out[grow] = bj[h];
               if constexpr (NC) {
@@ -401,78 +398,126 @@ k_wg_assign(const __grid_constant__ CUtensorMap mapX, const __grid_constant__ CU
         }
         mark(WG_P_EPI);
         if constexpr (UPD) {
-          // ---- per-cluster sums of the tile, from its X chunks still in shared memory.  The warpgroups take turns:
-          // warpgroup u = it & 1 waits for the other one's labels and forms the sums, while the other goes straight on
-          // to the next tile's MMAs.  The sums of tile it + 1 are formed by the other warpgroup after it has the
-          // labels of tile it + 1, which u writes only after this update: the updates (and the row order buffer)
-          // stay in tile order, and labels of at most two tiles are in use. ----
-          const int u = it & 1;
-          if (g != u) {
-            __syncwarp();
-            if (lane == 0) mbar_arrive(labfull(u));   // this warp's labels of the tile are written
-          } else {
-            mbar_wait_nocall(labfull(u), (uint32_t)((it >> 1) & 1));   // the other warpgroup's labels
-            asm volatile("bar.sync %0, 128;" ::"r"(1 + g) : "memory");    // ... and this one's
-            mark(WG_P_HAND);
-            {   // rank of row t in (label, row) order; rows past n sort last
-              const int t = tw;
-              const int mine = lab[t] < 0 ? KP : lab[t];
-              int rank = 0;
-#pragma unroll 8
-              for (int r = 0; r < WG_TM; ++r) {
-                const int o = lab[r] < 0 ? KP : lab[r];
-                rank += (o < mine || (o == mine && r < t)) ? 1 : 0;
-              }
-              srt_s[rank] = ((uint32_t)(mine < KP ? mine : 0xffff) << 16) | (uint32_t)t;
+          // ---- per-cluster sums of the tile, from its X chunks still in shared memory, by all 8 consumer warps.  A
+          // counting sort puts the valid rows in (label, row) order; each warp then adds whole runs of equal labels.
+          // Rows past n take no part.  Every warp passes the first barrier of tile it + 1 only after its sums of tile
+          // it, so the read-modify-writes of a row of S stay in tile order, and the counts and the row order are
+          // rewritten only after every warp has read them. ----
+          // (1) this warp's rows 16 warp + 8 h + q are held by lanes 4 q + h (h < 2); per label: how many, and the
+          // rank of each row among them in row order
+          const int hq = lane & 3;
+          const int64_t grow0 = (int64_t)tile * WG_TM + rr0;
+          const uint32_t key = hq == 0   ? (grow0 < args.n ? (uint32_t)bj[0] : (uint32_t)KP)
+                               : hq == 1 ? (grow0 + 8 < args.n ? (uint32_t)bj[1] : (uint32_t)KP)
+                                         : 0x10000u + (uint32_t)lane;   // lanes 2, 3 of a quad match no other lane
+          const bool own = hq < 2 && key < (uint32_t)KP;
+          const uint32_t mk = __match_any_sync(0xffffffffu, key);
+          const uint32_t lt = (1u << lane) - 1u;
+          const int wr = hq == 0 ? __popc(mk & 0x11111111u & lt) : __popc(mk & 0x11111111u) + __popc(mk & 0x22222222u & lt);
+          uint8_t* hist = hist_s + warp * KP;
+          if (lane < KP / 4) reinterpret_cast<uint32_t*>(hist)[lane] = 0u;
+          __syncwarp();
+          if (own && wr == 0) hist[key] = (uint8_t)__popc(mk & 0x33333333u);
+          mark(WG_P_SORT);
+          asm volatile("bar.sync 3, 256;" ::: "memory");   // every warp's counts of the tile
+          mark(WG_P_HAND);
+          // (2) rank = rows of smaller labels + rows of the same label in lower warps + wr.  Lane j holds labels
+          // 4 j .. 4 j + 3 as packed bytes: no byte exceeds the 128 rows of a tile, so the packed sums do not carry.
+          uint32_t tot = 0u, pre = 0u;
+          if (lane < KP / 4) {
+#pragma unroll
+            for (int w = 0; w < 8; ++w) {
+              const uint32_t v = reinterpret_cast<const uint32_t*>(hist_s + w * KP)[lane];
+              tot += v;
+              if (w < warp) pre += v;
             }
-            mark(WG_P_SORT);
-            asm volatile("bar.sync %0, 128;" ::"r"(1 + g) : "memory");   // row order complete
-            mark(WG_P_HAND);
-            if (tw < DP) {
-              const int col = tw;
-              // column col of row r: X slot of chunk col / 32, 16-B unit (col % 32) / 4 swizzled by r % 8
-              const uint8_t* cbase = smem_raw + G::OFF_X + ((it * NCH + col / WG_CHUNK) % G::SX) * WG_XBYTES + (col % 4) * 4;
-              const uint32_t unit = (uint32_t)((col % WG_CHUNK) / 4);
-              int cur = -1, run = 0;
-              float a = 0.f;
-#pragma unroll 1
-              for (int i0 = 0; i0 < WG_TM; i0 += 8) {   // 8 rows' loads in flight, then the adds in order
-                uint32_t e[8];
-                float x[8];
-#pragma unroll
-                for (int v = 0; v < 8; ++v) e[v] = srt_s[i0 + v];
-#pragma unroll
-                for (int v = 0; v < 8; ++v) {
-                  const uint32_t r = e[v] & 0xffffu;
-                  x[v] = *reinterpret_cast<const float*>(cbase + r * 128u + ((unit ^ (r & 7u)) << 4));
-                }
-#pragma unroll
-                for (int v = 0; v < 8; ++v) {
-                  const int l = (int)(e[v] >> 16);
-                  if (l == 0xffff) continue;   // rows past n sort last
-                  if (l != cur) {
-                    if (cur >= 0) {
-                      sum_s[cur * DP + col] += a;
-                      if (col == 0) cnt_s[cur] += run;
-                    }
-                    cur = l;
-                    a = 0.f;
-                    run = 0;
-                  }
-                  a += x[v];
-                  ++run;
-                }
-              }
-              if (cur >= 0) {
-                sum_s[cur * DP + col] += a;
-                if (col == 0) cnt_s[cur] += run;
-              }
-            }
-            __syncwarp();
-            // warp wi summed columns [32 wi, 32 wi + 32): chunk wi of the tile is consumed
-            if (lane == 0 && wi < NCH) mbar_arrive(xempty((it * NCH + wi) % G::SX));
-            mark(WG_P_SUMS);
           }
+          const int lsum = (int)((tot * 0x01010101u) >> 24);
+          int incl = lsum;
+#pragma unroll
+          for (int o = 1; o < 32; o <<= 1) {
+            const int v = __shfl_up_sync(0xffffffffu, incl, o);
+            if (lane >= o) incl += v;
+          }
+          const int nv = __shfl_sync(0xffffffffu, incl, 31);   // valid rows of the tile
+          const uint32_t first = tot * 0x01010100u + (uint32_t)(incl - lsum) * 0x01010101u + pre;
+          const uint32_t fb = __shfl_sync(0xffffffffu, first, (int)(key >> 2) & 31);
+          if (own) srt_s[((fb >> (8 * (key & 3u))) & 0xffu) + (uint32_t)wr] = (key << 16) | (uint32_t)(rr0 + 8 * hq);
+          mark(WG_P_SORT);
+          asm volatile("bar.sync 3, 256;" ::: "memory");   // row order complete
+          mark(WG_P_HAND);
+          // (3) warp w adds the runs that start at sorted positions [16 w, 16 w + 16): positions [p0, p1)
+          int p0 = 128, p1 = 128;
+          {
+            const uint4 e4 = *reinterpret_cast<const uint4*>(srt_s + 4 * lane);   // positions 4 lane + i
+            const uint32_t ev[4] = {e4.x, e4.y, e4.z, e4.w};
+            uint32_t prev = __shfl_up_sync(0xffffffffu, e4.w >> 16, 1);
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+              const int p = 4 * lane + i;
+              const uint32_t l = ev[i] >> 16;
+              if (p < nv && (p == 0 || l != prev)) {
+                if (p >= 16 * warp && p0 == 128) p0 = p;
+                if (p >= 16 * warp + 16 && p1 == 128) p1 = p;
+              }
+              prev = l;
+            }
+            p0 = min(__reduce_min_sync(0xffffffffu, p0), nv);
+            p1 = min(__reduce_min_sync(0xffffffffu, p1), nv);
+          }
+          // lane owns columns 4 lane .. 4 lane + 3: 16-byte unit lane % 8 (swizzled by row % 8) of chunk lane / 8
+          const bool act = lane < DP / 4;
+          const uint8_t* xbase = smem_raw + G::OFF_X + ((it * NCH + (act ? lane >> 3 : 0)) % G::SX) * WG_XBYTES;
+          const uint32_t unit = (uint32_t)(lane & 7);
+          float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
+          int cur = -1, run = 0;
+          auto flush = [&]() {   // one run: S[cur] += a, count += run length
+            if (act) {
+              float4* sp = reinterpret_cast<float4*>(sum_s + cur * DP) + lane;
+              float4 s = *sp;
+              s.x += a.x;
+              s.y += a.y;
+              s.z += a.z;
+              s.w += a.w;
+              *sp = s;
+            }
+            if (lane == 0) cnt_s[cur] += run;
+          };
+#pragma unroll 1
+          for (int i0 = p0; i0 < p1; i0 += 8) {   // 8 rows' loads in flight, then the adds in row order
+            uint32_t e[8];
+            float4 x[8];
+#pragma unroll
+            for (int v = 0; v < 8; ++v) e[v] = i0 + v < p1 ? srt_s[i0 + v] : 0xffffffffu;
+#pragma unroll
+            for (int v = 0; v < 8; ++v) {
+              const uint32_t r = e[v] & 127u;
+              x[v] = *reinterpret_cast<const float4*>(xbase + r * 128u + ((unit ^ (r & 7u)) << 4));
+            }
+#pragma unroll
+            for (int v = 0; v < 8; ++v) {
+              if (e[v] == 0xffffffffu) break;
+              const int l = (int)(e[v] >> 16);
+              if (l != cur) {
+                if (cur >= 0) flush();
+                cur = l;
+                a = make_float4(0.f, 0.f, 0.f, 0.f);
+                run = 0;
+              }
+              a.x += x[v].x;
+              a.y += x[v].y;
+              a.z += x[v].z;
+              a.w += x[v].w;
+              ++run;
+            }
+          }
+          if (cur >= 0) flush();
+          __syncwarp();
+          if (lane == 0) {   // this warp no longer reads the tile's X slots
+#pragma unroll
+            for (int c = 0; c < NCH; ++c) mbar_arrive(xempty((it * NCH + c) % G::SX));
+          }
+          mark(WG_P_SUMS);
         }
       }
     } else {
