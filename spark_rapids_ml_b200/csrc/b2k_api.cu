@@ -206,11 +206,13 @@ struct LoopBuffers {
 // Chunked assignment for cluster counts beyond one fused pass: the centres are cut into chunks of exactly CH (the last
 // chunk is [k - CH, k): the overlap is harmless for a min), each chunk runs one fused assign pass that yields the min
 // distance and label of every row within the chunk, and k_merge_chunk keeps the smaller distance (strict '<': lowest
-// cluster index on ties).  d <= 128: CH = 128 through the 3xTF32 kernel (exact, no fix-up); 128 < d <= 256: CH = 256
-// through the large-shape kernel (1xTF32 screening + exact fix-up).  Used for k > 256 (assign passes, and Lloyd with the
-// generic label-driven update) and — d <= 128 only — for k > 128 when the caller expects near-ties (the k-means||
-// candidate passes: candidates drawn from one blob are almost equidistant from its rows, which is the worst case of
-// the screening kernel and free for the 3xTF32 one).  Replaces the SIMT assign of the generic path for d % 4 == 0.
+// cluster index on ties).  d <= 128: CH = 128, through the 3xTF32 kernel (exact, no fix-up) where it has a KP = 128
+// instantiation, i.e. 32 < d <= 128; at d <= 32 the chunks take the large-shape kernel (1xTF32 screening + exact fix-up),
+// as every fused pass with 64 < k <= 128 there does.  128 < d <= 256: CH = 256 through the large-shape kernel.  Used for
+// k > 256 (assign passes, and Lloyd with the generic label-driven update) and — d <= 128 only — for k > 128 when the
+// caller expects near-ties (the k-means|| candidate passes: candidates drawn from one blob are almost equidistant from
+// its rows, which is the worst case of the screening kernel and free for the 3xTF32 one).  Replaces the SIMT assign of
+// the generic path for d % 4 == 0.
 // ------------------------------------------------------------------------------------------------
 namespace {
 // The path of one assign pass and where it keeps its scratch (assign_layout)

@@ -214,10 +214,12 @@ def test_adaptive_path_leaves_the_screening_kernel_on_near_tie_data():
     (6000, 256, 600, "blobs"),      # 3 chunks, the last one overlapping the second ([344, 600))
     (5000, 64, 257, "uniform"),     # the smallest chunked k; DP = 128 instantiation
     (3000, 128, 1024, "blobs"),
+    (5000, 32, 300, "blobs"),       # d <= 32: no 3xTF32 instantiation has KP = 128, the chunks run on the screening kernel
 ])
 def test_assign_and_lloyd_beyond_256_clusters_run_in_chunks(n, d, k, gen):
-    """k > 256 (d <= 256): the assignment runs as chunks of 128 (d <= 128, 3xTF32 kernel) or 256 centres (large-shape
-    kernel) merged by min distance; Lloyd keeps the generic label-driven update.  Same parity rule as every other path."""
+    """k > 256 (d <= 256): the assignment runs as chunks of 128 (d <= 128: the 3xTF32 kernel, or the large-shape kernel at
+    d <= 32) or 256 centres (large-shape kernel) merged by min distance; Lloyd keeps the generic label-driven update.
+    Same parity rule as every other path."""
     from spark_rapids_ml_b200 import _native
 
     X = ko.make_blobs(n, d, k, seed=9)[0] if gen == "blobs" else ko.make_uniform(n, d, seed=9)
@@ -228,7 +230,7 @@ def test_assign_and_lloyd_beyond_256_clusters_run_in_chunks(n, d, k, gen):
         before = c.stats()["fused_tc_launches"]
         labels, md = c.kmeans_assign(_dev(X), _dev(C0), want_mindist=True)
         st = c.stats()
-        ch = 128 if d <= 128 else 256     # d <= 128: exact 3xTF32 chunks; else the large-shape kernel
+        ch = 128 if d <= 128 else 256     # d <= 128: 128-centre chunks; else 256-centre chunks of the large-shape kernel
         assert st["last_path"] == 2 and st["fused_tc_launches"] - before == -(-k // ch)
         cmp = ko.compare_labels(X, C0, labels.cpu().numpy(), tau=TAU)
         assert cmp["n_mismatch_outside_margin"] == 0, cmp

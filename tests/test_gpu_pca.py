@@ -123,7 +123,8 @@ def _check_against_oracle(X, out, k, ctx):
     assert np.abs(Y - Yr).max() <= 1e-5 * np.abs(Yr).max()
 
 
-@pytest.mark.parametrize("d", [20, 128, 512])
+# 132, 260, 1020: a ragged last 128-feature block (also in the off-diagonal tiles); 1024 = B2K_PCA_MAX_D, 36 tiles
+@pytest.mark.parametrize("d", [4, 20, 128, 132, 260, 512, 1020, 1024])
 @pytest.mark.parametrize("kind", ["random", "blobs"])
 @pytest.mark.parametrize("path", [0, 1])
 def test_fit_matches_oracle(d, kind, path):
