@@ -22,6 +22,8 @@
  *   b2k_pca_finalize            the eigen step inside the above (EXTERNAL cuML: eigendecomposition of the covariance,
  *                               sign flip, explained variance ratio, singular values)
  *   b2k_pca_transform           feature.py:398-451 (PCAMG.transform with injected components_, mean added back)
+ *   b2k_knn_search              knn.py:662-804 (NearestNeighborsMG(handle).kneighbors(...) and the row -> id mapping
+ *                               of NearestNeighborsModel.kneighbors' fit function)
  *
  * Conventions
  *   - Plain C, no exceptions across the boundary: every call returns a b2k_status; the message for the
@@ -211,6 +213,28 @@ int b2k_pca_finalize(const double* cov, int d, int64_t n_total, int k, double* c
  * PCAModel.  fp32 accumulation in feature order.  Asynchronous on `stream`. */
 int b2k_pca_transform(b2k_ctx* ctx, const float* X, int64_t n, int d, const float* components, int k, float* out,
                       uintptr_t stream);
+
+/* ---- exact k-NN (Euclidean) ----
+ * Stands in for knn.py:662-804 (NearestNeighborsModel.kneighbors' fit function: cuML NearestNeighborsMG.kneighbors
+ * over NCCL, then the row -> id mapping).
+ *   items      device f32 [n_items_local, d] row-major: this rank's part of the index
+ *   item_ids   device int64 [n_items_local] or NULL (ids = global rows: rank 0's rows in order, then rank 1's, ...)
+ *   queries    device f32 [n_queries_local, d]
+ *   outputs    device [n_queries_local][k]: distances_out f32 = sqrt of the exact fp32 sum_f (q_f - x_f)^2 in feature
+ *              order, ascending; indices_out int64 = ids.  Ties of the reported distance: lowest global row first.
+ * Search on all ranks' items for every rank's queries.  The pass runs on wgmma (3xTF32 screening distances, exact
+ * recompute of the survivors) when d % 4 == 0, 4 <= d <= 128, k <= 64 and the queries are 16-byte aligned, else on the
+ * generic SIMT kernel (exact fp32 distances); k > 1024: B2K_ERR_UNSUPPORTED.  Option "kernel_path" as for PCA.
+ * Errors, decided on the allgathered sizes so that every rank fails together: k < 1, k > n_items_total, no item on any
+ * rank, d differing between ranks.  Ranks with no items or no queries are legal.  Collective across the communicator
+ * when one is initialised (allgathers of the sizes, the queries and the candidate lists); synchronises `stream` once
+ * after the size allgather.  Bitwise reproducible for the same input, rank count and device.
+ * Stats: last_path = the search pass that ran; with option "time_kernels" != 0, last_finalize_ms = the index prep
+ * (wgmma path), last_fused_ms = the search pass, last_reduce_ms = refine + merge, last_allreduce_ms = both allgathers,
+ * last_loop_ms = the whole call after the size allgather (device times, CUDA events). */
+int b2k_knn_search(b2k_ctx* ctx, const float* items, int64_t n_items_local, const int64_t* item_ids,
+                   const float* queries, int64_t n_queries_local, int d, int k, float* distances_out,
+                   int64_t* indices_out, uintptr_t stream);
 
 #ifdef __cplusplus
 }

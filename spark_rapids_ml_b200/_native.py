@@ -54,6 +54,7 @@ EXPORTED_SYMBOLS = (
     "b2k_pca_fit",
     "b2k_pca_finalize",
     "b2k_pca_transform",
+    "b2k_knn_search",
 )
 
 
@@ -131,6 +132,7 @@ def load_library() -> ctypes.CDLL:
     L.b2k_pca_fit.argtypes = [vp, vp, i64, i32, i32, vp, vp, vp, vp, ctypes.c_size_t]
     L.b2k_pca_finalize.argtypes = [vp, i32, i64, i32, vp, vp, vp]
     L.b2k_pca_transform.argtypes = [vp, vp, i64, i32, vp, i32, vp, ctypes.c_size_t]
+    L.b2k_knn_search.argtypes = [vp, vp, i64, vp, vp, i64, i32, i32, vp, vp, ctypes.c_size_t]
     for name in EXPORTED_SYMBOLS:
         if name not in ("b2k_last_error",):
             getattr(L, name).restype = i32
@@ -400,3 +402,26 @@ class Context:
                                                   self._stream()))
         t.cuda.current_stream(self.device).synchronize()  # C (possibly a temporary) must outlive the kernel
         return out
+
+    def knn_search(self, items: Any, queries: Any, k: int, item_ids: Any = None) -> Tuple[Any, Any]:
+        """NearestNeighborsMG.kneighbors equivalent (collective when a communicator is initialised): the k nearest of all
+        ranks' items for each of this rank's queries.  items [n_items, d] and queries [n_q, d] are float32 CUDA tensors
+        (either may have 0 rows), item_ids an int64 CUDA tensor [n_items] or None (ids = global rows).  Returns CUDA
+        tensors distances float32 [n_q, k] (Euclidean, ascending) and indices int64 [n_q, k] (ids)."""
+        t = self._torch
+        n, d = self._check_X(items)
+        nq, dq = self._check_X(queries)
+        if dq != d:
+            raise ValueError(f"queries have {dq} features, items {d}")
+        if item_ids is not None:
+            if not (item_ids.is_cuda and item_ids.dtype == t.int64 and item_ids.is_contiguous()
+                    and tuple(item_ids.shape) == (n,)):
+                raise ValueError("item_ids must be a contiguous int64 CUDA tensor [n_items]")
+        kk = max(int(k), 0)
+        dist = t.empty((nq, kk), dtype=t.float32, device=self.device)
+        idx = t.empty((nq, kk), dtype=t.int64, device=self.device)
+        with t.cuda.device(self.device):
+            self._check(self._L.b2k_knn_search(
+                self._h, items.data_ptr(), n, item_ids.data_ptr() if item_ids is not None else None,
+                queries.data_ptr(), nq, d, int(k), dist.data_ptr(), idx.data_ptr(), self._stream()))
+        return dist, idx

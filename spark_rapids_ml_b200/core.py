@@ -282,6 +282,7 @@ class _CumlCaller(_CumlParams, _CumlCommon):
                 df = df.repartition(num_workers)   # core.py:771-772
             is_local = True   # the local frame runs on this host: partition id doubles as the GPU id (core.py:377-384)
         params: Dict[str, Any] = {param_alias.cuml_init: dict(self.cuml_params), param_alias.fit_multiple_params: None}
+        extra_cols = [c for c in (alias.label, alias.row_number) if c in df.columns]
         cuml_fit_func = self._get_cuml_fit_func(dataset, None)
         (enable_nccl, require_ucx) = self._require_nccl_ucx()
         cuml_verbose = self.cuml_params.get("verbose", False)
@@ -304,13 +305,18 @@ class _CumlCaller(_CumlParams, _CumlCommon):
             with CumlContext(partition_id, num_workers, context, enable_nccl, require_ucx, device=gpu_id) as cc:
                 appender = DeviceRowAppender(cc.handle, dimension)
                 sizes: List[int] = []
+                # label / row-number columns the pre-processed frame carries (kneighbors): host arrays, per batch
+                extra: Dict[str, List[np.ndarray]] = {c: [] for c in extra_cols}
                 for pdf in pdf_iter:
                     sizes.append(_features_from_pdf(pdf, multi_col_names, appender, logger))
+                    for c in extra_cols:
+                        extra[c].append(np.asarray(pdf[c].to_numpy(), dtype=np.int64))
                 if len(sizes) == 0 or all(sz == 0 for sz in sizes):
                     raise RuntimeError(
                         "A python worker received no data.  Please increase amount of data or use fewer workers.")
                 X = appender.finish()
-                inputs: FitInputType = [(X, None, None)]
+                slots = [np.concatenate(extra[c]) if c in extra else None for c in (alias.label, alias.row_number)]
+                inputs: FitInputType = [(X, slots[0], slots[1])]
                 params[param_alias.handle] = cc.handle
                 params[param_alias.part_sizes] = sizes
                 params[param_alias.num_cols] = dimension

@@ -954,3 +954,20 @@ extern "C" int b2k_pca_transform(b2k_ctx* ctx, const float* X, int64_t n, int d,
   B2K_CUDA_OK(ctx, cudaSetDevice(ctx->device));
   return b2k_pca_transform_impl(ctx, X, n, d, components, k, out, reinterpret_cast<cudaStream_t>(stream));
 }
+
+// ------------------------------------------------------------------------------------------------
+// exact k-NN (b2k_knn.cu)
+// ------------------------------------------------------------------------------------------------
+extern "C" int b2k_knn_search(b2k_ctx* ctx, const float* items, int64_t n_items_local, const int64_t* item_ids,
+                              const float* queries, int64_t n_queries_local, int d, int k, float* distances_out,
+                              int64_t* indices_out, uintptr_t stream) {
+  if (!ctx) return b2k_fail(nullptr, B2K_ERR_INVALID, "b2k_knn_search: ctx is NULL");
+  if (n_items_local < 0 || n_queries_local < 0 || d <= 0 || (n_items_local > 0 && !items) ||
+      (n_queries_local > 0 && (!queries || !distances_out || !indices_out)))
+    return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_knn_search: bad items/queries/outputs/n/d");
+  if (n_items_local > (int64_t)0x7fffff00)
+    return b2k_fail(ctx, B2K_ERR_UNSUPPORTED, "b2k_knn_search: more than 2^31 - 256 items on one rank");
+  B2K_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  return b2k_knn_search_impl(ctx, items, n_items_local, item_ids, queries, n_queries_local, d, k, distances_out,
+                             indices_out, reinterpret_cast<cudaStream_t>(stream));
+}

@@ -13,7 +13,7 @@ namespace {
 typedef struct ncclComm* ncclComm_t;
 typedef struct { char internal[128]; } ncclUniqueId;
 enum { ncclSuccess_ = 0 };
-enum { ncclInt64_ = 4, ncclUint64_ = 5, ncclFloat32_ = 7, ncclFloat64_ = 8 };  // ncclDataType_t
+enum { ncclUint8_ = 1, ncclInt64_ = 4, ncclUint64_ = 5, ncclFloat32_ = 7, ncclFloat64_ = 8 };  // ncclDataType_t
 enum { ncclSum_ = 0 };                                                        // ncclRedOp_t
 
 struct NcclApi {
@@ -159,5 +159,17 @@ int b2k_comm_allgather_i64(b2k_ctx* ctx, const int64_t* send_dev, int64_t* recv_
   }
   int rc = nccl_api()->AllGather(send_dev, recv_dev, count_per_rank, ncclInt64_, ctx->nccl->comm, s);
   if (rc != ncclSuccess_) return nccl_fail(ctx, "ncclAllGather(i64)", rc);
+  return B2K_OK;
+}
+
+int b2k_comm_allgather_bytes(b2k_ctx* ctx, const void* send_dev, void* recv_dev, size_t bytes_per_rank,
+                             cudaStream_t s) {
+  if (!ctx->nccl || ctx->nranks == 1) {
+    if (send_dev != recv_dev)
+      B2K_CUDA_OK(ctx, cudaMemcpyAsync(recv_dev, send_dev, bytes_per_rank, cudaMemcpyDeviceToDevice, s));
+    return B2K_OK;
+  }
+  int rc = nccl_api()->AllGather(send_dev, recv_dev, bytes_per_rank, ncclUint8_, ctx->nccl->comm, s);
+  if (rc != ncclSuccess_) return nccl_fail(ctx, "ncclAllGather(u8)", rc);
   return B2K_OK;
 }

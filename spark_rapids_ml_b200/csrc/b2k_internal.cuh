@@ -242,6 +242,8 @@ int b2k_comm_allreduce_f64(b2k_ctx* ctx, double* buf, size_t count, cudaStream_t
 int b2k_comm_allgather_i64(b2k_ctx* ctx, const int64_t* send_dev, int64_t* recv_dev, size_t count_per_rank,
                            cudaStream_t s);
 int b2k_comm_allreduce_f32(b2k_ctx* ctx, float* buf, size_t count, cudaStream_t s);
+// recv [nranks][bytes_per_rank] <- every rank's send; send may be recv's own slot (in place).  One rank: a copy.
+int b2k_comm_allgather_bytes(b2k_ctx* ctx, const void* send_dev, void* recv_dev, size_t bytes_per_rank, cudaStream_t s);
 
 // ingest — b2k_ingest.cu (entry point is the C ABI itself)
 
@@ -256,3 +258,11 @@ int b2k_pca_finalize_impl(b2k_ctx* ctx, const double* cov, int d, int64_t n_tota
                           double* evr_out, double* sv_out);
 int b2k_pca_transform_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, const float* C, int k, float* Y,
                            cudaStream_t s);
+
+// ------------------------------------------------------------------------------------------------
+// exact k-NN — b2k_knn.cu (the C ABI entry point in b2k_api.cu checks its arguments, then calls this)
+// ------------------------------------------------------------------------------------------------
+constexpr int B2K_KNN_MAX_K = 1024;   // the generic path's per-query lists; the wgmma path takes k <= 64
+int b2k_knn_search_impl(b2k_ctx* ctx, const float* items, int64_t n_items, const int64_t* item_ids,
+                        const float* queries, int64_t nq_local, int d, int k, float* dist_out, int64_t* idx_out,
+                        cudaStream_t s);

@@ -114,6 +114,22 @@ class HasInputCols(Params):
         return self.getOrDefault(self.inputCols)
 
 
+class HasIDCol(Params):
+    """reference: params.py:127-141 — the column that identifies each row (k-NN items and queries)."""
+
+    idCol = Param("parent", "idCol", "id column name.", TypeConverters.toString)
+
+    def getIdCol(self) -> Optional[str]:
+        return self.getOrDefault(self.idCol)
+
+
+class HasLabelCol(Params):
+    labelCol = Param("parent", "labelCol", "label column name.", TypeConverters.toString)
+
+    def getLabelCol(self) -> str:
+        return self.getOrDefault(self.labelCol)
+
+
 class HasOutputCol(Params):
     outputCol = Param("parent", "outputCol", "output column name.", TypeConverters.toString)
 

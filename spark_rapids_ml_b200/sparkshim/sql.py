@@ -85,7 +85,7 @@ class LocalSession:
                     c = [v.toArray().tolist() for v in c]
                 arrays.append(pa.array(c, type=t) if t is not None else pa.array(c))
             table = pa.Table.from_arrays(arrays, names=names)
-        return LocalDataFrame(self, _split_table(table, num_partitions, self.max_records_per_batch))
+        return LocalDataFrame(self, _split_table(table, num_partitions, self.max_records_per_batch), table.schema)
 
     def from_numpy(self, X: np.ndarray, col: str = "features", num_partitions: int = 1,
                    extra: Optional[Dict[str, np.ndarray]] = None) -> "LocalDataFrame":
@@ -279,6 +279,37 @@ class LocalDataFrame:
 
     def repartition(self, n: int) -> "LocalDataFrame":
         return self._derive(_split_table(self._table(), n, self.sparkSession.max_records_per_batch), self._schema)
+
+    def union(self, other: "LocalDataFrame") -> "LocalDataFrame":
+        """DataFrame.union: the rows of both, matched by column position (names from this frame), partitions of this frame
+        first.  The column counts and types must agree."""
+        a, b = self._schema, other._schema
+        if len(a) != len(b):
+            raise ValueError(f"union needs the same number of columns: {len(a)} vs {len(b)}")
+        for fa, fb in zip(a, b):
+            if fa.type != fb.type:
+                raise ValueError(f"union: column '{fa.name}' is {fa.type}, the other frame's '{fb.name}' is {fb.type}")
+        theirs = [[pa.RecordBatch.from_arrays(bt.columns, schema=a) for bt in p] for p in other._parts]
+        return self._derive(self._parts + theirs, a)
+
+    def with_constant_column(self, name: str, value: int) -> "LocalDataFrame":
+        """withColumn(name, lit(value)) for an integer literal (Spark types it int)."""
+        parts = [[b.append_column(name, pa.array(np.full(b.num_rows, value, dtype=np.int32))) for b in p]
+                 for p in self._parts]
+        return self._derive(parts, self._schema.append(pa.field(name, pa.int32())))
+
+    def with_monotonically_increasing_id(self, name: str) -> "LocalDataFrame":
+        """select(monotonically_increasing_id().alias(name), "*"): Spark's id, partition_id << 33 | row in partition."""
+        parts = []
+        for pid, p in enumerate(self._parts):
+            nb, row = [], 0
+            for b in p:
+                ids = (np.int64(pid) << np.int64(33)) + np.arange(row, row + b.num_rows, dtype=np.int64)
+                nb.append(pa.RecordBatch.from_arrays([pa.array(ids)] + list(b.columns),
+                                                     names=[name] + b.schema.names))
+                row += b.num_rows
+            parts.append(nb)
+        return self._derive(parts, pa.schema([pa.field(name, pa.int64())] + list(self._schema)))
 
     def with_appended_column(self, name: str, per_partition_arrays: List[List[pa.Array]]) -> "LocalDataFrame":
         parts = []
