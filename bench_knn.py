@@ -17,6 +17,7 @@ import time
 import numpy as np
 
 DATASHEET_TF32 = 495e12
+TAU_C = 4e-6   # the parity rule's tolerance TAU_C (||q - m||^2 + max ||x - m||^2), m = item mean (tests/knn_oracle.py)
 
 
 def card() -> dict:
@@ -97,14 +98,15 @@ def main() -> None:
             sq = Q[: args.sample].double()
             X64 = X.double()
             xn64 = (X64 * X64).sum(1)
-            xmax = float(xn64.max())
+            m = X64.mean(0)
+            r2 = float(((X64 - m) ** 2).sum(1).max())
             bad = 0
             for q0 in range(0, sq.shape[0], 100):
                 q = sq[q0:q0 + 100]
                 d2 = (q * q).sum(1)[:, None] + xn64[None, :] - 2.0 * (q @ X64.T)
                 ref = torch.topk(d2, k, dim=1, largest=False).values
                 mine = torch.gather(d2, 1, idx[q0:q0 + 100])
-                tau = 1e-6 * ((q * q).sum(1) + xmax)
+                tau = TAU_C * (((q - m) ** 2).sum(1) + r2)
                 bad += int(((torch.sort(mine, 1).values - ref).abs() > tau[:, None]).any(1).sum())
             del X64, d2
             res = {"k": k, "path": path,

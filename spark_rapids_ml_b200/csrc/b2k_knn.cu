@@ -4,13 +4,15 @@
 //   queries allgather of every rank's queries, padded to the largest count: Q [nranks * nq_max][d].
 //   search  over the local index for every query, in work units = (tile of queries, index split):
 //             wgmma path (k_knn_wg, 3xTF32): d % 4 == 0, 4 <= d <= 128, k <= 64, 16-byte aligned queries;
-//               k_knn_prep writes the index as zero-padded tf32 hi/lo planes [n_pad][DP] and ||x||^2 (+inf padding).
-//               Screening distance ||x||^2 - 2 q.x; each row keeps its k best (screen, local row) in shared memory.
+//               everything in the frame of s = local item row 0 (non-finite components -> 0): k_knn_prep writes the
+//               index as zero-padded tf32 hi/lo planes of x - s [n_pad][DP] and ||x - s||^2 (+inf padding),
+//               k_knn_shift_q writes Qs = Q - s [nq][d].  Screening distance ||x - s||^2 - 2 (q - s).(x - s); each
+//               row keeps its k best (screen, local row) in shared memory.
 //             generic path (k_knn_generic, SIMT): every other shape with k <= 1024; direct sum (q - x)^2.
 //           Each unit writes its rows' lists to part [S][nq_all][k].
 //   refine  k_knn_refine: per query, merge the S lists in split order, recompute the exact fp32 distance
-//           sum_f (q_f - x_f)^2 (feature order) of the k survivors, re-sort by (exact distance, global row), map rows
-//           to ids -> cand [nq_all][k].
+//           sum_f (q_f - x_f)^2 (feature order, from the caller's unshifted rows) of the k survivors, re-sort by
+//           (exact distance, global row), map rows to ids -> cand [nq_all][k].
 //   gather  allgather of cand; k_knn_merge merges each own query's nranks lists in rank order -> sqrt(distance), id.
 // Nothing uses atomics: two calls with the same input, rank count and device are bitwise equal.
 #include <algorithm>
@@ -81,6 +83,15 @@ struct KnnArgs {
   int2* part;                // [S][nq][k] (screen distance bits, local row)
 };
 
+// The wgmma pass screens in the frame of the shift point s = item row 0 with every non-finite component replaced by 0
+// (a NaN or inf there would otherwise reach every item): the screen ||x - s||^2 - 2 (q - s).(x - s) orders the items as
+// ||q - x||^2 does, and its fp32 rounding scales with the data's spread rather than its distance from the origin.
+__device__ __forceinline__ float knn_shift(const float* __restrict__ X, int f) {
+  const float v = X[f];
+  return isfinite(v) ? v : 0.f;
+}
+
+// index planes of x - s (rounded once to fp32), zero-padded to [n_pad][DP], and ||x - s||^2 of those same values
 __global__ void __launch_bounds__(256) k_knn_prep(const float* __restrict__ X, int64_t n, int d, int64_t n_pad, int DP,
                                                   float* __restrict__ Xhi, float* __restrict__ Xlo,
                                                   float* __restrict__ norms) {
@@ -89,7 +100,7 @@ __global__ void __launch_bounds__(256) k_knn_prep(const float* __restrict__ X, i
   if (row >= n_pad) return;
   double s = 0.0;
   for (int t = lane; t < DP; t += 32) {
-    const float v = (row < n && t < d) ? X[row * d + t] : 0.f;
+    const float v = (row < n && t < d) ? X[row * d + t] - knn_shift(X, t) : 0.f;
     const uint32_t hb = rn_tf32_bits(v);
     Xhi[row * DP + t] = __uint_as_float(hb);
     Xlo[row * DP + t] = __uint_as_float(rn_tf32_bits(v - __uint_as_float(hb)));
@@ -100,12 +111,31 @@ __global__ void __launch_bounds__(256) k_knn_prep(const float* __restrict__ X, i
   if (lane == 0) norms[row] = row < n ? (float)s : __int_as_float(0x7f800000);
 }
 
+// q - s as the wgmma pass reads it.  rn_tf32_bits carries out of the mantissa for NaNs whose payload fills its top bits,
+// so the device's canonical NaN 0x7fffffff would split into hi = lo = -0 and a NaN query would be screened as finite;
+// 0x7fc00000 stays NaN as hi.  (An item needs no such care: its NaN norm makes its screen NaN.)
+__device__ __forceinline__ float knn_shifted_q(float q, float s) {
+  const float v = q - s;
+  return isnan(v) ? __int_as_float(0x7fc00000) : v;
+}
+
+// Qs = Q - s for the wgmma pass, [nq][d] with d % 4 == 0 and both buffers 16-byte aligned
+__global__ void __launch_bounds__(256) k_knn_shift_q(const float4* __restrict__ Q, int64_t n4, int d,
+                                                     const float* __restrict__ X, float4* __restrict__ Qs) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x) {
+    const int f = (int)(i * 4 % d);
+    const float4 q = Q[i];
+    Qs[i] = make_float4(knn_shifted_q(q.x, knn_shift(X, f)), knn_shifted_q(q.y, knn_shift(X, f + 1)),
+                        knn_shifted_q(q.z, knn_shift(X, f + 2)), knn_shifted_q(q.w, knn_shift(X, f + 3)));
+  }
+}
+
 // Persistent grid, static round-robin over units u = tile * S + split.  Warp 8 issues TMA: the unit's query tile
 // (NCH chunks, once per unit) and the split's index blocks, chunk by chunk, hi and lo planes into a ring of SC stages.
 // Consumer warpgroup g owns queries [64 g, 64 g + 64) of the tile; per block it accumulates lo.Xhi^T + hi.Xlo^T +
-// hi.Xhi^T (A = the query split in registers, as the 3xTF32 branch of k_wg_assign) into D[64 x 128].  The epilogue
-// screens ||x||^2 - 2 q.x against each row's current k-th best (a register threshold replicated over the row's quad);
-// the quad's lanes insert the candidates under it in turn.
+// hi.Xhi^T (A = the query split in registers, as the 3xTF32 branch of k_wg_assign) into D[64 x 128].  Q, X and the
+// norms all come shifted by s.  The epilogue screens ||x - s||^2 - 2 (q - s).(x - s) against each row's current k-th
+// best (a register threshold replicated over the row's quad); the quad's lanes insert the candidates under it in turn.
 template <int NCH>
 __global__ void __launch_bounds__(KW_NTHREADS, 1)
 k_knn_wg(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapHi,
@@ -555,13 +585,14 @@ int b2k_knn_search_impl(b2k_ctx* ctx, const float* items, int64_t n_items, const
   const int S = n_items == 0 ? 0
                              : (int)std::max<int64_t>(1, std::min<int64_t>({(2 * sm + ntiles - 1) / ntiles, item_tiles,
                                                                              (int64_t)KW_SMAX}));
-  float *Qall = nullptr, *Xhi = nullptr, *Xlo = nullptr, *norms = nullptr;
+  float *Qall = nullptr, *Qs = nullptr, *Xhi = nullptr, *Xlo = nullptr, *norms = nullptr;
   int2* part = nullptr;
   KnnCand *cand = nullptr, *cand_all = nullptr;
   B2K_TRY(b2k_scratch_layout(ctx, "kNN", [&](B2kLayout& L) -> int {
     sz_dev = L.take<int64_t>((size_t)3 * (nr + 1));
     if (nr > 1) Qall = L.take<float>((size_t)nq_all * d, 1024);
     if (wg && n_items > 0) {
+      Qs = L.take<float>((size_t)nq_all * d, 1024);
       Xhi = L.take<float>((size_t)n_pad * DP, 1024);
       Xlo = L.take<float>((size_t)n_pad * DP, 1024);
       norms = L.take<float>((size_t)n_pad);
@@ -589,12 +620,16 @@ int b2k_knn_search_impl(b2k_ctx* ctx, const float* items, int64_t n_items, const
     if (wg) {
       k_knn_prep<<<(unsigned)((n_pad * 32 + 255) / 256), 256, 0, s>>>(items, n_items, d, n_pad, DP, Xhi, Xlo, norms);
       B2K_CUDA_OK(ctx, cudaGetLastError());
-      ctx->stats.kernel_launches++;
+      const int64_t n4 = nq_all * d / 4;
+      k_knn_shift_q<<<(unsigned)std::min<int64_t>((n4 + 255) / 256, (int64_t)ctx->sm_count * 16), 256, 0, s>>>(
+          reinterpret_cast<const float4*>(Q), n4, d, items, reinterpret_cast<float4*>(Qs));
+      B2K_CUDA_OK(ctx, cudaGetLastError());
+      ctx->stats.kernel_launches += 2;
     }
     tm.mark(2, s);
     if (wg) {
       CUtensorMap mq, mh, ml;
-      B2K_TRY(b2k_encode_2d(ctx, &mq, Q, (uint64_t)d, (uint64_t)nq_all, (uint64_t)d * 4, KW_CHUNK, KW_TM,
+      B2K_TRY(b2k_encode_2d(ctx, &mq, Qs, (uint64_t)d, (uint64_t)nq_all, (uint64_t)d * 4, KW_CHUNK, KW_TM,
                             CU_TENSOR_MAP_L2_PROMOTION_L2_256B));
       B2K_TRY(b2k_encode_2d(ctx, &mh, Xhi, (uint64_t)DP, (uint64_t)n_pad, (uint64_t)DP * 4, KW_CHUNK, KW_N,
                             CU_TENSOR_MAP_L2_PROMOTION_L2_256B));
