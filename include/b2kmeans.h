@@ -24,6 +24,9 @@
  *   b2k_pca_transform           feature.py:398-451 (PCAMG.transform with injected components_, mean added back)
  *   b2k_knn_search              knn.py:662-804 (NearestNeighborsMG(handle).kneighbors(...) and the row -> id mapping
  *                               of NearestNeighborsModel.kneighbors' fit function)
+ *   b2k_linreg_moments          regression.py:546-607 (the passes over the data of LinearRegressionMG / RidgeMG / CDMG)
+ *   b2k_linreg_solve            the solvers inside them (normal equations, coordinate descent) and the rescaling
+ *   b2k_linreg_predict          regression.py:800-862 (LinearRegressionModel's transform: cuML predict)
  *
  * Conventions
  *   - Plain C, no exceptions across the boundary: every call returns a b2k_status; the message for the
@@ -235,6 +238,45 @@ int b2k_pca_transform(b2k_ctx* ctx, const float* X, int64_t n, int d, const floa
 int b2k_knn_search(b2k_ctx* ctx, const float* items, int64_t n_items_local, const int64_t* item_ids,
                    const float* queries, int64_t n_queries_local, int d, int k, float* distances_out,
                    int64_t* indices_out, uintptr_t stream);
+
+/* ---- linear regression (squared loss: OLS, ridge, lasso, elastic net) ----
+ * Stands in for regression.py:546-607 (LinearRegressionMG / RidgeMG / CDMG on the standardized data, then the
+ * coefficients scaled back).  Every fit needs only the centred second moments of [X | y], so one moments pass serves
+ * any number of solver settings.
+ *
+ * moments (collective): X device f32 [n_local, d], y device f32 [n_local], 1 <= d <= 1024 (d > 1024:
+ * B2K_ERR_UNSUPPORTED).  Host outputs: *n_total_out = rows over all ranks; mean_out [d + 1] = fp64 means of [X | y];
+ * moments_out [d + 1][d + 1] = sum (v - mean)(v - mean)^T over the rows v = [x | y], fp64.  Column sums of X and of y,
+ * then the Gram pass of PCA on X (wgmma or generic, chosen as for b2k_pca_fit, option "kernel_path" likewise) and k_xty
+ * for X^T y and y^T y, all centred on the fp32 means; the host removes that offset exactly.  Errors, decided on
+ * allreduced values so that every rank fails together: an empty partition on any rank; a NaN or an infinity in X or y
+ * (B2K_ERR_INVALID).  Synchronises `stream`.  Bitwise reproducible for the same input, rank count and device.
+ * Stats: last_path = the Gram pass that ran; with option "time_kernels" != 0, last_reduce_ms = the column-sum pass,
+ * last_fused_ms = the Gram pass, last_finalize_ms = the k_xty pass, last_allreduce_ms = both allreduces (device times)
+ * and last_loop_ms = the whole call (host clock). */
+int b2k_linreg_moments(b2k_ctx* ctx, const float* X, const float* y, int64_t n_local, int d, int64_t* n_total_out,
+                       double* mean_out, double* moments_out, uintptr_t stream);
+/* The solver, on the host (no context, no device), from the outputs of b2k_linreg_moments.  With mu = mean[0..d),
+ * muy = mean[d], population standard deviations sigma_j = sqrt(moments[j][j] / n_total) (sigma_y likewise):
+ *   centring   fit_intercept: mu, muy; else 0 and 0 (scaled, not centred)
+ *   scales     standardization: s_j = sigma_j (1 where sigma_j = 0), s_y = sigma_y; else 1
+ *   problem    z = (x - mu) / s, t = (y - muy) / s_y, lambda' = reg / s_y; minimise
+ *              (1/2n) sum (t - z.v)^2 + lambda' (l1_ratio |v|_1 + (1 - l1_ratio)/2 |v|^2)
+ *   result     coef_out [d] = v_j s_y / s_j; *intercept_out = muy - coef.mu with an intercept, else 0
+ * reg == 0 or l1_ratio == 0: Cholesky of A + lambda' (1 - l1_ratio) I (A = Z^T Z / n); when a pivot is <= d 2^-52 max
+ * diag, the minimum-norm solution of its eigendecomposition (eigenvalues <= d 2^-52 lambda_max count as 0); *n_iter_out
+ * = 0.  Otherwise cyclic coordinate descent from v = 0 in feature order, soft-thresholding at lambda' l1_ratio, stopped
+ * after a sweep with max |dv| <= tol max |v| or after max_iter sweeps; *n_iter_out = the sweeps.  A constant label under
+ * standardization: coef = 0 and intercept = muy (0 without an intercept) when fit_intercept or muy == 0, else s_y = |muy|.
+ * Errors (B2K_ERR_INVALID, through b2k_last_error(NULL)): reg < 0, l1_ratio outside [0, 1], max_iter < 0, tol < 0,
+ * n_total < 1, non-finite inputs; d > 1024: B2K_ERR_UNSUPPORTED.  n_iter_out may be NULL. */
+int b2k_linreg_solve(const double* mean, const double* moments, int d, int64_t n_total, double reg, double l1_ratio,
+                     int fit_intercept, int standardization, int max_iter, double tol, double* coef_out,
+                     double* intercept_out, int* n_iter_out);
+/* out [n] f64 = intercept + sum_j X[i][j] coef[j] (coef device f64 [d]), accumulated in fp64 in an order fixed by d
+ * alone.  Asynchronous on `stream`. */
+int b2k_linreg_predict(b2k_ctx* ctx, const float* X, int64_t n, int d, const double* coef, double intercept, double* out,
+                       uintptr_t stream);
 
 #ifdef __cplusplus
 }

@@ -55,6 +55,9 @@ EXPORTED_SYMBOLS = (
     "b2k_pca_finalize",
     "b2k_pca_transform",
     "b2k_knn_search",
+    "b2k_linreg_moments",
+    "b2k_linreg_solve",
+    "b2k_linreg_predict",
 )
 
 
@@ -133,6 +136,10 @@ def load_library() -> ctypes.CDLL:
     L.b2k_pca_finalize.argtypes = [vp, i32, i64, i32, vp, vp, vp]
     L.b2k_pca_transform.argtypes = [vp, vp, i64, i32, vp, i32, vp, ctypes.c_size_t]
     L.b2k_knn_search.argtypes = [vp, vp, i64, vp, vp, i64, i32, i32, vp, vp, ctypes.c_size_t]
+    L.b2k_linreg_moments.argtypes = [vp, vp, vp, i64, i32, ctypes.POINTER(i64), vp, vp, ctypes.c_size_t]
+    L.b2k_linreg_solve.argtypes = [vp, vp, i32, i64, f64, f64, i32, i32, i32, f64, vp, ctypes.POINTER(f64),
+                                   ctypes.POINTER(i32)]
+    L.b2k_linreg_predict.argtypes = [vp, vp, i64, i32, vp, f64, vp, ctypes.c_size_t]
     for name in EXPORTED_SYMBOLS:
         if name not in ("b2k_last_error",):
             getattr(L, name).restype = i32
@@ -166,6 +173,28 @@ def pca_finalize(cov: np.ndarray, n_total: int, k: int) -> Dict[str, np.ndarray]
     if rc != B2K_OK:
         raise B2KError(rc, (L.b2k_last_error(None) or b"").decode())
     return {"components_": comp, "explained_variance_ratio_": evr, "singular_values_": sv}
+
+
+def linreg_solve(mean: np.ndarray, moments: np.ndarray, n_total: int, reg: float = 0.0, l1_ratio: float = 0.0,
+                 fit_intercept: bool = True, standardization: bool = True, max_iter: int = 100,
+                 tol: float = 1e-6) -> Tuple[np.ndarray, float, int]:
+    """b2k_linreg_solve (host only): the fit from the outputs of Context.linreg_moments -> (coef [d] float64,
+    intercept, coordinate-descent sweeps)."""
+    L = load_library()
+    mean = np.ascontiguousarray(mean, dtype=np.float64)
+    moments = np.ascontiguousarray(moments, dtype=np.float64)
+    d = int(mean.shape[0]) - 1
+    if mean.ndim != 1 or moments.shape != (d + 1, d + 1):
+        raise ValueError("mean must be [d + 1] and moments [d + 1, d + 1]")
+    coef = np.zeros(max(d, 0), dtype=np.float64)
+    b = ctypes.c_double(0.0)
+    it = ctypes.c_int(0)
+    rc = L.b2k_linreg_solve(mean.ctypes.data, moments.ctypes.data, d, int(n_total), float(reg), float(l1_ratio),
+                            int(bool(fit_intercept)), int(bool(standardization)), int(max_iter), float(tol),
+                            coef.ctypes.data, ctypes.byref(b), ctypes.byref(it))
+    if rc != B2K_OK:
+        raise B2KError(rc, (L.b2k_last_error(None) or b"").decode())
+    return coef, float(b.value), int(it.value)
 
 
 def _stream_handle(torch_mod: Any, device: Any) -> int:
@@ -425,3 +454,33 @@ class Context:
                 self._h, items.data_ptr(), n, item_ids.data_ptr() if item_ids is not None else None,
                 queries.data_ptr(), nq, d, int(k), dist.data_ptr(), idx.data_ptr(), self._stream()))
         return dist, idx
+
+    def linreg_moments(self, X: Any, y: Any) -> Tuple[int, np.ndarray, np.ndarray]:
+        """The passes over the data of a linear regression fit (collective when a communicator is initialised): X [n, d]
+        and y [n] float32 CUDA tensors -> (n_total, mean [d + 1], centred moments [d + 1, d + 1] of [X | y]), host
+        float64."""
+        t = self._torch
+        n, d = self._check_X(X)
+        if not (y.is_cuda and y.dtype == t.float32 and y.is_contiguous() and tuple(y.shape) == (n,)):
+            raise ValueError(f"y must be a contiguous float32 CUDA tensor [{n}]")
+        n_total = ctypes.c_int64(0)
+        mean = np.zeros(d + 1, dtype=np.float64)
+        mom = np.zeros((d + 1, d + 1), dtype=np.float64)
+        with t.cuda.device(self.device):
+            self._check(self._L.b2k_linreg_moments(self._h, X.data_ptr(), y.data_ptr(), n, d, ctypes.byref(n_total),
+                                                   mean.ctypes.data, mom.ctypes.data, self._stream()))
+        return int(n_total.value), mean, mom
+
+    def linreg_predict(self, X: Any, coef: Any, intercept: float) -> Any:
+        """intercept + X . coef, accumulated in fp64 -> float64 CUDA tensor [n]."""
+        t = self._torch
+        n, d = self._check_X(X)
+        w = t.as_tensor(coef, dtype=t.float64, device=self.device).contiguous()
+        if tuple(w.shape) != (d,):
+            raise ValueError(f"coef must be [{d}]")
+        out = t.empty((n,), dtype=t.float64, device=self.device)
+        with t.cuda.device(self.device):
+            self._check(self._L.b2k_linreg_predict(self._h, X.data_ptr(), n, d, w.data_ptr(), float(intercept),
+                                                   out.data_ptr(), self._stream()))
+        t.cuda.current_stream(self.device).synchronize()  # w (possibly a temporary) must outlive the kernel
+        return out

@@ -213,6 +213,12 @@ class _CumlCaller(_CumlParams, _CumlCommon):
     def _fit_array_order(self) -> str:
         return "C"
 
+    def _fit_label_col(self) -> Optional[str]:
+        """The label column of a supervised estimator: the pre-processed frame carries it as alias.label, and the fit
+        function receives it in slot 2 as a float32 device vector.  None: slot 2 is whatever alias.label the frame
+        carries (kneighbors' item / query tags), as int64 host values."""
+        return None
+
     def _validate_parameters(self) -> None:
         """reference round-trips the params through the JVM estimator (core.py:579-602); without a JVM the
         same constraints are checked here."""
@@ -283,6 +289,7 @@ class _CumlCaller(_CumlParams, _CumlCommon):
             is_local = True   # the local frame runs on this host: partition id doubles as the GPU id (core.py:377-384)
         params: Dict[str, Any] = {param_alias.cuml_init: dict(self.cuml_params), param_alias.fit_multiple_params: None}
         extra_cols = [c for c in (alias.label, alias.row_number) if c in df.columns]
+        float_label = self._fit_label_col() is not None
         cuml_fit_func = self._get_cuml_fit_func(dataset, None)
         (enable_nccl, require_ucx) = self._require_nccl_ucx()
         cuml_verbose = self.cuml_params.get("verbose", False)
@@ -310,12 +317,19 @@ class _CumlCaller(_CumlParams, _CumlCommon):
                 for pdf in pdf_iter:
                     sizes.append(_features_from_pdf(pdf, multi_col_names, appender, logger))
                     for c in extra_cols:
-                        extra[c].append(np.asarray(pdf[c].to_numpy(), dtype=np.int64))
+                        if float_label and c == alias.label:
+                            extra[c].append(np.asarray(pdf[c].to_numpy(), dtype=np.float32))
+                        else:
+                            extra[c].append(np.asarray(pdf[c].to_numpy(), dtype=np.int64))
                 if len(sizes) == 0 or all(sz == 0 for sz in sizes):
                     raise RuntimeError(
                         "A python worker received no data.  Please increase amount of data or use fewer workers.")
                 X = appender.finish()
                 slots = [np.concatenate(extra[c]) if c in extra else None for c in (alias.label, alias.row_number)]
+                if float_label:
+                    import torch
+
+                    slots[0] = torch.from_numpy(slots[0]).to(X.device)
                 inputs: FitInputType = [(X, slots[0], slots[1])]
                 params[param_alias.handle] = cc.handle
                 params[param_alias.part_sizes] = sizes

@@ -971,3 +971,34 @@ extern "C" int b2k_knn_search(b2k_ctx* ctx, const float* items, int64_t n_items_
   return b2k_knn_search_impl(ctx, items, n_items_local, item_ids, queries, n_queries_local, d, k, distances_out,
                              indices_out, reinterpret_cast<cudaStream_t>(stream));
 }
+
+// ------------------------------------------------------------------------------------------------
+// linear regression (b2k_linreg.cu)
+// ------------------------------------------------------------------------------------------------
+extern "C" int b2k_linreg_moments(b2k_ctx* ctx, const float* X, const float* y, int64_t n_local, int d,
+                                  int64_t* n_total_out, double* mean_out, double* moments_out, uintptr_t stream) {
+  if (!ctx) return b2k_fail(nullptr, B2K_ERR_INVALID, "b2k_linreg_moments: ctx is NULL");
+  if (!X || !y || n_local < 0 || d <= 0) return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_linreg_moments: bad X/y/n/d");
+  if (!n_total_out || !mean_out || !moments_out)
+    return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_linreg_moments: NULL output");
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  B2K_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  B2K_TRY(check_no_empty_partition(ctx, "b2k_linreg_moments", n_local, s));
+  return b2k_linreg_moments_impl(ctx, X, y, n_local, d, n_total_out, mean_out, moments_out, s);
+}
+
+extern "C" int b2k_linreg_solve(const double* mean, const double* moments, int d, int64_t n_total, double reg,
+                                double l1_ratio, int fit_intercept, int standardization, int max_iter, double tol,
+                                double* coef_out, double* intercept_out, int* n_iter_out) {
+  return b2k_linreg_solve_impl(mean, moments, d, n_total, reg, l1_ratio, fit_intercept, standardization, max_iter, tol,
+                               coef_out, intercept_out, n_iter_out);
+}
+
+extern "C" int b2k_linreg_predict(b2k_ctx* ctx, const float* X, int64_t n, int d, const double* coef, double intercept,
+                                  double* out, uintptr_t stream) {
+  if (!ctx) return b2k_fail(nullptr, B2K_ERR_INVALID, "b2k_linreg_predict: ctx is NULL");
+  if (!X || !coef || !out || n < 0 || d <= 0)
+    return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_linreg_predict: bad X/coef/out/n/d");
+  B2K_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  return b2k_linreg_predict_impl(ctx, X, n, d, coef, intercept, out, reinterpret_cast<cudaStream_t>(stream));
+}

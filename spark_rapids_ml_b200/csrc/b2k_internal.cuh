@@ -5,6 +5,7 @@
 #include <stdint.h>
 
 #include <string>
+#include <vector>
 
 #include "../../include/b2kmeans.h"
 
@@ -251,6 +252,21 @@ int b2k_comm_allgather_bytes(b2k_ctx* ctx, const void* send_dev, void* recv_dev,
 // PCA — b2k_pca.cu (the C ABI entry points in b2k_api.cu check their arguments and the partitions, then call these)
 // ------------------------------------------------------------------------------------------------
 constexpr int B2K_PCA_MAX_D = 1024;   // both Gram paths, the projection kernel and the host eigen step
+// The passes PCA and linear regression share (collective): column sums, then the Gram matrix of X centred on the fp32
+// means mu32 = fl32(mu), on the path kernel_path selects.  With a label y [n] (else NULL), also the label's sum and, by
+// k_xty (b2k_linreg.cu), sum (x - mu32) (y - muy32) and sum (y - muy32)^2.  The offsets are left for the caller to
+// remove exactly with delta.  Fails with B2K_ERR_INVALID, on every rank alike, when fewer than min_rows rows exist.
+struct B2kMoments {
+  int64_t n_total = 0;
+  std::vector<double> mu;      // [d] (+ [1] label) means, fp64
+  std::vector<double> delta;   // mu - fl32(mu)
+  std::vector<double> G;       // [d][d] Gram about mu32 (+ [d] X^T y, [1] y^T y about (mu32, muy32)), allreduced
+};
+int b2k_moments_impl(b2k_ctx* ctx, const char* who, const float* X, const float* y, int64_t n, int d, int64_t min_rows,
+                     B2kMoments* m, cudaStream_t s);
+// Symmetric eigendecomposition (Householder + implicit QL): A = Z^T diag(w) Z, rows of Z the eigenvectors; A is
+// destroyed.  False if an eigenvalue needs more than 60 QL sweeps.
+bool b2k_sym_eig(std::vector<double>& A, int n, std::vector<double>& w, std::vector<double>& Z);
 int b2k_pca_fit_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, int k, double* mean_out, double* components_out,
                      double* evr_out, double* sv_out, cudaStream_t s);
 // ctx may be NULL (b2k_pca_finalize): errors then go to b2k_last_error(NULL)
@@ -266,3 +282,20 @@ constexpr int B2K_KNN_MAX_K = 1024;   // the generic path's per-query lists; the
 int b2k_knn_search_impl(b2k_ctx* ctx, const float* items, int64_t n_items, const int64_t* item_ids,
                         const float* queries, int64_t nq_local, int d, int k, float* dist_out, int64_t* idx_out,
                         cudaStream_t s);
+
+// ------------------------------------------------------------------------------------------------
+// linear regression — b2k_linreg.cu (the C ABI entry points in b2k_api.cu check their arguments, then call these)
+// ------------------------------------------------------------------------------------------------
+constexpr int B2K_LINREG_MAX_D = B2K_PCA_MAX_D;   // the moments ride on PCA's Gram passes
+// row spans of k_xty's fp64 partials for (n, d): the caller lays out spans * (d + 1) doubles for b2k_launch_xty
+int b2k_xty_spans(const b2k_ctx* ctx, int64_t n, int d);
+// out [d + 1] = [sum (x - mu32) (y - muy32) | sum (y - muy32)^2], fp64, folded over the spans in order
+int b2k_launch_xty(b2k_ctx* ctx, const float* X, const float* y, int64_t n, int d, const float* mu32, float muy32,
+                   int spans, double* part, double* out, cudaStream_t s);
+int b2k_linreg_moments_impl(b2k_ctx* ctx, const float* X, const float* y, int64_t n, int d, int64_t* n_total_out,
+                            double* mean_out, double* moments_out, cudaStream_t s);
+int b2k_linreg_solve_impl(const double* mean, const double* moments, int d, int64_t n_total, double reg,
+                          double l1_ratio, int fit_intercept, int standardization, int max_iter, double tol,
+                          double* coef_out, double* intercept_out, int* n_iter_out);
+int b2k_linreg_predict_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, const double* coef, double intercept,
+                            double* out, cudaStream_t s);

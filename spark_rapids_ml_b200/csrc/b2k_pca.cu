@@ -208,6 +208,9 @@ struct Timer {   // CUDA events around the device phases when option time_kernel
   }
 };
 
+
+}  // namespace
+
 // ---------------------------------------------------------------------------------------------------------------------
 // host eigen step
 // ---------------------------------------------------------------------------------------------------------------------
@@ -218,7 +221,7 @@ struct Timer {   // CUDA events around the device phases when option time_kernel
 //  2. implicit QL with Wilkinson-type shifts on T; each plane rotation of rows (i, i + 1) of T is applied to rows i and
 //     i + 1 of Z.
 // Returns false if an eigenvalue needs more than 60 QL sweeps.
-bool sym_eig(std::vector<double>& A, int n, std::vector<double>& w, std::vector<double>& Z) {
+bool b2k_sym_eig(std::vector<double>& A, int n, std::vector<double>& w, std::vector<double>& Z) {
   Z.assign((size_t)n * n, 0.0);
   for (int i = 0; i < n; ++i) Z[(size_t)i * n + i] = 1.0;
   std::vector<double> v(n), p(n), zs(n);
@@ -319,8 +322,6 @@ bool sym_eig(std::vector<double>& A, int n, std::vector<double>& w, std::vector<
   }
   return true;
 }
-}  // namespace
-
 int b2k_pca_finalize_impl(b2k_ctx* ctx, const double* cov, int d, int64_t n_total, int k, double* components_out,
                           double* evr_out, double* sv_out) {
   if (!cov || !components_out || !evr_out || !sv_out)
@@ -345,7 +346,7 @@ int b2k_pca_finalize_impl(b2k_ctx* ctx, const double* cov, int d, int64_t n_tota
     trace += cov[(size_t)i * d + i];
   }
   std::vector<double> w, Z;
-  if (!sym_eig(A, d, w, Z)) return b2k_fail(ctx, B2K_ERR_INVALID, "PCA: the eigensolver did not converge");
+  if (!b2k_sym_eig(A, d, w, Z)) return b2k_fail(ctx, B2K_ERR_INVALID, "PCA: the eigensolver did not converge");
   std::vector<int> order(d);
   std::iota(order.begin(), order.end(), 0);
   std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return w[a] > w[b]; });
@@ -363,20 +364,8 @@ int b2k_pca_finalize_impl(b2k_ctx* ctx, const double* cov, int d, int64_t n_tota
   return B2K_OK;
 }
 
-int b2k_pca_fit_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, int k, double* mean_out, double* components_out,
-                     double* evr_out, double* sv_out, cudaStream_t s) {
-  using clk = std::chrono::steady_clock;
-  const auto t_begin = clk::now();
-  if (!mean_out || !components_out || !evr_out || !sv_out)
-    return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_pca_fit: NULL output");
-  if (d > B2K_PCA_MAX_D)
-    return b2k_fail(ctx, B2K_ERR_UNSUPPORTED, "PCA supports d <= " + std::to_string(B2K_PCA_MAX_D) + ", got d = " +
-                                                  std::to_string(d));
-  if (k < 1) return b2k_fail(ctx, B2K_ERR_INVALID, "PCA: k must be >= 1, got " + std::to_string(k));
-  if (k > d)
-    return b2k_fail(ctx, B2K_ERR_INVALID, "source vector size " + std::to_string(d) + " must be no less than k=" +
-                                              std::to_string(k));
-  if (n > (int64_t)0x7fffff00) return b2k_fail(ctx, B2K_ERR_UNSUPPORTED, "PCA: more than 2^31 - 256 rows on one rank");
+int b2k_moments_impl(b2k_ctx* ctx, const char* who, const float* X, const float* y, int64_t n, int d, int64_t min_rows,
+                     B2kMoments* m, cudaStream_t s) {
   const bool wg_ok = d % 4 == 0 && (reinterpret_cast<uintptr_t>(X) & 15u) == 0;
   if (ctx->kernel_path == B2K_PATH_FUSED && !wg_ok)
     return b2k_fail(ctx, B2K_ERR_UNSUPPORTED, "kernel_path=2 requested but the wgmma Gram pass needs d % 4 == 0 and a "
@@ -389,6 +378,9 @@ int b2k_pca_fit_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, int k, doub
   const int64_t nspan_max = std::max<int64_t>(1, (n + 63) / 64);
   const int nspan = (int)std::min<int64_t>(std::max(1, (8 * ctx->sm_count + ncb - 1) / ncb), nspan_max);
   const int64_t span_rows = std::max<int64_t>(1, (n + nspan - 1) / nspan);
+  const int yspan = (int)std::min<int64_t>(8 * ctx->sm_count, nspan_max);   // the label: one column block
+  const int64_t yspan_rows = std::max<int64_t>(1, (n + yspan - 1) / yspan);
+  const int xty_spans = y ? b2k_xty_spans(ctx, n, d) : 0;
   const int nblk = (d + GW_BLK - 1) / GW_BLK, ntile = nblk * (nblk + 1) / 2;
   const int nrange = (int)std::max<int64_t>(1, (n + GW_RANGE - 1) / GW_RANGE);
   int sm = ctx->sm_count;
@@ -399,47 +391,71 @@ int b2k_pca_fit_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, int k, doub
   const int S = (int)std::max<int64_t>(1, std::min<int64_t>({64, (int64_t)((64u << 20) / (dd * 8)), (n + GG_T - 1) / GG_T}));
   const int64_t gspan = std::max<int64_t>(1, (n + S - 1) / S);
   const size_t part_len = wg ? (size_t)P * ntile * GW_BLK * GW_BLK : (size_t)S * dd;   // fp64 partials
-  double *colp, *sums, *G, *part;
+  const size_t nsum = (size_t)d + (y ? 2 : 1), nmom = dd + (y ? (size_t)d + 1 : 0);
+  double *colp, *sums, *G, *part, *ycolp = nullptr, *xtyp = nullptr;
   float* mu32_dev;
-  B2K_TRY(b2k_scratch_layout(ctx, "PCA", [&](B2kLayout& L) -> int {
+  B2K_TRY(b2k_scratch_layout(ctx, who, [&](B2kLayout& L) -> int {
     colp = L.take<double>((size_t)nspan * d);
-    sums = L.take<double>((size_t)d + 1);
+    sums = L.take<double>(nsum);
     mu32_dev = L.take<float>((size_t)nblk * GW_BLK);
-    G = L.take<double>(dd);
+    G = L.take<double>(nmom);   // [d][d] Gram (+ [d] X^T y, [1] y^T y)
     part = L.take<double>(part_len, 1024);
+    if (y) {
+      ycolp = L.take<double>((size_t)yspan);
+      xtyp = L.take<double>((size_t)xty_spans * (d + 1));
+    }
     return B2K_OK;
   }));
 
-  // ---- pass 1: column sums, allreduce of [d sums | n] ----
+  // ---- pass 1: column sums, allreduce of [d sums | n] (with a label: [d sums | label sum | n]) ----
   tm.mark(0, s);
   if (n > 0) {
     k_colsum<<<dim3(nspan, ncb), dim3(CS_TX, CS_TY), 0, s>>>(X, n, d, span_rows, colp);
     B2K_CUDA_OK(ctx, cudaGetLastError());
     ctx->stats.kernel_launches++;
+    if (y) {
+      k_colsum<<<dim3(yspan, 1), dim3(CS_TX, CS_TY), 0, s>>>(y, n, 1, yspan_rows, ycolp);
+      B2K_CUDA_OK(ctx, cudaGetLastError());
+      ctx->stats.kernel_launches++;
+    }
   } else {
     B2K_CUDA_OK(ctx, cudaMemsetAsync(colp, 0, (size_t)nspan * d * 8, s));
+    if (y) B2K_CUDA_OK(ctx, cudaMemsetAsync(ycolp, 0, (size_t)yspan * 8, s));
   }
   k_colsum_fold<<<(d + 1 + 255) / 256, 256, 0, s>>>(colp, nspan, d, n, sums);
   B2K_CUDA_OK(ctx, cudaGetLastError());
   ctx->stats.kernel_launches++;
+  if (y) {   // sums[d] <- label sum, sums[d + 1] <- n
+    k_colsum_fold<<<1, 32, 0, s>>>(ycolp, yspan, 1, n, sums + d);
+    B2K_CUDA_OK(ctx, cudaGetLastError());
+    ctx->stats.kernel_launches++;
+  }
   tm.mark(1, s);
-  B2K_TRY(b2k_comm_allreduce_f64(ctx, sums, (size_t)d + 1, s));
+  B2K_TRY(b2k_comm_allreduce_f64(ctx, sums, nsum, s));
   tm.mark(2, s);
-  std::vector<double> hs(d + 1);
-  B2K_CUDA_OK(ctx, cudaMemcpyAsync(hs.data(), sums, (size_t)(d + 1) * 8, cudaMemcpyDeviceToHost, s));
+  std::vector<double> hs(nsum);
+  B2K_CUDA_OK(ctx, cudaMemcpyAsync(hs.data(), sums, nsum * 8, cudaMemcpyDeviceToHost, s));
   B2K_CUDA_OK(ctx, cudaStreamSynchronize(s));
-  const int64_t n_total = (int64_t)std::llround(hs[d]);
-  if (n_total < 2) return b2k_fail(ctx, B2K_ERR_INVALID, "PCA needs at least 2 rows, got " + std::to_string(n_total));
-  std::vector<double> mu(d), delta(d);
+  const int64_t n_total = (int64_t)std::llround(hs[nsum - 1]);
+  if (n_total < min_rows)
+    return b2k_fail(ctx, B2K_ERR_INVALID, std::string(who) + " needs at least " + std::to_string(min_rows) +
+                                              " rows, got " + std::to_string(n_total));
+  const int dm = (int)nsum - 1;   // means: d features (+ the label)
+  m->n_total = n_total;
+  m->mu.assign(dm, 0.0);
+  m->delta.assign(dm, 0.0);
   std::vector<float> mu32((size_t)nblk * GW_BLK, 0.f);
-  for (int c = 0; c < d; ++c) {
-    mu[c] = hs[c] / (double)n_total;
-    mu32[c] = (float)mu[c];
-    delta[c] = mu[c] - (double)mu32[c];
+  float muy32 = 0.f;
+  for (int c = 0; c < dm; ++c) {
+    m->mu[c] = hs[c] / (double)n_total;
+    const float f = (float)m->mu[c];
+    if (c < d) mu32[c] = f;
+    else muy32 = f;
+    m->delta[c] = m->mu[c] - (double)f;
   }
   B2K_CUDA_OK(ctx, cudaMemcpyAsync(mu32_dev, mu32.data(), mu32.size() * 4, cudaMemcpyHostToDevice, s));
 
-  // ---- pass 2: Gram matrix of the data centred on mu32, allreduce ----
+  // ---- pass 2: Gram matrix of the data centred on mu32 (and X^T y), allreduce ----
   tm.mark(3, s);
   const int fold_blocks = (int)((dd + 255) / 256);
   if (wg) {
@@ -479,24 +495,51 @@ int b2k_pca_fit_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, int k, doub
   ctx->stats.kernel_launches++;
   ctx->stats.last_path = wg ? B2K_PATH_FUSED : B2K_PATH_GENERIC;
   tm.mark(4, s);
-  B2K_TRY(b2k_comm_allreduce_f64(ctx, G, dd, s));
+  if (y) B2K_TRY(b2k_launch_xty(ctx, X, y, n, d, mu32_dev, muy32, xty_spans, xtyp, G + dd, s));
+  tm.mark(6, s);
+  B2K_TRY(b2k_comm_allreduce_f64(ctx, G, nmom, s));
   tm.mark(5, s);
-  std::vector<double> cov(dd);
-  B2K_CUDA_OK(ctx, cudaMemcpyAsync(cov.data(), G, dd * 8, cudaMemcpyDeviceToHost, s));
+  m->G.resize(nmom);
+  B2K_CUDA_OK(ctx, cudaMemcpyAsync(m->G.data(), G, nmom * 8, cudaMemcpyDeviceToHost, s));
   B2K_CUDA_OK(ctx, cudaStreamSynchronize(s));
+  if (tm.on) {
+    ctx->stats.last_reduce_ms = tm.ms(0, 1);
+    ctx->stats.last_allreduce_ms = tm.ms(1, 2) + tm.ms(6, 5);
+    ctx->stats.last_fused_ms = tm.ms(3, 4);
+    if (y) ctx->stats.last_finalize_ms = tm.ms(4, 6);
+  }
+  return B2K_OK;
+}
+
+int b2k_pca_fit_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, int k, double* mean_out, double* components_out,
+                     double* evr_out, double* sv_out, cudaStream_t s) {
+  using clk = std::chrono::steady_clock;
+  const auto t_begin = clk::now();
+  if (!mean_out || !components_out || !evr_out || !sv_out)
+    return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_pca_fit: NULL output");
+  if (d > B2K_PCA_MAX_D)
+    return b2k_fail(ctx, B2K_ERR_UNSUPPORTED, "PCA supports d <= " + std::to_string(B2K_PCA_MAX_D) + ", got d = " +
+                                                  std::to_string(d));
+  if (k < 1) return b2k_fail(ctx, B2K_ERR_INVALID, "PCA: k must be >= 1, got " + std::to_string(k));
+  if (k > d)
+    return b2k_fail(ctx, B2K_ERR_INVALID, "source vector size " + std::to_string(d) + " must be no less than k=" +
+                                              std::to_string(k));
+  if (n > (int64_t)0x7fffff00) return b2k_fail(ctx, B2K_ERR_UNSUPPORTED, "PCA: more than 2^31 - 256 rows on one rank");
+  B2kMoments m;
+  B2K_TRY(b2k_moments_impl(ctx, "PCA", X, nullptr, n, d, 2, &m, s));
 
   // ---- host: exact removal of the mu32 offset, eigen step ----
   const auto t_eig = clk::now();
+  const int64_t n_total = m.n_total;
+  const std::vector<double>& delta = m.delta;
+  std::vector<double>& cov = m.G;
   const double nt = (double)n_total, inv = 1.0 / (double)(n_total - 1);
   for (int i = 0; i < d; ++i)
     for (int j = 0; j < d; ++j) cov[(size_t)i * d + j] = (cov[(size_t)i * d + j] - nt * delta[i] * delta[j]) * inv;
   B2K_TRY(b2k_pca_finalize_impl(ctx, cov.data(), d, n_total, k, components_out, evr_out, sv_out));
-  std::copy(mu.begin(), mu.end(), mean_out);
+  std::copy(m.mu.begin(), m.mu.end(), mean_out);
   const auto t_end = clk::now();
-  if (tm.on) {
-    ctx->stats.last_reduce_ms = tm.ms(0, 1);
-    ctx->stats.last_allreduce_ms = tm.ms(1, 2) + tm.ms(4, 5);
-    ctx->stats.last_fused_ms = tm.ms(3, 4);
+  if (ctx->time_kernels) {
     ctx->stats.last_finalize_ms = std::chrono::duration<double, std::milli>(t_end - t_eig).count();
     ctx->stats.last_loop_ms = std::chrono::duration<double, std::milli>(t_end - t_begin).count();
   }

@@ -1,5 +1,6 @@
 """No-import-change mode: after `import spark_rapids_ml_b200.install`, user code that says
-`from pyspark.ml.clustering import KMeans` (or KMeansModel, or `from pyspark.ml.feature import PCA` / PCAModel) receives
+`from pyspark.ml.clustering import KMeans` (or KMeansModel, or `from pyspark.ml.feature import PCA` / PCAModel, or
+`from pyspark.ml.regression import LinearRegression` / LinearRegressionModel) receives
 this package's accelerated classes; every other attribute of those modules, and every access made from inside pyspark.ml
 or from this package itself, still resolves to pyspark's own module.  Reference behaviour:
 python/src/spark_rapids_ml/install.py:21-81 (a proxy module per pyspark.ml sub-module whose __getattr__ looks at the
@@ -16,7 +17,8 @@ import sys
 import types
 from typing import Any, Dict, Tuple
 
-ACCELERATED: Dict[str, Tuple[str, ...]] = {"clustering": ("KMeans", "KMeansModel"), "feature": ("PCA", "PCAModel")}
+ACCELERATED: Dict[str, Tuple[str, ...]] = {"clustering": ("KMeans", "KMeansModel"), "feature": ("PCA", "PCAModel"),
+                                           "regression": ("LinearRegression", "LinearRegressionModel")}
 
 _PKG_DIR = os.path.dirname(os.path.abspath(__file__))
 

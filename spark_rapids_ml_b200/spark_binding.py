@@ -62,15 +62,30 @@ def pre_process_data(est: Any, dataset: Any, data_alias: str) -> Tuple[Any, Opti
                 inner = "float" if f32 else "double"
         else:
             raise ValueError("Unsupported input type.")
-        df = dataset.select(feat)
+        df = dataset.select(feat, *_label_cols(est, dataset))
         first = df.first()
         if first is None:
             raise RuntimeError("A python worker received no data.  Please increase amount of data or use fewer workers.")
         return df, None, len(first[data_alias]), inner
     assert input_cols is not None
     want = FloatType() if f32 else DoubleType()
-    df = dataset.select(*[col(c).cast(want).alias(c) for c in input_cols])                              # :543-557
+    df = dataset.select(*[col(c).cast(want).alias(c) for c in input_cols], *_label_cols(est, dataset))  # :543-557
     return df, list(input_cols), len(input_cols), "float" if f32 else "double"
+
+
+def _label_cols(est: Any, dataset: Any) -> List[Any]:
+    """The label of a supervised estimator as a float32 column named alias.label (reference core.py:500-508)."""
+    from pyspark.sql.functions import col
+    from pyspark.sql.types import FloatType
+
+    from .core import alias
+
+    label = est._fit_label_col()
+    if label is None:
+        return []
+    if label not in dataset.columns:
+        raise ValueError(f"label column '{label}' not found in {dataset.columns}")
+    return [col(label).cast(FloatType()).alias(alias.label)]
 
 
 def run_barrier_fit(df: Any, train_udf: Callable[[Iterator[pd.DataFrame]], Iterator[pd.DataFrame]], out_schema: Any,
