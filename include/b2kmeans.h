@@ -27,6 +27,11 @@
  *   b2k_linreg_moments          regression.py:546-607 (the passes over the data of LinearRegressionMG / RidgeMG / CDMG)
  *   b2k_linreg_solve            the solvers inside them (normal equations, coordinate descent) and the rescaling
  *   b2k_linreg_predict          regression.py:800-862 (LinearRegressionModel's transform: cuML predict)
+ *   b2k_logreg_labels           classification.py:1075-1103 (the classes cuML finds and the label checks after them)
+ *   b2k_logreg_eval             one loss-and-gradient evaluation of cuML's qn solver behind LogisticRegressionMG
+ *   b2k_logreg_minimize         cuML's qn solver (L-BFGS / OWL-QN) itself
+ *   b2k_logreg_fit              classification.py:984-1171 (LogisticRegressionMG.fit per param map, rescaling, centring)
+ *   b2k_logreg_predict          classification.py:1455-1553 (LogisticRegressionModel's transform)
  *
  * Conventions
  *   - Plain C, no exceptions across the boundary: every call returns a b2k_status; the message for the
@@ -276,6 +281,81 @@ int b2k_linreg_solve(const double* mean, const double* moments, int d, int64_t n
 /* out [n] f64 = intercept + sum_j X[i][j] coef[j] (coef device f64 [d]), accumulated in fp64 in an order fixed by d
  * alone.  Asynchronous on `stream`. */
 int b2k_linreg_predict(b2k_ctx* ctx, const float* X, int64_t n, int d, const double* coef, double intercept, double* out,
+                       uintptr_t stream);
+
+/* ---- logistic regression (binomial and multinomial, L2 / L1 / elastic net, MLlib's objective) ----
+ * With K' = 1 (binomial) or K (multinomial) margins per row, coefficients W [K'][d] and intercepts b [K'], the fit
+ * minimises (1/n) sum_i l(W x_i + b, y_i) + reg ((1 - l1_ratio)/2 |V|^2 + l1_ratio |V|_1), where l is the logistic loss
+ * max(m, 0) + log1p(exp(-|m|)) - y m (binomial) or the softmax cross-entropy (log-sum-exp with the row maximum taken
+ * out), the intercepts are not penalised, and V = W diag(sigma) with standardization, else V = W.  sigma are the sample
+ * (n - 1) standard deviations of the features, MLlib's convention; a feature with sigma = 0 gets a coefficient of 0.
+ * Labels are the class values: integers in [0, 1024); classes = the sorted distinct label values.
+ *
+ * b2k_logreg_labels (collective) stands in for the class discovery of classification.py:1075-1103 (cuML's
+ * LogisticRegressionMG.fit and the label checks after it).  One pass over y [n_local] (device f32) and one allgather.
+ * Outputs (host): classes_out [<= 1024] f64, counts_out [<= 1024] rows per class, *n_classes_out, *n_total_out.
+ * Errors, decided on the gathered values so that every rank fails together (B2K_ERR_INVALID unless noted): an empty
+ * partition on any rank; a NaN or an infinity; "Labels MUST be in [0, 2147483647), but got v" (v the least label,
+ * the first sorted class the reference reports); "Labels MUST be Integers, but got v"; a label
+ * >= 1024 (B2K_ERR_UNSUPPORTED).  Synchronises `stream`. */
+int b2k_logreg_labels(b2k_ctx* ctx, const float* y, int64_t n_local, double* classes_out, int64_t* counts_out,
+                      int* n_classes_out, int64_t* n_total_out, uintptr_t stream);
+/* b2k_logreg_eval (collective) stands in for one loss-and-gradient evaluation inside cuML's qn solver: the loss
+ * (1/n) sum l and its gradient (no penalty) at W [kp][d], b [kp] (host f64), over X [n_local, d] and y [n_local] (device
+ * f32).  classes [n_classes] are the class values (b2k_logreg_labels); a row whose label is not one of them counts as no
+ * class.  kp = 1: the binomial loss with class index 1 the positive class.  Outputs (host): *loss_out, grad_out
+ * [kp][d + 1] = (1/n) sum r_k x_j, then (1/n) sum r_k in column d; *n_total_out (may be NULL).  The fused pass
+ * (k_logreg_eval) runs where its accumulators fit: K' classes per thread block of at most 16 with d * ceil(K'/KB) <=
+ * 256 NIT (binomial: d <= 1024; K <= 16: d <= 256); elsewhere the generic rows + X^T R passes.  Option "kernel_path" as
+ * for PCA; stats.last_path reports the pass; with "time_kernels", last_fused_ms = its device time.  Errors: an empty
+ * partition; d > 1024 (B2K_ERR_UNSUPPORTED).  Synchronises `stream`.  Bitwise reproducible for the same input, rank
+ * count and device. */
+int b2k_logreg_eval(b2k_ctx* ctx, const float* X, const float* y, int64_t n_local, int d, const double* classes,
+                    int n_classes, int kp, const double* W, const double* b, double* loss_out, double* grad_out,
+                    int64_t* n_total_out, uintptr_t stream);
+/* Objective of b2k_logreg_minimize: the smooth part f(x) and its gradient at x [n]; nonzero return aborts the
+ * minimisation with that status. */
+typedef int (*b2k_logreg_objective)(void* user, int n, const double* x, double* f, double* grad);
+/* b2k_logreg_minimize (host only, no device) stands in for cuML's qn solver (L-BFGS / OWL-QN): minimises f(x) + sum_i
+ * l1[i] |x_i| from x [n] (in: the start, out: the result); l1 may be NULL.  L-BFGS with memory 10 and a strong-Wolfe
+ * line search (c1 = 1e-4, c2 = 0.9) of at most 20 evaluations, first step 1/|d|; OWL-QN (any l1[i] > 0): the
+ * pseudo-gradient, orthant-projected steps and a backtracking line search of at most 20 evaluations.  Stops on Breeze's
+ * rules as MLlib applies them: iterations == max_iter; |F - max of the last 20 F| <= tol |F_0|; |pseudo-gradient| <=
+ * max(tol |F|, 1e-8); or a failed line search (x keeps the last accepted iterate).  F is the value with the L1 term.
+ * Outputs: *n_iter_out, *n_eval_out, *f_out (each may be NULL).  Errors through b2k_last_error(NULL): max_iter < 0,
+ * tol < 0, a negative or non-finite l1 weight, a non-finite start value. */
+int b2k_logreg_minimize(b2k_logreg_objective fn, void* user, int n, double* x, const double* l1, int max_iter,
+                        double tol, int* n_iter_out, int* n_eval_out, double* f_out);
+typedef struct b2k_logreg_params {
+  double reg;              /* regParam >= 0 */
+  double l1_ratio;         /* elasticNetParam in [0, 1] */
+  double tol;              /* >= 0 */
+  int32_t max_iter;        /* >= 0 */
+  int32_t fit_intercept;   /* 0 / 1 */
+  int32_t standardization; /* 0 / 1 */
+  int32_t family;          /* 0 auto (binomial for 2 classes), 1 binomial, 2 multinomial */
+} b2k_logreg_params;
+/* b2k_logreg_fit (collective) stands in for classification.py:984-1171 (LogisticRegressionMG.fit per param map, the
+ * rescaling and the intercept centring).  classes / counts / n_classes from b2k_logreg_labels.  One column-moments
+ * pass (sums, then centred squares, fp64), then per setting params[f]: L-BFGS / OWL-QN through b2k_logreg_eval in the
+ * solver frame theta = [V | b], intercepts started at MLlib's log-odds of the priors; then W = V / sigma, and for
+ * multinomial fits the intercepts centred over the classes (with an intercept) and, when reg == 0, the coefficients
+ * centred per feature.  Outputs (host), per setting f: coef_out [f][K][d] (rows past kp_out[f] zero), intercept_out
+ * [f][K], kp_out[f] = K' and n_iter_out[f] = iterations.  One class (0 or 1): zero coefficients, intercept +inf (class 1)
+ * or -inf, 0 iterations; another single class value is an error.  Errors (B2K_ERR_INVALID): those of the params
+ * ("maxIter given invalid value -1", "C or regParam given an invalid or unsupported value -1.0", ...), "Binomial family
+ * only supports 1 or 2 outcome classes but found K.", an empty partition, a NaN or an infinity in X; d > 1024:
+ * B2K_ERR_UNSUPPORTED.  Synchronises `stream`; bitwise reproducible for the same input, rank count and device.
+ * stats.last_n_iter = the last setting's iterations; with "time_kernels", last_loop_ms = the whole call. */
+int b2k_logreg_fit(b2k_ctx* ctx, const float* X, const float* y, int64_t n_local, int d, const double* classes,
+                   const int64_t* counts, int n_classes, int n_fits, const b2k_logreg_params* params, double* coef_out,
+                   double* intercept_out, int* kp_out, int* n_iter_out, uintptr_t stream);
+/* b2k_logreg_predict stands in for classification.py:1455-1553 (LogisticRegressionModel's transform): margins m = W x +
+ * b in fp64 (W device f64 [kp][d], b device f64 [kp]); with nout = 2 for kp = 1, else kp: raw_out [n][nout] = [-m, m]
+ * or the margins, prob_out [n][nout] = [1 - s, s] (s the sigmoid) or the softmax, pred_out [n] = class_values[argmax]
+ * (class_values device f64 [nout]; binomial: m > 0).  Asynchronous on `stream`. */
+int b2k_logreg_predict(b2k_ctx* ctx, const float* X, int64_t n, int d, int kp, const double* W, const double* b,
+                       const double* class_values, double* raw_out, double* prob_out, double* pred_out,
                        uintptr_t stream);
 
 #ifdef __cplusplus

@@ -9,7 +9,7 @@ from __future__ import annotations
 import ctypes
 import os
 import subprocess
-from typing import Any, Dict, Optional, Sequence, Tuple
+from typing import Any, Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
 
@@ -58,13 +58,35 @@ EXPORTED_SYMBOLS = (
     "b2k_linreg_moments",
     "b2k_linreg_solve",
     "b2k_linreg_predict",
+    "b2k_logreg_labels",
+    "b2k_logreg_eval",
+    "b2k_logreg_minimize",
+    "b2k_logreg_fit",
+    "b2k_logreg_predict",
 )
+
+FAMILY_CODES = {"auto": 0, "binomial": 1, "multinomial": 2}
+# int (*)(void* user, int n, const double* x, double* f, double* grad)
+LOGREG_OBJECTIVE = ctypes.CFUNCTYPE(ctypes.c_int, ctypes.c_void_p, ctypes.c_int, ctypes.POINTER(ctypes.c_double),
+                                    ctypes.POINTER(ctypes.c_double), ctypes.POINTER(ctypes.c_double))
 
 
 class B2KError(RuntimeError):
     def __init__(self, code: int, msg: str):
         super().__init__(f"libb2kmeans error {code}: {msg}")
         self.code = code
+
+
+class LogregParams(ctypes.Structure):
+    _fields_ = [
+        ("reg", ctypes.c_double),
+        ("l1_ratio", ctypes.c_double),
+        ("tol", ctypes.c_double),
+        ("max_iter", ctypes.c_int32),
+        ("fit_intercept", ctypes.c_int32),
+        ("standardization", ctypes.c_int32),
+        ("family", ctypes.c_int32),
+    ]
 
 
 class Stats(ctypes.Structure):
@@ -140,6 +162,14 @@ def load_library() -> ctypes.CDLL:
     L.b2k_linreg_solve.argtypes = [vp, vp, i32, i64, f64, f64, i32, i32, i32, f64, vp, ctypes.POINTER(f64),
                                    ctypes.POINTER(i32)]
     L.b2k_linreg_predict.argtypes = [vp, vp, i64, i32, vp, f64, vp, ctypes.c_size_t]
+    L.b2k_logreg_labels.argtypes = [vp, vp, i64, vp, vp, ctypes.POINTER(i32), ctypes.POINTER(i64), ctypes.c_size_t]
+    L.b2k_logreg_eval.argtypes = [vp, vp, vp, i64, i32, vp, i32, i32, vp, vp, ctypes.POINTER(f64), vp,
+                                  ctypes.POINTER(i64), ctypes.c_size_t]
+    L.b2k_logreg_minimize.argtypes = [LOGREG_OBJECTIVE, vp, i32, vp, vp, i32, f64, ctypes.POINTER(i32),
+                                      ctypes.POINTER(i32), ctypes.POINTER(f64)]
+    L.b2k_logreg_fit.argtypes = [vp, vp, vp, i64, i32, vp, vp, i32, i32, ctypes.POINTER(LogregParams), vp, vp, vp, vp,
+                                 ctypes.c_size_t]
+    L.b2k_logreg_predict.argtypes = [vp, vp, i64, i32, i32, vp, vp, vp, vp, vp, vp, ctypes.c_size_t]
     for name in EXPORTED_SYMBOLS:
         if name not in ("b2k_last_error",):
             getattr(L, name).restype = i32
@@ -195,6 +225,39 @@ def linreg_solve(mean: np.ndarray, moments: np.ndarray, n_total: int, reg: float
     if rc != B2K_OK:
         raise B2KError(rc, (L.b2k_last_error(None) or b"").decode())
     return coef, float(b.value), int(it.value)
+
+
+def logreg_minimize(fun: Any, x0: np.ndarray, l1: Optional[np.ndarray] = None, max_iter: int = 100,
+                    tol: float = 1e-6) -> Tuple[np.ndarray, int, int, float]:
+    """b2k_logreg_minimize (host only): minimise fun(x) -> (f, grad) plus sum l1 |x| from x0 -> (x, iterations,
+    evaluations, final value with the L1 term).  An exception raised by fun aborts the minimisation and is re-raised."""
+    L = load_library()
+    x = np.array(x0, dtype=np.float64, copy=True)
+    n = int(x.shape[0])
+    l1a = None if l1 is None else np.ascontiguousarray(l1, dtype=np.float64)
+    if l1a is not None and l1a.shape != (n,):
+        raise ValueError(f"l1 must be [{n}]")
+    err: list = []
+
+    def _cb(_user: Any, m: int, xp: Any, fp: Any, gp: Any) -> int:
+        try:
+            f, g = fun(np.ctypeslib.as_array(xp, shape=(m,)).copy())
+            fp[0] = float(f)
+            np.ctypeslib.as_array(gp, shape=(m,))[:] = np.asarray(g, dtype=np.float64)
+            return 0
+        except Exception as e:  # noqa: BLE001 - handed back to the caller below
+            err.append(e)
+            return 1
+
+    cb = LOGREG_OBJECTIVE(_cb)
+    it, ev, fv = ctypes.c_int(0), ctypes.c_int(0), ctypes.c_double(0.0)
+    rc = L.b2k_logreg_minimize(cb, None, n, x.ctypes.data, l1a.ctypes.data if l1a is not None else None,
+                               int(max_iter), float(tol), ctypes.byref(it), ctypes.byref(ev), ctypes.byref(fv))
+    if err:
+        raise err[0]
+    if rc != B2K_OK:
+        raise B2KError(rc, (L.b2k_last_error(None) or b"").decode())
+    return x, int(it.value), int(ev.value), float(fv.value)
 
 
 def _stream_handle(torch_mod: Any, device: Any) -> int:
@@ -484,3 +547,89 @@ class Context:
                                                    out.data_ptr(), self._stream()))
         t.cuda.current_stream(self.device).synchronize()  # w (possibly a temporary) must outlive the kernel
         return out
+
+    # -- logistic regression ----------------------------------------------------------------
+    def _check_y(self, y: Any, n: int) -> None:
+        t = self._torch
+        if not (y.is_cuda and y.dtype == t.float32 and y.is_contiguous() and tuple(y.shape) == (n,)):
+            raise ValueError(f"y must be a contiguous float32 CUDA tensor [{n}]")
+
+    def logreg_labels(self, y: Any) -> Tuple[np.ndarray, np.ndarray, int]:
+        """The label pass (collective): y [n] float32 CUDA tensor -> (classes float64 [K], counts int64 [K], n_total)."""
+        n = int(y.shape[0]) if y.dim() == 1 else -1
+        self._check_y(y, n)
+        cls = np.zeros(1024, dtype=np.float64)
+        cnt = np.zeros(1024, dtype=np.int64)
+        k, nt = ctypes.c_int(0), ctypes.c_int64(0)
+        with self._torch.cuda.device(self.device):
+            self._check(self._L.b2k_logreg_labels(self._h, y.data_ptr(), n, cls.ctypes.data, cnt.ctypes.data,
+                                                  ctypes.byref(k), ctypes.byref(nt), self._stream()))
+        return cls[: k.value].copy(), cnt[: k.value].copy(), int(nt.value)
+
+    def logreg_eval(self, X: Any, y: Any, classes: Sequence[float], W: np.ndarray, b: np.ndarray
+                    ) -> Tuple[float, np.ndarray, np.ndarray, int]:
+        """One loss-and-gradient evaluation (collective): (1/n) sum loss and its gradient at W [kp, d], b [kp] (no
+        penalty) -> (loss, dW [kp, d], db [kp], n_total)."""
+        n, d = self._check_X(X)
+        self._check_y(y, n)
+        cls = np.ascontiguousarray(classes, dtype=np.float64)
+        W = np.ascontiguousarray(W, dtype=np.float64)
+        kp = int(W.shape[0])
+        b = np.ascontiguousarray(b, dtype=np.float64)
+        if W.shape != (kp, d) or b.shape != (kp,):
+            raise ValueError(f"W must be [kp, {d}] and b [kp]")
+        loss = ctypes.c_double(0.0)
+        grad = np.zeros((kp, d + 1), dtype=np.float64)
+        nt = ctypes.c_int64(0)
+        with self._torch.cuda.device(self.device):
+            self._check(self._L.b2k_logreg_eval(self._h, X.data_ptr(), y.data_ptr(), n, d, cls.ctypes.data, int(cls.size),
+                                                kp, W.ctypes.data, b.ctypes.data, ctypes.byref(loss), grad.ctypes.data,
+                                                ctypes.byref(nt), self._stream()))
+        return float(loss.value), grad[:, :d].copy(), grad[:, d].copy(), int(nt.value)
+
+    def logreg_fit(self, X: Any, y: Any, classes: np.ndarray, counts: np.ndarray, settings: Sequence[Dict[str, Any]]
+                   ) -> List[Tuple[np.ndarray, np.ndarray, int]]:
+        """Fits (collective), one per setting dict (reg, l1_ratio, tol, max_iter, fit_intercept, standardization,
+        family) from one column-moments pass -> [(coef [kp, d], intercept [kp], iterations)]."""
+        n, d = self._check_X(X)
+        self._check_y(y, n)
+        cls = np.ascontiguousarray(classes, dtype=np.float64)
+        cnt = np.ascontiguousarray(counts, dtype=np.int64)
+        K, m = int(cls.size), len(settings)
+        prm = (LogregParams * m)(*[LogregParams(float(s["reg"]), float(s["l1_ratio"]), float(s["tol"]),
+                                                int(s["max_iter"]), int(bool(s["fit_intercept"])),
+                                                int(bool(s["standardization"])), FAMILY_CODES[s["family"]])
+                                   for s in settings])
+        coef = np.zeros((m, K, d), dtype=np.float64)
+        icpt = np.zeros((m, K), dtype=np.float64)
+        kp = np.zeros(m, dtype=np.int32)
+        it = np.zeros(m, dtype=np.int32)
+        with self._torch.cuda.device(self.device):
+            self._check(self._L.b2k_logreg_fit(self._h, X.data_ptr(), y.data_ptr(), n, d, cls.ctypes.data, cnt.ctypes.data,
+                                               K, m, prm, coef.ctypes.data, icpt.ctypes.data, kp.ctypes.data,
+                                               it.ctypes.data, self._stream()))
+        return [(coef[f, : kp[f]].copy(), icpt[f, : kp[f]].copy(), int(it[f])) for f in range(m)]
+
+    def logreg_predict(self, X: Any, W: Any, b: Any, class_values: Sequence[float]) -> Tuple[Any, Any, Any]:
+        """rawPrediction [n, nout], probability [n, nout] and prediction [n] as float64 CUDA tensors (nout = 2 for a
+        binomial W [1, d])."""
+        t = self._torch
+        n, d = self._check_X(X)
+        Wd = t.as_tensor(np.ascontiguousarray(W, dtype=np.float64), device=self.device).contiguous()
+        bd = t.as_tensor(np.ascontiguousarray(b, dtype=np.float64), device=self.device).contiguous()
+        kp = int(Wd.shape[0])
+        if tuple(Wd.shape) != (kp, d) or tuple(bd.shape) != (kp,):
+            raise ValueError(f"W must be [kp, {d}] and b [kp]")
+        nout = 2 if kp == 1 else kp
+        cv = t.as_tensor(np.ascontiguousarray(class_values, dtype=np.float64), device=self.device).contiguous()
+        if tuple(cv.shape) != (nout,):
+            raise ValueError(f"class_values must be [{nout}]")
+        raw = t.empty((n, nout), dtype=t.float64, device=self.device)
+        prob = t.empty((n, nout), dtype=t.float64, device=self.device)
+        pred = t.empty((n,), dtype=t.float64, device=self.device)
+        with t.cuda.device(self.device):
+            self._check(self._L.b2k_logreg_predict(self._h, X.data_ptr(), n, d, kp, Wd.data_ptr(), bd.data_ptr(),
+                                                   cv.data_ptr(), raw.data_ptr(), prob.data_ptr(), pred.data_ptr(),
+                                                   self._stream()))
+        t.cuda.current_stream(self.device).synchronize()  # Wd, bd, cv (temporaries) must outlive the kernel
+        return raw, prob, pred

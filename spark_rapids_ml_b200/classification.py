@@ -1,0 +1,592 @@
+"""LogisticRegression / LogisticRegressionModel — the reference's distributed logistic regression surface
+(python/src/spark_rapids_ml/classification.py:679-1614), with the cuML calls replaced by libb2kmeans (hand-written sm_90a
+CUDA behind include/b2kmeans.h).
+
+  LogisticRegressionClass (param and value mappings, cuML defaults)            classification.py:679-747
+  _LogisticRegressionCumlParams (featuresCol(s), label, prediction columns)    classification.py:750-819
+  LogisticRegression (keyword-only ctor, setters, fit function, fitMultiple)   classification.py:822-1303
+  LogisticRegressionModel (coefficients, intercepts, transform, _combine)      classification.py:1306-1614
+
+Semantics (b2k_logreg_labels / b2k_logreg_fit): MLlib's objective, (1/n) sum of the logistic (binomial) or softmax
+(multinomial) loss + regParam ((1 - elasticNetParam)/2 |V|^2 + elasticNetParam |V|_1), V the coefficients scaled by the
+sample standard deviations of the features with standardization.  Every optimiser step is one fused pass over the
+device-resident rows (margins, residuals and the gradient X^T R in one read of X, fp64) and one allreduce; L-BFGS /
+OWL-QN runs on the host in fp64.  transform() appends rawPrediction and probability (double vectors) and prediction
+(the class value of the largest margin, a double).
+
+Differences that are deliberate: with regParam = 0 a multinomial fit centres its coefficients per feature, as MLlib
+does (the reference reports wherever its solver stopped on a problem without a unique solution); the classes are the
+sorted distinct label values and the prediction is the class value, not its index; labels must be below 1024.  No CPU
+fallback: cpu(), predict(), predictRaw(), predictProbability() and evaluate() raise NotImplementedError; weightCol,
+threshold(s), the coefficient / intercept bounds and sparse input raise ValueError; there is no training summary.
+"""
+from __future__ import annotations
+
+from typing import Any, Callable, Dict, Iterator, List, Optional, Sequence, Tuple, Union
+
+import numpy as np
+import pandas as pd
+import pyarrow as pa
+
+from .core import FitInputType, _append_transform_features, _CumlEstimator, _CumlModelWithPredictionCol, _CumlCommon
+from .core import _transform_context, alias, param_alias
+from .params import HasFeaturesCol, HasFeaturesCols, HasLabelCol, HasPredictionCol, P, _CumlClass, _CumlParams
+from .regression import _ModelIterator
+from .sparkshim import BarrierTaskContext, LocalDataFrame, Param, Row, TypeConverters, keyword_only
+
+
+class LogisticRegressionClass(_CumlClass):
+    @classmethod
+    def _param_mapping(cls) -> Dict[str, Optional[str]]:
+        return {
+            "maxIter": "max_iter",
+            "regParam": "C",
+            "elasticNetParam": "l1_ratio",
+            "tol": "tol",
+            "fitIntercept": "fit_intercept",
+            "threshold": None,
+            "thresholds": None,
+            "standardization": "standardization",
+            "weightCol": None,
+            "aggregationDepth": "",
+            "family": "",
+            "lowerBoundsOnCoefficients": None,
+            "upperBoundsOnCoefficients": None,
+            "lowerBoundsOnIntercepts": None,
+            "upperBoundsOnIntercepts": None,
+            "maxBlockSizeInMB": "",
+        }
+
+    @classmethod
+    def _param_value_mapping(cls) -> Dict[str, Callable[[Any], Union[None, str, float, int]]]:
+        return {"C": lambda x: 1 / x if x > 0.0 else (0.0 if x == 0.0 else None)}
+
+    def _get_cuml_params_default(self) -> Dict[str, Any]:
+        return {"fit_intercept": True, "standardization": False, "verbose": False, "C": 1.0, "penalty": "l2",
+                "l1_ratio": None, "max_iter": 1000, "tol": 0.0001}
+
+    @classmethod
+    def _reg_params_value_mapping(cls, reg_param: float, elasticNet_param: float) -> Tuple[Optional[str], float, float]:
+        """Spark's (regParam, elasticNetParam) -> cuML's (penalty, C, l1_ratio)."""
+        if reg_param == 0.0:
+            return None, 0.0, elasticNet_param
+        penalty = "l2" if elasticNet_param == 0.0 else "l1" if elasticNet_param == 1.0 else "elasticnet"
+        return penalty, 1.0 / reg_param, elasticNet_param
+
+    def _pyspark_class(self) -> Optional[type]:
+        return None  # pyspark.ml.classification.LogisticRegression when pyspark is installed
+
+
+class _LogisticRegressionParams(HasFeaturesCol, HasLabelCol, HasPredictionCol):
+    """pyspark.ml.classification._LogisticRegressionParams stand-in, with Spark's defaults."""
+
+    maxIter = Param("parent", "maxIter", "max number of iterations (>= 0).", TypeConverters.toInt)
+    regParam = Param("parent", "regParam", "regularization parameter (>= 0).", TypeConverters.toFloat)
+    elasticNetParam = Param("parent", "elasticNetParam", "the ElasticNet mixing parameter, in range [0, 1]. For alpha "
+                            "= 0, the penalty is an L2 penalty. For alpha = 1, it is an L1 penalty.",
+                            TypeConverters.toFloat)
+    tol = Param("parent", "tol", "the convergence tolerance for iterative algorithms (>= 0).", TypeConverters.toFloat)
+    fitIntercept = Param("parent", "fitIntercept", "whether to fit an intercept term.")
+    standardization = Param("parent", "standardization", "whether to standardize the training features before fitting "
+                            "the model.")
+    threshold = Param("parent", "threshold", "Threshold in binary classification prediction, in range [0, 1].",
+                      TypeConverters.toFloat)
+    thresholds = Param("parent", "thresholds", "Thresholds in multi-class classification to adjust the probability of "
+                       "predicting each class.")
+    weightCol = Param("parent", "weightCol", "weight column name.", TypeConverters.toString)
+    aggregationDepth = Param("parent", "aggregationDepth", "suggested depth for treeAggregate (>= 2).",
+                             TypeConverters.toInt)
+    family = Param("parent", "family", "The name of family which is a description of the label distribution to be used "
+                   "in the model. Supported options: auto, binomial, multinomial", TypeConverters.toString)
+    lowerBoundsOnCoefficients = Param("parent", "lowerBoundsOnCoefficients", "The lower bounds on coefficients.")
+    upperBoundsOnCoefficients = Param("parent", "upperBoundsOnCoefficients", "The upper bounds on coefficients.")
+    lowerBoundsOnIntercepts = Param("parent", "lowerBoundsOnIntercepts", "The lower bounds on intercepts.")
+    upperBoundsOnIntercepts = Param("parent", "upperBoundsOnIntercepts", "The upper bounds on intercepts.")
+    maxBlockSizeInMB = Param("parent", "maxBlockSizeInMB", "maximum memory in MB for stacking input data.",
+                             TypeConverters.toFloat)
+    probabilityCol = Param("parent", "probabilityCol", "Column name for predicted class conditional probabilities.",
+                           TypeConverters.toString)
+    rawPredictionCol = Param("parent", "rawPredictionCol", "raw prediction (a.k.a. confidence) column name.",
+                             TypeConverters.toString)
+
+    def __init__(self) -> None:
+        super().__init__()
+        self._setDefault(labelCol="label", maxIter=100, regParam=0.0, elasticNetParam=0.0, tol=1e-6,
+                         fitIntercept=True, threshold=0.5, standardization=True, aggregationDepth=2, family="auto",
+                         maxBlockSizeInMB=0.0, probabilityCol="probability", rawPredictionCol="rawPrediction")
+
+    def getMaxIter(self) -> int:
+        return self.getOrDefault(self.maxIter)
+
+    def getRegParam(self) -> float:
+        return self.getOrDefault(self.regParam)
+
+    def getElasticNetParam(self) -> float:
+        return self.getOrDefault(self.elasticNetParam)
+
+    def getTol(self) -> float:
+        return self.getOrDefault(self.tol)
+
+    def getFitIntercept(self) -> bool:
+        return self.getOrDefault(self.fitIntercept)
+
+    def getStandardization(self) -> bool:
+        return self.getOrDefault(self.standardization)
+
+    def getFamily(self) -> str:
+        return self.getOrDefault(self.family)
+
+    def getThreshold(self) -> float:
+        return self.getOrDefault(self.threshold)
+
+    def getProbabilityCol(self) -> str:
+        return self.getOrDefault(self.probabilityCol)
+
+    def getRawPredictionCol(self) -> str:
+        return self.getOrDefault(self.rawPredictionCol)
+
+
+class _LogisticRegressionCumlParams(_CumlParams, _LogisticRegressionParams, HasFeaturesCols):
+    """Shared Spark Params of LogisticRegression and LogisticRegressionModel (reference: classification.py:750-819)."""
+
+    def getFeaturesCol(self) -> Union[str, List[str]]:  # type: ignore[override]
+        if self.isDefined(self.featuresCols):
+            return self.getFeaturesCols()
+        if self.isDefined(self.featuresCol):
+            return self.getOrDefault("featuresCol")
+        raise RuntimeError("featuresCol is not set")
+
+    def setFeaturesCol(self: P, value: Union[str, List[str]]) -> P:
+        if isinstance(value, str):
+            self._set_params(featuresCol=value)
+        else:
+            self._set_params(featuresCols=value)
+        return self
+
+    def setFeaturesCols(self: P, value: List[str]) -> P:
+        return self._set_params(featuresCols=value)
+
+    def setLabelCol(self: P, value: str) -> P:
+        return self._set_params(labelCol=value)
+
+    def setPredictionCol(self: P, value: str) -> P:
+        return self._set_params(predictionCol=value)
+
+    def setProbabilityCol(self: P, value: str) -> P:
+        return self._set_params(probabilityCol=value)
+
+    def setRawPredictionCol(self: P, value: str) -> P:
+        return self._set_params(rawPredictionCol=value)
+
+    def setThreshold(self: P, value: float) -> P:
+        return self._set_params(threshold=value)
+
+    def setThresholds(self: P, value: List[float]) -> P:
+        return self._set_params(thresholds=value)
+
+
+# Params a fitMultiple map may change while every map is still fitted from one ingest, label pass and moments pass
+_SOLVER_PARAMS = frozenset(("regParam", "elasticNetParam", "maxIter", "tol", "fitIntercept", "standardization",
+                            "family"))
+
+
+def _fit_settings(est: "_LogisticRegressionCumlParams") -> Dict[str, Any]:
+    family = est.getFamily().lower()
+    if family not in ("auto", "binomial", "multinomial"):
+        raise ValueError(f"family given invalid value {est.getFamily()}")
+    return {"reg": float(est.getRegParam()), "l1_ratio": float(est.getElasticNetParam()), "tol": float(est.getTol()),
+            "max_iter": int(est.getMaxIter()), "fit_intercept": bool(est.getFitIntercept()),
+            "standardization": bool(est.getStandardization()), "family": family}
+
+
+def _check_settings(s: Dict[str, Any]) -> None:
+    """The errors b2k_logreg_fit would return, raised on the driver before any task starts."""
+    if s["max_iter"] < 0:
+        raise ValueError(f"maxIter given invalid value {s['max_iter']}")
+    if not s["reg"] >= 0:
+        raise ValueError(f"C or regParam given an invalid or unsupported value {s['reg']!r}")
+    if not 0 <= s["l1_ratio"] <= 1:
+        raise ValueError(f"elasticNetParam given invalid value {s['l1_ratio']!r}")
+    if not s["tol"] >= 0:
+        raise ValueError(f"tol given invalid value {s['tol']!r}")
+
+
+class LogisticRegression(LogisticRegressionClass, _CumlEstimator, _LogisticRegressionCumlParams):
+    """Logistic regression on H100: binomial or multinomial, with no penalty, L2, L1 or the elastic net, with or without
+    an intercept and standardization.  One barrier task per GPU holds its partition on the device; the label pass and
+    a column-moments pass run once, then every L-BFGS / OWL-QN step evaluates the loss and gradient in one fused fp64
+    pass over the rows and one NCCL allreduce.  Parameters as in the reference (classification.py:822-955):
+    featuresCol (str for an array column, list of str for scalar columns), labelCol, predictionCol, probabilityCol,
+    rawPredictionCol, maxIter (100), regParam (0.0), elasticNetParam (0.0), tol (1e-6), fitIntercept (True),
+    standardization (True), family ("auto"), num_workers, verbose.
+
+    >>> from spark_rapids_ml_b200.classification import LogisticRegression
+    >>> df = session.createDataFrame([([1.0, 2.0], 1.0), ([1.0, 3.0], 1.0), ([2.0, 1.0], 0.0), ([3.0, 1.0], 0.0)],
+    ...                              "features array<float>, label float")
+    >>> LogisticRegression(regParam=0.01).fit(df).coefficients   # [-2.48197, 2.48197]
+    """
+
+    @keyword_only
+    def __init__(self, *, featuresCol: Union[str, List[str]] = "features", labelCol: str = "label",
+                 predictionCol: str = "prediction", probabilityCol: str = "probability",
+                 rawPredictionCol: str = "rawPrediction", maxIter: int = 100, regParam: float = 0.0,
+                 elasticNetParam: float = 0.0, tol: float = 1e-6, fitIntercept: bool = True,
+                 standardization: bool = True, enable_sparse_data_optim: Optional[bool] = None,
+                 float32_inputs: bool = True, num_workers: Optional[int] = None, verbose: Union[int, bool] = False,
+                 **kwargs: Any) -> None:
+        super().__init__()
+        self._handle_param_spark_confs()
+        self._set_cuml_reg_params()
+        self._input_kwargs.pop("kwargs", None)
+        self._input_kwargs.update(kwargs)
+        if self._input_kwargs.pop("enable_sparse_data_optim", None):
+            raise ValueError("sparse input is not supported by spark_rapids_ml_b200's LogisticRegression")
+        if self._input_kwargs.get("num_workers", None) is None:
+            self._input_kwargs.pop("num_workers", None)
+        self._set_params(**self._input_kwargs)
+        self._fit_grid: Optional[List[Dict[str, Any]]] = None
+
+    def _set_cuml_reg_params(self) -> "LogisticRegression":
+        penalty, C, l1_ratio = self._reg_params_value_mapping(self.getRegParam(), self.getElasticNetParam())
+        self._cuml_params["penalty"] = penalty
+        self._cuml_params["C"] = C
+        self._cuml_params["l1_ratio"] = l1_ratio
+        return self
+
+    def _set_params(self, **kwargs: Any) -> "LogisticRegression":
+        super()._set_params(**kwargs)
+        if "regParam" in kwargs or "elasticNetParam" in kwargs:
+            self._set_cuml_reg_params()
+        return self
+
+    def setMaxIter(self, value: int) -> "LogisticRegression":
+        return self._set_params(maxIter=value)
+
+    def setRegParam(self, value: float) -> "LogisticRegression":
+        return self._set_params(regParam=value)
+
+    def setElasticNetParam(self, value: float) -> "LogisticRegression":
+        return self._set_params(elasticNetParam=value)
+
+    def setTol(self, value: float) -> "LogisticRegression":
+        return self._set_params(tol=value)
+
+    def setFitIntercept(self, value: bool) -> "LogisticRegression":
+        return self._set_params(fitIntercept=value)
+
+    def setStandardization(self, value: bool) -> "LogisticRegression":
+        return self._set_params(standardization=value)
+
+    def setFamily(self, value: str) -> "LogisticRegression":
+        return self._set_params(family=value)
+
+    def setWeightCol(self, value: str) -> "LogisticRegression":
+        raise ValueError("'weightCol' is not supported by cuML.")
+
+    def _validate_parameters(self) -> None:
+        super()._validate_parameters()
+        _check_settings(_fit_settings(self))
+
+    def _fit_label_col(self) -> Optional[str]:
+        return self.getLabelCol()
+
+    def _pre_process_data(self, dataset: LocalDataFrame) -> Tuple[LocalDataFrame, Optional[List[str]], int, str]:
+        """The feature columns as for every estimator, plus the label cast to float32 as alias.label."""
+        label = self.getLabelCol()
+        if label not in dataset.columns:
+            raise ValueError(f"label column '{label}' not found in {dataset.columns}")
+        df, multi_col_names, dimension, ftype = super()._pre_process_data(dataset)
+        df = df.with_appended_column(alias.label, [[b.column(label).cast(pa.float32()) for b in p] for p in dataset._parts])
+        return df, multi_col_names, dimension, ftype
+
+    def _get_cuml_fit_func(self, dataset: Any, extra_params: Optional[List[Dict[str, Any]]] = None
+                           ) -> Callable[[FitInputType, Dict[str, Any]], Dict[str, Any]]:
+        grid = self._fit_grid if self._fit_grid is not None else [_fit_settings(self)]
+
+        def _cuml_fit(dfs: FitInputType, params: Dict[str, Any]) -> Dict[str, Any]:
+            # stands in for LogisticRegressionMG(handle, ...).fit(...) per param map, the rescaling and the intercept
+            # centring — classification.py:984-1192; one label pass and one moments pass serve every map
+            ctx = params[param_alias.handle]
+            if len(dfs) != 1:
+                raise RuntimeError("the worker scaffold hands the fit function ONE device matrix per partition")
+            X, y, _ = dfs[0]
+            classes, counts, _n = ctx.logreg_labels(y)
+            fits = ctx.logreg_fit(X, y, classes, counts, grid)
+            out: Dict[str, List[Any]] = {"coef_": [], "intercept_": [], "classes_": [], "n_cols": [], "dtype": [],
+                                         "num_iters": []}
+            for coef, icpt, iters in fits:
+                out["coef_"].append(coef.tolist())
+                out["intercept_"].append(icpt.tolist())
+                out["classes_"].append(classes.tolist())
+                out["n_cols"].append(params[param_alias.num_cols])
+                out["dtype"].append("float32")
+                out["num_iters"].append(iters)
+            return out
+
+        return _cuml_fit
+
+    def _out_schema(self) -> Any:
+        return ("coef_ array<array<double>>, intercept_ array<double>, classes_ array<double>, n_cols int, "
+                "dtype string, num_iters int")
+
+    def _create_pyspark_model(self, result: Row) -> "LogisticRegressionModel":
+        r = result.asDict()
+        if len(r["classes_"]) == 1:
+            if self.getFitIntercept() is False:
+                raise ValueError("All labels belong to a single class and fitIntercept=false. This is not supported.  "
+                                 "Please use fitIntercept=true.")
+            self.logger.warning("All labels are the same value and fitIntercept=true, so the coefficients will be "
+                                "zeros. Training is not needed.")
+        return LogisticRegressionModel(coef_=[list(c) for c in r["coef_"]], intercept_=list(r["intercept_"]),
+                                       classes_=list(r["classes_"]), n_cols=int(r["n_cols"]), dtype=str(r["dtype"]),
+                                       num_iters=int(r["num_iters"]))
+
+    def _enable_fit_multiple_in_single_pass(self) -> bool:
+        return True
+
+    def fitMultiple(self, dataset: Any, paramMaps: Sequence[Dict[Any, Any]]) -> Iterator[Tuple[int, Any]]:
+        """(index, model) per param map, in map order.  When every map changes only fit params (regParam,
+        elasticNetParam, maxIter, tol, fitIntercept, standardization, family), one ingest, one label pass and one
+        moments pass serve all maps, each then optimised on its own; otherwise each map is one fit."""
+        if paramMaps and all(p.name in _SOLVER_PARAMS for pm in paramMaps for p in pm):
+            est = self.copy()
+            est._fit_grid = [_fit_settings(self.copy(pm)) for pm in paramMaps]
+            for s in est._fit_grid:
+                _check_settings(s)
+            if est._use_cpu_fallback():
+                raise ValueError("a Spark Param without GPU support is set and spark_rapids_ml_b200 has no CPU fallback")
+            return _ModelIterator(est._fit_internal(dataset, list(paramMaps)))
+        return _ModelIterator([self.copy(pm)._fit(dataset) for pm in paramMaps])
+
+
+class LogisticRegressionModel(LogisticRegressionClass, _CumlModelWithPredictionCol, _LogisticRegressionCumlParams):
+    """reference: classification.py:1306-1614.  transform() appends rawPredictionCol and probabilityCol (double
+    vectors) and predictionCol (double)."""
+
+    def __init__(self, coef_: Union[List[List[float]], List[List[List[float]]]],
+                 intercept_: Union[List[float], List[List[float]]], classes_: List[float], n_cols: int, dtype: str,
+                 num_iters: int) -> None:
+        super().__init__(dtype=dtype, n_cols=n_cols, coef_=coef_, intercept_=intercept_, classes_=classes_,
+                         num_iters=num_iters)
+        self.coef_ = coef_
+        self.intercept_ = intercept_
+        self.classes_ = classes_
+        self._num_classes = len(self.classes_)
+        self.num_iters = num_iters
+
+    def _get_num_models(self) -> int:
+        return 1 if isinstance(self.intercept_[0], float) else len(self.intercept_)
+
+    @property
+    def coefficients(self) -> Any:
+        """pyspark DenseVector when pyspark.ml.linalg provides it, else a numpy array."""
+        if isinstance(self.coef_[0][0], float):
+            if len(self.coef_) == 1:
+                return _dense(self.coef_[0])
+            raise Exception("Multinomial models contain a matrix of coefficients, use coefficientMatrix instead.")
+        raise Exception("coefficients not defined for multi-model instance")
+
+    @property
+    def intercept(self) -> float:
+        if isinstance(self.intercept_[0], float):
+            if len(self.intercept_) == 1:
+                return self.intercept_[0]  # type: ignore[return-value]
+            raise Exception("Multinomial models contain a vector of intercepts, use interceptVector instead.")
+        raise Exception("intercept not defined for multi-model instance")
+
+    @property
+    def coefficientMatrix(self) -> Any:
+        """pyspark DenseMatrix when pyspark.ml.linalg provides it, else a numpy array [numCoefficientSets, numFeatures]."""
+        if isinstance(self.coef_[0][0], float):
+            rows, cols = len(self.coef_), len(self.coef_[0])
+            flat = [float(c) for row in self.coef_ for c in row]  # type: ignore[union-attr]
+            try:
+                from pyspark.ml.linalg import DenseMatrix
+            except ImportError:
+                return np.array(flat, dtype=np.float64).reshape(rows, cols)
+            return DenseMatrix(numRows=rows, numCols=cols, values=flat, isTransposed=True)
+        raise Exception("coefficientMatrix not defined for multi-model instance")
+
+    @property
+    def interceptVector(self) -> Any:
+        """Spark's interceptVector.compressed: sparse when 1.5 (nnz + 1) < size (pyspark vectors when available)."""
+        if isinstance(self.intercept_[0], float):
+            nnz = int(np.count_nonzero(self.intercept_))
+            size = len(self.intercept_)
+            if 1.5 * (nnz + 1.0) < size:
+                try:
+                    from pyspark.ml.linalg import Vectors
+                except ImportError:
+                    return _SparseIntercepts(size, {i: float(v) for i, v in enumerate(self.intercept_) if v != 0})
+                return Vectors.sparse(size, {i: float(v) for i, v in enumerate(self.intercept_)})
+            return _dense(self.intercept_)  # type: ignore[arg-type]
+        raise Exception("interceptVector not defined for multi-model instance")
+
+    @property
+    def numClasses(self) -> int:
+        return self._num_classes
+
+    @property
+    def hasSummary(self) -> bool:
+        return False
+
+    @property
+    def summary(self) -> Any:
+        raise RuntimeError("No training summary available for this %s" % self.__class__.__name__)
+
+    def predict(self, value: Any) -> float:
+        raise NotImplementedError("LogisticRegressionModel.predict() of a single vector is not supported; use transform()")
+
+    def predictRaw(self, value: Any) -> Any:
+        raise NotImplementedError("LogisticRegressionModel.predictRaw() of a single vector is not supported; use "
+                                  "transform()")
+
+    def predictProbability(self, value: Any) -> Any:
+        raise NotImplementedError("LogisticRegressionModel.predictProbability() of a single vector is not supported; "
+                                  "use transform()")
+
+    def evaluate(self, dataset: Any) -> Any:
+        raise NotImplementedError("LogisticRegressionModel.evaluate() is not supported in this build")
+
+    def cpu(self) -> Any:
+        raise NotImplementedError("LogisticRegressionModel.cpu() builds a JVM pyspark.ml model; no JVM/pyspark in this "
+                                  "build")
+
+    @classmethod
+    def _combine(cls, models: List["LogisticRegressionModel"]) -> "LogisticRegressionModel":
+        """One model holding several fits' coefficients (reference classification.py:1557-1572)."""
+        assert len(models) > 0 and all(isinstance(m, cls) for m in models)
+        first = models[0]
+        attrs = dict(first._get_model_attributes() or {})
+        attrs["coef_"] = [m.coef_ for m in models]
+        attrs["intercept_"] = [m.intercept_ for m in models]
+        out = cls(**attrs)
+        first._copyValues(out)
+        first._copy_cuml_params(out)
+        return out
+
+    def _out_schema(self, input_schema: Any = None) -> str:
+        return "double"
+
+    def _device_model(self) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+        if self._get_num_models() != 1:
+            raise NotImplementedError("transform() of a combined multi-model instance is not supported")
+        W = np.asarray(self.coef_, dtype=np.float64)
+        b = np.asarray(self.intercept_, dtype=np.float64)
+        cls = np.asarray(self.classes_, dtype=np.float64)
+        if W.shape[0] == 1 and cls.size == 1:   # one label seen: the binomial model of that label
+            cls = np.array([0.0, 1.0])
+        return W, b, cls
+
+    def _get_cuml_transform_func(self, dataset: Any, eval_metric_info: Any = None
+                                 ) -> Tuple[Callable, Callable, Optional[Callable]]:
+        W, b, cls = self._device_model()
+        n_cols = int(self.n_cols)
+
+        class _DeviceLogReg:
+            def __init__(self, gpu: int) -> None:
+                self.ctx = _transform_context(gpu)
+
+            def close(self) -> None:   # the context stays with the process
+                pass
+
+        def _construct(gpu: int = 0) -> Any:
+            return _DeviceLogReg(gpu)
+
+        def _transform_many(lr: Any, dfs: List[Union[pd.DataFrame, np.ndarray]]) -> List[pd.DataFrame]:
+            """Several input batches in ONE device pass: every batch is ingested into the same device matrix, one
+            b2k_logreg_predict covers all rows, one read-back, one frame (rawPrediction, probability, prediction) per
+            input batch."""
+            from .utils import DeviceRowAppender
+
+            sizes = [len(df) for df in dfs]
+            total = sum(sizes)
+            nout = 2 if W.shape[0] == 1 else W.shape[0]
+            if total == 0:
+                return [pd.DataFrame({"raw": [], "prob": [], "pred": pd.Series([], dtype="float64")}) for _ in dfs]
+            app = DeviceRowAppender(lr.ctx, n_cols, first_capacity=total)
+            for df, n_b in zip(dfs, sizes):
+                if n_b:
+                    _append_transform_features(app, df, n_cols)
+            raw, prob, pred = lr.ctx.logreg_predict(app.finish(), W, b, cls[:nout] if W.shape[0] > 1 else cls[:2])
+            raw, prob, pred = raw.cpu().numpy(), prob.cpu().numpy(), pred.cpu().numpy()
+            out, o = [], 0
+            for n_b in sizes:
+                out.append(pd.DataFrame({"raw": list(raw[o:o + n_b]), "prob": list(prob[o:o + n_b]),
+                                         "pred": pred[o:o + n_b]}))
+                o += n_b
+            return out
+
+        def _transform_internal(lr: Any, df: Union[pd.DataFrame, np.ndarray]) -> pd.DataFrame:
+            return _transform_many(lr, [df])[0]
+
+        _transform_internal.many = _transform_many  # type: ignore[attr-defined]
+        _transform_internal.row_bytes = 4 * n_cols + 8 * (2 * max(2, W.shape[0]) + 1)  # type: ignore[attr-defined]
+        return _construct, _transform_internal, None
+
+    def _transform(self, dataset: Any) -> Any:
+        """Appends rawPredictionCol, probabilityCol (list<double>) and predictionCol (double) to a local frame."""
+        from .core import HAVE_PYSPARK, _iter_transform
+
+        if HAVE_PYSPARK:
+            from . import spark_binding
+
+            if spark_binding.is_spark_dataframe(dataset):
+                raise NotImplementedError("LogisticRegressionModel.transform() of a pyspark DataFrame is not supported in "
+                                          "this build; transform a local frame")
+        input_col, input_cols = self._get_input_columns()
+        construct, transform_internal, _ = self._get_cuml_transform_func(dataset)
+        cols: Dict[str, List[List[pa.Array]]] = {"raw": [], "prob": [], "pred": []}
+        state: Dict[str, Any] = {}
+        for pid, part in enumerate(dataset._parts):
+            def frames(part: Any = part, pid: int = pid) -> Iterator[Any]:
+                from .sparkshim.sql import _batches_to_pdf_iter
+
+                def selected() -> Iterator[pa.RecordBatch]:
+                    for batch in part:
+                        if "model" not in state:
+                            gpu = _CumlCommon._set_gpu_device(BarrierTaskContext(pid, len(dataset._parts)), True, True)
+                            state["model"] = construct(gpu)
+                        if input_cols:
+                            yield batch.select(list(input_cols))
+                        else:
+                            yield batch.select([input_col]).rename_columns([alias.data])
+
+                return _batches_to_pdf_iter(selected(), dataset.arrow_backed_pandas)
+
+            per = {k: [] for k in cols}
+            for res in _iter_transform(transform_internal, lambda: state["model"], frames()):
+                for k in ("raw", "prob"):
+                    rows = list(res[k])
+                    width = len(rows[0]) if rows else 0
+                    vals = np.asarray(rows, dtype=np.float64).reshape(-1) if rows else np.zeros(0)
+                    offs = np.arange(0, len(rows) * width + 1, max(width, 1), dtype=np.int32)[: len(rows) + 1]
+                    per[k].append(pa.ListArray.from_arrays(pa.array(offs), pa.array(vals, type=pa.float64())))
+                per["pred"].append(pa.array(np.asarray(res["pred"], dtype=np.float64), type=pa.float64()))
+            for k in cols:
+                cols[k].append(per[k])
+        out = dataset.with_appended_column(self.getRawPredictionCol(), cols["raw"])
+        out = out.with_appended_column(self.getProbabilityCol(), cols["prob"])
+        return out.with_appended_column(self.getOrDefault("predictionCol"), cols["pred"])
+
+
+def _dense(values: Sequence[float]) -> Any:
+    try:
+        from pyspark.ml.linalg import DenseVector
+    except ImportError:
+        return np.array(values, dtype=np.float64)
+    return DenseVector(list(values))
+
+
+class _SparseIntercepts:
+    """A sparse vector (size, {index: value}) without pyspark: toArray() gives the dense values."""
+
+    def __init__(self, size: int, values: Dict[int, float]) -> None:
+        self.size = size
+        self.values = values
+
+    def toArray(self) -> np.ndarray:
+        a = np.zeros(self.size, dtype=np.float64)
+        for i, v in self.values.items():
+            a[i] = v
+        return a

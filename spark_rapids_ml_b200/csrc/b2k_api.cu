@@ -1002,3 +1002,62 @@ extern "C" int b2k_linreg_predict(b2k_ctx* ctx, const float* X, int64_t n, int d
   B2K_CUDA_OK(ctx, cudaSetDevice(ctx->device));
   return b2k_linreg_predict_impl(ctx, X, n, d, coef, intercept, out, reinterpret_cast<cudaStream_t>(stream));
 }
+
+// ------------------------------------------------------------------------------------------------
+// logistic regression (b2k_logreg.cu)
+// ------------------------------------------------------------------------------------------------
+extern "C" int b2k_logreg_labels(b2k_ctx* ctx, const float* y, int64_t n_local, double* classes_out, int64_t* counts_out,
+                                 int* n_classes_out, int64_t* n_total_out, uintptr_t stream) {
+  if (!ctx) return b2k_fail(nullptr, B2K_ERR_INVALID, "b2k_logreg_labels: ctx is NULL");
+  // an empty partition may come with no buffer: the collective check below reports it on every rank
+  if ((!y && n_local > 0) || n_local < 0) return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_logreg_labels: bad y/n");
+  if (!classes_out || !counts_out || !n_classes_out) return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_logreg_labels: NULL output");
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  B2K_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  B2K_TRY(check_no_empty_partition(ctx, "b2k_logreg_labels", n_local, s));
+  return b2k_logreg_labels_impl(ctx, y, n_local, classes_out, counts_out, n_classes_out, n_total_out, s);
+}
+
+extern "C" int b2k_logreg_eval(b2k_ctx* ctx, const float* X, const float* y, int64_t n_local, int d, const double* classes,
+                               int n_classes, int kp, const double* W, const double* b, double* loss_out,
+                               double* grad_out, int64_t* n_total_out, uintptr_t stream) {
+  if (!ctx) return b2k_fail(nullptr, B2K_ERR_INVALID, "b2k_logreg_eval: ctx is NULL");
+  if (((!X || !y) && n_local > 0) || n_local < 0 || d <= 0)
+    return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_logreg_eval: bad X/y/n/d");
+  if (!classes || !W || !b || !loss_out || !grad_out) return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_logreg_eval: NULL argument");
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  B2K_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  B2K_TRY(check_no_empty_partition(ctx, "b2k_logreg_eval", n_local, s));
+  return b2k_logreg_eval_impl(ctx, X, y, n_local, d, classes, n_classes, kp, W, b, loss_out, grad_out, n_total_out, s);
+}
+
+extern "C" int b2k_logreg_minimize(b2k_logreg_objective fn, void* user, int n, double* x, const double* l1, int max_iter,
+                                   double tol, int* n_iter_out, int* n_eval_out, double* f_out) {
+  return b2k_logreg_minimize_impl(fn, user, n, x, l1, max_iter, tol, n_iter_out, n_eval_out, f_out);
+}
+
+extern "C" int b2k_logreg_fit(b2k_ctx* ctx, const float* X, const float* y, int64_t n_local, int d, const double* classes,
+                              const int64_t* counts, int n_classes, int n_fits, const b2k_logreg_params* params,
+                              double* coef_out, double* intercept_out, int* kp_out, int* n_iter_out, uintptr_t stream) {
+  if (!ctx) return b2k_fail(nullptr, B2K_ERR_INVALID, "b2k_logreg_fit: ctx is NULL");
+  if (((!X || !y) && n_local > 0) || n_local < 0 || d <= 0)
+    return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_logreg_fit: bad X/y/n/d");
+  if (!classes || !counts || n_fits < 1 || !params || !coef_out || !intercept_out || !kp_out || !n_iter_out)
+    return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_logreg_fit: NULL argument or n_fits < 1");
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  B2K_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  B2K_TRY(check_no_empty_partition(ctx, "b2k_logreg_fit", n_local, s));
+  return b2k_logreg_fit_impl(ctx, X, y, n_local, d, classes, counts, n_classes, n_fits, params, coef_out, intercept_out,
+                             kp_out, n_iter_out, s);
+}
+
+extern "C" int b2k_logreg_predict(b2k_ctx* ctx, const float* X, int64_t n, int d, int kp, const double* W, const double* b,
+                                  const double* class_values, double* raw_out, double* prob_out, double* pred_out,
+                                  uintptr_t stream) {
+  if (!ctx) return b2k_fail(nullptr, B2K_ERR_INVALID, "b2k_logreg_predict: ctx is NULL");
+  if (!X || !W || !b || !class_values || !raw_out || !prob_out || !pred_out || n < 0 || d <= 0 || kp < 1)
+    return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_logreg_predict: bad X/W/b/outputs/n/d/kp");
+  B2K_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  return b2k_logreg_predict_impl(ctx, X, n, d, kp, W, b, class_values, raw_out, prob_out, pred_out,
+                                 reinterpret_cast<cudaStream_t>(stream));
+}

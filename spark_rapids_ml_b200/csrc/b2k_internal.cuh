@@ -299,3 +299,26 @@ int b2k_linreg_solve_impl(const double* mean, const double* moments, int d, int6
                           double* coef_out, double* intercept_out, int* n_iter_out);
 int b2k_linreg_predict_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, const double* coef, double intercept,
                             double* out, cudaStream_t s);
+
+// ------------------------------------------------------------------------------------------------
+// logistic regression — b2k_logreg.cu (the C ABI entry points in b2k_api.cu check their arguments, then call these)
+// ------------------------------------------------------------------------------------------------
+constexpr int B2K_LOGREG_MAX_D = B2K_PCA_MAX_D;
+constexpr int B2K_LOGREG_MAX_CLASSES = 1024;   // label values in [0, 1024): the label pass counts each value
+// Column moments (b2k_pca.cu, collective): *n_total, mu [d] = fp64 means, ssq [d] = sum (x - mu)^2, from column sums
+// and a pass of squares centred on mu32 = fl32(mu) with the offset removed exactly.  Two f64 allreduces.
+int b2k_colstats_impl(b2k_ctx* ctx, const char* who, const float* X, int64_t n, int d, int64_t* n_total,
+                      std::vector<double>* mu, std::vector<double>* ssq, cudaStream_t s);
+int b2k_logreg_labels_impl(b2k_ctx* ctx, const float* y, int64_t n, double* classes_out, int64_t* counts_out,
+                           int* n_classes_out, int64_t* n_total_out, cudaStream_t s);
+int b2k_logreg_eval_impl(b2k_ctx* ctx, const float* X, const float* y, int64_t n, int d, const double* classes,
+                         int n_classes, int kp, const double* W, const double* b, double* loss_out, double* grad_out,
+                         int64_t* n_total_out, cudaStream_t s);
+int b2k_logreg_minimize_impl(b2k_logreg_objective fn, void* user, int n, double* x_io, const double* l1, int max_iter,
+                             double tol, int* n_iter_out, int* n_eval_out, double* f_out);
+int b2k_logreg_fit_impl(b2k_ctx* ctx, const float* X, const float* y, int64_t n, int d, const double* classes,
+                        const int64_t* counts, int n_classes, int n_fits, const b2k_logreg_params* prm,
+                        double* coef_out, double* intercept_out, int* kp_out, int* n_iter_out, cudaStream_t s);
+int b2k_logreg_predict_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, int kp, const double* W, const double* b,
+                            const double* class_values, double* raw_out, double* prob_out, double* pred_out,
+                            cudaStream_t s);

@@ -47,6 +47,32 @@ k_colsum(const float* __restrict__ X, int64_t n, int d, int64_t span_rows, doubl
   }
 }
 
+// part[span][c] = sum (x_c - mu32_c)^2 over the span's rows: k_colsum's layout, the fp32 difference exact in fp64
+__global__ void __launch_bounds__(CS_TX * CS_TY)
+k_colsq(const float* __restrict__ X, int64_t n, int d, const float* __restrict__ mu, int64_t span_rows,
+        double* __restrict__ part) {
+  __shared__ double red[CS_TY][CS_TX];
+  const int c = blockIdx.y * CS_TX + threadIdx.x;
+  const int64_t r0 = (int64_t)blockIdx.x * span_rows;
+  const int64_t r1 = min(n, r0 + span_rows);
+  double s = 0.0;
+  if (c < d) {
+    const double m = (double)mu[c];
+#pragma unroll 4
+    for (int64_t r = r0 + threadIdx.y; r < r1; r += CS_TY) {
+      const double t = (double)X[r * d + c] - m;
+      s = fma(t, t, s);
+    }
+  }
+  red[threadIdx.y][threadIdx.x] = s;
+  __syncthreads();
+  if (threadIdx.y == 0 && c < d) {
+    double t = 0.0;
+    for (int y = 0; y < CS_TY; ++y) t += red[y][threadIdx.x];
+    part[(size_t)blockIdx.x * d + c] = t;
+  }
+}
+
 // sums[c] = sum over spans in order; sums[d] = n (the allreduce turns it into n_total)
 __global__ void k_colsum_fold(const double* __restrict__ part, int nspan, int d, int64_t n, double* __restrict__ sums) {
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
@@ -508,6 +534,65 @@ int b2k_moments_impl(b2k_ctx* ctx, const char* who, const float* X, const float*
     ctx->stats.last_fused_ms = tm.ms(3, 4);
     if (y) ctx->stats.last_finalize_ms = tm.ms(4, 6);
   }
+  return B2K_OK;
+}
+
+int b2k_colstats_impl(b2k_ctx* ctx, const char* who, const float* X, int64_t n, int d, int64_t* n_total,
+                      std::vector<double>* mu, std::vector<double>* ssq, cudaStream_t s) {
+  const int ncb = (d + CS_TX - 1) / CS_TX;
+  const int64_t nspan_max = std::max<int64_t>(1, (n + 63) / 64);
+  const int nspan = (int)std::min<int64_t>(std::max(1, (8 * ctx->sm_count + ncb - 1) / ncb), nspan_max);
+  const int64_t span_rows = std::max<int64_t>(1, (n + nspan - 1) / nspan);
+  double *colp, *sums, *sq;
+  float* mu32_dev;
+  B2K_TRY(b2k_scratch_layout(ctx, who, [&](B2kLayout& L) -> int {
+    colp = L.take<double>((size_t)nspan * d);
+    sums = L.take<double>((size_t)d + 1);
+    sq = L.take<double>((size_t)d + 1);
+    mu32_dev = L.take<float>((size_t)d);
+    return B2K_OK;
+  }));
+  // sums and n, allreduced; then the centred squares on mu32
+  if (n > 0) {
+    k_colsum<<<dim3(nspan, ncb), dim3(CS_TX, CS_TY), 0, s>>>(X, n, d, span_rows, colp);
+    B2K_CUDA_OK(ctx, cudaGetLastError());
+    ctx->stats.kernel_launches++;
+  } else {
+    B2K_CUDA_OK(ctx, cudaMemsetAsync(colp, 0, (size_t)nspan * d * 8, s));
+  }
+  k_colsum_fold<<<(d + 1 + 255) / 256, 256, 0, s>>>(colp, nspan, d, n, sums);
+  B2K_CUDA_OK(ctx, cudaGetLastError());
+  ctx->stats.kernel_launches++;
+  B2K_TRY(b2k_comm_allreduce_f64(ctx, sums, (size_t)d + 1, s));
+  std::vector<double> hs((size_t)d + 1);
+  B2K_CUDA_OK(ctx, cudaMemcpyAsync(hs.data(), sums, hs.size() * 8, cudaMemcpyDeviceToHost, s));
+  B2K_CUDA_OK(ctx, cudaStreamSynchronize(s));
+  const int64_t nt = (int64_t)std::llround(hs[d]);
+  if (nt < 1) return b2k_fail(ctx, B2K_ERR_INVALID, std::string(who) + " needs at least 1 row, got 0");
+  mu->assign(d, 0.0);
+  std::vector<float> mu32(d);
+  for (int c = 0; c < d; ++c) {
+    (*mu)[c] = hs[c] / (double)nt;
+    mu32[c] = (float)(*mu)[c];
+  }
+  B2K_CUDA_OK(ctx, cudaMemcpyAsync(mu32_dev, mu32.data(), (size_t)d * 4, cudaMemcpyHostToDevice, s));
+  if (n > 0) {
+    k_colsq<<<dim3(nspan, ncb), dim3(CS_TX, CS_TY), 0, s>>>(X, n, d, mu32_dev, span_rows, colp);
+    B2K_CUDA_OK(ctx, cudaGetLastError());
+    ctx->stats.kernel_launches++;
+  }
+  k_colsum_fold<<<(d + 1 + 255) / 256, 256, 0, s>>>(colp, nspan, d, 0, sq);
+  B2K_CUDA_OK(ctx, cudaGetLastError());
+  ctx->stats.kernel_launches++;
+  B2K_TRY(b2k_comm_allreduce_f64(ctx, sq, (size_t)d, s));
+  ssq->assign(d, 0.0);
+  B2K_CUDA_OK(ctx, cudaMemcpyAsync(ssq->data(), sq, (size_t)d * 8, cudaMemcpyDeviceToHost, s));
+  B2K_CUDA_OK(ctx, cudaStreamSynchronize(s));
+  for (int c = 0; c < d; ++c) {   // sum (x - mu)^2 = sum (x - mu32)^2 - n (mu - mu32)^2
+    const double dl = (*mu)[c] - (double)mu32[c];
+    (*ssq)[c] -= (double)nt * dl * dl;
+  }
+  *n_total = nt;
   return B2K_OK;
 }
 
