@@ -138,7 +138,8 @@ int b2k_ctx_destroy(b2k_ctx* ctx);
  *   "time_kernels"     0/1/2: CUDA events around every fused launch; 2 = also around the partial fold, the allreduce and
  *                      finalize
  *   "check_every"      iterations between host convergence polls, default 4
- *   "grid_limit"       cap on persistent CTAs, 0 = #SMs
+ *   "grid_limit"       cap on persistent CTAs, 0 = #SMs; also caps the CTAs of the fused logistic pass (0 = as many as
+ *                      fit on every SM at once)
  *   "variant_t"        1 = route every shape with k, d <= 256 through the large-shape kernel b2k_fused_t.cu; default 0 =
  *                      only shapes the 3xTF32 kernel does not cover
  *   "collect_recheck"  1 = lloyd/assign synchronise and fill b2k_stats.recheck_*
@@ -305,9 +306,12 @@ int b2k_logreg_labels(b2k_ctx* ctx, const float* y, int64_t n_local, double* cla
  * f32).  classes [n_classes] are the class values (b2k_logreg_labels); a row whose label is not one of them counts as no
  * class.  kp = 1: the binomial loss with class index 1 the positive class.  Outputs (host): *loss_out, grad_out
  * [kp][d + 1] = (1/n) sum r_k x_j, then (1/n) sum r_k in column d; *n_total_out (may be NULL).  The fused pass
- * (k_logreg_eval) runs where its accumulators fit: K' classes per thread block of at most 16 with d * ceil(K'/KB) <=
- * 256 NIT (binomial: d <= 1024; K <= 16: d <= 256); elsewhere the generic rows + X^T R passes.  Option "kernel_path" as
- * for PCA; stats.last_path reports the pass; with "time_kernels", last_fused_ms = its device time.  Errors: an empty
+ * (k_logreg_eval) runs where its accumulators and its shared memory fit: a class block of KB = 1, 2, 4, 8 or 16 (the
+ * least >= K', at most 16) and d * ceil(K'/KB) <= 256 NIT (NIT = 4 for KB <= 4, 2 for KB = 8, 1 for KB = 16), i.e.
+ * K' <= 4 at every d <= 1024, K' <= 8 at d <= 512, K' <= 16 at d <= 256, K' <= 32 at d <= 128 and so on, while its
+ * shared memory fits the device's opt-in limit (which alone bounds K' at small d); elsewhere the generic rows + X^T R
+ * passes.  Option "kernel_path" as for PCA, option "grid_limit" caps the fused pass's CTAs; stats.last_path reports the
+ * pass; with "time_kernels", last_fused_ms = its device time.  Errors: an empty
  * partition; d > 1024 (B2K_ERR_UNSUPPORTED).  Synchronises `stream`.  Bitwise reproducible for the same input, rank
  * count and device. */
 int b2k_logreg_eval(b2k_ctx* ctx, const float* X, const float* y, int64_t n_local, int d, const double* classes,

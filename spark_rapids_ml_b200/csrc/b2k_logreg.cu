@@ -868,7 +868,9 @@ int eval_device(b2k_ctx* ctx, const EvalCall& e, const double* W, const double* 
     int per_sm = 0;
     B2K_CUDA_OK(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fp.kern, LR_THREADS, smem));
     const int64_t tiles = std::max<int64_t>(1, (n + tr - 1) / tr);
-    const int64_t g0 = std::min<int64_t>(tiles, (int64_t)std::max(1, per_sm) * ctx->sm_count);
+    int64_t cap = (int64_t)std::max(1, per_sm) * ctx->sm_count;
+    if (ctx->grid_limit > 0 && ctx->grid_limit < cap) cap = ctx->grid_limit;
+    const int64_t g0 = std::min<int64_t>(tiles, cap);
     span_rows = (tiles + g0 - 1) / g0 * tr;
     grid = (int)std::max<int64_t>(1, (n + span_rows - 1) / span_rows);
     P = grid * fused_shape(d, kp, fp.KB, tr).rg;

@@ -29,8 +29,10 @@ def sigma(X: np.ndarray) -> np.ndarray:
 
 
 def loss_grad(X: np.ndarray, yi: np.ndarray, W: np.ndarray, b: np.ndarray) -> Tuple[float, np.ndarray, np.ndarray]:
-    """(1/n) sum l and its gradient (dW [kp, d], db [kp]) at (W, b); yi are class indices."""
+    """(1/n) sum l and its gradient (dW [kp, d], db [kp]) at (W, b); yi are class indices, -1 for a row whose label is
+    none of the classes: its one-hot is zero (binomial: a negative row), as b2k_logreg_eval counts it."""
     X = np.asarray(X, dtype=np.float64)
+    yi = np.asarray(yi)
     n = X.shape[0]
     M = X @ np.asarray(W, dtype=np.float64).T + np.asarray(b, dtype=np.float64)
     kp = M.shape[1]
@@ -44,9 +46,11 @@ def loss_grad(X: np.ndarray, yi: np.ndarray, W: np.ndarray, b: np.ndarray) -> Tu
     else:
         mx = M.max(axis=1, keepdims=True)
         lse = mx[:, 0] + np.log(np.exp(M - mx).sum(axis=1))
-        loss = lse - M[np.arange(n), yi]
+        rows = np.flatnonzero(yi >= 0)
+        loss = lse.copy()
+        loss[rows] -= M[rows, yi[rows]]
         R = np.exp(M - lse[:, None])
-        R[np.arange(n), yi] -= 1.0
+        R[rows, yi[rows]] -= 1.0
     return float(loss.sum() / n), R.T @ X / n, R.sum(axis=0) / n
 
 

@@ -126,6 +126,28 @@ def test_stable_loss_at_large_margins():
             assert np.isfinite(loss) and np.all(np.isfinite(gW)) and np.all(np.isfinite(gb))
 
 
+def test_a_row_of_no_class_has_a_zero_one_hot():
+    rng = np.random.default_rng(11)
+    X = rng.normal(size=(6, 3))
+    for kp in (1, 4):
+        W, b = rng.normal(size=(kp, 3)), rng.normal(size=kp)
+        yi = np.array([0, 1, -1, 1, -1, 0]) if kp == 1 else np.array([0, 3, -1, 2, -1, 1])
+        loss, gW, gb = lo.loss_grad(X, yi, W, b)
+        M = X @ W.T + b
+        if kp == 1:   # a row of no class is a negative row
+            P = 1.0 / (1.0 + np.exp(-M))
+            L = np.log1p(np.exp(M[:, 0])) - (yi == 1) * M[:, 0]
+            Y = (yi == 1).astype(float)[:, None]
+        else:   # the loss is log-sum-exp alone and the residuals the softmax alone
+            P = np.exp(M) / np.exp(M).sum(axis=1, keepdims=True)
+            L = np.log(np.exp(M).sum(axis=1)) - np.where(yi >= 0, M[np.arange(6), np.maximum(yi, 0)], 0.0)
+            Y = np.zeros((6, kp))
+            Y[yi >= 0, yi[yi >= 0]] = 1.0
+        np.testing.assert_allclose(loss, L.mean(), rtol=1e-14)
+        np.testing.assert_allclose(gW, (P - Y).T @ X / 6, rtol=1e-12, atol=1e-15)
+        np.testing.assert_allclose(gb, (P - Y).sum(axis=0) / 6, rtol=1e-12, atol=1e-15)
+
+
 def test_known_answers_of_mllib_through_the_host_optimizer():
     """MLlib's published answers (tests/golden), to 1e-4 (the reference holds itself to 1e-3).  They pin the sample
     (n - 1) standard deviation: with the population one the standardized binomial coefficient is 2.678, not 2.482."""
