@@ -160,7 +160,9 @@ int b2k_get_stats(const b2k_ctx* ctx, b2k_stats* out);
 int b2k_get_fused_profile(b2k_ctx* ctx, long long* out, int64_t cap, int* grid_out, int* warps_out);
 int b2k_reset_stats(b2k_ctx* ctx);
 
-/* ---- communicator (NCCL over NVLink; one rank per process per GPU) ---- */
+/* ---- communicator (NCCL over NVLink; one rank per process per GPU).  libnccl is loaded at the first call: the library
+ * named by the environment variable B2K_NCCL_LIB when it is set (failing to load it is B2K_ERR_NCCL), else
+ * libnccl.so.2. ---- */
 int b2k_comm_unique_id(char out[B2K_UNIQUE_ID_BYTES]); /* rank 0 only */
 int b2k_comm_init(b2k_ctx* ctx, int nranks, int rank, const char uid[B2K_UNIQUE_ID_BYTES]);
 int b2k_comm_destroy(b2k_ctx* ctx);
@@ -182,14 +184,17 @@ int b2k_ingest_append(b2k_ctx* ctx, float* dst, int64_t n_max, int d, int64_t ro
  *   n_init         must be 1 (the reference forces n_init=1, clustering.py:316-319)
  *   centers_out    device f32 [k, d]
  *   n_iter_out, inertia_out   host; inertia_out may be NULL (skips the extra assign pass)
- * Collective across the communicator when one is initialised: every rank must call it. ---- */
+ * Collective across the communicator when one is initialised: every rank must call it.  An empty partition on any
+ * rank (n_local == 0, X may then be NULL) fails on every rank together. ---- */
 int b2k_kmeans_fit(b2k_ctx* ctx, const float* X, int64_t n_local, int d, int k, int init_mode,
                    const float* init_centers, int max_iter, double tol, uint64_t seed, double oversampling,
                    int n_init, float* centers_out, int* n_iter_out, double* inertia_out, uintptr_t stream);
 
 /* ---- the Lloyd loop alone, in place on device centers[k,d]: at most max_iter iterations of
  * {assign + per-cluster partial sums (one pass over X), allreduce(sum,count), finalize, convergence}.
- * shift_out (host, may be NULL) receives the last sum_j||dc_j||^2. ---- */
+ * shift_out (host, may be NULL) receives the last sum_j||dc_j||^2.  Collective like b2k_kmeans_fit: its sizes are
+ * allgathered first, so an empty partition on any rank (n_local == 0, X may then be NULL) fails on every rank together
+ * instead of running a loop whose allreduces would need every rank. ---- */
 int b2k_kmeans_lloyd(b2k_ctx* ctx, const float* X, int64_t n_local, int d, int k, float* centers,
                      int max_iter, double tol, int* n_iter_out, double* shift_out, uintptr_t stream);
 
@@ -210,7 +215,7 @@ int b2k_kmeans_assign(b2k_ctx* ctx, const float* X, int64_t n, int d, const floa
  * trace(covariance); singular_values_out [k] = sqrt(lambda_i (n_total - 1)).  Eigenvalues below 0 (rounding) count as 0.
  * Zero total variance (constant features) is not an error: the ratios and singular values are 0 and the components are
  * the first k unit vectors.  Errors: k < 1, k > d ("source vector size d must be no less than k"), n_total < 2, an
- * empty partition on any rank.  Collective across the communicator when one is initialised; synchronises `stream`
+ * empty partition on any rank (X may then be NULL; every rank fails together).  Collective across the communicator when one is initialised; synchronises `stream`
  * before returning.  Bitwise reproducible for the same input, rank count and device. */
 int b2k_pca_fit(b2k_ctx* ctx, const float* X, int64_t n_local, int d, int k, double* mean_out, double* components_out,
                 double* explained_variance_ratio_out, double* singular_values_out, uintptr_t stream);
@@ -255,9 +260,9 @@ int b2k_knn_search(b2k_ctx* ctx, const float* items, int64_t n_items_local, cons
  * moments_out [d + 1][d + 1] = sum (v - mean)(v - mean)^T over the rows v = [x | y], fp64.  Column sums of X and of y,
  * then the Gram pass of PCA on X (wgmma or generic, chosen as for b2k_pca_fit, option "kernel_path" likewise) and k_xty
  * for X^T y and y^T y, all centred on the fp32 means; the host removes that offset exactly.  Errors, decided on
- * allreduced values so that every rank fails together: an empty partition on any rank; a NaN or an infinity in X or y
- * (B2K_ERR_INVALID).  Synchronises `stream`.  Bitwise reproducible for the same input, rank count and device.
- * Stats: last_path = the Gram pass that ran; with option "time_kernels" != 0, last_reduce_ms = the column-sum pass,
+ * allreduced values so that every rank fails together: an empty partition on any rank (X and y may then be NULL); a NaN
+ * or an infinity in X or y (B2K_ERR_INVALID).  Synchronises `stream`.  Bitwise reproducible for the same input, rank
+ * count and device.  Stats: last_path = the Gram pass that ran; with option "time_kernels" != 0, last_reduce_ms = the column-sum pass,
  * last_fused_ms = the Gram pass, last_finalize_ms = the k_xty pass, last_allreduce_ms = both allreduces (device times)
  * and last_loop_ms = the whole call (host clock). */
 int b2k_linreg_moments(b2k_ctx* ctx, const float* X, const float* y, int64_t n_local, int d, int64_t* n_total_out,

@@ -152,9 +152,11 @@ int b2k_scratch_reserve(b2k_ctx* ctx, size_t bytes) {
 }
 
 namespace {
+// An empty partition may come with no buffer (torch reports data_ptr() == 0 for an empty tensor): the collective
+// callers then reach check_no_empty_partition, which fails on every rank together.
 int check_shape(b2k_ctx* ctx, const char* who, const void* X, int64_t n, int d, int k) {
   if (!ctx) return b2k_fail(nullptr, B2K_ERR_INVALID, std::string(who) + ": ctx is NULL");
-  if (!X || n < 0 || d <= 0 || k <= 0)
+  if ((!X && n > 0) || n < 0 || d <= 0 || k <= 0)
     return b2k_fail(ctx, B2K_ERR_INVALID, std::string(who) + ": bad X/n/d/k");
   return B2K_OK;
 }
@@ -471,13 +473,18 @@ static int lloyd_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, int k, flo
   return B2K_OK;
 }
 
+namespace {
+int check_no_empty_partition(b2k_ctx* ctx, const char* who, int64_t n_local, cudaStream_t s);
+}
+
 extern "C" int b2k_kmeans_lloyd(b2k_ctx* ctx, const float* X, int64_t n_local, int d, int k, float* centers,
                                 int max_iter, double tol, int* n_iter_out, double* shift_out, uintptr_t stream) {
   B2K_TRY(check_shape(ctx, "b2k_kmeans_lloyd", X, n_local, d, k));
   if (!centers) return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_kmeans_lloyd: centers is NULL");
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   B2K_CUDA_OK(ctx, cudaSetDevice(ctx->device));
-  return lloyd_impl(ctx, X, n_local, d, k, centers, max_iter, tol, n_iter_out, shift_out,
-                    reinterpret_cast<cudaStream_t>(stream));
+  B2K_TRY(check_no_empty_partition(ctx, "b2k_kmeans_lloyd", n_local, s));
+  return lloyd_impl(ctx, X, n_local, d, k, centers, max_iter, tol, n_iter_out, shift_out, s);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -932,7 +939,8 @@ extern "C" int b2k_pca_fit(b2k_ctx* ctx, const float* X, int64_t n_local, int d,
                            double* components_out, double* explained_variance_ratio_out, double* singular_values_out,
                            uintptr_t stream) {
   if (!ctx) return b2k_fail(nullptr, B2K_ERR_INVALID, "b2k_pca_fit: ctx is NULL");
-  if (!X || n_local < 0 || d <= 0) return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_pca_fit: bad X/n/d");
+  // an empty partition may come with no buffer: the collective check below reports it on every rank
+  if ((!X && n_local > 0) || n_local < 0 || d <= 0) return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_pca_fit: bad X/n/d");
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   B2K_CUDA_OK(ctx, cudaSetDevice(ctx->device));
   B2K_TRY(check_no_empty_partition(ctx, "b2k_pca_fit", n_local, s));
@@ -978,7 +986,9 @@ extern "C" int b2k_knn_search(b2k_ctx* ctx, const float* items, int64_t n_items_
 extern "C" int b2k_linreg_moments(b2k_ctx* ctx, const float* X, const float* y, int64_t n_local, int d,
                                   int64_t* n_total_out, double* mean_out, double* moments_out, uintptr_t stream) {
   if (!ctx) return b2k_fail(nullptr, B2K_ERR_INVALID, "b2k_linreg_moments: ctx is NULL");
-  if (!X || !y || n_local < 0 || d <= 0) return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_linreg_moments: bad X/y/n/d");
+  // an empty partition may come with no buffers: the collective check below reports it on every rank
+  if (((!X || !y) && n_local > 0) || n_local < 0 || d <= 0)
+    return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_linreg_moments: bad X/y/n/d");
   if (!n_total_out || !mean_out || !moments_out)
     return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_linreg_moments: NULL output");
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);

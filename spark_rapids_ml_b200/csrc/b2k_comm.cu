@@ -1,8 +1,9 @@
 // NCCL communicator lifecycle + the per-iteration allreduce of the fused [k*d sums | k counts | cost]
 // buffer (reference: common/cuml_context.py:75-81,123-131,158-175 and the two raft::comms allreduce calls
-// inside cuML's KMeansMG — SURVEY.md §8a a-8, a-11).  libnccl is resolved at run time (dlopen of the
-// copy torch already mapped, or the system one), so the library itself has no link-time NCCL dependency
-// and single-GPU users never touch it.
+// inside cuML's KMeansMG — SURVEY.md §8a a-8, a-11).  libnccl is resolved at run time, once per process: the
+// library named by B2K_NCCL_LIB when that is set (a failure to load it is an error, never a fall-back), else the
+// copy torch already mapped or the system one.  So the library has no link-time NCCL dependency and single-GPU
+// users never touch it.
 #include <dlfcn.h>
 #include <string.h>
 
@@ -34,18 +35,28 @@ NcclApi* nccl_api() {
   static bool tried = false;
   if (tried) return &api;
   tried = true;
-  const char* names[] = {"libnccl.so.2", "libnccl.so"};
-  for (const char* nm : names) {
-    api.h = dlopen(nm, RTLD_NOW | RTLD_GLOBAL);
-    if (api.h) break;
-  }
-  if (!api.h) {
-    const char* env = getenv("B2K_NCCL_LIB");
-    if (env) api.h = dlopen(env, RTLD_NOW | RTLD_GLOBAL);
-  }
-  if (!api.h) {
-    api.load_err = std::string("cannot dlopen libnccl.so.2 (set B2K_NCCL_LIB): ") + (dlerror() ? dlerror() : "");
-    return &api;
+  // The override is loaded first: once torch is imported, libnccl.so.2 is already mapped, so a dlopen of that name
+  // always succeeds and an override consulted only after it would never take effect.  RTLD_LOCAL keeps the override's
+  // nccl* symbols out of the global namespace, where torch's NCCL resolves its own.
+  const char* env = getenv("B2K_NCCL_LIB");
+  if (env && *env) {
+    api.h = dlopen(env, RTLD_NOW | RTLD_LOCAL);
+    if (!api.h) {
+      const char* e = dlerror();
+      api.load_err = std::string("cannot dlopen B2K_NCCL_LIB=") + env + ": " + (e ? e : "");
+      return &api;
+    }
+  } else {
+    const char* names[] = {"libnccl.so.2", "libnccl.so"};
+    for (const char* nm : names) {
+      api.h = dlopen(nm, RTLD_NOW | RTLD_GLOBAL);
+      if (api.h) break;
+    }
+    if (!api.h) {
+      const char* e = dlerror();
+      api.load_err = std::string("cannot dlopen libnccl.so.2 (set B2K_NCCL_LIB): ") + (e ? e : "");
+      return &api;
+    }
   }
 #define B2K_SYM(field, name)                                               \
   *(void**)(&api.field) = dlsym(api.h, name);                              \

@@ -545,9 +545,11 @@ int b2k_knn_search_impl(b2k_ctx* ctx, const float* items, int64_t n_items, const
   B2K_CUDA_OK(ctx, cudaStreamSynchronize(s));
   int64_t n_total = 0, row0 = 0, nq_max = 0, nq_total = 0;
   for (int r = 0; r < nr; ++r) {
-    if (sz[3 * r + 2] != d)
+    // judged against rank 0's d, on gathered values only: every rank reports the same rank and the same message
+    if (sz[3 * r + 2] != sz[2])
       return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_knn_search: d differs between ranks (rank " + std::to_string(r) +
-                                                " has d = " + std::to_string(sz[3 * r + 2]) + ")");
+                                                " has d = " + std::to_string(sz[3 * r + 2]) + ", rank 0 has d = " +
+                                                std::to_string(sz[2]) + ")");
     if (r < ctx->rank) row0 += sz[3 * r];
     n_total += sz[3 * r];
     nq_max = std::max(nq_max, sz[3 * r + 1]);
