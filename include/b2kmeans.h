@@ -32,6 +32,8 @@
  *   b2k_logreg_minimize         cuML's qn solver (L-BFGS / OWL-QN) itself
  *   b2k_logreg_fit              classification.py:984-1171 (LogisticRegressionMG.fit per param map, rescaling, centring)
  *   b2k_logreg_predict          classification.py:1455-1553 (LogisticRegressionModel's transform)
+ *   b2k_dbscan_fit              clustering.py:1049-1186 (DBSCANModel's fit function: cuML DBSCANMG(handle).fit_predict
+ *                               over NCCL + UCX, labels gathered on rank 0)
  *
  * Conventions
  *   - Plain C, no exceptions across the boundary: every call returns a b2k_status; the message for the
@@ -366,6 +368,39 @@ int b2k_logreg_fit(b2k_ctx* ctx, const float* X, const float* y, int64_t n_local
 int b2k_logreg_predict(b2k_ctx* ctx, const float* X, int64_t n, int d, int kp, const double* W, const double* b,
                        const double* class_values, double* raw_out, double* prob_out, double* pred_out,
                        uintptr_t stream);
+
+/* ---- DBSCAN (euclidean or cosine) ----
+ * Stands in for clustering.py:1049-1186 (DBSCANModel's fit function: cuML DBSCANMG.fit_predict).  Semantics, with the
+ * rows in global order (rank 0's rows in order, then rank 1's, ...):
+ *   adjacency  rows i and j are adjacent when dist(i, j) <= eps, evaluated in fp64 from the float32 values:
+ *              metric 0 (euclidean): sum_f ((double)x_if - (double)x_jf)^2 <= eps^2 (eps^2 formed in fp64);
+ *              metric 1 (cosine):    1 - x_i.x_j / (|x_i| |x_j|) <= eps, |x| = sqrt(sum_f x_f^2), all in fp64;
+ *              every sum in feature order, every operation rounded once (no fused multiply-add).  A row is adjacent to
+ *              itself.
+ *   core       a row with >= min_samples adjacent rows, itself included.
+ *   clusters   the connected components of the graph of core rows, numbered 0..C-1 by their lowest global row.
+ *   border     a non-core row with an adjacent core row takes the cluster of the adjacent core row of lowest global row
+ *              (order-free; scikit-learn's expansion order can give a row that touches two clusters the other one).
+ *   noise      every other row: -1.
+ * Outputs (device, this rank's rows): labels_out int32 [n_local], core_out uint8 [n_local] (may be NULL); host:
+ * *n_clusters_out = C.  Every rank ends up holding all rows (allgather of X padded to the largest shard: n_total d 4
+ * bytes, plus 2 n_total DP 4 bytes of tf32 planes on the wgmma pass, DP = 32, 64 or 128), one parent array per rank of
+ * the others (nranks n_total 4 bytes) and n_total bytes of core flags.
+ * Passes: a count pass, then a union pass over core columns (lock-free union-find, lowest root wins).  They run on
+ * wgmma (3xTF32 screen with a proven error bound, pairs inside the bound decided by the fp64 rule) when d % 4 == 0,
+ * 4 <= d <= 128 and X is 16-byte aligned, else on the generic SIMT pass (the fp64 rule on every pair).  Options
+ * "kernel_path" and "grid_limit" as for b2k_knn_search.
+ * Errors, decided on allgathered values so that every rank fails together (B2K_ERR_INVALID unless noted): eps not
+ * finite or <= 0; min_samples < 1; metric not 0 or 1; no row on any rank; d differing between ranks; "DBSCAN input
+ * contains NaN or infinity"; cosine with a zero row; 2^31 - 256 rows or more (B2K_ERR_UNSUPPORTED).  A rank with no rows
+ * is legal (X and labels_out may then be NULL).  Collective; synchronises `stream`.  The labels and core flags depend
+ * only on the rows in global order: not on the rank count, the shard boundaries, the pass or the order of atomics.
+ * Stats: last_path = the pass that ran; with option "time_kernels" != 0, last_finalize_ms = row allgather and prep,
+ * last_fused_ms = the count pass, last_reduce_ms = core allgather and the union pass, last_allreduce_ms = merge and
+ * labels, last_loop_ms = all of them (device times, CUDA events); with option "collect_recheck" = 1,
+ * recheck_candidates = pairs of the wgmma pass decided by the fp64 rule and recheck_rows = unions attempted. */
+int b2k_dbscan_fit(b2k_ctx* ctx, const float* X, int64_t n_local, int d, double eps, int min_samples, int metric,
+                   int32_t* labels_out, uint8_t* core_out, int64_t* n_clusters_out, uintptr_t stream);
 
 #ifdef __cplusplus
 }

@@ -63,9 +63,11 @@ EXPORTED_SYMBOLS = (
     "b2k_logreg_minimize",
     "b2k_logreg_fit",
     "b2k_logreg_predict",
+    "b2k_dbscan_fit",
 )
 
 FAMILY_CODES = {"auto": 0, "binomial": 1, "multinomial": 2}
+METRIC_CODES = {"euclidean": 0, "cosine": 1}
 # int (*)(void* user, int n, const double* x, double* f, double* grad)
 LOGREG_OBJECTIVE = ctypes.CFUNCTYPE(ctypes.c_int, ctypes.c_void_p, ctypes.c_int, ctypes.POINTER(ctypes.c_double),
                                     ctypes.POINTER(ctypes.c_double), ctypes.POINTER(ctypes.c_double))
@@ -170,6 +172,7 @@ def load_library() -> ctypes.CDLL:
     L.b2k_logreg_fit.argtypes = [vp, vp, vp, i64, i32, vp, vp, i32, i32, ctypes.POINTER(LogregParams), vp, vp, vp, vp,
                                  ctypes.c_size_t]
     L.b2k_logreg_predict.argtypes = [vp, vp, i64, i32, i32, vp, vp, vp, vp, vp, vp, ctypes.c_size_t]
+    L.b2k_dbscan_fit.argtypes = [vp, vp, i64, i32, f64, i32, i32, vp, vp, ctypes.POINTER(i64), ctypes.c_size_t]
     for name in EXPORTED_SYMBOLS:
         if name not in ("b2k_last_error",):
             getattr(L, name).restype = i32
@@ -633,3 +636,21 @@ class Context:
                                                    self._stream()))
         t.cuda.current_stream(self.device).synchronize()  # Wd, bd, cv (temporaries) must outlive the kernel
         return raw, prob, pred
+
+    # -- DBSCAN -----------------------------------------------------------------------------
+    def dbscan_fit(self, X: Any, eps: float, min_samples: int, metric: str = "euclidean") -> Tuple[Any, Any, int]:
+        """DBSCAN over all ranks' rows (collective when a communicator is initialised): X [n, d] float32 CUDA tensor (may
+        have 0 rows) -> (labels int32 [n], core flags bool [n], both CUDA tensors for this rank's rows, and the number of
+        clusters).  metric is "euclidean" or "cosine"."""
+        t = self._torch
+        n, d = self._check_X(X)
+        if metric not in METRIC_CODES:
+            raise ValueError(f"metric must be one of {sorted(METRIC_CODES)}, got {metric!r}")
+        labels = t.empty((n,), dtype=t.int32, device=self.device)
+        core = t.empty((n,), dtype=t.uint8, device=self.device)
+        ncl = ctypes.c_int64(0)
+        with t.cuda.device(self.device):
+            self._check(self._L.b2k_dbscan_fit(self._h, X.data_ptr(), n, d, float(eps), int(min_samples),
+                                               METRIC_CODES[metric], labels.data_ptr(), core.data_ptr(),
+                                               ctypes.byref(ncl), self._stream()))
+        return labels, core.bool(), int(ncl.value)

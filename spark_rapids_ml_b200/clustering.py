@@ -8,9 +8,12 @@ Same names, argument meaning and error behaviour as the reference:
   KMeans (keyword-only ctor, setters, _get_cuml_fit_func, _out_schema,
           _create_pyspark_model, _merge_model_chunks)                                clustering.py:189-502
   KMeansModel (clusterCenters, hasSummary, predict, _get_cuml_transform_func)        clustering.py:505-604
+  DBSCANClass, _DBSCANCumlParams, DBSCAN (lazy fit), DBSCANModel.transform             clustering.py:607-1186
 
 Differences that are deliberate: no CPU fallback (cpu() / single-vector predict need a JVM and raise), and the
-fit function receives a DEVICE matrix from the worker scaffold instead of host arrays to concatenate.
+fit function receives a DEVICE matrix from the worker scaffold instead of host arrays to concatenate.  DBSCAN: every
+rank returns the labels of its own rows (the reference's come from rank 0 only), and transform of a pyspark DataFrame
+raises NotImplementedError.
 """
 from __future__ import annotations
 
@@ -18,11 +21,12 @@ from typing import Any, Callable, Dict, List, Optional, Sequence, Tuple, Union
 
 import numpy as np
 import pandas as pd
+import pyarrow as pa
 
-from .core import (FitInputType, _append_transform_features, _CumlEstimator, _CumlModelWithPredictionCol,
-                   _transform_context, param_alias)
-from .params import HasFeaturesCols, P, _CumlClass, _CumlParams, _KMeansParams
-from .sparkshim import Row, keyword_only
+from .core import (FitInputType, _append_transform_features, _CumlCaller, _CumlEstimator, _CumlModelWithPredictionCol,
+                   _transform_context, alias, param_alias)
+from .params import HasFeaturesCol, HasFeaturesCols, HasIDCol, HasPredictionCol, P, _CumlClass, _CumlParams, _KMeansParams
+from .sparkshim import HAVE_PYSPARK, Param, Row, TypeConverters, keyword_only
 from .utils import get_logger
 
 
@@ -307,3 +311,228 @@ class KMeansModel(KMeansClass, _CumlModelWithPredictionCol, _KMeansCumlParams):
         _transform_internal.many = _transform_many  # type: ignore[attr-defined]
         _transform_internal.row_bytes = 4 * int(n_cols or 1)  # type: ignore[attr-defined]
         return _construct_kmeans, _transform_internal, None
+
+
+# ---- DBSCAN (reference: clustering.py:607-1186) ----
+class DBSCANClass(_CumlClass):
+    @classmethod
+    def _param_mapping(cls) -> Dict[str, Optional[str]]:
+        return {}
+
+    def _get_cuml_params_default(self) -> Dict[str, Any]:
+        return {"eps": 0.5, "min_samples": 5, "metric": "euclidean", "algorithm": "brute", "verbose": False,
+                "max_mbytes_per_batch": None}
+
+    def _pyspark_class(self) -> Optional[type]:
+        return None   # pyspark.ml has no DBSCAN
+
+
+class _DBSCANCumlParams(_CumlParams, HasFeaturesCol, HasFeaturesCols, HasIDCol, HasPredictionCol):
+    """Shared Spark Params of DBSCAN and DBSCANModel (reference: clustering.py:626-730)."""
+
+    def __init__(self) -> None:
+        super().__init__()
+        self._setDefault(eps=0.5, min_samples=5, metric="euclidean", algorithm="brute", max_mbytes_per_batch=None,
+                         idCol=alias.row_number)
+
+    eps = Param("parent", "eps", "The maximum distance between 2 points such they reside in the same neighborhood.",
+                TypeConverters.toFloat)
+    min_samples = Param("parent", "min_samples", "The number of samples in a neighborhood such that this group can be "
+                        "considered as an important core point (including the point itself).", TypeConverters.toInt)
+    metric = Param("parent", "metric", "The metric to use when calculating distances between points.Spark Rapids ML "
+                   "does not support the 'precomputed' mode from sklearn and cuML, please use those libraries instead.",
+                   TypeConverters.toString)
+    algorithm = Param("parent", "algorithm", "The algorithm to be used by for nearest neighbor computations.",
+                      TypeConverters.toString)
+    max_mbytes_per_batch = Param("parent", "max_mbytes_per_batch", "Calculate batch size using no more than this "
+                                 "number of megabytes for the pairwise distance computation.", TypeConverters.toInt)
+
+    def getFeaturesCol(self) -> Union[str, List[str]]:  # type: ignore[override]
+        if self.isDefined(self.featuresCols):
+            return self.getFeaturesCols()
+        if self.isDefined(self.featuresCol):
+            return self.getOrDefault("featuresCol")
+        raise RuntimeError("featuresCol is not set")
+
+    def setFeaturesCol(self: P, value: Union[str, List[str]]) -> P:
+        if isinstance(value, str):
+            self._set_params(featuresCol=value)
+        else:
+            self._set_params(featuresCols=value)
+        return self
+
+    def setFeaturesCols(self: P, value: List[str]) -> P:
+        return self._set_params(featuresCols=value)
+
+    def setPredictionCol(self: P, value: str) -> P:
+        self._set_params(predictionCol=value)
+        return self
+
+    def setIdCol(self: P, value: str) -> P:
+        self._set_params(idCol=value)
+        return self
+
+
+def _no_pyspark(dataset: Any) -> None:
+    if HAVE_PYSPARK:
+        from . import spark_binding
+
+        if spark_binding.is_spark_dataframe(dataset):
+            raise NotImplementedError("DBSCANModel.transform of a pyspark DataFrame is not supported yet; use a local "
+                                      "frame")
+
+
+class DBSCAN(DBSCANClass, _CumlEstimator, _DBSCANCumlParams):
+    """DBSCAN on H100 (reference: clustering.py:733-934).  fit() is lazy and returns a DBSCANModel; the clustering runs
+    in DBSCANModel.transform, one barrier task per GPU over the whole frame.  Parameters: eps (0.5), min_samples (5),
+    metric ("euclidean" | "cosine"), algorithm ("brute" | "rbc": both run the same exact pass), max_mbytes_per_batch
+    (accepted, unused: no pass here is batched by memory), featuresCol, predictionCol, idCol, num_workers, verbose.
+
+    Labels follow include/b2kmeans.h: clusters are numbered by their lowest row; a border row that touches two clusters
+    takes the cluster of its lowest adjacent core row, where scikit-learn and cuML take whichever expands first.
+
+    >>> from spark_rapids_ml_b200.clustering import DBSCAN
+    >>> df = session.createDataFrame([([1.0, 1.0],), ([1.0, 2.0],), ([5.0, 5.0],), ([5.0, 6.0],)], ["features"])
+    >>> DBSCAN(eps=2.0, min_samples=2).fit(df).transform(df).collect()   # prediction 0, 0, 1, 1
+    """
+
+    @keyword_only
+    def __init__(self, *, featuresCol: Union[str, List[str]] = "features", predictionCol: str = "prediction",
+                 eps: float = 0.5, min_samples: int = 5, metric: str = "euclidean", algorithm: str = "brute",
+                 max_mbytes_per_batch: Optional[int] = None, num_workers: Optional[int] = None,
+                 verbose: Union[int, bool] = False, idCol: str = alias.row_number, **kwargs: Any) -> None:
+        super().__init__()
+        self._handle_param_spark_confs()
+        self._input_kwargs.pop("kwargs", None)
+        self._input_kwargs.update(kwargs)
+        if self._input_kwargs.get("num_workers", None) is None:
+            self._input_kwargs.pop("num_workers", None)
+        self._set_params(**self._input_kwargs)
+        self.cuml_params["calc_core_sample_indices"] = False   # core-sample indices are not supported
+
+    def setEps(self: P, value: float) -> P:
+        return self._set_params(eps=value)
+
+    def getEps(self) -> float:
+        return self.getOrDefault("eps")
+
+    def setMinSamples(self: P, value: int) -> P:
+        return self._set_params(min_samples=value)
+
+    def getMinSamples(self) -> int:
+        return self.getOrDefault("min_samples")
+
+    def setMetric(self: P, value: str) -> P:
+        return self._set_params(metric=value)
+
+    def getMetric(self) -> str:
+        return self.getOrDefault("metric")
+
+    def setAlgorithm(self: P, value: str) -> P:
+        return self._set_params(algorithm=value)
+
+    def getAlgorithm(self) -> str:
+        return self.getOrDefault("algorithm")
+
+    def setMaxMbytesPerBatch(self: P, value: Optional[int]) -> P:
+        return self._set_params(max_mbytes_per_batch=value)
+
+    def getMaxMbytesPerBatch(self) -> Optional[int]:
+        return self.getOrDefault("max_mbytes_per_batch")
+
+    def _fit(self, dataset: Any) -> "DBSCANModel":
+        if self.getMetric() == "precomputed":
+            raise ValueError("Spark Rapids ML does not support the 'precomputed' mode from sklearn and cuML, please "
+                             "use those libraries instead")
+        _validate_dbscan_params(self)
+        model = DBSCANModel(n_cols=0, dtype="")
+        model._num_workers = self._num_workers
+        model._float32_inputs = self._float32_inputs
+        self._copyValues(model)
+        self._copy_cuml_params(model)
+        return model
+
+    def _create_pyspark_model(self, result: Row) -> Any:
+        raise NotImplementedError("DBSCAN does not support model creation from Row")
+
+    def _get_cuml_fit_func(self, dataset: Any, extra_params: Optional[List[Dict[str, Any]]] = None) -> Any:
+        raise NotImplementedError("DBSCAN does not fit and generate model")
+
+    def _out_schema(self) -> Any:
+        raise NotImplementedError("DBSCAN does not output for fit and generate model")
+
+
+def _validate_dbscan_params(p: Any) -> None:
+    metric, algorithm = p.getOrDefault("metric"), p.getOrDefault("algorithm")
+    if metric not in ("euclidean", "cosine"):
+        raise ValueError(f"metric {metric!r} is not supported: use 'euclidean' or 'cosine'")
+    if algorithm not in ("brute", "rbc"):
+        raise ValueError(f"algorithm {algorithm!r} is not supported: use 'brute' or 'rbc'")
+
+
+class DBSCANModel(DBSCANClass, _CumlModelWithPredictionCol, _CumlCaller, _DBSCANCumlParams):
+    """reference: clustering.py:937-1186.  transform(frame) clusters the frame's rows (one barrier task per GPU, each
+    rank's labels for its own rows) and appends the int32 predictionCol in the frame's row order, matching rows by idCol
+    or, when the frame has no such column, by a monotonically increasing `unique_id`."""
+
+    def __init__(self, n_cols: int, dtype: str) -> None:
+        super().__init__(n_cols=n_cols, dtype=dtype)
+        self._setDefault(idCol=alias.row_number)
+
+    def _out_schema(self, input_schema: Any = None) -> Any:
+        return f"{self._get_prediction_name()} int, {alias.row_number} long"
+
+    def _get_prediction_name(self) -> str:
+        return self.getOrDefault("predictionCol")
+
+    def _require_nccl_ucx(self) -> Tuple[bool, bool]:
+        return (True, False)
+
+    def _get_cuml_transform_func(self, dataset: Any, eval_metric_info: Any = None) -> Any:
+        raise NotImplementedError("DBSCAN does not have a separate transform UDF")
+
+    def _pre_process_data(self, dataset: Any) -> Tuple[Any, Optional[List[str]], int, str]:
+        """The feature columns as for every estimator, plus the row id as alias.row_number (int64)."""
+        df, multi_col_names, dimension, ftype = _CumlCaller._pre_process_data(self, dataset)
+        id_col = self.getIdCol()
+        df = df.with_appended_column(alias.row_number,
+                                     [[b.column(id_col).cast(pa.int64()) for b in p] for p in dataset._parts])
+        return df, multi_col_names, dimension, ftype
+
+    def _get_cuml_fit_func(self, dataset: Any, extra_params: Optional[List[Dict[str, Any]]] = None
+                           ) -> Callable[[FitInputType, Dict[str, Any]], Dict[str, Any]]:
+        pred_name = self._get_prediction_name()
+
+        def _cuml_fit(dfs: FitInputType, params: Dict[str, Any]) -> Dict[str, Any]:
+            # stands in for DBSCANMG(handle).fit_predict (clustering.py:1049-1098); every rank returns its own rows
+            ctx = params[param_alias.handle]
+            X, _, row_number = dfs[0]
+            init = params[param_alias.cuml_init]
+            labels, _, _ = ctx.dbscan_fit(X, float(init["eps"]), int(init["min_samples"]), init["metric"])
+            return {pred_name: labels.cpu().numpy(), alias.row_number: row_number}
+
+        return _cuml_fit
+
+    def _transform(self, dataset: Any) -> Any:
+        _no_pyspark(dataset)
+        _validate_dbscan_params(self)
+        id_col = self.getIdCol()
+        with_id = dataset if id_col in dataset.columns else dataset.with_monotonically_increasing_id(id_col)
+        input_col, input_cols = self._get_input_columns()
+        cols = [id_col] + ([input_col] if input_col is not None else list(input_cols))
+        res = self._call_cuml_fit_func(with_id.select(cols).repartition(self.num_workers), partially_collect=False)
+        table = res._table()
+        got_ids = np.asarray(table.column(alias.row_number).to_numpy(), dtype=np.int64)
+        got = np.asarray(table.column(self._get_prediction_name()).to_numpy(), dtype=np.int32)
+        order = np.argsort(got_ids, kind="stable")
+        got_ids, got = got_ids[order], got[order]
+        if np.any(got_ids[1:] == got_ids[:-1]):
+            raise ValueError(f"idCol '{id_col}' must identify each row: it has repeated values")
+        out_parts = []
+        for p in with_id._parts:
+            arrs = []
+            for b in p:
+                ids = np.asarray(b.column(id_col).cast(pa.int64()).to_numpy(), dtype=np.int64)
+                arrs.append(pa.array(got[np.searchsorted(got_ids, ids)], type=pa.int32()))
+            out_parts.append(arrs)
+        return dataset.with_appended_column(self._get_prediction_name(), out_parts)

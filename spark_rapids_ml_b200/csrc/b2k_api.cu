@@ -981,6 +981,21 @@ extern "C" int b2k_knn_search(b2k_ctx* ctx, const float* items, int64_t n_items_
 }
 
 // ------------------------------------------------------------------------------------------------
+// DBSCAN (b2k_dbscan.cu)
+// ------------------------------------------------------------------------------------------------
+extern "C" int b2k_dbscan_fit(b2k_ctx* ctx, const float* X, int64_t n_local, int d, double eps, int min_samples,
+                              int metric, int32_t* labels_out, uint8_t* core_out, int64_t* n_clusters_out,
+                              uintptr_t stream) {
+  if (!ctx) return b2k_fail(nullptr, B2K_ERR_INVALID, "b2k_dbscan_fit: ctx is NULL");
+  // an empty partition may come with no buffers; every value check runs after the size allgather, on every rank alike
+  if (n_local < 0 || d <= 0 || (n_local > 0 && (!X || !labels_out)) || !n_clusters_out)
+    return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_dbscan_fit: bad X/labels_out/n_clusters_out/n/d");
+  B2K_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  return b2k_dbscan_fit_impl(ctx, X, n_local, d, eps, min_samples, metric, labels_out, core_out, n_clusters_out,
+                             reinterpret_cast<cudaStream_t>(stream));
+}
+
+// ------------------------------------------------------------------------------------------------
 // linear regression (b2k_linreg.cu)
 // ------------------------------------------------------------------------------------------------
 extern "C" int b2k_linreg_moments(b2k_ctx* ctx, const float* X, const float* y, int64_t n_local, int d,

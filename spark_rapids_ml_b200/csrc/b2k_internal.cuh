@@ -284,6 +284,12 @@ int b2k_knn_search_impl(b2k_ctx* ctx, const float* items, int64_t n_items, const
                         cudaStream_t s);
 
 // ------------------------------------------------------------------------------------------------
+// DBSCAN — b2k_dbscan.cu (the C ABI entry point in b2k_api.cu checks its arguments, then calls this)
+// ------------------------------------------------------------------------------------------------
+int b2k_dbscan_fit_impl(b2k_ctx* ctx, const float* X, int64_t n_local, int d, double eps, int min_samples, int metric,
+                        int32_t* labels_out, uint8_t* core_out, int64_t* n_clusters_out, cudaStream_t s);
+
+// ------------------------------------------------------------------------------------------------
 // linear regression — b2k_linreg.cu (the C ABI entry points in b2k_api.cu check their arguments, then call these)
 // ------------------------------------------------------------------------------------------------
 constexpr int B2K_LINREG_MAX_D = B2K_PCA_MAX_D;   // the moments ride on PCA's Gram passes
