@@ -34,6 +34,9 @@
  *   b2k_logreg_predict          classification.py:1455-1553 (LogisticRegressionModel's transform)
  *   b2k_dbscan_fit              clustering.py:1049-1186 (DBSCANModel's fit function: cuML DBSCANMG(handle).fit_predict
  *                               over NCCL + UCX, labels gathered on rank 0)
+ *   b2k_rf_fit / b2k_rf_forest  tree.py:343-527 (the per-worker cuML RandomForest fits and the treelite models they
+ *                               return), classification.py:285-676, regression.py:865-1147
+ *   b2k_rf_predict              tree.py:670- (the model's transform: cuML's forest inference over treelite)
  *
  * Conventions
  *   - Plain C, no exceptions across the boundary: every call returns a b2k_status; the message for the
@@ -148,6 +151,8 @@ int b2k_ctx_destroy(b2k_ctx* ctx);
  *   "adaptive_path"    see b2k_stats.path_switch_iter
  *   "ingest_threads"   host threads of the pageable -> pinned staging copy of b2k_ingest_append; 0 = default: 4, capped
  *                      by half of the CPUs the process may use
+ *   "rf_group_nodes"   b2k_rf_fit: cap on the nodes of one histogram pass, 0 = as many as fit (tests)
+ *   "rf_flush_tiles"   b2k_rf_fit: cap on the tiles a CTA of the cluster pass adds between flushes, 0 = the bound (tests)
  *   "profile_fused"    0/1; the k, d <= 128 fused kernel runs a separately compiled instantiation that records per-warp
  *                      phase cycle counters, read back with b2k_get_fused_profile; the large-shape kernel rejects it
  *                      with B2K_ERR_UNSUPPORTED
@@ -401,6 +406,118 @@ int b2k_logreg_predict(b2k_ctx* ctx, const float* X, int64_t n, int d, int kp, c
  * recheck_candidates = pairs of the wgmma pass decided by the fp64 rule and recheck_rows = unions attempted. */
 int b2k_dbscan_fit(b2k_ctx* ctx, const float* X, int64_t n_local, int d, double eps, int min_samples, int metric,
                    int32_t* labels_out, uint8_t* core_out, int64_t* n_clusters_out, uintptr_t stream);
+
+/* ---- random forests (classification: gini / entropy; regression: variance) ----
+ * Stands in for tree.py / classification.py:285-676 / regression.py:865-1147 (cuML's RandomForest*MG fits on each
+ * worker's partition).  Unlike the reference, every tree is grown from the histograms of ALL ranks' rows, level by
+ * level, with one int64 allreduce per histogram pass (MLlib's design), so the forest depends only on the rows in global
+ * order (rank 0's rows, then rank 1's, ...) and the params: not on the rank count, the shard boundaries, the pass or the
+ * order of atomics.  Semantics (tests/rf_oracle.py restates them in NumPy):
+ *   hash       h(seed, stream, tree, index), SplitMix64's finaliser chained (below); streams B2K_RF_BOOT,
+ *              B2K_RF_SAMPLE, B2K_RF_FEAT.
+ *   bootstrap  bootstrap = 1: row r of tree t has weight w = Poisson(1) drawn by inverse CDF from u = h(seed, BOOT, t,
+ *              r) >> 32 against B2K_RF_POISSON_CDF (below), capped at 12; else w = 1.  Every statistic is an integer
+ *              sum of w.
+ *   thresholds row r is in the sample iff h(seed, SAMPLE, 0, r) < (uint64)ldexp(f, 64), f = M / n_total with M =
+ *              max(max_bins^2, 10000) (every row when M >= n_total).  Per feature, the sample values (-0.0 read as +0.0)
+ *              sorted: s_0 <= ... <= s_{m-1}, distinct values v_0 < ... < v_{u-1}.  mid(a, b) = fl32(((double)a +
+ *              (double)b) / 2), replaced by a when it equals b.  u <= max_bins: thresholds mid(v_i, v_{i+1}), i < u - 1;
+ *              else mid(s_{p-1}, s_p) at p = floor(j m / max_bins), j = 1..max_bins-1, duplicates dropped.  A feature has
+ *              nthr <= max_bins - 1 ascending thresholds t_0 < t_1 < ... and nthr + 1 bins; bin(x) = #{thresholds < x}
+ *              in float32, so x <= t_b <=> bin(x) <= b: training routes rows by bin, prediction by threshold, alike.
+ *   features   each node draws features_per_node features of d: a partial Fisher-Yates shuffle of 0..d-1 whose step j
+ *              swaps slot j with slot j + h(seed, FEAT, t, heap d + j) % (d - j), heap the node's heap index (root 1,
+ *              children 2 heap and 2 heap + 1); the first features_per_node slots, sorted ascending.
+ *   statistics classification: per class c_k = sum w (N = sum_k c_k).  Regression: labels on a fixed-point grid, y_q =
+ *              rint(y 2^(24-e)) with 2^(e-1) < max|y| <= 2^e over all ranks (q = 2^(e-24); q = 1 when max|y| = 0), so
+ *              that W = sum w and S = sum w y_q are exact integers: labels are resolved to max|y| 2^-24, a deliberate
+ *              semantic.
+ *   gain       fp64, each operation rounded once (no fused multiply-add), in this order:
+ *                gini     s = 0; s = s + p_k p_k over k ascending (p_k = c_k / N); imp = 1 - s
+ *                entropy  s = 0; s = s - p_k L(p_k) over k ascending with c_k > 0; imp = s, where L = b2k_rf_log2 below
+ *                         (written in + - * / only, so the host and NumPy agree bit for bit)
+ *                gain     a = N_L / N; b = N_R / N; g = (imp - a imp_L) - b imp_R
+ *                variance D = S_L W - S W_L (exact, 128-bit); g = (double)D; g = g g; g = g / (W_L W_R); g = g / W;
+ *                         g = g / W; g = g q^2   (= the variance reduction of y; the sum of y^2 cancels)
+ *              A candidate (feature, bin b: left = bin <= b) is valid when both sides weigh >= min_instances.  The best
+ *              has the highest gain; ties go to the lowest feature, then the lowest bin.  A node is a leaf when its
+ *              depth is max_depth, it is pure (one class; classification), it has no valid candidate, or the best gain
+ *              is <= 0 or below min_info_gain (MLlib's rule).
+ *   values     classification: c_k / N for k < n_values (n_values = max label + 1); regression: ((double)S q) / W.  A
+ *              node of weight 0 (a root whose bootstrap drew no row) has value 0.  Every node carries its value.
+ *   numbering  per tree, breadth first: the root is node 0; the nodes of one level, in order, append their children
+ *              (left, then right).
+ * b2k_rf_fit (collective): X device f32 [n_local, d], y device f32 [n_local] (class values 0, 1, ... or targets).
+ * Histograms hold (tree, node, feature slot, bin) x {c_0..c_{C-1} | W, S} of the nodes of one level.  Passes: a finite
+ * check and an allgather of the sizes; the label pass of b2k_logreg_labels (classification; its label rules apply); the
+ * sample select and an allgather of the sample; the host sort and thresholds; k_rf_bin (X -> uint8 bins, n_local d
+ * bytes); per level and node group, one histogram pass, one int64 allreduce, the host split choice, then k_rf_route.
+ * The histogram pass runs on an 8-CTA thread-block cluster that shards the group's histogram over its CTAs' shared
+ * memory (u32 counts, u64 label sums, remote shared atomics, flushed with int64 global atomics at least every
+ * 2^28 rows per cluster, option "rf_flush_tiles" lowers that for tests); node groups are sized to the cluster's shared
+ * memory.  Where one node's histogram exceeds it, the generic pass adds every update with int64 global atomics.  Option
+ * "kernel_path" = B2K_PATH_GENERIC forces the generic pass, B2K_PATH_FUSED fails with B2K_ERR_UNSUPPORTED where the
+ * cluster pass cannot run; option "grid_limit" caps the CTAs; option "rf_group_nodes" caps the nodes of one group.
+ * Outputs: *n_values_out = C (classification) or 1; *n_nodes_out = nodes of the forest, read with b2k_rf_forest;
+ * level_ms_out [max_depth + 1] (may be NULL; needs "time_kernels") = device time of each level's histogram passes;
+ * level_updates_out [max_depth + 1] (may be NULL) = (row, tree, feature slot) updates with w > 0 of each level, all
+ * ranks.  Errors, decided on gathered values so that every rank fails together (B2K_ERR_INVALID unless noted):
+ * "maxDepth given invalid value -1", "maxBins given invalid value -1" (max_bins outside [2, 256]), n_trees < 1,
+ * min_instances < 1, min_info_gain < 0 or not finite, features_per_node outside [1, d], impurity outside 0..2, max_depth
+ * > 16 (B2K_ERR_UNSUPPORTED), an empty partition on any rank, d differing between ranks, "RandomForest input contains NaN
+ * or infinity", and the label rules of b2k_logreg_labels (classification).  Synchronises `stream`.
+ * Stats: last_path = the histogram pass that ran; last_n_iter = levels; recheck_rows = histogram passes;
+ * recheck_candidates = bytes allreduced by them; with "time_kernels": last_finalize_ms = checks, labels, sample, sort
+ * and thresholds (host clock), last_reduce_ms = k_rf_bin, last_fused_ms = every histogram pass, last_allreduce_ms =
+ * their allreduces (device times), last_loop_ms = the whole call (host clock). */
+#define B2K_RF_MAX_DEPTH 16
+#define B2K_RF_MAX_BINS 256
+#define B2K_RF_BOOT 1
+#define B2K_RF_SAMPLE 2
+#define B2K_RF_FEAT 3
+#define B2K_RF_POISSON_CAP 12
+/* The hash, in uint64 wrap-around arithmetic, with G = B2K_RF_GOLDEN:
+ *   mix(z)                           z ^= z >> 30; z *= B2K_RF_MIX1; z ^= z >> 27; z *= B2K_RF_MIX2; z ^= z >> 31
+ *   h(seed, stream, tree, index)   = mix(mix(mix(seed + stream G) + tree G) + index G)
+ * The bootstrap weight of u (the top 32 bits of h) is the least k with u < B2K_RF_POISSON_CDF[k] (floor(2^32 CDF(k))
+ * of Poisson(1), k = 0..11), else B2K_RF_POISSON_CAP. */
+#define B2K_RF_GOLDEN 0x9E3779B97F4A7C15ull
+#define B2K_RF_MIX1 0xBF58476D1CE4E5B9ull
+#define B2K_RF_MIX2 0x94D049BB133111EBull
+#define B2K_RF_POISSON_CDF                                                                                         \
+  {1580030168u, 3160060337u, 3950075421u, 4213413783u, 4279248373u, 4292415291u, 4294609777u, 4294923276u,         \
+   4294962463u, 4294966817u, 4294967252u, 4294967292u}
+typedef struct b2k_rf_params {
+  int32_t n_trees;           /* >= 1 */
+  int32_t max_depth;         /* 0..16 */
+  int32_t max_bins;          /* 2..256 */
+  int32_t min_instances;     /* >= 1 (minInstancesPerNode, in bootstrap weight) */
+  int32_t features_per_node; /* 1..d (featureSubsetStrategy resolved by the caller) */
+  int32_t bootstrap;         /* 0 / 1 */
+  int32_t impurity;          /* 0 gini, 1 entropy (classification); 2 variance (regression) */
+  int32_t reserved;          /* 0 */
+  double min_info_gain;      /* >= 0 */
+  uint64_t seed;
+} b2k_rf_params;
+int b2k_rf_fit(b2k_ctx* ctx, const float* X, const float* y, int64_t n_local, int d, const b2k_rf_params* params,
+               int* n_values_out, int64_t* n_nodes_out, double* level_ms_out, int64_t* level_updates_out,
+               uintptr_t stream);
+/* The forest of the context's last successful b2k_rf_fit, host outputs (V = *n_values_out): tree_offsets_out [T + 1]
+ * (tree t is nodes [off_t, off_t+1)); per node: feature_out (-1 for a leaf), threshold_out (go left when x <= t),
+ * children_out [2] (tree-local indices, -1 for a leaf), gain_out (0 for a leaf), count_out (N or W), value_out [V]. */
+int b2k_rf_forest(b2k_ctx* ctx, int64_t* tree_offsets_out, int32_t* feature_out, float* threshold_out,
+                  int32_t* children_out, double* gain_out, int64_t* count_out, double* value_out);
+/* Prediction (k_rf_predict) over X [n, d] with a forest in device arrays laid out as b2k_rf_forest's output (any
+ * tree-local child indices; nodes staged in shared memory when the forest fits, else read through L1/L2).
+ * classification = 1: raw_out [n][V] = sum of the leaves' values in tree order (fp64), prob_out [n][V] = raw / sum_k raw
+ * (0 when that sum is 0), pred_out [n] = argmax_k raw (lowest k on a tie).  classification = 0: pred_out [n] = sum of
+ * the leaves' values in tree order / T; raw_out and prob_out unused (may be NULL).  Asynchronous on `stream`. */
+int b2k_rf_predict(b2k_ctx* ctx, const float* X, int64_t n, int d, int n_trees, const int64_t* tree_offsets,
+                   const int32_t* feature, const float* threshold, const int32_t* children, const double* value,
+                   int n_values, int classification, double* raw_out, double* prob_out, double* pred_out,
+                   uintptr_t stream);
+/* L(p) of the entropy above, p in (0, 1]: p = m 2^E (frexp; m < 0.7071067811865476: m = 2m, E = E - 1), z = (m - 1)
+ * / (m + 1), z2 = z z, a = 1.0 / 25; a = a z2 + 1.0 / (2i + 1) for i = 11..0; L = ((z a) 2) 1.4426950408889634 + E. */
 
 #ifdef __cplusplus
 }

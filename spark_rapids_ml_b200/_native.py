@@ -64,10 +64,14 @@ EXPORTED_SYMBOLS = (
     "b2k_logreg_fit",
     "b2k_logreg_predict",
     "b2k_dbscan_fit",
+    "b2k_rf_fit",
+    "b2k_rf_forest",
+    "b2k_rf_predict",
 )
 
 FAMILY_CODES = {"auto": 0, "binomial": 1, "multinomial": 2}
 METRIC_CODES = {"euclidean": 0, "cosine": 1}
+IMPURITY_CODES = {"gini": 0, "entropy": 1, "variance": 2}
 # int (*)(void* user, int n, const double* x, double* f, double* grad)
 LOGREG_OBJECTIVE = ctypes.CFUNCTYPE(ctypes.c_int, ctypes.c_void_p, ctypes.c_int, ctypes.POINTER(ctypes.c_double),
                                     ctypes.POINTER(ctypes.c_double), ctypes.POINTER(ctypes.c_double))
@@ -88,6 +92,21 @@ class LogregParams(ctypes.Structure):
         ("fit_intercept", ctypes.c_int32),
         ("standardization", ctypes.c_int32),
         ("family", ctypes.c_int32),
+    ]
+
+
+class RfParams(ctypes.Structure):
+    _fields_ = [
+        ("n_trees", ctypes.c_int32),
+        ("max_depth", ctypes.c_int32),
+        ("max_bins", ctypes.c_int32),
+        ("min_instances", ctypes.c_int32),
+        ("features_per_node", ctypes.c_int32),
+        ("bootstrap", ctypes.c_int32),
+        ("impurity", ctypes.c_int32),
+        ("reserved", ctypes.c_int32),
+        ("min_info_gain", ctypes.c_double),
+        ("seed", ctypes.c_uint64),
     ]
 
 
@@ -173,6 +192,10 @@ def load_library() -> ctypes.CDLL:
                                  ctypes.c_size_t]
     L.b2k_logreg_predict.argtypes = [vp, vp, i64, i32, i32, vp, vp, vp, vp, vp, vp, ctypes.c_size_t]
     L.b2k_dbscan_fit.argtypes = [vp, vp, i64, i32, f64, i32, i32, vp, vp, ctypes.POINTER(i64), ctypes.c_size_t]
+    L.b2k_rf_fit.argtypes = [vp, vp, vp, i64, i32, ctypes.POINTER(RfParams), ctypes.POINTER(i32), ctypes.POINTER(i64),
+                             vp, vp, ctypes.c_size_t]
+    L.b2k_rf_forest.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp]
+    L.b2k_rf_predict.argtypes = [vp, vp, i64, i32, i32, vp, vp, vp, vp, vp, i32, i32, vp, vp, vp, ctypes.c_size_t]
     for name in EXPORTED_SYMBOLS:
         if name not in ("b2k_last_error",):
             getattr(L, name).restype = i32
@@ -654,3 +677,65 @@ class Context:
                                                METRIC_CODES[metric], labels.data_ptr(), core.data_ptr(),
                                                ctypes.byref(ncl), self._stream()))
         return labels, core.bool(), int(ncl.value)
+
+    # -- random forests ---------------------------------------------------------------------
+    def rf_fit(self, X: Any, y: Any, *, n_trees: int = 20, max_depth: int = 5, max_bins: int = 32,
+               min_instances: int = 1, features_per_node: Optional[int] = None, bootstrap: bool = True,
+               impurity: str = "gini", min_info_gain: float = 0.0, seed: int = 0) -> Dict[str, Any]:
+        """A random forest over all ranks' rows (collective when a communicator is initialised): X [n, d] and y [n]
+        float32 CUDA tensors (either may have 0 rows on a rank that then fails with every other).  impurity "gini" or
+        "entropy" (classification, y the class values) or "variance" (regression).  Returns host arrays:
+        tree_offsets int64 [T + 1], feature int32 [N] (-1 for a leaf), threshold float32 [N], children int32 [N, 2],
+        gain float64 [N], count int64 [N], value float64 [N, V], and n_values V, level_ms [max_depth + 1] (with option
+        time_kernels), level_updates [max_depth + 1]."""
+        n, d = self._check_X(X)
+        self._check_y(y, n)
+        if impurity not in IMPURITY_CODES:
+            raise ValueError(f"impurity must be one of {sorted(IMPURITY_CODES)}, got {impurity!r}")
+        prm = RfParams(int(n_trees), int(max_depth), int(max_bins), int(min_instances),
+                       int(d if features_per_node is None else features_per_node), int(bool(bootstrap)),
+                       IMPURITY_CODES[impurity], 0, float(min_info_gain), int(seed) & 0xFFFFFFFFFFFFFFFF)
+        nv, nn = ctypes.c_int(0), ctypes.c_int64(0)
+        L = max(int(max_depth), 0) + 1
+        lms = np.zeros(L, dtype=np.float64)
+        lup = np.zeros(L, dtype=np.int64)
+        with self._torch.cuda.device(self.device):
+            self._check(self._L.b2k_rf_fit(self._h, X.data_ptr(), y.data_ptr(), n, d, ctypes.byref(prm),
+                                           ctypes.byref(nv), ctypes.byref(nn), lms.ctypes.data, lup.ctypes.data,
+                                           self._stream()))
+        V, N, T = int(nv.value), int(nn.value), int(n_trees)
+        out = {"tree_offsets": np.zeros(T + 1, dtype=np.int64), "feature": np.zeros(N, dtype=np.int32),
+               "threshold": np.zeros(N, dtype=np.float32), "children": np.zeros((N, 2), dtype=np.int32),
+               "gain": np.zeros(N, dtype=np.float64), "count": np.zeros(N, dtype=np.int64),
+               "value": np.zeros((N, V), dtype=np.float64)}
+        self._check(self._L.b2k_rf_forest(self._h, *[out[key].ctypes.data for key in
+                                                     ("tree_offsets", "feature", "threshold", "children", "gain",
+                                                      "count", "value")]))
+        out.update(n_values=V, level_ms=lms, level_updates=lup)
+        return out
+
+    def rf_predict(self, X: Any, forest: Dict[str, Any], classification: bool) -> Tuple[Any, Any, Any]:
+        """k_rf_predict over X [n, d] with a forest laid out as rf_fit's output -> float64 CUDA tensors rawPrediction
+        [n, V], probability [n, V] and prediction [n] (classification; prediction = the class index), or (None, None,
+        prediction [n]) for regression."""
+        t = self._torch
+        n, d = self._check_X(X)
+        off = np.ascontiguousarray(forest["tree_offsets"], dtype=np.int64)
+        T = int(off.size) - 1
+        value = np.ascontiguousarray(forest["value"], dtype=np.float64)
+        V = int(value.shape[1])
+        dev = {key: t.as_tensor(np.ascontiguousarray(forest[key], dtype=dt), device=self.device)
+               for key, dt in (("feature", np.int32), ("threshold", np.float32), ("children", np.int32))}
+        offd = t.as_tensor(off, device=self.device)
+        vald = t.as_tensor(value, device=self.device)
+        raw = t.empty((n, V), dtype=t.float64, device=self.device) if classification else None
+        prob = t.empty((n, V), dtype=t.float64, device=self.device) if classification else None
+        pred = t.empty((n,), dtype=t.float64, device=self.device)
+        with t.cuda.device(self.device):
+            self._check(self._L.b2k_rf_predict(self._h, X.data_ptr(), n, d, T, offd.data_ptr(),
+                                               dev["feature"].data_ptr(), dev["threshold"].data_ptr(),
+                                               dev["children"].data_ptr(), vald.data_ptr(), V, int(bool(classification)),
+                                               raw.data_ptr() if raw is not None else None,
+                                               prob.data_ptr() if prob is not None else None, pred.data_ptr(),
+                                               self._stream()))
+        return raw, prob, pred

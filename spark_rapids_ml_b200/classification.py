@@ -32,6 +32,7 @@ from .core import FitInputType, _append_transform_features, _CumlEstimator, _Cum
 from .core import _transform_context, alias, param_alias
 from .params import HasFeaturesCol, HasFeaturesCols, HasLabelCol, HasPredictionCol, P, _CumlClass, _CumlParams
 from .regression import _ModelIterator
+from .tree import _RandomForestEstimator, _RandomForestModel
 from .sparkshim import BarrierTaskContext, LocalDataFrame, Param, Row, TypeConverters, keyword_only
 
 
@@ -590,3 +591,83 @@ class _SparseIntercepts:
         for i, v in self.values.items():
             a[i] = v
         return a
+
+
+class RandomForestClassifier(_RandomForestEstimator):
+    """Random forest classification on H100 (reference classification.py:285-498).  Every tree is grown from the gini
+    or entropy histograms of all workers' rows, with one allreduce per histogram pass, so the forest does not depend on
+    the number of workers.  Parameters as in the reference: featuresCol (str or list of str), labelCol, predictionCol,
+    probabilityCol, rawPredictionCol, maxDepth (5), maxBins (32), minInstancesPerNode (1), minInfoGain (0.0), impurity
+    ("gini"), numTrees (20), featureSubsetStrategy ("auto"), seed, bootstrap (True), num_workers, verbose.  Labels are
+    the class indices 0, 1, ...; numClasses = max label + 1.
+
+    >>> from spark_rapids_ml_b200.classification import RandomForestClassifier
+    >>> df = session.createDataFrame([([1.0, 2.0], 1.0), ([1.0, 3.0], 1.0), ([2.0, 1.0], 0.0), ([3.0, 1.0], 0.0)],
+    ...                              "features array<float>, label float")
+    >>> RandomForestClassifier(numTrees=3, bootstrap=False).fit(df).transform(df)
+    """
+
+    probabilityCol = Param("parent", "probabilityCol", "Column name for predicted class conditional probabilities.",
+                           TypeConverters.toString)
+    rawPredictionCol = Param("parent", "rawPredictionCol", "raw prediction (a.k.a. confidence) column name.",
+                             TypeConverters.toString)
+
+    @keyword_only
+    def __init__(self, *, featuresCol: Union[str, List[str]] = "features", labelCol: str = "label",
+                 predictionCol: str = "prediction", probabilityCol: str = "probability",
+                 rawPredictionCol: str = "rawPrediction", maxDepth: int = 5, maxBins: int = 32,
+                 minInstancesPerNode: int = 1, minInfoGain: float = 0.0, maxMemoryInMB: int = 256,
+                 cacheNodeIds: bool = False, checkpointInterval: int = 10, impurity: str = "gini", numTrees: int = 20,
+                 featureSubsetStrategy: str = "auto", seed: Optional[int] = None, subsamplingRate: float = 1.0,
+                 leafCol: str = "", minWeightFractionPerNode: float = 0.0, weightCol: Optional[str] = None,
+                 bootstrap: Optional[bool] = True, num_workers: Optional[int] = None, verbose: Union[int, bool] = False,
+                 **kwargs: Any) -> None:
+        super().__init__(**kwargs)
+
+    def _init_defaults(self) -> None:
+        self._setDefault(impurity="gini", probabilityCol="probability", rawPredictionCol="rawPrediction")
+
+    def _is_classification(self) -> bool:
+        return True
+
+    def _model_class(self) -> Any:
+        return RandomForestClassificationModel
+
+    def setProbabilityCol(self, value: str) -> "RandomForestClassifier":
+        return self._set_params(probabilityCol=value)
+
+    def setRawPredictionCol(self, value: str) -> "RandomForestClassifier":
+        return self._set_params(rawPredictionCol=value)
+
+
+class RandomForestClassificationModel(_RandomForestModel):
+    """reference: classification.py:501-676.  transform() appends rawPredictionCol (the sum of the trees' leaf
+    probabilities), probabilityCol (raw normalised) and predictionCol (the class of the largest raw value)."""
+
+    probabilityCol = RandomForestClassifier.probabilityCol
+    rawPredictionCol = RandomForestClassifier.rawPredictionCol
+
+    def _init_defaults(self) -> None:
+        self._setDefault(impurity="gini", probabilityCol="probability", rawPredictionCol="rawPrediction")
+
+    def _is_classification(self) -> bool:
+        return True
+
+    @property
+    def numClasses(self) -> int:
+        return self._num_classes
+
+    def setProbabilityCol(self, value: str) -> "RandomForestClassificationModel":
+        return self._set_params(probabilityCol=value)
+
+    def setRawPredictionCol(self, value: str) -> "RandomForestClassificationModel":
+        return self._set_params(rawPredictionCol=value)
+
+    def predictRaw(self, value: Any) -> Any:
+        raise NotImplementedError("predictRaw() of a single vector is not supported; use transform()")
+
+    def predictProbability(self, value: Any) -> Any:
+        raise NotImplementedError("predictProbability() of a single vector is not supported; use transform()")
+
+    def evaluate(self, dataset: Any) -> Any:
+        raise NotImplementedError("RandomForestClassificationModel.evaluate() is not supported in this build")

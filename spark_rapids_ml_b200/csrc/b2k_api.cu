@@ -115,6 +115,9 @@ extern "C" int b2k_ctx_set_option(b2k_ctx* ctx, const char* key, int64_t value) 
   } else if (k == "grid_limit") {
     if (value < 0) return b2k_fail(ctx, B2K_ERR_INVALID, "grid_limit must be >= 0");
     ctx->grid_limit = (int)value;
+  } else if (k == "rf_group_nodes" || k == "rf_flush_tiles") {
+    if (value < 0 || value > (1 << 30)) return b2k_fail(ctx, B2K_ERR_INVALID, k + " must be in [0, 2^30]");
+    (k == "rf_group_nodes" ? ctx->rf_group_nodes : ctx->rf_flush_tiles) = (int)value;
   } else {
     return b2k_fail(ctx, B2K_ERR_INVALID, "unknown option: " + k);
   }
@@ -993,6 +996,43 @@ extern "C" int b2k_dbscan_fit(b2k_ctx* ctx, const float* X, int64_t n_local, int
   B2K_CUDA_OK(ctx, cudaSetDevice(ctx->device));
   return b2k_dbscan_fit_impl(ctx, X, n_local, d, eps, min_samples, metric, labels_out, core_out, n_clusters_out,
                              reinterpret_cast<cudaStream_t>(stream));
+}
+
+// ------------------------------------------------------------------------------------------------
+// random forests (b2k_rf.cu)
+// ------------------------------------------------------------------------------------------------
+extern "C" int b2k_rf_fit(b2k_ctx* ctx, const float* X, const float* y, int64_t n_local, int d,
+                          const b2k_rf_params* params, int* n_values_out, int64_t* n_nodes_out, double* level_ms_out,
+                          int64_t* level_updates_out, uintptr_t stream) {
+  if (!ctx) return b2k_fail(nullptr, B2K_ERR_INVALID, "b2k_rf_fit: ctx is NULL");
+  // an empty partition may come with no buffers; every value check runs after the size allgather, on every rank alike
+  if (n_local < 0 || d <= 0 || (n_local > 0 && (!X || !y)) || !params || !n_values_out || !n_nodes_out)
+    return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_rf_fit: bad X/y/params/outputs/n/d");
+  B2K_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  return b2k_rf_fit_impl(ctx, X, y, n_local, d, *params, n_values_out, n_nodes_out, level_ms_out, level_updates_out,
+                         reinterpret_cast<cudaStream_t>(stream));
+}
+
+extern "C" int b2k_rf_forest(b2k_ctx* ctx, int64_t* tree_offsets_out, int32_t* feature_out, float* threshold_out,
+                             int32_t* children_out, double* gain_out, int64_t* count_out, double* value_out) {
+  if (!ctx) return b2k_fail(nullptr, B2K_ERR_INVALID, "b2k_rf_forest: ctx is NULL");
+  if (!tree_offsets_out || !feature_out || !threshold_out || !children_out || !gain_out || !count_out || !value_out)
+    return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_rf_forest: NULL output");
+  return b2k_rf_forest_impl(ctx, tree_offsets_out, feature_out, threshold_out, children_out, gain_out, count_out,
+                            value_out);
+}
+
+extern "C" int b2k_rf_predict(b2k_ctx* ctx, const float* X, int64_t n, int d, int n_trees, const int64_t* tree_offsets,
+                              const int32_t* feature, const float* threshold, const int32_t* children,
+                              const double* value, int n_values, int classification, double* raw_out,
+                              double* prob_out, double* pred_out, uintptr_t stream) {
+  if (!ctx) return b2k_fail(nullptr, B2K_ERR_INVALID, "b2k_rf_predict: ctx is NULL");
+  if (n < 0 || d <= 0 || n_trees < 1 || n_values < 1 || (n > 0 && (!X || !pred_out)) || !tree_offsets || !feature ||
+      !threshold || !children || !value || (classification && n > 0 && (!raw_out || !prob_out)))
+    return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_rf_predict: bad arguments");
+  B2K_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  return b2k_rf_predict_impl(ctx, X, n, d, n_trees, tree_offsets, feature, threshold, children, value, n_values,
+                             classification, raw_out, prob_out, pred_out, reinterpret_cast<cudaStream_t>(stream));
 }
 
 // ------------------------------------------------------------------------------------------------

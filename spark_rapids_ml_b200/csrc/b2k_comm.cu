@@ -161,6 +161,14 @@ int b2k_comm_allreduce_f32(b2k_ctx* ctx, float* buf, size_t count, cudaStream_t 
   return B2K_OK;
 }
 
+int b2k_comm_allreduce_i64(b2k_ctx* ctx, int64_t* buf, size_t count, cudaStream_t s) {
+  if (!ctx->nccl || ctx->nranks == 1) return B2K_OK;
+  int rc = nccl_api()->AllReduce(buf, buf, count, ncclInt64_, ncclSum_, ctx->nccl->comm, s);
+  ctx->stats.nccl_allreduces++;
+  if (rc != ncclSuccess_) return nccl_fail(ctx, "ncclAllReduce(i64)", rc);
+  return B2K_OK;
+}
+
 int b2k_comm_allgather_i64(b2k_ctx* ctx, const int64_t* send_dev, int64_t* recv_dev, size_t count_per_rank,
                            cudaStream_t s) {
   if (!ctx->nccl || ctx->nranks == 1) {

@@ -4,6 +4,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -79,6 +80,10 @@ struct b2k_ctx {
   B2kLoopState* h_state = nullptr;
   // TMA descriptor encoder (driver entry point, resolved lazily)
   void* encode_tiled = nullptr;
+  // random forests (b2k_rf.cu): the forest of the last b2k_rf_fit, read by b2k_rf_forest; test switches
+  std::shared_ptr<void> rf_forest;
+  int rf_group_nodes = 0;   // option "rf_group_nodes": cap on the nodes of one histogram pass (0 = capacity)
+  int rf_flush_tiles = 0;   // option "rf_flush_tiles": tiles per CTA between flushes of the cluster pass (0 = the bound)
   b2k_stats stats{};
 };
 
@@ -243,6 +248,8 @@ int b2k_comm_allreduce_f64(b2k_ctx* ctx, double* buf, size_t count, cudaStream_t
 int b2k_comm_allgather_i64(b2k_ctx* ctx, const int64_t* send_dev, int64_t* recv_dev, size_t count_per_rank,
                            cudaStream_t s);
 int b2k_comm_allreduce_f32(b2k_ctx* ctx, float* buf, size_t count, cudaStream_t s);
+// exact integer sums (the random-forest histograms): every rank gets the same bits whatever the reduction order
+int b2k_comm_allreduce_i64(b2k_ctx* ctx, int64_t* buf, size_t count, cudaStream_t s);
 // recv [nranks][bytes_per_rank] <- every rank's send; send may be recv's own slot (in place).  One rank: a copy.
 int b2k_comm_allgather_bytes(b2k_ctx* ctx, const void* send_dev, void* recv_dev, size_t bytes_per_rank, cudaStream_t s);
 
@@ -288,6 +295,19 @@ int b2k_knn_search_impl(b2k_ctx* ctx, const float* items, int64_t n_items, const
 // ------------------------------------------------------------------------------------------------
 int b2k_dbscan_fit_impl(b2k_ctx* ctx, const float* X, int64_t n_local, int d, double eps, int min_samples, int metric,
                         int32_t* labels_out, uint8_t* core_out, int64_t* n_clusters_out, cudaStream_t s);
+
+// ------------------------------------------------------------------------------------------------
+// random forests — b2k_rf.cu (the C ABI entry points in b2k_api.cu check their arguments, then call these)
+// ------------------------------------------------------------------------------------------------
+int b2k_rf_fit_impl(b2k_ctx* ctx, const float* X, const float* y, int64_t n_local, int d, const b2k_rf_params& p,
+                    int* n_values_out, int64_t* n_nodes_out, double* level_ms_out, int64_t* level_updates_out,
+                    cudaStream_t s);
+int b2k_rf_forest_impl(b2k_ctx* ctx, int64_t* tree_offsets_out, int32_t* feature_out, float* threshold_out,
+                       int32_t* children_out, double* gain_out, int64_t* count_out, double* value_out);
+int b2k_rf_predict_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, int n_trees, const int64_t* tree_offsets,
+                        const int32_t* feature, const float* threshold, const int32_t* children, const double* value,
+                        int n_values, int classification, double* raw_out, double* prob_out, double* pred_out,
+                        cudaStream_t s);
 
 // ------------------------------------------------------------------------------------------------
 // linear regression — b2k_linreg.cu (the C ABI entry points in b2k_api.cu check their arguments, then call these)

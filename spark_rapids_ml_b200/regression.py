@@ -405,3 +405,55 @@ class LinearRegressionModel(LinearRegressionClass, _CumlModelWithPredictionCol, 
         _transform_internal.many = _transform_many  # type: ignore[attr-defined]
         _transform_internal.row_bytes = 4 * n_cols + 8  # type: ignore[attr-defined]
         return _construct, _transform_internal, None
+
+
+from .tree import _RandomForestEstimator, _RandomForestModel  # noqa: E402  (tree.py imports this module lazily)
+
+
+class RandomForestRegressor(_RandomForestEstimator):
+    """Random forest regression on H100 (reference regression.py:865-1048).  Every tree is grown from the variance
+    histograms of all workers' rows, with one allreduce per histogram pass, so the forest does not depend on the number
+    of workers.  Labels are resolved to max|y| 2^-24 (DESIGN.md §15).  Parameters as in the reference: featuresCol (str
+    or list of str), labelCol, predictionCol, maxDepth (5), maxBins (32), minInstancesPerNode (1), minInfoGain (0.0),
+    impurity ("variance"), numTrees (20), featureSubsetStrategy ("auto"), seed, bootstrap (True), num_workers,
+    verbose.
+
+    >>> from spark_rapids_ml_b200.regression import RandomForestRegressor
+    >>> df = session.createDataFrame([([1.0, 2.0], 1.5), ([1.0, 3.0], 2.5), ([2.0, 1.0], 0.5), ([3.0, 1.0], 0.0)],
+    ...                              "features array<float>, label float")
+    >>> RandomForestRegressor(numTrees=3, bootstrap=False).fit(df).transform(df)
+    """
+
+    @keyword_only
+    def __init__(self, *, featuresCol: Union[str, List[str]] = "features", labelCol: str = "label",
+                 predictionCol: str = "prediction", maxDepth: int = 5, maxBins: int = 32, minInstancesPerNode: int = 1,
+                 minInfoGain: float = 0.0, maxMemoryInMB: int = 256, cacheNodeIds: bool = False,
+                 checkpointInterval: int = 10, impurity: str = "variance", subsamplingRate: float = 1.0,
+                 seed: Optional[int] = None, numTrees: int = 20, featureSubsetStrategy: str = "auto",
+                 leafCol: str = "", minWeightFractionPerNode: float = 0.0, weightCol: Optional[str] = None,
+                 bootstrap: Optional[bool] = True, num_workers: Optional[int] = None, verbose: Union[int, bool] = False,
+                 **kwargs: Any) -> None:
+        super().__init__(**kwargs)
+
+    def _init_defaults(self) -> None:
+        self._setDefault(impurity="variance")
+
+    def _is_classification(self) -> bool:
+        return False
+
+    def _model_class(self) -> Any:
+        return RandomForestRegressionModel
+
+
+class RandomForestRegressionModel(_RandomForestModel):
+    """reference: regression.py:1051-1147.  transform() appends predictionCol, the mean of the trees' leaf values in
+    tree order."""
+
+    def _init_defaults(self) -> None:
+        self._setDefault(impurity="variance")
+
+    def _is_classification(self) -> bool:
+        return False
+
+    def evaluate(self, dataset: Any) -> Any:
+        raise NotImplementedError("RandomForestRegressionModel.evaluate() is not supported in this build")
