@@ -519,6 +519,53 @@ int b2k_rf_predict(b2k_ctx* ctx, const float* X, int64_t n, int d, int n_trees, 
 /* L(p) of the entropy above, p in (0, 1]: p = m 2^E (frexp; m < 0.7071067811865476: m = 2m, E = E - 1), z = (m - 1)
  * / (m + 1), z2 = z z, a = 1.0 / 25; a = a z2 + 1.0 / (2i + 1) for i = 11..0; L = ((z a) 2) 1.4426950408889634 + E. */
 
+/* ---- evaluation (b2k_eval.cu): M models scored on one validation set in one read of X ----
+ * Replaces the reference's multi-model transform-and-evaluate loop (python core.py:1572-1693, classification.py:161-282),
+ * which reads X once per model per batch and hands every row's outputs to the host metric code.  Here a CTA stages a
+ * tile of rows of X [n, d] (device f32, row-major) and y [n] (device f32) in shared memory and evaluates every model from
+ * it, so X is read from HBM once per call, whatever M is, unless the models' accumulators exceed one CTA's shared memory
+ * (at most 32 models, or fewer for large n_classes, per chunk); the call then splits the models into chunks, one read of
+ * X each, with the same results.
+ * Each model's per-row prediction has exactly the bits its own predict entry point writes (b2k_linreg_predict,
+ * b2k_logreg_predict, b2k_rf_predict): the per-row code is one definition, shared.
+ * Classification (n_classes = C = 1 + max(the largest label, the largest class value a model can predict); the labels
+ * must follow b2k_logreg_labels' rule and its messages: integers in [0, 1024); n == 0 gives C from the models alone):
+ *   label_count_out [C]  rows per label value
+ *   tp_out [M][C]        rows whose prediction equals their label, by label
+ *   fp_out [M][C]        rows whose prediction differs from their label, by the predicted class value
+ *   loss_out [M]         sum over rows of -log(max(p_y, eps)) in fp64, p_y = the model's probability vector at index y
+ *                        (as the probability column transform() writes it; 0 when y is past its end)
+ * Regression: reg_out [M][3][5], for the columns (label, label - prediction, prediction) in fp64:
+ *   {count, mean, m2n = sum (x - mean)^2, m2 = sum x^2, l1 = sum |x|}.  Per tile, mean and m2n are formed about the
+ *   tile's mean; tiles, then CTAs in CTA order, merge by Chan's update (n = na + nb, delta = mb - ma, mean = ma + delta
+ *   nb / n, m2n = m2n_a + m2n_b + delta^2 na nb / n), so a label with a large offset keeps its precision.
+ * Integer counts are summed with atomics (exact, order-free); fp64 sums use per-CTA partials folded in CTA order.  The
+ * grid depends on the device, the shape and option "grid_limit" alone: two calls on the same input give the same bits.
+ * n == 0 is legal and gives zero accumulators.  The work runs on `stream`; the call returns once the accumulators are
+ * copied to the host (it synchronises `stream`). */
+#define B2K_EVAL_IDENTITY 0 /* linear regression: b + x . w */
+#define B2K_EVAL_LOGISTIC 1 /* binomial logistic regression (one row of W; class values [2]) */
+#define B2K_EVAL_SOFTMAX 2  /* multinomial logistic regression (K' >= 2 rows of W; class values [K']) */
+#define B2K_EVAL_REG_COLS 3
+#define B2K_EVAL_REG_STATS 5
+/* M linear models, all identity (regression) or all logistic / softmax (classification, mixed K' allowed).  Host
+ * arrays: kind [M]; row_offsets [M + 1] (model i owns rows row_offsets[i] .. row_offsets[i + 1] - 1 of W and b,
+ * row_offsets[0] = 0); W [rows][d] fp64; b [rows] fp64; class_values (classification) = per model, in order, the class
+ * value of each prediction index (2 for logistic, K' for softmax: prediction = class_values[argmax]).  d <= 1024. */
+int b2k_eval_linear(b2k_ctx* ctx, const float* X, const float* y, int64_t n, int d, int n_models, const int32_t* kind,
+                    const int32_t* row_offsets, const double* W, const double* b, const double* class_values,
+                    int n_classes, double eps, int64_t* label_count_out, int64_t* tp_out, int64_t* fp_out,
+                    double* loss_out, double* reg_out, uintptr_t stream);
+/* M forests in b2k_rf_predict's layout, concatenated, host arrays: n_trees [M], n_values [M] (V; 1 for regression),
+ * tree_offsets [sum (T_i + 1)] (each forest's own offsets, starting at 0), then per node, all forests' nodes in order:
+ * feature, threshold, children [2] (tree-local) and value [V_i].  Forests may differ in trees, depth and bins.
+ * classification = 1: prediction = argmax of the summed leaf values, p = raw / sum raw (as b2k_rf_predict). */
+int b2k_eval_forest(b2k_ctx* ctx, const float* X, const float* y, int64_t n, int d, int n_models, int classification,
+                    const int32_t* n_trees, const int32_t* n_values, const int64_t* tree_offsets,
+                    const int32_t* feature, const float* threshold, const int32_t* children, const double* value,
+                    int n_classes, double eps, int64_t* label_count_out, int64_t* tp_out, int64_t* fp_out,
+                    double* loss_out, double* reg_out, uintptr_t stream);
+
 #ifdef __cplusplus
 }
 #endif

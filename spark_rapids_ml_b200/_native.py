@@ -67,7 +67,11 @@ EXPORTED_SYMBOLS = (
     "b2k_rf_fit",
     "b2k_rf_forest",
     "b2k_rf_predict",
+    "b2k_eval_linear",
+    "b2k_eval_forest",
 )
+
+EVAL_KINDS = {"identity": 0, "logistic": 1, "softmax": 2}
 
 FAMILY_CODES = {"auto": 0, "binomial": 1, "multinomial": 2}
 METRIC_CODES = {"euclidean": 0, "cosine": 1}
@@ -196,6 +200,10 @@ def load_library() -> ctypes.CDLL:
                              vp, vp, ctypes.c_size_t]
     L.b2k_rf_forest.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp]
     L.b2k_rf_predict.argtypes = [vp, vp, i64, i32, i32, vp, vp, vp, vp, vp, i32, i32, vp, vp, vp, ctypes.c_size_t]
+    L.b2k_eval_linear.argtypes = [vp, vp, vp, i64, i32, i32, vp, vp, vp, vp, vp, i32, f64, vp, vp, vp, vp, vp,
+                                  ctypes.c_size_t]
+    L.b2k_eval_forest.argtypes = [vp, vp, vp, i64, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, i32, f64, vp, vp, vp, vp,
+                                  vp, ctypes.c_size_t]
     for name in EXPORTED_SYMBOLS:
         if name not in ("b2k_last_error",):
             getattr(L, name).restype = i32
@@ -739,3 +747,84 @@ class Context:
                                                prob.data_ptr() if prob is not None else None, pred.data_ptr(),
                                                self._stream()))
         return raw, prob, pred
+
+    # -- evaluation -------------------------------------------------------------------------
+    def _eval_out(self, m: int, C: int, classification: bool) -> Dict[str, np.ndarray]:
+        if classification:
+            return {"label_count": np.zeros(max(C, 1), dtype=np.int64), "tp": np.zeros((m, max(C, 1)), dtype=np.int64),
+                    "fp": np.zeros((m, max(C, 1)), dtype=np.int64), "loss": np.zeros(m, dtype=np.float64)}
+        return {"reg": np.zeros((m, 3, 5), dtype=np.float64)}
+
+    def _eval_result(self, out: Dict[str, np.ndarray], n: int, C: int, classification: bool) -> Dict[str, Any]:
+        if classification:
+            return {"n": n, "label_count": out["label_count"][:C].copy(), "tp": out["tp"][:, :C].copy(),
+                    "fp": out["fp"][:, :C].copy(), "loss": out["loss"]}
+        return {"n": n, "reg": out["reg"]}
+
+    def eval_linear(self, X: Any, y: Any, models: Sequence[Dict[str, Any]], eps: float = 1e-15) -> Dict[str, Any]:
+        """b2k_eval_linear: M linear models scored on (X [n, d], y [n]) float32 CUDA tensors in one read of X.  Each
+        model is a dict: kind ("identity", "logistic" or "softmax"), W [K', d], b [K'] and, for the logistic kinds,
+        class_values [2 or K'].  Returns host arrays: classification {n, label_count [C], tp [M, C], fp [M, C],
+        loss [M]} (C = 1 + the largest label or class value), regression {n, reg [M, 3, 5]} (columns label,
+        label - prediction, prediction; stats count, mean, m2n, m2, l1)."""
+        n, d = self._check_X(X)
+        self._check_y(y, n)
+        m = len(models)
+        kinds = np.array([EVAL_KINDS[md["kind"]] for md in models], dtype=np.int32)
+        Ws = [np.ascontiguousarray(md["W"], dtype=np.float64).reshape(-1, d) for md in models]
+        rows = np.zeros(m + 1, dtype=np.int32)
+        rows[1:] = np.cumsum([w.shape[0] for w in Ws])
+        W = np.ascontiguousarray(np.concatenate(Ws, axis=0))
+        b = np.ascontiguousarray(np.concatenate([np.asarray(md["b"], dtype=np.float64).reshape(-1) for md in models]))
+        classification = bool(kinds[0] != 0)
+        cv = (np.ascontiguousarray(np.concatenate([np.asarray(md["class_values"], dtype=np.float64).reshape(-1)
+                                                   for md in models])) if classification else np.zeros(1))
+        C = self._eval_classes(y, n, int(cv.max()) + 1 if classification and cv.size else 0) if classification else 0
+        out = self._eval_out(m, C, classification)
+        with self._torch.cuda.device(self.device):
+            self._check(self._L.b2k_eval_linear(
+                self._h, X.data_ptr(), y.data_ptr(), n, d, m, kinds.ctypes.data, rows.ctypes.data, W.ctypes.data,
+                b.ctypes.data, cv.ctypes.data, C, float(eps), *self._eval_ptrs(out, classification), self._stream()))
+        return self._eval_result(out, n, C, classification)
+
+    def eval_forest(self, X: Any, y: Any, forests: Sequence[Dict[str, Any]], classification: bool,
+                    eps: float = 1e-15) -> Dict[str, Any]:
+        """b2k_eval_forest: M forests (each laid out as rf_fit's output) scored on (X, y) in one read of X.  Returns
+        what eval_linear returns."""
+        n, d = self._check_X(X)
+        self._check_y(y, n)
+        m = len(forests)
+        offs = [np.ascontiguousarray(f["tree_offsets"], dtype=np.int64) for f in forests]
+        vals = [np.ascontiguousarray(f["value"], dtype=np.float64) for f in forests]
+        nt = np.array([o.size - 1 for o in offs], dtype=np.int32)
+        nv = np.array([v.shape[1] for v in vals], dtype=np.int32)
+        off = np.ascontiguousarray(np.concatenate(offs))
+        feat = np.ascontiguousarray(np.concatenate([np.asarray(f["feature"], dtype=np.int32) for f in forests]))
+        thr = np.ascontiguousarray(np.concatenate([np.asarray(f["threshold"], dtype=np.float32) for f in forests]))
+        ch = np.ascontiguousarray(np.concatenate([np.asarray(f["children"], dtype=np.int32).reshape(-1, 2)
+                                                  for f in forests]))
+        val = np.ascontiguousarray(np.concatenate([v.reshape(-1) for v in vals]))
+        C = self._eval_classes(y, n, int(nv.max())) if classification else 0
+        out = self._eval_out(m, C, classification)
+        with self._torch.cuda.device(self.device):
+            self._check(self._L.b2k_eval_forest(
+                self._h, X.data_ptr(), y.data_ptr(), n, d, m, int(bool(classification)), nt.ctypes.data,
+                nv.ctypes.data, off.ctypes.data, feat.ctypes.data, thr.ctypes.data, ch.ctypes.data, val.ctypes.data, C,
+                float(eps), *self._eval_ptrs(out, classification), self._stream()))
+        return self._eval_result(out, n, C, classification)
+
+    def _eval_classes(self, y: Any, n: int, c_models: int) -> int:
+        """C = 1 + max(the largest label, the models' largest class); a bad label is reported by the pass itself."""
+        if n == 0:
+            return c_models
+        t = self._torch
+        finite = t.isfinite(y)
+        mx = float(y[finite].max().item()) if bool(finite.any().item()) else 0.0
+        return max(c_models, int(mx) + 1 if 0 <= mx < 1024 and mx == int(mx) else 1)
+
+    @staticmethod
+    def _eval_ptrs(out: Dict[str, np.ndarray], classification: bool) -> List[Any]:
+        if classification:
+            return [out["label_count"].ctypes.data, out["tp"].ctypes.data, out["fp"].ctypes.data,
+                    out["loss"].ctypes.data, None]
+        return [None, None, None, None, out["reg"].ctypes.data]

@@ -345,6 +345,11 @@ class LogisticRegression(LogisticRegressionClass, _CumlEstimator, _LogisticRegre
     def _enable_fit_multiple_in_single_pass(self) -> bool:
         return True
 
+    def _supportsTransformEvaluate(self, evaluator: Any) -> bool:
+        from .core import _supports_transform_evaluate
+
+        return _supports_transform_evaluate(True, evaluator)
+
     def fitMultiple(self, dataset: Any, paramMaps: Sequence[Dict[Any, Any]]) -> Iterator[Tuple[int, Any]]:
         """(index, model) per param map, in map order.  When every map changes only fit params (regParam,
         elasticNetParam, maxIter, tol, fitIntercept, standardization, family), one ingest, one label pass and one
@@ -479,8 +484,41 @@ class LogisticRegressionModel(LogisticRegressionClass, _CumlModelWithPredictionC
             cls = np.array([0.0, 1.0])
         return W, b, cls
 
+    def _eval_models(self) -> List[Dict[str, Any]]:
+        """Each model of this (combined) instance as b2k_eval_linear takes it, with the class values transform() uses."""
+        n = self._get_num_models()
+        coefs = [self.coef_] if n == 1 else list(self.coef_)
+        icpts = [self.intercept_] if n == 1 else list(self.intercept_)
+        out = []
+        for c, i in zip(coefs, icpts):
+            W = np.asarray(c, dtype=np.float64)
+            b = np.asarray(i, dtype=np.float64).reshape(-1)
+            cls = np.asarray(self.classes_, dtype=np.float64)
+            if W.shape[0] == 1 and cls.size == 1:
+                cls = np.array([0.0, 1.0])
+            kp = int(W.shape[0])
+            out.append({"kind": "logistic" if kp == 1 else "softmax", "W": W, "b": b,
+                        "class_values": cls[:2] if kp == 1 else cls[:kp]})
+        return out
+
     def _get_cuml_transform_func(self, dataset: Any, eval_metric_info: Any = None
                                  ) -> Tuple[Callable, Callable, Optional[Callable]]:
+        if eval_metric_info is not None:
+            from .core import _class_accs
+
+            if not eval_metric_info["classification"]:
+                raise NotImplementedError("LogisticRegressionModel is evaluated with a MulticlassClassificationEvaluator")
+            models = self._eval_models()
+            eps = eval_metric_info["eps"]
+
+            class _Holder:
+                def __init__(self, gpu: int) -> None:
+                    self.ctx = _transform_context(gpu)
+
+            def _evaluate(h: Any, X: Any, y: Any) -> List[Dict[str, Any]]:
+                return _class_accs(h.ctx.eval_linear(X, y, models, eps))
+
+            return _Holder, None, _evaluate  # type: ignore[return-value]
         W, b, cls = self._device_model()
         n_cols = int(self.n_cols)
 

@@ -489,6 +489,108 @@ def _iter_transform(transform_internal: Callable, get_model: Callable[[], Any], 
         yield from many(get_model(), group)
 
 
+def _supports_transform_evaluate(classification: bool, evaluator: Any) -> bool:
+    """Whether the single-pass evaluation serves (estimator kind, evaluator): a classifier with a
+    MulticlassClassificationEvaluator and a metric of metrics.MULTICLASS_METRICS, or a regressor with a
+    RegressionEvaluator."""
+    from . import metrics
+
+    name = type(evaluator).__name__
+    try:
+        metric = evaluator.getMetricName()
+    except Exception:
+        return False
+    if classification:
+        return name == "MulticlassClassificationEvaluator" and metric in metrics.MULTICLASS_METRICS
+    return name == "RegressionEvaluator" and metric in metrics.REGRESSION_METRICS
+
+
+def _eval_metric_info(evaluator: Any) -> Dict[str, Any]:
+    """What the device pass and the metric need from an evaluator (pyspark's or the local one)."""
+    if evaluator.isSet("weightCol") and evaluator.getOrDefault("weightCol"):
+        raise NotImplementedError("weightCol is not supported by the single-pass evaluation")
+    info = {"metric": evaluator.getMetricName(), "labelCol": evaluator.getLabelCol()}
+    if type(evaluator).__name__ == "MulticlassClassificationEvaluator":
+        info.update(classification=True, eps=float(evaluator.getEps()), metricLabel=float(evaluator.getMetricLabel()),
+                    beta=float(evaluator.getBeta()))
+    else:
+        info.update(classification=False, eps=0.0, throughOrigin=bool(evaluator.getThroughOrigin()))
+    return info
+
+
+def _transform_evaluate_internal(model: Any, dataset: Any, evaluator: Any) -> List[float]:
+    """One metric per model of a (combined) model on a local frame (reference core.py:1572-1693).  Each partition's
+    features and label are ingested as transform() ingests them, in groups of up to TRANSFORM_GROUP_ROWS rows; each
+    group is one device evaluation pass (the model's third transform function) that returns every model's
+    accumulators; the accumulators merge on the host in partition and group order.  The label goes to the device as
+    float32, as the fits read it: a float64 label that float32 cannot hold is scored at its float32 rounding."""
+    from . import metrics
+    from .sparkshim.sql import _batches_to_pdf_iter
+    from .utils import DeviceRowAppender
+
+    if HAVE_PYSPARK:
+        from . import spark_binding
+
+        if spark_binding.is_spark_dataframe(dataset):
+            raise NotImplementedError(f"{type(model).__name__}._transformEvaluate() of a pyspark DataFrame is not "
+                                      "supported in this build; evaluate a local frame")
+    info = _eval_metric_info(evaluator)
+    construct, _, evaluate = model._get_cuml_transform_func(dataset, info)
+    if evaluate is None:
+        raise NotImplementedError(f"{type(model).__name__} has no single-pass evaluation")
+    input_col, input_cols = model._get_input_columns()
+    label_col = info["labelCol"]
+    n_cols = int(model.n_cols)
+    state: Dict[str, Any] = {}
+    accs: Optional[List[Dict[str, Any]]] = None
+
+    def run(group: List[pa.RecordBatch]) -> None:
+        nonlocal accs
+        import torch
+
+        feats = [b.select(list(input_cols)) if input_cols else b.select([input_col]).rename_columns([alias.data])
+                 for b in group]
+        y = np.concatenate([np.asarray(b.column(label_col).to_numpy(zero_copy_only=False), dtype=np.float32)
+                            for b in group]) if group else np.zeros(0, np.float32)
+        m = state["model"]
+        app = DeviceRowAppender(m.ctx, n_cols, first_capacity=max(1, int(y.size)))
+        for pdf in _batches_to_pdf_iter(feats, dataset.arrow_backed_pandas):
+            if len(pdf):
+                _append_transform_features(app, pdf, n_cols)
+        X = app.finish()
+        yd = torch.as_tensor(y).to(m.ctx.device)
+        got = evaluate(m, X, yd)
+        accs = got if accs is None else [metrics.merge_all([a, b], info["classification"]) for a, b in zip(accs, got)]
+
+    limit = max(1, min(TRANSFORM_GROUP_ROWS, TRANSFORM_GROUP_BYTES // (4 * n_cols + 4)))   # as _iter_transform
+    for pid, part in enumerate(dataset._parts):
+        if "model" not in state:
+            gpu = _CumlCommon._set_gpu_device(BarrierTaskContext(pid, len(dataset._parts)), True, True)
+            state["model"] = construct(gpu)
+        group: List[pa.RecordBatch] = []
+        rows = 0
+        for batch in part:
+            group.append(batch)
+            rows += batch.num_rows
+            if rows >= limit:
+                run(group)
+                group, rows = [], 0
+        if group or accs is None:
+            run(group)
+    assert accs is not None
+    if info["classification"]:
+        return [metrics.multiclass_metric(a, info["metric"], info["metricLabel"], info["beta"]) for a in accs]
+    return [metrics.regression_metric(a, info["metric"], info["throughOrigin"]) for a in accs]
+
+
+def _class_accs(res: Dict[str, Any]) -> List[Dict[str, Any]]:
+    """Per-model accumulators of one Context.eval_* result."""
+    if "reg" in res:
+        return [{"n": res["n"], "reg": r} for r in res["reg"]]
+    return [{"n": res["n"], "label_count": res["label_count"], "tp": t, "fp": f, "loss": float(l)}
+            for t, f, l in zip(res["tp"], res["fp"], res["loss"])]
+
+
 def _parse_conf_bool(v: str) -> bool:
     if v not in ("true", "false"):
         raise ValueError(v)
@@ -710,6 +812,11 @@ class _CumlModel(ModelBase, _CumlParams, _CumlCommon):
     if not HAVE_PYSPARK:   # pyspark.ml.Transformer.transform(dataset, params) -> self._transform(dataset) otherwise
         def transform(self, dataset: LocalDataFrame) -> LocalDataFrame:
             return self._transform(dataset)
+
+    def _transformEvaluate(self, dataset: Any, evaluator: Any, params: Optional[Dict[Any, Any]] = None) -> List[float]:
+        """The evaluator's metric for every model of this (combined) model on a local frame, one device pass per
+        ingest group (reference core.py:1572-1693)."""
+        return _transform_evaluate_internal(self.copy(params) if params else self, dataset, evaluator)
 
 
 class _CumlModelWithColumns(_CumlModel):

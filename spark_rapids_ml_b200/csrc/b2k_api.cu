@@ -1126,3 +1126,42 @@ extern "C" int b2k_logreg_predict(b2k_ctx* ctx, const float* X, int64_t n, int d
   return b2k_logreg_predict_impl(ctx, X, n, d, kp, W, b, class_values, raw_out, prob_out, pred_out,
                                  reinterpret_cast<cudaStream_t>(stream));
 }
+
+// ------------------------------------------------------------------------------------------------
+// evaluation (b2k_eval.cu)
+// ------------------------------------------------------------------------------------------------
+static bool eval_outputs_ok(int classification, int64_t* label_count_out, int64_t* tp_out, int64_t* fp_out,
+                            double* loss_out, double* reg_out) {
+  return classification ? (label_count_out && tp_out && fp_out && loss_out) : reg_out != nullptr;
+}
+
+extern "C" int b2k_eval_linear(b2k_ctx* ctx, const float* X, const float* y, int64_t n, int d, int n_models,
+                               const int32_t* kind, const int32_t* row_offsets, const double* W, const double* b,
+                               const double* class_values, int n_classes, double eps, int64_t* label_count_out,
+                               int64_t* tp_out, int64_t* fp_out, double* loss_out, double* reg_out, uintptr_t stream) {
+  if (!ctx) return b2k_fail(nullptr, B2K_ERR_INVALID, "b2k_eval_linear: ctx is NULL");
+  if (n < 0 || d <= 0 || n_models < 1 || (n > 0 && (!X || !y)) || !kind || !row_offsets || !W || !b ||
+      !(eps >= 0.0) || !eval_outputs_ok(kind[0] != B2K_EVAL_IDENTITY, label_count_out, tp_out, fp_out, loss_out, reg_out) ||
+      (kind[0] != B2K_EVAL_IDENTITY && !class_values))
+    return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_eval_linear: bad arguments");
+  B2K_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  return b2k_eval_linear_impl(ctx, X, y, n, d, n_models, kind, row_offsets, W, b, class_values, n_classes, eps,
+                              label_count_out, tp_out, fp_out, loss_out, reg_out, reinterpret_cast<cudaStream_t>(stream));
+}
+
+extern "C" int b2k_eval_forest(b2k_ctx* ctx, const float* X, const float* y, int64_t n, int d, int n_models,
+                               int classification, const int32_t* n_trees, const int32_t* n_values,
+                               const int64_t* tree_offsets, const int32_t* feature, const float* threshold,
+                               const int32_t* children, const double* value, int n_classes, double eps,
+                               int64_t* label_count_out, int64_t* tp_out, int64_t* fp_out, double* loss_out,
+                               double* reg_out, uintptr_t stream) {
+  if (!ctx) return b2k_fail(nullptr, B2K_ERR_INVALID, "b2k_eval_forest: ctx is NULL");
+  if (n < 0 || d <= 0 || n_models < 1 || (n > 0 && (!X || !y)) || !n_trees || !n_values || !tree_offsets || !feature ||
+      !threshold || !children || !value || !(eps >= 0.0) ||
+      !eval_outputs_ok(classification, label_count_out, tp_out, fp_out, loss_out, reg_out))
+    return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_eval_forest: bad arguments");
+  B2K_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  return b2k_eval_forest_impl(ctx, X, y, n, d, n_models, classification, n_trees, n_values, tree_offsets, feature,
+                              threshold, children, value, n_classes, eps, label_count_out, tp_out, fp_out, loss_out,
+                              reg_out, reinterpret_cast<cudaStream_t>(stream));
+}

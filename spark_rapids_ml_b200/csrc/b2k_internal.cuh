@@ -348,3 +348,16 @@ int b2k_logreg_fit_impl(b2k_ctx* ctx, const float* X, const float* y, int64_t n,
 int b2k_logreg_predict_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, int kp, const double* W, const double* b,
                             const double* class_values, double* raw_out, double* prob_out, double* pred_out,
                             cudaStream_t s);
+
+// ------------------------------------------------------------------------------------------------
+// evaluation — b2k_eval.cu (the C ABI entry points in b2k_api.cu check their arguments, then call these)
+// ------------------------------------------------------------------------------------------------
+int b2k_eval_linear_impl(b2k_ctx* ctx, const float* X, const float* y, int64_t n, int d, int m, const int32_t* kind,
+                         const int32_t* row_offsets, const double* W, const double* b, const double* class_values,
+                         int n_classes, double eps, int64_t* label_count_out, int64_t* tp_out, int64_t* fp_out,
+                         double* loss_out, double* reg_out, cudaStream_t s);
+int b2k_eval_forest_impl(b2k_ctx* ctx, const float* X, const float* y, int64_t n, int d, int m, int classification,
+                         const int32_t* n_trees, const int32_t* n_values, const int64_t* tree_offsets,
+                         const int32_t* feature, const float* threshold, const int32_t* children, const double* value,
+                         int n_classes, double eps, int64_t* label_count_out, int64_t* tp_out, int64_t* fp_out,
+                         double* loss_out, double* reg_out, cudaStream_t s);

@@ -17,6 +17,7 @@
 #include <vector>
 
 #include "b2k_internal.cuh"
+#include "b2k_rows.cuh"
 
 namespace {
 
@@ -80,37 +81,13 @@ k_linreg_predict(const float* __restrict__ X, int64_t n, int d, const double* __
   for (int64_t r0 = warp * rpw; r0 < n; r0 += nwarp * rpw) {
     const int64_t row = r0 + grp;
     double acc = 0.0;
-    if (row < n) {
-      const float* x = X + row * d;
-#pragma unroll 4
-      for (int k = 4 * sub; k < d; k += 4 * L) {
-        float4 v;
-        if (VEC) {
-          v = __ldcs(reinterpret_cast<const float4*>(x + k));
-        } else {
-          v.x = __ldcs(x + k);
-          v.y = k + 1 < d ? __ldcs(x + k + 1) : 0.f;
-          v.z = k + 2 < d ? __ldcs(x + k + 2) : 0.f;
-          v.w = k + 3 < d ? __ldcs(x + k + 3) : 0.f;
-        }
-        const double2 w01 = *reinterpret_cast<const double2*>(w_s + k);
-        const double2 w23 = *reinterpret_cast<const double2*>(w_s + k + 2);
-        acc = fma((double)v.x, w01.x, acc);
-        acc = fma((double)v.y, w01.y, acc);
-        acc = fma((double)v.z, w23.x, acc);
-        acc = fma((double)v.w, w23.y, acc);
-      }
-    }
-    for (int o = L >> 1; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+    if (row < n) acc = b2k_linear_lane(B2kRowLdcs<VEC>{X + row * d, d}, d, w_s, sub, L);
+    acc = b2k_lanes_sum(acc, L);
     if (sub == 0 && row < n) __stcs(out + row, b + acc);
   }
 }
 
-int predict_lanes(int d) {   // lanes per row: the least power of two covering ceil(d / 4), at most 32
-  int L = 1;
-  while (L < 32 && 4 * L < d) L <<= 1;
-  return L;
-}
+int predict_lanes(int d) { return b2k_row_lanes(d); }
 
 bool finite_all(const double* v, size_t m) {
   for (size_t i = 0; i < m; ++i)

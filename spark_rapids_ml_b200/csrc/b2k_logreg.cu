@@ -27,6 +27,7 @@
 #include <vector>
 
 #include "b2k_internal.cuh"
+#include "b2k_rows.cuh"
 
 namespace {
 
@@ -369,33 +370,9 @@ k_logreg_rows(const float* __restrict__ X, int64_t n, int d, int kp, const doubl
       double acc[RC];
 #pragma unroll
       for (int q = 0; q < RC; ++q) acc[q] = 0.0;
-      if (valid) {
-        for (int j = 4 * sub; j < d; j += 4 * L) {
-          float4 v;
-          if (VEC) {
-            v = __ldg(reinterpret_cast<const float4*>(x + j));
-          } else {
-            v.x = __ldg(x + j);
-            v.y = j + 1 < d ? __ldg(x + j + 1) : 0.f;
-            v.z = j + 2 < d ? __ldg(x + j + 2) : 0.f;
-            v.w = j + 3 < d ? __ldg(x + j + 3) : 0.f;
-          }
+      if (valid) b2k_logistic_lanes<RC>(B2kRowLdg<VEC>{x, d}, d, kp, k0, W, d, sub, L, acc);
 #pragma unroll
-          for (int q = 0; q < RC; ++q) {
-            const int k = k0 + q;
-            if (k < kp) {
-              const double* w = W + (size_t)k * d + j;
-              acc[q] = fma((double)v.x, __ldg(w), acc[q]);
-              if (j + 1 < d) acc[q] = fma((double)v.y, __ldg(w + 1), acc[q]);
-              if (j + 2 < d) acc[q] = fma((double)v.z, __ldg(w + 2), acc[q]);
-              if (j + 3 < d) acc[q] = fma((double)v.w, __ldg(w + 3), acc[q]);
-            }
-          }
-        }
-      }
-#pragma unroll
-      for (int q = 0; q < RC; ++q)
-        for (int o = L >> 1; o > 0; o >>= 1) acc[q] += __shfl_xor_sync(0xffffffffu, acc[q], o);
+      for (int q = 0; q < RC; ++q) acc[q] = b2k_lanes_sum(acc[q], L);
       if (sub == 0 && valid) {
 #pragma unroll
         for (int q = 0; q < RC; ++q) {
@@ -409,22 +386,16 @@ k_logreg_rows(const float* __restrict__ X, int64_t n, int d, int kp, const doubl
       loss[row] = row_loss_residual(mrow, kp, class_of(y[row], cmap));
     } else if (kp == 1) {
       const double m = mrow[1];
-      const double e = exp(-fabs(m));
-      const double p1 = m >= 0.0 ? 1.0 / (1.0 + e) : e / (1.0 + e);
+      const double p1 = b2k_sigmoid(m);
       mrow[0] = -m;
       prob[row * 2 + 0] = 1.0 - p1;
       prob[row * 2 + 1] = p1;
       pred[row] = cls_val[m > 0.0 ? 1 : 0];
     } else {
-      double mx = mrow[0];
-      int am = 0;
-      for (int k = 1; k < kp; ++k)
-        if (mrow[k] > mx) {
-          mx = mrow[k];
-          am = k;
-        }
-      double s = 0.0;
-      for (int k = 0; k < kp; ++k) s += exp(mrow[k] - mx);
+      const B2kArgmax ax = b2k_softmax_argmax(mrow, kp);
+      const double mx = ax.mx;
+      const int am = ax.am;
+      const double s = b2k_softmax_denominator(mrow, kp, mx);
       for (int k = 0; k < kp; ++k) prob[row * kp + k] = exp(mrow[k] - mx) / s;
       pred[row] = cls_val[am];
     }
@@ -461,11 +432,7 @@ k_logreg_xtr(const float* __restrict__ X, int64_t rows, int d, int kp, const dou
   }
 }
 
-int row_lanes(int d) {   // lanes per row: the least power of two covering ceil(d / 4), at most 32
-  int L = 1;
-  while (L < 32 && 4 * L < d) L <<= 1;
-  return L;
-}
+int row_lanes(int d) { return b2k_row_lanes(d); }
 
 // ------------------------------------------------------------------------------------------------
 // fused dispatch

@@ -11,6 +11,7 @@
 #include <vector>
 
 #include "b2k_internal.cuh"
+#include "b2k_rows.cuh"
 
 namespace cg = cooperative_groups;
 
@@ -297,11 +298,7 @@ __global__ void __launch_bounds__(RF_NT) k_rf_route(const uint8_t* __restrict__ 
 }
 
 // ---- prediction ----
-struct PNode {
-  int32_t f;
-  float t;
-  int32_t l, r;
-};
+using PNode = B2kPNode;
 template <bool SMEM>
 __global__ void __launch_bounds__(RF_NT) k_rf_predict(const float* __restrict__ X, int64_t n, int d, int T,
                                                       const int64_t* __restrict__ off, const PNode* __restrict__ nodes,
@@ -322,8 +319,7 @@ __global__ void __launch_bounds__(RF_NT) k_rf_predict(const float* __restrict__ 
       for (int k = 0; k < V; ++k) raw[r * V + k] = 0.0;
     for (int t = 0; t < T; ++t) {
       const PNode* tree = P + __ldg(off + t);
-      int i = 0;
-      for (int f = tree[0].f; f >= 0; f = tree[i].f) i = __ldg(x + f) <= tree[i].t ? tree[i].l : tree[i].r;
+      const int i = b2k_rf_leaf(tree, B2kFeatLdg{x});
       const int64_t o = __ldg(off + t);
       const double* v = value + (o + i) * V;
       if (cls) {
@@ -333,7 +329,7 @@ __global__ void __launch_bounds__(RF_NT) k_rf_predict(const float* __restrict__ 
       }
     }
     if (cls) {
-      double tot = 0.0;
+      double tot = 0.0;   // b2k_rf_class_best's order, kept inline: the call form spills here
       int best = 0;
       for (int k = 0; k < V; ++k) {
         const double a = raw[r * V + k];

@@ -289,6 +289,11 @@ class LinearRegression(LinearRegressionClass, _CumlEstimator, _LinearRegressionC
     def _enable_fit_multiple_in_single_pass(self) -> bool:
         return True
 
+    def _supportsTransformEvaluate(self, evaluator: Any) -> bool:
+        from .core import _supports_transform_evaluate
+
+        return _supports_transform_evaluate(False, evaluator)
+
     def fitMultiple(self, dataset: Any, paramMaps: Sequence[Dict[Any, Any]]) -> Iterator[Tuple[int, Any]]:
         """(index, model) per param map, in map order.  When every map changes only solver params (regParam,
         elasticNetParam, maxIter, tol, fitIntercept, standardization), one pass over the data serves all maps;
@@ -361,8 +366,31 @@ class LinearRegressionModel(LinearRegressionClass, _CumlModelWithPredictionCol, 
     def _out_schema(self, input_schema: Any = None) -> str:
         return "double"
 
+    @classmethod
+    def _combine(cls, models: List["LinearRegressionModel"]) -> "LinearRegressionModel":
+        """One model holding several fits' coefficients, for the single-pass evaluation (reference
+        classification.py:1557-1572 does this for logistic regression)."""
+        assert len(models) > 0 and all(isinstance(m, cls) for m in models)
+        first = models[0]
+        attrs = dict(first._get_model_attributes() or {})
+        attrs["coef_"] = [list(m.coef_) for m in models]
+        attrs["intercept_"] = [float(m.intercept_) for m in models]
+        out = cls(**attrs)
+        first._copyValues(out)
+        first._copy_cuml_params(out)
+        return out
+
+    def _models(self) -> List[Tuple[List[float], float]]:
+        if isinstance(self.intercept_, (list, tuple)):
+            return [(list(c), float(b)) for c, b in zip(self.coef_, self.intercept_)]
+        return [(list(self.coef_), float(self.intercept_))]
+
     def _get_cuml_transform_func(self, dataset: Any, eval_metric_info: Any = None
                                  ) -> Tuple[Callable, Callable, Optional[Callable]]:
+        if eval_metric_info is not None:
+            return self._eval_func(eval_metric_info)
+        if isinstance(self.intercept_, (list, tuple)):
+            raise NotImplementedError("transform() of a combined multi-model instance is not supported")
         coef_, intercept_ = self.coef_, float(self.intercept_)
         n_cols = int(self.n_cols)
 
@@ -405,6 +433,24 @@ class LinearRegressionModel(LinearRegressionClass, _CumlModelWithPredictionCol, 
         _transform_internal.many = _transform_many  # type: ignore[attr-defined]
         _transform_internal.row_bytes = 4 * n_cols + 8  # type: ignore[attr-defined]
         return _construct, _transform_internal, None
+
+    def _eval_func(self, info: Dict[str, Any]) -> Tuple[Callable, Any, Callable]:
+        """(construct, None, evaluate): evaluate(holder, X, y) scores every model on one device pass
+        (b2k_eval_linear, identity kind) and returns their accumulators."""
+        from .core import _class_accs
+
+        if info["classification"]:
+            raise NotImplementedError("LinearRegressionModel is evaluated with a RegressionEvaluator")
+        models = [{"kind": "identity", "W": np.asarray([c], dtype=np.float64), "b": [b]} for c, b in self._models()]
+
+        class _Holder:
+            def __init__(self, gpu: int) -> None:
+                self.ctx = _transform_context(gpu)
+
+        def _evaluate(h: Any, X: Any, y: Any) -> List[Dict[str, Any]]:
+            return _class_accs(h.ctx.eval_linear(X, y, models))
+
+        return _Holder, None, _evaluate
 
 
 from .tree import _RandomForestEstimator, _RandomForestModel  # noqa: E402  (tree.py imports this module lazily)

@@ -1,0 +1,137 @@
+"""Local stand-ins for pyspark.ml.evaluation's MulticlassClassificationEvaluator and RegressionEvaluator: Spark's params,
+defaults and isLargerBetter(); evaluate() of a local frame reads the label, prediction (and probability) columns and
+computes in fp64 on the host (spark_rapids_ml_b200.metrics)."""
+from __future__ import annotations
+
+from typing import Any, Dict, Optional
+
+import numpy as np
+
+from .params import Param, Params, TypeConverters, keyword_only
+
+
+class _Evaluator(Params):
+    labelCol = Param("parent", "labelCol", "label column name.", TypeConverters.toString)
+    predictionCol = Param("parent", "predictionCol", "prediction column name.", TypeConverters.toString)
+    weightCol = Param("parent", "weightCol", "weight column name.", TypeConverters.toString)
+    metricName = Param("parent", "metricName", "metric name in evaluation", TypeConverters.toString)
+
+    def _init(self, kwargs: Dict[str, Any]) -> None:
+        super().__init__()
+        self._setDefault(labelCol="label", predictionCol="prediction")
+        self._set(**{k: v for k, v in kwargs.items() if v is not None})
+
+    def getLabelCol(self) -> str:
+        return self.getOrDefault("labelCol")
+
+    def getPredictionCol(self) -> str:
+        return self.getOrDefault("predictionCol")
+
+    def getMetricName(self) -> str:
+        return self.getOrDefault("metricName")
+
+    def setMetricName(self, value: str) -> "_Evaluator":
+        return self._set(metricName=value)
+
+    def setLabelCol(self, value: str) -> "_Evaluator":
+        return self._set(labelCol=value)
+
+    def setPredictionCol(self, value: str) -> "_Evaluator":
+        return self._set(predictionCol=value)
+
+    def _column(self, dataset: Any, name: str) -> Any:
+        if self.isSet("weightCol") and self.getOrDefault("weightCol"):
+            raise NotImplementedError("weightCol is not supported by this evaluator")
+        return dataset.select(name).toPandas()[name]
+
+    def evaluate(self, dataset: Any, params: Optional[Dict[Param, Any]] = None) -> float:
+        return (self.copy(params) if params else self)._evaluate(dataset)
+
+    def _evaluate(self, dataset: Any) -> float:
+        raise NotImplementedError
+
+    def isLargerBetter(self) -> bool:
+        raise NotImplementedError
+
+
+class MulticlassClassificationEvaluator(_Evaluator):
+    """pyspark.ml.evaluation.MulticlassClassificationEvaluator: metricName (default "f1"), metricLabel (0.0), beta
+    (1.0), eps (1e-15, logLoss), probabilityCol ("probability")."""
+
+    metricLabel = Param("parent", "metricLabel", "The class whose metric will be computed in truePositiveRateByLabel|"
+                        "falsePositiveRateByLabel|precisionByLabel|recallByLabel|fMeasureByLabel.",
+                        TypeConverters.toFloat)
+    beta = Param("parent", "beta", "The beta value used in weightedFMeasure|fMeasureByLabel.", TypeConverters.toFloat)
+    eps = Param("parent", "eps", "log-loss is undefined for p=0, so the probability of the label is clipped "
+                "below at eps: -log(max(p, eps)).", TypeConverters.toFloat)
+    probabilityCol = Param("parent", "probabilityCol", "Column name for predicted class conditional probabilities.",
+                           TypeConverters.toString)
+
+    @keyword_only
+    def __init__(self, *, predictionCol: str = "prediction", labelCol: str = "label", metricName: str = "f1",
+                 weightCol: Optional[str] = None, metricLabel: float = 0.0, beta: float = 1.0,
+                 probabilityCol: str = "probability", eps: float = 1e-15) -> None:
+        self._init({})
+        self._setDefault(metricName="f1", metricLabel=0.0, beta=1.0, eps=1e-15, probabilityCol="probability")
+        self._set(**{k: v for k, v in self._input_kwargs.items() if v is not None})
+
+    def getMetricLabel(self) -> float:
+        return self.getOrDefault("metricLabel")
+
+    def getBeta(self) -> float:
+        return self.getOrDefault("beta")
+
+    def getEps(self) -> float:
+        return self.getOrDefault("eps")
+
+    def getProbabilityCol(self) -> str:
+        return self.getOrDefault("probabilityCol")
+
+    def isLargerBetter(self) -> bool:
+        return self.getMetricName() not in ("weightedFalsePositiveRate", "falsePositiveRateByLabel", "logLoss",
+                                            "hammingLoss")
+
+    def _evaluate(self, dataset: Any) -> float:
+        from .. import metrics
+
+        name = self.getMetricName()
+        if name not in metrics.MULTICLASS_METRICS:
+            raise ValueError(f"Unsupported metric name, found {name}")
+        y = np.asarray(self._column(dataset, self.getLabelCol()), dtype=np.float64)
+        p = np.asarray(self._column(dataset, self.getPredictionCol()), dtype=np.float64)
+        probs = None
+        if name == "logLoss":
+            col = list(self._column(dataset, self.getProbabilityCol()))
+            probs = np.asarray([np.asarray(v, dtype=np.float64) for v in col]) if col else np.zeros((0, 1))
+        acc = metrics.class_accumulators(y, p, probs, self.getEps())
+        return metrics.multiclass_metric(acc, name, self.getMetricLabel(), self.getBeta())
+
+
+class RegressionEvaluator(_Evaluator):
+    """pyspark.ml.evaluation.RegressionEvaluator: metricName (default "rmse"), throughOrigin (False)."""
+
+    throughOrigin = Param("parent", "throughOrigin", "whether the regression is through the origin.",
+                          TypeConverters.identity)
+
+    @keyword_only
+    def __init__(self, *, predictionCol: str = "prediction", labelCol: str = "label", metricName: str = "rmse",
+                 weightCol: Optional[str] = None, throughOrigin: bool = False) -> None:
+        self._init({})
+        self._setDefault(metricName="rmse", throughOrigin=False)
+        self._set(**{k: v for k, v in self._input_kwargs.items() if v is not None})
+
+    def getThroughOrigin(self) -> bool:
+        return bool(self.getOrDefault("throughOrigin"))
+
+    def isLargerBetter(self) -> bool:
+        return self.getMetricName() in ("r2", "var")
+
+    def _evaluate(self, dataset: Any) -> float:
+        from .. import metrics
+
+        name = self.getMetricName()
+        if name not in metrics.REGRESSION_METRICS:
+            raise ValueError(f"Unsupported metric name, found {name}")
+        y = np.asarray(self._column(dataset, self.getLabelCol()), dtype=np.float64)
+        p = np.asarray(self._column(dataset, self.getPredictionCol()), dtype=np.float64)
+        return metrics.regression_metric(metrics.reg_accumulators(y, p), name, self.getThroughOrigin())

@@ -340,6 +340,11 @@ class _RandomForestEstimator(_RandomForestClass, _CumlEstimator, _RandomForestCu
     def _enable_fit_multiple_in_single_pass(self) -> bool:
         return True
 
+    def _supportsTransformEvaluate(self, evaluator: Any) -> bool:
+        from .core import _supports_transform_evaluate
+
+        return _supports_transform_evaluate(self._is_classification(), evaluator)
+
     def _model_class(self) -> Any:
         raise NotImplementedError
 
@@ -545,6 +550,8 @@ class _RandomForestModel(_RandomForestClass, _CumlModelWithPredictionCol, _Rando
 
     def _get_cuml_transform_func(self, dataset: Any, eval_metric_info: Any = None
                                  ) -> Tuple[Callable, Callable, Optional[Callable]]:
+        if eval_metric_info is not None:
+            return self._eval_func(eval_metric_info)
         forest = self._flat()
         n_cols = int(self.n_cols)
         classification = self._is_classification()
@@ -589,6 +596,29 @@ class _RandomForestModel(_RandomForestClass, _CumlModelWithPredictionCol, _Rando
         _transform_internal.many = _transform_many  # type: ignore[attr-defined]
         _transform_internal.row_bytes = 4 * n_cols + 8 * (2 * V + 1)  # type: ignore[attr-defined]
         return _construct, _transform_internal, None
+
+    def _eval_func(self, info: Dict[str, Any]) -> Tuple[Callable, Any, Callable]:
+        """(construct, None, evaluate): evaluate(holder, X, y) scores every forest of this (combined) model in one
+        device pass (b2k_eval_forest) and returns their accumulators."""
+        from .core import _class_accs
+
+        classification = self._is_classification()
+        if info["classification"] != classification:
+            raise NotImplementedError(f"{type(self).__name__} is evaluated with a "
+                                      f"{'MulticlassClassification' if classification else 'Regression'}Evaluator")
+        V = self._num_classes if classification else 1
+        jsons = self._model_json if isinstance(self._model_json, list) else [self._model_json]
+        forests = [json_to_forest(j, V) for j in jsons]
+        eps = info["eps"]
+
+        class _Holder:
+            def __init__(self, gpu: int) -> None:
+                self.ctx = _transform_context(gpu)
+
+        def _evaluate(h: Any, X: Any, y: Any) -> List[Dict[str, Any]]:
+            return _class_accs(h.ctx.eval_forest(X, y, forests, classification, eps))
+
+        return _Holder, None, _evaluate
 
     def _transform(self, dataset: Any) -> Any:
         """Appends rawPredictionCol and probabilityCol (list<double>, classification) and predictionCol (double) to a
