@@ -37,6 +37,8 @@
  *   b2k_rf_fit / b2k_rf_forest  tree.py:343-527 (the per-worker cuML RandomForest fits and the treelite models they
  *                               return), classification.py:285-676, regression.py:865-1147
  *   b2k_rf_predict              tree.py:670- (the model's transform: cuML's forest inference over treelite)
+ *   b2k_umap_fit / _graph       umap.py:1009-1065 (UMAP's fit function: cuML UMAP(...).fit on one partition)
+ *   b2k_umap_transform          umap.py:1449-1551 (UMAPModel's transform: cuML UMAP.transform)
  *
  * Conventions
  *   - Plain C, no exceptions across the boundary: every call returns a b2k_status; the message for the
@@ -565,6 +567,69 @@ int b2k_eval_forest(b2k_ctx* ctx, const float* X, const float* y, int64_t n, int
                     const int32_t* feature, const float* threshold, const int32_t* children, const double* value,
                     int n_classes, double eps, int64_t* label_count_out, int64_t* tp_out, int64_t* fp_out,
                     double* loss_out, double* reg_out, uintptr_t stream);
+
+/* ---- UMAP (euclidean) ----
+ * b2k_umap_fit stands in for umap.py:1009-1065 (the fit function: cuML UMAP(...).fit on the rows coalesced to one
+ * partition), b2k_umap_transform for umap.py:1449-1551 (UMAPModel's transform: cuML UMAP.transform against the model's
+ * raw data and embedding).  Both run on one GPU and make no collective call.
+ * Semantics (McInnes, Healy & Melville 2018; tests/umap_oracle.py restates each step in fp64 NumPy):
+ *   kNN        exact Euclidean k-NN of the rows against themselves, k = n_neighbors (1 <= k <= n), ties to the lower row;
+ *              the row itself is recognised by its index.
+ *   membership per row, fp64: rho = the local_connectivity-th non-zero distance (interpolated for a fraction; the
+ *              largest when fewer); sigma by 64 bisection steps on sum_{j != self} exp(-max(0, d_j - rho) / sigma)
+ *              = log2(k), tolerance 1e-5, floored at 1e-3 times the row's mean distance (rho > 0) or the mean of all
+ *              distances (rho == 0); w_ij = exp(-max(0, d_ij - rho_i) / sigma_i), 1 at or below rho, 0 for the self edge.
+ *   graph      W = mix (P + P^T - P o P^T) + (1 - mix) P o P^T, mix = set_op_mix_ratio: CSR, columns ascending, no zeros.
+ *   labels     (optional int32 [n], -1 unknown) w_ij *= exp(-1) if either label is unknown, exp(-5) if they differ; each
+ *              row divided by its largest weight; then W = W + W^T - W o W^T.
+ *   schedule   edges with w < max(w) / n_epochs never fire; epochs_per_sample = max(w) / w, per negative sample that
+ *              over negative_sample_rate, state in fp64.
+ *   init       0: uniform [-10, 10] from umap_hash; 1: the n_components leading non-trivial eigenvectors of
+ *              D^-1/2 W D^-1/2 (block subspace iteration, SpMM on the device, fp64 Rayleigh-Ritz on the host), scaled
+ *              to max |.| = 10 plus N(0, 1e-4) noise, or 0 when the graph has more than one connected component; both
+ *              then rescaled per column to [0, 10].  2: embedding_out holds the start on entry, used as it is.
+ *   layout     epochs e = 0 .. n_epochs - 1, alpha = learning_rate (1 - e / n_epochs); an edge is due when its next
+ *              epoch <= e.  Due edge (i, j): attraction -2ab d2^(b-1) / (a d2^b + 1) (y_i - y_j) per component clipped to
+ *              +-4, on i and (negated) on j; then floor((e - next_neg) / epn) negatives k = umap_hash(seed, e, edge, q)
+ *              mod n, each (k != i) repelling i by 2 gamma b / ((0.001 + d2)(a d2^b + 1)) (y_i - y_k) clipped to +-4,
+ *              or 4 per component when d2 = 0.  Every update reads the positions of the start of the epoch; a vertex
+ *              moves by alpha times the fixed-order sum of its contributions.  Positions are fp32.
+ * params: n_epochs >= 1 (resolved by the caller); option "stop_after_epochs" = E > 0 stops the layout after E epochs.
+ * info_out (may be NULL) [8]: n, k, nnz of W, epochs run, init used (0 random, 1 spectral, 2 given), Ritz residual
+ * max ||M x - theta x|| of the spectral init, n_components, max(w).  Stats: last_finalize_ms = kNN, last_reduce_ms =
+ * graph and schedule, last_allreduce_ms = init, last_fused_ms = layout (device times); last_path 2 for the
+ * lane-parallel-edge layout (n_components <= 4), 1 otherwise.  Errors (B2K_ERR_INVALID): n < 2, a non-finite value in
+ * X ("UMAP input contains NaN or infinity"), a parameter out of range. */
+typedef struct b2k_umap_params {
+  int32_t n_neighbors;
+  int32_t n_components;         /* 1 .. 100 */
+  int32_t n_epochs;
+  int32_t init;                 /* 0 random, 1 spectral, 2 given (fit only) */
+  int32_t negative_sample_rate;
+  int32_t reserved;
+  double local_connectivity;
+  double set_op_mix_ratio;
+  double learning_rate;
+  double repulsion_strength;
+  double a, b;
+  uint64_t seed;
+} b2k_umap_params;
+int b2k_umap_fit(b2k_ctx* ctx, const float* X, int64_t n, int d, const int32_t* labels, const b2k_umap_params* params,
+                 float* embedding_out, double* info_out, uintptr_t stream);
+/* The last fit's intermediates, host arrays, any may be NULL: knn_idx [n][k], knn_dist [n][k], rho [n], sigma [n],
+ * indptr [n + 1], indices [nnz], weights [nnz], epochs_per_sample [nnz] (+inf: never fires), init [n][C] (the start of
+ * the layout), ritz_values [C] and ritz_vectors [n][C] (spectral init only). */
+int b2k_umap_graph(b2k_ctx* ctx, int64_t* knn_idx, float* knn_dist, double* rho, double* sigma, int64_t* indptr,
+                   int32_t* indices, double* weights, double* epochs_per_sample, float* init, double* ritz_values,
+                   double* ritz_vectors);
+/* Each query row: its k exact neighbours among X_train [n_train][d]; memberships as above with no self edge and the
+ * sigma floor from the row's own mean; the edges with w < max_row(w) / n_epochs never fire, epochs_per_sample =
+ * max_row(w) / w; start = the w-weighted mean of the neighbours' embedding rows (fp64); then n_epochs epochs (0 allowed)
+ * moving the query only, negatives k = umap_hash(seed, e, idx_0 n_train + idx_j, q) mod n_train (idx_0 the nearest
+ * neighbour, idx_j the edge's), all in one kernel.  A row's result depends on that row alone.  A query with a non-finite
+ * component gets a NaN row. */
+int b2k_umap_transform(b2k_ctx* ctx, const float* X_train, const float* embedding, int64_t n_train, int d, const float* Q,
+                       int64_t nq, const b2k_umap_params* params, float* out, uintptr_t stream);
 
 #ifdef __cplusplus
 }

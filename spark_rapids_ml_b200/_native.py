@@ -69,6 +69,9 @@ EXPORTED_SYMBOLS = (
     "b2k_rf_predict",
     "b2k_eval_linear",
     "b2k_eval_forest",
+    "b2k_umap_fit",
+    "b2k_umap_graph",
+    "b2k_umap_transform",
 )
 
 EVAL_KINDS = {"identity": 0, "logistic": 1, "softmax": 2}
@@ -112,6 +115,38 @@ class RfParams(ctypes.Structure):
         ("min_info_gain", ctypes.c_double),
         ("seed", ctypes.c_uint64),
     ]
+
+
+class UmapParams(ctypes.Structure):
+    _fields_ = [
+        ("n_neighbors", ctypes.c_int32),
+        ("n_components", ctypes.c_int32),
+        ("n_epochs", ctypes.c_int32),
+        ("init", ctypes.c_int32),
+        ("negative_sample_rate", ctypes.c_int32),
+        ("reserved", ctypes.c_int32),
+        ("local_connectivity", ctypes.c_double),
+        ("set_op_mix_ratio", ctypes.c_double),
+        ("learning_rate", ctypes.c_double),
+        ("repulsion_strength", ctypes.c_double),
+        ("a", ctypes.c_double),
+        ("b", ctypes.c_double),
+        ("seed", ctypes.c_uint64),
+    ]
+
+
+UMAP_INIT_CODES = {"random": 0, "spectral": 1, "given": 2}
+
+
+def umap_params(n_neighbors: int = 15, n_components: int = 2, n_epochs: int = 200, init: str = "spectral",
+                negative_sample_rate: int = 5, local_connectivity: float = 1.0, set_op_mix_ratio: float = 1.0,
+                learning_rate: float = 1.0, repulsion_strength: float = 1.0, a: float = 1.577, b: float = 0.895,
+                seed: int = 0) -> UmapParams:
+    """b2k_umap_params from keyword values (n_epochs resolved by the caller)."""
+    return UmapParams(int(n_neighbors), int(n_components), int(n_epochs), UMAP_INIT_CODES[init],
+                      int(negative_sample_rate), 0, float(local_connectivity), float(set_op_mix_ratio),
+                      float(learning_rate), float(repulsion_strength), float(a), float(b),
+                      int(seed) & 0xFFFFFFFFFFFFFFFF)
 
 
 class Stats(ctypes.Structure):
@@ -204,6 +239,9 @@ def load_library() -> ctypes.CDLL:
                                   ctypes.c_size_t]
     L.b2k_eval_forest.argtypes = [vp, vp, vp, i64, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, i32, f64, vp, vp, vp, vp,
                                   vp, ctypes.c_size_t]
+    L.b2k_umap_fit.argtypes = [vp, vp, i64, i32, vp, ctypes.POINTER(UmapParams), vp, vp, ctypes.c_size_t]
+    L.b2k_umap_graph.argtypes = [vp] + [vp] * 11
+    L.b2k_umap_transform.argtypes = [vp, vp, vp, i64, i32, vp, i64, ctypes.POINTER(UmapParams), vp, ctypes.c_size_t]
     for name in EXPORTED_SYMBOLS:
         if name not in ("b2k_last_error",):
             getattr(L, name).restype = i32
@@ -828,3 +866,57 @@ class Context:
             return [out["label_count"].ctypes.data, out["tp"].ctypes.data, out["fp"].ctypes.data,
                     out["loss"].ctypes.data, None]
         return [None, None, None, None, out["reg"].ctypes.data]
+
+    # -- UMAP -------------------------------------------------------------------------------
+    def umap_fit(self, X: Any, params: UmapParams, labels: Any = None, init: Any = None) -> Tuple[Any, Dict[str, Any]]:
+        """b2k_umap_fit on one GPU: X [n, d] float32 CUDA tensor, labels an int32 CUDA tensor [n] (-1 unknown) or None,
+        init a float32 [n, C] start (params.init must then be 2).  Returns (embedding float32 CUDA tensor [n, C],
+        info dict: n, k, nnz, epochs, init_used, ritz_residual, max_weight)."""
+        t = self._torch
+        n, d = self._check_X(X)
+        C = int(params.n_components)
+        emb = t.empty((n, max(C, 1)), dtype=t.float32, device=self.device)
+        if init is not None:
+            emb.copy_(t.as_tensor(init, dtype=t.float32, device=self.device).reshape(n, C))
+        if labels is not None and not (labels.is_cuda and labels.dtype == t.int32 and labels.is_contiguous()
+                                       and tuple(labels.shape) == (n,)):
+            raise ValueError(f"labels must be a contiguous int32 CUDA tensor [{n}]")
+        info = np.zeros(8, dtype=np.float64)
+        with t.cuda.device(self.device):
+            self._check(self._L.b2k_umap_fit(self._h, X.data_ptr(), n, d,
+                                             labels.data_ptr() if labels is not None else None, ctypes.byref(params),
+                                             emb.data_ptr(), info.ctypes.data, self._stream()))
+        keys = ("n", "k", "nnz", "epochs", "init_used", "ritz_residual", "n_components", "max_weight")
+        out = {key: (float(v) if key in ("ritz_residual", "max_weight") else int(v)) for key, v in zip(keys, info)}
+        return emb, out
+
+    def umap_graph(self, info: Dict[str, Any]) -> Dict[str, np.ndarray]:
+        """The intermediates of the last umap_fit (b2k_umap_graph) as host arrays, sized from its info dict."""
+        n, k, nnz, C = info["n"], info["k"], info["nnz"], info["n_components"]
+        g = {"knn_idx": np.zeros((n, k), np.int64), "knn_dist": np.zeros((n, k), np.float32),
+             "rho": np.zeros(n), "sigma": np.zeros(n), "indptr": np.zeros(n + 1, np.int64),
+             "indices": np.zeros(nnz, np.int32), "weights": np.zeros(nnz), "epochs_per_sample": np.zeros(nnz),
+             "init": np.zeros((n, C), np.float32), "ritz_values": np.zeros(C), "ritz_vectors": np.zeros((n, C))}
+        self._check(self._L.b2k_umap_graph(self._h, *[g[key].ctypes.data for key in
+                                                      ("knn_idx", "knn_dist", "rho", "sigma", "indptr", "indices",
+                                                       "weights", "epochs_per_sample", "init", "ritz_values",
+                                                       "ritz_vectors")]))
+        return g
+
+    def umap_transform(self, X_train: Any, embedding: Any, Q: Any, params: UmapParams) -> Any:
+        """b2k_umap_transform: Q [nq, d] against the model (X_train [n, d], embedding [n, C], float32 CUDA tensors) ->
+        float32 CUDA tensor [nq, C]; params.n_epochs is the transform's epoch count."""
+        t = self._torch
+        n, d = self._check_X(X_train)
+        nq, dq = self._check_X(Q)
+        C = int(params.n_components)
+        if dq != d:
+            raise ValueError(f"queries have {dq} features, the model {d}")
+        if tuple(embedding.shape) != (n, C) or not embedding.is_contiguous() or embedding.dtype != t.float32:
+            raise ValueError(f"embedding must be a contiguous float32 CUDA tensor [{n}, {C}]")
+        out = t.empty((nq, C), dtype=t.float32, device=self.device)
+        with t.cuda.device(self.device):
+            self._check(self._L.b2k_umap_transform(self._h, X_train.data_ptr(), embedding.data_ptr(), n, d,
+                                                   Q.data_ptr(), nq, ctypes.byref(params), out.data_ptr(),
+                                                   self._stream()))
+        return out

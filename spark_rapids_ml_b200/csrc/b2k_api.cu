@@ -115,6 +115,9 @@ extern "C" int b2k_ctx_set_option(b2k_ctx* ctx, const char* key, int64_t value) 
   } else if (k == "grid_limit") {
     if (value < 0) return b2k_fail(ctx, B2K_ERR_INVALID, "grid_limit must be >= 0");
     ctx->grid_limit = (int)value;
+  } else if (k == "stop_after_epochs") {
+    if (value < 0 || value > (1 << 30)) return b2k_fail(ctx, B2K_ERR_INVALID, "stop_after_epochs must be in [0, 2^30]");
+    ctx->umap_stop_epochs = (int)value;
   } else if (k == "rf_group_nodes" || k == "rf_flush_tiles") {
     if (value < 0 || value > (1 << 30)) return b2k_fail(ctx, B2K_ERR_INVALID, k + " must be in [0, 2^30]");
     (k == "rf_group_nodes" ? ctx->rf_group_nodes : ctx->rf_flush_tiles) = (int)value;
@@ -1164,4 +1167,36 @@ extern "C" int b2k_eval_forest(b2k_ctx* ctx, const float* X, const float* y, int
   return b2k_eval_forest_impl(ctx, X, y, n, d, n_models, classification, n_trees, n_values, tree_offsets, feature,
                               threshold, children, value, n_classes, eps, label_count_out, tp_out, fp_out, loss_out,
                               reg_out, reinterpret_cast<cudaStream_t>(stream));
+}
+
+// ------------------------------------------------------------------------------------------------
+// UMAP (b2k_umap.cu)
+// ------------------------------------------------------------------------------------------------
+extern "C" int b2k_umap_fit(b2k_ctx* ctx, const float* X, int64_t n, int d, const int32_t* labels,
+                            const b2k_umap_params* params, float* embedding_out, double* info_out, uintptr_t stream) {
+  if (!ctx) return b2k_fail(nullptr, B2K_ERR_INVALID, "b2k_umap_fit: ctx is NULL");
+  if (!params || !embedding_out || n < 0 || d < 1 || (n > 0 && !X))
+    return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_umap_fit: bad X/params/embedding_out/n/d");
+  B2K_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  return b2k_umap_fit_impl(ctx, X, n, d, labels, *params, embedding_out, info_out,
+                           reinterpret_cast<cudaStream_t>(stream));
+}
+
+extern "C" int b2k_umap_graph(b2k_ctx* ctx, int64_t* knn_idx, float* knn_dist, double* rho, double* sigma,
+                              int64_t* indptr, int32_t* indices, double* weights, double* epochs_per_sample,
+                              float* init, double* ritz_values, double* ritz_vectors) {
+  if (!ctx) return b2k_fail(nullptr, B2K_ERR_INVALID, "b2k_umap_graph: ctx is NULL");
+  return b2k_umap_graph_impl(ctx, knn_idx, knn_dist, rho, sigma, indptr, indices, weights, epochs_per_sample, init,
+                             ritz_values, ritz_vectors);
+}
+
+extern "C" int b2k_umap_transform(b2k_ctx* ctx, const float* X_train, const float* embedding, int64_t n_train, int d,
+                                  const float* Q, int64_t nq, const b2k_umap_params* params, float* out,
+                                  uintptr_t stream) {
+  if (!ctx) return b2k_fail(nullptr, B2K_ERR_INVALID, "b2k_umap_transform: ctx is NULL");
+  if (!params || !X_train || !embedding || n_train < 0 || nq < 0 || d < 1 || (nq > 0 && (!Q || !out)))
+    return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_umap_transform: bad X_train/embedding/Q/out/params/sizes");
+  B2K_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  return b2k_umap_transform_impl(ctx, X_train, embedding, n_train, d, Q, nq, *params, out,
+                                 reinterpret_cast<cudaStream_t>(stream));
 }

@@ -84,6 +84,9 @@ struct b2k_ctx {
   std::shared_ptr<void> rf_forest;
   int rf_group_nodes = 0;   // option "rf_group_nodes": cap on the nodes of one histogram pass (0 = capacity)
   int rf_flush_tiles = 0;   // option "rf_flush_tiles": tiles per CTA between flushes of the cluster pass (0 = the bound)
+  // UMAP (b2k_umap.cu): the graph of the last b2k_umap_fit, read by b2k_umap_graph; option "stop_after_epochs" (tests)
+  std::shared_ptr<void> umap_graph;
+  int umap_stop_epochs = 0;
   b2k_stats stats{};
 };
 
@@ -289,6 +292,21 @@ constexpr int B2K_KNN_MAX_K = 1024;   // the generic path's per-query lists; the
 int b2k_knn_search_impl(b2k_ctx* ctx, const float* items, int64_t n_items, const int64_t* item_ids,
                         const float* queries, int64_t nq_local, int d, int k, float* dist_out, int64_t* idx_out,
                         cudaStream_t s);
+// The same search on one rank with no collective (UMAP's graph and transform): the k nearest of items [n_items, d] for
+// each of queries [nq, d] -> sqrt(distance) ascending, ties to the lower row, and the item row.  1 <= k <= n_items.
+int b2k_knn_local_impl(b2k_ctx* ctx, const float* items, int64_t n_items, const float* queries, int64_t nq, int d,
+                       int k, float* dist_out, int64_t* idx_out, cudaStream_t s);
+
+// ------------------------------------------------------------------------------------------------
+// UMAP — b2k_umap.cu (the C ABI entry points in b2k_api.cu check their arguments, then call these)
+// ------------------------------------------------------------------------------------------------
+int b2k_umap_fit_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, const int32_t* labels,
+                      const b2k_umap_params& p, float* embedding_out, double* info_out, cudaStream_t s);
+int b2k_umap_transform_impl(b2k_ctx* ctx, const float* X_train, const float* Y_train, int64_t n_train, int d,
+                            const float* Q, int64_t nq, const b2k_umap_params& p, float* out, cudaStream_t s);
+int b2k_umap_graph_impl(b2k_ctx* ctx, int64_t* knn_idx, float* knn_dist, double* rho, double* sigma, int64_t* indptr,
+                        int32_t* indices, double* weights, double* eps, float* init, double* ritz_values,
+                        double* ritz_vectors);
 
 // ------------------------------------------------------------------------------------------------
 // DBSCAN — b2k_dbscan.cu (the C ABI entry point in b2k_api.cu checks its arguments, then calls this)

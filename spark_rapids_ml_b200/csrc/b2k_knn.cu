@@ -479,6 +479,111 @@ int launch_wg(b2k_ctx* ctx, int grid, const CUtensorMap& mq, const CUtensorMap& 
   B2K_CUDA_OK(ctx, cudaGetLastError());
   return B2K_OK;
 }
+// The local search: plan, prep, search and refine of queries Q [nq][d] against this rank's items, with no collective.
+struct KnnLocal {
+  bool wg = false;
+  int DP = 0, S = 0;
+  int64_t nblk = 0, n_pad = 0, ntiles = 0;
+  float *Qs = nullptr, *Xhi = nullptr, *Xlo = nullptr, *norms = nullptr;
+  int2* part = nullptr;
+};
+
+int knn_local_plan(b2k_ctx* ctx, int64_t n_items, int64_t nq, int d, int k, bool q_aligned, KnnLocal* p) {
+  const bool wg_ok = d % 4 == 0 && d >= 4 && d <= 128 && k <= KW_KMAX && q_aligned;
+  if (ctx->kernel_path == B2K_PATH_FUSED && !wg_ok)
+    return b2k_fail(ctx, B2K_ERR_UNSUPPORTED, "kernel_path=2 requested but the wgmma kNN pass needs d % 4 == 0, "
+                                              "4 <= d <= 128, k <= 64 and 16-byte aligned queries (d = " +
+                                                  std::to_string(d) + ", k = " + std::to_string(k) + ")");
+  p->wg = wg_ok && ctx->kernel_path != B2K_PATH_GENERIC;
+  int sm = ctx->sm_count;
+  if (ctx->grid_limit > 0 && ctx->grid_limit < sm) sm = ctx->grid_limit;
+  p->DP = d <= 32 ? 32 : d <= 64 ? 64 : 128;
+  p->nblk = (n_items + KW_N - 1) / KW_N;
+  p->n_pad = p->nblk * KW_N;
+  const int64_t qt = p->wg ? KW_TM : GQ;
+  p->ntiles = (nq + qt - 1) / qt;
+  const int64_t item_tiles = p->wg ? p->nblk : (n_items + GN - 1) / GN;
+  // splits of the index: at least about 2 units per SM, at most one tile of the index per split
+  p->S = n_items == 0 ? 0
+                      : (int)std::max<int64_t>(1, std::min<int64_t>({(2 * sm + p->ntiles - 1) / p->ntiles, item_tiles,
+                                                                     (int64_t)KW_SMAX}));
+  return B2K_OK;
+}
+
+void knn_local_take(B2kLayout& L, KnnLocal* p, int64_t n_items, int64_t nq, int d, int k) {
+  if (p->wg && n_items > 0) {
+    p->Qs = L.take<float>((size_t)nq * d, 1024);
+    p->Xhi = L.take<float>((size_t)p->n_pad * p->DP, 1024);
+    p->Xlo = L.take<float>((size_t)p->n_pad * p->DP, 1024);
+    p->norms = L.take<float>((size_t)p->n_pad);
+  }
+  p->part = L.take<int2>((size_t)std::max(p->S, 1) * nq * k);
+}
+
+// marks 2 (after prep), 3 (after search) and 4 (after refine) of tm
+int knn_local_run(b2k_ctx* ctx, const KnnLocal& p, const float* items, int64_t n_items, const int64_t* item_ids,
+                  const float* Q, int64_t nq, int d, int k, int64_t row0, KnnCand* cand, Timer& tm, cudaStream_t s) {
+  // ---- search of the local index for every query ----
+  if (n_items > 0) {
+    if (p.wg) {
+      k_knn_prep<<<(unsigned)((p.n_pad * 32 + 255) / 256), 256, 0, s>>>(items, n_items, d, p.n_pad, p.DP, p.Xhi, p.Xlo,
+                                                                        p.norms);
+      B2K_CUDA_OK(ctx, cudaGetLastError());
+      const int64_t n4 = nq * d / 4;
+      k_knn_shift_q<<<(unsigned)std::min<int64_t>((n4 + 255) / 256, (int64_t)ctx->sm_count * 16), 256, 0, s>>>(
+          reinterpret_cast<const float4*>(Q), n4, d, items, reinterpret_cast<float4*>(p.Qs));
+      B2K_CUDA_OK(ctx, cudaGetLastError());
+      ctx->stats.kernel_launches += 2;
+    }
+    tm.mark(2, s);
+    if (p.wg) {
+      CUtensorMap mq, mh, ml;
+      B2K_TRY(b2k_encode_2d(ctx, &mq, p.Qs, (uint64_t)d, (uint64_t)nq, (uint64_t)d * 4, KW_CHUNK, KW_TM,
+                            CU_TENSOR_MAP_L2_PROMOTION_L2_256B));
+      B2K_TRY(b2k_encode_2d(ctx, &mh, p.Xhi, (uint64_t)p.DP, (uint64_t)p.n_pad, (uint64_t)p.DP * 4, KW_CHUNK, KW_N,
+                            CU_TENSOR_MAP_L2_PROMOTION_L2_256B));
+      B2K_TRY(b2k_encode_2d(ctx, &ml, p.Xlo, (uint64_t)p.DP, (uint64_t)p.n_pad, (uint64_t)p.DP * 4, KW_CHUNK, KW_N,
+                            CU_TENSOR_MAP_L2_PROMOTION_L2_256B));
+      KnnArgs a{};
+      a.nq = nq;
+      a.ntiles = (int)p.ntiles;
+      a.S = p.S;
+      a.nblk = (int)p.nblk;
+      a.k = k;
+      a.n_items = n_items;
+      a.norms = p.norms;
+      a.part = p.part;
+      int sm = ctx->sm_count;
+      if (ctx->grid_limit > 0 && ctx->grid_limit < sm) sm = ctx->grid_limit;
+      const int grid = (int)std::min<int64_t>(sm, p.ntiles * p.S);
+      if (p.DP == 32) B2K_TRY(launch_wg<1>(ctx, grid, mq, mh, ml, a, s));
+      else if (p.DP == 64) B2K_TRY(launch_wg<2>(ctx, grid, mq, mh, ml, a, s));
+      else B2K_TRY(launch_wg<4>(ctx, grid, mq, mh, ml, a, s));
+      ctx->stats.fused_tc_launches++;
+    } else {
+      const size_t smem = (size_t)GQ * k * sizeof(int2);
+      B2K_CUDA_OK(ctx, cudaFuncSetAttribute(k_knn_generic, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+      k_knn_generic<<<(unsigned)(p.ntiles * p.S), G_NTHREADS, smem, s>>>(Q, nq, items, n_items, d, k, p.S, p.part);
+      B2K_CUDA_OK(ctx, cudaGetLastError());
+      ctx->stats.generic_launches++;
+    }
+    ctx->stats.kernel_launches++;
+  } else {
+    tm.mark(2, s);
+  }
+  ctx->stats.last_path = p.wg ? B2K_PATH_FUSED : B2K_PATH_GENERIC;
+  tm.mark(3, s);
+
+  // ---- refine ----
+  const size_t rf_smem = (size_t)RF_WARPS * 2 * k * 4;
+  B2K_CUDA_OK(ctx, cudaFuncSetAttribute(k_knn_refine, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rf_smem));
+  k_knn_refine<<<(unsigned)((nq + RF_WARPS - 1) / RF_WARPS), RF_WARPS * 32, rf_smem, s>>>(
+      p.part, p.S, nq, k, Q, items, n_items, d, row0, item_ids, cand);
+  B2K_CUDA_OK(ctx, cudaGetLastError());
+  ctx->stats.kernel_launches++;
+  tm.mark(4, s);
+  return B2K_OK;
+}
 }  // namespace
 
 int b2k_knn_search_impl(b2k_ctx* ctx, const float* items, int64_t n_items, const int64_t* item_ids,
@@ -524,37 +629,14 @@ int b2k_knn_search_impl(b2k_ctx* ctx, const float* items, int64_t n_items, const
   // ---- plan ----
   const int64_t nq_all = nr > 1 ? nq_max * nr : nq_local;
   const bool q_aligned = nr > 1 || (reinterpret_cast<uintptr_t>(queries) & 15u) == 0;
-  const bool wg_ok = d % 4 == 0 && d >= 4 && d <= 128 && k <= KW_KMAX && q_aligned;
-  if (ctx->kernel_path == B2K_PATH_FUSED && !wg_ok)
-    return b2k_fail(ctx, B2K_ERR_UNSUPPORTED, "kernel_path=2 requested but the wgmma kNN pass needs d % 4 == 0, "
-                                              "4 <= d <= 128, k <= 64 and 16-byte aligned queries (d = " +
-                                                  std::to_string(d) + ", k = " + std::to_string(k) + ")");
-  const bool wg = wg_ok && ctx->kernel_path != B2K_PATH_GENERIC;
-  int sm = ctx->sm_count;
-  if (ctx->grid_limit > 0 && ctx->grid_limit < sm) sm = ctx->grid_limit;
-  const int DP = d <= 32 ? 32 : d <= 64 ? 64 : 128;
-  const int64_t nblk = (n_items + KW_N - 1) / KW_N;
-  const int64_t n_pad = nblk * KW_N;
-  const int64_t qt = wg ? KW_TM : GQ;
-  const int64_t ntiles = (nq_all + qt - 1) / qt;
-  const int64_t item_tiles = wg ? nblk : (n_items + GN - 1) / GN;
-  // splits of the index: at least about 2 units per SM, at most one tile of the index per split
-  const int S = n_items == 0 ? 0
-                             : (int)std::max<int64_t>(1, std::min<int64_t>({(2 * sm + ntiles - 1) / ntiles, item_tiles,
-                                                                             (int64_t)KW_SMAX}));
-  float *Qall = nullptr, *Qs = nullptr, *Xhi = nullptr, *Xlo = nullptr, *norms = nullptr;
-  int2* part = nullptr;
+  KnnLocal lp;
+  B2K_TRY(knn_local_plan(ctx, n_items, nq_all, d, k, q_aligned, &lp));
+  float* Qall = nullptr;
   KnnCand *cand = nullptr, *cand_all = nullptr;
   B2K_TRY(b2k_scratch_layout(ctx, "kNN", [&](B2kLayout& L) -> int {
     sz_dev = L.take<int64_t>((size_t)3 * (nr + 1));
     if (nr > 1) Qall = L.take<float>((size_t)nq_all * d, 1024);
-    if (wg && n_items > 0) {
-      Qs = L.take<float>((size_t)nq_all * d, 1024);
-      Xhi = L.take<float>((size_t)n_pad * DP, 1024);
-      Xlo = L.take<float>((size_t)n_pad * DP, 1024);
-      norms = L.take<float>((size_t)n_pad);
-    }
-    part = L.take<int2>((size_t)std::max(S, 1) * nq_all * k);
+    knn_local_take(L, &lp, n_items, nq_all, d, k);
     cand = L.take<KnnCand>((size_t)nq_all * k);
     if (nr > 1) cand_all = L.take<KnnCand>((size_t)nr * nq_all * k);
     return B2K_OK;
@@ -571,63 +653,9 @@ int b2k_knn_search_impl(b2k_ctx* ctx, const float* items, int64_t n_items, const
     Q = Qall;
   }
   tm.mark(1, s);
+  B2K_TRY(knn_local_run(ctx, lp, items, n_items, item_ids, Q, nq_all, d, k, row0, cand, tm, s));
 
-  // ---- search of the local index for every query ----
-  if (n_items > 0) {
-    if (wg) {
-      k_knn_prep<<<(unsigned)((n_pad * 32 + 255) / 256), 256, 0, s>>>(items, n_items, d, n_pad, DP, Xhi, Xlo, norms);
-      B2K_CUDA_OK(ctx, cudaGetLastError());
-      const int64_t n4 = nq_all * d / 4;
-      k_knn_shift_q<<<(unsigned)std::min<int64_t>((n4 + 255) / 256, (int64_t)ctx->sm_count * 16), 256, 0, s>>>(
-          reinterpret_cast<const float4*>(Q), n4, d, items, reinterpret_cast<float4*>(Qs));
-      B2K_CUDA_OK(ctx, cudaGetLastError());
-      ctx->stats.kernel_launches += 2;
-    }
-    tm.mark(2, s);
-    if (wg) {
-      CUtensorMap mq, mh, ml;
-      B2K_TRY(b2k_encode_2d(ctx, &mq, Qs, (uint64_t)d, (uint64_t)nq_all, (uint64_t)d * 4, KW_CHUNK, KW_TM,
-                            CU_TENSOR_MAP_L2_PROMOTION_L2_256B));
-      B2K_TRY(b2k_encode_2d(ctx, &mh, Xhi, (uint64_t)DP, (uint64_t)n_pad, (uint64_t)DP * 4, KW_CHUNK, KW_N,
-                            CU_TENSOR_MAP_L2_PROMOTION_L2_256B));
-      B2K_TRY(b2k_encode_2d(ctx, &ml, Xlo, (uint64_t)DP, (uint64_t)n_pad, (uint64_t)DP * 4, KW_CHUNK, KW_N,
-                            CU_TENSOR_MAP_L2_PROMOTION_L2_256B));
-      KnnArgs a{};
-      a.nq = nq_all;
-      a.ntiles = (int)ntiles;
-      a.S = S;
-      a.nblk = (int)nblk;
-      a.k = k;
-      a.n_items = n_items;
-      a.norms = norms;
-      a.part = part;
-      const int grid = (int)std::min<int64_t>(sm, ntiles * S);
-      if (DP == 32) B2K_TRY(launch_wg<1>(ctx, grid, mq, mh, ml, a, s));
-      else if (DP == 64) B2K_TRY(launch_wg<2>(ctx, grid, mq, mh, ml, a, s));
-      else B2K_TRY(launch_wg<4>(ctx, grid, mq, mh, ml, a, s));
-      ctx->stats.fused_tc_launches++;
-    } else {
-      const size_t smem = (size_t)GQ * k * sizeof(int2);
-      B2K_CUDA_OK(ctx, cudaFuncSetAttribute(k_knn_generic, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-      k_knn_generic<<<(unsigned)(ntiles * S), G_NTHREADS, smem, s>>>(Q, nq_all, items, n_items, d, k, S, part);
-      B2K_CUDA_OK(ctx, cudaGetLastError());
-      ctx->stats.generic_launches++;
-    }
-    ctx->stats.kernel_launches++;
-  } else {
-    tm.mark(2, s);
-  }
-  ctx->stats.last_path = wg ? B2K_PATH_FUSED : B2K_PATH_GENERIC;
-  tm.mark(3, s);
-
-  // ---- refine, candidate allgather, merge of the own queries in rank order ----
-  const size_t rf_smem = (size_t)RF_WARPS * 2 * k * 4;
-  B2K_CUDA_OK(ctx, cudaFuncSetAttribute(k_knn_refine, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rf_smem));
-  k_knn_refine<<<(unsigned)((nq_all + RF_WARPS - 1) / RF_WARPS), RF_WARPS * 32, rf_smem, s>>>(
-      part, S, nq_all, k, Q, items, n_items, d, row0, item_ids, cand);
-  B2K_CUDA_OK(ctx, cudaGetLastError());
-  ctx->stats.kernel_launches++;
-  tm.mark(4, s);
+  // ---- candidate allgather, merge of the own queries in rank order ----
   const KnnCand* all = cand;
   if (nr > 1) {
     B2K_TRY(b2k_comm_allgather_bytes(ctx, cand, cand_all, (size_t)nq_all * k * sizeof(KnnCand), s));
@@ -649,5 +677,25 @@ int b2k_knn_search_impl(b2k_ctx* ctx, const float* items, int64_t n_items, const
     ctx->stats.last_allreduce_ms = tm.ms(0, 1) + tm.ms(4, 5);   // query and candidate all-gathers
     ctx->stats.last_loop_ms = tm.ms(0, 6);
   }
+  return B2K_OK;
+}
+
+int b2k_knn_local_impl(b2k_ctx* ctx, const float* items, int64_t n_items, const float* queries, int64_t nq, int d,
+                       int k, float* dist_out, int64_t* idx_out, cudaStream_t s) {
+  if (nq == 0) return B2K_OK;
+  Timer tm(false);
+  KnnLocal lp;
+  B2K_TRY(knn_local_plan(ctx, n_items, nq, d, k, (reinterpret_cast<uintptr_t>(queries) & 15u) == 0, &lp));
+  KnnCand* cand = nullptr;
+  B2K_TRY(b2k_scratch_layout(ctx, "kNN local", [&](B2kLayout& L) -> int {
+    knn_local_take(L, &lp, n_items, nq, d, k);
+    cand = L.take<KnnCand>((size_t)nq * k);
+    return B2K_OK;
+  }));
+  B2K_TRY(knn_local_run(ctx, lp, items, n_items, nullptr, queries, nq, d, k, 0, cand, tm, s));
+  k_knn_merge<<<(unsigned)((nq + RF_WARPS - 1) / RF_WARPS), RF_WARPS * 32, 0, s>>>(cand, 1, nq, 0, nq, k, dist_out,
+                                                                                    idx_out);
+  B2K_CUDA_OK(ctx, cudaGetLastError());
+  ctx->stats.kernel_launches++;
   return B2K_OK;
 }
