@@ -39,6 +39,8 @@
  *   b2k_rf_predict              tree.py:670- (the model's transform: cuML's forest inference over treelite)
  *   b2k_umap_fit / _graph       umap.py:1009-1065 (UMAP's fit function: cuML UMAP(...).fit on one partition)
  *   b2k_umap_transform          umap.py:1449-1551 (UMAPModel's transform: cuML UMAP.transform)
+ *   b2k_ivf_search              knn.py:1406-1692 (ApproximateNearestNeighborsModel.kneighbors with algorithm "ivfflat":
+ *                               the cuVS IVF-Flat build and search per partition and the top-k aggregation)
  *
  * Conventions
  *   - Plain C, no exceptions across the boundary: every call returns a b2k_status; the message for the
@@ -129,6 +131,7 @@ typedef struct b2k_stats {
   int64_t path_switch_iter;    /* iteration from which the last Lloyd loop left the large-shape wgmma kernel for the
                                   generic kernels because most rows needed the exact fix-up (option "adaptive_path",
                                   default 1; only with kernel_path = auto); -1 = it did not */
+  double last_probe_ms;        /* b2k_ivf_search with option "time_kernels" != 0: the probe selection (device time) */
 } b2k_stats;
 /* b2k_pca_fit reuses the fields: last_path = the Gram pass that ran (B2K_PATH_FUSED = wgmma, B2K_PATH_GENERIC = SIMT);
  * with option "time_kernels" != 0, last_reduce_ms = the column-sum pass, last_fused_ms = the Gram pass, last_allreduce_ms
@@ -258,6 +261,47 @@ int b2k_pca_transform(b2k_ctx* ctx, const float* X, int64_t n, int d, const floa
 int b2k_knn_search(b2k_ctx* ctx, const float* items, int64_t n_items_local, const int64_t* item_ids,
                    const float* queries, int64_t n_queries_local, int d, int k, float* distances_out,
                    int64_t* indices_out, uintptr_t stream);
+
+/* ---- approximate k-NN: IVF-Flat (Euclidean) ----
+ * Stands in for knn.py:1406-1692 (ApproximateNearestNeighborsModel.kneighbors, algorithm "ivfflat").  Arguments as for
+ * b2k_knn_search, plus:
+ *   nlist, nprobe  lists of the index and lists probed per query; nprobe is clamped to nlist
+ *   n_iters, train_fraction   the Lloyd run of the coarse quantizer (train = 1)
+ *   metric         B2K_IVF_EUCLIDEAN (distance) or B2K_IVF_SQEUCLIDEAN (the squared fp32 sum)
+ *   centers        device f32 [nlist, d]: used as given when train = 0; with train = 1 it receives the trained centres
+ *   item_list_out  device int32 [n_items_local] or NULL: the list of each local item
+ *   probe_out      device int32 [n_queries_local][nprobe (clamped)] or NULL: the lists each query probes, nearest first
+ *                  (-1 where a query with a NaN component probes nothing)
+ * One index over all ranks' items, so that for fixed centres the result depends neither on the rank count nor on how
+ * the rows are partitioned:
+ *   - Training subset: global row r (rank 0's rows in order, then rank 1's, ...) is a training row when
+ *     floor((r + 1) f) > floor(r f), f = train_fraction in (0, 1].  The training rows of all ranks are allgathered
+ *     in global row order and every rank runs b2k_kmeans_fit on them as one rank: init B2K_INIT_RANDOM with seed
+ *     B2K_IVF_SEED, max_iter = n_iters, tol = float32 tiny.  Ranks without a training row take part; the centres do not
+ *     depend on the rank count.  Each rank holds (ranks + 1) x the largest rank's training rows meanwhile.
+ *     nlist <= training rows.
+ *   - Lists: each item goes to its nearest centre by b2k_kmeans_assign (ties to the lowest centre).
+ *   - Probes: per query, the nprobe nearest centres under the exact k-NN rule (ties to the lower list).
+ *   - Result: per query, the exact k-NN result of b2k_knn_search over the items of its probed lists (fp32 distance
+ *     recomputed, sorted by (distance, global row)).  With nprobe = nlist it is b2k_knn_search's result.
+ *   - Fewer than k items found: the remaining distances are +inf and their ids the first entry's id, or INT64_MAX when
+ *     nothing was found.  A query with a NaN component finds nothing.
+ * The scan runs on wgmma (3xTF32 screening, exact recompute of the survivors) under b2k_knn_search's conditions, else on
+ * the generic SIMT kernel; option "kernel_path" selects the scan pass only (the build and probe steps choose their own).
+ * Errors, decided on allgathered sizes and flags so that every rank fails together: those of b2k_knn_search; an item
+ * with a non-finite component (B2K_ERR_INVALID); nlist < 1; nprobe < 1; nprobe > 256 after clamping
+ * (B2K_ERR_UNSUPPORTED); an unknown metric.  Collective across the communicator when one is initialised; synchronises
+ * `stream`.  Nothing uses atomics: bitwise reproducible for the same input, rank count and device.
+ * Stats: last_path = the scan pass that ran; with option "time_kernels" != 0, last_finalize_ms = the build (subset,
+ * Lloyd, assign, sort and prep), last_probe_ms = the probe selection, last_fused_ms = the scan passes, last_reduce_ms =
+ * the pair sort and query gather, refine and merge, last_allreduce_ms = both allgathers, last_loop_ms = the whole call
+ * after the size allgather (device times, CUDA events). */
+#define B2K_IVF_SEED 20240613ULL
+typedef enum b2k_ivf_metric { B2K_IVF_EUCLIDEAN = 0, B2K_IVF_SQEUCLIDEAN = 1 } b2k_ivf_metric;
+int b2k_ivf_search(b2k_ctx* ctx, const float* items, int64_t n_items_local, const int64_t* item_ids,
+                   const float* queries, int64_t n_queries_local, int d, int k, int nlist, int nprobe, int n_iters,
+                   double train_fraction, int metric, int train, float* centers, int32_t* item_list_out,
+                   int32_t* probe_out, float* distances_out, int64_t* indices_out, uintptr_t stream);
 
 /* ---- linear regression (squared loss: OLS, ridge, lasso, elastic net) ----
  * Stands in for regression.py:546-607 (LinearRegressionMG / RidgeMG / CDMG on the standardized data, then the

@@ -55,6 +55,7 @@ EXPORTED_SYMBOLS = (
     "b2k_pca_finalize",
     "b2k_pca_transform",
     "b2k_knn_search",
+    "b2k_ivf_search",
     "b2k_linreg_moments",
     "b2k_linreg_solve",
     "b2k_linreg_predict",
@@ -165,6 +166,7 @@ class Stats(ctypes.Structure):
         ("recheck_rows", ctypes.c_int64),
         ("recheck_candidates", ctypes.c_int64),
         ("path_switch_iter", ctypes.c_int64),
+        ("last_probe_ms", ctypes.c_double),
     ]
 
 
@@ -218,6 +220,8 @@ def load_library() -> ctypes.CDLL:
     L.b2k_pca_finalize.argtypes = [vp, i32, i64, i32, vp, vp, vp]
     L.b2k_pca_transform.argtypes = [vp, vp, i64, i32, vp, i32, vp, ctypes.c_size_t]
     L.b2k_knn_search.argtypes = [vp, vp, i64, vp, vp, i64, i32, i32, vp, vp, ctypes.c_size_t]
+    L.b2k_ivf_search.argtypes = [vp, vp, i64, vp, vp, i64, i32, i32, i32, i32, i32, f64, i32, i32, vp, vp, vp, vp, vp,
+                                 ctypes.c_size_t]
     L.b2k_linreg_moments.argtypes = [vp, vp, vp, i64, i32, ctypes.POINTER(i64), vp, vp, ctypes.c_size_t]
     L.b2k_linreg_solve.argtypes = [vp, vp, i32, i64, f64, f64, i32, i32, i32, f64, vp, ctypes.POINTER(f64),
                                    ctypes.POINTER(i32)]
@@ -589,6 +593,50 @@ class Context:
                 self._h, items.data_ptr(), n, item_ids.data_ptr() if item_ids is not None else None,
                 queries.data_ptr(), nq, d, int(k), dist.data_ptr(), idx.data_ptr(), self._stream()))
         return dist, idx
+
+    IVF_METRICS = {"euclidean": 0, "l2": 0, "sqeuclidean": 1}
+
+    def ivf_search(self, items: Any, queries: Any, k: int, nlist: int, nprobe: int, item_ids: Any = None,
+                   centers: Any = None, n_iters: int = 20, train_fraction: float = 0.5, metric: str = "euclidean",
+                   return_lists: bool = False) -> Tuple[Any, ...]:
+        """IVF-Flat search (b2k_ivf_search; collective when a communicator is initialised): the k nearest items of each
+        of this rank's queries among the items of its nprobe nearest lists.  Arguments as for knn_search; centers is a
+        float32 CUDA tensor [nlist, d] used as given, or None to train them on all ranks' items.  Returns (distances,
+        indices, centers) as CUDA tensors, plus (item lists int32 [n_items], probes int32 [n_q, min(nprobe, nlist)])
+        with return_lists."""
+        t = self._torch
+        n, d = self._check_X(items)
+        nq, dq = self._check_X(queries)
+        if dq != d:
+            raise ValueError(f"queries have {dq} features, items {d}")
+        if metric not in self.IVF_METRICS:
+            raise ValueError(f"metric {metric!r} is not supported by IVF-Flat (supported: {sorted(self.IVF_METRICS)})")
+        if item_ids is not None:
+            if not (item_ids.is_cuda and item_ids.dtype == t.int64 and item_ids.is_contiguous()
+                    and tuple(item_ids.shape) == (n,)):
+                raise ValueError("item_ids must be a contiguous int64 CUDA tensor [n_items]")
+        nl = max(int(nlist), 1)
+        train = centers is None
+        if train:
+            C = t.empty((nl, d), dtype=t.float32, device=self.device)
+        else:
+            if not (centers.is_cuda and centers.dtype == t.float32 and centers.is_contiguous()
+                    and tuple(centers.shape) == (int(nlist), d)):
+                raise ValueError(f"centers must be a contiguous float32 CUDA tensor [{nlist}, {d}]")
+            C = centers.clone()
+        kk = max(int(k), 0)
+        npr = max(min(int(nprobe), nl), 0)
+        dist = t.empty((nq, kk), dtype=t.float32, device=self.device)
+        idx = t.empty((nq, kk), dtype=t.int64, device=self.device)
+        lists = t.empty((n,), dtype=t.int32, device=self.device) if return_lists else None
+        probes = t.empty((nq, npr), dtype=t.int32, device=self.device) if return_lists else None
+        ptr = lambda x: x.data_ptr() if x is not None else None   # noqa: E731
+        with t.cuda.device(self.device):
+            self._check(self._L.b2k_ivf_search(
+                self._h, items.data_ptr(), n, ptr(item_ids), queries.data_ptr(), nq, d, int(k), int(nlist), int(nprobe),
+                int(n_iters), float(train_fraction), self.IVF_METRICS[metric], int(train), C.data_ptr(), ptr(lists),
+                ptr(probes), dist.data_ptr(), idx.data_ptr(), self._stream()))
+        return (dist, idx, C, lists, probes) if return_lists else (dist, idx, C)
 
     def linreg_moments(self, X: Any, y: Any) -> Tuple[int, np.ndarray, np.ndarray]:
         """The passes over the data of a linear regression fit (collective when a communicator is initialised): X [n, d]

@@ -987,6 +987,26 @@ extern "C" int b2k_knn_search(b2k_ctx* ctx, const float* items, int64_t n_items_
 }
 
 // ------------------------------------------------------------------------------------------------
+// approximate k-NN, IVF-Flat (b2k_ivf.cu)
+// ------------------------------------------------------------------------------------------------
+extern "C" int b2k_ivf_search(b2k_ctx* ctx, const float* items, int64_t n_items_local, const int64_t* item_ids,
+                              const float* queries, int64_t n_queries_local, int d, int k, int nlist, int nprobe,
+                              int n_iters, double train_fraction, int metric, int train, float* centers,
+                              int32_t* item_list_out, int32_t* probe_out, float* distances_out, int64_t* indices_out,
+                              uintptr_t stream) {
+  if (!ctx) return b2k_fail(nullptr, B2K_ERR_INVALID, "b2k_ivf_search: ctx is NULL");
+  if (n_items_local < 0 || n_queries_local < 0 || d <= 0 || !centers || (n_items_local > 0 && !items) ||
+      (n_queries_local > 0 && (!queries || !distances_out || !indices_out)))
+    return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_ivf_search: bad items/queries/centers/outputs/n/d");
+  if (n_items_local > (int64_t)0x7fffff00)
+    return b2k_fail(ctx, B2K_ERR_UNSUPPORTED, "b2k_ivf_search: more than 2^31 - 256 items on one rank");
+  B2K_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  return b2k_ivf_search_impl(ctx, items, n_items_local, item_ids, queries, n_queries_local, d, k, nlist, nprobe, n_iters,
+                             train_fraction, metric, train, centers, item_list_out, probe_out, distances_out,
+                             indices_out, reinterpret_cast<cudaStream_t>(stream));
+}
+
+// ------------------------------------------------------------------------------------------------
 // DBSCAN (b2k_dbscan.cu)
 // ------------------------------------------------------------------------------------------------
 extern "C" int b2k_dbscan_fit(b2k_ctx* ctx, const float* X, int64_t n_local, int d, double eps, int min_samples,

@@ -839,7 +839,8 @@ int b2k_dbscan_fit_impl(b2k_ctx* ctx, const float* X, int64_t n_local, int d, do
   CUtensorMap mq, mh, ml;
   if (wg) {
     const float* src = metric == 1 ? Y : Xall;   // shifted by its global row 0
-    k_knn_prep<<<(unsigned)((n_pad * 32 + 255) / 256), 256, 0, s>>>(src, n_total, d, n_pad, DP, Xhi, Xlo, norms);
+    k_knn_prep<<<(unsigned)((n_pad * 32 + 255) / 256), 256, 0, s>>>(src, n_total, d, nullptr, n_pad, DP, Xhi, Xlo,
+                                                                         norms);
     B2K_CUDA_OK(ctx, cudaGetLastError());
     ctx->stats.kernel_launches++;
     if (n_local > 0) {

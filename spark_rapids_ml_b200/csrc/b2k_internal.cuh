@@ -138,6 +138,26 @@ struct B2kLayout {
   }
 };
 
+// Device buffers owned by one call that outlive the scratch layouts of the calls it makes (stream-ordered allocation).
+struct DevBuf {
+  void* p = nullptr;
+  cudaStream_t s = nullptr;
+  ~DevBuf() {
+    if (p) cudaFreeAsync(p, s);
+  }
+};
+template <typename T>
+int dalloc(b2k_ctx* ctx, DevBuf& b, size_t count, cudaStream_t s, T** out) {
+  if (b.p) {
+    B2K_CUDA_OK(ctx, cudaFreeAsync(b.p, s));
+    b.p = nullptr;
+  }
+  b.s = s;
+  B2K_CUDA_OK(ctx, cudaMallocAsync(&b.p, (count > 0 ? count : 1) * sizeof(T), s));
+  *out = static_cast<T*>(b.p);
+  return B2K_OK;
+}
+
 // Runs `layout` (int(B2kLayout&)) to measure, grows ctx->scratch to that size, then runs it over the scratch to place.
 template <typename F>
 int b2k_scratch_layout(b2k_ctx* ctx, const char* who, F&& layout) {
@@ -296,6 +316,77 @@ int b2k_knn_search_impl(b2k_ctx* ctx, const float* items, int64_t n_items, const
 // each of queries [nq, d] -> sqrt(distance) ascending, ties to the lower row, and the item row.  1 <= k <= n_items.
 int b2k_knn_local_impl(b2k_ctx* ctx, const float* items, int64_t n_items, const float* queries, int64_t nq, int d,
                        int k, float* dist_out, int64_t* idx_out, cudaStream_t s);
+
+// The passes of the search that IVF-Flat (b2k_ivf.cu) runs on its own index layout.
+constexpr int B2K_KNN_WG_QROWS = 128;   // query rows of a wgmma unit
+constexpr int B2K_KNN_WG_BLOCK = 128;   // index rows per block of the wgmma pass (a unit's index range is in blocks)
+constexpr int B2K_KNN_GEN_QROWS = 16;   // query rows of a generic unit (its index range is in item rows)
+constexpr int B2K_KNN_MAX_LISTS = 256;  // partial lists one refine merges per query
+// one candidate of the refined lists that cross NCCL (16 bytes)
+struct KnnCand {
+  float d;        // exact squared distance, +inf for padding
+  int32_t grow;   // global row, INT32_MAX for padding
+  int64_t id;     // the user's item id (global row when no ids are given), -1 for padding
+};
+// One work unit of a search pass: query rows [row0, row0 + nrows) against the index range [lo, hi); row r of the unit
+// writes its k best (screen distance bits, index row) to part[out0 + r][k].
+struct KnnUnit {
+  int64_t out0;
+  int row0, nrows;
+  int lo, hi;
+};
+// true when the wgmma pass takes the shape (d % 4 == 0, 4 <= d <= 128, k <= 64); the padded width DP it then uses
+bool b2k_knn_wg_shape(int d, int k);
+int b2k_knn_wg_dp(int d);
+// index planes of x - s for the wgmma pass, s = X row 0: row p of the planes is X row perm[p] (perm NULL: p < n), or
+// padding (zeros, +inf norm) where perm[p] < 0 / p >= n
+int b2k_knn_prep_launch(b2k_ctx* ctx, const float* X, int64_t n, int d, const int32_t* perm, int64_t n_pad, int DP,
+                        float* Xhi, float* Xlo, float* norms, cudaStream_t s);
+// one search pass over a unit table (device, nunits entries).  wgmma: Q = shifted queries [nq][d] (16-byte aligned),
+// the planes and norms of b2k_knn_prep_launch; generic: Q unshifted, item row r of the index is X row xperm[r] (xperm
+// NULL: r)
+int b2k_knn_scan_launch(b2k_ctx* ctx, bool wg, int DP, const float* Q, int64_t nq, const float* X, const int32_t* xperm,
+                        const float* Xhi, const float* Xlo, const float* norms, int64_t n_pad, int d, int k,
+                        const KnnUnit* units, int nunits, int2* part, cudaStream_t s);
+// refine: per query row of Q [nq][d], merge its nl partial lists (list l at part row slots[q * nl + l], -1 = none; slots
+// NULL: l * nq + q), map index rows through perm (NULL: identity) to local item rows, recompute exact fp32 distances
+// against X and sort by (distance, global row) -> cand [nq][k]
+int b2k_knn_refine_launch(b2k_ctx* ctx, const int2* part, int nl, const int32_t* slots, const int32_t* perm, int64_t nq,
+                          int k, const float* Q, const float* X, int64_t n_items, int d, int64_t row0,
+                          const int64_t* ids, KnnCand* cand, cudaStream_t s);
+// merge of own queries [q0, q0 + nq_own) over nranks candidate lists -> distances (sqrt, or squared) and ids; fill: past
+// the found items the id is the first entry's id, or INT64_MAX when nothing was found
+int b2k_knn_merge_launch(b2k_ctx* ctx, const KnnCand* all, int nranks, int64_t nq_all, int64_t q0, int64_t nq_own, int k,
+                         bool squared, bool fill, float* dist_out, int64_t* idx_out, cudaStream_t s);
+
+struct B2kTimer {   // CUDA events around the device phases when option time_kernels is set
+  cudaEvent_t ev[12] = {};
+  bool on = false;
+  explicit B2kTimer(bool enable) : on(enable) {
+    if (on)
+      for (auto& e : ev) cudaEventCreate(&e);
+  }
+  ~B2kTimer() {
+    if (on)
+      for (auto& e : ev) cudaEventDestroy(e);
+  }
+  void mark(int i, cudaStream_t s) {
+    if (on) cudaEventRecord(ev[i], s);
+  }
+  double ms(int a, int b) const {
+    float t = 0.f;
+    if (on) cudaEventElapsedTime(&t, ev[a], ev[b]);
+    return (double)t;
+  }
+};
+
+// ------------------------------------------------------------------------------------------------
+// approximate k-NN (IVF-Flat) — b2k_ivf.cu (the C ABI entry point in b2k_api.cu checks its arguments, then calls this)
+// ------------------------------------------------------------------------------------------------
+int b2k_ivf_search_impl(b2k_ctx* ctx, const float* items, int64_t n_items, const int64_t* item_ids,
+                        const float* queries, int64_t nq_local, int d, int k, int nlist, int nprobe, int n_iters,
+                        double train_fraction, int metric, int train, float* centers, int32_t* item_list_out,
+                        int32_t* probe_out, float* dist_out, int64_t* idx_out, cudaStream_t s);
 
 // ------------------------------------------------------------------------------------------------
 // UMAP — b2k_umap.cu (the C ABI entry points in b2k_api.cu check their arguments, then call these)

@@ -2,7 +2,8 @@
 //
 //   sizes   allgather of (n_items, n_queries, d) per rank; every size error is decided on the gathered values.
 //   queries allgather of every rank's queries, padded to the largest count: Q [nranks * nq_max][d].
-//   search  over the local index for every query, in work units = (tile of queries, index split):
+//   search  over the local index for every query, in work units = (tile of queries, index split), given to the passes
+//           as a unit table {query rows, index range, output row} that IVF-Flat (b2k_ivf.cu) fills with its own units:
 //             wgmma path (k_knn_wg, 3xTF32): d % 4 == 0, 4 <= d <= 128, k <= 64, 16-byte aligned queries;
 //               everything in the frame of s = local item row 0 (non-finite components -> 0): k_knn_prep writes the
 //               index as zero-padded tf32 hi/lo planes of x - s [n_pad][DP] and ||x - s||^2 (+inf padding),
@@ -23,12 +24,6 @@
 namespace {
 #include "b2k_ptx.cuh"
 
-// one candidate of the refined lists that cross NCCL (16 bytes)
-struct KnnCand {
-  float d;        // exact squared distance, +inf for padding
-  int32_t grow;   // global row, INT32_MAX for padding
-  int64_t id;     // the user's item id (global row when no ids are given), -1 for padding
-};
 static_assert(sizeof(KnnCand) == 16, "KnnCand crosses NCCL as 16 bytes");
 
 __device__ __forceinline__ bool key_less(float da, int ra, float db, int rb) { return da < db || (da == db && ra < rb); }
@@ -52,7 +47,8 @@ constexpr int KW_N = 128;                   // index rows per block (wgmma N)
 constexpr int KW_CHUNK = 32;                // f32 per 128-byte swizzle row
 constexpr int KW_KMAX = 64;                 // largest k of the wgmma path
 constexpr int KW_NTHREADS = 384;            // 8 consumer warps + a producer warpgroup (one warp issues)
-constexpr int KW_SMAX = 256;                // index splits (the merge keeps 8 list heads per lane)
+constexpr int KW_SMAX = B2K_KNN_MAX_LISTS;  // index splits (the merge keeps 8 list heads per lane)
+static_assert(KW_TM == B2K_KNN_WG_QROWS && KW_N == B2K_KNN_WG_BLOCK, "unit geometry shared with b2k_ivf.cu");
 
 template <int NCH>
 struct KnnWgCfg {
@@ -73,20 +69,17 @@ struct KnnWgCfg {
 static_assert(KnnWgCfg<4>::SMEM_BYTES == 192 * 1024 + 48, "cfg5 layout");
 
 struct KnnArgs {
-  int64_t nq;                // query rows (all ranks, padded)
-  int ntiles;                // query tiles
-  int S;                     // index splits
-  int nblk;                  // index blocks of KW_N rows
+  const KnnUnit* units;      // [nunits], index ranges in blocks of KW_N rows
+  int nunits;
   int k;
-  int64_t n_items;           // local index rows
-  const float* norms;        // [nblk * KW_N] ||x||^2, +inf past n_items
-  int2* part;                // [S][nq][k] (screen distance bits, local row)
+  const float* norms;        // [blocks * KW_N] ||x - s||^2, +inf on padding rows
+  int2* part;                // rows of k (screen distance bits, index row)
 };
 
 #include "b2k_knn_prep.cuh"
 
-// Persistent grid, static round-robin over units u = tile * S + split.  Warp 8 issues TMA: the unit's query tile
-// (NCH chunks, once per unit) and the split's index blocks, chunk by chunk, hi and lo planes into a ring of SC stages.
+// Persistent grid, static round-robin over the unit table.  Warp 8 issues TMA: the unit's query tile (NCH chunks, once
+// per unit) and its index blocks, chunk by chunk, hi and lo planes into a ring of SC stages.
 // Consumer warpgroup g owns queries [64 g, 64 g + 64) of the tile; per block it accumulates lo.Xhi^T + hi.Xlo^T +
 // hi.Xhi^T (A = the query split in registers, as the 3xTF32 branch of k_wg_assign) into D[64 x 128].  Q, X and the
 // norms all come shifted by s.  The epilogue screens ||x - s||^2 - 2 (q - s).(x - s) against each row's current k-th
@@ -116,7 +109,7 @@ k_knn_wg(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUten
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
-  const int nunits = args.ntiles * args.S;
+  const int nunits = args.nunits;
   const int nit = (int)blockIdx.x < nunits ? (nunits - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
   const int k = args.k;
 
@@ -127,14 +120,12 @@ k_knn_wg(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUten
       tma_prefetch_desc(&mapLo);
       int q = 0;
       for (int it = 0; it < nit; ++it) {
-        const int u = (int)blockIdx.x + it * (int)gridDim.x;
-        const int tile = u / args.S, split = u % args.S;
-        const int b0 = (int)((int64_t)split * args.nblk / args.S), b1 = (int)((int64_t)(split + 1) * args.nblk / args.S);
+        const KnnUnit un = args.units[(int)blockIdx.x + it * (int)gridDim.x];
         mbar_wait_nocall(qempty, (uint32_t)((it & 1) ^ 1));
         mbar_expect_tx(qfull, (uint32_t)(NCH * G::QBYTES));
         for (int c = 0; c < NCH; ++c)
-          tma_load_2d(base + (uint32_t)(G::OFF_Q + c * G::QBYTES), &mapQ, qfull, c * KW_CHUNK, tile * KW_TM);
-        for (int b = b0; b < b1; ++b) {
+          tma_load_2d(base + (uint32_t)(G::OFF_Q + c * G::QBYTES), &mapQ, qfull, c * KW_CHUNK, un.row0);
+        for (int b = un.lo; b < un.hi; ++b) {
 #pragma unroll 1
           for (int c = 0; c < NCH; ++c, ++q) {
             const int cs = q % G::SC;
@@ -159,9 +150,7 @@ k_knn_wg(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUten
   float acc[R];
   int q = 0;
   for (int it = 0; it < nit; ++it) {
-    const int u = (int)blockIdx.x + it * (int)gridDim.x;
-    const int tile = u / args.S, split = u % args.S;
-    const int b0 = (int)((int64_t)split * args.nblk / args.S), b1 = (int)((int64_t)(split + 1) * args.nblk / args.S);
+    const KnnUnit un = args.units[(int)blockIdx.x + it * (int)gridDim.x];
     for (int e = lane & 3; e < k; e += 4) {
       L[0][e] = make_int2(0x7f800000, 0x7fffffff);
       L[1][e] = make_int2(0x7f800000, 0x7fffffff);
@@ -169,7 +158,7 @@ k_knn_wg(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUten
     __syncwarp();
     float thr[2] = {__int_as_float(0x7f800000), __int_as_float(0x7f800000)};
     mbar_wait_nocall(qfull, (uint32_t)(it & 1));
-    for (int b = b0; b < b1; ++b) {
+    for (int b = un.lo; b < un.hi; ++b) {
 #pragma unroll
       for (int c = 0; c < NCH; ++c, ++q) {
         const int cs = q % G::SC;
@@ -239,9 +228,9 @@ k_knn_wg(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUten
     __syncwarp();
     if (lane == 0) mbar_arrive(qempty);   // every A fragment of this unit has been read
     for (int h = 0; h < 2; ++h) {
-      const int64_t qrow = (int64_t)tile * KW_TM + rr0 + 8 * h;
-      if (qrow < args.nq) {
-        int2* o = args.part + ((size_t)split * args.nq + qrow) * k;
+      const int r = rr0 + 8 * h;
+      if (r < un.nrows) {
+        int2* o = args.part + (size_t)(un.out0 + r) * k;
         for (int e = lane & 3; e < k; e += 4) o[e] = L[h][e];
       }
     }
@@ -249,36 +238,33 @@ k_knn_wg(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUten
   }
 }
 
-// generic search: CTA = GQ queries x one index split; thread (qi = tid / 8, il = tid % 8) forms the exact fp32 sums
-// (q - x)^2 in feature order of items il + 8 u (u < 8) of each 64-item tile; the 8 threads of a query insert in turn
-constexpr int GQ = 16, GN = 64, GC = 32, G_NTHREADS = 128;
+// generic search: CTA = one unit of GQ queries x an item row range; thread (qi = tid / 8, il = tid % 8) forms the exact
+// fp32 sums (q - x)^2 in feature order of items il + 8 u (u < 8) of each 64-item tile; the 8 threads of a query insert
+// in turn
+constexpr int GQ = B2K_KNN_GEN_QROWS, GN = 64, GC = 32, G_NTHREADS = 128;
 __global__ void __launch_bounds__(G_NTHREADS, 1)
-k_knn_generic(const float* __restrict__ Q, int64_t nq, const float* __restrict__ X, int64_t n_items, int d, int k,
-              int S, int2* __restrict__ part) {
+k_knn_generic(const float* __restrict__ Q, const float* __restrict__ X, const int32_t* __restrict__ xperm, int d, int k,
+              const KnnUnit* __restrict__ units, int2* __restrict__ part) {
   extern __shared__ int2 gl[];   // [GQ][k]
   __shared__ float qs[GQ][GC + 1], xs[GN][GC + 1];
-  const int tile = blockIdx.x / S, split = blockIdx.x % S;
-  const int64_t ntx = (n_items + GN - 1) / GN;
-  const int64_t t0 = split * ntx / S, t1 = (split + 1) * ntx / S;
+  const KnnUnit un = units[blockIdx.x];
   const int qi = threadIdx.x >> 3, il = threadIdx.x & 7;
-  const int64_t qrow = (int64_t)tile * GQ + qi;
   int2* L = gl + (size_t)qi * k;
   for (int e = il; e < k; e += 8) L[e] = make_int2(0x7f800000, 0x7fffffff);
   __syncwarp();
   float thr = __int_as_float(0x7f800000);
-  for (int64_t t = t0; t < t1; ++t) {
+  for (int64_t t = un.lo; t < un.hi; t += GN) {
     float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
     for (int f0 = 0; f0 < d; f0 += GC) {
       __syncthreads();
       for (int e = threadIdx.x; e < GQ * GC; e += G_NTHREADS) {
         const int r = e / GC, c = e % GC;
-        const int64_t qr = (int64_t)tile * GQ + r;
-        qs[r][c] = (qr < nq && f0 + c < d) ? Q[qr * d + f0 + c] : 0.f;
+        qs[r][c] = (r < un.nrows && f0 + c < d) ? Q[(int64_t)(un.row0 + r) * d + f0 + c] : 0.f;
       }
       for (int e = threadIdx.x; e < GN * GC; e += G_NTHREADS) {
         const int r = e / GC, c = e % GC;
-        const int64_t xr = t * GN + r;
-        xs[r][c] = (xr < n_items && f0 + c < d) ? X[xr * d + f0 + c] : 0.f;
+        const int64_t xr = t + r;
+        xs[r][c] = (xr < un.hi && f0 + c < d) ? X[(xperm != nullptr ? (int64_t)xperm[xr] : xr) * d + f0 + c] : 0.f;
       }
       __syncthreads();
       const int fc = min(GC, d - f0);
@@ -291,7 +277,7 @@ k_knn_generic(const float* __restrict__ Q, int64_t nq, const float* __restrict__
         }
       }
     }
-    const int nv = n_items - t * GN < GN ? (int)(n_items - t * GN) : GN;   // valid items of the tile
+    const int nv = un.hi - t < GN ? (int)(un.hi - t) : GN;   // valid items of the tile
     bool cand = false;
 #pragma unroll
     for (int u = 0; u < 8; ++u) cand |= il + 8 * u < nv && acc[u] <= thr;
@@ -302,7 +288,7 @@ k_knn_generic(const float* __restrict__ Q, int64_t nq, const float* __restrict__
 #pragma unroll
           for (int u = 0; u < 8; ++u) {
             if (il + 8 * u < nv && acc[u] <= thr) {
-              list_insert(L, k, acc[u], (int)(t * GN + il + 8 * u));
+              list_insert(L, k, acc[u], (int)(t + il + 8 * u));
               thr = __int_as_float(L[k - 1].x);
             }
           }
@@ -312,8 +298,8 @@ k_knn_generic(const float* __restrict__ Q, int64_t nq, const float* __restrict__
       thr = __int_as_float(L[k - 1].x);
     }
   }
-  if (qrow < nq) {
-    int2* o = part + ((size_t)split * nq + qrow) * k;
+  if (qi < un.nrows) {
+    int2* o = part + (size_t)(un.out0 + qi) * k;
     for (int e = il; e < k; e += 8) o[e] = L[e];
   }
 }
@@ -364,31 +350,41 @@ __device__ __forceinline__ void warp_merge(int nl, int k, Head head, Emit emit) 
   }
 }
 
-// refine: warp per query row of Q.  Survivors = the k smallest (screen, local row) of the S lists; their exact fp32
+// refine: warp per query row of Q.  Survivors = the k smallest (screen, local row) of the nl lists; their exact fp32
 // distances are recomputed in feature order and the list re-sorted by (exact distance, global row, survivor position).
+// A list is sorted by (screen, index row), and index rows order as local rows within one list, so each list is also
+// sorted by (screen, local row) and the merge may key on the local row.
 constexpr int RF_WARPS = 4;
 __global__ void __launch_bounds__(RF_WARPS * 32)
-k_knn_refine(const int2* __restrict__ part, int S, int64_t nq, int k, const float* __restrict__ Q,
-             const float* __restrict__ X, int64_t n_items, int d, int64_t row0, const int64_t* __restrict__ ids,
-             KnnCand* __restrict__ cand) {
+k_knn_refine(const int2* __restrict__ part, int nl, const int32_t* __restrict__ slots, const int32_t* __restrict__ perm,
+             int64_t nq, int k, const float* __restrict__ Q, const float* __restrict__ X, int64_t n_items, int d,
+             int64_t row0, const int64_t* __restrict__ ids, KnnCand* __restrict__ cand) {
   extern __shared__ int rf_smem[];   // per warp: rows [k] (int), then exact distances [k] (float)
   const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int64_t qrow = (int64_t)blockIdx.x * RF_WARPS + w;
   if (qrow >= nq) return;
   int* rows = rf_smem + (size_t)w * 2 * k;
   float* ex = reinterpret_cast<float*>(rows + k);
-  if (S == 0) {
+  // entry p of list l as (screen bits, local row); a missing list reads as empty
+  auto entry = [&](int l, int p) -> int2 {
+    const int64_t sl = slots != nullptr ? (int64_t)slots[qrow * nl + l] : (int64_t)l * nq + qrow;
+    if (sl < 0) return make_int2(0x7f800000, 0x7fffffff);
+    int2 e = part[(size_t)sl * k + p];
+    if (perm != nullptr && e.y >= 0 && e.y != 0x7fffffff) e.y = perm[e.y];
+    return e;
+  };
+  if (nl == 0) {
     for (int t = lane; t < k; t += 32) rows[t] = -1;
   } else {
     warp_merge(
-        S, k,
+        nl, k,
         [&](int l, int p, float* dd, int* rr) {
-          const int2 e = part[((size_t)l * nq + qrow) * k + p];
+          const int2 e = entry(l, p);
           *dd = __int_as_float(e.x);
           *rr = e.y;
         },
         [&](int t, int l, int p) {
-          const int2 e = part[((size_t)l * nq + qrow) * k + p];
+          const int2 e = entry(l, p);
           rows[t] = e.y < n_items && e.y >= 0 ? e.y : -1;
         });
   }
@@ -430,7 +426,7 @@ k_knn_refine(const int2* __restrict__ part, int S, int64_t nq, int k, const floa
 // merge: warp per own query qi; list r = all[r][q0 + qi][0, k) for r < nranks, in rank order
 __global__ void __launch_bounds__(RF_WARPS * 32)
 k_knn_merge(const KnnCand* __restrict__ all, int nranks, int64_t nq_all, int64_t q0, int64_t nq_own, int k,
-            float* __restrict__ dist_out, int64_t* __restrict__ idx_out) {
+            bool squared, bool fill, float* __restrict__ dist_out, int64_t* idx_out) {
   const int w = threadIdx.x >> 5;
   const int64_t qi = (int64_t)blockIdx.x * RF_WARPS + w;
   if (qi >= nq_own) return;
@@ -444,31 +440,13 @@ k_knn_merge(const KnnCand* __restrict__ all, int nranks, int64_t nq_all, int64_t
       },
       [&](int t, int l, int p) {
         const KnnCand& c = at(l, p);
-        dist_out[qi * k + t] = sqrtf(c.d);
-        idx_out[qi * k + t] = c.id;
+        dist_out[qi * k + t] = squared ? c.d : sqrtf(c.d);
+        // entry 0 was written by its lane before warp_merge's __syncwarp
+        idx_out[qi * k + t] = !fill || c.grow != 0x7fffffff ? c.id : t == 0 ? INT64_MAX : idx_out[qi * k];
       });
 }
 
-struct Timer {   // CUDA events around the device phases when option time_kernels is set
-  cudaEvent_t ev[7] = {};
-  bool on = false;
-  explicit Timer(bool enable) : on(enable) {
-    if (on)
-      for (auto& e : ev) cudaEventCreate(&e);
-  }
-  ~Timer() {
-    if (on)
-      for (auto& e : ev) cudaEventDestroy(e);
-  }
-  void mark(int i, cudaStream_t s) {
-    if (on) cudaEventRecord(ev[i], s);
-  }
-  double ms(int a, int b) const {
-    float t = 0.f;
-    if (on) cudaEventElapsedTime(&t, ev[a], ev[b]);
-    return (double)t;
-  }
-};
+using Timer = B2kTimer;
 
 template <int NCH>
 int launch_wg(b2k_ctx* ctx, int grid, const CUtensorMap& mq, const CUtensorMap& mh, const CUtensorMap& ml,
@@ -485,11 +463,12 @@ struct KnnLocal {
   int DP = 0, S = 0;
   int64_t nblk = 0, n_pad = 0, ntiles = 0;
   float *Qs = nullptr, *Xhi = nullptr, *Xlo = nullptr, *norms = nullptr;
+  KnnUnit* units = nullptr;
   int2* part = nullptr;
 };
 
 int knn_local_plan(b2k_ctx* ctx, int64_t n_items, int64_t nq, int d, int k, bool q_aligned, KnnLocal* p) {
-  const bool wg_ok = d % 4 == 0 && d >= 4 && d <= 128 && k <= KW_KMAX && q_aligned;
+  const bool wg_ok = b2k_knn_wg_shape(d, k) && q_aligned;
   if (ctx->kernel_path == B2K_PATH_FUSED && !wg_ok)
     return b2k_fail(ctx, B2K_ERR_UNSUPPORTED, "kernel_path=2 requested but the wgmma kNN pass needs d % 4 == 0, "
                                               "4 <= d <= 128, k <= 64 and 16-byte aligned queries (d = " +
@@ -497,7 +476,7 @@ int knn_local_plan(b2k_ctx* ctx, int64_t n_items, int64_t nq, int d, int k, bool
   p->wg = wg_ok && ctx->kernel_path != B2K_PATH_GENERIC;
   int sm = ctx->sm_count;
   if (ctx->grid_limit > 0 && ctx->grid_limit < sm) sm = ctx->grid_limit;
-  p->DP = d <= 32 ? 32 : d <= 64 ? 64 : 128;
+  p->DP = b2k_knn_wg_dp(d);
   p->nblk = (n_items + KW_N - 1) / KW_N;
   p->n_pad = p->nblk * KW_N;
   const int64_t qt = p->wg ? KW_TM : GQ;
@@ -517,6 +496,7 @@ void knn_local_take(B2kLayout& L, KnnLocal* p, int64_t n_items, int64_t nq, int 
     p->Xlo = L.take<float>((size_t)p->n_pad * p->DP, 1024);
     p->norms = L.take<float>((size_t)p->n_pad);
   }
+  p->units = L.take<KnnUnit>((size_t)std::max<int64_t>(p->ntiles * p->S, 1));
   p->part = L.take<int2>((size_t)std::max(p->S, 1) * nq * k);
 }
 
@@ -525,49 +505,31 @@ int knn_local_run(b2k_ctx* ctx, const KnnLocal& p, const float* items, int64_t n
                   const float* Q, int64_t nq, int d, int k, int64_t row0, KnnCand* cand, Timer& tm, cudaStream_t s) {
   // ---- search of the local index for every query ----
   if (n_items > 0) {
+    // units u = tile * S + split: a tile of queries against one split of the index
+    const int64_t qt = p.wg ? KW_TM : GQ, ntx = p.wg ? p.nblk : (n_items + GN - 1) / GN;
+    std::vector<KnnUnit> units((size_t)(p.ntiles * p.S));
+    for (int64_t tile = 0; tile < p.ntiles; ++tile)
+      for (int split = 0; split < p.S; ++split) {
+        KnnUnit& u = units[(size_t)(tile * p.S + split)];
+        u.row0 = (int)(tile * qt);
+        u.nrows = (int)std::min<int64_t>(qt, nq - tile * qt);
+        u.out0 = (int64_t)split * nq + tile * qt;
+        const int64_t t0 = split * ntx / p.S, t1 = (split + 1) * ntx / p.S;
+        u.lo = p.wg ? (int)t0 : (int)(t0 * GN);
+        u.hi = p.wg ? (int)t1 : (int)std::min<int64_t>(t1 * GN, n_items);
+      }
+    B2K_CUDA_OK(ctx, cudaMemcpyAsync(p.units, units.data(), units.size() * sizeof(KnnUnit), cudaMemcpyHostToDevice, s));
     if (p.wg) {
-      k_knn_prep<<<(unsigned)((p.n_pad * 32 + 255) / 256), 256, 0, s>>>(items, n_items, d, p.n_pad, p.DP, p.Xhi, p.Xlo,
-                                                                        p.norms);
-      B2K_CUDA_OK(ctx, cudaGetLastError());
+      B2K_TRY(b2k_knn_prep_launch(ctx, items, n_items, d, nullptr, p.n_pad, p.DP, p.Xhi, p.Xlo, p.norms, s));
       const int64_t n4 = nq * d / 4;
       k_knn_shift_q<<<(unsigned)std::min<int64_t>((n4 + 255) / 256, (int64_t)ctx->sm_count * 16), 256, 0, s>>>(
           reinterpret_cast<const float4*>(Q), n4, d, items, reinterpret_cast<float4*>(p.Qs));
       B2K_CUDA_OK(ctx, cudaGetLastError());
-      ctx->stats.kernel_launches += 2;
+      ctx->stats.kernel_launches++;
     }
     tm.mark(2, s);
-    if (p.wg) {
-      CUtensorMap mq, mh, ml;
-      B2K_TRY(b2k_encode_2d(ctx, &mq, p.Qs, (uint64_t)d, (uint64_t)nq, (uint64_t)d * 4, KW_CHUNK, KW_TM,
-                            CU_TENSOR_MAP_L2_PROMOTION_L2_256B));
-      B2K_TRY(b2k_encode_2d(ctx, &mh, p.Xhi, (uint64_t)p.DP, (uint64_t)p.n_pad, (uint64_t)p.DP * 4, KW_CHUNK, KW_N,
-                            CU_TENSOR_MAP_L2_PROMOTION_L2_256B));
-      B2K_TRY(b2k_encode_2d(ctx, &ml, p.Xlo, (uint64_t)p.DP, (uint64_t)p.n_pad, (uint64_t)p.DP * 4, KW_CHUNK, KW_N,
-                            CU_TENSOR_MAP_L2_PROMOTION_L2_256B));
-      KnnArgs a{};
-      a.nq = nq;
-      a.ntiles = (int)p.ntiles;
-      a.S = p.S;
-      a.nblk = (int)p.nblk;
-      a.k = k;
-      a.n_items = n_items;
-      a.norms = p.norms;
-      a.part = p.part;
-      int sm = ctx->sm_count;
-      if (ctx->grid_limit > 0 && ctx->grid_limit < sm) sm = ctx->grid_limit;
-      const int grid = (int)std::min<int64_t>(sm, p.ntiles * p.S);
-      if (p.DP == 32) B2K_TRY(launch_wg<1>(ctx, grid, mq, mh, ml, a, s));
-      else if (p.DP == 64) B2K_TRY(launch_wg<2>(ctx, grid, mq, mh, ml, a, s));
-      else B2K_TRY(launch_wg<4>(ctx, grid, mq, mh, ml, a, s));
-      ctx->stats.fused_tc_launches++;
-    } else {
-      const size_t smem = (size_t)GQ * k * sizeof(int2);
-      B2K_CUDA_OK(ctx, cudaFuncSetAttribute(k_knn_generic, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-      k_knn_generic<<<(unsigned)(p.ntiles * p.S), G_NTHREADS, smem, s>>>(Q, nq, items, n_items, d, k, p.S, p.part);
-      B2K_CUDA_OK(ctx, cudaGetLastError());
-      ctx->stats.generic_launches++;
-    }
-    ctx->stats.kernel_launches++;
+    B2K_TRY(b2k_knn_scan_launch(ctx, p.wg, p.DP, p.wg ? p.Qs : Q, nq, items, nullptr, p.Xhi, p.Xlo, p.norms, p.n_pad, d,
+                                k, p.units, (int)units.size(), p.part, s));
   } else {
     tm.mark(2, s);
   }
@@ -575,16 +537,83 @@ int knn_local_run(b2k_ctx* ctx, const KnnLocal& p, const float* items, int64_t n
   tm.mark(3, s);
 
   // ---- refine ----
-  const size_t rf_smem = (size_t)RF_WARPS * 2 * k * 4;
-  B2K_CUDA_OK(ctx, cudaFuncSetAttribute(k_knn_refine, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rf_smem));
-  k_knn_refine<<<(unsigned)((nq + RF_WARPS - 1) / RF_WARPS), RF_WARPS * 32, rf_smem, s>>>(
-      p.part, p.S, nq, k, Q, items, n_items, d, row0, item_ids, cand);
-  B2K_CUDA_OK(ctx, cudaGetLastError());
-  ctx->stats.kernel_launches++;
+  B2K_TRY(b2k_knn_refine_launch(ctx, p.part, p.S, nullptr, nullptr, nq, k, Q, items, n_items, d, row0, item_ids, cand,
+                                s));
   tm.mark(4, s);
   return B2K_OK;
 }
 }  // namespace
+
+bool b2k_knn_wg_shape(int d, int k) { return d % 4 == 0 && d >= 4 && d <= 128 && k <= KW_KMAX; }
+int b2k_knn_wg_dp(int d) { return d <= 32 ? 32 : d <= 64 ? 64 : 128; }
+
+int b2k_knn_prep_launch(b2k_ctx* ctx, const float* X, int64_t n, int d, const int32_t* perm, int64_t n_pad, int DP,
+                        float* Xhi, float* Xlo, float* norms, cudaStream_t s) {
+  if (n_pad == 0) return B2K_OK;
+  k_knn_prep<<<(unsigned)((n_pad * 32 + 255) / 256), 256, 0, s>>>(X, n, d, perm, n_pad, DP, Xhi, Xlo, norms);
+  B2K_CUDA_OK(ctx, cudaGetLastError());
+  ctx->stats.kernel_launches++;
+  return B2K_OK;
+}
+
+int b2k_knn_scan_launch(b2k_ctx* ctx, bool wg, int DP, const float* Q, int64_t nq, const float* X, const int32_t* xperm,
+                        const float* Xhi, const float* Xlo, const float* norms, int64_t n_pad, int d, int k,
+                        const KnnUnit* units, int nunits, int2* part, cudaStream_t s) {
+  if (nunits == 0) return B2K_OK;
+  if (wg) {
+    CUtensorMap mq, mh, ml;
+    B2K_TRY(b2k_encode_2d(ctx, &mq, Q, (uint64_t)d, (uint64_t)nq, (uint64_t)d * 4, KW_CHUNK, KW_TM,
+                          CU_TENSOR_MAP_L2_PROMOTION_L2_256B));
+    B2K_TRY(b2k_encode_2d(ctx, &mh, Xhi, (uint64_t)DP, (uint64_t)n_pad, (uint64_t)DP * 4, KW_CHUNK, KW_N,
+                          CU_TENSOR_MAP_L2_PROMOTION_L2_256B));
+    B2K_TRY(b2k_encode_2d(ctx, &ml, Xlo, (uint64_t)DP, (uint64_t)n_pad, (uint64_t)DP * 4, KW_CHUNK, KW_N,
+                          CU_TENSOR_MAP_L2_PROMOTION_L2_256B));
+    KnnArgs a{};
+    a.units = units;
+    a.nunits = nunits;
+    a.k = k;
+    a.norms = norms;
+    a.part = part;
+    int sm = ctx->sm_count;
+    if (ctx->grid_limit > 0 && ctx->grid_limit < sm) sm = ctx->grid_limit;
+    const int grid = std::min(sm, nunits);
+    if (DP == 32) B2K_TRY(launch_wg<1>(ctx, grid, mq, mh, ml, a, s));
+    else if (DP == 64) B2K_TRY(launch_wg<2>(ctx, grid, mq, mh, ml, a, s));
+    else B2K_TRY(launch_wg<4>(ctx, grid, mq, mh, ml, a, s));
+    ctx->stats.fused_tc_launches++;
+  } else {
+    const size_t smem = (size_t)GQ * k * sizeof(int2);
+    B2K_CUDA_OK(ctx, cudaFuncSetAttribute(k_knn_generic, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    k_knn_generic<<<(unsigned)nunits, G_NTHREADS, smem, s>>>(Q, X, xperm, d, k, units, part);
+    B2K_CUDA_OK(ctx, cudaGetLastError());
+    ctx->stats.generic_launches++;
+  }
+  ctx->stats.kernel_launches++;
+  return B2K_OK;
+}
+
+int b2k_knn_refine_launch(b2k_ctx* ctx, const int2* part, int nl, const int32_t* slots, const int32_t* perm, int64_t nq,
+                          int k, const float* Q, const float* X, int64_t n_items, int d, int64_t row0,
+                          const int64_t* ids, KnnCand* cand, cudaStream_t s) {
+  if (nq == 0) return B2K_OK;
+  const size_t rf_smem = (size_t)RF_WARPS * 2 * k * 4;
+  B2K_CUDA_OK(ctx, cudaFuncSetAttribute(k_knn_refine, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rf_smem));
+  k_knn_refine<<<(unsigned)((nq + RF_WARPS - 1) / RF_WARPS), RF_WARPS * 32, rf_smem, s>>>(
+      part, nl, slots, perm, nq, k, Q, X, n_items, d, row0, ids, cand);
+  B2K_CUDA_OK(ctx, cudaGetLastError());
+  ctx->stats.kernel_launches++;
+  return B2K_OK;
+}
+
+int b2k_knn_merge_launch(b2k_ctx* ctx, const KnnCand* all, int nranks, int64_t nq_all, int64_t q0, int64_t nq_own, int k,
+                         bool squared, bool fill, float* dist_out, int64_t* idx_out, cudaStream_t s) {
+  if (nq_own == 0) return B2K_OK;
+  k_knn_merge<<<(unsigned)((nq_own + RF_WARPS - 1) / RF_WARPS), RF_WARPS * 32, 0, s>>>(
+      all, nranks, nq_all, q0, nq_own, k, squared, fill, dist_out, idx_out);
+  B2K_CUDA_OK(ctx, cudaGetLastError());
+  ctx->stats.kernel_launches++;
+  return B2K_OK;
+}
 
 int b2k_knn_search_impl(b2k_ctx* ctx, const float* items, int64_t n_items, const int64_t* item_ids,
                         const float* queries, int64_t nq_local, int d, int k, float* dist_out, int64_t* idx_out,
@@ -662,12 +691,8 @@ int b2k_knn_search_impl(b2k_ctx* ctx, const float* items, int64_t n_items, const
     all = cand_all;
   }
   tm.mark(5, s);
-  if (nq_local > 0) {
-    k_knn_merge<<<(unsigned)((nq_local + RF_WARPS - 1) / RF_WARPS), RF_WARPS * 32, 0, s>>>(
-        all, nr, nq_all, nr > 1 ? (int64_t)ctx->rank * nq_max : 0, nq_local, k, dist_out, idx_out);
-    B2K_CUDA_OK(ctx, cudaGetLastError());
-    ctx->stats.kernel_launches++;
-  }
+  B2K_TRY(b2k_knn_merge_launch(ctx, all, nr, nq_all, nr > 1 ? (int64_t)ctx->rank * nq_max : 0, nq_local, k, false,
+                               false, dist_out, idx_out, s));
   tm.mark(6, s);
   if (tm.on) {
     B2K_CUDA_OK(ctx, cudaStreamSynchronize(s));
@@ -693,9 +718,5 @@ int b2k_knn_local_impl(b2k_ctx* ctx, const float* items, int64_t n_items, const 
     return B2K_OK;
   }));
   B2K_TRY(knn_local_run(ctx, lp, items, n_items, nullptr, queries, nq, d, k, 0, cand, tm, s));
-  k_knn_merge<<<(unsigned)((nq + RF_WARPS - 1) / RF_WARPS), RF_WARPS * 32, 0, s>>>(cand, 1, nq, 0, nq, k, dist_out,
-                                                                                    idx_out);
-  B2K_CUDA_OK(ctx, cudaGetLastError());
-  ctx->stats.kernel_launches++;
-  return B2K_OK;
+  return b2k_knn_merge_launch(ctx, cand, 1, nq, 0, nq, k, false, false, dist_out, idx_out, s);
 }

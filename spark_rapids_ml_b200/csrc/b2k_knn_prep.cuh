@@ -9,16 +9,19 @@ __device__ __forceinline__ float knn_shift(const float* __restrict__ X, int f) {
   return isfinite(v) ? v : 0.f;
 }
 
-// index planes of x - s (rounded once to fp32), zero-padded to [n_pad][DP], and ||x - s||^2 of those same values
-__global__ void __launch_bounds__(256) k_knn_prep(const float* __restrict__ X, int64_t n, int d, int64_t n_pad, int DP,
+// index planes of x - s (rounded once to fp32), zero-padded to [n_pad][DP], and ||x - s||^2 of those same values.
+// Plane row p holds X row perm[p] (perm NULL: row p); rows with perm[p] < 0 or p >= n are padding (+inf norm).
+__global__ void __launch_bounds__(256) k_knn_prep(const float* __restrict__ X, int64_t n, int d,
+                                                  const int32_t* __restrict__ perm, int64_t n_pad, int DP,
                                                   float* __restrict__ Xhi, float* __restrict__ Xlo,
                                                   float* __restrict__ norms) {
   const int64_t row = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (row >= n_pad) return;
+  const int64_t src = perm != nullptr ? (int64_t)perm[row] : row < n ? row : -1;
   double s = 0.0;
   for (int t = lane; t < DP; t += 32) {
-    const float v = (row < n && t < d) ? X[row * d + t] - knn_shift(X, t) : 0.f;
+    const float v = (src >= 0 && t < d) ? X[src * d + t] - knn_shift(X, t) : 0.f;
     const uint32_t hb = rn_tf32_bits(v);
     Xhi[row * DP + t] = __uint_as_float(hb);
     Xlo[row * DP + t] = __uint_as_float(rn_tf32_bits(v - __uint_as_float(hb)));
@@ -26,7 +29,7 @@ __global__ void __launch_bounds__(256) k_knn_prep(const float* __restrict__ X, i
   }
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-  if (lane == 0) norms[row] = row < n ? (float)s : __int_as_float(0x7f800000);
+  if (lane == 0) norms[row] = src >= 0 ? (float)s : __int_as_float(0x7f800000);
 }
 
 // q - s as the wgmma pass reads it.  rn_tf32_bits carries out of the mantissa for NaNs whose payload fills its top bits,

@@ -23,26 +23,6 @@ constexpr int64_t RF_FLUSH_ROWS = 1LL << 28; // rows a cluster may add between f
                                              // so no u32 count can wrap; the u64 label sums then hold |S| <= 2^52.6
 constexpr size_t RF_STAGE_MAX = 64 * 1024;   // bytes of one staged tile of the cluster pass
 
-// ---- device buffers owned by one b2k_rf_fit call (stream-ordered allocation) ----
-struct DevBuf {
-  void* p = nullptr;
-  cudaStream_t s = nullptr;
-  ~DevBuf() {
-    if (p) cudaFreeAsync(p, s);
-  }
-};
-template <typename T>
-int dalloc(b2k_ctx* ctx, DevBuf& b, size_t count, cudaStream_t s, T** out) {
-  if (b.p) {
-    B2K_CUDA_OK(ctx, cudaFreeAsync(b.p, s));
-    b.p = nullptr;
-  }
-  b.s = s;
-  B2K_CUDA_OK(ctx, cudaMallocAsync(&b.p, std::max<size_t>(count, 1) * sizeof(T), s));
-  *out = static_cast<T*>(b.p);
-  return B2K_OK;
-}
-
 // The hash and the bootstrap draw of include/b2kmeans.h ("random forests"), on the host and the device alike.
 __host__ __device__ __forceinline__ uint64_t rf_mix(uint64_t z) {
   z ^= z >> 30;

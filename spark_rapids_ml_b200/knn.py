@@ -198,7 +198,7 @@ class NearestNeighborsModel(_CumlCaller, _CumlModel, NearestNeighborsClass, _Nea
         raise NotImplementedError("exactNearestNeighborsJoin needs DataFrame joins, which the local frame lacks")
 
     def approxNearestNeighbors(self, *args: Any, **kwargs: Any) -> Any:
-        raise NotImplementedError("approximate nearest neighbours (index structures) are outside this project's scope")
+        raise NotImplementedError("approxNearestNeighbors is not provided: use ApproximateNearestNeighbors")
 
     def write(self) -> Any:
         raise NotImplementedError(f"NearestNeighborsModel {_NO_PERSIST}")
@@ -250,10 +250,14 @@ class NearestNeighborsModel(_CumlCaller, _CumlModel, NearestNeighborsClass, _Nea
         super()._validate_parameters()
         self._validate_k()
 
+    def _search(self, ctx: Any, items: Any, queries: Any, ids: Any, params: Dict[str, Any]) -> Tuple[Any, Any]:
+        return ctx.knn_search(items, queries, int(params["n_neighbors"]), ids)
+
     def _get_cuml_fit_func(self, dataset: Any, extra_params: Optional[List[Dict[str, Any]]] = None
                            ) -> Callable[[FitInputType, Dict[str, Any]], Dict[str, Any]]:
         label_isdata, label_isquery = self._label_isdata, self._label_isquery
         qname = f"query_{self._getIdColOrDefault()}"
+        search = self._search
 
         def _cuml_fit(dfs: FitInputType, params: Dict[str, Any]) -> Dict[str, Any]:
             # stands in for NearestNeighborsMG(handle).kneighbors(...) and the row -> id mapping (knn.py:662-804)
@@ -267,8 +271,187 @@ class NearestNeighborsModel(_CumlCaller, _CumlModel, NearestNeighborsClass, _Nea
             items = X.index_select(0, sel(is_item)).contiguous()
             queries = X.index_select(0, sel(is_query)).contiguous()
             ids = torch.from_numpy(np.ascontiguousarray(row_number[is_item])).to(X.device)
-            dist, idx = ctx.knn_search(items, queries, int(params[param_alias.cuml_init]["n_neighbors"]), ids)
+            dist, idx = search(ctx, items, queries, ids, params[param_alias.cuml_init])
             return {qname: row_number[is_query], "indices": list(idx.cpu().numpy()),
                     "distances": list(dist.cpu().numpy())}
 
         return _cuml_fit
+
+
+# ---- approximate search: IVF-Flat (reference knn.py:838-1723) ----
+_IVF_KEYS = {"nlist": "nlist", "n_lists": "nlist", "nprobe": "nprobe", "n_probes": "nprobe",
+             "kmeans_n_iters": "kmeans_n_iters", "kmeans_trainset_fraction": "kmeans_trainset_fraction"}
+_IVF_DEFAULTS = {"nlist": 1024, "nprobe": 20, "kmeans_n_iters": 20, "kmeans_trainset_fraction": 0.5}
+
+
+def _check_algorithm(value: Optional[str]) -> None:
+    if value in ("ivfpq", "cagra"):
+        raise ValueError(f"algorithm '{value}' is not supported yet; use 'ivfflat'")
+    if value != "ivfflat":
+        raise ValueError(f"algorithm must be 'ivfflat' (got {value!r})")
+
+
+def _ivf_params(algo_params: Optional[Dict[str, Any]]) -> Dict[str, Any]:
+    """algoParams with the reference's aliases resolved (nlist / n_lists, nprobe / n_probes) and defaults filled in."""
+    out = dict(_IVF_DEFAULTS)
+    for key, v in (algo_params or {}).items():
+        if key not in _IVF_KEYS:
+            raise ValueError(f"algoParams key '{key}' is not supported by ivfflat (supported: {sorted(_IVF_KEYS)})")
+        out[_IVF_KEYS[key]] = v
+    return out
+
+
+def _check_metric(value: str) -> None:
+    if value not in ("euclidean", "l2", "sqeuclidean"):
+        raise ValueError(f"metric '{value}' is not supported by ivfflat (supported: euclidean, l2, sqeuclidean)")
+
+
+def _to_dict(v: Any) -> Any:
+    return v if v is None or isinstance(v, dict) else dict(v)
+
+
+class ApproximateNearestNeighborsClass(_CumlClass):
+    @classmethod
+    def _param_mapping(cls) -> Dict[str, Optional[str]]:
+        return {"k": "n_neighbors", "algorithm": "algorithm", "metric": "metric", "algoParams": "algo_params"}
+
+    def _get_cuml_params_default(self) -> Dict[str, Any]:
+        return {"n_neighbors": 5, "verbose": False, "algorithm": "ivfflat", "metric": "euclidean", "algo_params": None}
+
+
+class _ApproximateNearestNeighborsParams(_NearestNeighborsCumlParams):
+    """reference: knn.py:861-935."""
+
+    algorithm = Param("parent", "algorithm", "The algorithm to use for approximate nearest neighbors search.",
+                      TypeConverters.toString)
+    algoParams = Param("parent", "algoParams", "The parameters to use to set up a neighbor algorithm.", _to_dict)
+    metric = Param("parent", "metric", "The distance metric to use.", TypeConverters.toString)
+
+    def _set_ann_defaults(self) -> None:   # the estimator and the model run NearestNeighbors(Model).__init__
+        self._setDefault(algorithm="ivfflat", algoParams=None, metric="euclidean")
+
+    def setAlgorithm(self: P, value: str) -> P:
+        _check_algorithm(value)
+        return self._set_params(algorithm=value)
+
+    def getAlgorithm(self) -> str:
+        return self.getOrDefault("algorithm")
+
+    def setAlgoParams(self: P, value: Dict[str, Any]) -> P:
+        return self._set_params(algoParams=value)
+
+    def getAlgoParams(self) -> Dict[str, Any]:
+        return self.getOrDefault("algoParams")
+
+    def setMetric(self: P, value: str) -> P:
+        _check_metric(value)
+        return self._set_params(metric=value)
+
+    def getMetric(self) -> str:
+        return self.getOrDefault("metric")
+
+    def _validate_ann(self) -> Dict[str, Any]:
+        _check_algorithm(self.cuml_params.get("algorithm"))
+        _check_metric(self.cuml_params.get("metric"))
+        return _ivf_params(self.cuml_params.get("algo_params"))
+
+
+class ApproximateNearestNeighbors(ApproximateNearestNeighborsClass, _ApproximateNearestNeighborsParams,
+                                  NearestNeighbors):
+    """Approximate k nearest neighbours, IVF-Flat, on H100 (reference: knn.py:938-1217).  fit() is lazy, as for
+    NearestNeighbors; kneighbors() builds one index over all items (one coarse quantizer trained on a subset of every
+    GPU's items, see include/b2kmeans.h b2k_ivf_search) and probes the nprobe nearest lists of each query.  The
+    reference builds one index per partition instead, so its results depend on the partitioning; these do not.
+
+    algoParams: nlist / n_lists (default 1024), nprobe / n_probes (default 20, clamped to nlist), kmeans_n_iters
+    (default 20), kmeans_trainset_fraction (default 0.5).  metric: euclidean, l2 or sqeuclidean.  Queries that find
+    fewer than k items report +inf past the found ones, with the first id (or 2^63 - 1 when nothing was found).
+
+    >>> items = session.createDataFrame([(i, [float(i), float(i)]) for i in range(6)], "id int, features array<float>")
+    >>> knn = ApproximateNearestNeighbors(k=2).setInputCol("features").setIdCol("id")
+    >>> model = knn.setAlgoParams({"nlist": 2, "nprobe": 1}).fit(items)
+    """
+
+    @keyword_only
+    def __init__(self, *, k: Optional[int] = None, algorithm: str = "ivfflat",
+                 metric: str = "euclidean", algoParams: Optional[Dict[str, Any]] = None,
+                 inputCol: Optional[Union[str, List[str]]] = None, idCol: Optional[str] = None,
+                 num_workers: Optional[int] = None, verbose: Union[int, bool] = False, **kwargs: Any) -> None:
+        _check_algorithm(algorithm)
+        _check_metric(metric)
+        kw = dict(self._input_kwargs)
+        NearestNeighbors.__init__.__wrapped__(self, **{key: v for key, v in kw.items()
+                                                      if key not in ("algorithm", "metric", "algoParams")})
+        self._set_ann_defaults()
+        for key in ("algorithm", "metric", "algoParams"):
+            if key in kw:
+                self._set_params(**{key: kw[key]})
+
+    def _fit(self, item_df: LocalDataFrame) -> "ApproximateNearestNeighborsModel":
+        _no_pyspark(item_df)
+        self._validate_k()
+        item_df_withid = self._ensureIdCol(item_df)
+        processed = item_df_withid.with_constant_column(alias.label, self._label_isdata)
+        model = ApproximateNearestNeighborsModel(item_df_withid, processed, self._label_isdata, self._label_isquery)
+        model._num_workers = self._num_workers
+        model._float32_inputs = self._float32_inputs
+        self._copyValues(model)
+        self._copy_cuml_params(model)
+        return model
+
+    def write(self) -> Any:
+        raise NotImplementedError(f"ApproximateNearestNeighbors {_NO_PERSIST}")
+
+    @classmethod
+    def read(cls) -> Any:
+        raise NotImplementedError(f"ApproximateNearestNeighbors {_NO_PERSIST}")
+
+    def save(self, path: str, overwrite: bool = False) -> None:
+        raise NotImplementedError(f"ApproximateNearestNeighbors {_NO_PERSIST}")
+
+    @classmethod
+    def load(cls, path: str) -> Any:
+        raise NotImplementedError(f"ApproximateNearestNeighbors {_NO_PERSIST}")
+
+
+class ApproximateNearestNeighborsModel(ApproximateNearestNeighborsClass, _ApproximateNearestNeighborsParams,
+                                       NearestNeighborsModel):
+    """reference: knn.py:1219-1723.  kneighbors shares NearestNeighborsModel's barrier task over the union frame; only
+    the search it runs differs."""
+
+    def __init__(self, item_df_withid: LocalDataFrame, processed_item_df: LocalDataFrame, label_isdata: int,
+                 label_isquery: int) -> None:
+        NearestNeighborsModel.__init__(self, item_df_withid, processed_item_df, label_isdata, label_isquery)
+        self._set_ann_defaults()
+
+    def exactNearestNeighborsJoin(self, query_df: Any, distCol: str = "distCol") -> Any:
+        raise NotImplementedError("ApproximateNearestNeighborsModel has no exactNearestNeighborsJoin")
+
+    def approxSimilarityJoin(self, query_df: Any, distCol: str = "distCol") -> Any:
+        raise NotImplementedError("approxSimilarityJoin needs DataFrame joins, which the local frame lacks")
+
+    def write(self) -> Any:
+        raise NotImplementedError(f"ApproximateNearestNeighborsModel {_NO_PERSIST}")
+
+    @classmethod
+    def read(cls) -> Any:
+        raise NotImplementedError(f"ApproximateNearestNeighborsModel {_NO_PERSIST}")
+
+    def save(self, path: str, overwrite: bool = False) -> None:
+        raise NotImplementedError(f"ApproximateNearestNeighborsModel {_NO_PERSIST}")
+
+    @classmethod
+    def load(cls, path: str) -> Any:
+        raise NotImplementedError(f"ApproximateNearestNeighborsModel {_NO_PERSIST}")
+
+    def kneighbors(self, query_df: LocalDataFrame, sort_knn_df_by_query_id: bool = True
+                   ) -> Tuple[LocalDataFrame, LocalDataFrame, LocalDataFrame]:
+        self._validate_ann()
+        return super().kneighbors(query_df, sort_knn_df_by_query_id)
+
+    def _search(self, ctx: Any, items: Any, queries: Any, ids: Any, params: Dict[str, Any]) -> Tuple[Any, Any]:
+        ivf = _ivf_params(params["algo_params"])
+        dist, idx, _ = ctx.ivf_search(items, queries, int(params["n_neighbors"]), int(ivf["nlist"]),
+                                      int(ivf["nprobe"]), ids, n_iters=int(ivf["kmeans_n_iters"]),
+                                      train_fraction=float(ivf["kmeans_trainset_fraction"]), metric=params["metric"])
+        return dist, idx
