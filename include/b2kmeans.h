@@ -612,6 +612,45 @@ int b2k_eval_forest(b2k_ctx* ctx, const float* X, const float* y, int64_t n, int
                     int n_classes, double eps, int64_t* label_count_out, int64_t* tp_out, int64_t* fp_out,
                     double* loss_out, double* reg_out, uintptr_t stream);
 
+/* ---- binary evaluation (b2k_eval.cu scores, b2k_binary.cu curve): areaUnderROC / areaUnderPR of M models ----
+ * Semantics: Spark's BinaryClassificationEvaluator / BinaryClassificationMetrics with unit weights
+ * (tests/binary_oracle.py restates them in fp64 NumPy):
+ *   score    element 1 of the model's rawPrediction; a row is positive when its label > 0.5, else negative.
+ *   curve    the rows grouped by distinct score in descending order, in the order of Java's Double.compare (-0.0 below
+ *            +0.0; NaN one value, above +inf); each distinct score carries its (positives, negatives).  numBins > 0
+ *            with D distinct scores: g = D / numBins (integer division); when g >= 2, each run of g consecutive distinct
+ *            scores is one point (the last run may be shorter), else every distinct score is a point.  Spark groups per
+ *            partition of its sorted RDD; here the whole ordered list is one partition.  Cumulative counts give each
+ *            point's TP and FP; P and N are the totals.
+ *   ROC      (0, 0), then (FPR, TPR) = (FP / N, TP / P) per point, then (1, 1).
+ *   PR       (0, precision of the first point), then (recall, precision) = (TP / P, TP / (TP + FP)) per point.
+ *   area     the sum of the trapezoids (x1 - x0) (y1 + y0) / 2 over consecutive points, fp64.
+ *   guards   FPR = 0 when N = 0, recall = TPR = 0 when P = 0, precision = 1 when TP + FP = 0: the rules of Spark's
+ *            FalsePositiveRate, Recall and Precision in BinaryClassificationMetricComputers.  So a single-class set has
+ *            areaUnderROC 0 (all negative) or 1 (all positive), and areaUnderPR 0 (all negative) or 1 (all positive).
+ *            These guards are the one point of this statement not yet checked against Spark's sources.
+ * The score passes stage tiles of X [n, d] and y [n] (device f32) as b2k_eval_linear / b2k_eval_forest do, and write
+ * each model's score of row r to scores[i * ld_scores + r] (device f64) with the bits its own predict entry point writes
+ * at rawPrediction[r][1], and pos[r] = y[r] > 0.5 (device u8; may be NULL).  y must be finite.  Both return after
+ * enqueueing the pass on `stream` (the label check synchronises it first).  Models as b2k_eval_linear takes them, all of
+ * kind B2K_EVAL_LOGISTIC or B2K_EVAL_SOFTMAX (class values are not needed) ... */
+int b2k_eval_linear_scores(b2k_ctx* ctx, const float* X, const float* y, int64_t n, int d, int n_models,
+                           const int32_t* kind, const int32_t* row_offsets, const double* W, const double* b,
+                           double* scores, int64_t ld_scores, uint8_t* pos, uintptr_t stream);
+/* ... and forests as b2k_eval_forest takes them, classification, each with n_values >= 2. */
+int b2k_eval_forest_scores(b2k_ctx* ctx, const float* X, const float* y, int64_t n, int d, int n_models,
+                           const int32_t* n_trees, const int32_t* n_values, const int64_t* tree_offsets,
+                           const int32_t* feature, const float* threshold, const int32_t* children,
+                           const double* value, double* scores, int64_t ld_scores, uint8_t* pos, uintptr_t stream);
+/* out [M] (host) = the metric of each model from scores [M][n] and pos [n] (device), 1 <= n < 2^31, num_bins >= 0.  Per
+ * model: a radix sort of (score key, label bit), integer scans for the distinct scores and positives, then the
+ * trapezoids, whose fp64 partials fold in a fixed order.  No atomics: two calls on the same input give the same bits.
+ * Device memory of about 50 n bytes is allocated for the call.  Synchronises `stream`. */
+#define B2K_BINARY_ROC 0
+#define B2K_BINARY_PR 1
+int b2k_eval_binary(b2k_ctx* ctx, const double* scores, const uint8_t* pos, int64_t n, int n_models, int num_bins,
+                    int metric, double* out, uintptr_t stream);
+
 /* ---- UMAP (euclidean) ----
  * b2k_umap_fit stands in for umap.py:1009-1065 (the fit function: cuML UMAP(...).fit on the rows coalesced to one
  * partition), b2k_umap_transform for umap.py:1449-1551 (UMAPModel's transform: cuML UMAP.transform against the model's

@@ -70,12 +70,16 @@ EXPORTED_SYMBOLS = (
     "b2k_rf_predict",
     "b2k_eval_linear",
     "b2k_eval_forest",
+    "b2k_eval_linear_scores",
+    "b2k_eval_forest_scores",
+    "b2k_eval_binary",
     "b2k_umap_fit",
     "b2k_umap_graph",
     "b2k_umap_transform",
 )
 
 EVAL_KINDS = {"identity": 0, "logistic": 1, "softmax": 2}
+BINARY_METRICS = {"areaUnderROC": 0, "areaUnderPR": 1}
 
 FAMILY_CODES = {"auto": 0, "binomial": 1, "multinomial": 2}
 METRIC_CODES = {"euclidean": 0, "cosine": 1}
@@ -243,6 +247,10 @@ def load_library() -> ctypes.CDLL:
                                   ctypes.c_size_t]
     L.b2k_eval_forest.argtypes = [vp, vp, vp, i64, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, i32, f64, vp, vp, vp, vp,
                                   vp, ctypes.c_size_t]
+    L.b2k_eval_linear_scores.argtypes = [vp, vp, vp, i64, i32, i32, vp, vp, vp, vp, vp, i64, vp, ctypes.c_size_t]
+    L.b2k_eval_forest_scores.argtypes = [vp, vp, vp, i64, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, i64, vp,
+                                         ctypes.c_size_t]
+    L.b2k_eval_binary.argtypes = [vp, vp, vp, i64, i32, i32, i32, vp, ctypes.c_size_t]
     L.b2k_umap_fit.argtypes = [vp, vp, i64, i32, vp, ctypes.POINTER(UmapParams), vp, vp, ctypes.c_size_t]
     L.b2k_umap_graph.argtypes = [vp] + [vp] * 11
     L.b2k_umap_transform.argtypes = [vp, vp, vp, i64, i32, vp, i64, ctypes.POINTER(UmapParams), vp, ctypes.c_size_t]
@@ -856,12 +864,7 @@ class Context:
         n, d = self._check_X(X)
         self._check_y(y, n)
         m = len(models)
-        kinds = np.array([EVAL_KINDS[md["kind"]] for md in models], dtype=np.int32)
-        Ws = [np.ascontiguousarray(md["W"], dtype=np.float64).reshape(-1, d) for md in models]
-        rows = np.zeros(m + 1, dtype=np.int32)
-        rows[1:] = np.cumsum([w.shape[0] for w in Ws])
-        W = np.ascontiguousarray(np.concatenate(Ws, axis=0))
-        b = np.ascontiguousarray(np.concatenate([np.asarray(md["b"], dtype=np.float64).reshape(-1) for md in models]))
+        kinds, rows, W, b = self._linear_table(models, d)
         classification = bool(kinds[0] != 0)
         cv = (np.ascontiguousarray(np.concatenate([np.asarray(md["class_values"], dtype=np.float64).reshape(-1)
                                                    for md in models])) if classification else np.zeros(1))
@@ -880,6 +883,30 @@ class Context:
         n, d = self._check_X(X)
         self._check_y(y, n)
         m = len(forests)
+        nt, nv, *arrays = self._forest_table(forests)
+        C = self._eval_classes(y, n, int(nv.max())) if classification else 0
+        out = self._eval_out(m, C, classification)
+        with self._torch.cuda.device(self.device):
+            self._check(self._L.b2k_eval_forest(
+                self._h, X.data_ptr(), y.data_ptr(), n, d, m, int(bool(classification)), nt.ctypes.data,
+                nv.ctypes.data, *[a.ctypes.data for a in arrays], C, float(eps), *self._eval_ptrs(out, classification),
+                self._stream()))
+        return self._eval_result(out, n, C, classification)
+
+    @staticmethod
+    def _linear_table(models: Sequence[Dict[str, Any]], d: int) -> Tuple[np.ndarray, ...]:
+        """kind [M], row_offsets [M + 1], W [rows, d] and b [rows] of b2k_eval_linear's model arguments."""
+        kinds = np.array([EVAL_KINDS[md["kind"]] for md in models], dtype=np.int32)
+        Ws = [np.ascontiguousarray(md["W"], dtype=np.float64).reshape(-1, d) for md in models]
+        rows = np.zeros(len(models) + 1, dtype=np.int32)
+        rows[1:] = np.cumsum([w.shape[0] for w in Ws])
+        W = np.ascontiguousarray(np.concatenate(Ws, axis=0))
+        b = np.ascontiguousarray(np.concatenate([np.asarray(md["b"], dtype=np.float64).reshape(-1) for md in models]))
+        return kinds, rows, W, b
+
+    @staticmethod
+    def _forest_table(forests: Sequence[Dict[str, Any]]) -> Tuple[np.ndarray, ...]:
+        """n_trees, n_values, tree_offsets, feature, threshold, children and value of b2k_eval_forest's arguments."""
         offs = [np.ascontiguousarray(f["tree_offsets"], dtype=np.int64) for f in forests]
         vals = [np.ascontiguousarray(f["value"], dtype=np.float64) for f in forests]
         nt = np.array([o.size - 1 for o in offs], dtype=np.int32)
@@ -890,14 +917,68 @@ class Context:
         ch = np.ascontiguousarray(np.concatenate([np.asarray(f["children"], dtype=np.int32).reshape(-1, 2)
                                                   for f in forests]))
         val = np.ascontiguousarray(np.concatenate([v.reshape(-1) for v in vals]))
-        C = self._eval_classes(y, n, int(nv.max())) if classification else 0
-        out = self._eval_out(m, C, classification)
+        return nt, nv, off, feat, thr, ch, val
+
+    # -- binary evaluation ------------------------------------------------------------------
+    def binary_buffers(self, n_models: int, n: int) -> Tuple[Any, Any]:
+        """Device buffers of the binary scores of n_models models over n rows: scores [M, n] float64 and pos [n] uint8.
+        Their n x M x 9 bytes are checked against the device's free memory first."""
+        t = self._torch
+        need = int(n) * int(n_models) * 9
+        free, _ = t.cuda.mem_get_info(self.device)
+        if need > free:
+            raise MemoryError(f"binary evaluation: the scores of {n_models} models over {n} rows need {need} bytes of "
+                              f"device memory, and {free} are free; evaluate fewer rows or fewer models at once")
+        return (t.empty((int(n_models), int(n)), dtype=t.float64, device=self.device),
+                t.empty((int(n),), dtype=t.uint8, device=self.device))
+
+    def _check_binary_out(self, scores: Any, pos: Any, m: int, row0: int, n: int) -> None:
+        t = self._torch
+        if not (scores.is_cuda and scores.dtype == t.float64 and scores.dim() == 2 and scores.is_contiguous()
+                and scores.shape[0] == m and pos.is_cuda and pos.dtype == t.uint8 and pos.is_contiguous()
+                and pos.shape == (scores.shape[1],) and 0 <= row0 and row0 + n <= scores.shape[1]):
+            raise ValueError(f"scores must be a contiguous float64 CUDA tensor [{m}, N] and pos uint8 [N], N >= "
+                             f"row0 + n = {row0 + n}")
+
+    def binary_scores_linear(self, X: Any, y: Any, models: Sequence[Dict[str, Any]], scores: Any, pos: Any,
+                             row0: int = 0) -> None:
+        """b2k_eval_linear_scores: scores[i, row0 + r] = rawPrediction[r][1] of logistic model i (kind "logistic" or
+        "softmax", as eval_linear takes them) on (X [n, d], y [n]), pos[row0 + r] = y[r] > 0.5; one read of X."""
+        n, d = self._check_X(X)
+        self._check_y(y, n)
+        m = len(models)
+        self._check_binary_out(scores, pos, m, row0, n)
+        kinds, rows, W, b = self._linear_table(models, d)
         with self._torch.cuda.device(self.device):
-            self._check(self._L.b2k_eval_forest(
-                self._h, X.data_ptr(), y.data_ptr(), n, d, m, int(bool(classification)), nt.ctypes.data,
-                nv.ctypes.data, off.ctypes.data, feat.ctypes.data, thr.ctypes.data, ch.ctypes.data, val.ctypes.data, C,
-                float(eps), *self._eval_ptrs(out, classification), self._stream()))
-        return self._eval_result(out, n, C, classification)
+            self._check(self._L.b2k_eval_linear_scores(
+                self._h, X.data_ptr(), y.data_ptr(), n, d, m, kinds.ctypes.data, rows.ctypes.data, W.ctypes.data,
+                b.ctypes.data, scores.data_ptr() + 8 * row0, scores.shape[1], pos.data_ptr() + row0, self._stream()))
+
+    def binary_scores_forest(self, X: Any, y: Any, forests: Sequence[Dict[str, Any]], scores: Any, pos: Any,
+                             row0: int = 0) -> None:
+        """b2k_eval_forest_scores: as binary_scores_linear for classification forests (rf_fit's layout, >= 2 values)."""
+        n, d = self._check_X(X)
+        self._check_y(y, n)
+        m = len(forests)
+        self._check_binary_out(scores, pos, m, row0, n)
+        nt, nv, *arrays = self._forest_table(forests)
+        with self._torch.cuda.device(self.device):
+            self._check(self._L.b2k_eval_forest_scores(
+                self._h, X.data_ptr(), y.data_ptr(), n, d, m, nt.ctypes.data, nv.ctypes.data,
+                *[a.ctypes.data for a in arrays], scores.data_ptr() + 8 * row0, scores.shape[1],
+                pos.data_ptr() + row0, self._stream()))
+
+    def eval_binary(self, scores: Any, pos: Any, num_bins: int, metric: str) -> np.ndarray:
+        """b2k_eval_binary: areaUnderROC or areaUnderPR of each row of scores [M, n] with the label bits pos [n]
+        (Spark's BinaryClassificationMetrics with numBins, the whole list of distinct scores as one partition)."""
+        m = int(scores.shape[0])
+        self._check_binary_out(scores, pos, m, 0, 0)
+        out = np.zeros(m, dtype=np.float64)
+        with self._torch.cuda.device(self.device):
+            self._check(self._L.b2k_eval_binary(self._h, scores.data_ptr(), pos.data_ptr(), scores.shape[1], m,
+                                                int(num_bins), BINARY_METRICS[metric], out.ctypes.data,
+                                                self._stream()))
+        return out
 
     def _eval_classes(self, y: Any, n: int, c_models: int) -> int:
         """C = 1 + max(the largest label, the models' largest class); a bad label is reported by the pass itself."""

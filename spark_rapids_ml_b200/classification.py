@@ -515,6 +515,13 @@ class LogisticRegressionModel(LogisticRegressionClass, _CumlModelWithPredictionC
                 def __init__(self, gpu: int) -> None:
                     self.ctx = _transform_context(gpu)
 
+            if eval_metric_info["binary"]:
+                def _scores(h: Any, X: Any, y: Any, scores: Any, pos: Any, row0: int) -> None:
+                    h.ctx.binary_scores_linear(X, y, models, scores, pos, row0)
+
+                _scores.n_models = len(models)  # type: ignore[attr-defined]
+                return _Holder, None, _scores  # type: ignore[return-value]
+
             def _evaluate(h: Any, X: Any, y: Any) -> List[Dict[str, Any]]:
                 return _class_accs(h.ctx.eval_linear(X, y, models, eps))
 

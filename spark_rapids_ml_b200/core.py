@@ -491,8 +491,8 @@ def _iter_transform(transform_internal: Callable, get_model: Callable[[], Any], 
 
 def _supports_transform_evaluate(classification: bool, evaluator: Any) -> bool:
     """Whether the single-pass evaluation serves (estimator kind, evaluator): a classifier with a
-    MulticlassClassificationEvaluator and a metric of metrics.MULTICLASS_METRICS, or a regressor with a
-    RegressionEvaluator."""
+    MulticlassClassificationEvaluator and a metric of metrics.MULTICLASS_METRICS or a BinaryClassificationEvaluator
+    and a metric of metrics.BINARY_METRICS, or a regressor with a RegressionEvaluator."""
     from . import metrics
 
     name = type(evaluator).__name__
@@ -501,7 +501,8 @@ def _supports_transform_evaluate(classification: bool, evaluator: Any) -> bool:
     except Exception:
         return False
     if classification:
-        return name == "MulticlassClassificationEvaluator" and metric in metrics.MULTICLASS_METRICS
+        return ((name == "MulticlassClassificationEvaluator" and metric in metrics.MULTICLASS_METRICS) or
+                (name == "BinaryClassificationEvaluator" and metric in metrics.BINARY_METRICS))
     return name == "RegressionEvaluator" and metric in metrics.REGRESSION_METRICS
 
 
@@ -509,10 +510,16 @@ def _eval_metric_info(evaluator: Any) -> Dict[str, Any]:
     """What the device pass and the metric need from an evaluator (pyspark's or the local one)."""
     if evaluator.isSet("weightCol") and evaluator.getOrDefault("weightCol"):
         raise NotImplementedError("weightCol is not supported by the single-pass evaluation")
-    info = {"metric": evaluator.getMetricName(), "labelCol": evaluator.getLabelCol()}
+    info = {"metric": evaluator.getMetricName(), "labelCol": evaluator.getLabelCol(), "binary": False}
     if type(evaluator).__name__ == "MulticlassClassificationEvaluator":
         info.update(classification=True, eps=float(evaluator.getEps()), metricLabel=float(evaluator.getMetricLabel()),
                     beta=float(evaluator.getBeta()))
+    elif type(evaluator).__name__ == "BinaryClassificationEvaluator":
+        num_bins = int(evaluator.getNumBins())
+        if num_bins < 0:
+            raise ValueError(f"numBins must be >= 0, got {num_bins}")
+        info.update(classification=True, binary=True, eps=0.0, numBins=num_bins,
+                    rawPredictionCol=evaluator.getRawPredictionCol())
     else:
         info.update(classification=False, eps=0.0, throughOrigin=bool(evaluator.getThroughOrigin()))
     return info
@@ -523,7 +530,10 @@ def _transform_evaluate_internal(model: Any, dataset: Any, evaluator: Any) -> Li
     features and label are ingested as transform() ingests them, in groups of up to TRANSFORM_GROUP_ROWS rows; each
     group is one device evaluation pass (the model's third transform function) that returns every model's
     accumulators; the accumulators merge on the host in partition and group order.  The label goes to the device as
-    float32, as the fits read it: a float64 label that float32 cannot hold is scored at its float32 rounding."""
+    float32, as the fits read it: a float64 label that float32 cannot hold is scored at its float32 rounding.
+    A BinaryClassificationEvaluator needs every row's score at once: each group's pass appends every model's scores
+    and the label bits to device buffers sized for the whole frame (checked against the free device memory before the
+    first group), and one curve pass over them gives every model's area at the end."""
     from . import metrics
     from .sparkshim.sql import _batches_to_pdf_iter
     from .utils import DeviceRowAppender
@@ -559,14 +569,23 @@ def _transform_evaluate_internal(model: Any, dataset: Any, evaluator: Any) -> Li
                 _append_transform_features(app, pdf, n_cols)
         X = app.finish()
         yd = torch.as_tensor(y).to(m.ctx.device)
+        if binary:
+            evaluate(m, X, yd, state["scores"], state["pos"], state["row0"])
+            state["row0"] += int(y.size)
+            accs = []   # a group ran; the metrics come from the curve pass at the end
+            return
         got = evaluate(m, X, yd)
         accs = got if accs is None else [metrics.merge_all([a, b], info["classification"]) for a, b in zip(accs, got)]
 
+    binary = info["binary"]
     limit = max(1, min(TRANSFORM_GROUP_ROWS, TRANSFORM_GROUP_BYTES // (4 * n_cols + 4)))   # as _iter_transform
     for pid, part in enumerate(dataset._parts):
         if "model" not in state:
             gpu = _CumlCommon._set_gpu_device(BarrierTaskContext(pid, len(dataset._parts)), True, True)
             state["model"] = construct(gpu)
+            if binary:
+                state["scores"], state["pos"] = state["model"].ctx.binary_buffers(evaluate.n_models, dataset.count())
+                state["row0"] = 0
         group: List[pa.RecordBatch] = []
         rows = 0
         for batch in part:
@@ -578,6 +597,9 @@ def _transform_evaluate_internal(model: Any, dataset: Any, evaluator: Any) -> Li
         if group or accs is None:
             run(group)
     assert accs is not None
+    if binary:
+        return [float(v) for v in state["model"].ctx.eval_binary(state["scores"], state["pos"], info["numBins"],
+                                                                  info["metric"])]
     if info["classification"]:
         return [metrics.multiclass_metric(a, info["metric"], info["metricLabel"], info["beta"]) for a in accs]
     return [metrics.regression_metric(a, info["metric"], info["throughOrigin"]) for a in accs]

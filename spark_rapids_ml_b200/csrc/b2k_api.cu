@@ -1189,6 +1189,42 @@ extern "C" int b2k_eval_forest(b2k_ctx* ctx, const float* X, const float* y, int
                               reg_out, reinterpret_cast<cudaStream_t>(stream));
 }
 
+extern "C" int b2k_eval_linear_scores(b2k_ctx* ctx, const float* X, const float* y, int64_t n, int d, int n_models,
+                                      const int32_t* kind, const int32_t* row_offsets, const double* W, const double* b,
+                                      double* scores, int64_t ld_scores, uint8_t* pos, uintptr_t stream) {
+  if (!ctx) return b2k_fail(nullptr, B2K_ERR_INVALID, "b2k_eval_linear_scores: ctx is NULL");
+  if (n < 0 || d <= 0 || n_models < 1 || ld_scores < n || (n > 0 && (!X || !y || !scores)) || !kind ||
+      !row_offsets || !W || !b)
+    return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_eval_linear_scores: bad arguments");
+  B2K_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  return b2k_eval_linear_scores_impl(ctx, X, y, n, d, n_models, kind, row_offsets, W, b, scores, ld_scores, pos,
+                                     reinterpret_cast<cudaStream_t>(stream));
+}
+
+extern "C" int b2k_eval_forest_scores(b2k_ctx* ctx, const float* X, const float* y, int64_t n, int d, int n_models,
+                                      const int32_t* n_trees, const int32_t* n_values, const int64_t* tree_offsets,
+                                      const int32_t* feature, const float* threshold, const int32_t* children,
+                                      const double* value, double* scores, int64_t ld_scores, uint8_t* pos,
+                                      uintptr_t stream) {
+  if (!ctx) return b2k_fail(nullptr, B2K_ERR_INVALID, "b2k_eval_forest_scores: ctx is NULL");
+  if (n < 0 || d <= 0 || n_models < 1 || ld_scores < n || (n > 0 && (!X || !y || !scores)) || !n_trees ||
+      !n_values || !tree_offsets || !feature || !threshold || !children || !value)
+    return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_eval_forest_scores: bad arguments");
+  B2K_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  return b2k_eval_forest_scores_impl(ctx, X, y, n, d, n_models, n_trees, n_values, tree_offsets, feature, threshold,
+                                     children, value, scores, ld_scores, pos, reinterpret_cast<cudaStream_t>(stream));
+}
+
+extern "C" int b2k_eval_binary(b2k_ctx* ctx, const double* scores, const uint8_t* pos, int64_t n, int n_models,
+                               int num_bins, int metric, double* out, uintptr_t stream) {
+  if (!ctx) return b2k_fail(nullptr, B2K_ERR_INVALID, "b2k_eval_binary: ctx is NULL");
+  if (!scores || !pos || !out || n_models < 1 || num_bins < 0 || (metric != B2K_BINARY_ROC && metric != B2K_BINARY_PR))
+    return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_eval_binary: bad arguments");
+  B2K_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  return b2k_eval_binary_impl(ctx, scores, pos, n, n_models, num_bins, metric, out,
+                              reinterpret_cast<cudaStream_t>(stream));
+}
+
 // ------------------------------------------------------------------------------------------------
 // UMAP (b2k_umap.cu)
 // ------------------------------------------------------------------------------------------------

@@ -9,6 +9,9 @@
 //            prediction) into shared memory, then one warp per (model, column) reduces them in a fixed order and
 //            folds them into the CTA's running accumulators (Chan's merge for the regression moments).
 //   fold     k_eval_fold: per model, the CTAs' fp64 partials in CTA order.
+//   scores   k_score_linear / k_score_forest (binary evaluation): the same staged tile, but every model's score of
+//            every row (element 1 of its rawPrediction) goes to global memory, with the label bit y > 0.5; the curve
+//            pass over them is b2k_binary.cu.
 // The grid depends on the device and the shape alone, so two calls on the same input give the same bits.
 #include <algorithm>
 #include <cmath>
@@ -390,6 +393,84 @@ __global__ void __launch_bounds__(EV_NT, 2) k_eval_forest(ForestArgs a) {
   flush_cta<CLS>(lc, tf, acc, a.m, a.C, a.labels, a.counts, a.part);
 }
 
+// ---- binary scores ----
+// Where the score passes write: row r of model mi at scores[mi * ld + r]; pos[r] = y > 0.5 (NULL: not written).
+struct ScoreOut {
+  double* scores;
+  int64_t ld;
+  uint8_t* pos;
+};
+
+__device__ __forceinline__ void write_pos(const float* ys, int64_t t0, int tr, uint8_t* pos) {
+  if (pos)
+    for (int i = threadIdx.x; i < tr; i += EV_NT) pos[t0 + i] = ys[i] > 0.5f ? 1 : 0;
+}
+
+// Logistic kinds: rawPrediction[1] of k_logreg_rows, the margin of class 1 (binomial: raw = [-m, m], so m itself).
+// Only classes 0 and 1 are formed; each class's FMA chain is the one k_logreg_rows runs, whatever the chunk width.
+template <bool VEC>
+__global__ void __launch_bounds__(EV_NT, 2) k_score_linear(LinArgs a, ScoreOut o) {
+  extern __shared__ __align__(16) unsigned char ev_smem[];
+  const EvCarve cv = ev_carve(a.TR, a.dpad, 0, 0, false);
+  float* xs = reinterpret_cast<float*>(ev_smem + cv.xs);
+  float* ys = reinterpret_cast<float*>(ev_smem + cv.ys);
+  const int d = a.d, L = a.L, TR = a.TR;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, sub = lane & (L - 1), grp = lane / L, rpw = 32 / L;
+  const int rps = EV_NW * rpw;
+  for (int64_t t0 = (int64_t)blockIdx.x * TR; t0 < a.n; t0 += (int64_t)gridDim.x * TR) {
+    const int tr = (int)min((int64_t)TR, a.n - t0);
+    __syncthreads();
+    stage_tile<VEC>(a.X, a.y, t0, tr, d, a.dpad, xs, ys);
+    __syncthreads();
+    write_pos(ys, t0, tr, o.pos);
+    for (int mi = 0; mi < a.m; ++mi) {
+      const int w0 = a.row0[mi], kp = a.row0[mi + 1] - w0, c = kp == 1 ? 0 : 1;
+      const double* Wm = a.W + (size_t)w0 * a.dpad;
+      for (int s = warp * rpw; s < tr; s += rps) {
+        const int r = s + grp;
+        const bool valid = r < tr;
+        double ac[2] = {0.0, 0.0};
+        if (valid) b2k_logistic_lanes<2>(B2kRowSmem{xs + (size_t)r * a.dpad}, d, kp, 0, Wm, a.dpad, sub, L, ac);
+        const double m = b2k_lanes_sum(c ? ac[1] : ac[0], L);
+        if (sub == 0 && valid) o.scores[mi * o.ld + t0 + r] = a.b[w0 + c] + m;
+      }
+    }
+  }
+}
+
+// Classification forests: rawPrediction[1] of k_rf_predict, the trees' values of class 1 summed in tree order.
+template <bool VEC>
+__global__ void __launch_bounds__(EV_NT, 2) k_score_forest(ForestArgs a, ScoreOut o) {
+  extern __shared__ __align__(16) unsigned char ev_smem[];
+  const EvCarve cv = ev_carve(a.TR, a.dpad, 0, 0, false);
+  float* xs = reinterpret_cast<float*>(ev_smem + cv.xs);
+  float* ys = reinterpret_cast<float*>(ev_smem + cv.ys);
+  const int TR = a.TR, G = EV_NT / TR;
+  const int r = threadIdx.x % TR, g = threadIdx.x / TR;
+  for (int64_t t0 = (int64_t)blockIdx.x * TR; t0 < a.n; t0 += (int64_t)gridDim.x * TR) {
+    const int tr = (int)min((int64_t)TR, a.n - t0);
+    __syncthreads();
+    stage_tile<VEC>(a.X, a.y, t0, tr, a.d, a.dpad, xs, ys);
+    __syncthreads();
+    write_pos(ys, t0, tr, o.pos);
+    if (g < G && r < tr) {
+      const B2kFeatSmem xf{xs + (size_t)r * a.dpad};
+      for (int mi = g; mi < a.m; mi += G) {
+        const EvForest F = a.forests[mi];
+        const int64_t* off = a.off + F.off0;
+        const double* value = a.value + F.val0 + 1;
+        const B2kPNode* P = a.nodes + F.node0;
+        double raw1 = 0.0;
+        for (int t = 0; t < F.T; ++t) {
+          const int64_t ot = __ldg(off + t);
+          raw1 = __dadd_rn(raw1, __ldg(value + (ot + b2k_rf_leaf(P + ot, xf)) * F.V));
+        }
+        o.scores[mi * o.ld + t0 + r] = raw1;
+      }
+    }
+  }
+}
+
 // out [m][1 | NREG] = the CTAs' partials folded in CTA order
 template <bool CLS>
 __global__ void k_eval_fold(const double* __restrict__ part, int P, int m, double* __restrict__ out) {
@@ -422,10 +503,12 @@ std::string num(double v) {
   return b;
 }
 
-// The label rule of b2k_logreg_labels on y, with its messages; *C = max label + 1 (0 when n == 0).
-int check_labels(b2k_ctx* ctx, const float* y, int64_t n, int* C, cudaStream_t s) {
-  *C = 0;
-  if (n == 0) return B2K_OK;
+// y's least and largest finite values, least non-integer (inf: none) and whether any value is non-finite (n > 0).
+struct LabelStats {
+  double mn, mx, ni;
+  bool bad;
+};
+int label_stats(b2k_ctx* ctx, const float* y, int64_t n, LabelStats* st, cudaStream_t s) {
   const int spans = (int)std::max<int64_t>(1, std::min<int64_t>(4 * ctx->sm_count, (n + 1023) / 1024));
   const int64_t span_rows = (n + spans - 1) / spans;
   float* part;
@@ -446,7 +529,18 @@ int check_labels(b2k_ctx* ctx, const float* y, int64_t n, int* C, cudaStream_t s
     ni = std::min(ni, (double)h[i * 4 + 2]);
     bad = std::max(bad, (double)h[i * 4 + 3]);
   }
-  if (bad > 0.0) return b2k_fail(ctx, B2K_ERR_INVALID, "evaluation: the label holds a NaN or an infinity");
+  *st = LabelStats{mn, mx, ni, bad > 0.0};
+  return B2K_OK;
+}
+
+// The label rule of b2k_logreg_labels on y, with its messages; *C = max label + 1 (0 when n == 0).
+int check_labels(b2k_ctx* ctx, const float* y, int64_t n, int* C, cudaStream_t s) {
+  *C = 0;
+  if (n == 0) return B2K_OK;
+  LabelStats st;
+  B2K_TRY(label_stats(ctx, y, n, &st, s));
+  const double mn = st.mn, mx = st.mx, ni = st.ni;
+  if (st.bad) return b2k_fail(ctx, B2K_ERR_INVALID, "evaluation: the label holds a NaN or an infinity");
   if (mn < 0.0) return b2k_fail(ctx, B2K_ERR_INVALID, "Labels MUST be in [0, 2147483647), but got " + num(mn));
   if (std::isfinite(ni)) return b2k_fail(ctx, B2K_ERR_INVALID, "Labels MUST be Integers, but got " + num(ni));
   if (mx >= 2147483647.0) return b2k_fail(ctx, B2K_ERR_INVALID, "Labels MUST be in [0, 2147483647), but got " + num(mx));
@@ -519,7 +613,138 @@ int finish_chunk(b2k_ctx* ctx, bool cls, int first, int mc, int C, int64_t n, in
   return B2K_OK;
 }
 
+// The forests' table: F [m] and the totals of tree offsets (off0), nodes (node0) and values (val0) of all forests, and
+// the most values of one forest.  Each forest needs n_values >= min_values (and exactly 1 when min_values is 0).
+int forest_table(b2k_ctx* ctx, const char* who, int m, int d, int min_values, const int32_t* n_trees,
+                 const int32_t* n_values, const int64_t* tree_offsets, const int32_t* feature, std::vector<EvForest>& F,
+                 int64_t& off0, int64_t& node0, int64_t& val0, int& vmax) {
+  const std::string w = who;
+  for (int i = 0; i < m; ++i) {
+    if (n_trees[i] < 1 || n_values[i] < std::max(1, min_values) || (min_values == 0 && n_values[i] != 1))
+      return b2k_fail(ctx, B2K_ERR_INVALID, w + ": forest " + std::to_string(i) +
+                                                (min_values == 2 ? " needs n_trees >= 1 and n_values >= 2"
+                                                                 : " needs n_trees >= 1 and n_values >= 1 (1 for "
+                                                                   "regression)"));
+    const int64_t* off = tree_offsets + off0;
+    if (off[0] != 0)
+      return b2k_fail(ctx, B2K_ERR_INVALID, w + ": the tree offsets of forest " + std::to_string(i) + " must start at 0");
+    for (int t = 0; t < n_trees[i]; ++t)
+      if (off[t + 1] <= off[t])
+        return b2k_fail(ctx, B2K_ERR_INVALID, w + ": forest " + std::to_string(i) + " has an empty tree");
+    F[i] = EvForest{off0, node0, val0, n_trees[i], n_values[i]};
+    const int64_t nn = off[n_trees[i]];
+    for (int64_t j = 0; j < nn; ++j)
+      if (feature[node0 + j] >= d)
+        return b2k_fail(ctx, B2K_ERR_INVALID, w + ": a node splits on feature " + std::to_string(feature[node0 + j]) +
+                                                  " >= d = " + std::to_string(d));
+    off0 += n_trees[i] + 1;
+    node0 += nn;
+    val0 += nn * n_values[i];
+    vmax = std::max(vmax, n_values[i]);
+  }
+  return B2K_OK;
+}
+
+// The binary passes' label rule: y finite (any value; positive when > 0.5).
+int check_binary_labels(b2k_ctx* ctx, const float* y, int64_t n, cudaStream_t s) {
+  if (n == 0) return B2K_OK;
+  LabelStats st;
+  B2K_TRY(label_stats(ctx, y, n, &st, s));
+  if (st.bad) return b2k_fail(ctx, B2K_ERR_INVALID, "evaluation: the label holds a NaN or an infinity");
+  return B2K_OK;
+}
+
 }  // namespace
+
+int b2k_eval_linear_scores_impl(b2k_ctx* ctx, const float* X, const float* y, int64_t n, int d, int m,
+                                const int32_t* kind, const int32_t* row_offsets, const double* W, const double* b,
+                                double* scores, int64_t ld_scores, uint8_t* pos, cudaStream_t s) {
+  if (d > B2K_LOGREG_MAX_D)
+    return b2k_fail(ctx, B2K_ERR_UNSUPPORTED, "evaluation supports d <= " + std::to_string(B2K_LOGREG_MAX_D));
+  int nrows = 0;
+  for (int i = 0; i < m; ++i) {
+    const int kp = row_offsets[i + 1] - row_offsets[i];
+    if (!(kind[i] == B2K_EVAL_LOGISTIC ? kp == 1 : kind[i] == B2K_EVAL_SOFTMAX && kp >= 2) || row_offsets[i] != nrows)
+      return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_eval_linear_scores: model " + std::to_string(i) +
+                                                " has a bad kind or row range (logistic holds 1 row, softmax >= 2)");
+    nrows += kp;
+  }
+  B2K_TRY(check_binary_labels(ctx, y, n, s));
+  if (n == 0) return B2K_OK;
+  const int dpad = (d + 3) & ~3, L = b2k_row_lanes(d);
+  const int TR = tile_rows(dpad, EV_NW * (32 / L), EV_TILE_BYTES);
+  const bool vec = d % 4 == 0 && (reinterpret_cast<uintptr_t>(X) & 15u) == 0;
+  std::vector<double> Wp((size_t)nrows * dpad, 0.0);
+  for (int r = 0; r < nrows; ++r) std::copy(W + (size_t)r * d, W + (size_t)(r + 1) * d, Wp.begin() + (size_t)r * dpad);
+  const size_t smem = ev_carve(TR, dpad, 0, 0, false).bytes;
+  const void* kern = vec ? (const void*)k_score_linear<true> : (const void*)k_score_linear<false>;
+  int grid = 0;
+  B2K_TRY(pass_grid(ctx, kern, smem, n, TR, &grid));
+  int* row0_d;
+  double *W_d, *b_d;
+  B2K_TRY(b2k_scratch_layout(ctx, "binary scores", [&](B2kLayout& Ly) -> int {
+    row0_d = Ly.take<int>(m + 1);
+    W_d = Ly.take<double>((size_t)nrows * dpad);
+    b_d = Ly.take<double>(nrows);
+    return B2K_OK;
+  }));
+  B2K_CUDA_OK(ctx, cudaMemcpyAsync(row0_d, row_offsets, (m + 1) * 4, cudaMemcpyHostToDevice, s));
+  B2K_CUDA_OK(ctx, cudaMemcpyAsync(W_d, Wp.data(), Wp.size() * 8, cudaMemcpyHostToDevice, s));
+  B2K_CUDA_OK(ctx, cudaMemcpyAsync(b_d, b, (size_t)nrows * 8, cudaMemcpyHostToDevice, s));
+  LinArgs a{X, y, n, d, dpad, L, TR, m, 0, nullptr, row0_d, W_d, b_d, nullptr, nullptr, 0.0, nullptr, 1,
+            nullptr, nullptr, nullptr};
+  const ScoreOut o{scores, ld_scores, pos};
+  if (vec) k_score_linear<true><<<grid, EV_NT, smem, s>>>(a, o);
+  else k_score_linear<false><<<grid, EV_NT, smem, s>>>(a, o);
+  B2K_CUDA_OK(ctx, cudaGetLastError());
+  ctx->stats.kernel_launches++;
+  return B2K_OK;
+}
+
+int b2k_eval_forest_scores_impl(b2k_ctx* ctx, const float* X, const float* y, int64_t n, int d, int m,
+                                const int32_t* n_trees, const int32_t* n_values, const int64_t* tree_offsets,
+                                const int32_t* feature, const float* threshold, const int32_t* children,
+                                const double* value, double* scores, int64_t ld_scores, uint8_t* pos, cudaStream_t s) {
+  std::vector<EvForest> F(m);
+  int64_t off0 = 0, node0 = 0, val0 = 0;
+  int vmax = 1;
+  B2K_TRY(forest_table(ctx, "b2k_eval_forest_scores", m, d, 2, n_trees, n_values, tree_offsets, feature, F, off0,
+                       node0, val0, vmax));
+  B2K_TRY(check_binary_labels(ctx, y, n, s));
+  if (n == 0) return B2K_OK;
+  std::vector<B2kPNode> pn((size_t)node0);
+  for (int64_t j = 0; j < node0; ++j)
+    pn[j] = B2kPNode{feature[j], threshold[j], children[2 * j], children[2 * j + 1]};
+  const int dpad = (d + 3) & ~3;
+  const int TR = tile_rows(dpad, 1, EV_FTILE_BYTES);
+  const bool vec = d % 4 == 0 && (reinterpret_cast<uintptr_t>(X) & 15u) == 0;
+  const size_t smem = ev_carve(TR, dpad, 0, 0, false).bytes;
+  const void* kern = vec ? (const void*)k_score_forest<true> : (const void*)k_score_forest<false>;
+  int grid = 0;
+  B2K_TRY(pass_grid(ctx, kern, smem, n, TR, &grid));
+  EvForest* F_d;
+  int64_t* off_d;
+  B2kPNode* nodes_d;
+  double* val_d;
+  B2K_TRY(b2k_scratch_layout(ctx, "binary scores", [&](B2kLayout& Ly) -> int {
+    F_d = Ly.take<EvForest>(m);
+    off_d = Ly.take<int64_t>(off0);
+    nodes_d = Ly.take<B2kPNode>(node0);
+    val_d = Ly.take<double>(val0);
+    return B2K_OK;
+  }));
+  B2K_CUDA_OK(ctx, cudaMemcpyAsync(F_d, F.data(), m * sizeof(EvForest), cudaMemcpyHostToDevice, s));
+  B2K_CUDA_OK(ctx, cudaMemcpyAsync(off_d, tree_offsets, off0 * 8, cudaMemcpyHostToDevice, s));
+  B2K_CUDA_OK(ctx, cudaMemcpyAsync(nodes_d, pn.data(), node0 * sizeof(B2kPNode), cudaMemcpyHostToDevice, s));
+  B2K_CUDA_OK(ctx, cudaMemcpyAsync(val_d, value, val0 * 8, cudaMemcpyHostToDevice, s));
+  ForestArgs a{X, y, n, d, dpad, TR, m, 0, F_d, off_d, nodes_d, val_d, 0.0, nullptr, 1, nullptr, nullptr, nullptr};
+  const ScoreOut o{scores, ld_scores, pos};
+  if (vec) k_score_forest<true><<<grid, EV_NT, smem, s>>>(a, o);
+  else k_score_forest<false><<<grid, EV_NT, smem, s>>>(a, o);
+  B2K_CUDA_OK(ctx, cudaGetLastError());
+  ctx->stats.kernel_launches++;
+  return B2K_OK;
+}
 
 int b2k_eval_linear_impl(b2k_ctx* ctx, const float* X, const float* y, int64_t n, int d, int m, const int32_t* kind,
                          const int32_t* row_offsets, const double* W, const double* b, const double* class_values,
@@ -646,28 +871,8 @@ int b2k_eval_forest_impl(b2k_ctx* ctx, const float* X, const float* y, int64_t n
   std::vector<EvForest> F(m);
   int64_t off0 = 0, node0 = 0, val0 = 0;
   int vmax = 1;
-  for (int i = 0; i < m; ++i) {
-    if (n_trees[i] < 1 || n_values[i] < 1 || (!cls && n_values[i] != 1))
-      return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_eval_forest: forest " + std::to_string(i) +
-                                                " needs n_trees >= 1 and n_values >= 1 (1 for regression)");
-    const int64_t* off = tree_offsets + off0;
-    if (off[0] != 0)
-      return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_eval_forest: the tree offsets of forest " + std::to_string(i) +
-                                                " must start at 0");
-    for (int t = 0; t < n_trees[i]; ++t)
-      if (off[t + 1] <= off[t])
-        return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_eval_forest: forest " + std::to_string(i) + " has an empty tree");
-    F[i] = EvForest{off0, node0, val0, n_trees[i], n_values[i]};
-    const int64_t nn = off[n_trees[i]];
-    for (int64_t j = 0; j < nn; ++j)
-      if (feature[node0 + j] >= d)
-        return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_eval_forest: a node splits on feature " +
-                                                  std::to_string(feature[node0 + j]) + " >= d = " + std::to_string(d));
-    off0 += n_trees[i] + 1;
-    node0 += nn;
-    val0 += nn * n_values[i];
-    vmax = std::max(vmax, n_values[i]);
-  }
+  B2K_TRY(forest_table(ctx, "b2k_eval_forest", m, d, cls ? 1 : 0, n_trees, n_values, tree_offsets, feature, F, off0,
+                       node0, val0, vmax));
   int C = 0;
   if (cls) {
     B2K_TRY(check_labels(ctx, y, n, &C, s));

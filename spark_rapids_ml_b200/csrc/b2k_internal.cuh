@@ -470,3 +470,13 @@ int b2k_eval_forest_impl(b2k_ctx* ctx, const float* X, const float* y, int64_t n
                          const int32_t* feature, const float* threshold, const int32_t* children, const double* value,
                          int n_classes, double eps, int64_t* label_count_out, int64_t* tp_out, int64_t* fp_out,
                          double* loss_out, double* reg_out, cudaStream_t s);
+int b2k_eval_linear_scores_impl(b2k_ctx* ctx, const float* X, const float* y, int64_t n, int d, int m,
+                                const int32_t* kind, const int32_t* row_offsets, const double* W, const double* b,
+                                double* scores, int64_t ld_scores, uint8_t* pos, cudaStream_t s);
+int b2k_eval_forest_scores_impl(b2k_ctx* ctx, const float* X, const float* y, int64_t n, int d, int m,
+                                const int32_t* n_trees, const int32_t* n_values, const int64_t* tree_offsets,
+                                const int32_t* feature, const float* threshold, const int32_t* children,
+                                const double* value, double* scores, int64_t ld_scores, uint8_t* pos, cudaStream_t s);
+// b2k_binary.cu
+int b2k_eval_binary_impl(b2k_ctx* ctx, const double* scores, const uint8_t* pos, int64_t n, int m, int num_bins,
+                         int metric, double* out, cudaStream_t s);

@@ -1,5 +1,6 @@
 """Multiclass and regression metrics from per-model accumulators, written from Spark's MulticlassMetrics and
-RegressionMetrics definitions (unit weights).
+RegressionMetrics definitions (unit weights), and the binary metrics (areaUnderROC, areaUnderPR) of Spark's
+BinaryClassificationMetrics from scores and labels (binary_metric).
 
 The accumulators are what the device evaluation pass (Context.eval_linear / eval_forest) returns, and what the local
 evaluators form from a frame's columns on the host:
@@ -23,6 +24,7 @@ MULTICLASS_METRICS = ("f1", "accuracy", "weightedPrecision", "weightedRecall", "
                       "falsePositiveRateByLabel", "precisionByLabel", "recallByLabel", "fMeasureByLabel", "hammingLoss",
                       "logLoss")
 REGRESSION_METRICS = ("rmse", "mse", "r2", "mae", "var")
+BINARY_METRICS = ("areaUnderROC", "areaUnderPR")
 
 
 def _div(a: float, b: float) -> float:
@@ -191,3 +193,47 @@ def merge_all(accs: List[Dict[str, Any]], classification: bool) -> Dict[str, Any
     for a in accs[1:]:
         out = merge_class(out, a) if classification else merge_reg(out, a)
     return out
+
+
+# ---- binary ----
+def _descending_key(scores: np.ndarray) -> np.ndarray:
+    """uint64 keys whose ascending order is Java's Double.compare order descending: NaN (one value) first, then +inf
+    down to -inf, +0.0 before -0.0."""
+    b = np.where(np.isnan(scores), np.uint64(0x7FF8000000000000), np.ascontiguousarray(scores).view(np.uint64))
+    neg = (b >> np.uint64(63)) == 1
+    asc = np.where(neg, ~b, b | np.uint64(1 << 63))
+    return ~asc
+
+
+def binary_metric(scores: Any, labels: Any, metric: str, num_bins: int) -> float:
+    """Spark's BinaryClassificationMetrics(scoreAndLabels, numBins).areaUnderROC / areaUnderPR with unit weights, the
+    whole ordered list of distinct scores as one partition (include/b2kmeans.h "binary evaluation" states the rule).
+    A row is positive when its label > 0.5."""
+    if metric not in BINARY_METRICS:
+        raise ValueError(f"Unsupported metric name, found {metric}")
+    s = np.asarray(scores, dtype=np.float64).reshape(-1)
+    pos = np.asarray(labels, dtype=np.float64).reshape(-1) > 0.5
+    if s.size == 0:
+        raise ValueError("binary metrics need at least one row")
+    key = _descending_key(s)
+    order = np.argsort(key, kind="stable")
+    key, cpos = key[order], np.cumsum(pos[order])
+    starts = np.flatnonzero(np.r_[True, key[1:] != key[:-1]])   # first row of each distinct score
+    g = len(starts) // num_bins if num_bins > 0 else 0
+    if g >= 2:
+        starts = starts[::g]
+    last = np.r_[starts[1:], s.size] - 1                        # last row of each point
+    tp = cpos[last].astype(np.float64)
+    fp = (last + 1).astype(np.float64) - tp
+    P = float(cpos[-1])
+    N = float(s.size) - P
+    recall = tp / P if P > 0 else np.zeros_like(tp)
+    if metric == "areaUnderROC":
+        x = np.r_[0.0, fp / N if N > 0 else np.zeros_like(fp), 1.0]
+        y = np.r_[0.0, recall, 1.0]
+    else:
+        with np.errstate(invalid="ignore"):
+            precision = np.where(tp + fp == 0, 1.0, tp / (tp + fp))
+        x = np.r_[0.0, recall]
+        y = np.r_[precision[0], precision]
+    return float(np.sum((x[1:] - x[:-1]) * (y[1:] + y[:-1]) / 2.0))

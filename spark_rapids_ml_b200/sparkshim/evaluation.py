@@ -1,6 +1,6 @@
-"""Local stand-ins for pyspark.ml.evaluation's MulticlassClassificationEvaluator and RegressionEvaluator: Spark's params,
-defaults and isLargerBetter(); evaluate() of a local frame reads the label, prediction (and probability) columns and
-computes in fp64 on the host (spark_rapids_ml_b200.metrics)."""
+"""Local stand-ins for pyspark.ml.evaluation's MulticlassClassificationEvaluator, RegressionEvaluator and
+BinaryClassificationEvaluator: Spark's params, defaults and isLargerBetter(); evaluate() of a local frame reads the
+label, prediction (probability, rawPrediction) columns and computes in fp64 on the host (spark_rapids_ml_b200.metrics)."""
 from __future__ import annotations
 
 from typing import Any, Dict, Optional
@@ -135,3 +135,60 @@ class RegressionEvaluator(_Evaluator):
         y = np.asarray(self._column(dataset, self.getLabelCol()), dtype=np.float64)
         p = np.asarray(self._column(dataset, self.getPredictionCol()), dtype=np.float64)
         return metrics.regression_metric(metrics.reg_accumulators(y, p), name, self.getThroughOrigin())
+
+
+class BinaryClassificationEvaluator(_Evaluator):
+    """pyspark.ml.evaluation.BinaryClassificationEvaluator: metricName ("areaUnderROC" default, or "areaUnderPR"),
+    rawPredictionCol ("rawPrediction"), numBins (1000, >= 0).  The score of a row is element 1 of a vector
+    rawPrediction, or the value of a double one; the row is positive when its label > 0.5.  Spark down-samples the
+    curve to numBins points per partition of its sorted scores; here the whole ordered list is one partition, so with
+    numBins > 0 and more than 2 numBins distinct scores the value can differ from Spark's on a multi-partition RDD."""
+
+    rawPredictionCol = Param("parent", "rawPredictionCol", "raw prediction (a.k.a. confidence) column name.",
+                             TypeConverters.toString)
+    numBins = Param("parent", "numBins", "Number of bins to down-sample the curves (ROC curve, PR curve) in area "
+                    "computation. If 0, no down-sampling will occur. Must be >= 0.", TypeConverters.toInt)
+
+    @keyword_only
+    def __init__(self, *, rawPredictionCol: str = "rawPrediction", labelCol: str = "label",
+                 metricName: str = "areaUnderROC", weightCol: Optional[str] = None, numBins: int = 1000) -> None:
+        self._init({})
+        self._setDefault(metricName="areaUnderROC", rawPredictionCol="rawPrediction", numBins=1000)
+        self._set(**{k: v for k, v in self._input_kwargs.items() if v is not None})
+
+    def _set(self, **kwargs: Any) -> "BinaryClassificationEvaluator":
+        if kwargs.get("numBins") is not None and TypeConverters.toInt(kwargs["numBins"]) < 0:
+            raise ValueError(f"numBins must be >= 0, got {kwargs['numBins']}")
+        return super()._set(**kwargs)
+
+    def getRawPredictionCol(self) -> str:
+        return self.getOrDefault("rawPredictionCol")
+
+    def setRawPredictionCol(self, value: str) -> "BinaryClassificationEvaluator":
+        return self._set(rawPredictionCol=value)
+
+    def getNumBins(self) -> int:
+        return int(self.getOrDefault("numBins"))
+
+    def setNumBins(self, value: int) -> "BinaryClassificationEvaluator":
+        return self._set(numBins=value)
+
+    def isLargerBetter(self) -> bool:
+        return True
+
+    def _evaluate(self, dataset: Any) -> float:
+        from .. import metrics
+
+        name = self.getMetricName()
+        if name not in metrics.BINARY_METRICS:
+            raise ValueError(f"Unsupported metric name, found {name}")
+        y = np.asarray(self._column(dataset, self.getLabelCol()), dtype=np.float64)
+        raw = list(self._column(dataset, self.getRawPredictionCol()))
+        if raw and np.ndim(raw[0]) == 0:
+            s = np.asarray(raw, dtype=np.float64)
+        else:
+            if any(len(v) < 2 for v in raw):
+                raise ValueError(f"{self.getRawPredictionCol()} holds a vector of fewer than 2 elements: the binary "
+                                 "score is element 1")
+            s = np.asarray([v[1] for v in raw], dtype=np.float64)
+        return metrics.binary_metric(s, y, name, self.getNumBins())

@@ -599,7 +599,8 @@ class _RandomForestModel(_RandomForestClass, _CumlModelWithPredictionCol, _Rando
 
     def _eval_func(self, info: Dict[str, Any]) -> Tuple[Callable, Any, Callable]:
         """(construct, None, evaluate): evaluate(holder, X, y) scores every forest of this (combined) model in one
-        device pass (b2k_eval_forest) and returns their accumulators."""
+        device pass (b2k_eval_forest) and returns their accumulators; for a BinaryClassificationEvaluator,
+        evaluate(holder, X, y, scores, pos, row0) writes their binary scores (b2k_eval_forest_scores) instead."""
         from .core import _class_accs
 
         classification = self._is_classification()
@@ -614,6 +615,13 @@ class _RandomForestModel(_RandomForestClass, _CumlModelWithPredictionCol, _Rando
         class _Holder:
             def __init__(self, gpu: int) -> None:
                 self.ctx = _transform_context(gpu)
+
+        if info["binary"]:
+            def _scores(h: Any, X: Any, y: Any, scores: Any, pos: Any, row0: int) -> None:
+                h.ctx.binary_scores_forest(X, y, forests, scores, pos, row0)
+
+            _scores.n_models = len(forests)  # type: ignore[attr-defined]
+            return _Holder, None, _scores
 
         def _evaluate(h: Any, X: Any, y: Any) -> List[Dict[str, Any]]:
             return _class_accs(h.ctx.eval_forest(X, y, forests, classification, eps))
