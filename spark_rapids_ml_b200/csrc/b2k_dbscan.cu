@@ -30,28 +30,15 @@
 namespace {
 #include "b2k_ptx.cuh"
 #include "b2k_knn_prep.cuh"
+#include "b2k_pair_wg.cuh"
 
-constexpr int DB_TM = 128;       // local rows per tile (two consumer warpgroups x wgmma M = 64)
-constexpr int DB_N = 128;        // rows per column block (wgmma N)
-constexpr int DB_CHUNK = 32;     // f32 per 128-byte swizzle row
-constexpr int DB_NTHREADS = 384; // 8 consumer warps + a producer warpgroup (one warp issues)
 constexpr int DB_SMAX = 4096;    // column splits
 constexpr int DB_NONE = 0x7fffffff;
+constexpr int DB_SNAP = 2 * PW_N * 4 + 2 * PW_N;   // [2][128] column roots, [2][128] column core flags
 
-template <int NCH>
-struct DbWgCfg {
-  static constexpr int QBYTES = DB_TM * DB_CHUNK * 4;   // one row chunk: 16 KB
-  static constexpr int CBYTES = DB_N * DB_CHUNK * 4;    // one column chunk plane: 16 KB
-  static constexpr int SC = 2;                          // column stages of (hi, lo)
-  static constexpr int OFF_Q = 0;
-  static constexpr int OFF_C = OFF_Q + NCH * QBYTES;
-  static constexpr int OFF_SNAP = OFF_C + SC * 2 * CBYTES;   // [2][128] column roots, [2][128] column core flags
-  static constexpr int OFF_BAR = OFF_SNAP + 2 * DB_N * 4 + 2 * DB_N;
-  static constexpr int SMEM_BYTES = OFF_BAR + 8 * (2 + 2 * SC);
-  static_assert(OFF_C % 1024 == 0 && CBYTES % 1024 == 0, "swizzle atoms need 1 KB alignment");
-  static_assert(SMEM_BYTES + 1024 <= 227 * 1024, "smem");
-};
 // d = 128: row tile 64 KB + two column stages 64 KB + snapshots 1.25 KB
+template <int NCH>
+using DbWgCfg = PairWgCfg<NCH, DB_SNAP>;
 static_assert(DbWgCfg<4>::SMEM_BYTES == 128 * 1024 + 1280 + 48, "d = 128 layout");
 
 struct DbArgs {
@@ -120,9 +107,7 @@ __device__ __forceinline__ int db_unite(int* parent, int a, int b) {
 __device__ __forceinline__ void db_bar_consumers() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
 // Persistent grid, static round-robin over units u = tile * S + split: tile = 128 local rows, split = a range of the
-// column blocks of all rows.  Producer and 3xTF32 main loop as k_knn_wg (b2k_knn.cu): warp 8 loads the unit's row tile
-// once and the split's column blocks (hi, lo planes) chunk by chunk through an SC-stage ring; consumer warpgroup g
-// accumulates lo.Xhi^T + hi.Xlo^T + hi.Xhi^T for rows [64 g, 64 g + 64) with the row split in registers.
+// column blocks of all rows.  Producer and 3xTF32 main loop of b2k_pair_wg.cuh, as k_knn_wg.
 // The epilogue decides every (row, column) pair of the block with the screen and, in the band, the fp64 rule:
 //   UNION = false  counts adjacent columns per row (integer atomics once per unit);
 //   UNION = true   columns that are not core are skipped (so are blocks with no core row, by both roles); for a core
@@ -131,70 +116,37 @@ __device__ __forceinline__ void db_bar_consumers() { asm volatile("bar.sync 1, 2
 //                  block; both only ever lag the truth by merges, so equal values mean one set.  A non-core row keeps
 //                  the lowest adjacent core column and records it with atomicMin once per unit.
 template <int NCH, bool UNION>
-__global__ void __launch_bounds__(DB_NTHREADS, 1)
+__global__ void __launch_bounds__(PW_NTHREADS, 1)
 k_db_wg(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapHi,
         const __grid_constant__ CUtensorMap mapLo, const DbArgs args) {
   using G = DbWgCfg<NCH>;
-  constexpr int R = DB_N / 2;
+  constexpr int R = PW_N / 2;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   const uint32_t base = smem_u32(smem_raw);
-  if ((base & 1023u) != 0u) __trap();   // 128B-swizzle atoms need a 1 KB aligned base
-  const uint32_t bars = base + G::OFF_BAR;
-  const uint32_t qfull = bars, qempty = bars + 8u;
-  auto cfull = [&](int s) -> uint32_t { return bars + 16u + 8u * (uint32_t)s; };
-  auto cempty = [&](int s) -> uint32_t { return bars + 16u + 8u * (uint32_t)(G::SC + s); };
-  int* sroot = reinterpret_cast<int*>(smem_raw + G::OFF_SNAP);                    // [2][128]
-  uint8_t* score = smem_raw + G::OFF_SNAP + 2 * DB_N * 4;                         // [2][128]
+  const PairWgBars bars = pair_wg_init<G>(base);
+  int* sroot = reinterpret_cast<int*>(smem_raw + G::OFF_OWN);                     // [2][128]
+  uint8_t* score = smem_raw + G::OFF_OWN + 2 * PW_N * 4;                          // [2][128]
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (threadIdx.x == 0) {
-    mbar_init(qfull, 1);
-    mbar_init(qempty, 8);
-    for (int s = 0; s < G::SC; ++s) {
-      mbar_init(cfull(s), 1);
-      mbar_init(cempty(s), 8);
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncthreads();
   const int nunits = args.ntiles * args.S;
   const int nit = (int)blockIdx.x < nunits ? (nunits - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
 
   if (warp >= 8) {
-    if (warp == 8 && elect_one()) {
-      tma_prefetch_desc(&mapQ);
-      tma_prefetch_desc(&mapHi);
-      tma_prefetch_desc(&mapLo);
-      int q = 0;
-      for (int it = 0; it < nit; ++it) {
-        const int u = (int)blockIdx.x + it * (int)gridDim.x;
-        const int tile = u / args.S, split = u % args.S;
-        const int b0 = (int)((int64_t)split * args.nblk / args.S), b1 = (int)((int64_t)(split + 1) * args.nblk / args.S);
-        mbar_wait_nocall(qempty, (uint32_t)((it & 1) ^ 1));
-        mbar_expect_tx(qfull, (uint32_t)(NCH * G::QBYTES));
-        for (int c = 0; c < NCH; ++c)
-          tma_load_2d(base + (uint32_t)(G::OFF_Q + c * G::QBYTES), &mapQ, qfull, c * DB_CHUNK, tile * DB_TM);
-        for (int b = b0; b < b1; ++b) {
-          if (UNION && !args.blk_core[b]) continue;
-#pragma unroll 1
-          for (int c = 0; c < NCH; ++c, ++q) {
-            const int cs = q % G::SC;
-            mbar_wait_nocall(cempty(cs), (uint32_t)((q / G::SC) & 1) ^ 1u);
-            const uint32_t dst = base + (uint32_t)(G::OFF_C + cs * 2 * G::CBYTES);
-            mbar_expect_tx(cfull(cs), (uint32_t)(2 * G::CBYTES));
-            tma_load_2d(dst, &mapHi, cfull(cs), c * DB_CHUNK, b * DB_N);
-            tma_load_2d(dst + G::CBYTES, &mapLo, cfull(cs), c * DB_CHUNK, b * DB_N);
-          }
-        }
-      }
-    }
+    if (warp == 8 && elect_one())
+      pair_wg_produce<G>(
+          base, bars, &mapQ, &mapHi, &mapLo, nit,
+          [&](int it) {
+            const int u = (int)blockIdx.x + it * (int)gridDim.x;
+            const int tile = u / args.S, split = u % args.S;
+            return PairWgUnit{tile * PW_TM, (int)((int64_t)split * args.nblk / args.S),
+                              (int)((int64_t)(split + 1) * args.nblk / args.S)};
+          },
+          [&](int b) { return UNION && !args.blk_core[b]; });   // the consumers skip the same blocks
     __syncwarp();
     return;
   }
 
   const int g = warp >> 2, wi = warp & 3;
   const int rr0 = g * 64 + wi * 16 + (lane >> 2);   // this thread's rows rr0, rr0 + 8 of the tile
-  const uint32_t arow = (uint32_t)rr0 * 128u + (uint32_t)(lane & 3) * 4u;
-  const uint32_t asw = (uint32_t)(lane >> 2);
   float acc[R];
   int q = 0, par = 0;
   unsigned long long n_band = 0, n_union = 0;
@@ -208,7 +160,7 @@ k_db_wg(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtens
     int cnt[2] = {0, 0}, rootI[2] = {0, 0}, bm[2] = {DB_NONE, DB_NONE};
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      lrow[h] = (int64_t)tile * DB_TM + rr0 + 8 * h;
+      lrow[h] = (int64_t)tile * PW_TM + rr0 + 8 * h;
       grow[h] = args.row0 + lrow[h];
       vrow[h] = lrow[h] < args.n_local;
       ni[h] = vrow[h] ? __ldg(args.norms + grow[h]) : 0.f;
@@ -217,54 +169,17 @@ k_db_wg(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtens
         rootI[h] = (int)grow[h];
       }
     }
-    mbar_wait_nocall(qfull, (uint32_t)(it & 1));
+    mbar_wait_nocall(bars.qfull(), (uint32_t)(it & 1));
     for (int b = b0; b < b1; ++b) {
-      if (UNION && !args.blk_core[b]) continue;
-#pragma unroll
-      for (int c = 0; c < NCH; ++c, ++q) {
-        const int cs = q % G::SC;
-        const uint8_t* xp = smem_raw + G::OFF_Q + c * G::QBYTES;
-        const uint32_t cst = base + (uint32_t)(G::OFF_C + cs * 2 * G::CBYTES);
-        // v = hi + lo, hi = RN_tf32(v), lo = RN_tf32(v - hi), in registers
-        uint32_t ah[DB_CHUNK / 8][4], al[DB_CHUNK / 8][4];
-#pragma unroll
-        for (int ks = 0; ks < DB_CHUNK / 8; ++ks) {
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {   // row rr0 + 8 (e & 1), column 8 ks + lane % 4 + 4 (e >> 1)
-            const uint32_t unit = (uint32_t)(2 * ks + (e >> 1));
-            const float v = *reinterpret_cast<const float*>(xp + arow + (uint32_t)(e & 1) * 1024u + ((unit ^ asw) << 4));
-            ah[ks][e] = rn_tf32_bits(v);
-            al[ks][e] = rn_tf32_bits(v - __uint_as_float(ah[ks][e]));
-          }
-        }
-#pragma unroll
-        for (int ks = 0; ks < DB_CHUNK / 8; ++ks) {
-          reg_fence(ah[ks]);
-          reg_fence(al[ks]);
-        }
-        mbar_wait_nocall(cfull(cs), (uint32_t)((q / G::SC) & 1));
-        wgmma_fence();
-#pragma unroll
-        for (int ks = 0; ks < DB_CHUNK / 8; ++ks) {
-          const uint64_t dh = make_kmajor_sw128_desc(cst + ks * 32);
-          const uint64_t dl = make_kmajor_sw128_desc(cst + G::CBYTES + ks * 32);
-          wgmma_tf32_rs<DB_N>(acc, al[ks], dh, (c | ks) != 0 ? 1u : 0u);   // small terms first
-          wgmma_tf32_rs<DB_N>(acc, ah[ks], dl, 1u);
-          wgmma_tf32_rs<DB_N>(acc, ah[ks], dh, 1u);
-        }
-        wgmma_commit();
-        wgmma_wait0();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(cempty(cs));
-      }
-      reg_fence(acc);
+      if (UNION && !args.blk_core[b]) continue;   // as the producer
+      pair_wg_block<G>(smem_raw, base, bars, rr0, lane, acc, q);
       if (UNION) {   // snapshot of the block's column roots and core flags; double-buffered, one barrier per block
         const int t = threadIdx.x;
-        if (t < DB_N) {
-          const int64_t col = (int64_t)b * DB_N + t;
+        if (t < PW_N) {
+          const int64_t col = (int64_t)b * PW_N + t;
           const bool c = col < args.n_total && args.core[col] != 0;
-          score[par * DB_N + t] = c;
-          sroot[par * DB_N + t] = c ? db_find(args.parent, (int)col) : -1;
+          score[par * PW_N + t] = c;
+          sroot[par * PW_N + t] = c ? db_find(args.parent, (int)col) : -1;
         }
 #pragma unroll
         for (int h = 0; h < 2; ++h)
@@ -273,16 +188,16 @@ k_db_wg(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtens
       }
       // ---- epilogue: acc[i] is row rr0 + 8 ((i >> 1) & 1), block column 8 (i >> 2) + 2 (lane & 3) + (i & 1) ----
       const int cb = 2 * (lane & 3);
-      const float* nb = args.norms + (size_t)b * DB_N + cb;
+      const float* nb = args.norms + (size_t)b * PW_N + cb;
 #pragma unroll
       for (int i = 0; i < R; ++i) {
         const int h = (i >> 1) & 1;
         const int cl = 8 * (i >> 2) + cb + (i & 1);
-        const int64_t col = (int64_t)b * DB_N + cl;
+        const int64_t col = (int64_t)b * PW_N + cl;
         if (!vrow[h] || col >= args.n_total) continue;
         if (UNION) {
-          if (!score[par * DB_N + cl]) continue;
-          if (coreI[h] ? rootI[h] == sroot[par * DB_N + cl] : col >= bm[h]) continue;
+          if (!score[par * PW_N + cl]) continue;
+          if (coreI[h] ? rootI[h] == sroot[par * PW_N + cl] : col >= bm[h]) continue;
         }
         const float nj = __ldg(nb + 8 * (i >> 2) + (i & 1));
         const float S = fmaf(-2.f, acc[i], nj) + ni[h];
@@ -301,7 +216,7 @@ k_db_wg(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtens
         if (!UNION) {
           ++cnt[h];
         } else if (coreI[h]) {
-          rootI[h] = db_unite(args.parent, rootI[h], sroot[par * DB_N + cl]);
+          rootI[h] = db_unite(args.parent, rootI[h], sroot[par * PW_N + cl]);
           ++n_union;
         } else {
           bm[h] = (int)col;
@@ -310,7 +225,7 @@ k_db_wg(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtens
       par ^= 1;
     }
     __syncwarp();
-    if (lane == 0) mbar_arrive(qempty);   // every A fragment of this unit has been read
+    if (lane == 0) mbar_arrive(bars.qempty());   // every A fragment of this unit has been read
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       if (!UNION) {   // the quad's four lanes hold the same row
@@ -617,45 +532,6 @@ __global__ void __launch_bounds__(256) k_db_labels(const int* __restrict__ paren
   }
 }
 
-struct Timer {   // CUDA events around the device phases when option time_kernels is set
-  cudaEvent_t ev[5] = {};
-  bool on = false;
-  explicit Timer(bool enable) : on(enable) {
-    if (on)
-      for (auto& e : ev) cudaEventCreate(&e);
-  }
-  ~Timer() {
-    if (on)
-      for (auto& e : ev) cudaEventDestroy(e);
-  }
-  void mark(int i, cudaStream_t s) {
-    if (on) cudaEventRecord(ev[i], s);
-  }
-  double ms(int a, int b) const {
-    float t = 0.f;
-    if (on) cudaEventElapsedTime(&t, ev[a], ev[b]);
-    return (double)t;
-  }
-};
-
-template <int NCH, bool UNION>
-int launch_wg(b2k_ctx* ctx, int grid, const CUtensorMap& mq, const CUtensorMap& mh, const CUtensorMap& ml,
-              const DbArgs& a, cudaStream_t s) {
-  const int smem = DbWgCfg<NCH>::SMEM_BYTES;
-  B2K_CUDA_OK(ctx, cudaFuncSetAttribute(k_db_wg<NCH, UNION>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  k_db_wg<NCH, UNION><<<grid, DB_NTHREADS, smem, s>>>(mq, mh, ml, a);
-  B2K_CUDA_OK(ctx, cudaGetLastError());
-  return B2K_OK;
-}
-
-template <bool UNION>
-int launch_wg_dp(b2k_ctx* ctx, int DP, int grid, const CUtensorMap& mq, const CUtensorMap& mh, const CUtensorMap& ml,
-                 const DbArgs& a, cudaStream_t s) {
-  if (DP == 32) return launch_wg<1, UNION>(ctx, grid, mq, mh, ml, a, s);
-  if (DP == 64) return launch_wg<2, UNION>(ctx, grid, mq, mh, ml, a, s);
-  return launch_wg<4, UNION>(ctx, grid, mq, mh, ml, a, s);
-}
-
 unsigned grid_1d(int64_t n, int sm) { return (unsigned)std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, (int64_t)sm * 16)); }
 }  // namespace
 
@@ -689,7 +565,7 @@ static void b2k_dbscan_bound(int d, int metric, double E, float* coef, float* B0
 int b2k_dbscan_fit_impl(b2k_ctx* ctx, const float* X, int64_t n_local, int d, double eps, int min_samples, int metric,
                         int32_t* labels_out, uint8_t* core_out, int64_t* n_clusters_out, cudaStream_t s) {
   const int nr = ctx->nranks;
-  Timer tm(ctx->time_kernels != 0);
+  B2kTimer tm(ctx->time_kernels != 0);
   // ---- sizes and input checks of every rank; each error is decided on them, identically on every rank ----
   constexpr int NS = 4;   // n_local, d, non-finite values, zero rows
   int64_t* sz_dev;
@@ -743,17 +619,17 @@ int b2k_dbscan_fit_impl(b2k_ctx* ctx, const float* X, int64_t n_local, int d, do
   // ---- plan ----
   const double E = metric == 0 ? eps * eps : 2.0 * eps;
   const bool x_aligned = nr > 1 || (reinterpret_cast<uintptr_t>(X) & 15u) == 0;
-  const bool wg_ok = d % 4 == 0 && d >= 4 && d <= 128 && x_aligned && E < 1e30;
+  const bool wg_ok = b2k_knn_wg_width(d) && x_aligned && E < 1e30;
   if (ctx->kernel_path == B2K_PATH_FUSED && !wg_ok)
     return b2k_fail(ctx, B2K_ERR_UNSUPPORTED, "kernel_path=2 requested but the wgmma DBSCAN pass needs d % 4 == 0, "
                                               "4 <= d <= 128 and 16-byte aligned X (d = " + std::to_string(d) + ")");
   const bool wg = wg_ok && ctx->kernel_path != B2K_PATH_GENERIC;
   int sm = ctx->sm_count;
   if (ctx->grid_limit > 0 && ctx->grid_limit < sm) sm = ctx->grid_limit;
-  const int DP = d <= 32 ? 32 : d <= 64 ? 64 : 128;
-  const int64_t nblk = wg ? (n_total + DB_N - 1) / DB_N : (n_total + GCL - 1) / GCL;
-  const int64_t n_pad = ((n_total + DB_N - 1) / DB_N) * DB_N;
-  const int64_t ntiles = wg ? (n_local + DB_TM - 1) / DB_TM : (n_local + GR - 1) / GR;
+  const int DP = b2k_knn_wg_dp(d);
+  const int64_t nblk = wg ? (n_total + PW_N - 1) / PW_N : (n_total + GCL - 1) / GCL;
+  const int64_t n_pad = ((n_total + PW_N - 1) / PW_N) * PW_N;
+  const int64_t ntiles = wg ? (n_local + PW_TM - 1) / PW_TM : (n_local + GR - 1) / GR;
   // column splits: at least about 2 units per SM, at most one block per split
   const int S = (int)std::max<int64_t>(
       1, std::min<int64_t>({(2 * (int64_t)sm + std::max<int64_t>(ntiles, 1) - 1) / std::max<int64_t>(ntiles, 1), nblk,
@@ -836,27 +712,13 @@ int b2k_dbscan_fit_impl(b2k_ctx* ctx, const float* X, int64_t n_local, int d, do
   a.parent = parent;
   a.bmin = bmin;
   a.stat = ctx->collect_recheck ? stat : nullptr;
-  CUtensorMap mq, mh, ml;
+  PairWgMaps maps;
   if (wg) {
     const float* src = metric == 1 ? Y : Xall;   // shifted by its global row 0
-    k_knn_prep<<<(unsigned)((n_pad * 32 + 255) / 256), 256, 0, s>>>(src, n_total, d, nullptr, n_pad, DP, Xhi, Xlo,
-                                                                         norms);
-    B2K_CUDA_OK(ctx, cudaGetLastError());
-    ctx->stats.kernel_launches++;
-    if (n_local > 0) {
-      const int64_t n4 = n_local * d / 4;
-      k_knn_shift_q<<<(unsigned)std::min<int64_t>((n4 + 255) / 256, (int64_t)gsm * 16), 256, 0, s>>>(
-          reinterpret_cast<const float4*>(src + (size_t)row0 * d), n4, d, src, reinterpret_cast<float4*>(Vs));
-      B2K_CUDA_OK(ctx, cudaGetLastError());
-      ctx->stats.kernel_launches++;
-    }
+    B2K_TRY(b2k_knn_prep_launch(ctx, src, n_total, d, nullptr, n_pad, DP, Xhi, Xlo, norms, s));
+    B2K_TRY(b2k_knn_shift_launch(ctx, src + (size_t)row0 * d, n_local, d, src, Vs, s));
     a.norms = norms;
-    B2K_TRY(b2k_encode_2d(ctx, &mq, Vs, (uint64_t)d, (uint64_t)std::max<int64_t>(n_local, 1), (uint64_t)d * 4, DB_CHUNK,
-                          DB_TM, CU_TENSOR_MAP_L2_PROMOTION_L2_256B));
-    B2K_TRY(b2k_encode_2d(ctx, &mh, Xhi, (uint64_t)DP, (uint64_t)n_pad, (uint64_t)DP * 4, DB_CHUNK, DB_N,
-                          CU_TENSOR_MAP_L2_PROMOTION_L2_256B));
-    B2K_TRY(b2k_encode_2d(ctx, &ml, Xlo, (uint64_t)DP, (uint64_t)n_pad, (uint64_t)DP * 4, DB_CHUNK, DB_N,
-                          CU_TENSOR_MAP_L2_PROMOTION_L2_256B));
+    B2K_TRY(pair_wg_maps(ctx, Vs, std::max<int64_t>(n_local, 1), d, Xhi, Xlo, n_pad, DP, &maps));
   }
   const int grid = (int)std::min<int64_t>(sm, ntiles * S);
   tm.mark(1, s);
@@ -864,7 +726,8 @@ int b2k_dbscan_fit_impl(b2k_ctx* ctx, const float* X, int64_t n_local, int d, do
   // ---- count pass ----
   if (ntiles > 0) {
     if (wg) {
-      B2K_TRY(launch_wg_dp<false>(ctx, DP, grid, mq, mh, ml, a, s));
+      B2K_TRY(pair_wg_launch<DB_SNAP>(
+          ctx, DP, [](auto nch) { return k_db_wg<decltype(nch)::value, false>; }, grid, maps, a, s));
       ctx->stats.fused_tc_launches++;
     } else {
       if (metric == 1) k_db_generic<false, true><<<(unsigned)(ntiles * S), G_NTHREADS, 0, s>>>(a);
@@ -895,14 +758,15 @@ int b2k_dbscan_fit_impl(b2k_ctx* ctx, const float* X, int64_t n_local, int d, do
     B2K_CUDA_OK(ctx, cudaGetLastError());
     ctx->stats.kernel_launches++;
   }
-  k_db_blk_core<<<grid_1d(nblk, gsm), 256, 0, s>>>(core, n_total, wg ? DB_N : GCL, nblk, blk);
+  k_db_blk_core<<<grid_1d(nblk, gsm), 256, 0, s>>>(core, n_total, wg ? PW_N : GCL, nblk, blk);
   B2K_CUDA_OK(ctx, cudaGetLastError());
   ctx->stats.kernel_launches++;
 
   // ---- union pass ----
   if (ntiles > 0) {
     if (wg) {
-      B2K_TRY(launch_wg_dp<true>(ctx, DP, grid, mq, mh, ml, a, s));
+      B2K_TRY(pair_wg_launch<DB_SNAP>(
+          ctx, DP, [](auto nch) { return k_db_wg<decltype(nch)::value, true>; }, grid, maps, a, s));
       ctx->stats.fused_tc_launches++;
     } else {
       if (metric == 1) k_db_generic<true, true><<<(unsigned)(ntiles * S), G_NTHREADS, 0, s>>>(a);

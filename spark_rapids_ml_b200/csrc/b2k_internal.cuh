@@ -335,13 +335,17 @@ struct KnnUnit {
   int row0, nrows;
   int lo, hi;
 };
-// true when the wgmma pass takes the shape (d % 4 == 0, 4 <= d <= 128, k <= 64); the padded width DP it then uses
+// true when the wgmma pair-distance pipeline (b2k_pair_wg.cuh: k-NN, IVF-Flat, DBSCAN) takes the width (d % 4 == 0,
+// 4 <= d <= 128); true when the k-NN wgmma pass takes the shape (that width and k <= 64); the padded width DP they use
+bool b2k_knn_wg_width(int d);
 bool b2k_knn_wg_shape(int d, int k);
 int b2k_knn_wg_dp(int d);
 // index planes of x - s for the wgmma pass, s = X row 0: row p of the planes is X row perm[p] (perm NULL: p < n), or
 // padding (zeros, +inf norm) where perm[p] < 0 / p >= n
 int b2k_knn_prep_launch(b2k_ctx* ctx, const float* X, int64_t n, int d, const int32_t* perm, int64_t n_pad, int DP,
                         float* Xhi, float* Xlo, float* norms, cudaStream_t s);
+// Qs = Q - s [nq][d] for the wgmma pass, s = X row 0 as above; d % 4 == 0, Q and Qs 16-byte aligned
+int b2k_knn_shift_launch(b2k_ctx* ctx, const float* Q, int64_t nq, int d, const float* X, float* Qs, cudaStream_t s);
 // one search pass over a unit table (device, nunits entries).  wgmma: Q = shifted queries [nq][d] (16-byte aligned),
 // the planes and norms of b2k_knn_prep_launch; generic: Q unshifted, item row r of the index is X row xperm[r] (xperm
 // NULL: r)

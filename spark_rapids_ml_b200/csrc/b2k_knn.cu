@@ -23,6 +23,7 @@
 
 namespace {
 #include "b2k_ptx.cuh"
+#include "b2k_pair_wg.cuh"
 
 static_assert(sizeof(KnnCand) == 16, "KnnCand crosses NCCL as 16 bytes");
 
@@ -42,110 +43,58 @@ __device__ __forceinline__ void list_insert(int2* L, int k, float d, int r) {
   L[p] = make_int2(__float_as_int(d), r);
 }
 
-constexpr int KW_TM = 128;                  // queries per tile (two consumer warpgroups x wgmma M = 64)
-constexpr int KW_N = 128;                   // index rows per block (wgmma N)
-constexpr int KW_CHUNK = 32;                // f32 per 128-byte swizzle row
 constexpr int KW_KMAX = 64;                 // largest k of the wgmma path
-constexpr int KW_NTHREADS = 384;            // 8 consumer warps + a producer warpgroup (one warp issues)
 constexpr int KW_SMAX = B2K_KNN_MAX_LISTS;  // index splits (the merge keeps 8 list heads per lane)
-static_assert(KW_TM == B2K_KNN_WG_QROWS && KW_N == B2K_KNN_WG_BLOCK, "unit geometry shared with b2k_ivf.cu");
+constexpr int KW_LBYTES = PW_TM * KW_KMAX * 8;   // row lists [128][64] (screen distance bits, row)
 
-template <int NCH>
-struct KnnWgCfg {
-  static constexpr int DP = NCH * KW_CHUNK;
-  static constexpr int QBYTES = KW_TM * KW_CHUNK * 4;   // one query chunk: 16 KB
-  static constexpr int CBYTES = KW_N * KW_CHUNK * 4;    // one index chunk plane: 16 KB
-  static constexpr int SC = 2;                           // index stages of (hi, lo)
-  static constexpr int OFF_Q = 0;
-  static constexpr int OFF_C = OFF_Q + NCH * QBYTES;
-  static constexpr int OFF_L = OFF_C + SC * 2 * CBYTES;
-  static constexpr int LBYTES = KW_TM * KW_KMAX * 8;    // [128][64] (screen distance, row)
-  static constexpr int OFF_BAR = OFF_L + LBYTES;
-  static constexpr int SMEM_BYTES = OFF_BAR + 8 * (2 + 2 * SC);
-  static_assert(OFF_C % 1024 == 0 && CBYTES % 1024 == 0, "swizzle atoms need 1 KB alignment");
-  static_assert(SMEM_BYTES + 1024 <= 227 * 1024, "smem");
-};
 // d = 128: query tile 64 KB + two index stages 64 KB + lists 64 KB
+template <int NCH>
+using KnnWgCfg = PairWgCfg<NCH, KW_LBYTES>;
 static_assert(KnnWgCfg<4>::SMEM_BYTES == 192 * 1024 + 48, "cfg5 layout");
 
 struct KnnArgs {
-  const KnnUnit* units;      // [nunits], index ranges in blocks of KW_N rows
+  const KnnUnit* units;      // [nunits], index ranges in blocks of PW_N rows
   int nunits;
   int k;
-  const float* norms;        // [blocks * KW_N] ||x - s||^2, +inf on padding rows
+  const float* norms;        // [blocks * PW_N] ||x - s||^2, +inf on padding rows
   int2* part;                // rows of k (screen distance bits, index row)
 };
 
 #include "b2k_knn_prep.cuh"
 
-// Persistent grid, static round-robin over the unit table.  Warp 8 issues TMA: the unit's query tile (NCH chunks, once
-// per unit) and its index blocks, chunk by chunk, hi and lo planes into a ring of SC stages.
-// Consumer warpgroup g owns queries [64 g, 64 g + 64) of the tile; per block it accumulates lo.Xhi^T + hi.Xlo^T +
-// hi.Xhi^T (A = the query split in registers, as the 3xTF32 branch of k_wg_assign) into D[64 x 128].  Q, X and the
+// Persistent grid, static round-robin over the unit table; producer and main loop of b2k_pair_wg.cuh.  Q, X and the
 // norms all come shifted by s.  The epilogue screens ||x - s||^2 - 2 (q - s).(x - s) against each row's current k-th
 // best (a register threshold replicated over the row's quad); the quad's lanes insert the candidates under it in turn.
 template <int NCH>
-__global__ void __launch_bounds__(KW_NTHREADS, 1)
+__global__ void __launch_bounds__(PW_NTHREADS, 1)
 k_knn_wg(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapHi,
          const __grid_constant__ CUtensorMap mapLo, const KnnArgs args) {
   using G = KnnWgCfg<NCH>;
-  constexpr int R = KW_N / 2;
+  constexpr int R = PW_N / 2;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   const uint32_t base = smem_u32(smem_raw);
-  if ((base & 1023u) != 0u) __trap();   // 128B-swizzle atoms need a 1 KB aligned base
-  const uint32_t bars = base + G::OFF_BAR;
-  const uint32_t qfull = bars, qempty = bars + 8u;
-  auto cfull = [&](int s) -> uint32_t { return bars + 16u + 8u * (uint32_t)s; };
-  auto cempty = [&](int s) -> uint32_t { return bars + 16u + 8u * (uint32_t)(G::SC + s); };
-  int2* lists = reinterpret_cast<int2*>(smem_raw + G::OFF_L);
+  const PairWgBars bars = pair_wg_init<G>(base);
+  int2* lists = reinterpret_cast<int2*>(smem_raw + G::OFF_OWN);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (threadIdx.x == 0) {
-    mbar_init(qfull, 1);
-    mbar_init(qempty, 8);
-    for (int s = 0; s < G::SC; ++s) {
-      mbar_init(cfull(s), 1);
-      mbar_init(cempty(s), 8);
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncthreads();
   const int nunits = args.nunits;
   const int nit = (int)blockIdx.x < nunits ? (nunits - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
   const int k = args.k;
 
   if (warp >= 8) {
-    if (warp == 8 && elect_one()) {
-      tma_prefetch_desc(&mapQ);
-      tma_prefetch_desc(&mapHi);
-      tma_prefetch_desc(&mapLo);
-      int q = 0;
-      for (int it = 0; it < nit; ++it) {
-        const KnnUnit un = args.units[(int)blockIdx.x + it * (int)gridDim.x];
-        mbar_wait_nocall(qempty, (uint32_t)((it & 1) ^ 1));
-        mbar_expect_tx(qfull, (uint32_t)(NCH * G::QBYTES));
-        for (int c = 0; c < NCH; ++c)
-          tma_load_2d(base + (uint32_t)(G::OFF_Q + c * G::QBYTES), &mapQ, qfull, c * KW_CHUNK, un.row0);
-        for (int b = un.lo; b < un.hi; ++b) {
-#pragma unroll 1
-          for (int c = 0; c < NCH; ++c, ++q) {
-            const int cs = q % G::SC;
-            mbar_wait_nocall(cempty(cs), (uint32_t)((q / G::SC) & 1) ^ 1u);
-            const uint32_t dst = base + (uint32_t)(G::OFF_C + cs * 2 * G::CBYTES);
-            mbar_expect_tx(cfull(cs), (uint32_t)(2 * G::CBYTES));
-            tma_load_2d(dst, &mapHi, cfull(cs), c * KW_CHUNK, b * KW_N);
-            tma_load_2d(dst + G::CBYTES, &mapLo, cfull(cs), c * KW_CHUNK, b * KW_N);
-          }
-        }
-      }
-    }
+    if (warp == 8 && elect_one())
+      pair_wg_produce<G>(
+          base, bars, &mapQ, &mapHi, &mapLo, nit,
+          [&](int it) {
+            const KnnUnit un = args.units[(int)blockIdx.x + it * (int)gridDim.x];
+            return PairWgUnit{un.row0, un.lo, un.hi};
+          },
+          [](int) { return false; });
     __syncwarp();
     return;
   }
 
   const int g = warp >> 2, wi = warp & 3;
   const int rr0 = g * 64 + wi * 16 + (lane >> 2);   // this thread's rows rr0, rr0 + 8 of the tile
-  const uint32_t arow = (uint32_t)rr0 * 128u + (uint32_t)(lane & 3) * 4u;
-  const uint32_t asw = (uint32_t)(lane >> 2);
   int2* L[2] = {lists + (size_t)rr0 * KW_KMAX, lists + (size_t)(rr0 + 8) * KW_KMAX};
   float acc[R];
   int q = 0;
@@ -157,48 +106,11 @@ k_knn_wg(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUten
     }
     __syncwarp();
     float thr[2] = {__int_as_float(0x7f800000), __int_as_float(0x7f800000)};
-    mbar_wait_nocall(qfull, (uint32_t)(it & 1));
+    mbar_wait_nocall(bars.qfull(), (uint32_t)(it & 1));
     for (int b = un.lo; b < un.hi; ++b) {
-#pragma unroll
-      for (int c = 0; c < NCH; ++c, ++q) {
-        const int cs = q % G::SC;
-        const uint8_t* xp = smem_raw + G::OFF_Q + c * G::QBYTES;
-        const uint32_t cst = base + (uint32_t)(G::OFF_C + cs * 2 * G::CBYTES);
-        // q = hi + lo, hi = RN_tf32(q), lo = RN_tf32(q - hi), in registers
-        uint32_t ah[KW_CHUNK / 8][4], al[KW_CHUNK / 8][4];
-#pragma unroll
-        for (int ks = 0; ks < KW_CHUNK / 8; ++ks) {
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {   // row rr0 + 8 (e & 1), column 8 ks + lane % 4 + 4 (e >> 1)
-            const uint32_t unit = (uint32_t)(2 * ks + (e >> 1));
-            const float v = *reinterpret_cast<const float*>(xp + arow + (uint32_t)(e & 1) * 1024u + ((unit ^ asw) << 4));
-            ah[ks][e] = rn_tf32_bits(v);
-            al[ks][e] = rn_tf32_bits(v - __uint_as_float(ah[ks][e]));
-          }
-        }
-#pragma unroll
-        for (int ks = 0; ks < KW_CHUNK / 8; ++ks) {
-          reg_fence(ah[ks]);
-          reg_fence(al[ks]);
-        }
-        mbar_wait_nocall(cfull(cs), (uint32_t)((q / G::SC) & 1));
-        wgmma_fence();
-#pragma unroll
-        for (int ks = 0; ks < KW_CHUNK / 8; ++ks) {
-          const uint64_t dh = make_kmajor_sw128_desc(cst + ks * 32);
-          const uint64_t dl = make_kmajor_sw128_desc(cst + G::CBYTES + ks * 32);
-          wgmma_tf32_rs<KW_N>(acc, al[ks], dh, (c | ks) != 0 ? 1u : 0u);   // small terms first
-          wgmma_tf32_rs<KW_N>(acc, ah[ks], dl, 1u);
-          wgmma_tf32_rs<KW_N>(acc, ah[ks], dh, 1u);
-        }
-        wgmma_commit();
-        wgmma_wait0();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(cempty(cs));
-      }
-      reg_fence(acc);
+      pair_wg_block<G>(smem_raw, base, bars, rr0, lane, acc, q);
       // ---- epilogue: acc[i] is row rr0 + 8 ((i >> 1) & 1), block column 8 (i >> 2) + 2 (lane & 3) + (i & 1) ----
-      const float* nb = args.norms + (size_t)b * KW_N + 2 * (lane & 3);
+      const float* nb = args.norms + (size_t)b * PW_N + 2 * (lane & 3);
       bool cand = false;
 #pragma unroll
       for (int i = 0; i < R; ++i) {
@@ -214,7 +126,7 @@ k_knn_wg(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUten
             for (int i = 0; i < R; ++i) {
               const int h = (i >> 1) & 1;
               if (acc[i] <= thr[h] && acc[i] < __int_as_float(0x7f800000)) {
-                list_insert(L[h], k, acc[i], b * KW_N + 8 * (i >> 2) + 2 * (lane & 3) + (i & 1));
+                list_insert(L[h], k, acc[i], b * PW_N + 8 * (i >> 2) + 2 * (lane & 3) + (i & 1));
                 thr[h] = __int_as_float(L[h][k - 1].x);
               }
             }
@@ -226,7 +138,7 @@ k_knn_wg(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUten
       }
     }
     __syncwarp();
-    if (lane == 0) mbar_arrive(qempty);   // every A fragment of this unit has been read
+    if (lane == 0) mbar_arrive(bars.qempty());   // every A fragment of this unit has been read
     for (int h = 0; h < 2; ++h) {
       const int r = rr0 + 8 * h;
       if (r < un.nrows) {
@@ -446,17 +358,6 @@ k_knn_merge(const KnnCand* __restrict__ all, int nranks, int64_t nq_all, int64_t
       });
 }
 
-using Timer = B2kTimer;
-
-template <int NCH>
-int launch_wg(b2k_ctx* ctx, int grid, const CUtensorMap& mq, const CUtensorMap& mh, const CUtensorMap& ml,
-              const KnnArgs& a, cudaStream_t s) {
-  const int smem = KnnWgCfg<NCH>::SMEM_BYTES;
-  B2K_CUDA_OK(ctx, cudaFuncSetAttribute(k_knn_wg<NCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  k_knn_wg<NCH><<<grid, KW_NTHREADS, smem, s>>>(mq, mh, ml, a);
-  B2K_CUDA_OK(ctx, cudaGetLastError());
-  return B2K_OK;
-}
 // The local search: plan, prep, search and refine of queries Q [nq][d] against this rank's items, with no collective.
 struct KnnLocal {
   bool wg = false;
@@ -477,9 +378,9 @@ int knn_local_plan(b2k_ctx* ctx, int64_t n_items, int64_t nq, int d, int k, bool
   int sm = ctx->sm_count;
   if (ctx->grid_limit > 0 && ctx->grid_limit < sm) sm = ctx->grid_limit;
   p->DP = b2k_knn_wg_dp(d);
-  p->nblk = (n_items + KW_N - 1) / KW_N;
-  p->n_pad = p->nblk * KW_N;
-  const int64_t qt = p->wg ? KW_TM : GQ;
+  p->nblk = (n_items + PW_N - 1) / PW_N;
+  p->n_pad = p->nblk * PW_N;
+  const int64_t qt = p->wg ? PW_TM : GQ;
   p->ntiles = (nq + qt - 1) / qt;
   const int64_t item_tiles = p->wg ? p->nblk : (n_items + GN - 1) / GN;
   // splits of the index: at least about 2 units per SM, at most one tile of the index per split
@@ -502,11 +403,11 @@ void knn_local_take(B2kLayout& L, KnnLocal* p, int64_t n_items, int64_t nq, int 
 
 // marks 2 (after prep), 3 (after search) and 4 (after refine) of tm
 int knn_local_run(b2k_ctx* ctx, const KnnLocal& p, const float* items, int64_t n_items, const int64_t* item_ids,
-                  const float* Q, int64_t nq, int d, int k, int64_t row0, KnnCand* cand, Timer& tm, cudaStream_t s) {
+                  const float* Q, int64_t nq, int d, int k, int64_t row0, KnnCand* cand, B2kTimer& tm, cudaStream_t s) {
   // ---- search of the local index for every query ----
   if (n_items > 0) {
     // units u = tile * S + split: a tile of queries against one split of the index
-    const int64_t qt = p.wg ? KW_TM : GQ, ntx = p.wg ? p.nblk : (n_items + GN - 1) / GN;
+    const int64_t qt = p.wg ? PW_TM : GQ, ntx = p.wg ? p.nblk : (n_items + GN - 1) / GN;
     std::vector<KnnUnit> units((size_t)(p.ntiles * p.S));
     for (int64_t tile = 0; tile < p.ntiles; ++tile)
       for (int split = 0; split < p.S; ++split) {
@@ -521,11 +422,7 @@ int knn_local_run(b2k_ctx* ctx, const KnnLocal& p, const float* items, int64_t n
     B2K_CUDA_OK(ctx, cudaMemcpyAsync(p.units, units.data(), units.size() * sizeof(KnnUnit), cudaMemcpyHostToDevice, s));
     if (p.wg) {
       B2K_TRY(b2k_knn_prep_launch(ctx, items, n_items, d, nullptr, p.n_pad, p.DP, p.Xhi, p.Xlo, p.norms, s));
-      const int64_t n4 = nq * d / 4;
-      k_knn_shift_q<<<(unsigned)std::min<int64_t>((n4 + 255) / 256, (int64_t)ctx->sm_count * 16), 256, 0, s>>>(
-          reinterpret_cast<const float4*>(Q), n4, d, items, reinterpret_cast<float4*>(p.Qs));
-      B2K_CUDA_OK(ctx, cudaGetLastError());
-      ctx->stats.kernel_launches++;
+      B2K_TRY(b2k_knn_shift_launch(ctx, Q, nq, d, items, p.Qs, s));
     }
     tm.mark(2, s);
     B2K_TRY(b2k_knn_scan_launch(ctx, p.wg, p.DP, p.wg ? p.Qs : Q, nq, items, nullptr, p.Xhi, p.Xlo, p.norms, p.n_pad, d,
@@ -544,7 +441,8 @@ int knn_local_run(b2k_ctx* ctx, const KnnLocal& p, const float* items, int64_t n
 }
 }  // namespace
 
-bool b2k_knn_wg_shape(int d, int k) { return d % 4 == 0 && d >= 4 && d <= 128 && k <= KW_KMAX; }
+bool b2k_knn_wg_width(int d) { return d % 4 == 0 && d >= 4 && d <= 128; }
+bool b2k_knn_wg_shape(int d, int k) { return b2k_knn_wg_width(d) && k <= KW_KMAX; }
 int b2k_knn_wg_dp(int d) { return d <= 32 ? 32 : d <= 64 ? 64 : 128; }
 
 int b2k_knn_prep_launch(b2k_ctx* ctx, const float* X, int64_t n, int d, const int32_t* perm, int64_t n_pad, int DP,
@@ -556,18 +454,23 @@ int b2k_knn_prep_launch(b2k_ctx* ctx, const float* X, int64_t n, int d, const in
   return B2K_OK;
 }
 
+int b2k_knn_shift_launch(b2k_ctx* ctx, const float* Q, int64_t nq, int d, const float* X, float* Qs, cudaStream_t s) {
+  if (nq == 0) return B2K_OK;
+  const int64_t n4 = nq * d / 4;
+  k_knn_shift_q<<<(unsigned)std::min<int64_t>((n4 + 255) / 256, (int64_t)ctx->sm_count * 16), 256, 0, s>>>(
+      reinterpret_cast<const float4*>(Q), n4, d, X, reinterpret_cast<float4*>(Qs));
+  B2K_CUDA_OK(ctx, cudaGetLastError());
+  ctx->stats.kernel_launches++;
+  return B2K_OK;
+}
+
 int b2k_knn_scan_launch(b2k_ctx* ctx, bool wg, int DP, const float* Q, int64_t nq, const float* X, const int32_t* xperm,
                         const float* Xhi, const float* Xlo, const float* norms, int64_t n_pad, int d, int k,
                         const KnnUnit* units, int nunits, int2* part, cudaStream_t s) {
   if (nunits == 0) return B2K_OK;
   if (wg) {
-    CUtensorMap mq, mh, ml;
-    B2K_TRY(b2k_encode_2d(ctx, &mq, Q, (uint64_t)d, (uint64_t)nq, (uint64_t)d * 4, KW_CHUNK, KW_TM,
-                          CU_TENSOR_MAP_L2_PROMOTION_L2_256B));
-    B2K_TRY(b2k_encode_2d(ctx, &mh, Xhi, (uint64_t)DP, (uint64_t)n_pad, (uint64_t)DP * 4, KW_CHUNK, KW_N,
-                          CU_TENSOR_MAP_L2_PROMOTION_L2_256B));
-    B2K_TRY(b2k_encode_2d(ctx, &ml, Xlo, (uint64_t)DP, (uint64_t)n_pad, (uint64_t)DP * 4, KW_CHUNK, KW_N,
-                          CU_TENSOR_MAP_L2_PROMOTION_L2_256B));
+    PairWgMaps maps;
+    B2K_TRY(pair_wg_maps(ctx, Q, nq, d, Xhi, Xlo, n_pad, DP, &maps));
     KnnArgs a{};
     a.units = units;
     a.nunits = nunits;
@@ -577,13 +480,15 @@ int b2k_knn_scan_launch(b2k_ctx* ctx, bool wg, int DP, const float* Q, int64_t n
     int sm = ctx->sm_count;
     if (ctx->grid_limit > 0 && ctx->grid_limit < sm) sm = ctx->grid_limit;
     const int grid = std::min(sm, nunits);
-    if (DP == 32) B2K_TRY(launch_wg<1>(ctx, grid, mq, mh, ml, a, s));
-    else if (DP == 64) B2K_TRY(launch_wg<2>(ctx, grid, mq, mh, ml, a, s));
-    else B2K_TRY(launch_wg<4>(ctx, grid, mq, mh, ml, a, s));
+    B2K_TRY(pair_wg_launch<KW_LBYTES>(
+        ctx, DP, [](auto nch) { return k_knn_wg<decltype(nch)::value>; }, grid, maps, a, s));
     ctx->stats.fused_tc_launches++;
   } else {
+    // The attribute is per function and process-wide, so it is set for the largest k: ranks running as threads of one
+    // process, at different k, never lower it under each other's launches.
     const size_t smem = (size_t)GQ * k * sizeof(int2);
-    B2K_CUDA_OK(ctx, cudaFuncSetAttribute(k_knn_generic, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    B2K_CUDA_OK(ctx, cudaFuncSetAttribute(k_knn_generic, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                          (int)((size_t)GQ * B2K_KNN_MAX_K * sizeof(int2))));
     k_knn_generic<<<(unsigned)nunits, G_NTHREADS, smem, s>>>(Q, X, xperm, d, k, units, part);
     B2K_CUDA_OK(ctx, cudaGetLastError());
     ctx->stats.generic_launches++;
@@ -597,7 +502,8 @@ int b2k_knn_refine_launch(b2k_ctx* ctx, const int2* part, int nl, const int32_t*
                           const int64_t* ids, KnnCand* cand, cudaStream_t s) {
   if (nq == 0) return B2K_OK;
   const size_t rf_smem = (size_t)RF_WARPS * 2 * k * 4;
-  B2K_CUDA_OK(ctx, cudaFuncSetAttribute(k_knn_refine, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rf_smem));
+  B2K_CUDA_OK(ctx, cudaFuncSetAttribute(k_knn_refine, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        RF_WARPS * 2 * B2K_KNN_MAX_K * 4));   // the largest k, as for k_knn_generic
   k_knn_refine<<<(unsigned)((nq + RF_WARPS - 1) / RF_WARPS), RF_WARPS * 32, rf_smem, s>>>(
       part, nl, slots, perm, nq, k, Q, X, n_items, d, row0, ids, cand);
   B2K_CUDA_OK(ctx, cudaGetLastError());
@@ -619,7 +525,7 @@ int b2k_knn_search_impl(b2k_ctx* ctx, const float* items, int64_t n_items, const
                         const float* queries, int64_t nq_local, int d, int k, float* dist_out, int64_t* idx_out,
                         cudaStream_t s) {
   const int nr = ctx->nranks;
-  Timer tm(ctx->time_kernels != 0);
+  B2kTimer tm(ctx->time_kernels != 0);
   // ---- sizes of every rank; each error is decided on them, identically on every rank ----
   int64_t* sz_dev;
   B2K_TRY(b2k_scratch_layout(ctx, "kNN sizes", [&](B2kLayout& L) -> int {
@@ -708,7 +614,7 @@ int b2k_knn_search_impl(b2k_ctx* ctx, const float* items, int64_t n_items, const
 int b2k_knn_local_impl(b2k_ctx* ctx, const float* items, int64_t n_items, const float* queries, int64_t nq, int d,
                        int k, float* dist_out, int64_t* idx_out, cudaStream_t s) {
   if (nq == 0) return B2K_OK;
-  Timer tm(false);
+  B2kTimer tm(false);
   KnnLocal lp;
   B2K_TRY(knn_local_plan(ctx, n_items, nq, d, k, (reinterpret_cast<uintptr_t>(queries) & 15u) == 0, &lp));
   KnnCand* cand = nullptr;

@@ -467,27 +467,6 @@ bool fused_fits(const b2k_ctx* ctx, int d, int kp) {
   return p.kern && fused_smem(d, kp, p.KB) <= ctx->smem_optin;
 }
 
-struct Timer {   // CUDA events around the evaluation pass when option time_kernels is set
-  cudaEvent_t ev[2] = {};
-  bool on = false;
-  explicit Timer(bool enable) : on(enable) {
-    if (on)
-      for (auto& e : ev) cudaEventCreate(&e);
-  }
-  ~Timer() {
-    if (on)
-      for (auto& e : ev) cudaEventDestroy(e);
-  }
-  void mark(int i, cudaStream_t s) {
-    if (on) cudaEventRecord(ev[i], s);
-  }
-  double ms() const {
-    float t = 0.f;
-    if (on) cudaEventElapsedTime(&t, ev[0], ev[1]);
-    return (double)t;
-  }
-};
-
 std::string num(double v) {   // Python's repr of a float
   if (std::isnan(v)) return "nan";
   if (std::isinf(v)) return v > 0 ? "inf" : "-inf";
@@ -865,7 +844,7 @@ int eval_device(b2k_ctx* ctx, const EvalCall& e, const double* W, const double* 
   B2K_CUDA_OK(ctx, cudaMemcpyAsync(Wd, W, (size_t)kp * d * 8, cudaMemcpyHostToDevice, s));
   B2K_CUDA_OK(ctx, cudaMemcpyAsync(bd, b, (size_t)kp * 8, cudaMemcpyHostToDevice, s));
   B2K_CUDA_OK(ctx, cudaMemcpyAsync(cmap, e.cmap->data(), MAXC * 4, cudaMemcpyHostToDevice, s));
-  Timer tm(ctx->time_kernels != 0);
+  B2kTimer tm(ctx->time_kernels != 0);
   tm.mark(0, s);
   if (n == 0) {
     B2K_CUDA_OK(ctx, cudaMemsetAsync(part, 0, (size_t)P * M * 8, s));
@@ -901,7 +880,7 @@ int eval_device(b2k_ctx* ctx, const EvalCall& e, const double* W, const double* 
   B2K_CUDA_OK(ctx, cudaMemcpyAsync(out_host, out, ((size_t)M + 1) * 8, cudaMemcpyDeviceToHost, s));
   B2K_CUDA_OK(ctx, cudaStreamSynchronize(s));
   ctx->stats.last_path = fused ? B2K_PATH_FUSED : B2K_PATH_GENERIC;
-  if (tm.on) ctx->stats.last_fused_ms = tm.ms();
+  if (tm.on) ctx->stats.last_fused_ms = tm.ms(0, 1);
   return B2K_OK;
 }
 

@@ -213,28 +213,6 @@ k_project(const float* __restrict__ X, int64_t n, int d, const float* __restrict
   }
 }
 
-struct Timer {   // CUDA events around the device phases when option time_kernels is set
-  cudaEvent_t ev[8] = {};
-  bool on = false;
-  explicit Timer(bool enable) : on(enable) {
-    if (on)
-      for (auto& e : ev) cudaEventCreate(&e);
-  }
-  ~Timer() {
-    if (on)
-      for (auto& e : ev) cudaEventDestroy(e);
-  }
-  void mark(int i, cudaStream_t s) {
-    if (on) cudaEventRecord(ev[i], s);
-  }
-  double ms(int a, int b) const {
-    float t = 0.f;
-    if (on) cudaEventElapsedTime(&t, ev[a], ev[b]);
-    return (double)t;
-  }
-};
-
-
 }  // namespace
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -397,7 +375,7 @@ int b2k_moments_impl(b2k_ctx* ctx, const char* who, const float* X, const float*
     return b2k_fail(ctx, B2K_ERR_UNSUPPORTED, "kernel_path=2 requested but the wgmma Gram pass needs d % 4 == 0 and a "
                                               "16-byte aligned X (d = " + std::to_string(d) + ")");
   const bool wg = wg_ok && ctx->kernel_path != B2K_PATH_GENERIC;
-  Timer tm(ctx->time_kernels != 0);
+  B2kTimer tm(ctx->time_kernels != 0);
 
   // ---- plan and scratch ----
   const int ncb = (d + CS_TX - 1) / CS_TX;

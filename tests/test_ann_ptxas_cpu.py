@@ -1,6 +1,6 @@
 """The search passes that IVF-Flat shares with exact k-NN (b2k_knn.cu: the wgmma and generic scans, the refine, the
-merge, the prep) and IVF-Flat's own kernels (b2k_ivf.cu) compile for sm_90a with no spills (ptxas -v, the library's
-flags)."""
+merge, the prep), IVF-Flat's own kernels (b2k_ivf.cu) and DBSCAN's count and union passes (b2k_dbscan.cu, on the same
+wgmma pipeline) compile for sm_90a with no spills (ptxas -v, the library's flags)."""
 import os
 import re
 import subprocess
@@ -33,10 +33,12 @@ def _entries(src, tmp_path):
                     "k_knn_prep", "k_knn_shift_q"]),
     ("b2k_ivf.cu", ["k_ivf_nonfinite", "k_ivf_train_rows", "k_ivf_offsets", "k_ivf_perm", "k_ivf_pairs", "k_ivf_slots",
                     "k_ivf_gather_q", "k_ivf_narrow"]),
+    ("b2k_dbscan.cu", ["k_db_wgILi1ELb0", "k_db_wgILi2ELb0", "k_db_wgILi4ELb0", "k_db_wgILi1ELb1", "k_db_wgILi2ELb1",
+                       "k_db_wgILi4ELb1", "k_db_generic"]),
 ])
 def test_search_kernels_have_no_spills(tmp_path, src, names):
     entries = _entries(src, tmp_path)
     for n in names:
         assert any(n in e for e in entries), (n, sorted(entries))
-    spilled = {e: v for e, v in entries.items() if ("k_knn" in e or "k_ivf" in e) and (v[1] or v[2])}
+    spilled = {e: v for e, v in entries.items() if ("k_knn" in e or "k_ivf" in e or "k_db" in e) and (v[1] or v[2])}
     assert not spilled, spilled
