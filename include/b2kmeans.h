@@ -41,6 +41,9 @@
  *   b2k_umap_transform          umap.py:1449-1551 (UMAPModel's transform: cuML UMAP.transform)
  *   b2k_ivf_search              knn.py:1406-1692 (ApproximateNearestNeighborsModel.kneighbors with algorithm "ivfflat":
  *                               the cuVS IVF-Flat build and search per partition and the top-k aggregation)
+ *   b2k_silhouette              none: the reference has no clustering evaluator (its DBSCAN benchmark collects the
+ *                               frame and calls scikit-learn's silhouette_score); stands in for Spark's
+ *                               pyspark.ml.evaluation.ClusteringEvaluator (metricName "silhouette")
  *
  * Conventions
  *   - Plain C, no exceptions across the boundary: every call returns a b2k_status; the message for the
@@ -650,6 +653,48 @@ int b2k_eval_forest_scores(b2k_ctx* ctx, const float* X, const float* y, int64_t
 #define B2K_BINARY_PR 1
 int b2k_eval_binary(b2k_ctx* ctx, const double* scores, const uint8_t* pos, int64_t n, int n_models, int num_bins,
                     int metric, double* out, uintptr_t stream);
+
+/* ---- silhouette (b2k_silhouette.cu): Spark's ClusteringEvaluator, metricName "silhouette" ----
+ * No reference interface: Spark computes it in closed form (ClusteringEvaluator / SquaredEuclideanSilhouette /
+ * CosineSilhouette); tests/silhouette_oracle.py restates the rule in fp64 NumPy.  X device f32 [n_local][d] (this rank's
+ * rows), cluster_ids device int64 [n_local] (any values; -1 is a cluster like any other), metric 0 squaredEuclidean or 1
+ * cosine; *out (host) = the metric.  Rule, over the rows of all ranks (n rows, clusters = the distinct ids):
+ *   rows     y = x (metric 0), or y = fl32(x / |x|) with |x| = sqrt of the feature-order fp64 sum of squares (metric 1,
+ *            DBSCAN's rule), so that ||y_i - y_j||^2 = 2 (1 - cos) up to the rounding of y.
+ *   D(i, c)  = the mean of ||y_i - y_j||^2 over the members j of cluster c (all of them) = ||y_i - mu_c||^2 + Psi_c, mu_c
+ *            the mean of c's rows and Psi_c = sum_{j in c} ||y_j - mu_c||^2 / N_c.
+ *   s_i      row i in cluster A: 0 if N_A = 1; else a = D(i, A) N_A / (N_A - 1), b = min_{c != A} D(i, c), s_i = 1 - a/b
+ *            (a < b), b/a - 1 (a > b), 0 (a = b).  The metric is sum_i s_i / n.  (Cosine's s equals Spark's: the
+ *            factor 2 cancels in a / b.)  = scikit-learn's silhouette_score, metric "sqeuclidean" or "cosine".
+ * Spark forms D as ||x||^2 + sum ||y||^2 / N - 2 x.sum y / N, which cancels on offset data; here D is formed in a frame
+ * shifted by the global mean (wgmma) or as a sum of fp64 squared differences (generic).
+ * Passes: the cluster ids (per-rank CUB sort-unique, allgather of the counts and values, host merge; K <= 65536), one
+ * statistics pass over X (fp64 per-cluster sums of y and ||y||^2, fixed-order folds, one f64 allreduce of K (d + 2) + 2
+ * values), then the silhouette pass: wgmma (3xTF32 products of the tile rows y - m with the shifted means fl32(mu_c - m),
+ * m = fl32(the global mean of y)) when d % 4 == 0, 4 <= d <= 128 and X is 16-byte aligned on every rank, else the
+ * generic SIMT pass (fp64).  Option "kernel_path" = B2K_PATH_GENERIC forces the generic pass, B2K_PATH_FUSED fails with
+ * B2K_ERR_UNSUPPORTED where wgmma cannot run; option "grid_limit" caps the CTAs of the silhouette pass.
+ * Error bound (wgmma; the generic pass is inside it too): u = 2^-24, nb = 3 ceil(d / 8), N_ic = ||y_i - m||^2 +
+ * ||mu_c - m||^2.  The fp32 screen of b2k_dbscan_fit (norms, split, wgmma model, epilogue, shift) gives
+ * (23.02 + 36.08 (1 + nb)) u N_ic for ||y'_i - mu'_c||^2; the rounding of mu'_c = fl32(mu_c - m) is inside its shift term,
+ * and the fp32 add of fl32(Psi_c) costs 2 u (3.1 N_ic + Psi_c).  Psi_c in fp64 (sums over at most L_c = 256 + d + N_c +
+ * 8 sequential adds per term): |dPsi_c| <= (3 L_c + d + 6) 2^-53 Q_c / N_c, Q_c = sum ||y||^2 over c.  Cosine adds 8.1 u
+ * (the rounding of y).  So |D~ - D| <= delta(i, c) = (31.3 + 36.08 (1 + nb)) u N_ic + 2.01 u Psi_c + |dPsi_c| (+ 8.1 u).
+ * With da = delta(i, A) N_A / (N_A - 1) and db = max_{c != A} delta(i, c), s_i lies in [s(a + da, b - db), s(a - da,
+ * b + db)] (s falls with a and rises with b; arguments clamp at 0); the metric is within beta = the mean of the
+ * half-widths (+ (n + 8) 2^-53) of the exact value.
+ * Errors, decided on allgathered or allreduced values so that every rank fails together (B2K_ERR_INVALID unless noted):
+ * metric not 0 or 1; no row on any rank; d differing between ranks; "Number of clusters must be greater than one." (fewer
+ * than 2 distinct ids); more than 65536 distinct ids (B2K_ERR_UNSUPPORTED); a NaN or infinite feature; cosine with a
+ * zero row.  A rank with no rows takes part (X and cluster_ids may then be NULL).  Collective; synchronises `stream`.
+ * Deterministic: no floating-point atomics, every fp64 sum in a fixed order, so two calls with the same input, rank
+ * count and device give the same bits, and every rank gets the same value.
+ * Stats: last_path = the silhouette pass that ran; with option "time_kernels" != 0, last_finalize_ms = the cluster ids,
+ * last_reduce_ms = the statistics pass, its allreduce and the means, last_fused_ms = the silhouette pass (with the
+ * means' planes), last_allreduce_ms = the final allreduce, last_loop_ms = the whole call (device times, CUDA events). */
+#define B2K_SILHOUETTE_MAX_CLUSTERS 65536
+int b2k_silhouette(b2k_ctx* ctx, const float* X, int64_t n_local, int d, const int64_t* cluster_ids, int metric,
+                   double* out, uintptr_t stream);
 
 /* ---- UMAP (euclidean) ----
  * b2k_umap_fit stands in for umap.py:1009-1065 (the fit function: cuML UMAP(...).fit on the rows coalesced to one

@@ -76,10 +76,12 @@ EXPORTED_SYMBOLS = (
     "b2k_umap_fit",
     "b2k_umap_graph",
     "b2k_umap_transform",
+    "b2k_silhouette",
 )
 
 EVAL_KINDS = {"identity": 0, "logistic": 1, "softmax": 2}
 BINARY_METRICS = {"areaUnderROC": 0, "areaUnderPR": 1}
+SILHOUETTE_METRICS = {"squaredEuclidean": 0, "cosine": 1}
 
 FAMILY_CODES = {"auto": 0, "binomial": 1, "multinomial": 2}
 METRIC_CODES = {"euclidean": 0, "cosine": 1}
@@ -254,6 +256,7 @@ def load_library() -> ctypes.CDLL:
     L.b2k_umap_fit.argtypes = [vp, vp, i64, i32, vp, ctypes.POINTER(UmapParams), vp, vp, ctypes.c_size_t]
     L.b2k_umap_graph.argtypes = [vp] + [vp] * 11
     L.b2k_umap_transform.argtypes = [vp, vp, vp, i64, i32, vp, i64, ctypes.POINTER(UmapParams), vp, ctypes.c_size_t]
+    L.b2k_silhouette.argtypes = [vp, vp, i64, i32, vp, i32, ctypes.POINTER(f64), ctypes.c_size_t]
     for name in EXPORTED_SYMBOLS:
         if name not in ("b2k_last_error",):
             getattr(L, name).restype = i32
@@ -779,6 +782,27 @@ class Context:
                                                METRIC_CODES[metric], labels.data_ptr(), core.data_ptr(),
                                                ctypes.byref(ncl), self._stream()))
         return labels, core.bool(), int(ncl.value)
+
+    # -- silhouette -------------------------------------------------------------------------
+    def silhouette(self, X: Any, cluster_ids: Any, distance_measure: str = "squaredEuclidean") -> float:
+        """b2k_silhouette over all ranks' rows (collective when a communicator is initialised): X [n, d] float32 and
+        cluster_ids [n] int64 CUDA tensors (n may be 0) -> Spark's silhouette, the same value on every rank.
+        distance_measure is "squaredEuclidean" or "cosine"."""
+        t = self._torch
+        n, d = self._check_X(X)
+        if distance_measure not in SILHOUETTE_METRICS:
+            raise ValueError(f"distance_measure must be one of {sorted(SILHOUETTE_METRICS)}, got {distance_measure!r}")
+        if not (cluster_ids.is_cuda and cluster_ids.dtype == t.int64 and cluster_ids.dim() == 1 and
+                cluster_ids.is_contiguous() and int(cluster_ids.shape[0]) == n):
+            raise ValueError("cluster_ids must be a contiguous int64 CUDA tensor [n]")
+        if cluster_ids.device.index != self.device_index:
+            raise ValueError("cluster_ids lives on a different device than this context")
+        out = ctypes.c_double(0.0)
+        with t.cuda.device(self.device):
+            self._check(self._L.b2k_silhouette(self._h, X.data_ptr(), n, d, cluster_ids.data_ptr(),
+                                               SILHOUETTE_METRICS[distance_measure], ctypes.byref(out),
+                                               self._stream()))
+        return float(out.value)
 
     # -- random forests ---------------------------------------------------------------------
     def rf_fit(self, X: Any, y: Any, *, n_trees: int = 20, max_depth: int = 5, max_bins: int = 32,

@@ -1022,6 +1022,19 @@ extern "C" int b2k_dbscan_fit(b2k_ctx* ctx, const float* X, int64_t n_local, int
 }
 
 // ------------------------------------------------------------------------------------------------
+// silhouette (b2k_silhouette.cu)
+// ------------------------------------------------------------------------------------------------
+extern "C" int b2k_silhouette(b2k_ctx* ctx, const float* X, int64_t n_local, int d, const int64_t* cluster_ids,
+                              int metric, double* out, uintptr_t stream) {
+  if (!ctx) return b2k_fail(nullptr, B2K_ERR_INVALID, "b2k_silhouette: ctx is NULL");
+  // an empty partition may come with no buffers; every value check runs after the size allgather, on every rank alike
+  if (n_local < 0 || d <= 0 || (n_local > 0 && (!X || !cluster_ids)) || !out)
+    return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_silhouette: bad X/cluster_ids/out/n/d");
+  B2K_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  return b2k_silhouette_impl(ctx, X, n_local, d, cluster_ids, metric, out, reinterpret_cast<cudaStream_t>(stream));
+}
+
+// ------------------------------------------------------------------------------------------------
 // random forests (b2k_rf.cu)
 // ------------------------------------------------------------------------------------------------
 extern "C" int b2k_rf_fit(b2k_ctx* ctx, const float* X, const float* y, int64_t n_local, int d,

@@ -192,3 +192,48 @@ class BinaryClassificationEvaluator(_Evaluator):
                                  "score is element 1")
             s = np.asarray([v[1] for v in raw], dtype=np.float64)
         return metrics.binary_metric(s, y, name, self.getNumBins())
+
+
+class ClusteringEvaluator(_Evaluator):
+    """pyspark.ml.evaluation.ClusteringEvaluator's params: featuresCol ("features"), predictionCol ("prediction"),
+    metricName ("silhouette", the only one), distanceMeasure ("squaredEuclidean" or "cosine"), weightCol.  Values
+    outside those sets raise ValueError with Spark's ParamValidators wording.  evaluate() is spark_rapids_ml_b200.
+    evaluation.ClusteringEvaluator's (on the device)."""
+
+    featuresCol = Param("parent", "featuresCol", "features column name.", TypeConverters.identity)
+    distanceMeasure = Param("parent", "distanceMeasure", "The distance measure. Supported options: "
+                            "'squaredEuclidean' and 'cosine'.", TypeConverters.toString)
+    _ALLOWED = {"metricName": ("silhouette",), "distanceMeasure": ("squaredEuclidean", "cosine")}
+
+    @keyword_only
+    def __init__(self, *, predictionCol: str = "prediction", featuresCol: Any = "features",
+                 metricName: str = "silhouette", distanceMeasure: str = "squaredEuclidean",
+                 weightCol: Optional[str] = None) -> None:
+        self._init({})
+        self._setDefault(featuresCol="features", metricName="silhouette", distanceMeasure="squaredEuclidean")
+        self._set(**{k: v for k, v in self._input_kwargs.items() if v is not None})
+
+    def _set(self, **kwargs: Any) -> "ClusteringEvaluator":
+        for name, allowed in self._ALLOWED.items():
+            v = kwargs.get(name)
+            if v is not None and v not in allowed:
+                raise ValueError(f"{self.uid} parameter {name} given invalid value {v}.")
+        return super()._set(**kwargs)
+
+    def getFeaturesCol(self) -> Any:
+        return self.getOrDefault("featuresCol")
+
+    def setFeaturesCol(self, value: Any) -> "ClusteringEvaluator":
+        return self._set(featuresCol=value)
+
+    def getDistanceMeasure(self) -> str:
+        return self.getOrDefault("distanceMeasure")
+
+    def setDistanceMeasure(self, value: str) -> "ClusteringEvaluator":
+        return self._set(distanceMeasure=value)
+
+    def setWeightCol(self, value: str) -> "ClusteringEvaluator":
+        return self._set(weightCol=value)
+
+    def isLargerBetter(self) -> bool:
+        return True
