@@ -25,15 +25,13 @@ from __future__ import annotations
 from typing import Any, Callable, Dict, Iterator, List, Optional, Sequence, Tuple, Union
 
 import numpy as np
-import pandas as pd
 import pyarrow as pa
 
-from .core import FitInputType, _append_transform_features, _CumlEstimator, _CumlModelWithPredictionCol, _CumlCommon
-from .core import _transform_context, alias, param_alias
+from .core import FitInputType, _CumlEstimator, _CumlModelWithPredictionCol, _DeviceModel, alias, param_alias
 from .params import HasFeaturesCol, HasFeaturesCols, HasLabelCol, HasPredictionCol, P, _CumlClass, _CumlParams
 from .regression import _ModelIterator
 from .tree import _RandomForestEstimator, _RandomForestModel
-from .sparkshim import BarrierTaskContext, LocalDataFrame, Param, Row, TypeConverters, keyword_only
+from .sparkshim import LocalDataFrame, Param, Row, TypeConverters, keyword_only
 
 
 class LogisticRegressionClass(_CumlClass):
@@ -511,109 +509,26 @@ class LogisticRegressionModel(LogisticRegressionClass, _CumlModelWithPredictionC
             models = self._eval_models()
             eps = eval_metric_info["eps"]
 
-            class _Holder:
-                def __init__(self, gpu: int) -> None:
-                    self.ctx = _transform_context(gpu)
-
             if eval_metric_info["binary"]:
                 def _scores(h: Any, X: Any, y: Any, scores: Any, pos: Any, row0: int) -> None:
                     h.ctx.binary_scores_linear(X, y, models, scores, pos, row0)
 
                 _scores.n_models = len(models)  # type: ignore[attr-defined]
-                return _Holder, None, _scores  # type: ignore[return-value]
+                return _DeviceModel, None, _scores  # type: ignore[return-value]
 
             def _evaluate(h: Any, X: Any, y: Any) -> List[Dict[str, Any]]:
                 return _class_accs(h.ctx.eval_linear(X, y, models, eps))
 
-            return _Holder, None, _evaluate  # type: ignore[return-value]
+            return _DeviceModel, None, _evaluate  # type: ignore[return-value]
         W, b, cls = self._device_model()
-        n_cols = int(self.n_cols)
+        class_values = cls[:max(2, W.shape[0])]
+        transform = self._grouped_transform(lambda m, X: m.ctx.logreg_predict(X, W, b, class_values),
+                                            4 * int(self.n_cols) + 8 * (2 * max(2, W.shape[0]) + 1))
+        return _DeviceModel, transform, None
 
-        class _DeviceLogReg:
-            def __init__(self, gpu: int) -> None:
-                self.ctx = _transform_context(gpu)
-
-            def close(self) -> None:   # the context stays with the process
-                pass
-
-        def _construct(gpu: int = 0) -> Any:
-            return _DeviceLogReg(gpu)
-
-        def _transform_many(lr: Any, dfs: List[Union[pd.DataFrame, np.ndarray]]) -> List[pd.DataFrame]:
-            """Several input batches in ONE device pass: every batch is ingested into the same device matrix, one
-            b2k_logreg_predict covers all rows, one read-back, one frame (rawPrediction, probability, prediction) per
-            input batch."""
-            from .utils import DeviceRowAppender
-
-            sizes = [len(df) for df in dfs]
-            total = sum(sizes)
-            nout = 2 if W.shape[0] == 1 else W.shape[0]
-            if total == 0:
-                return [pd.DataFrame({"raw": [], "prob": [], "pred": pd.Series([], dtype="float64")}) for _ in dfs]
-            app = DeviceRowAppender(lr.ctx, n_cols, first_capacity=total)
-            for df, n_b in zip(dfs, sizes):
-                if n_b:
-                    _append_transform_features(app, df, n_cols)
-            raw, prob, pred = lr.ctx.logreg_predict(app.finish(), W, b, cls[:nout] if W.shape[0] > 1 else cls[:2])
-            raw, prob, pred = raw.cpu().numpy(), prob.cpu().numpy(), pred.cpu().numpy()
-            out, o = [], 0
-            for n_b in sizes:
-                out.append(pd.DataFrame({"raw": list(raw[o:o + n_b]), "prob": list(prob[o:o + n_b]),
-                                         "pred": pred[o:o + n_b]}))
-                o += n_b
-            return out
-
-        def _transform_internal(lr: Any, df: Union[pd.DataFrame, np.ndarray]) -> pd.DataFrame:
-            return _transform_many(lr, [df])[0]
-
-        _transform_internal.many = _transform_many  # type: ignore[attr-defined]
-        _transform_internal.row_bytes = 4 * n_cols + 8 * (2 * max(2, W.shape[0]) + 1)  # type: ignore[attr-defined]
-        return _construct, _transform_internal, None
-
-    def _transform(self, dataset: Any) -> Any:
-        """Appends rawPredictionCol, probabilityCol (list<double>) and predictionCol (double) to a local frame."""
-        from .core import HAVE_PYSPARK, _iter_transform
-
-        if HAVE_PYSPARK:
-            from . import spark_binding
-
-            if spark_binding.is_spark_dataframe(dataset):
-                raise NotImplementedError("LogisticRegressionModel.transform() of a pyspark DataFrame is not supported in "
-                                          "this build; transform a local frame")
-        input_col, input_cols = self._get_input_columns()
-        construct, transform_internal, _ = self._get_cuml_transform_func(dataset)
-        cols: Dict[str, List[List[pa.Array]]] = {"raw": [], "prob": [], "pred": []}
-        state: Dict[str, Any] = {}
-        for pid, part in enumerate(dataset._parts):
-            def frames(part: Any = part, pid: int = pid) -> Iterator[Any]:
-                from .sparkshim.sql import _batches_to_pdf_iter
-
-                def selected() -> Iterator[pa.RecordBatch]:
-                    for batch in part:
-                        if "model" not in state:
-                            gpu = _CumlCommon._set_gpu_device(BarrierTaskContext(pid, len(dataset._parts)), True, True)
-                            state["model"] = construct(gpu)
-                        if input_cols:
-                            yield batch.select(list(input_cols))
-                        else:
-                            yield batch.select([input_col]).rename_columns([alias.data])
-
-                return _batches_to_pdf_iter(selected(), dataset.arrow_backed_pandas)
-
-            per = {k: [] for k in cols}
-            for res in _iter_transform(transform_internal, lambda: state["model"], frames()):
-                for k in ("raw", "prob"):
-                    rows = list(res[k])
-                    width = len(rows[0]) if rows else 0
-                    vals = np.asarray(rows, dtype=np.float64).reshape(-1) if rows else np.zeros(0)
-                    offs = np.arange(0, len(rows) * width + 1, max(width, 1), dtype=np.int32)[: len(rows) + 1]
-                    per[k].append(pa.ListArray.from_arrays(pa.array(offs), pa.array(vals, type=pa.float64())))
-                per["pred"].append(pa.array(np.asarray(res["pred"], dtype=np.float64), type=pa.float64()))
-            for k in cols:
-                cols[k].append(per[k])
-        out = dataset.with_appended_column(self.getRawPredictionCol(), cols["raw"])
-        out = out.with_appended_column(self.getProbabilityCol(), cols["prob"])
-        return out.with_appended_column(self.getOrDefault("predictionCol"), cols["pred"])
+    def _transform_outputs(self) -> List[Tuple[str, str]]:
+        return [(self.getRawPredictionCol(), "array<double>"), (self.getProbabilityCol(), "array<double>"),
+                (self.getOrDefault("predictionCol"), "double")]
 
 
 def _dense(values: Sequence[float]) -> Any:

@@ -17,14 +17,14 @@ raises NotImplementedError.
 """
 from __future__ import annotations
 
+import functools
 from typing import Any, Callable, Dict, List, Optional, Sequence, Tuple, Union
 
 import numpy as np
-import pandas as pd
 import pyarrow as pa
 
-from .core import (FitInputType, _append_transform_features, _CumlCaller, _CumlEstimator, _CumlModelWithPredictionCol,
-                   _transform_context, alias, param_alias)
+from .core import (FitInputType, _CumlCaller, _CumlEstimator, _CumlModelWithPredictionCol, _DeviceModel, alias,
+                   param_alias)
 from .params import HasFeaturesCol, HasFeaturesCols, HasIDCol, HasPredictionCol, P, _CumlClass, _CumlParams, _KMeansParams
 from .sparkshim import HAVE_PYSPARK, Param, Row, TypeConverters, keyword_only
 from .utils import get_logger
@@ -265,52 +265,11 @@ class KMeansModel(KMeansClass, _CumlModelWithPredictionCol, _KMeansCumlParams):
 
     def _get_cuml_transform_func(self, dataset: Any, eval_metric_info: Any = None
                                  ) -> Tuple[Callable, Callable, Optional[Callable]]:
-        cluster_centers_ = self.cluster_centers_
-        n_cols = self.n_cols
-
-        class _DeviceKMeans:  # the injected-centers predictor (clustering.py:582-596)
-            def __init__(self, gpu: int) -> None:
-                import torch
-
-                self.ctx = _transform_context(gpu)
-                self.C = torch.tensor(cluster_centers_, dtype=torch.float32, device=self.ctx.device)
-
-            def close(self) -> None:   # the context (pinned staging, scratch, copy threads) stays with the process
-                self.C = None
-
-        def _construct_kmeans(gpu: int = 0) -> Any:
-            return _DeviceKMeans(gpu)
-
-        def _transform_many(kmeans: Any, dfs: List[Union[pd.DataFrame, np.ndarray]]) -> List[pd.Series]:
-            """Several input batches in ONE device pass: every batch is ingested into the same device matrix, one
-            b2k_kmeans_assign labels all rows, one read-back, one Series per input batch (same order, same lengths).
-            The per-batch host overhead (allocation, launches, a synchronising read-back) is what a 10 000-row Arrow batch
-            costs most; core._iter_transform groups batches up to ~1 M rows."""
-            from .utils import DeviceRowAppender
-
-            sizes = [len(df) for df in dfs]
-            total = sum(sizes)
-            if total == 0:
-                return [pd.Series([], dtype="int32") for _ in dfs]
-            app = DeviceRowAppender(kmeans.ctx, n_cols, first_capacity=total)
-            for df, n_b in zip(dfs, sizes):
-                if n_b:
-                    _append_transform_features(app, df, n_cols)
-            X = app.finish()
-            labels, _ = kmeans.ctx.kmeans_assign(X, kmeans.C)
-            host = labels.cpu().numpy()
-            out, o = [], 0
-            for n_b in sizes:
-                out.append(pd.Series(host[o:o + n_b]))
-                o += n_b
-            return out
-
-        def _transform_internal(kmeans: Any, df: Union[pd.DataFrame, np.ndarray]) -> pd.Series:
-            return _transform_many(kmeans, [df])[0]
-
-        _transform_internal.many = _transform_many  # type: ignore[attr-defined]
-        _transform_internal.row_bytes = 4 * int(n_cols or 1)  # type: ignore[attr-defined]
-        return _construct_kmeans, _transform_internal, None
+        # the injected-centers predictor (clustering.py:582-596): b2k_kmeans_assign labels a group's rows
+        construct = functools.partial(_DeviceModel, C=np.asarray(self.cluster_centers_, dtype=np.float32))
+        transform = self._grouped_transform(lambda m, X: (m.ctx.kmeans_assign(X, m.arrays["C"])[0],),
+                                            4 * int(self.n_cols or 1))
+        return construct, transform, None
 
 
 # ---- DBSCAN (reference: clustering.py:607-1186) ----

@@ -25,7 +25,7 @@ import os
 import uuid
 from abc import abstractmethod
 from collections import namedtuple
-from typing import Any, Callable, Dict, Iterator, List, Optional, Sequence, Tuple, Union
+from typing import Any, Callable, Dict, Iterable, Iterator, List, Optional, Sequence, Tuple, Union
 
 import numpy as np
 import pandas as pd
@@ -174,20 +174,78 @@ def _close_transform_contexts() -> None:
         _TRANSFORM_CONTEXTS.clear()
 
 
+class _DeviceModel:
+    """A model placed on one GPU for transform and evaluation: the process's context for that GPU and the model's
+    arrays, uploaded once with their NumPy dtype."""
+
+    def __init__(self, gpu: int, **arrays: np.ndarray) -> None:
+        import torch
+
+        self.ctx = _transform_context(gpu)
+        self.arrays = {k: torch.from_numpy(np.ascontiguousarray(a)).to(self.ctx.device) for k, a in arrays.items()}
+
+    def close(self) -> None:   # the context (pinned staging, scratch, copy threads) stays with the process
+        self.arrays = {}
+
+
 _ARROW_SCALARS = {"int": pa.int32(), "float": pa.float32(), "double": pa.float64()}
 
 
-def _transform_result_array(res: Any, out_type: str) -> pa.Array:
-    """One transform result (a pandas Series) as the Arrow array of the model's output type: "int" or "array<float>" /
-    "array<double>" (one fixed-width vector per row)."""
+def _out_dtype(out_type: str) -> Any:
+    """The NumPy dtype of an output type's values: "int" / "double", or the element of "array<float>" / "array<double>"."""
+    return _ARROW_SCALARS[out_type[len("array<"):-1] if out_type.startswith("array<") else out_type].to_pandas_dtype()
+
+
+def _transform_result_array(res: np.ndarray, out_type: str) -> pa.Array:
+    """One output of one frame as the Arrow array of its type: one value per row ("int", "double") or, from a 2-D
+    array, one fixed-width vector per row ("array<float>", "array<double>")."""
     if out_type.startswith("array<"):
         elem = _ARROW_SCALARS[out_type[len("array<"):-1]]
-        rows = list(res)
-        width = len(rows[0]) if rows else 0
-        vals = np.asarray(rows, dtype=elem.to_pandas_dtype()).reshape(-1) if rows else np.zeros(0, elem.to_pandas_dtype())
-        offsets = np.arange(0, len(rows) * width + 1, max(width, 1), dtype=np.int32)[: len(rows) + 1]
+        vals = np.ascontiguousarray(res, dtype=elem.to_pandas_dtype()).reshape(-1)
+        offsets = np.arange(len(res) + 1, dtype=np.int32) * np.int32(res.shape[1])
         return pa.ListArray.from_arrays(pa.array(offsets), pa.array(vals, type=elem))
-    return pa.array(np.asarray(res), type=_ARROW_SCALARS[out_type])
+    return pa.array(np.asarray(res, dtype=_out_dtype(out_type)), type=_ARROW_SCALARS[out_type])
+
+
+def _ingest(ctx: Any, frames: Iterable[Any], n_cols: int, rows: int) -> Any:
+    """Every non-empty frame, in order, as the rows of one device matrix (`rows` in all)."""
+    app = DeviceRowAppender(ctx, n_cols, first_capacity=max(1, rows))
+    for f in frames:
+        if len(f):
+            _append_transform_features(app, f, n_cols)
+    return app.finish()
+
+
+class _GroupedTransform:
+    """A model's transform function: a group of frames in one device pass.  Every non-empty frame is ingested into one
+    device matrix, `predict(device_model, X)` returns one CUDA tensor per output type (the first dimension is the row),
+    each output is read back once, and each frame gets its rows of every output, in order.  A group without rows makes
+    no device call: its frames get zero-length outputs of each type's dtype.  `row_bytes`, the device bytes per row,
+    bounds a group's size (TRANSFORM_GROUP_BYTES)."""
+
+    def __init__(self, predict: Callable[[Any, Any], Sequence[Any]], n_cols: int, row_bytes: int,
+                 out_types: Sequence[str]) -> None:
+        self.predict = predict
+        self.n_cols = n_cols
+        self.row_bytes = row_bytes
+        self.out_types = list(out_types)
+
+    def __call__(self, model: Any, frames: List[Any]) -> List[Tuple[np.ndarray, ...]]:
+        sizes = [len(f) for f in frames]
+        total = sum(sizes)
+        if total == 0:
+            return [tuple(np.zeros((0, 0) if t.startswith("array<") else 0, _out_dtype(t)) for t in self.out_types)
+                    for _ in frames]
+        host = [t.cpu().numpy() for t in self.predict(model, _ingest(model.ctx, frames, self.n_cols, total))]
+        ends = np.cumsum(sizes)
+        return [tuple(h[e - n:e] for h in host) for n, e in zip(sizes, ends)]
+
+
+def _select_features(batches: Iterable[pa.RecordBatch], input_col: Optional[str],
+                     input_cols: Optional[List[str]]) -> Iterator[pa.RecordBatch]:
+    """The feature columns of each batch, a single one renamed to alias.data at the Arrow level (zero-copy)."""
+    for b in batches:
+        yield b.select(list(input_cols)) if input_cols else b.select([input_col]).rename_columns([alias.data])
 
 
 
@@ -462,31 +520,31 @@ class _CumlEstimator(EstimatorBase, _CumlCaller):
         return cls.read().load(path)
 
 
-TRANSFORM_GROUP_ROWS = 1 << 20    # rows labelled per device pass when the transform function can take several batches ...
-TRANSFORM_GROUP_BYTES = 2 << 30   # ... and the cap on the device matrix they form (transform function's `row_bytes`)
+TRANSFORM_GROUP_ROWS = 1 << 20    # rows per device pass of transform and evaluation ...
+TRANSFORM_GROUP_BYTES = 2 << 30   # ... and the cap on the device bytes they take (`row_bytes` per row)
 
 
-def _iter_transform(transform_internal: Callable, get_model: Callable[[], Any], frames: Iterator[Any]) -> Iterator[Any]:
-    """One result per input frame, in order.  When the model's transform function offers `.many` (KMeans), consecutive
-    frames are grouped up to TRANSFORM_GROUP_ROWS rows and labelled in one device pass; otherwise frame by frame, as the
-    reference does (core.py:1900-1915)."""
-    many = getattr(transform_internal, "many", None)
-    if many is None:
-        for f in frames:
-            yield transform_internal(get_model(), f)
-        return
-    row_bytes = max(1, int(getattr(transform_internal, "row_bytes", 1)))
-    limit = max(1, min(TRANSFORM_GROUP_ROWS, TRANSFORM_GROUP_BYTES // row_bytes))
+def _row_groups(items: Iterable[Any], row_bytes: int) -> Iterator[List[Any]]:
+    """Consecutive frames or batches, in order, in groups that end once they reach TRANSFORM_GROUP_ROWS rows or
+    TRANSFORM_GROUP_BYTES at `row_bytes` per row; the last group may be smaller."""
+    limit = max(1, min(TRANSFORM_GROUP_ROWS, TRANSFORM_GROUP_BYTES // max(1, row_bytes)))
     group: List[Any] = []
     rows = 0
-    for f in frames:
-        group.append(f)
-        rows += len(f)
+    for it in items:
+        group.append(it)
+        rows += len(it)
         if rows >= limit:
-            yield from many(get_model(), group)
+            yield group
             group, rows = [], 0
     if group:
-        yield from many(get_model(), group)
+        yield group
+
+
+def _iter_transform(transform: Callable, model: Any, frames: Iterable[Any]) -> Iterator[Any]:
+    """One result per input frame, in order: `transform` (a model's grouped transform function) takes each group of
+    consecutive frames in one device pass."""
+    for group in _row_groups(frames, transform.row_bytes):
+        yield from transform(model, group)
 
 
 def _supports_transform_evaluate(classification: bool, evaluator: Any) -> bool:
@@ -536,7 +594,6 @@ def _transform_evaluate_internal(model: Any, dataset: Any, evaluator: Any) -> Li
     first group), and one curve pass over them gives every model's area at the end."""
     from . import metrics
     from .sparkshim.sql import _batches_to_pdf_iter
-    from .utils import DeviceRowAppender
 
     if HAVE_PYSPARK:
         from . import spark_binding
@@ -558,16 +615,11 @@ def _transform_evaluate_internal(model: Any, dataset: Any, evaluator: Any) -> Li
         nonlocal accs
         import torch
 
-        feats = [b.select(list(input_cols)) if input_cols else b.select([input_col]).rename_columns([alias.data])
-                 for b in group]
         y = np.concatenate([np.asarray(b.column(label_col).to_numpy(zero_copy_only=False), dtype=np.float32)
                             for b in group]) if group else np.zeros(0, np.float32)
         m = state["model"]
-        app = DeviceRowAppender(m.ctx, n_cols, first_capacity=max(1, int(y.size)))
-        for pdf in _batches_to_pdf_iter(feats, dataset.arrow_backed_pandas):
-            if len(pdf):
-                _append_transform_features(app, pdf, n_cols)
-        X = app.finish()
+        X = _ingest(m.ctx, _batches_to_pdf_iter(_select_features(group, input_col, input_cols),
+                                                dataset.arrow_backed_pandas), n_cols, int(y.size))
         yd = torch.as_tensor(y).to(m.ctx.device)
         if binary:
             evaluate(m, X, yd, state["scores"], state["pos"], state["row0"])
@@ -578,7 +630,6 @@ def _transform_evaluate_internal(model: Any, dataset: Any, evaluator: Any) -> Li
         accs = got if accs is None else [metrics.merge_all([a, b], info["classification"]) for a, b in zip(accs, got)]
 
     binary = info["binary"]
-    limit = max(1, min(TRANSFORM_GROUP_ROWS, TRANSFORM_GROUP_BYTES // (4 * n_cols + 4)))   # as _iter_transform
     for pid, part in enumerate(dataset._parts):
         if "model" not in state:
             gpu = _CumlCommon._set_gpu_device(BarrierTaskContext(pid, len(dataset._parts)), True, True)
@@ -586,16 +637,10 @@ def _transform_evaluate_internal(model: Any, dataset: Any, evaluator: Any) -> Li
             if binary:
                 state["scores"], state["pos"] = state["model"].ctx.binary_buffers(evaluate.n_models, dataset.count())
                 state["row0"] = 0
-        group: List[pa.RecordBatch] = []
-        rows = 0
-        for batch in part:
-            group.append(batch)
-            rows += batch.num_rows
-            if rows >= limit:
-                run(group)
-                group, rows = [], 0
-        if group or accs is None:
+        for group in _row_groups(part, 4 * n_cols + 4):   # X and the float32 label
             run(group)
+        if accs is None:   # the first partition is empty: one pass over no rows still gives every model's accumulators
+            run([])
     assert accs is not None
     if binary:
         return [float(v) for v in state["model"].ctx.eval_binary(state["scores"], state["pos"], info["numBins"],
@@ -841,6 +886,16 @@ class _CumlModel(ModelBase, _CumlParams, _CumlCommon):
         return _transform_evaluate_internal(self.copy(params) if params else self, dataset, evaluator)
 
 
+def _no_spark_transform(model: Any, dataset: Any) -> None:
+    """transform() of a pyspark DataFrame is a pandas_udf of one output column: other models refuse it."""
+    if HAVE_PYSPARK:
+        from . import spark_binding
+
+        if spark_binding.is_spark_dataframe(dataset):
+            raise NotImplementedError(f"{type(model).__name__}.transform() of a pyspark DataFrame is not supported in "
+                                      "this build; transform a local frame")
+
+
 class _CumlModelWithColumns(_CumlModel):
     """reference: core.py:1797-1941 — keeps the input columns and appends the output column."""
 
@@ -848,7 +903,22 @@ class _CumlModelWithColumns(_CumlModel):
         """The column transform() appends: predictionCol here, outputCol for a feature transformer."""
         return self.getOrDefault("predictionCol")
 
+    def _transform_outputs(self) -> List[Tuple[str, str]]:
+        """The (column name, Arrow type) of each column transform() appends, in order: one per output of the grouped
+        transform function."""
+        return [(self._output_col_name(), self._out_schema(None))]
+
+    def _grouped_transform(self, predict: Callable[[Any, Any], Sequence[Any]], row_bytes: int) -> _GroupedTransform:
+        """This model's grouped transform function: `predict(device_model, X)` returns one CUDA tensor per column of
+        _transform_outputs(); `row_bytes` is the device bytes a row takes."""
+        return _GroupedTransform(predict, int(self.n_cols), row_bytes, [t for _, t in self._transform_outputs()])
+
     def _transform(self, dataset: Any) -> Any:
+        from .sparkshim.sql import _batches_to_pdf_iter
+
+        outputs = self._transform_outputs()
+        if len(outputs) > 1:
+            _no_spark_transform(self, dataset)
         if HAVE_PYSPARK:
             from . import spark_binding
 
@@ -856,34 +926,25 @@ class _CumlModelWithColumns(_CumlModel):
                 return spark_binding.transform_with_pandas_udf(
                     self, dataset, alias.data, lambda ctx, local: _CumlCommon._set_gpu_device(ctx, local, True))
         input_col, input_cols = self._get_input_columns()
-        construct, transform_internal, _ = self._get_cuml_transform_func(dataset)
-        pred_name = self._output_col_name()
-        out_type = self._out_schema(dataset.schema)
-        n_cols = self.n_cols
-        out_parts: List[List[pa.Array]] = []
-        state: Dict[str, Any] = {}
+        construct, transform, _ = self._get_cuml_transform_func(dataset)
+        cols: List[List[List[pa.Array]]] = [[] for _ in outputs]   # output -> partition -> one array per batch
+        model = None
         for pid, part in enumerate(dataset._parts):
-            def frames(part: Any = part, pid: int = pid) -> Iterator[Any]:
-                from .sparkshim.sql import _batches_to_pdf_iter
-
-                def selected() -> Iterator[pa.RecordBatch]:   # feature columns only, renamed at the Arrow level (zero-copy)
-                    for batch in part:
-                        if "model" not in state:
-                            gpu = _CumlCommon._set_gpu_device(BarrierTaskContext(pid, len(dataset._parts)), True, True)
-                            state["model"] = construct(gpu)
-                        if input_cols:
-                            yield batch.select(list(input_cols))
-                        else:
-                            yield batch.select([input_col]).rename_columns([alias.data])
-
-                return _batches_to_pdf_iter(selected(), dataset.arrow_backed_pandas)
-
-            out_parts.append([_transform_result_array(res, out_type)
-                              for res in _iter_transform(transform_internal, lambda: state["model"], frames())])
-        if "model" in state and hasattr(state["model"], "close"):
-            state["model"].close()
-        assert n_cols is None or n_cols > 0
-        return dataset.with_appended_column(pred_name, out_parts)
+            if part and model is None:   # on the GPU of the first partition with a batch
+                model = construct(_CumlCommon._set_gpu_device(BarrierTaskContext(pid, len(dataset._parts)), True, True))
+            frames = _batches_to_pdf_iter(_select_features(part, input_col, input_cols), dataset.arrow_backed_pandas)
+            per: List[List[pa.Array]] = [[] for _ in outputs]
+            for res in _iter_transform(transform, model, frames):
+                for arrs, r, (_, out_type) in zip(per, res, outputs):
+                    arrs.append(_transform_result_array(r, out_type))
+            for c, arrs in zip(cols, per):
+                c.append(arrs)
+        if model is not None:
+            model.close()
+        out = dataset
+        for (name, _), parts in zip(outputs, cols):
+            out = out.with_appended_column(name, parts)
+        return out
 
 
 class _CumlModelWithPredictionCol(_CumlModelWithColumns):

@@ -19,14 +19,13 @@ matrix from the worker scaffold instead of host arrays.
 """
 from __future__ import annotations
 
+import functools
 import itertools
 from typing import Any, Callable, Dict, List, Optional, Tuple, Union
 
 import numpy as np
-import pandas as pd
 
-from .core import (FitInputType, _append_transform_features, _CumlEstimator, _CumlModelWithColumns,
-                   _transform_context, param_alias)
+from .core import FitInputType, _CumlEstimator, _CumlModelWithColumns, _DeviceModel, param_alias
 from .params import HasInputCols, P, _CumlClass, _CumlParams, _PCAParams
 from .sparkshim import Row, keyword_only
 
@@ -185,45 +184,7 @@ class PCAModel(PCAClass, _CumlModelWithColumns, _PCACumlParams):
 
     def _get_cuml_transform_func(self, dataset: Any, eval_metric_info: Any = None
                                  ) -> Tuple[Callable, Callable, Optional[Callable]]:
-        components_ = self.components_
-        n_cols = int(self.n_cols)
-
-        class _DevicePCA:
-            def __init__(self, gpu: int) -> None:
-                import torch
-
-                self.ctx = _transform_context(gpu)
-                self.C = torch.tensor(components_, dtype=torch.float32, device=self.ctx.device)
-
-            def close(self) -> None:   # the context stays with the process
-                self.C = None
-
-        def _construct_pca(gpu: int = 0) -> Any:
-            return _DevicePCA(gpu)
-
-        def _transform_many(pca: Any, dfs: List[Union[pd.DataFrame, np.ndarray]]) -> List[pd.Series]:
-            """Several input batches in ONE device pass: every batch is ingested into the same device matrix, one
-            b2k_pca_transform projects all rows, one read-back, one Series per input batch."""
-            from .utils import DeviceRowAppender
-
-            sizes = [len(df) for df in dfs]
-            total = sum(sizes)
-            if total == 0:
-                return [pd.Series([], dtype=object) for _ in dfs]
-            app = DeviceRowAppender(pca.ctx, n_cols, first_capacity=total)
-            for df, n_b in zip(dfs, sizes):
-                if n_b:
-                    _append_transform_features(app, df, n_cols)
-            host = pca.ctx.pca_transform(app.finish(), pca.C).cpu().numpy()
-            out, o = [], 0
-            for n_b in sizes:
-                out.append(pd.Series(list(host[o:o + n_b])))
-                o += n_b
-            return out
-
-        def _transform_internal(pca: Any, df: Union[pd.DataFrame, np.ndarray]) -> pd.Series:
-            return _transform_many(pca, [df])[0]
-
-        _transform_internal.many = _transform_many  # type: ignore[attr-defined]
-        _transform_internal.row_bytes = 4 * (n_cols + len(components_))  # type: ignore[attr-defined]
-        return _construct_pca, _transform_internal, None
+        construct = functools.partial(_DeviceModel, C=np.asarray(self.components_, dtype=np.float32))
+        transform = self._grouped_transform(lambda m, X: (m.ctx.pca_transform(X, m.arrays["C"]),),
+                                            4 * (int(self.n_cols) + len(self.components_)))
+        return construct, transform, None

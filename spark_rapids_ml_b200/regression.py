@@ -22,15 +22,14 @@ evaluate() and summary raise NotImplementedError; loss="huber", solver="l-bfgs" 
 """
 from __future__ import annotations
 
+import functools
 import threading
 from typing import Any, Callable, Dict, Iterator, List, Optional, Sequence, Tuple, Union
 
 import numpy as np
-import pandas as pd
 import pyarrow as pa
 
-from .core import (FitInputType, _append_transform_features, _CumlEstimator, _CumlModelWithPredictionCol,
-                   _transform_context, alias, param_alias)
+from .core import FitInputType, _CumlEstimator, _CumlModelWithPredictionCol, _DeviceModel, alias, param_alias
 from .params import HasFeaturesCol, HasFeaturesCols, HasLabelCol, HasPredictionCol, P, _CumlClass, _CumlParams
 from .sparkshim import LocalDataFrame, Param, Row, TypeConverters, keyword_only
 
@@ -391,51 +390,14 @@ class LinearRegressionModel(LinearRegressionClass, _CumlModelWithPredictionCol, 
             return self._eval_func(eval_metric_info)
         if isinstance(self.intercept_, (list, tuple)):
             raise NotImplementedError("transform() of a combined multi-model instance is not supported")
-        coef_, intercept_ = self.coef_, float(self.intercept_)
-        n_cols = int(self.n_cols)
-
-        class _DeviceLinReg:
-            def __init__(self, gpu: int) -> None:
-                import torch
-
-                self.ctx = _transform_context(gpu)
-                self.w = torch.tensor(coef_, dtype=torch.float64, device=self.ctx.device)
-
-            def close(self) -> None:   # the context stays with the process
-                self.w = None
-
-        def _construct(gpu: int = 0) -> Any:
-            return _DeviceLinReg(gpu)
-
-        def _transform_many(lr: Any, dfs: List[Union[pd.DataFrame, np.ndarray]]) -> List[pd.Series]:
-            """Several input batches in ONE device pass: every batch is ingested into the same device matrix, one
-            b2k_linreg_predict covers all rows, one read-back, one Series per input batch."""
-            from .utils import DeviceRowAppender
-
-            sizes = [len(df) for df in dfs]
-            total = sum(sizes)
-            if total == 0:
-                return [pd.Series([], dtype="float64") for _ in dfs]
-            app = DeviceRowAppender(lr.ctx, n_cols, first_capacity=total)
-            for df, n_b in zip(dfs, sizes):
-                if n_b:
-                    _append_transform_features(app, df, n_cols)
-            host = lr.ctx.linreg_predict(app.finish(), lr.w, intercept_).cpu().numpy()
-            out, o = [], 0
-            for n_b in sizes:
-                out.append(pd.Series(host[o:o + n_b]))
-                o += n_b
-            return out
-
-        def _transform_internal(lr: Any, df: Union[pd.DataFrame, np.ndarray]) -> pd.Series:
-            return _transform_many(lr, [df])[0]
-
-        _transform_internal.many = _transform_many  # type: ignore[attr-defined]
-        _transform_internal.row_bytes = 4 * n_cols + 8  # type: ignore[attr-defined]
-        return _construct, _transform_internal, None
+        intercept_ = float(self.intercept_)
+        construct = functools.partial(_DeviceModel, w=np.asarray(self.coef_, dtype=np.float64))
+        transform = self._grouped_transform(lambda m, X: (m.ctx.linreg_predict(X, m.arrays["w"], intercept_),),
+                                            4 * int(self.n_cols) + 8)
+        return construct, transform, None
 
     def _eval_func(self, info: Dict[str, Any]) -> Tuple[Callable, Any, Callable]:
-        """(construct, None, evaluate): evaluate(holder, X, y) scores every model on one device pass
+        """(construct, None, evaluate): evaluate(device model, X, y) scores every model on one device pass
         (b2k_eval_linear, identity kind) and returns their accumulators."""
         from .core import _class_accs
 
@@ -443,14 +405,10 @@ class LinearRegressionModel(LinearRegressionClass, _CumlModelWithPredictionCol, 
             raise NotImplementedError("LinearRegressionModel is evaluated with a RegressionEvaluator")
         models = [{"kind": "identity", "W": np.asarray([c], dtype=np.float64), "b": [b]} for c, b in self._models()]
 
-        class _Holder:
-            def __init__(self, gpu: int) -> None:
-                self.ctx = _transform_context(gpu)
-
         def _evaluate(h: Any, X: Any, y: Any) -> List[Dict[str, Any]]:
             return _class_accs(h.ctx.eval_linear(X, y, models))
 
-        return _Holder, None, _evaluate
+        return _DeviceModel, None, _evaluate
 
 
 from .tree import _RandomForestEstimator, _RandomForestModel  # noqa: E402  (tree.py imports this module lazily)

@@ -170,7 +170,7 @@ def transform_with_pandas_udf(model: Any, dataset: Any, data_alias: str, set_gpu
     from pyspark.sql.functions import col, pandas_udf, struct
 
     input_col, input_cols = model._get_input_columns()
-    construct, transform_internal, _ = model._get_cuml_transform_func(dataset)
+    construct, transform, _ = model._get_cuml_transform_func(dataset)
     local = is_local(dataset)
     if input_col is not None:
         dtype = dataset.schema[input_col].dataType
@@ -188,12 +188,12 @@ def transform_with_pandas_udf(model: Any, dataset: Any, data_alias: str, set_gpu
         gpu = set_gpu(TaskContext.get(), local)
         device_model = construct(gpu)
         try:
-            from .core import _iter_transform   # groups consecutive batches into one device pass where possible
+            from .core import _iter_transform   # groups consecutive batches into one device pass
 
-            yield from _iter_transform(transform_internal, lambda: device_model, iterator)
+            for (res,) in _iter_transform(transform, device_model, iterator):
+                yield pd.Series(list(res) if res.ndim == 2 else res)   # one vector per row: an array<...> column
         finally:
-            if hasattr(device_model, "close"):
-                device_model.close()
+            device_model.close()
 
     return dataset.withColumn(model._output_col_name(), predict_udf(struct(*select_cols)))
 

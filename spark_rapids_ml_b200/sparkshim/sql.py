@@ -312,8 +312,15 @@ class LocalDataFrame:
         return self._derive(parts, pa.schema([pa.field(name, pa.int64())] + list(self._schema)))
 
     def with_appended_column(self, name: str, per_partition_arrays: List[List[pa.Array]]) -> "LocalDataFrame":
+        """Column `name` appended from one array per batch of each partition; a missing or extra array is an error
+        rather than rows dropped from the frame."""
+        if len(per_partition_arrays) != len(self._parts):
+            raise ValueError(f"column '{name}': {len(per_partition_arrays)} partitions of arrays for a frame of "
+                             f"{len(self._parts)} partitions")
         parts = []
-        for p, arrs in zip(self._parts, per_partition_arrays):
+        for pid, (p, arrs) in enumerate(zip(self._parts, per_partition_arrays)):
+            if len(arrs) != len(p):
+                raise ValueError(f"column '{name}': partition {pid} has {len(p)} batches but {len(arrs)} arrays")
             parts.append([b.append_column(name, a) for b, a in zip(p, arrs)])
         return self._derive(parts)
 

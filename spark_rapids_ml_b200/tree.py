@@ -21,13 +21,12 @@ import math
 from typing import Any, Callable, Dict, Iterator, List, Optional, Sequence, Tuple, Union
 
 import numpy as np
-import pandas as pd
 import pyarrow as pa
 
-from .core import FitInputType, _append_transform_features, _CumlEstimator, _CumlModelWithPredictionCol, _CumlCommon
-from .core import _transform_context, alias, param_alias
+from .core import (FitInputType, _CumlEstimator, _CumlModelWithPredictionCol, _DeviceModel, _no_spark_transform, alias,
+                   param_alias)
 from .params import HasFeaturesCol, HasFeaturesCols, HasLabelCol, HasPredictionCol, P, _CumlClass, _CumlParams
-from .sparkshim import BarrierTaskContext, LocalDataFrame, Param, Row, TypeConverters
+from .sparkshim import LocalDataFrame, Param, Row, TypeConverters
 
 MAX_DEPTH = 16          # b2k_rf_fit's limit
 MAX_BINS = (2, 256)     # bins are uint8
@@ -553,54 +552,30 @@ class _RandomForestModel(_RandomForestClass, _CumlModelWithPredictionCol, _Rando
         if eval_metric_info is not None:
             return self._eval_func(eval_metric_info)
         forest = self._flat()
-        n_cols = int(self.n_cols)
         classification = self._is_classification()
+
+        def predict(m: Any, X: Any) -> Tuple[Any, ...]:   # k_rf_predict: (raw, prob, pred), or (None, None, pred)
+            raw, prob, pred = m.ctx.rf_predict(X, forest, classification)
+            return (raw, prob, pred) if classification else (pred,)
+
         V = int(forest["value"].shape[1])
+        return _DeviceModel, self._grouped_transform(predict, 4 * int(self.n_cols) + 8 * (2 * V + 1)), None
 
-        class _DeviceForest:
-            def __init__(self, gpu: int) -> None:
-                self.ctx = _transform_context(gpu)
+    def _transform_outputs(self) -> List[Tuple[str, str]]:
+        pred = (self.getOrDefault("predictionCol"), "double")
+        if not self._is_classification():
+            return [pred]
+        return [(self.getOrDefault("rawPredictionCol"), "array<double>"),
+                (self.getOrDefault("probabilityCol"), "array<double>"), pred]
 
-            def close(self) -> None:   # the context stays with the process
-                pass
-
-        def _construct(gpu: int = 0) -> Any:
-            return _DeviceForest(gpu)
-
-        def _transform_many(m: Any, dfs: List[Union[pd.DataFrame, np.ndarray]]) -> List[pd.DataFrame]:
-            """Several input batches in ONE device pass (k_rf_predict), one frame per input batch."""
-            from .utils import DeviceRowAppender
-
-            sizes = [len(df) for df in dfs]
-            total = sum(sizes)
-            if total == 0:
-                return [pd.DataFrame({"raw": [], "prob": [], "pred": pd.Series([], dtype="float64")}) for _ in dfs]
-            app = DeviceRowAppender(m.ctx, n_cols, first_capacity=total)
-            for df, n_b in zip(dfs, sizes):
-                if n_b:
-                    _append_transform_features(app, df, n_cols)
-            raw, prob, pred = m.ctx.rf_predict(app.finish(), forest, classification)
-            pred = pred.cpu().numpy()
-            raw = raw.cpu().numpy() if raw is not None else np.zeros((total, 0))
-            prob = prob.cpu().numpy() if prob is not None else np.zeros((total, 0))
-            out, o = [], 0
-            for n_b in sizes:
-                out.append(pd.DataFrame({"raw": list(raw[o:o + n_b]), "prob": list(prob[o:o + n_b]),
-                                         "pred": pred[o:o + n_b]}))
-                o += n_b
-            return out
-
-        def _transform_internal(m: Any, df: Union[pd.DataFrame, np.ndarray]) -> pd.DataFrame:
-            return _transform_many(m, [df])[0]
-
-        _transform_internal.many = _transform_many  # type: ignore[attr-defined]
-        _transform_internal.row_bytes = 4 * n_cols + 8 * (2 * V + 1)  # type: ignore[attr-defined]
-        return _construct, _transform_internal, None
+    def _transform(self, dataset: Any) -> Any:
+        _no_spark_transform(self, dataset)   # the regressor too: a forest has no pandas_udf transform
+        return super()._transform(dataset)
 
     def _eval_func(self, info: Dict[str, Any]) -> Tuple[Callable, Any, Callable]:
-        """(construct, None, evaluate): evaluate(holder, X, y) scores every forest of this (combined) model in one
-        device pass (b2k_eval_forest) and returns their accumulators; for a BinaryClassificationEvaluator,
-        evaluate(holder, X, y, scores, pos, row0) writes their binary scores (b2k_eval_forest_scores) instead."""
+        """(construct, None, evaluate): evaluate(device model, X, y) scores every forest of this (combined) model in
+        one device pass (b2k_eval_forest) and returns their accumulators; for a BinaryClassificationEvaluator,
+        evaluate(device model, X, y, scores, pos, row0) writes their binary scores (b2k_eval_forest_scores) instead."""
         from .core import _class_accs
 
         classification = self._is_classification()
@@ -612,68 +587,14 @@ class _RandomForestModel(_RandomForestClass, _CumlModelWithPredictionCol, _Rando
         forests = [json_to_forest(j, V) for j in jsons]
         eps = info["eps"]
 
-        class _Holder:
-            def __init__(self, gpu: int) -> None:
-                self.ctx = _transform_context(gpu)
-
         if info["binary"]:
             def _scores(h: Any, X: Any, y: Any, scores: Any, pos: Any, row0: int) -> None:
                 h.ctx.binary_scores_forest(X, y, forests, scores, pos, row0)
 
             _scores.n_models = len(forests)  # type: ignore[attr-defined]
-            return _Holder, None, _scores
+            return _DeviceModel, None, _scores
 
         def _evaluate(h: Any, X: Any, y: Any) -> List[Dict[str, Any]]:
             return _class_accs(h.ctx.eval_forest(X, y, forests, classification, eps))
 
-        return _Holder, None, _evaluate
-
-    def _transform(self, dataset: Any) -> Any:
-        """Appends rawPredictionCol and probabilityCol (list<double>, classification) and predictionCol (double) to a
-        local frame."""
-        from .core import HAVE_PYSPARK, _iter_transform
-
-        if HAVE_PYSPARK:
-            from . import spark_binding
-
-            if spark_binding.is_spark_dataframe(dataset):
-                raise NotImplementedError(f"{type(self).__name__}.transform() of a pyspark DataFrame is not supported in "
-                                          "this build; transform a local frame")
-        input_col, input_cols = self._get_input_columns()
-        construct, transform_internal, _ = self._get_cuml_transform_func(dataset)
-        classification = self._is_classification()
-        cols: Dict[str, List[List[pa.Array]]] = {"raw": [], "prob": [], "pred": []}
-        state: Dict[str, Any] = {}
-        for pid, part in enumerate(dataset._parts):
-            def frames(part: Any = part, pid: int = pid) -> Iterator[Any]:
-                from .sparkshim.sql import _batches_to_pdf_iter
-
-                def selected() -> Iterator[pa.RecordBatch]:
-                    for batch in part:
-                        if "model" not in state:
-                            gpu = _CumlCommon._set_gpu_device(BarrierTaskContext(pid, len(dataset._parts)), True, True)
-                            state["model"] = construct(gpu)
-                        if input_cols:
-                            yield batch.select(list(input_cols))
-                        else:
-                            yield batch.select([input_col]).rename_columns([alias.data])
-
-                return _batches_to_pdf_iter(selected(), dataset.arrow_backed_pandas)
-
-            per: Dict[str, List[pa.Array]] = {k: [] for k in cols}
-            for res in _iter_transform(transform_internal, lambda: state["model"], frames()):
-                if classification:
-                    for k in ("raw", "prob"):
-                        rows = list(res[k])
-                        width = len(rows[0]) if rows else 0
-                        vals = np.asarray(rows, dtype=np.float64).reshape(-1) if rows else np.zeros(0)
-                        offs = np.arange(0, len(rows) * width + 1, max(width, 1), dtype=np.int32)[: len(rows) + 1]
-                        per[k].append(pa.ListArray.from_arrays(pa.array(offs), pa.array(vals, type=pa.float64())))
-                per["pred"].append(pa.array(np.asarray(res["pred"], dtype=np.float64), type=pa.float64()))
-            for k in cols:
-                cols[k].append(per[k])
-        out = dataset
-        if classification:
-            out = out.with_appended_column(self.getOrDefault("rawPredictionCol"), cols["raw"])
-            out = out.with_appended_column(self.getOrDefault("probabilityCol"), cols["prob"])
-        return out.with_appended_column(self.getOrDefault("predictionCol"), cols["pred"])
+        return _DeviceModel, None, _evaluate

@@ -12,16 +12,16 @@ accepted and unused.  The layout is the epoch-synchronous, deterministic form of
 """
 from __future__ import annotations
 
+import functools
 import json
 import os
 from typing import Any, Callable, Dict, List, Optional, Tuple, Union
 
 import numpy as np
-import pandas as pd
 import pyarrow as pa
 
-from .core import (FitInputType, _append_transform_features, _CumlEstimator, _CumlModelWithColumns, _save_metadata,
-                   _load_metadata, _reset_uid, _set_params_from_metadata, _transform_context, alias, param_alias)
+from .core import (FitInputType, _CumlEstimator, _CumlModelWithColumns, _DeviceModel, _save_metadata, _load_metadata,
+                   _reset_uid, _set_params_from_metadata, alias, param_alias)
 from .params import HasFeaturesCol, HasFeaturesCols, HasLabelCol, HasOutputCol, P, _CumlClass, _CumlParams
 from .sparkshim import HAVE_PYSPARK, Param, TypeConverters, keyword_only
 from .utils import get_logger
@@ -386,41 +386,11 @@ class UMAPModel(UMAPClass, _CumlModelWithColumns, _UMAPCumlParams):
         n_epochs = (100 if n_train <= 10000 else 30) if n_epochs is None else int(n_epochs) // 3
         params = _device_params(cp, k, n_epochs, "random", int(cp.get("random_state") or 0))
 
-        class _DeviceUMAP:
-            def __init__(self, gpu: int) -> None:
-                import torch
+        def predict(m: Any, Q: Any) -> Tuple[Any]:
+            return (m.ctx.umap_transform(m.arrays["X"], m.arrays["E"], Q, params),)
 
-                self.ctx = _transform_context(gpu)
-                self.X = torch.from_numpy(raw).to(self.ctx.device).contiguous()
-                self.E = torch.from_numpy(emb).to(self.ctx.device).contiguous()
-
-            def close(self) -> None:
-                self.X = self.E = None
-
-        def _transform_many(m: Any, dfs: List[Union[pd.DataFrame, np.ndarray]]) -> List[pd.Series]:
-            from .utils import DeviceRowAppender
-
-            sizes = [len(df) for df in dfs]
-            total = sum(sizes)
-            if total == 0:
-                return [pd.Series([], dtype=object) for _ in dfs]
-            app = DeviceRowAppender(m.ctx, n_cols, first_capacity=total)
-            for df, n_b in zip(dfs, sizes):
-                if n_b:
-                    _append_transform_features(app, df, n_cols)
-            host = m.ctx.umap_transform(m.X, m.E, app.finish(), params).cpu().numpy()
-            out, o = [], 0
-            for n_b in sizes:
-                out.append(pd.Series(list(host[o:o + n_b])))
-                o += n_b
-            return out
-
-        def _transform_internal(m: Any, df: Union[pd.DataFrame, np.ndarray]) -> pd.Series:
-            return _transform_many(m, [df])[0]
-
-        _transform_internal.many = _transform_many  # type: ignore[attr-defined]
-        _transform_internal.row_bytes = 4 * (n_cols + int(emb.shape[1]))  # type: ignore[attr-defined]
-        return (lambda gpu=0: _DeviceUMAP(gpu)), _transform_internal, None
+        construct = functools.partial(_DeviceModel, X=raw, E=emb)
+        return construct, self._grouped_transform(predict, 4 * (n_cols + int(emb.shape[1]))), None
 
     # -- persistence in the reference's layout (umap.py:1553-1640): metadata, data/metadata.json and two parquet files
     def write(self) -> Any:

@@ -283,7 +283,6 @@ _STUBS = '''
 import numpy as np, pandas as pd, torch
 import spark_rapids_ml_b200.core as core
 import spark_rapids_ml_b200.utils as utils
-import spark_rapids_ml_b200.regression as reg
 import spark_rapids_ml_b200.common.cuml_context as cc
 
 class HostAppender:
@@ -317,7 +316,7 @@ class HostContext:
 core.DeviceRowAppender = utils.DeviceRowAppender = HostAppender
 cc.CumlContext = HostContext
 core._CumlCommon._set_gpu_device = staticmethod(lambda context, is_local, is_transform=False: 0)
-reg._transform_context = lambda gpu: HostHandle()
+core._transform_context = lambda gpu: HostHandle()
 '''
 
 _LOCAL = '''
@@ -367,7 +366,7 @@ def _run(script: str, with_fake_pyspark: bool) -> dict:
     return json.loads([ln for ln in r.stdout.splitlines() if ln.startswith("RESULT ")][-1][len("RESULT "):])
 
 
-def test_local_frames_carry_the_label_and_fit_multiple_takes_one_pass():
+def test_local_frames_carry_the_label_and_fit_multiple_takes_one_pass_with_core_context_stub():
     res = _run(_STUBS + _LOCAL, with_fake_pyspark=False)
     assert res["coef_err"] < 1e-9 and res["b_err"] < 1e-9, res
     assert res["pred_err"] < 1e-9 and res["pred_is_double"] == "double", res

@@ -259,7 +259,6 @@ import numpy as np, pandas as pd, torch
 import logreg_oracle as lo
 import spark_rapids_ml_b200.core as core
 import spark_rapids_ml_b200.utils as utils
-import spark_rapids_ml_b200.classification as clf
 import spark_rapids_ml_b200.common.cuml_context as cc
 from spark_rapids_ml_b200 import _native
 
@@ -305,7 +304,7 @@ class HostContext:
 core.DeviceRowAppender = utils.DeviceRowAppender = HostAppender
 cc.CumlContext = HostContext
 core._CumlCommon._set_gpu_device = staticmethod(lambda context, is_local, is_transform=False: 0)
-clf._transform_context = lambda gpu: HostHandle()
+core._transform_context = lambda gpu: HostHandle()
 '''
 
 _LOCAL = '''
@@ -358,7 +357,7 @@ def _run(script: str, with_fake_pyspark: bool) -> dict:
     return json.loads([ln for ln in r.stdout.splitlines() if ln.startswith("RESULT ")][-1][len("RESULT "):])
 
 
-def test_estimator_end_to_end_on_local_frames():
+def test_estimator_end_to_end_on_local_frames_with_core_context_stub():
     res = _run(_STUBS + _LOCAL, with_fake_pyspark=False)
     assert res["coef_err"] < 1e-6 and res["b_err"] < 1e-6, res
     assert res["prob_err"] < 1e-6 and res["raw_err"] < 1e-5 and res["pred_same"], res

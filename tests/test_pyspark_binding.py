@@ -76,13 +76,21 @@ def host_fit_func(self, dataset, extra_params=None):
     return fit
 KMeans._get_cuml_fit_func = host_fit_func
 
+class HostModel:
+    def __init__(self, C): self.C = C
+    def close(self): pass
+
 def host_transform_func(self, dataset, eval_metric_info=None):
     C = np.asarray(self.cluster_centers_)
-    def construct(gpu=0): return C
-    def transform(model, df):
-        col = df[core.alias.data] if hasattr(df, "columns") and core.alias.data in df.columns else df
-        A = np.array([np.asarray(r, dtype=np.float64) for r in col])
-        return pd.Series(((A[:, None, :] - model[None]) ** 2).sum(-1).argmin(1).astype("int32"))
+    def construct(gpu=0): return HostModel(C)
+    def transform(model, dfs):
+        out = []
+        for df in dfs:
+            col = df[core.alias.data] if hasattr(df, "columns") and core.alias.data in df.columns else df
+            A = np.array([np.asarray(r, dtype=np.float64) for r in col])
+            out.append((((A[:, None, :] - model.C[None]) ** 2).sum(-1).argmin(1).astype("int32"),))
+        return out
+    transform.row_bytes = 4 * C.shape[1]
     return construct, transform, None
 KMeansModel._get_cuml_transform_func = host_transform_func
 '''
@@ -132,7 +140,7 @@ def _check(results: dict) -> None:
         assert r["pred_ok"] and r["pred_col"] and r["n_centers"] == 4, (kind, r)
 
 
-def test_pyspark_branch_wiring_with_host_stand_ins():
+def test_pyspark_branch_wiring_with_grouped_host_stand_ins():
     _check(_run(_COMMON + _CPU_STUBS + _BODY))
 
 

@@ -140,36 +140,29 @@ def test_world_size_2_gloo_row_sharding_matches_single_rank():
     np.testing.assert_array_equal(got[0], ref["centers"])    # and equal the single-rank oracle exactly
 
 
-def test_transform_batches_are_grouped_in_order():
-    """core._iter_transform: a transform function that offers `.many` sees consecutive batches in groups bounded by rows
-    and bytes; results come back one per batch, in order; without `.many` it is called batch by batch."""
+def test_grouped_transform_sees_batches_in_row_and_byte_capped_groups_in_order():
+    """core._iter_transform: a model's grouped transform function sees consecutive batches in groups bounded by rows
+    and bytes; results come back one per batch, in order."""
     import pandas as pd
     from spark_rapids_ml_b200 import core
 
     frames = [pd.DataFrame({"a": range(i * 10, i * 10 + n)}) for i, n in enumerate([3, 0, 5, 2, 7, 1])]
     calls = []
 
-    def one(model, f):
-        calls.append(("one", len(f)))
-        return pd.Series(f["a"].to_numpy() + model)
-
     def many(model, fs):
         calls.append(("many", [len(f) for f in fs]))
         return [pd.Series(f["a"].to_numpy() + model) for f in fs]
 
     want = [list(f["a"] + 100) for f in frames]
-    assert [list(r) for r in core._iter_transform(one, lambda: 100, iter(frames))] == want
-    assert [c[0] for c in calls] == ["one"] * 6
-    del calls[:]
-    one.many, one.row_bytes = many, 8
+    many.row_bytes = 8
     old = core.TRANSFORM_GROUP_ROWS, core.TRANSFORM_GROUP_BYTES
     try:
         core.TRANSFORM_GROUP_ROWS, core.TRANSFORM_GROUP_BYTES = 8, 1 << 30
-        assert [list(r) for r in core._iter_transform(one, lambda: 100, iter(frames))] == want
+        assert [list(r) for r in core._iter_transform(many, 100, iter(frames))] == want
         assert calls == [("many", [3, 0, 5]), ("many", [2, 7]), ("many", [1])]
         del calls[:]
         core.TRANSFORM_GROUP_ROWS, core.TRANSFORM_GROUP_BYTES = 1 << 20, 8 * 4      # the byte cap: 4 rows per group
-        assert [list(r) for r in core._iter_transform(one, lambda: 100, iter(frames))] == want
+        assert [list(r) for r in core._iter_transform(many, 100, iter(frames))] == want
         assert calls == [("many", [3, 0, 5]), ("many", [2, 7]), ("many", [1])]
     finally:
         core.TRANSFORM_GROUP_ROWS, core.TRANSFORM_GROUP_BYTES = old
