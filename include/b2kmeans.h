@@ -44,6 +44,8 @@
  *   b2k_silhouette              none: the reference has no clustering evaluator (its DBSCAN benchmark collects the
  *                               frame and calls scikit-learn's silhouette_score); stands in for Spark's
  *                               pyspark.ml.evaluation.ClusteringEvaluator (metricName "silhouette")
+ *   b2k_silhouette_multi        none: the reference tunes KMeans with pyspark's CrossValidator, scoring each model on
+ *                               the CPU; here one device pass scores every model of a param grid
  *
  * Conventions
  *   - Plain C, no exceptions across the boundary: every call returns a b2k_status; the message for the
@@ -695,6 +697,19 @@ int b2k_eval_binary(b2k_ctx* ctx, const double* scores, const uint8_t* pos, int6
 #define B2K_SILHOUETTE_MAX_CLUSTERS 65536
 int b2k_silhouette(b2k_ctx* ctx, const float* X, int64_t n_local, int d, const int64_t* cluster_ids, int metric,
                    double* out, uintptr_t stream);
+/* b2k_silhouette_multi: the silhouette of n_models >= 1 clusterings of the same rows in one call.  cluster_ids is a host
+ * array of n_models device int64 [n_local] arrays; out (host) [n_models].  out[m] has exactly the bits that
+ * b2k_silhouette(ctx, X, n_local, d, cluster_ids[m], metric, ...) returns, for any rank count, grid_limit and kernel_path.
+ * Per model: the ids and statistics passes of b2k_silhouette and its shift m.  Models whose m has the same bits form a
+ * shift group; a group's shifted means are packed one model after another into shared blocks of 128 (wgmma) or tiles
+ * of 64 (generic), and one silhouette pass per chunk of at most B2K_SILHOUETTE_MULTI_CHUNK models scores all of them in
+ * one read of X.  Stats: fused_tc_launches / generic_launches grow by one per (group, chunk); with "time_kernels",
+ * last_finalize_ms / last_reduce_ms / last_fused_ms are the ids, statistics and silhouette passes summed over models
+ * and groups.  Errors: those of b2k_silhouette, prefixed with "model m: " for the first model that fails (every rank
+ * fails together); n_models < 1 is B2K_ERR_INVALID.  Collective; synchronises `stream`. */
+#define B2K_SILHOUETTE_MULTI_CHUNK 16
+int b2k_silhouette_multi(b2k_ctx* ctx, const float* X, int64_t n_local, int d, int n_models,
+                         const int64_t* const* cluster_ids, int metric, double* out, uintptr_t stream);
 
 /* ---- UMAP (euclidean) ----
  * b2k_umap_fit stands in for umap.py:1009-1065 (the fit function: cuML UMAP(...).fit on the rows coalesced to one

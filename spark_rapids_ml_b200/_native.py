@@ -77,6 +77,7 @@ EXPORTED_SYMBOLS = (
     "b2k_umap_graph",
     "b2k_umap_transform",
     "b2k_silhouette",
+    "b2k_silhouette_multi",
 )
 
 EVAL_KINDS = {"identity": 0, "logistic": 1, "softmax": 2}
@@ -257,6 +258,7 @@ def load_library() -> ctypes.CDLL:
     L.b2k_umap_graph.argtypes = [vp] + [vp] * 11
     L.b2k_umap_transform.argtypes = [vp, vp, vp, i64, i32, vp, i64, ctypes.POINTER(UmapParams), vp, ctypes.c_size_t]
     L.b2k_silhouette.argtypes = [vp, vp, i64, i32, vp, i32, ctypes.POINTER(f64), ctypes.c_size_t]
+    L.b2k_silhouette_multi.argtypes = [vp, vp, i64, i32, i32, vp, i32, vp, ctypes.c_size_t]
     for name in EXPORTED_SYMBOLS:
         if name not in ("b2k_last_error",):
             getattr(L, name).restype = i32
@@ -803,6 +805,32 @@ class Context:
                                                SILHOUETTE_METRICS[distance_measure], ctypes.byref(out),
                                                self._stream()))
         return float(out.value)
+
+    def silhouette_multi(self, X: Any, ids_list: Sequence[Any], distance_measure: str = "squaredEuclidean") -> List[float]:
+        """b2k_silhouette_multi: the silhouette of several clusterings of the same rows (collective when a communicator
+        is initialised).  X [n, d] float32 and each of ids_list [n] int64 CUDA tensors -> one value per clustering,
+        each with the bits Context.silhouette returns for it; one device pass over X serves the models whose shifts
+        agree."""
+        t = self._torch
+        n, d = self._check_X(X)
+        if distance_measure not in SILHOUETTE_METRICS:
+            raise ValueError(f"distance_measure must be one of {sorted(SILHOUETTE_METRICS)}, got {distance_measure!r}")
+        ids_list = list(ids_list)
+        if not ids_list:
+            raise ValueError("ids_list must hold at least one cluster-id tensor")
+        for ids in ids_list:
+            if not (ids.is_cuda and ids.dtype == t.int64 and ids.dim() == 1 and ids.is_contiguous() and
+                    int(ids.shape[0]) == n):
+                raise ValueError("every cluster-id tensor must be a contiguous int64 CUDA tensor [n]")
+            if ids.device.index != self.device_index:
+                raise ValueError("cluster ids live on a different device than this context")
+        M = len(ids_list)
+        ptrs = (ctypes.c_void_p * M)(*[ids.data_ptr() for ids in ids_list])
+        out = (ctypes.c_double * M)()
+        with t.cuda.device(self.device):
+            self._check(self._L.b2k_silhouette_multi(self._h, X.data_ptr(), n, d, M, ptrs,
+                                                     SILHOUETTE_METRICS[distance_measure], out, self._stream()))
+        return [float(v) for v in out]
 
     # -- random forests ---------------------------------------------------------------------
     def rf_fit(self, X: Any, y: Any, *, n_trees: int = 20, max_depth: int = 5, max_bins: int = 32,

@@ -8,6 +8,9 @@ Same names, argument meaning and error behaviour as the reference:
   KMeans (keyword-only ctor, setters, _get_cuml_fit_func, _out_schema,
           _create_pyspark_model, _merge_model_chunks)                                clustering.py:189-502
   KMeansModel (clusterCenters, hasSummary, predict, _get_cuml_transform_func)        clustering.py:505-604
+  KMeans.fitMultiple / KMeansModel._transformEvaluate: CrossValidator(KMeans, ClusteringEvaluator), which the
+  reference hands to pyspark's CrossValidator (GPU fits, CPU silhouette); here every fold's grid fits from one ingest
+  and its models are scored in one device silhouette pass (b2k_silhouette_multi)
   DBSCANClass, _DBSCANCumlParams, DBSCAN (lazy fit), DBSCANModel.transform             clustering.py:607-1186
 
 Differences that are deliberate: no CPU fallback (cpu() / single-vector predict need a JVM and raise), and the
@@ -18,7 +21,7 @@ raises NotImplementedError.
 from __future__ import annotations
 
 import functools
-from typing import Any, Callable, Dict, List, Optional, Sequence, Tuple, Union
+from typing import Any, Callable, Dict, Iterator, List, Optional, Sequence, Tuple, Union
 
 import numpy as np
 import pyarrow as pa
@@ -132,6 +135,7 @@ class KMeans(KMeansClass, _CumlEstimator, _KMeansCumlParams):
                  seed: Optional[int] = None, num_workers: Optional[int] = None,
                  verbose: Union[int, bool] = False, **kwargs: Any) -> None:
         super().__init__()
+        self._fit_grid: Optional[List[Dict[str, Any]]] = None
         self._handle_param_spark_confs()   # session-wide defaults for arguments not passed (clustering.py:315)
         # if the user does not override it, n_init = 1 to match Spark behaviour (clustering.py:316-319)
         if "n_init" not in self._input_kwargs:
@@ -170,8 +174,19 @@ class KMeans(KMeansClass, _CumlEstimator, _KMeansCumlParams):
     def _get_cuml_fit_func(self, dataset: Any, extra_params: Optional[List[Dict[str, Any]]] = None
                            ) -> Callable[[FitInputType, Dict[str, Any]], Dict[str, Any]]:
         cls = self.__class__
+        grid = self._fit_grid
 
         def _cuml_fit(dfs: FitInputType, params: Dict[str, Any]) -> Dict[str, Any]:
+            if grid is None:
+                return _fit_one(dfs, params)
+            rows: Dict[str, List[Any]] = {}
+            for init in grid:   # one fit per param map on the same device matrix, in map order
+                for key, v in _fit_one(dfs, {**params, param_alias.cuml_init: init,
+                                             param_alias.fit_multiple_params: True}).items():
+                    rows.setdefault(key, []).extend(v)
+            return rows
+
+        def _fit_one(dfs: FitInputType, params: Dict[str, Any]) -> Dict[str, Any]:
             # stands in for KMeansMG(handle, **cuml_init).fit(concated) — clustering.py:381-415
             ctx = params[param_alias.handle]
             init = dict(params[param_alias.cuml_init])
@@ -203,6 +218,31 @@ class KMeans(KMeansClass, _CumlEstimator, _KMeansCumlParams):
                     "n_cols": [n_cols] * len(chunks), "dtype": [dtype_str] * len(chunks)}
 
         return _cuml_fit
+
+    def _supportsTransformEvaluate(self, evaluator: Any) -> bool:
+        """CrossValidator scores KMeans models with a ClusteringEvaluator's silhouette, either distance measure."""
+        return _supports_silhouette(evaluator)
+
+    def fitMultiple(self, dataset: Any, paramMaps: Sequence[Dict[Any, Any]]) -> Iterator[Tuple[int, Any]]:
+        """(index, model) per param map, in map order.  When every map changes only k, maxIter, tol, seed or
+        initMode, one ingest serves all maps: one barrier task per GPU fits each map in turn on the same device matrix,
+        and each model equals est.copy(map).fit(dataset).  Otherwise each map is one fit."""
+        from .regression import _ModelIterator
+
+        maps = list(paramMaps)
+        if not _kmeans_grid_shares_ingest(maps):
+            return _ModelIterator([self.copy(pm)._fit(dataset) for pm in maps])
+        copies = [self.copy(pm) for pm in maps]
+        for c in copies:
+            c._validate_parameters()
+        est = self.copy()
+        est._fit_grid = [dict(c.cuml_params) for c in copies]
+        if est._use_cpu_fallback():
+            raise ValueError("a Spark Param without GPU support is set and spark_rapids_ml_b200 has no CPU fallback")
+        models = est._fit_internal(dataset, maps)
+        for m, c in zip(models, copies):
+            c._copy_cuml_params(m)
+        return _ModelIterator(models)
 
     def _out_schema(self) -> Any:
         # reference: clustering.py:458-468
@@ -263,6 +303,50 @@ class KMeansModel(KMeansClass, _CumlModelWithPredictionCol, _KMeansCumlParams):
     def _transform_array_order(self) -> str:
         return "C"
 
+    def _center_sets(self) -> List[List[List[float]]]:
+        """The centres of each model of this (combined) model."""
+        c = self.cluster_centers_
+        return [c] if len(c) == 0 or not isinstance(c[0][0], (list, tuple)) else list(c)  # type: ignore[list-item]
+
+    @classmethod
+    def _combine(cls, models: List["KMeansModel"]) -> "KMeansModel":
+        """One model holding several fits' centre sets, for _transformEvaluate."""
+        assert len(models) > 0 and all(isinstance(m, cls) for m in models)
+        first = models[0]
+        out = cls(cluster_centers_=[m.cluster_centers_ for m in models], n_cols=first.n_cols, dtype=first.dtype)
+        first._copyValues(out)
+        first._copy_cuml_params(out)
+        return out
+
+    def _transformEvaluate(self, dataset: Any, evaluator: Any, params: Optional[Dict[Any, Any]] = None) -> List[float]:
+        """The silhouette of every model of this (combined) model on a local frame, with the worker count and
+        repartitioning that ClusteringEvaluator.evaluate uses: one barrier task per GPU ingests the features once,
+        labels the rows with each model's centres as transform() does (b2k_kmeans_assign) and scores every model in one
+        b2k_silhouette_multi call.  The evaluator's predictionCol is not read: the labels come from the models."""
+        from .evaluation import _SilhouetteMultiCaller
+
+        model = self.copy(params) if params else self
+        if HAVE_PYSPARK:
+            from . import spark_binding
+
+            if spark_binding.is_spark_dataframe(dataset):
+                raise NotImplementedError("KMeansModel._transformEvaluate() of a pyspark DataFrame is not supported in "
+                                          "this build; evaluate a local frame")
+        if not _supports_silhouette(evaluator):
+            raise NotImplementedError(f"KMeansModel._transformEvaluate() does not support {type(evaluator).__name__}")
+        if evaluator.isSet("weightCol") and evaluator.getOrDefault("weightCol"):
+            raise NotImplementedError("weightCol is not supported by the device evaluation")
+        ev_features, features = evaluator.getOrDefault("featuresCol"), model.getFeaturesCol()
+        if list(np.atleast_1d(ev_features)) != list(np.atleast_1d(features)):
+            raise NotImplementedError(f"the evaluator's featuresCol {ev_features!r} differs from the model's "
+                                      f"featuresCol {features!r}: the device evaluation reads one features column")
+        if dataset.count() == 0:
+            raise ValueError("ClusteringEvaluator: the frame has no rows")
+        caller = _SilhouetteMultiCaller(features, model._center_sets(), evaluator.getDistanceMeasure())
+        res = caller._call_cuml_fit_func(dataset, partially_collect=True)
+        rows = res if isinstance(res, list) else res.collect()
+        return [float(v) for v in rows[0]["silhouette"]]
+
     def _get_cuml_transform_func(self, dataset: Any, eval_metric_info: Any = None
                                  ) -> Tuple[Callable, Callable, Optional[Callable]]:
         # the injected-centers predictor (clustering.py:582-596): b2k_kmeans_assign labels a group's rows
@@ -270,6 +354,24 @@ class KMeansModel(KMeansClass, _CumlModelWithPredictionCol, _KMeansCumlParams):
         transform = self._grouped_transform(lambda m, X: (m.ctx.kmeans_assign(X, m.arrays["C"])[0],),
                                             4 * int(self.n_cols or 1))
         return construct, transform, None
+
+
+def _supports_silhouette(evaluator: Any) -> bool:
+    if type(evaluator).__name__ != "ClusteringEvaluator":
+        return False
+    try:
+        return (evaluator.getMetricName() == "silhouette" and
+                evaluator.getDistanceMeasure() in ("squaredEuclidean", "cosine"))
+    except Exception:
+        return False
+
+
+_GRID_FIT_PARAMS = frozenset({"k", "maxIter", "tol", "seed", "initMode"})
+
+
+def _kmeans_grid_shares_ingest(paramMaps: Sequence[Dict[Any, Any]]) -> bool:
+    """Whether KMeans.fitMultiple fits these maps from one ingest: every map changes only per-fit params."""
+    return bool(paramMaps) and all(p.name in _GRID_FIT_PARAMS for pm in paramMaps for p in pm)
 
 
 # ---- DBSCAN (reference: clustering.py:607-1186) ----

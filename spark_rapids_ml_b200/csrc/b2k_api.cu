@@ -1034,6 +1034,21 @@ extern "C" int b2k_silhouette(b2k_ctx* ctx, const float* X, int64_t n_local, int
   return b2k_silhouette_impl(ctx, X, n_local, d, cluster_ids, metric, out, reinterpret_cast<cudaStream_t>(stream));
 }
 
+extern "C" int b2k_silhouette_multi(b2k_ctx* ctx, const float* X, int64_t n_local, int d, int n_models,
+                                    const int64_t* const* cluster_ids, int metric, double* out, uintptr_t stream) {
+  if (!ctx) return b2k_fail(nullptr, B2K_ERR_INVALID, "b2k_silhouette_multi: ctx is NULL");
+  if (n_models < 1 || !cluster_ids)
+    return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_silhouette_multi: n_models must be >= 1 with cluster_ids[n_models]");
+  if (n_local < 0 || d <= 0 || (n_local > 0 && !X) || !out)
+    return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_silhouette_multi: bad X/out/n/d");
+  for (int m = 0; m < n_models; ++m)
+    if (n_local > 0 && !cluster_ids[m])
+      return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_silhouette_multi: cluster_ids[" + std::to_string(m) + "] is NULL");
+  B2K_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  return b2k_silhouette_multi_impl(ctx, X, n_local, d, n_models, cluster_ids, metric, out,
+                                   reinterpret_cast<cudaStream_t>(stream));
+}
+
 // ------------------------------------------------------------------------------------------------
 // random forests (b2k_rf.cu)
 // ------------------------------------------------------------------------------------------------

@@ -20,6 +20,9 @@
 //              operand is the hi / lo planes of the shifted means (k_knn_prep over a zero row and the means).
 //              D = fl32(fl32(n_c - 2 acc) + n_i) + Psi_c in fp32, within the bound of include/b2kmeans.h.
 //     generic  (k_sil_generic, SIMT): every shape; D = sum_f (y_f - mu_c,f)^2 + Psi_c in fp64.
+// b2k_silhouette_multi scores several clusterings of the same rows: per model the ids and statistics passes above,
+// then one silhouette pass (k_sil_wg_multi / k_sil_generic_multi) per shift group and chunk of models over their means
+// packed side by side, with the bits of each model's own call.
 // No floating-point atomics: integer counters only, every fp64 sum in a fixed order for a given grid, so two calls on
 // the same input, rank count and device give the same bits.
 #include <cub/device/device_radix_sort.cuh>
@@ -28,6 +31,7 @@
 
 #include <algorithm>
 #include <cmath>
+#include <cstring>
 #include <string>
 #include <vector>
 
@@ -235,6 +239,12 @@ __global__ void __launch_bounds__(256) k_sil_means(const double* __restrict__ st
   if (psi32 != nullptr) psi32[c] = (float)p;
 }
 
+// b2k_silhouette_multi: the k_knn_prep permutation of a group's packed means, plane row c <- Mz row c + 1
+__global__ void __launch_bounds__(256) k_sil_mperm(int K, int64_t k_pad, int32_t* __restrict__ mperm) {
+  const int64_t c = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (c < k_pad) mperm[c] = c < K ? (int32_t)(c + 1) : -1;
+}
+
 // ---- silhouette, wgmma ----
 constexpr int SIL_OWN = PW_TM * 4 + 256 * 8;   // the tile's row norms, the consumers' sums
 template <int NCH>
@@ -428,15 +438,301 @@ __global__ void __launch_bounds__(G_NT, 1) k_sil_generic(const SilArgs a) {
   }
 }
 
+// ---- b2k_silhouette_multi: the means of several models packed into one column space ----
+// A shift group's models are segments [off[j], off[j + 1]) of the packed clusters, in model order, with no padding
+// between them (a segment may start inside a block).  A launch serves a chunk of at most SIL_MC models; its per (row,
+// model) state lives in shared memory, so its cost does not grow with the chunk.  Each (row, cluster) D is formed
+// exactly as in the one-model passes, d_own / d_min are a select and a min, and each thread adds its rows' s_i per model
+// in the same order as there, so every model's sum has the bits of its own b2k_silhouette call.
+constexpr int SIL_MC = B2K_SILHOUETTE_MULTI_CHUNK;
+
+struct SilMultiArgs {
+  int64_t n;
+  int ntiles, d, nm;             // nm: models in this chunk
+  int blo, bhi;                  // wgmma: the blocks of means the chunk's segments touch
+  const float* X;
+  const double* nrm;
+  const float* shift;            // wgmma: the group's m [d]
+  const float* cnorm;            // wgmma: [packed k_pad]
+  const float* psi32;            // wgmma: [packed]
+  const double* mu;              // generic: [packed][d]
+  const double* psi;             // generic: [packed]
+  const double* cnt;             // [packed]
+  int off[SIL_MC + 1];           // the chunk's segments, packed columns
+  const int32_t* cid[SIL_MC];    // each model's dense cluster of each row [n]
+  double* part;                  // per model j, per CTA: part[j grid + CTA]
+};
+
+// The per-thread sums of the one-model passes fold over every thread in order; the threads that add no row keep +0.0,
+// and +0.0 changes no partial sum (none is ever -0.0), so folding only the adding threads, in order, gives the same bits.
+constexpr int SILM_OWN = PW_TM * 4 + SIL_MC * PW_TM * 8 + SIL_MC * 64 * 8;   // norms, (d_own, d_min), per-thread sums
+template <int NCH>
+using SilMultiWgCfg = PairWgCfg<NCH, SILM_OWN>;
+
+template <int NCH, bool COS>
+__global__ void __launch_bounds__(PW_NTHREADS, 1)
+k_sil_wg_multi(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapHi,
+               const __grid_constant__ CUtensorMap mapLo, const __grid_constant__ SilMultiArgs a) {
+  using G = SilMultiWgCfg<NCH>;
+  constexpr int R = PW_N / 2;
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  const uint32_t base = smem_u32(smem_raw);
+  const PairWgBars bars = pair_wg_init<G>(base);
+  float* snx = reinterpret_cast<float*>(smem_raw + G::OFF_OWN);
+  float* st_own = snx + PW_TM;                       // [SIL_MC][PW_TM]
+  float* st_min = st_own + SIL_MC * PW_TM;           // [SIL_MC][PW_TM]
+  double* sred = reinterpret_cast<double*>(st_min + SIL_MC * PW_TM);   // [SIL_MC][64]
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int nit = (int)blockIdx.x < a.ntiles ? (a.ntiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
+
+  if (warp >= 8) {
+    if (warp == 8 && elect_one())
+      pair_wg_produce<G>(
+          base, bars, &mapQ, &mapHi, &mapLo, nit,
+          [&](int it) { return PairWgUnit{((int)blockIdx.x + it * (int)gridDim.x) * PW_TM, a.blo, a.bhi}; },
+          [](int) { return false; });
+    __syncwarp();
+    return;
+  }
+
+  const int g = warp >> 2, wi = warp & 3;
+  const int wr0 = g * 64 + wi * 16;
+  const int rr0 = wr0 + (lane >> 2);
+  const bool lead = (lane & 3) == 0;                 // the quad's four lanes hold the same rows
+  double* my_sum = sred + (threadIdx.x >> 2);        // the adding threads in thread order
+  if (lead)
+    for (int j = 0; j < a.nm; ++j) my_sum[j * 64] = 0.0;
+  float acc[R];
+  int q = 0;
+  for (int it = 0; it < nit; ++it) {
+    const int64_t t0 = ((int64_t)blockIdx.x + (int64_t)it * gridDim.x) * PW_TM;
+    mbar_wait_nocall(bars.qfull(), (uint32_t)(it & 1));
+    for (int k = 0; k < 16; ++k) {   // y - m in place, as k_sil_wg
+      const int r = wr0 + k;
+      const int64_t row = t0 + r;
+      double s2 = 0.0;
+      if (row < a.n) {
+        for (int col = lane; col < a.d; col += 32) {
+          const int cc = col & 31;
+          float* p = reinterpret_cast<float*>(smem_raw + G::OFF_Q + (col >> 5) * G::QBYTES + r * 128 +
+                                              ((((cc >> 2) ^ (r & 7))) << 4) + (cc & 3) * 4);
+          const float v = sil_y(*p, COS ? a.nrm : nullptr, row) - __ldg(a.shift + col);
+          *p = v;
+          s2 += (double)v * (double)v;
+        }
+      }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) s2 += __shfl_xor_sync(0xffffffffu, s2, o);
+      if (lane == 0) snx[r] = (float)s2;
+    }
+    __syncwarp();
+    int64_t row[2];
+    float nx[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      row[h] = t0 + rr0 + 8 * h;
+      nx[h] = snx[rr0 + 8 * h];
+      if (lead)
+        for (int j = 0; j < a.nm; ++j) {
+          st_own[j * PW_TM + rr0 + 8 * h] = -INFINITY;
+          st_min[j * PW_TM + rr0 + 8 * h] = INFINITY;
+        }
+    }
+    for (int b = a.blo; b < a.bhi; ++b) {
+      pair_wg_block<G>(smem_raw, base, bars, rr0, lane, acc, q);
+      const int cb = b * PW_N + 2 * (lane & 3);
+      for (int j = 0; j < a.nm; ++j) {   // the segments this block meets (uniform over the CTA)
+        const int lo = a.off[j], hi = a.off[j + 1];
+        if (hi <= b * PW_N || lo >= (b + 1) * PW_N) continue;
+        int own[2];
+        float d_own[2], d_min[2];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          own[h] = row[h] < a.n ? lo + __ldg(a.cid[j] + row[h]) : -1;
+          d_own[h] = -INFINITY;
+          d_min[h] = INFINITY;
+        }
+#pragma unroll
+        for (int i = 0; i < R; ++i) {
+          const int h = (i >> 1) & 1;
+          const int c = cb + 8 * (i >> 2) + (i & 1);
+          if ((unsigned)(c - lo) >= (unsigned)(hi - lo)) continue;
+          const float S = fmaf(-2.f, acc[i], __ldg(a.cnorm + c)) + nx[h];
+          const float D = S + __ldg(a.psi32 + c);
+          if (c == own[h]) d_own[h] = D;
+          else d_min[h] = fminf(d_min[h], D);
+        }
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          d_min[h] = fminf(d_min[h], __shfl_xor_sync(0xffffffffu, d_min[h], 1));
+          d_min[h] = fminf(d_min[h], __shfl_xor_sync(0xffffffffu, d_min[h], 2));
+          d_own[h] = fmaxf(d_own[h], __shfl_xor_sync(0xffffffffu, d_own[h], 1));
+          d_own[h] = fmaxf(d_own[h], __shfl_xor_sync(0xffffffffu, d_own[h], 2));
+          if (lead) {
+            float* po = st_own + j * PW_TM + rr0 + 8 * h;
+            float* pm = st_min + j * PW_TM + rr0 + 8 * h;
+            *po = fmaxf(*po, d_own[h]);
+            *pm = fminf(*pm, d_min[h]);
+          }
+        }
+      }
+    }
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    __syncwarp();
+    if (lane == 0) mbar_arrive(bars.qempty());
+    if (lead)
+      for (int j = 0; j < a.nm; ++j)
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+          if (row[h] < a.n) {
+            const int own = __ldg(a.cid[j] + row[h]);
+            my_sum[j * 64] += sil_s((double)st_own[j * PW_TM + rr0 + 8 * h], (double)st_min[j * PW_TM + rr0 + 8 * h],
+                                    __ldg(a.cnt + a.off[j] + own));
+          }
+  }
+  sil_bar_consumers();
+  if (threadIdx.x < a.nm) {
+    const int j = threadIdx.x;
+    double t = 0.0;
+    for (int i = 0; i < 64; ++i) t += sred[j * 64 + i];
+    a.part[(int64_t)j * gridDim.x + blockIdx.x] = t;
+  }
+}
+
+// generic: k_sil_generic's tiles over the chunk's packed clusters [off[0], off[nm])
+constexpr int SILM_GEN_SMEM = 2 * GF * (GR + 1) * 8 + 2 * SIL_MC * GR * 8 + SIL_MC * 16 * 8;
+template <bool COS>
+__global__ void __launch_bounds__(G_NT, 1) k_sil_generic_multi(const __grid_constant__ SilMultiArgs a) {
+  extern __shared__ __align__(16) uint8_t gsm[];
+  double(*xr)[GR + 1] = reinterpret_cast<double(*)[GR + 1]>(gsm);
+  double(*mc)[GC + 1] = reinterpret_cast<double(*)[GC + 1]>(gsm + GF * (GR + 1) * 8);
+  double* st_own = reinterpret_cast<double*>(gsm + 2 * GF * (GR + 1) * 8);   // [SIL_MC][GR]
+  double* st_min = st_own + SIL_MC * GR;                                      // [SIL_MC][GR]
+  double* sred = st_min + SIL_MC * GR;                                        // [SIL_MC][16]
+  const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
+  const int d = a.d;
+  const int cbeg = a.off[0], cend = a.off[a.nm];
+  if (tx == 0)
+    for (int j = 0; j < a.nm; ++j) sred[j * 16 + ty] = 0.0;
+  for (int tile = blockIdx.x; tile < a.ntiles; tile += gridDim.x) {
+    int64_t row[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      row[i] = (int64_t)tile * GR + ty + 16 * i;
+      if (tx == 0)
+        for (int j = 0; j < a.nm; ++j) {
+          st_own[j * GR + ty + 16 * i] = -INFINITY;
+          st_min[j * GR + ty + 16 * i] = INFINITY;
+        }
+    }
+    for (int c0 = cbeg; c0 < cend; c0 += GC) {
+      double acc[4][4];
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) acc[i][j] = 0.0;
+      for (int f0 = 0; f0 < d; f0 += GF) {
+        __syncthreads();
+        for (int e = threadIdx.x; e < GF * GR; e += G_NT) {
+          const int r = e / GF, c = e % GF;
+          const int64_t gr = (int64_t)tile * GR + r;
+          const int f = f0 + c, cl = c0 + r;
+          xr[c][r] = (gr < a.n && f < d) ? (double)sil_y(a.X[gr * d + f], COS ? a.nrm : nullptr, gr) : 0.0;
+          mc[c][r] = (cl < cend && f < d) ? a.mu[(int64_t)cl * d + f] : 0.0;
+        }
+        __syncthreads();
+        const int fc = min(GF, d - f0);
+        for (int c = 0; c < fc; ++c) {
+          double vr[4], vc[4];
+#pragma unroll
+          for (int i = 0; i < 4; ++i) vr[i] = xr[c][ty + 16 * i];
+#pragma unroll
+          for (int j = 0; j < 4; ++j) vc[j] = mc[c][tx + 16 * j];
+#pragma unroll
+          for (int i = 0; i < 4; ++i)
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+              const double t = vr[i] - vc[j];
+              acc[i][j] = fma(t, t, acc[i][j]);
+            }
+        }
+      }
+      for (int m = 0; m < a.nm; ++m) {   // the segments this tile meets (uniform over the CTA)
+        const int lo = a.off[m], hi = a.off[m + 1];
+        if (hi <= c0 || lo >= c0 + GC) continue;
+        int own[4];
+        double d_own[4], d_min[4];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          own[i] = row[i] < a.n ? lo + a.cid[m][row[i]] : -1;
+          d_own[i] = -INFINITY;
+          d_min[i] = INFINITY;
+        }
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const int cl = c0 + tx + 16 * j;
+          if (cl < lo || cl >= hi) continue;
+          const double p = a.psi[cl];
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            const double D = acc[i][j] + p;
+            if (cl == own[i]) d_own[i] = D;
+            else d_min[i] = fmin(d_min[i], D);
+          }
+        }
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+#pragma unroll
+          for (int o = 1; o < 16; o <<= 1) {
+            d_min[i] = fmin(d_min[i], __shfl_xor_sync(0xffffffffu, d_min[i], o));
+            d_own[i] = fmax(d_own[i], __shfl_xor_sync(0xffffffffu, d_own[i], o));
+          }
+          if (tx == 0) {
+            double* po = st_own + m * GR + ty + 16 * i;
+            double* pm = st_min + m * GR + ty + 16 * i;
+            *po = fmax(*po, d_own[i]);
+            *pm = fmin(*pm, d_min[i]);
+          }
+        }
+      }
+    }
+    if (tx == 0)
+      for (int m = 0; m < a.nm; ++m)
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+          if (row[i] < a.n)
+            sred[m * 16 + ty] += sil_s(st_own[m * GR + ty + 16 * i], st_min[m * GR + ty + 16 * i],
+                                       a.cnt[a.off[m] + a.cid[m][row[i]]]);
+  }
+  __syncthreads();
+  if (threadIdx.x < a.nm) {
+    const int m = threadIdx.x;
+    double t = 0.0;
+    for (int i = 0; i < 16; ++i) t += sred[m * 16 + i];
+    a.part[(int64_t)m * gridDim.x + blockIdx.x] = t;
+  }
+}
+
 unsigned grid_1d(int64_t n, int sm) {
   return (unsigned)std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, (int64_t)sm * 16));
 }
 }  // namespace
 
-int b2k_silhouette_impl(b2k_ctx* ctx, const float* X, int64_t n_local, int d, const int64_t* ids, int metric,
-                        double* out, cudaStream_t s) {
+// One model's cluster ids and statistics: what the silhouette pass needs besides X, and the pass b2k_silhouette runs
+struct SilModel {
+  int64_t K = 0, n_total = 0;
+  bool wg = false;
+  DevBuf b_cid, b_nrm, b_stat;
+  int32_t* cid = nullptr;   // dense cluster of each row [n]
+  double* nrm = nullptr;    // cosine: ||x|| [n]
+  double* stat = nullptr;   // [K][d + 2] + 2, allreduced
+};
+
+// The ids and statistics passes of one model and every check of b2k_silhouette, in its order.  tm: marks 0 (start) and
+// 1 (ids done).
+int sil_prepare(b2k_ctx* ctx, const float* X, int64_t n_local, int d, const int64_t* ids, int metric, B2kTimer& tm,
+                SilModel& md, cudaStream_t s) {
   const int nr = ctx->nranks;
-  B2kTimer tm(ctx->time_kernels != 0);
   const bool cosine = metric == 1;
   const int64_t n = n_local;
   // ---- ids: sort, runs ----
@@ -454,6 +750,8 @@ int b2k_silhouette_impl(b2k_ctx* ctx, const float* X, int64_t n_local, int d, co
   int32_t *rows = nullptr, *perm = nullptr, *cid = nullptr;
   double* nrm = nullptr;
   void* tmp = nullptr;
+  B2K_TRY(dalloc(ctx, md.b_cid, (size_t)ni, s, &cid));
+  if (cosine) B2K_TRY(dalloc(ctx, md.b_nrm, (size_t)ni, s, &nrm));
   B2K_TRY(b2k_scratch_layout(ctx, "silhouette", [&](B2kLayout& L) -> int {
     sz_dev = L.take<int64_t>((size_t)NS * (nr + 1));
     nruns = L.take<int64_t>(1);
@@ -463,8 +761,6 @@ int b2k_silhouette_impl(b2k_ctx* ctx, const float* X, int64_t n_local, int d, co
     roff = L.take<int64_t>((size_t)ni + 2);
     rows = L.take<int32_t>((size_t)ni);
     perm = L.take<int32_t>((size_t)ni);
-    cid = L.take<int32_t>((size_t)ni);
-    if (cosine) nrm = L.take<double>((size_t)ni);
     tmp = L.take<char>(tmp_bytes);
     return B2K_OK;
   }));
@@ -549,10 +845,10 @@ int b2k_silhouette_impl(b2k_ctx* ctx, const float* X, int64_t n_local, int d, co
   // ---- statistics ----
   const int64_t nch = (n + SIL_SC - 1) / SIL_SC;
   const size_t slen = (size_t)K * (d + 2) + 2;
-  DevBuf b_piece, b_stat;
+  DevBuf b_piece;
   double *piece = nullptr, *stat = nullptr;
   B2K_TRY(dalloc(ctx, b_piece, (size_t)std::max<int64_t>(nch + kl, 1) * (d + 1), s, &piece));
-  B2K_TRY(dalloc(ctx, b_stat, slen, s, &stat));
+  B2K_TRY(dalloc(ctx, md.b_stat, slen, s, &stat));
   unsigned long long* bad = reinterpret_cast<unsigned long long*>(sz_dev);   // the sizes are on the host now
   B2K_CUDA_OK(ctx, cudaMemsetAsync(stat, 0, slen * 8, s));
   B2K_CUDA_OK(ctx, cudaMemsetAsync(bad, 0, 2 * sizeof(unsigned long long), s));
@@ -580,7 +876,25 @@ int b2k_silhouette_impl(b2k_ctx* ctx, const float* X, int64_t n_local, int d, co
   if (ctx->kernel_path == B2K_PATH_FUSED && !wg_ok)
     return b2k_fail(ctx, B2K_ERR_UNSUPPORTED, "kernel_path=2 requested but the wgmma silhouette pass needs d % 4 == 0, "
                                               "4 <= d <= 128 and 16-byte aligned X (d = " + std::to_string(d) + ")");
-  const bool wg = wg_ok && ctx->kernel_path != B2K_PATH_GENERIC;
+  md.wg = wg_ok && ctx->kernel_path != B2K_PATH_GENERIC;
+  md.K = K;
+  md.n_total = n_total;
+  md.cid = cid;
+  md.nrm = nrm;
+  md.stat = stat;
+  return B2K_OK;
+}
+
+int b2k_silhouette_impl(b2k_ctx* ctx, const float* X, int64_t n_local, int d, const int64_t* ids, int metric,
+                        double* out, cudaStream_t s) {
+  B2kTimer tm(ctx->time_kernels != 0);
+  const bool cosine = metric == 1;
+  const int64_t n = n_local;
+  SilModel md;
+  B2K_TRY(sil_prepare(ctx, X, n_local, d, ids, metric, tm, md, s));
+  const bool wg = md.wg;
+  const int64_t K = md.K, n_total = md.n_total;
+  double* stat = md.stat;
   int sm = ctx->sm_count;
   if (ctx->grid_limit > 0 && ctx->grid_limit < sm) sm = ctx->grid_limit;
   const int DP = b2k_knn_wg_dp(d);
@@ -616,8 +930,8 @@ int b2k_silhouette_impl(b2k_ctx* ctx, const float* X, int64_t n_local, int d, co
   a.K = (int)K;
   a.d = d;
   a.X = X;
-  a.cid = cid;
-  a.nrm = nrm;
+  a.cid = md.cid;
+  a.nrm = md.nrm;
   a.cnt = cnt;
   a.shift = shift;
   a.cnorm = cnorm;
@@ -675,6 +989,187 @@ int b2k_silhouette_impl(b2k_ctx* ctx, const float* X, int64_t n_local, int d, co
     ctx->stats.last_fused_ms = tm.ms(2, 3);      // silhouette pass (with the means' planes)
     ctx->stats.last_allreduce_ms = tm.ms(3, 4);  // [sum s | n]
     ctx->stats.last_loop_ms = tm.ms(0, 4);
+  }
+  return B2K_OK;
+}
+
+int b2k_silhouette_multi_impl(b2k_ctx* ctx, const float* X, int64_t n_local, int d, int n_models,
+                              const int64_t* const* ids, int metric, double* out, cudaStream_t s) {
+  const bool on = ctx->time_kernels != 0;
+  const bool cosine = metric == 1;
+  const int64_t n = n_local;
+  const int M = n_models;
+  double ms_ids = 0.0, ms_stats = 0.0, ms_pass = 0.0, ms_red = 0.0;
+  B2kTimer tall(on);
+  tall.mark(0, s);
+
+  // ---- per model: ids, statistics and the shift m, exactly as b2k_silhouette forms them ----
+  std::vector<SilModel> md(M);
+  std::vector<DevBuf> b_shift(M);
+  std::vector<float*> shift(M, nullptr);
+  std::vector<std::vector<float>> shift_h(M, std::vector<float>((size_t)d));
+  for (int m = 0; m < M; ++m) {
+    B2kTimer tm(on);
+    const int rc = sil_prepare(ctx, X, n, d, ids[m], metric, tm, md[m], s);
+    if (rc != B2K_OK) return b2k_fail(ctx, rc, "model " + std::to_string(m) + ": " + ctx->err);
+    B2K_TRY(dalloc(ctx, b_shift[m], (size_t)d, s, &shift[m]));
+    k_sil_shift<<<(unsigned)d, 256, 0, s>>>(md[m].stat, (int)md[m].K, d, (double)md[m].n_total, shift[m]);
+    B2K_CUDA_OK(ctx, cudaGetLastError());
+    ctx->stats.kernel_launches++;
+    B2K_CUDA_OK(ctx, cudaMemcpyAsync(shift_h[m].data(), shift[m], (size_t)d * 4, cudaMemcpyDeviceToHost, s));
+    tm.mark(2, s);
+    B2K_CUDA_OK(ctx, cudaStreamSynchronize(s));
+    ms_ids += tm.ms(0, 1);
+    ms_stats += tm.ms(1, 2);
+  }
+  const bool wg = md[0].wg;   // decided by d, alignment and kernel_path: the same for every model
+  int sm = ctx->sm_count;
+  if (ctx->grid_limit > 0 && ctx->grid_limit < sm) sm = ctx->grid_limit;
+  const int DP = b2k_knn_wg_dp(d);
+
+  // ---- shift groups: models whose m has the same bits share one tile rewrite y - m, so one pass ----
+  std::vector<std::vector<int>> groups;
+  for (int m = 0; m < M; ++m) {
+    bool put = false;
+    for (auto& g : groups)
+      if (std::memcmp(shift_h[g[0]].data(), shift_h[m].data(), (size_t)d * 4) == 0) {
+        g.push_back(m);
+        put = true;
+        break;
+      }
+    if (!put) groups.push_back({m});
+  }
+
+  int grid = 0;
+  int64_t ntiles = 0;
+  if (wg) {
+    ntiles = (n + PW_TM - 1) / PW_TM;
+    grid = (int)std::min<int64_t>(sm, ntiles);
+  } else {
+    ntiles = (n + GR - 1) / GR;
+    grid = (int)std::min<int64_t>(ntiles, (int64_t)sm * (ctx->grid_limit > 0 ? 1 : 8));
+  }
+  DevBuf b_sum;
+  double* sum = nullptr;   // [M][2] = {sum s, n}
+  B2K_TRY(dalloc(ctx, b_sum, (size_t)2 * M, s, &sum));
+  for (const auto& g : groups) {
+    B2kTimer tm(on);
+    tm.mark(0, s);
+    std::vector<int64_t> off(g.size() + 1, 0);
+    for (size_t j = 0; j < g.size(); ++j) off[j + 1] = off[j] + md[g[j]].K;
+    const int64_t Kt = off.back();
+    const int64_t k_pad = (Kt + PW_N - 1) / PW_N * PW_N;
+    DevBuf b_cnt, b_mu, b_psi, b_mz, b_mperm, b_psi32, b_hi, b_lo, b_cn, b_part;
+    double *cnt = nullptr, *mu = nullptr, *psi = nullptr, *part = nullptr;
+    float *Mz = nullptr, *psi32 = nullptr, *Xhi = nullptr, *Xlo = nullptr, *cnorm = nullptr;
+    int32_t* mperm = nullptr;
+    B2K_TRY(dalloc(ctx, b_cnt, (size_t)Kt, s, &cnt));
+    B2K_TRY(dalloc(ctx, b_psi, (size_t)Kt, s, &psi));
+    if (wg) {
+      B2K_TRY(dalloc(ctx, b_mz, (size_t)(Kt + 1) * d, s, &Mz));
+      B2K_TRY(dalloc(ctx, b_mperm, (size_t)k_pad, s, &mperm));
+      B2K_TRY(dalloc(ctx, b_psi32, (size_t)Kt, s, &psi32));
+      B2K_TRY(dalloc(ctx, b_hi, (size_t)k_pad * DP, s, &Xhi));
+      B2K_TRY(dalloc(ctx, b_lo, (size_t)k_pad * DP, s, &Xlo));
+      B2K_TRY(dalloc(ctx, b_cn, (size_t)k_pad, s, &cnorm));
+    } else {
+      B2K_TRY(dalloc(ctx, b_mu, (size_t)Kt * d, s, &mu));
+    }
+    // Model j's means go to Mz rows off[j] + 1 ..; k_sil_means also zeroes the row before them (its own zero row),
+    // which is model j - 1's last mean: running the models last to first rewrites that row after it was zeroed.
+    for (size_t jj = g.size(); jj-- > 0;) {
+      const SilModel& mj = md[g[jj]];
+      const int64_t o = off[jj];
+      k_sil_means<<<(unsigned)((std::max<int64_t>(mj.K, d) + 255) / 256), 256, 0, s>>>(
+          mj.stat, (int)mj.K, d, shift[g[jj]], 0, cnt + o, mu != nullptr ? mu + o * d : nullptr, psi + o,
+          Mz != nullptr ? Mz + o * d : nullptr, nullptr, psi32 != nullptr ? psi32 + o : nullptr);
+      B2K_CUDA_OK(ctx, cudaGetLastError());
+      ctx->stats.kernel_launches++;
+    }
+    if (wg) {
+      k_sil_mperm<<<(unsigned)((k_pad + 255) / 256), 256, 0, s>>>((int)Kt, k_pad, mperm);
+      B2K_CUDA_OK(ctx, cudaGetLastError());
+      ctx->stats.kernel_launches++;
+    }
+    tm.mark(1, s);
+    B2K_TRY(dalloc(ctx, b_part, (size_t)std::max(grid, 1) * SIL_MC, s, &part));
+    PairWgMaps maps;
+    if (wg && grid > 0) {
+      B2K_TRY(b2k_knn_prep_launch(ctx, Mz, Kt + 1, d, mperm, k_pad, DP, Xhi, Xlo, cnorm, s));
+      B2K_TRY(pair_wg_maps(ctx, X, n, d, Xhi, Xlo, k_pad, DP, &maps));
+    }
+    for (size_t c0 = 0; c0 < g.size(); c0 += SIL_MC) {
+      const int nm = (int)std::min<size_t>(SIL_MC, g.size() - c0);
+      SilMultiArgs a{};
+      a.n = n;
+      a.ntiles = (int)ntiles;
+      a.d = d;
+      a.nm = nm;
+      a.X = X;
+      a.nrm = md[g[c0]].nrm;   // every model's norms are the same values of X
+      a.shift = shift[g[0]];
+      a.cnorm = cnorm;
+      a.psi32 = psi32;
+      a.mu = mu;
+      a.psi = psi;
+      a.cnt = cnt;
+      for (int j = 0; j <= nm; ++j) a.off[j] = (int)off[c0 + j];
+      for (int j = 0; j < nm; ++j) a.cid[j] = md[g[c0 + j]].cid;
+      a.blo = (int)(off[c0] / PW_N);
+      a.bhi = (int)((off[c0 + nm] + PW_N - 1) / PW_N);
+      a.part = part;
+      if (grid > 0) {
+        if (wg) {
+          if (cosine)
+            B2K_TRY(pair_wg_launch<SILM_OWN>(
+                ctx, DP, [](auto nch) { return k_sil_wg_multi<decltype(nch)::value, true>; }, grid, maps, a, s));
+          else
+            B2K_TRY(pair_wg_launch<SILM_OWN>(
+                ctx, DP, [](auto nch) { return k_sil_wg_multi<decltype(nch)::value, false>; }, grid, maps, a, s));
+          ctx->stats.fused_tc_launches++;
+        } else {
+          const auto k = cosine ? k_sil_generic_multi<true> : k_sil_generic_multi<false>;
+          B2K_CUDA_OK(ctx, cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, SILM_GEN_SMEM));
+          k<<<(unsigned)grid, G_NT, SILM_GEN_SMEM, s>>>(a);
+          B2K_CUDA_OK(ctx, cudaGetLastError());
+          ctx->stats.generic_launches++;
+        }
+        ctx->stats.kernel_launches++;
+      }
+      for (int j = 0; j < nm; ++j) {
+        double* sm_j = sum + 2 * g[c0 + j];
+        if (grid > 0) B2K_TRY(b2k_launch_fold_f64(ctx, part + (size_t)j * grid, grid, sm_j, s));
+        else B2K_CUDA_OK(ctx, cudaMemsetAsync(sm_j, 0, sizeof(double), s));
+      }
+    }
+    tm.mark(2, s);
+    B2K_CUDA_OK(ctx, cudaStreamSynchronize(s));   // the group's buffers are freed on return of this scope
+    ms_stats += tm.ms(0, 1);
+    ms_pass += tm.ms(1, 2);
+  }
+  ctx->stats.last_path = wg ? B2K_PATH_FUSED : B2K_PATH_GENERIC;
+
+  // ---- one [sum s | n] allreduce per model, as b2k_silhouette does ----
+  B2kTimer tr(on);
+  tr.mark(0, s);
+  const double nd = (double)n;
+  std::vector<double> res((size_t)2 * M);
+  for (int m = 0; m < M; ++m) {
+    B2K_CUDA_OK(ctx, cudaMemcpyAsync(sum + 2 * m + 1, &nd, sizeof(double), cudaMemcpyHostToDevice, s));
+    B2K_TRY(b2k_comm_allreduce_f64(ctx, sum + 2 * m, 2, s));
+  }
+  B2K_CUDA_OK(ctx, cudaMemcpyAsync(res.data(), sum, res.size() * 8, cudaMemcpyDeviceToHost, s));
+  tr.mark(1, s);
+  tall.mark(1, s);
+  B2K_CUDA_OK(ctx, cudaStreamSynchronize(s));
+  for (int m = 0; m < M; ++m) out[m] = res[2 * m] / res[2 * m + 1];
+  if (on) {
+    ms_red = tr.ms(0, 1);
+    ctx->stats.last_finalize_ms = ms_ids;
+    ctx->stats.last_reduce_ms = ms_stats;
+    ctx->stats.last_fused_ms = ms_pass;
+    ctx->stats.last_allreduce_ms = ms_red;
+    ctx->stats.last_loop_ms = tall.ms(0, 1);
   }
   return B2K_OK;
 }

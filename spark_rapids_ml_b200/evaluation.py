@@ -88,6 +88,35 @@ class _SilhouetteCaller(_CumlCaller, HasFeaturesCol, HasFeaturesCols):
         return _cuml_fit
 
 
+class _SilhouetteMultiCaller(_SilhouetteCaller):
+    """_SilhouetteCaller's barrier task for KMeansModel._transformEvaluate: the rows are labelled on the device with
+    each centre set as KMeansModel.transform labels them (Context.kmeans_assign), then one Context.silhouette_multi
+    call scores every set; rank 0's values are returned."""
+
+    def __init__(self, features: Any, center_sets: List[Any], distance: str) -> None:
+        super().__init__(features, "", distance)
+        self._center_sets = [np.asarray(c, dtype=np.float32) for c in center_sets]
+
+    def _out_schema(self) -> Any:
+        return "silhouette array<double>"
+
+    def _pre_process_data(self, dataset: Any) -> Tuple[Any, Optional[List[str]], int, str]:
+        return _CumlCaller._pre_process_data(self, dataset)
+
+    def _get_cuml_fit_func(self, dataset: Any, extra_params: Optional[List[Dict[str, Any]]] = None) -> Any:
+        distance, center_sets = self._distance, self._center_sets
+
+        def _cuml_fit(dfs: Any, params: Dict[str, Any]) -> Dict[str, Any]:
+            import torch
+
+            ctx = params[param_alias.handle]
+            X = dfs[0][0]
+            ids = [ctx.kmeans_assign(X, torch.from_numpy(C).to(X.device))[0].to(torch.int64) for C in center_sets]
+            return {"silhouette": [ctx.silhouette_multi(X, ids, distance)]}
+
+        return _cuml_fit
+
+
 class ClusteringEvaluator(_ClusteringEvaluatorBase):
     """pyspark.ml.evaluation.ClusteringEvaluator on the device: metricName "silhouette", distanceMeasure
     "squaredEuclidean" (default) or "cosine", featuresCol (an array column or a list of numeric columns, as
