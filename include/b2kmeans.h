@@ -657,10 +657,12 @@ int b2k_eval_binary(b2k_ctx* ctx, const double* scores, const uint8_t* pos, int6
                     int metric, double* out, uintptr_t stream);
 
 /* ---- silhouette (b2k_silhouette.cu): Spark's ClusteringEvaluator, metricName "silhouette" ----
- * No reference interface: Spark computes it in closed form (ClusteringEvaluator / SquaredEuclideanSilhouette /
- * CosineSilhouette); tests/silhouette_oracle.py restates the rule in fp64 NumPy.  X device f32 [n_local][d] (this rank's
- * rows), cluster_ids device int64 [n_local] (any values; -1 is a cluster like any other), metric 0 squaredEuclidean or 1
- * cosine; *out (host) = the metric.  Rule, over the rows of all ranks (n rows, clusters = the distinct ids):
+ * b2k_silhouette is the one-model case of b2k_silhouette_multi below: the same passes with n_models = 1, and its errors
+ * without the "model 0: " prefix.  No reference interface: Spark computes it in closed form (ClusteringEvaluator /
+ * SquaredEuclideanSilhouette / CosineSilhouette); tests/silhouette_oracle.py restates the rule in fp64 NumPy.  X device
+ * f32 [n_local][d] (this rank's rows), cluster_ids device int64 [n_local] (any values; -1 is a cluster like any other),
+ * metric 0 squaredEuclidean or 1 cosine; *out (host) = the metric.  Rule, over the rows of all ranks (n rows, clusters =
+ * the distinct ids):
  *   rows     y = x (metric 0), or y = fl32(x / |x|) with |x| = sqrt of the feature-order fp64 sum of squares (metric 1,
  *            DBSCAN's rule), so that ||y_i - y_j||^2 = 2 (1 - cos) up to the rounding of y.
  *   D(i, c)  = the mean of ||y_i - y_j||^2 over the members j of cluster c (all of them) = ||y_i - mu_c||^2 + Psi_c, mu_c
@@ -698,8 +700,9 @@ int b2k_eval_binary(b2k_ctx* ctx, const double* scores, const uint8_t* pos, int6
 int b2k_silhouette(b2k_ctx* ctx, const float* X, int64_t n_local, int d, const int64_t* cluster_ids, int metric,
                    double* out, uintptr_t stream);
 /* b2k_silhouette_multi: the silhouette of n_models >= 1 clusterings of the same rows in one call.  cluster_ids is a host
- * array of n_models device int64 [n_local] arrays; out (host) [n_models].  out[m] has exactly the bits that
- * b2k_silhouette(ctx, X, n_local, d, cluster_ids[m], metric, ...) returns, for any rank count, grid_limit and kernel_path.
+ * array of n_models device int64 [n_local] arrays; out (host) [n_models].  A model's bits do not depend on which models
+ * share the call: out[m] has exactly the bits that b2k_silhouette(ctx, X, n_local, d, cluster_ids[m], metric, ...)
+ * returns, for any rank count, grid_limit and kernel_path.
  * Per model: the ids and statistics passes of b2k_silhouette and its shift m.  Models whose m has the same bits form a
  * shift group; a group's shifted means are packed one model after another into shared blocks of 128 (wgmma) or tiles
  * of 64 (generic), and one silhouette pass per chunk of at most B2K_SILHOUETTE_MULTI_CHUNK models scores all of them in

@@ -1031,7 +1031,8 @@ extern "C" int b2k_silhouette(b2k_ctx* ctx, const float* X, int64_t n_local, int
   if (n_local < 0 || d <= 0 || (n_local > 0 && (!X || !cluster_ids)) || !out)
     return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_silhouette: bad X/cluster_ids/out/n/d");
   B2K_CUDA_OK(ctx, cudaSetDevice(ctx->device));
-  return b2k_silhouette_impl(ctx, X, n_local, d, cluster_ids, metric, out, reinterpret_cast<cudaStream_t>(stream));
+  return b2k_silhouette_impl(ctx, X, n_local, d, 1, &cluster_ids, metric, out, nullptr,
+                             reinterpret_cast<cudaStream_t>(stream));
 }
 
 extern "C" int b2k_silhouette_multi(b2k_ctx* ctx, const float* X, int64_t n_local, int d, int n_models,
@@ -1045,8 +1046,11 @@ extern "C" int b2k_silhouette_multi(b2k_ctx* ctx, const float* X, int64_t n_loca
     if (n_local > 0 && !cluster_ids[m])
       return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_silhouette_multi: cluster_ids[" + std::to_string(m) + "] is NULL");
   B2K_CUDA_OK(ctx, cudaSetDevice(ctx->device));
-  return b2k_silhouette_multi_impl(ctx, X, n_local, d, n_models, cluster_ids, metric, out,
-                                   reinterpret_cast<cudaStream_t>(stream));
+  int failed = -1;
+  const int rc = b2k_silhouette_impl(ctx, X, n_local, d, n_models, cluster_ids, metric, out, &failed,
+                                     reinterpret_cast<cudaStream_t>(stream));
+  if (rc != B2K_OK && failed >= 0) return b2k_fail(ctx, rc, "model " + std::to_string(failed) + ": " + ctx->err);
+  return rc;
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -385,12 +385,11 @@ struct B2kTimer {   // CUDA events around the device phases when option time_ker
 };
 
 // ------------------------------------------------------------------------------------------------
-// silhouette — b2k_silhouette.cu (the C ABI entry point in b2k_api.cu checks its arguments, then calls this)
+// silhouette — b2k_silhouette.cu (the C ABI entry points in b2k_api.cu check their arguments, then call this with
+// one model or several; on an error of one model's ids or statistics, *failed_model (if not NULL) = that model)
 // ------------------------------------------------------------------------------------------------
-int b2k_silhouette_impl(b2k_ctx* ctx, const float* X, int64_t n_local, int d, const int64_t* ids, int metric,
-                        double* out, cudaStream_t s);
-int b2k_silhouette_multi_impl(b2k_ctx* ctx, const float* X, int64_t n_local, int d, int n_models,
-                              const int64_t* const* ids, int metric, double* out, cudaStream_t s);
+int b2k_silhouette_impl(b2k_ctx* ctx, const float* X, int64_t n_local, int d, int n_models, const int64_t* const* ids,
+                        int metric, double* out, int* failed_model, cudaStream_t s);
 
 // ------------------------------------------------------------------------------------------------
 // approximate k-NN (IVF-Flat) — b2k_ivf.cu (the C ABI entry point in b2k_api.cu checks its arguments, then calls this)

@@ -1,30 +1,30 @@
-// Silhouette (sm_90a): b2k_silhouette, the metric of Spark's ClusteringEvaluator in its closed form, squared Euclidean
-// or cosine.  Rows y are x (squared Euclidean) or fl32(x / ||x||) with the fp64 norm (cosine: DBSCAN's k_db_normalize
-// rule); cosine is then the squared Euclidean silhouette of the y, since ||y - z||^2 = 2 (1 - cos) for unit rows and s is
-// a ratio.  Passes:
+// Silhouette (sm_90a): b2k_silhouette and b2k_silhouette_multi, the metric of Spark's ClusteringEvaluator in its closed
+// form, squared Euclidean or cosine, for 1 .. n clusterings (models) of the same rows; b2k_silhouette is the one-model
+// case.  Rows y are x (squared Euclidean) or fl32(x / ||x||) with the fp64 norm (cosine: DBSCAN's k_db_normalize rule);
+// cosine is then the squared Euclidean silhouette of the y, since ||y - z||^2 = 2 (1 - cos) for unit rows and s is a
+// ratio.  Passes:
 //
-//   ids         per rank: a CUB radix sort of (id, row) and a run-length encode -> the local distinct ids ascending, the
-//               rows of each (perm) and its row offsets.  Allgather of the sizes, then of the distinct ids (padded to the
-//               largest count); the host merges them into the K global ids and maps each local run to its dense index;
-//               cid[row] = that index.
-//   statistics  one read of X in perm order (k_sil_stats): chunks of SIL_SC sorted rows write, per run they meet, the
-//               fp64 sums of y_f and of ||y||^2 as one piece; k_sil_stats_fold adds each run's pieces in chunk order into
-//               stat [K][d + 2] = {sum y, sum ||y||^2, N}.  Two integer counters (non-finite values, zero rows) follow;
-//               one f64 allreduce.  Then on the device: the shift m = fl32(sum_c sum y / n) (k_sil_shift), and per
-//               cluster mu_c, Psi_c = sum ||y||^2 / N_c - ||mu_c||^2 in fp64 and the shifted means fl32(mu_c - m).
-//   silhouette  D(i, c) = ||y_i - mu_c||^2 + Psi_c over every cluster c; a = D(i, A) N_A / (N_A - 1), b = min over c != A;
-//               s_i; per-CTA fp64 sums of s_i folded in CTA order; one allreduce of [sum s | n].
+//   ids         per model and rank: a CUB radix sort of (id, row) and a run-length encode -> the local distinct ids
+//               ascending, the rows of each (perm) and its row offsets.  Allgather of the sizes, then of the distinct ids
+//               (padded to the largest count); the host merges them into the K global ids and maps each local run to its
+//               dense index; cid[row] = that index.
+//   statistics  per model, one read of X in perm order (k_sil_stats): chunks of SIL_SC sorted rows write, per run they
+//               meet, the fp64 sums of y_f and of ||y||^2 as one piece; k_sil_stats_fold adds each run's pieces in chunk
+//               order into stat [K][d + 2] = {sum y, sum ||y||^2, N}.  Two integer counters (non-finite values, zero
+//               rows) follow; one f64 allreduce.  Then on the device: the shift m = fl32(sum_c sum y / n) (k_sil_shift),
+//               and per cluster mu_c, Psi_c = sum ||y||^2 / N_c - ||mu_c||^2 in fp64 and the shifted means fl32(mu_c - m).
+//   silhouette  models whose m has the same bits form a shift group; a group's means are packed side by side, and one
+//               pass per chunk of at most B2K_SILHOUETTE_MULTI_CHUNK models forms D(i, c) = ||y_i - mu_c||^2 + Psi_c over
+//               every cluster c of each model; a = D(i, A) N_A / (N_A - 1), b = min over c != A; s_i; per model,
+//               per-CTA fp64 sums of s_i folded in CTA order; one allreduce of [sum s | n] per model.
 //     wgmma    (k_sil_wg, 3xTF32): d % 4 == 0, 4 <= d <= 128, 16-byte aligned X.  The tile operand is X itself (TMA);
 //              each consumer warp rewrites its 16 rows of the tile in shared memory once per tile as y - m (one fp32
 //              rounding) and takes their fp64 norms, so the pipeline of b2k_pair_wg.cuh runs unchanged; the block
-//              operand is the hi / lo planes of the shifted means (k_knn_prep over a zero row and the means).
+//              operand is the hi / lo planes of the shifted means (k_knn_prep over a zero row and the packed means).
 //              D = fl32(fl32(n_c - 2 acc) + n_i) + Psi_c in fp32, within the bound of include/b2kmeans.h.
 //     generic  (k_sil_generic, SIMT): every shape; D = sum_f (y_f - mu_c,f)^2 + Psi_c in fp64.
-// b2k_silhouette_multi scores several clusterings of the same rows: per model the ids and statistics passes above,
-// then one silhouette pass (k_sil_wg_multi / k_sil_generic_multi) per shift group and chunk of models over their means
-// packed side by side, with the bits of each model's own call.
-// No floating-point atomics: integer counters only, every fp64 sum in a fixed order for a given grid, so two calls on
-// the same input, rank count and device give the same bits.
+// A model's bits do not depend on which models share the call.  No floating-point atomics: integer counters only, every
+// fp64 sum in a fixed order for a given grid, so two calls on the same input, rank count and device give the same bits.
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_run_length_encode.cuh>
 #include <cub/device/device_scan.cuh>
@@ -45,21 +45,6 @@ namespace {
 constexpr int SIL_SC = 256;      // sorted rows per statistics chunk
 constexpr int ST_NT = 128;       // threads of the statistics kernels (one feature each)
 constexpr int SIL_KMAX = B2K_SILHOUETTE_MAX_CLUSTERS;
-
-struct SilArgs {
-  int64_t n;                     // this rank's rows
-  int ntiles, nblk, K, d;
-  const float* X;                // [n][d]
-  const int32_t* cid;            // dense cluster of each row [n]
-  const double* nrm;             // cosine: fp64 ||x|| [n]; NULL otherwise
-  const double* cnt;             // N_c [K]
-  const float* shift;            // wgmma: m [d]
-  const float* cnorm;            // wgmma: ||fl32(mu_c - m)||^2 [K_pad] (fp32 of the fp64 sum)
-  const float* psi32;            // wgmma: fl32(Psi_c) [K]
-  const double* mu;              // generic: mu_c [K][d]
-  const double* psi;             // generic: Psi_c [K]
-  double* part;                  // per-CTA sum of s_i [grid]
-};
 
 __device__ __forceinline__ float sil_y(float x, const double* nrm, int64_t row) {
   return nrm != nullptr ? (float)__ddiv_rn((double)x, nrm[row]) : x;
@@ -214,24 +199,23 @@ __global__ void __launch_bounds__(256) k_sil_shift(const double* __restrict__ st
   if (threadIdx.x == 0) shift[f] = (float)(red[0] / n_total);
 }
 
-// per cluster: cnt, mu (fp64), Psi; wgmma: rows 1 .. K of Mz = fl32(mu - m) (row 0 zero), perm of k_knn_prep, fl32(Psi)
+// per cluster of one model: cnt, mu (fp64), Psi; wgmma: the shifted means fl32(mu - m) into Mz [K][d], fl32(Psi)
 __global__ void __launch_bounds__(256) k_sil_means(const double* __restrict__ stat, int K, int d,
-                                                   const float* __restrict__ shift, int64_t k_pad,
-                                                   double* __restrict__ cnt, double* __restrict__ mu,
-                                                   double* __restrict__ psi, float* __restrict__ Mz,
-                                                   int32_t* __restrict__ mperm, float* __restrict__ psi32) {
+                                                   const float* __restrict__ shift, double* __restrict__ cnt,
+                                                   double* __restrict__ mu, double* __restrict__ psi,
+                                                   float* __restrict__ Mz, float* __restrict__ psi32) {
   const int64_t c = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (Mz != nullptr && c < k_pad) mperm[c] = c < K ? (int32_t)(c + 1) : -1;
-  if (Mz != nullptr && c < d) Mz[c] = 0.f;
   if (c >= K) return;
   const double* st = stat + c * (d + 2);
   const double N = st[d + 1];
+  double* mu_c = mu != nullptr ? mu + c * d : nullptr;
+  float* mz_c = Mz != nullptr ? Mz + c * d : nullptr;
   double m2 = 0.0;
   for (int f = 0; f < d; ++f) {
     const double v = st[f] / N;
     m2 += v * v;
-    if (mu != nullptr) mu[c * d + f] = v;
-    if (Mz != nullptr) Mz[(c + 1) * d + f] = (float)(v - (double)shift[f]);
+    if (mu_c != nullptr) mu_c[f] = v;
+    if (mz_c != nullptr) mz_c[f] = (float)(v - (double)shift[f]);
   }
   const double p = st[d] / N - m2;
   cnt[c] = N;
@@ -239,214 +223,25 @@ __global__ void __launch_bounds__(256) k_sil_means(const double* __restrict__ st
   if (psi32 != nullptr) psi32[c] = (float)p;
 }
 
-// b2k_silhouette_multi: the k_knn_prep permutation of a group's packed means, plane row c <- Mz row c + 1
-__global__ void __launch_bounds__(256) k_sil_mperm(int K, int64_t k_pad, int32_t* __restrict__ mperm) {
+// wgmma: a group's packed means Mz = [zero row; K means]: the zero row, and the k_knn_prep permutation that takes
+// plane row c from Mz row c + 1
+__global__ void __launch_bounds__(256) k_sil_mperm(int K, int64_t k_pad, int d, float* __restrict__ Mz,
+                                                   int32_t* __restrict__ mperm) {
   const int64_t c = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (c < d) Mz[c] = 0.f;
   if (c < k_pad) mperm[c] = c < K ? (int32_t)(c + 1) : -1;
 }
 
-// ---- silhouette, wgmma ----
-constexpr int SIL_OWN = PW_TM * 4 + 256 * 8;   // the tile's row norms, the consumers' sums
-template <int NCH>
-using SilWgCfg = PairWgCfg<NCH, SIL_OWN>;
-
-__device__ __forceinline__ void sil_bar_consumers() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
-
-// Persistent grid, static round-robin over tiles of PW_TM rows; a unit is one tile against every block of the means.
-template <int NCH, bool COS>
-__global__ void __launch_bounds__(PW_NTHREADS, 1)
-k_sil_wg(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapHi,
-         const __grid_constant__ CUtensorMap mapLo, const SilArgs a) {
-  using G = SilWgCfg<NCH>;
-  constexpr int R = PW_N / 2;
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  const uint32_t base = smem_u32(smem_raw);
-  const PairWgBars bars = pair_wg_init<G>(base);
-  float* snx = reinterpret_cast<float*>(smem_raw + G::OFF_OWN);
-  double* sred = reinterpret_cast<double*>(smem_raw + G::OFF_OWN + PW_TM * 4);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int nit = (int)blockIdx.x < a.ntiles ? (a.ntiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
-
-  if (warp >= 8) {
-    if (warp == 8 && elect_one())
-      pair_wg_produce<G>(
-          base, bars, &mapQ, &mapHi, &mapLo, nit,
-          [&](int it) { return PairWgUnit{((int)blockIdx.x + it * (int)gridDim.x) * PW_TM, 0, a.nblk}; },
-          [](int) { return false; });
-    __syncwarp();
-    return;
-  }
-
-  const int g = warp >> 2, wi = warp & 3;
-  const int wr0 = g * 64 + wi * 16;                 // this warp's 16 rows of the tile
-  const int rr0 = wr0 + (lane >> 2);                // this thread's rows rr0, rr0 + 8
-  float acc[R];
-  int q = 0;
-  double ssum = 0.0;
-  for (int it = 0; it < nit; ++it) {
-    const int64_t t0 = ((int64_t)blockIdx.x + (int64_t)it * gridDim.x) * PW_TM;
-    mbar_wait_nocall(bars.qfull(), (uint32_t)(it & 1));
-    // y - m in place (128B swizzle: row r, column cc of chunk c at r 128 + ((cc / 4) ^ (r % 8)) 16 + (cc % 4) 4)
-    for (int k = 0; k < 16; ++k) {
-      const int r = wr0 + k;
-      const int64_t row = t0 + r;
-      double s2 = 0.0;
-      if (row < a.n) {
-        for (int col = lane; col < a.d; col += 32) {
-          const int cc = col & 31;
-          float* p = reinterpret_cast<float*>(smem_raw + G::OFF_Q + (col >> 5) * G::QBYTES + r * 128 +
-                                              ((((cc >> 2) ^ (r & 7))) << 4) + (cc & 3) * 4);
-          const float v = sil_y(*p, COS ? a.nrm : nullptr, row) - __ldg(a.shift + col);
-          *p = v;
-          s2 += (double)v * (double)v;
-        }
-      }
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) s2 += __shfl_xor_sync(0xffffffffu, s2, o);
-      if (lane == 0) snx[r] = (float)s2;
-    }
-    __syncwarp();
-    int64_t row[2];
-    int own[2];
-    float nx[2], d_own[2], d_min[2];
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      row[h] = t0 + rr0 + 8 * h;
-      own[h] = row[h] < a.n ? __ldg(a.cid + row[h]) : -1;
-      nx[h] = snx[rr0 + 8 * h];
-      d_own[h] = -INFINITY;
-      d_min[h] = INFINITY;
-    }
-    for (int b = 0; b < a.nblk; ++b) {
-      pair_wg_block<G>(smem_raw, base, bars, rr0, lane, acc, q);
-      // acc[i] is row rr0 + 8 ((i >> 1) & 1), block column 8 (i >> 2) + 2 (lane & 3) + (i & 1)
-      const int cb = b * PW_N + 2 * (lane & 3);
-#pragma unroll
-      for (int i = 0; i < R; ++i) {
-        const int h = (i >> 1) & 1;
-        const int c = cb + 8 * (i >> 2) + (i & 1);
-        if (c >= a.K) continue;
-        const float S = fmaf(-2.f, acc[i], __ldg(a.cnorm + c)) + nx[h];
-        const float D = S + __ldg(a.psi32 + c);
-        if (c == own[h]) d_own[h] = D;
-        else d_min[h] = fminf(d_min[h], D);
-      }
-    }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // the rewritten tile before the next TMA write
-    __syncwarp();
-    if (lane == 0) mbar_arrive(bars.qempty());
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {   // the quad's four lanes hold the same rows
-      d_min[h] = fminf(d_min[h], __shfl_xor_sync(0xffffffffu, d_min[h], 1));
-      d_min[h] = fminf(d_min[h], __shfl_xor_sync(0xffffffffu, d_min[h], 2));
-      d_own[h] = fmaxf(d_own[h], __shfl_xor_sync(0xffffffffu, d_own[h], 1));
-      d_own[h] = fmaxf(d_own[h], __shfl_xor_sync(0xffffffffu, d_own[h], 2));
-      if ((lane & 3) == 0 && own[h] >= 0) ssum += sil_s((double)d_own[h], (double)d_min[h], __ldg(a.cnt + own[h]));
-    }
-  }
-  sred[threadIdx.x] = ssum;
-  sil_bar_consumers();
-  if (threadIdx.x == 0) {
-    double t = 0.0;
-    for (int i = 0; i < 256; ++i) t += sred[i];
-    a.part[blockIdx.x] = t;
-  }
-}
-
-// ---- silhouette, generic: CTA = 64 rows x tiles of 64 clusters; thread (ty, tx) owns rows ty + 16 i and clusters
-// tx + 16 j (i, j < 4), fp64 sums over features staged 32 at a time ----
-constexpr int GR = 64, GC = 64, GF = 32, G_NT = 256;
-template <bool COS>
-__global__ void __launch_bounds__(G_NT, 1) k_sil_generic(const SilArgs a) {
-  __shared__ double xr[GF][GR + 1], mc[GF][GC + 1];
-  __shared__ double sred[G_NT];
-  const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
-  const int d = a.d;
-  double ssum = 0.0;
-  for (int tile = blockIdx.x; tile < a.ntiles; tile += gridDim.x) {
-    int64_t row[4];
-    int own[4];
-    double d_own[4], d_min[4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      row[i] = (int64_t)tile * GR + ty + 16 * i;
-      own[i] = row[i] < a.n ? a.cid[row[i]] : -1;
-      d_own[i] = -INFINITY;
-      d_min[i] = INFINITY;
-    }
-    for (int c0 = 0; c0 < a.K; c0 += GC) {
-      double acc[4][4];
-#pragma unroll
-      for (int i = 0; i < 4; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) acc[i][j] = 0.0;
-      for (int f0 = 0; f0 < d; f0 += GF) {
-        __syncthreads();
-        for (int e = threadIdx.x; e < GF * GR; e += G_NT) {
-          const int r = e / GF, c = e % GF;
-          const int64_t gr = (int64_t)tile * GR + r;
-          const int f = f0 + c, cl = c0 + r;
-          xr[c][r] = (gr < a.n && f < d) ? (double)sil_y(a.X[gr * d + f], COS ? a.nrm : nullptr, gr) : 0.0;
-          mc[c][r] = (cl < a.K && f < d) ? a.mu[(int64_t)cl * d + f] : 0.0;
-        }
-        __syncthreads();
-        const int fc = min(GF, d - f0);
-        for (int c = 0; c < fc; ++c) {
-          double vr[4], vc[4];
-#pragma unroll
-          for (int i = 0; i < 4; ++i) vr[i] = xr[c][ty + 16 * i];
-#pragma unroll
-          for (int j = 0; j < 4; ++j) vc[j] = mc[c][tx + 16 * j];
-#pragma unroll
-          for (int i = 0; i < 4; ++i)
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              const double t = vr[i] - vc[j];
-              acc[i][j] = fma(t, t, acc[i][j]);
-            }
-        }
-      }
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const int cl = c0 + tx + 16 * j;
-        if (cl >= a.K) continue;
-        const double p = a.psi[cl];
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const double D = acc[i][j] + p;
-          if (cl == own[i]) d_own[i] = D;
-          else d_min[i] = fmin(d_min[i], D);
-        }
-      }
-    }
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {   // the 16 lanes of a half warp hold the same rows
-#pragma unroll
-      for (int o = 1; o < 16; o <<= 1) {
-        d_min[i] = fmin(d_min[i], __shfl_xor_sync(0xffffffffu, d_min[i], o));
-        d_own[i] = fmax(d_own[i], __shfl_xor_sync(0xffffffffu, d_own[i], o));
-      }
-      if (tx == 0 && own[i] >= 0) ssum += sil_s(d_own[i], d_min[i], a.cnt[own[i]]);
-    }
-  }
-  sred[threadIdx.x] = ssum;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double t = 0.0;
-    for (int i = 0; i < G_NT; ++i) t += sred[i];
-    a.part[blockIdx.x] = t;
-  }
-}
-
-// ---- b2k_silhouette_multi: the means of several models packed into one column space ----
+// ---- silhouette pass: the means of several models packed into one column space ----
 // A shift group's models are segments [off[j], off[j + 1]) of the packed clusters, in model order, with no padding
-// between them (a segment may start inside a block).  A launch serves a chunk of at most SIL_MC models; its per (row,
-// model) state lives in shared memory, so its cost does not grow with the chunk.  Each (row, cluster) D is formed
-// exactly as in the one-model passes, d_own / d_min are a select and a min, and each thread adds its rows' s_i per model
-// in the same order as there, so every model's sum has the bits of its own b2k_silhouette call.
+// between them (a segment may start inside a block); b2k_silhouette is a group of one model.  A launch serves a chunk
+// of at most SIL_MC models; its per (row, model) state lives in shared memory, so its cost does not grow with the
+// chunk.  Each (row, cluster) D depends only on the row's tile and that cluster's mean, d_own / d_min are a select and
+// a min, and each thread adds its rows' s_i per model in tile order, so a model's bits do not depend on which models
+// share the launch.
 constexpr int SIL_MC = B2K_SILHOUETTE_MULTI_CHUNK;
 
-struct SilMultiArgs {
+struct SilArgs {
   int64_t n;
   int ntiles, d, nm;             // nm: models in this chunk
   int blo, bhi;                  // wgmma: the blocks of means the chunk's segments touch
@@ -463,17 +258,21 @@ struct SilMultiArgs {
   double* part;                  // per model j, per CTA: part[j grid + CTA]
 };
 
-// The per-thread sums of the one-model passes fold over every thread in order; the threads that add no row keep +0.0,
-// and +0.0 changes no partial sum (none is ever -0.0), so folding only the adding threads, in order, gives the same bits.
-constexpr int SILM_OWN = PW_TM * 4 + SIL_MC * PW_TM * 8 + SIL_MC * 64 * 8;   // norms, (d_own, d_min), per-thread sums
+// ---- wgmma ----
+constexpr int SIL_OWN = PW_TM * 4 + SIL_MC * PW_TM * 8 + SIL_MC * 64 * 8;   // norms, (d_own, d_min), per-thread sums
 template <int NCH>
-using SilMultiWgCfg = PairWgCfg<NCH, SILM_OWN>;
+using SilWgCfg = PairWgCfg<NCH, SIL_OWN>;
 
+__device__ __forceinline__ void sil_bar_consumers() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
+
+// Persistent grid, static round-robin over tiles of PW_TM rows; a unit is one tile against the blocks of means the
+// chunk touches.  Per model, each thread that adds rows (a quad's first lane) keeps its own sum of s_i; thread j of the
+// consumers folds model j's sums in thread order.
 template <int NCH, bool COS>
 __global__ void __launch_bounds__(PW_NTHREADS, 1)
-k_sil_wg_multi(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapHi,
-               const __grid_constant__ CUtensorMap mapLo, const __grid_constant__ SilMultiArgs a) {
-  using G = SilMultiWgCfg<NCH>;
+k_sil_wg(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapHi,
+         const __grid_constant__ CUtensorMap mapLo, const __grid_constant__ SilArgs a) {
+  using G = SilWgCfg<NCH>;
   constexpr int R = PW_N / 2;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   const uint32_t base = smem_u32(smem_raw);
@@ -496,8 +295,8 @@ k_sil_wg_multi(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__
   }
 
   const int g = warp >> 2, wi = warp & 3;
-  const int wr0 = g * 64 + wi * 16;
-  const int rr0 = wr0 + (lane >> 2);
+  const int wr0 = g * 64 + wi * 16;                 // this warp's 16 rows of the tile
+  const int rr0 = wr0 + (lane >> 2);                // this thread's rows rr0, rr0 + 8
   const bool lead = (lane & 3) == 0;                 // the quad's four lanes hold the same rows
   double* my_sum = sred + (threadIdx.x >> 2);        // the adding threads in thread order
   if (lead)
@@ -507,7 +306,8 @@ k_sil_wg_multi(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__
   for (int it = 0; it < nit; ++it) {
     const int64_t t0 = ((int64_t)blockIdx.x + (int64_t)it * gridDim.x) * PW_TM;
     mbar_wait_nocall(bars.qfull(), (uint32_t)(it & 1));
-    for (int k = 0; k < 16; ++k) {   // y - m in place, as k_sil_wg
+    // y - m in place (128B swizzle: row r, column cc of chunk c at r 128 + ((cc / 4) ^ (r % 8)) 16 + (cc % 4) 4)
+    for (int k = 0; k < 16; ++k) {
       const int r = wr0 + k;
       const int64_t row = t0 + r;
       double s2 = 0.0;
@@ -540,6 +340,7 @@ k_sil_wg_multi(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__
     }
     for (int b = a.blo; b < a.bhi; ++b) {
       pair_wg_block<G>(smem_raw, base, bars, rr0, lane, acc, q);
+      // acc[i] is row rr0 + 8 ((i >> 1) & 1), block column 8 (i >> 2) + 2 (lane & 3) + (i & 1)
       const int cb = b * PW_N + 2 * (lane & 3);
       for (int j = 0; j < a.nm; ++j) {   // the segments this block meets (uniform over the CTA)
         const int lo = a.off[j], hi = a.off[j + 1];
@@ -577,7 +378,7 @@ k_sil_wg_multi(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__
         }
       }
     }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // the rewritten tile before the next TMA write
     __syncwarp();
     if (lane == 0) mbar_arrive(bars.qempty());
     if (lead)
@@ -599,10 +400,13 @@ k_sil_wg_multi(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__
   }
 }
 
-// generic: k_sil_generic's tiles over the chunk's packed clusters [off[0], off[nm])
-constexpr int SILM_GEN_SMEM = 2 * GF * (GR + 1) * 8 + 2 * SIL_MC * GR * 8 + SIL_MC * 16 * 8;
+// ---- generic: CTA = 64 rows x tiles of 64 of the chunk's packed clusters [off[0], off[nm]); thread (ty, tx) owns rows
+// ty + 16 i and clusters tx + 16 j (i, j < 4), fp64 sums over features staged 32 at a time; per model, the first thread
+// of each half warp keeps its sum of s_i ----
+constexpr int GR = 64, GC = 64, GF = 32, G_NT = 256;
+constexpr int SIL_GEN_SMEM = 2 * GF * (GR + 1) * 8 + 2 * SIL_MC * GR * 8 + SIL_MC * 16 * 8;
 template <bool COS>
-__global__ void __launch_bounds__(G_NT, 1) k_sil_generic_multi(const __grid_constant__ SilMultiArgs a) {
+__global__ void __launch_bounds__(G_NT, 1) k_sil_generic(const __grid_constant__ SilArgs a) {
   extern __shared__ __align__(16) uint8_t gsm[];
   double(*xr)[GR + 1] = reinterpret_cast<double(*)[GR + 1]>(gsm);
   double(*mc)[GC + 1] = reinterpret_cast<double(*)[GC + 1]>(gsm + GF * (GR + 1) * 8);
@@ -885,116 +689,8 @@ int sil_prepare(b2k_ctx* ctx, const float* X, int64_t n_local, int d, const int6
   return B2K_OK;
 }
 
-int b2k_silhouette_impl(b2k_ctx* ctx, const float* X, int64_t n_local, int d, const int64_t* ids, int metric,
-                        double* out, cudaStream_t s) {
-  B2kTimer tm(ctx->time_kernels != 0);
-  const bool cosine = metric == 1;
-  const int64_t n = n_local;
-  SilModel md;
-  B2K_TRY(sil_prepare(ctx, X, n_local, d, ids, metric, tm, md, s));
-  const bool wg = md.wg;
-  const int64_t K = md.K, n_total = md.n_total;
-  double* stat = md.stat;
-  int sm = ctx->sm_count;
-  if (ctx->grid_limit > 0 && ctx->grid_limit < sm) sm = ctx->grid_limit;
-  const int DP = b2k_knn_wg_dp(d);
-  const int64_t k_pad = (K + PW_N - 1) / PW_N * PW_N;
-  DevBuf b_cnt, b_mu, b_psi, b_shift, b_mz, b_mperm, b_psi32, b_hi, b_lo, b_cn, b_part, b_sum;
-  double *cnt = nullptr, *mu = nullptr, *psi = nullptr, *part = nullptr, *sum = nullptr;
-  float *shift = nullptr, *Mz = nullptr, *psi32 = nullptr, *Xhi = nullptr, *Xlo = nullptr, *cnorm = nullptr;
-  int32_t* mperm = nullptr;
-  B2K_TRY(dalloc(ctx, b_cnt, (size_t)K, s, &cnt));
-  B2K_TRY(dalloc(ctx, b_psi, (size_t)K, s, &psi));
-  B2K_TRY(dalloc(ctx, b_shift, (size_t)d, s, &shift));
-  if (wg) {
-    B2K_TRY(dalloc(ctx, b_mz, (size_t)(K + 1) * d, s, &Mz));
-    B2K_TRY(dalloc(ctx, b_mperm, (size_t)k_pad, s, &mperm));
-    B2K_TRY(dalloc(ctx, b_psi32, (size_t)K, s, &psi32));
-    B2K_TRY(dalloc(ctx, b_hi, (size_t)k_pad * DP, s, &Xhi));
-    B2K_TRY(dalloc(ctx, b_lo, (size_t)k_pad * DP, s, &Xlo));
-    B2K_TRY(dalloc(ctx, b_cn, (size_t)k_pad, s, &cnorm));
-  } else {
-    B2K_TRY(dalloc(ctx, b_mu, (size_t)K * d, s, &mu));
-  }
-  k_sil_shift<<<(unsigned)d, 256, 0, s>>>(stat, (int)K, d, (double)n_total, shift);
-  B2K_CUDA_OK(ctx, cudaGetLastError());
-  k_sil_means<<<(unsigned)((std::max<int64_t>(k_pad, d) + 255) / 256), 256, 0, s>>>(stat, (int)K, d, shift, k_pad,
-                                                                                    cnt, mu, psi, Mz, mperm, psi32);
-  B2K_CUDA_OK(ctx, cudaGetLastError());
-  ctx->stats.kernel_launches += 2;
-  tm.mark(2, s);
-
-  // ---- silhouette pass ----
-  SilArgs a{};
-  a.n = n;
-  a.K = (int)K;
-  a.d = d;
-  a.X = X;
-  a.cid = md.cid;
-  a.nrm = md.nrm;
-  a.cnt = cnt;
-  a.shift = shift;
-  a.cnorm = cnorm;
-  a.psi32 = psi32;
-  a.mu = mu;
-  a.psi = psi;
-  int grid = 0;
-  if (wg) {
-    B2K_TRY(b2k_knn_prep_launch(ctx, Mz, K + 1, d, mperm, k_pad, DP, Xhi, Xlo, cnorm, s));
-    a.ntiles = (int)((n + PW_TM - 1) / PW_TM);
-    a.nblk = (int)(k_pad / PW_N);
-    grid = std::min(sm, a.ntiles);
-  } else {
-    a.ntiles = (int)((n + GR - 1) / GR);
-    grid = (int)std::min<int64_t>(a.ntiles, (int64_t)sm * (ctx->grid_limit > 0 ? 1 : 8));
-  }
-  B2K_TRY(dalloc(ctx, b_part, (size_t)std::max(grid, 1), s, &part));
-  B2K_TRY(dalloc(ctx, b_sum, 2, s, &sum));
-  a.part = part;
-  if (grid > 0) {
-    if (wg) {
-      PairWgMaps maps;
-      B2K_TRY(pair_wg_maps(ctx, X, n, d, Xhi, Xlo, k_pad, DP, &maps));
-      if (cosine)
-        B2K_TRY(pair_wg_launch<SIL_OWN>(
-            ctx, DP, [](auto nch) { return k_sil_wg<decltype(nch)::value, true>; }, grid, maps, a, s));
-      else
-        B2K_TRY(pair_wg_launch<SIL_OWN>(
-            ctx, DP, [](auto nch) { return k_sil_wg<decltype(nch)::value, false>; }, grid, maps, a, s));
-      ctx->stats.fused_tc_launches++;
-    } else {
-      if (cosine) k_sil_generic<true><<<(unsigned)grid, G_NT, 0, s>>>(a);
-      else k_sil_generic<false><<<(unsigned)grid, G_NT, 0, s>>>(a);
-      B2K_CUDA_OK(ctx, cudaGetLastError());
-      ctx->stats.generic_launches++;
-    }
-    ctx->stats.kernel_launches++;
-    B2K_TRY(b2k_launch_fold_f64(ctx, part, grid, sum, s));
-  } else {
-    B2K_CUDA_OK(ctx, cudaMemsetAsync(sum, 0, sizeof(double), s));
-  }
-  ctx->stats.last_path = wg ? B2K_PATH_FUSED : B2K_PATH_GENERIC;
-  const double nd = (double)n;
-  B2K_CUDA_OK(ctx, cudaMemcpyAsync(sum + 1, &nd, sizeof(double), cudaMemcpyHostToDevice, s));
-  tm.mark(3, s);
-  B2K_TRY(b2k_comm_allreduce_f64(ctx, sum, 2, s));
-  double res[2] = {0.0, 0.0};
-  B2K_CUDA_OK(ctx, cudaMemcpyAsync(res, sum, sizeof(res), cudaMemcpyDeviceToHost, s));
-  tm.mark(4, s);
-  B2K_CUDA_OK(ctx, cudaStreamSynchronize(s));
-  *out = res[0] / res[1];
-  if (tm.on) {
-    ctx->stats.last_finalize_ms = tm.ms(0, 1);   // cluster ids
-    ctx->stats.last_reduce_ms = tm.ms(1, 2);     // statistics, their allreduce, means
-    ctx->stats.last_fused_ms = tm.ms(2, 3);      // silhouette pass (with the means' planes)
-    ctx->stats.last_allreduce_ms = tm.ms(3, 4);  // [sum s | n]
-    ctx->stats.last_loop_ms = tm.ms(0, 4);
-  }
-  return B2K_OK;
-}
-
-int b2k_silhouette_multi_impl(b2k_ctx* ctx, const float* X, int64_t n_local, int d, int n_models,
-                              const int64_t* const* ids, int metric, double* out, cudaStream_t s) {
+int b2k_silhouette_impl(b2k_ctx* ctx, const float* X, int64_t n_local, int d, int n_models, const int64_t* const* ids,
+                        int metric, double* out, int* failed_model, cudaStream_t s) {
   const bool on = ctx->time_kernels != 0;
   const bool cosine = metric == 1;
   const int64_t n = n_local;
@@ -1003,7 +699,7 @@ int b2k_silhouette_multi_impl(b2k_ctx* ctx, const float* X, int64_t n_local, int
   B2kTimer tall(on);
   tall.mark(0, s);
 
-  // ---- per model: ids, statistics and the shift m, exactly as b2k_silhouette forms them ----
+  // ---- per model: ids, statistics and the shift m ----
   std::vector<SilModel> md(M);
   std::vector<DevBuf> b_shift(M);
   std::vector<float*> shift(M, nullptr);
@@ -1011,7 +707,10 @@ int b2k_silhouette_multi_impl(b2k_ctx* ctx, const float* X, int64_t n_local, int
   for (int m = 0; m < M; ++m) {
     B2kTimer tm(on);
     const int rc = sil_prepare(ctx, X, n, d, ids[m], metric, tm, md[m], s);
-    if (rc != B2K_OK) return b2k_fail(ctx, rc, "model " + std::to_string(m) + ": " + ctx->err);
+    if (rc != B2K_OK) {
+      if (failed_model != nullptr) *failed_model = m;
+      return rc;
+    }
     B2K_TRY(dalloc(ctx, b_shift[m], (size_t)d, s, &shift[m]));
     k_sil_shift<<<(unsigned)d, 256, 0, s>>>(md[m].stat, (int)md[m].K, d, (double)md[m].n_total, shift[m]);
     B2K_CUDA_OK(ctx, cudaGetLastError());
@@ -1075,19 +774,17 @@ int b2k_silhouette_multi_impl(b2k_ctx* ctx, const float* X, int64_t n_local, int
     } else {
       B2K_TRY(dalloc(ctx, b_mu, (size_t)Kt * d, s, &mu));
     }
-    // Model j's means go to Mz rows off[j] + 1 ..; k_sil_means also zeroes the row before them (its own zero row),
-    // which is model j - 1's last mean: running the models last to first rewrites that row after it was zeroed.
-    for (size_t jj = g.size(); jj-- > 0;) {
-      const SilModel& mj = md[g[jj]];
-      const int64_t o = off[jj];
-      k_sil_means<<<(unsigned)((std::max<int64_t>(mj.K, d) + 255) / 256), 256, 0, s>>>(
-          mj.stat, (int)mj.K, d, shift[g[jj]], 0, cnt + o, mu != nullptr ? mu + o * d : nullptr, psi + o,
-          Mz != nullptr ? Mz + o * d : nullptr, nullptr, psi32 != nullptr ? psi32 + o : nullptr);
+    for (size_t j = 0; j < g.size(); ++j) {   // model j's means go to Mz rows off[j] + 1 ..
+      const SilModel& mj = md[g[j]];
+      const int64_t o = off[j];
+      k_sil_means<<<(unsigned)((mj.K + 255) / 256), 256, 0, s>>>(
+          mj.stat, (int)mj.K, d, shift[g[j]], cnt + o, mu != nullptr ? mu + o * d : nullptr, psi + o,
+          Mz != nullptr ? Mz + (o + 1) * d : nullptr, psi32 != nullptr ? psi32 + o : nullptr);
       B2K_CUDA_OK(ctx, cudaGetLastError());
       ctx->stats.kernel_launches++;
     }
     if (wg) {
-      k_sil_mperm<<<(unsigned)((k_pad + 255) / 256), 256, 0, s>>>((int)Kt, k_pad, mperm);
+      k_sil_mperm<<<(unsigned)((std::max<int64_t>(k_pad, d) + 255) / 256), 256, 0, s>>>((int)Kt, k_pad, d, Mz, mperm);
       B2K_CUDA_OK(ctx, cudaGetLastError());
       ctx->stats.kernel_launches++;
     }
@@ -1100,7 +797,7 @@ int b2k_silhouette_multi_impl(b2k_ctx* ctx, const float* X, int64_t n_local, int
     }
     for (size_t c0 = 0; c0 < g.size(); c0 += SIL_MC) {
       const int nm = (int)std::min<size_t>(SIL_MC, g.size() - c0);
-      SilMultiArgs a{};
+      SilArgs a{};
       a.n = n;
       a.ntiles = (int)ntiles;
       a.d = d;
@@ -1121,16 +818,16 @@ int b2k_silhouette_multi_impl(b2k_ctx* ctx, const float* X, int64_t n_local, int
       if (grid > 0) {
         if (wg) {
           if (cosine)
-            B2K_TRY(pair_wg_launch<SILM_OWN>(
-                ctx, DP, [](auto nch) { return k_sil_wg_multi<decltype(nch)::value, true>; }, grid, maps, a, s));
+            B2K_TRY(pair_wg_launch<SIL_OWN>(
+                ctx, DP, [](auto nch) { return k_sil_wg<decltype(nch)::value, true>; }, grid, maps, a, s));
           else
-            B2K_TRY(pair_wg_launch<SILM_OWN>(
-                ctx, DP, [](auto nch) { return k_sil_wg_multi<decltype(nch)::value, false>; }, grid, maps, a, s));
+            B2K_TRY(pair_wg_launch<SIL_OWN>(
+                ctx, DP, [](auto nch) { return k_sil_wg<decltype(nch)::value, false>; }, grid, maps, a, s));
           ctx->stats.fused_tc_launches++;
         } else {
-          const auto k = cosine ? k_sil_generic_multi<true> : k_sil_generic_multi<false>;
-          B2K_CUDA_OK(ctx, cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, SILM_GEN_SMEM));
-          k<<<(unsigned)grid, G_NT, SILM_GEN_SMEM, s>>>(a);
+          const auto k = cosine ? k_sil_generic<true> : k_sil_generic<false>;
+          B2K_CUDA_OK(ctx, cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, SIL_GEN_SMEM));
+          k<<<(unsigned)grid, G_NT, SIL_GEN_SMEM, s>>>(a);
           B2K_CUDA_OK(ctx, cudaGetLastError());
           ctx->stats.generic_launches++;
         }
@@ -1149,7 +846,7 @@ int b2k_silhouette_multi_impl(b2k_ctx* ctx, const float* X, int64_t n_local, int
   }
   ctx->stats.last_path = wg ? B2K_PATH_FUSED : B2K_PATH_GENERIC;
 
-  // ---- one [sum s | n] allreduce per model, as b2k_silhouette does ----
+  // ---- one [sum s | n] allreduce per model ----
   B2kTimer tr(on);
   tr.mark(0, s);
   const double nd = (double)n;
