@@ -32,6 +32,11 @@
  *   b2k_logreg_minimize         cuML's qn solver (L-BFGS / OWL-QN) itself
  *   b2k_logreg_fit              classification.py:984-1171 (LogisticRegressionMG.fit per param map, rescaling, centring)
  *   b2k_logreg_predict          classification.py:1455-1553 (LogisticRegressionModel's transform)
+ *   b2k_ingest_csr_append       core.py:193-264, 507-521 (_read_csr_matrix_from_unwrapped_spark_vec: Spark vector rows
+ *                               -> a per-partition scipy CSR matrix, the default with enable_sparse_data_optim=None)
+ *   b2k_logreg_eval_csr         one evaluation of cuML's qn solver on the CSR input of classification.py:1038-1060
+ *   b2k_logreg_fit_csr          classification.py:998-1171 with the CSR matrix (LogisticRegressionMG.fit on sparse rows)
+ *   b2k_logreg_predict_csr      classification.py:1455-1553 on sparse rows (cuML predict on a CSR matrix)
  *   b2k_dbscan_fit              clustering.py:1049-1186 (DBSCANModel's fit function: cuML DBSCANMG(handle).fit_predict
  *                               over NCCL + UCX, labels gathered on rank 0)
  *   b2k_rf_fit / b2k_rf_forest  tree.py:343-527 (the per-worker cuML RandomForest fits and the treelite models they
@@ -192,6 +197,23 @@ int b2k_comm_abort(b2k_ctx* ctx); /* callable after a CUDA/NCCL error; never blo
 int b2k_ingest_append(b2k_ctx* ctx, float* dst, int64_t n_max, int d, int64_t row0, const void* values,
                       const int32_t* offsets, int64_t n_b, int src_dtype, int layout, uintptr_t stream,
                       int64_t* rows_written);
+
+/* ---- sparse ingest (stands in for core.py:193-264, 507-521, the reference's CSR build from Spark vectors): one Arrow
+ * batch of a Spark VectorUDT column (struct<type: tinyint, size: int, indices: array<int>, values: array<double>>),
+ * given by its child buffers, appended as rows [row0, row0 + n_b) and entries [nnz0, nnz0 + nnz_b) of a device CSR
+ * (indptr int64 [n_max + 1], indices int32 and values f32 [nnz_max]).  type [n_b] int8 (0 sparse, 1 dense), size [n_b]
+ * int32 (read for sparse rows only), idx_offsets / val_offsets [n_b + 1] int32 and their child buffers idx_values int32
+ * and val_values (B2K_F64 or B2K_F32, rounded to f32); offsets index the whole child buffers, as Arrow's do.  A dense
+ * row becomes the entries 0 .. d - 1; stored zeros stay entries.  indptr[row0 + i + 1] is written for each row; the
+ * caller sets indptr[0] = 0.  Errors (B2K_ERR_INVALID), as the dense ingest checks row widths: a sparse row's size or a
+ * dense row's length other than d, a sparse row whose index count differs from its value count, a type other than
+ * 0 / 1; these fail on the ingesting rank only.  Index range, order and finiteness are checked on the device by the
+ * calls that read the rows.  Stages through the pinned buffers of
+ * b2k_ingest_append; *nnz_written = nnz_b.  Ordered on `stream`. ---- */
+int b2k_ingest_csr_append(b2k_ctx* ctx, int64_t* indptr, int32_t* indices, float* values, int64_t n_max,
+                          int64_t nnz_max, int64_t d, int64_t row0, int64_t nnz0, const int8_t* type, const int32_t* size,
+                          const int32_t* idx_offsets, const int32_t* idx_values, const int32_t* val_offsets,
+                          const void* val_values, int val_dtype, int64_t n_b, uintptr_t stream, int64_t* nnz_written);
 
 /* ---- fit: init + Lloyd loop + (optional) inertia against the final centers.
  *   X              device f32 [n_local, d] row-major (this rank's partition)
@@ -424,6 +446,44 @@ int b2k_logreg_fit(b2k_ctx* ctx, const float* X, const float* y, int64_t n_local
 int b2k_logreg_predict(b2k_ctx* ctx, const float* X, int64_t n, int d, int kp, const double* W, const double* b,
                        const double* class_values, double* raw_out, double* prob_out, double* pred_out,
                        uintptr_t stream);
+
+/* ---- sparse logistic regression: the objective, classes, label rules, optimiser, stopping rules, start and centring of
+ * b2k_logreg_fit, over rows in CSR: indptr [n_local + 1] int64 (indptr[0] = 0, indptr[n_local] = nnz_local), indices
+ * [nnz] int32, values [nnz] f32 (device); y [n_local] f32.  sigma counts the implicit zeros (sample deviations over all n
+ * rows); standardization scales and never centres, so a CSR fit and a dense fit of the same matrix solve the same
+ * problem and differ only by summation order.  All arithmetic fp64.  Caps (B2K_ERR_UNSUPPORTED): d < 2^31 and
+ * kp (d + 1) <= 2^25 (the host L-BFGS state holds about 20 vectors of that length).  Collective errors (every rank fails
+ * together, B2K_ERR_INVALID): an empty partition; "sparse features: an index is out of bounds for vectors of size d";
+ * "sparse features: the indices of a row must be strictly increasing"; "logistic regression: the features hold a NaN
+ * or an infinity".  The CSC copy is built once per call: rows are split into chunks whose residuals R [rows][kp] fp64
+ * stay under 256 MB, each chunk sorted by column with a stable radix sort.  One evaluation = per chunk a rows pass
+ * (margins, residuals, loss) and a CSC pass over fixed ranges of entries (columns cut at range boundaries are carried
+ * and folded in range order), then one f64 allreduce.  No floating-point atomics: bitwise reproducible for the same
+ * input, rank count, device and option "grid_limit" (which caps the rows pass's CTAs).  stats.generic_launches counts
+ * the evaluations (+1 each, whatever the number of row chunks).  With "time_kernels":
+ * last_fused_ms = the rows passes, last_reduce_ms = the CSC passes, last_allreduce_ms = the allreduce and read-back of
+ * the last evaluation; last_finalize_ms = the CSC build, last_probe_ms = the moments pass (fit), last_loop_ms = the whole
+ * fit.  Synchronise `stream`.
+ *
+ * b2k_logreg_eval_csr (collective) stands in for one evaluation of cuML's qn solver on the reference's CSR input
+ * (classification.py:1038-1060): outputs as b2k_logreg_eval (grad_out [kp][d + 1]); builds its own CSC (for tests and
+ * diagnostics).  b2k_logreg_fit_csr (collective) stands in for classification.py:998-1171 on sparse rows: outputs as
+ * b2k_logreg_fit; the CSC, the validation and the moments pass (sum x and nnz per column, one allreduce, then
+ * sum over the entries of (x - mu)^2 plus (n - nnz) mu^2, a second allreduce) serve all n_fits settings. */
+int b2k_logreg_eval_csr(b2k_ctx* ctx, const int64_t* indptr, const int32_t* indices, const float* values,
+                        int64_t n_local, int64_t nnz_local, int64_t d, const float* y, const double* classes,
+                        int n_classes, int kp, const double* W, const double* b, double* loss_out, double* grad_out,
+                        int64_t* n_total_out, uintptr_t stream);
+int b2k_logreg_fit_csr(b2k_ctx* ctx, const int64_t* indptr, const int32_t* indices, const float* values,
+                       int64_t n_local, int64_t nnz_local, int64_t d, const float* y, const double* classes,
+                       const int64_t* counts, int n_classes, int n_fits, const b2k_logreg_params* params,
+                       double* coef_out, double* intercept_out, int* kp_out, int* n_iter_out, uintptr_t stream);
+/* b2k_logreg_predict_csr stands in for classification.py:1455-1553 on sparse rows: the outputs of b2k_logreg_predict
+ * (W device f64 [kp][d], b, class_values as there) for n CSR rows, margins summed in fp64 by the rows pass's code.  The
+ * caps and the index / order / finiteness checks above apply (not collective).  Synchronises `stream` when it checks. */
+int b2k_logreg_predict_csr(b2k_ctx* ctx, const int64_t* indptr, const int32_t* indices, const float* values, int64_t n,
+                           int64_t nnz, int64_t d, int kp, const double* W, const double* b, const double* class_values,
+                           double* raw_out, double* prob_out, double* pred_out, uintptr_t stream);
 
 /* ---- DBSCAN (euclidean or cosine) ----
  * Stands in for clustering.py:1049-1186 (DBSCANModel's fit function: cuML DBSCANMG.fit_predict).  Semantics, with the

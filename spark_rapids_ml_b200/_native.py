@@ -64,6 +64,10 @@ EXPORTED_SYMBOLS = (
     "b2k_logreg_minimize",
     "b2k_logreg_fit",
     "b2k_logreg_predict",
+    "b2k_ingest_csr_append",
+    "b2k_logreg_eval_csr",
+    "b2k_logreg_fit_csr",
+    "b2k_logreg_predict_csr",
     "b2k_dbscan_fit",
     "b2k_rf_fit",
     "b2k_rf_forest",
@@ -241,6 +245,13 @@ def load_library() -> ctypes.CDLL:
     L.b2k_logreg_fit.argtypes = [vp, vp, vp, i64, i32, vp, vp, i32, i32, ctypes.POINTER(LogregParams), vp, vp, vp, vp,
                                  ctypes.c_size_t]
     L.b2k_logreg_predict.argtypes = [vp, vp, i64, i32, i32, vp, vp, vp, vp, vp, vp, ctypes.c_size_t]
+    L.b2k_ingest_csr_append.argtypes = [vp, vp, vp, vp, i64, i64, i64, i64, i64, vp, vp, vp, vp, vp, vp, i32, i64,
+                                        ctypes.c_size_t, ctypes.POINTER(i64)]
+    L.b2k_logreg_eval_csr.argtypes = [vp, vp, vp, vp, i64, i64, i64, vp, vp, i32, i32, vp, vp, ctypes.POINTER(f64), vp,
+                                      ctypes.POINTER(i64), ctypes.c_size_t]
+    L.b2k_logreg_fit_csr.argtypes = [vp, vp, vp, vp, i64, i64, i64, vp, vp, vp, i32, i32, ctypes.POINTER(LogregParams),
+                                     vp, vp, vp, vp, ctypes.c_size_t]
+    L.b2k_logreg_predict_csr.argtypes = [vp, vp, vp, vp, i64, i64, i64, i32, vp, vp, vp, vp, vp, vp, ctypes.c_size_t]
     L.b2k_dbscan_fit.argtypes = [vp, vp, i64, i32, f64, i32, i32, vp, vp, ctypes.POINTER(i64), ctypes.c_size_t]
     L.b2k_rf_fit.argtypes = [vp, vp, vp, i64, i32, ctypes.POINTER(RfParams), ctypes.POINTER(i32), ctypes.POINTER(i64),
                              vp, vp, ctypes.c_size_t]
@@ -764,6 +775,106 @@ class Context:
             self._check(self._L.b2k_logreg_predict(self._h, X.data_ptr(), n, d, kp, Wd.data_ptr(), bd.data_ptr(),
                                                    cv.data_ptr(), raw.data_ptr(), prob.data_ptr(), pred.data_ptr(),
                                                    self._stream()))
+        t.cuda.current_stream(self.device).synchronize()  # Wd, bd, cv (temporaries) must outlive the kernel
+        return raw, prob, pred
+
+    # -- sparse logistic regression: rows as a device CSR (indptr int64 [n + 1], indices int32, values float32) --------
+    def ingest_csr(self, indptr: Any, indices: Any, values: Any, d: int, row0: int, nnz0: int, type_: np.ndarray,
+                   size: np.ndarray, idx_offsets: np.ndarray, idx_values: np.ndarray, val_offsets: np.ndarray,
+                   val_values: np.ndarray) -> int:
+        """Append one batch of Spark vector rows, given by the Arrow child buffers of its struct column, at rows
+        [row0, row0 + n_b) and entries [nnz0, ...) of the device CSR -> the batch's entry count."""
+        code = _DTYPE_CODES.get(val_values.dtype)
+        if code not in (0, 1):
+            raise TypeError(f"unsupported vector value dtype {val_values.dtype}")
+        arrs = [np.ascontiguousarray(type_, dtype=np.int8), np.ascontiguousarray(size, dtype=np.int32),
+                np.ascontiguousarray(idx_offsets, dtype=np.int32), np.ascontiguousarray(idx_values, dtype=np.int32),
+                np.ascontiguousarray(val_offsets, dtype=np.int32), np.ascontiguousarray(val_values)]
+        wrote = ctypes.c_int64(0)
+        self._check(self._L.b2k_ingest_csr_append(
+            self._h, indptr.data_ptr(), indices.data_ptr(), values.data_ptr(), int(indptr.shape[0]) - 1,
+            int(indices.shape[0]), int(d), int(row0), int(nnz0), *[a.ctypes.data for a in arrs], code,
+            int(arrs[0].shape[0]), self._stream(), ctypes.byref(wrote)))
+        return int(wrote.value)
+
+    def _check_csr(self, X: Any, d: int) -> Tuple[int, int]:
+        t = self._torch
+        indptr, indices, values = X
+        ok = (indptr.dtype == t.int64 and indices.dtype == t.int32 and values.dtype == t.float32 and
+              all(a.is_cuda and a.dim() == 1 and a.is_contiguous() and a.device.index == self.device_index
+                  for a in X) and indices.shape == values.shape and indptr.shape[0] >= 1)
+        if not ok:
+            raise ValueError("X must be a CSR triple of contiguous CUDA tensors on this device: indptr int64 [n + 1], "
+                             "indices int32 [nnz], values float32 [nnz]")
+        if int(d) < 1:
+            raise ValueError("d must be >= 1")
+        return int(indptr.shape[0]) - 1, int(indices.shape[0])
+
+    def logreg_eval_csr(self, X: Any, d: int, y: Any, classes: Sequence[float], W: np.ndarray, b: np.ndarray
+                        ) -> Tuple[float, np.ndarray, np.ndarray, int]:
+        """logreg_eval on CSR rows X = (indptr, indices, values) of width d (collective; builds its own CSC)."""
+        n, nnz = self._check_csr(X, d)
+        self._check_y(y, n)
+        cls = np.ascontiguousarray(classes, dtype=np.float64)
+        W = np.ascontiguousarray(W, dtype=np.float64)
+        kp = int(W.shape[0])
+        b = np.ascontiguousarray(b, dtype=np.float64)
+        if W.shape != (kp, d) or b.shape != (kp,):
+            raise ValueError(f"W must be [kp, {d}] and b [kp]")
+        loss = ctypes.c_double(0.0)
+        grad = np.zeros((kp, d + 1), dtype=np.float64)
+        nt = ctypes.c_int64(0)
+        with self._torch.cuda.device(self.device):
+            self._check(self._L.b2k_logreg_eval_csr(self._h, *[a.data_ptr() for a in X], n, nnz, int(d), y.data_ptr(),
+                                                    cls.ctypes.data, int(cls.size), kp, W.ctypes.data, b.ctypes.data,
+                                                    ctypes.byref(loss), grad.ctypes.data, ctypes.byref(nt),
+                                                    self._stream()))
+        return float(loss.value), grad[:, :d].copy(), grad[:, d].copy(), int(nt.value)
+
+    def logreg_fit_csr(self, X: Any, d: int, y: Any, classes: np.ndarray, counts: np.ndarray,
+                       settings: Sequence[Dict[str, Any]]) -> List[Tuple[np.ndarray, np.ndarray, int]]:
+        """logreg_fit on CSR rows X = (indptr, indices, values) of width d: one CSC and one moments pass for every
+        setting (collective)."""
+        n, nnz = self._check_csr(X, d)
+        self._check_y(y, n)
+        cls = np.ascontiguousarray(classes, dtype=np.float64)
+        cnt = np.ascontiguousarray(counts, dtype=np.int64)
+        K, m = int(cls.size), len(settings)
+        prm = (LogregParams * m)(*[LogregParams(float(s["reg"]), float(s["l1_ratio"]), float(s["tol"]),
+                                                int(s["max_iter"]), int(bool(s["fit_intercept"])),
+                                                int(bool(s["standardization"])), FAMILY_CODES[s["family"]])
+                                   for s in settings])
+        coef = np.zeros((m, K, d), dtype=np.float64)
+        icpt = np.zeros((m, K), dtype=np.float64)
+        kp = np.zeros(m, dtype=np.int32)
+        it = np.zeros(m, dtype=np.int32)
+        with self._torch.cuda.device(self.device):
+            self._check(self._L.b2k_logreg_fit_csr(self._h, *[a.data_ptr() for a in X], n, nnz, int(d), y.data_ptr(),
+                                                   cls.ctypes.data, cnt.ctypes.data, K, m, prm, coef.ctypes.data,
+                                                   icpt.ctypes.data, kp.ctypes.data, it.ctypes.data, self._stream()))
+        return [(coef[f, : kp[f]].copy(), icpt[f, : kp[f]].copy(), int(it[f])) for f in range(m)]
+
+    def logreg_predict_csr(self, X: Any, d: int, W: Any, b: Any, class_values: Sequence[float]
+                           ) -> Tuple[Any, Any, Any]:
+        """logreg_predict on CSR rows X = (indptr, indices, values) of width d."""
+        t = self._torch
+        n, nnz = self._check_csr(X, d)
+        Wd = t.as_tensor(np.ascontiguousarray(W, dtype=np.float64), device=self.device).contiguous()
+        bd = t.as_tensor(np.ascontiguousarray(b, dtype=np.float64), device=self.device).contiguous()
+        kp = int(Wd.shape[0])
+        if tuple(Wd.shape) != (kp, d) or tuple(bd.shape) != (kp,):
+            raise ValueError(f"W must be [kp, {d}] and b [kp]")
+        nout = 2 if kp == 1 else kp
+        cv = t.as_tensor(np.ascontiguousarray(class_values, dtype=np.float64), device=self.device).contiguous()
+        if tuple(cv.shape) != (nout,):
+            raise ValueError(f"class_values must be [{nout}]")
+        raw = t.empty((n, nout), dtype=t.float64, device=self.device)
+        prob = t.empty((n, nout), dtype=t.float64, device=self.device)
+        pred = t.empty((n,), dtype=t.float64, device=self.device)
+        with t.cuda.device(self.device):
+            self._check(self._L.b2k_logreg_predict_csr(self._h, *[a.data_ptr() for a in X], n, nnz, int(d), kp,
+                                                       Wd.data_ptr(), bd.data_ptr(), cv.data_ptr(), raw.data_ptr(),
+                                                       prob.data_ptr(), pred.data_ptr(), self._stream()))
         t.cuda.current_stream(self.device).synchronize()  # Wd, bd, cv (temporaries) must outlive the kernel
         return raw, prob, pred
 

@@ -18,7 +18,16 @@ Differences that are deliberate: with regParam = 0 a multinomial fit centres its
 does (the reference reports wherever its solver stopped on a problem without a unique solution); the classes are the
 sorted distinct label values and the prediction is the class value, not its index; labels must be below 1024.  No CPU
 fallback: cpu(), predict(), predictRaw(), predictProbability() and evaluate() raise NotImplementedError; weightCol,
-threshold(s), the coefficient / intercept bounds and sparse input raise ValueError; there is no training summary.
+threshold(s), the coefficient / intercept bounds and enable_sparse_data_optim=True raise ValueError; there is no
+training summary.
+
+Sparse input (DESIGN §21): a local frame whose features are Spark vectors in their SQL layout, struct<type: tinyint,
+size: int, indices: array<int>, values: array<double>>, sparse and dense rows mixed.  With enable_sparse_data_optim=None
+(the default) and a sparse first row, the rows stay sparse: one device CSR per partition, a CSC copy built once per fit,
+and every evaluation is a rows pass and a column pass over the stored entries, so d may reach 2^25 / K' - 1 (K' = 1
+for a binomial fit, numClasses for a multinomial one: K' (d + 1) <= 2^25).  Otherwise (a dense first row, or enable_sparse_data_optim=False) the rows are densified
+into the dense path.  Both solve the same problem.  transform() of a vector struct column runs the CSR predict, for a
+model fitted either way; CrossValidator and _transformEvaluate of such a frame raise NotImplementedError.
 """
 from __future__ import annotations
 
@@ -32,6 +41,7 @@ from .params import HasFeaturesCol, HasFeaturesCols, HasLabelCol, HasPredictionC
 from .regression import _ModelIterator
 from .tree import _RandomForestEstimator, _RandomForestModel
 from .sparkshim import LocalDataFrame, Param, Row, TypeConverters, keyword_only
+from .utils import densify_vector_column, is_vector_struct
 
 
 class LogisticRegressionClass(_CumlClass):
@@ -238,8 +248,10 @@ class LogisticRegression(LogisticRegressionClass, _CumlEstimator, _LogisticRegre
         self._set_cuml_reg_params()
         self._input_kwargs.pop("kwargs", None)
         self._input_kwargs.update(kwargs)
-        if self._input_kwargs.pop("enable_sparse_data_optim", None):
-            raise ValueError("sparse input is not supported by spark_rapids_ml_b200's LogisticRegression")
+        self._sparse_data_optim = self._input_kwargs.pop("enable_sparse_data_optim", None)
+        if self._sparse_data_optim:
+            raise ValueError("enable_sparse_data_optim=True is not supported by spark_rapids_ml_b200's "
+                             "LogisticRegression; leave it at None (the default) to fit sparse vectors as CSR")
         if self._input_kwargs.get("num_workers", None) is None:
             self._input_kwargs.pop("num_workers", None)
         self._set_params(**self._input_kwargs)
@@ -294,9 +306,38 @@ class LogisticRegression(LogisticRegressionClass, _CumlEstimator, _LogisticRegre
         label = self.getLabelCol()
         if label not in dataset.columns:
             raise ValueError(f"label column '{label}' not found in {dataset.columns}")
-        df, multi_col_names, dimension, ftype = super()._pre_process_data(dataset)
+        vec = _vector_column(dataset, self.getFeaturesCol())
+        if vec is not None:
+            df, dimension, ftype = self._pre_process_vectors(dataset, vec)
+            multi_col_names = None
+        else:
+            df, multi_col_names, dimension, ftype = super()._pre_process_data(dataset)
         df = df.with_appended_column(alias.label, [[b.column(label).cast(pa.float32()) for b in p] for p in dataset._parts])
         return df, multi_col_names, dimension, ftype
+
+    def _pre_process_vectors(self, dataset: LocalDataFrame, col: str) -> Tuple[LocalDataFrame, int, str]:
+        """A vector struct column: kept as vectors for the CSR path ("csr") when enable_sparse_data_optim is None and
+        the first row is sparse, else densified to array<float> (the reference's rule, core.py:507-521)."""
+        df = dataset.select(col).withColumnRenamed(col, alias.data)
+        first = df.first()
+        if first is None:
+            raise RuntimeError("A python worker received no data.  Please increase amount of data or use fewer workers.")
+        v = first[alias.data]
+        if v is None:
+            raise ValueError("null feature rows are not supported")
+        sparse = v["type"] == 0
+        dimension = int(v["size"]) if sparse else len(v["values"])
+        if getattr(self, "_sparse_data_optim", None) is None and sparse:
+            return df, dimension, "csr"
+        parts = [[pa.RecordBatch.from_arrays([densify_vector_column(b.column(0), dimension)], names=[alias.data])
+                  for b in p] for p in df._parts]
+        return df._derive(parts, pa.schema([pa.field(alias.data, pa.list_(pa.float32()))])), dimension, "float"
+
+    def _check_tuning_input(self, dataset: Any) -> None:
+        """CrossValidator's single-pass evaluation reads dense rows: a vector struct frame is refused before any fit."""
+        if isinstance(dataset, LocalDataFrame) and _vector_column(dataset, self.getFeaturesCol()) is not None:
+            raise NotImplementedError("CrossValidator of LogisticRegression on sparse input (a vector struct features "
+                                      "column) is not supported: the single-pass evaluation kernels read dense rows")
 
     def _get_cuml_fit_func(self, dataset: Any, extra_params: Optional[List[Dict[str, Any]]] = None
                            ) -> Callable[[FitInputType, Dict[str, Any]], Dict[str, Any]]:
@@ -310,7 +351,10 @@ class LogisticRegression(LogisticRegressionClass, _CumlEstimator, _LogisticRegre
                 raise RuntimeError("the worker scaffold hands the fit function ONE device matrix per partition")
             X, y, _ = dfs[0]
             classes, counts, _n = ctx.logreg_labels(y)
-            fits = ctx.logreg_fit(X, y, classes, counts, grid)
+            if isinstance(X, tuple):   # the device CSR (indptr, indices, values) of a sparse frame
+                fits = ctx.logreg_fit_csr(X, params[param_alias.num_cols], y, classes, counts, grid)
+            else:
+                fits = ctx.logreg_fit(X, y, classes, counts, grid)
             out: Dict[str, List[Any]] = {"coef_": [], "intercept_": [], "classes_": [], "n_cols": [], "dtype": [],
                                          "num_iters": []}
             for coef, icpt, iters in fits:
@@ -522,13 +566,33 @@ class LogisticRegressionModel(LogisticRegressionClass, _CumlModelWithPredictionC
             return _DeviceModel, None, _evaluate  # type: ignore[return-value]
         W, b, cls = self._device_model()
         class_values = cls[:max(2, W.shape[0])]
-        transform = self._grouped_transform(lambda m, X: m.ctx.logreg_predict(X, W, b, class_values),
-                                            4 * int(self.n_cols) + 8 * (2 * max(2, W.shape[0]) + 1))
+        out_bytes = 8 * (2 * max(2, W.shape[0]) + 1)
+        if isinstance(dataset, LocalDataFrame) and _vector_column(dataset, self.getFeaturesCol()) is not None:
+            d = int(self.n_cols)
+            transform = self._grouped_transform(lambda m, X: m.ctx.logreg_predict_csr(X, d, W, b, class_values),
+                                                8 + out_bytes, sparse=True)
+        else:
+            transform = self._grouped_transform(lambda m, X: m.ctx.logreg_predict(X, W, b, class_values),
+                                                4 * int(self.n_cols) + out_bytes)
         return _DeviceModel, transform, None
+
+    def _transformEvaluate(self, dataset: Any, evaluator: Any, params: Optional[Dict[Any, Any]] = None) -> List[float]:
+        if isinstance(dataset, LocalDataFrame) and _vector_column(dataset, self.getFeaturesCol()) is not None:
+            raise NotImplementedError("LogisticRegressionModel._transformEvaluate() of sparse input (a vector struct "
+                                      "features column) is not supported: the single-pass evaluation kernels read "
+                                      "dense rows")
+        return super()._transformEvaluate(dataset, evaluator, params)
 
     def _transform_outputs(self) -> List[Tuple[str, str]]:
         return [(self.getRawPredictionCol(), "array<double>"), (self.getProbabilityCol(), "array<double>"),
                 (self.getOrDefault("predictionCol"), "double")]
+
+
+def _vector_column(dataset: LocalDataFrame, col: Any) -> Optional[str]:
+    """The features column when it is a single vector struct column of the frame, else None."""
+    if not isinstance(col, str) or dataset.schema is None or col not in dataset.columns:
+        return None
+    return col if is_vector_struct(dataset.schema.field(col).type) else None
 
 
 def _dense(values: Sequence[float]) -> Any:

@@ -34,7 +34,7 @@ import pyarrow as pa
 from .params import _CumlParams
 from .sparkshim import (HAVE_PYSPARK, BarrierTaskContext, EstimatorBase, LocalDataFrame, ModelBase, Params, Row,
                         get_session)
-from .utils import DeviceRowAppender, arrow_list_column_buffers, get_logger
+from .utils import DeviceCsrAppender, DeviceRowAppender, arrow_list_column_buffers, get_logger
 
 # same tags as the reference (core.py:128-175) so the worker-side column contract is recognisable
 Alias = namedtuple("Alias", ("featureVectorType", "featureVectorSize", "featureVectorIndices", "data", "label",
@@ -216,6 +216,24 @@ def _ingest(ctx: Any, frames: Iterable[Any], n_cols: int, rows: int) -> Any:
     return app.finish()
 
 
+def _ingest_csr(ctx: Any, frames: Iterable[Any], n_cols: int) -> Any:
+    """Every non-empty frame's vector struct column, in order, as the rows of one device CSR."""
+    app = DeviceCsrAppender(ctx, n_cols)
+    for f in frames:
+        if len(f):
+            app.append_column(f[alias.data])
+    return app.finish()
+
+
+def _vector_bytes(frame: Any) -> int:
+    """The device bytes of a frame's vector struct column as CSR entries: 12 per stored value."""
+    from .utils import _arrow_array
+
+    arr = _arrow_array(frame[alias.data])
+    offs = arr.flatten()[3].offsets
+    return 12 * (int(offs[-1].as_py()) - int(offs[0].as_py())) if len(arr) else 0
+
+
 class _GroupedTransform:
     """A model's transform function: a group of frames in one device pass.  Every non-empty frame is ingested into one
     device matrix, `predict(device_model, X)` returns one CUDA tensor per output type (the first dimension is the row),
@@ -224,11 +242,15 @@ class _GroupedTransform:
     bounds a group's size (TRANSFORM_GROUP_BYTES)."""
 
     def __init__(self, predict: Callable[[Any, Any], Sequence[Any]], n_cols: int, row_bytes: int,
-                 out_types: Sequence[str]) -> None:
+                 out_types: Sequence[str], sparse: bool = False) -> None:
         self.predict = predict
         self.n_cols = n_cols
         self.row_bytes = row_bytes
         self.out_types = list(out_types)
+        # sparse: the frames' features are a vector struct column, ingested as one device CSR (indptr, indices,
+        # values); `row_bytes` then counts the bytes per row of the outputs and groups are also capped by the entries'
+        # bytes (12 per stored entry)
+        self.sparse = sparse
 
     def __call__(self, model: Any, frames: List[Any]) -> List[Tuple[np.ndarray, ...]]:
         sizes = [len(f) for f in frames]
@@ -236,7 +258,8 @@ class _GroupedTransform:
         if total == 0:
             return [tuple(np.zeros((0, 0) if t.startswith("array<") else 0, _out_dtype(t)) for t in self.out_types)
                     for _ in frames]
-        host = [t.cpu().numpy() for t in self.predict(model, _ingest(model.ctx, frames, self.n_cols, total))]
+        X = _ingest_csr(model.ctx, frames, self.n_cols) if self.sparse else _ingest(model.ctx, frames, self.n_cols, total)
+        host = [t.cpu().numpy() for t in self.predict(model, X)]
         ends = np.cumsum(sizes)
         return [tuple(h[e - n:e] for h in host) for n, e in zip(sizes, ends)]
 
@@ -338,13 +361,15 @@ class _CumlCaller(_CumlParams, _CumlCommon):
             spark_df = spark_binding.is_spark_dataframe(dataset)
         num_workers = self.num_workers
         if spark_df:
-            df, multi_col_names, dimension, _ = spark_binding.pre_process_data(self, dataset, alias.data)
+            df, multi_col_names, dimension, ftype = spark_binding.pre_process_data(self, dataset, alias.data)
             is_local = spark_binding.is_local(dataset)
         else:
-            df, multi_col_names, dimension, _ = self._pre_process_data(dataset)
+            df, multi_col_names, dimension, ftype = self._pre_process_data(dataset)
             if df.getNumPartitions() != num_workers:
                 df = df.repartition(num_workers)   # core.py:771-772
             is_local = True   # the local frame runs on this host: partition id doubles as the GPU id (core.py:377-384)
+        # "csr": the features are Spark vectors kept sparse; the fit function gets the device CSR triple in slot 0
+        csr = ftype == "csr"
         params: Dict[str, Any] = {param_alias.cuml_init: dict(self.cuml_params), param_alias.fit_multiple_params: None}
         extra_cols = [c for c in (alias.label, alias.row_number) if c in df.columns]
         float_label = self._fit_label_col() is not None
@@ -368,12 +393,13 @@ class _CumlCaller(_CumlParams, _CumlCommon):
             gpu_id = _CumlCommon._set_gpu_device(context, is_local)
             logger.info("Loading data into device memory (b2k_ingest_append)")
             with CumlContext(partition_id, num_workers, context, enable_nccl, require_ucx, device=gpu_id) as cc:
-                appender = DeviceRowAppender(cc.handle, dimension)
+                appender = DeviceCsrAppender(cc.handle, dimension) if csr else DeviceRowAppender(cc.handle, dimension)
                 sizes: List[int] = []
                 # label / row-number columns the pre-processed frame carries (kneighbors): host arrays, per batch
                 extra: Dict[str, List[np.ndarray]] = {c: [] for c in extra_cols}
                 for pdf in pdf_iter:
-                    sizes.append(_features_from_pdf(pdf, multi_col_names, appender, logger))
+                    sizes.append(appender.append_column(pdf[alias.data]) if csr else
+                                 _features_from_pdf(pdf, multi_col_names, appender, logger))
                     for c in extra_cols:
                         if float_label and c == alias.label:
                             extra[c].append(np.asarray(pdf[c].to_numpy(), dtype=np.float32))
@@ -387,7 +413,7 @@ class _CumlCaller(_CumlParams, _CumlCommon):
                 if float_label:
                     import torch
 
-                    slots[0] = torch.from_numpy(slots[0]).to(X.device)
+                    slots[0] = torch.from_numpy(slots[0]).to(cc.handle.device)
                 inputs: FitInputType = [(X, slots[0], slots[1])]
                 params[param_alias.handle] = cc.handle
                 params[param_alias.part_sizes] = sizes
@@ -524,18 +550,22 @@ TRANSFORM_GROUP_ROWS = 1 << 20    # rows per device pass of transform and evalua
 TRANSFORM_GROUP_BYTES = 2 << 30   # ... and the cap on the device bytes they take (`row_bytes` per row)
 
 
-def _row_groups(items: Iterable[Any], row_bytes: int) -> Iterator[List[Any]]:
+def _row_groups(items: Iterable[Any], row_bytes: int,
+                extra_bytes: Optional[Callable[[Any], int]] = None) -> Iterator[List[Any]]:
     """Consecutive frames or batches, in order, in groups that end once they reach TRANSFORM_GROUP_ROWS rows or
-    TRANSFORM_GROUP_BYTES at `row_bytes` per row; the last group may be smaller."""
+    TRANSFORM_GROUP_BYTES at `row_bytes` per row (plus `extra_bytes(item)` per item when given); the last group may be
+    smaller."""
     limit = max(1, min(TRANSFORM_GROUP_ROWS, TRANSFORM_GROUP_BYTES // max(1, row_bytes)))
     group: List[Any] = []
-    rows = 0
+    rows = nbytes = 0
     for it in items:
         group.append(it)
         rows += len(it)
-        if rows >= limit:
+        if extra_bytes is not None:
+            nbytes += len(it) * row_bytes + extra_bytes(it)
+        if rows >= limit or nbytes >= TRANSFORM_GROUP_BYTES:
             yield group
-            group, rows = [], 0
+            group, rows, nbytes = [], 0, 0
     if group:
         yield group
 
@@ -543,7 +573,8 @@ def _row_groups(items: Iterable[Any], row_bytes: int) -> Iterator[List[Any]]:
 def _iter_transform(transform: Callable, model: Any, frames: Iterable[Any]) -> Iterator[Any]:
     """One result per input frame, in order: `transform` (a model's grouped transform function) takes each group of
     consecutive frames in one device pass."""
-    for group in _row_groups(frames, transform.row_bytes):
+    extra = _vector_bytes if getattr(transform, "sparse", False) else None
+    for group in _row_groups(frames, transform.row_bytes, extra):
         yield from transform(model, group)
 
 
@@ -908,10 +939,13 @@ class _CumlModelWithColumns(_CumlModel):
         transform function."""
         return [(self._output_col_name(), self._out_schema(None))]
 
-    def _grouped_transform(self, predict: Callable[[Any, Any], Sequence[Any]], row_bytes: int) -> _GroupedTransform:
+    def _grouped_transform(self, predict: Callable[[Any, Any], Sequence[Any]], row_bytes: int,
+                           sparse: bool = False) -> _GroupedTransform:
         """This model's grouped transform function: `predict(device_model, X)` returns one CUDA tensor per column of
-        _transform_outputs(); `row_bytes` is the device bytes a row takes."""
-        return _GroupedTransform(predict, int(self.n_cols), row_bytes, [t for _, t in self._transform_outputs()])
+        _transform_outputs(); `row_bytes` is the device bytes a row takes (sparse: X is a device CSR, see
+        _GroupedTransform)."""
+        return _GroupedTransform(predict, int(self.n_cols), row_bytes, [t for _, t in self._transform_outputs()],
+                                 sparse)
 
     def _transform(self, dataset: Any) -> Any:
         from .sparkshim.sql import _batches_to_pdf_iter

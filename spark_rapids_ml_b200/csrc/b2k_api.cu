@@ -1183,6 +1183,61 @@ extern "C" int b2k_logreg_predict(b2k_ctx* ctx, const float* X, int64_t n, int d
 }
 
 // ------------------------------------------------------------------------------------------------
+// sparse logistic regression (b2k_logreg_sparse.cu)
+// ------------------------------------------------------------------------------------------------
+static int check_csr(b2k_ctx* ctx, const char* who, const int64_t* indptr, const int32_t* indices, const float* values,
+                     int64_t n, int64_t nnz, int64_t d) {
+  if ((!indptr && n > 0) || ((!indices || !values) && nnz > 0) || n < 0 || nnz < 0 || d < 1)
+    return b2k_fail(ctx, B2K_ERR_INVALID, std::string(who) + ": bad indptr/indices/values/n/nnz/d");
+  return B2K_OK;
+}
+
+extern "C" int b2k_logreg_eval_csr(b2k_ctx* ctx, const int64_t* indptr, const int32_t* indices, const float* values,
+                                   int64_t n_local, int64_t nnz_local, int64_t d, const float* y, const double* classes,
+                                   int n_classes, int kp, const double* W, const double* b, double* loss_out,
+                                   double* grad_out, int64_t* n_total_out, uintptr_t stream) {
+  if (!ctx) return b2k_fail(nullptr, B2K_ERR_INVALID, "b2k_logreg_eval_csr: ctx is NULL");
+  B2K_TRY(check_csr(ctx, "b2k_logreg_eval_csr", indptr, indices, values, n_local, nnz_local, d));
+  if ((!y && n_local > 0) || !classes || !W || !b || !loss_out || !grad_out)
+    return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_logreg_eval_csr: NULL argument");
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  B2K_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  B2K_TRY(check_no_empty_partition(ctx, "b2k_logreg_eval_csr", n_local, s));
+  return b2k_logreg_eval_csr_impl(ctx, B2kCsr{indptr, indices, values, n_local, nnz_local, d}, y, classes, n_classes,
+                                  kp, W, b, loss_out, grad_out, n_total_out, s);
+}
+
+extern "C" int b2k_logreg_fit_csr(b2k_ctx* ctx, const int64_t* indptr, const int32_t* indices, const float* values,
+                                  int64_t n_local, int64_t nnz_local, int64_t d, const float* y, const double* classes,
+                                  const int64_t* counts, int n_classes, int n_fits, const b2k_logreg_params* params,
+                                  double* coef_out, double* intercept_out, int* kp_out, int* n_iter_out,
+                                  uintptr_t stream) {
+  if (!ctx) return b2k_fail(nullptr, B2K_ERR_INVALID, "b2k_logreg_fit_csr: ctx is NULL");
+  B2K_TRY(check_csr(ctx, "b2k_logreg_fit_csr", indptr, indices, values, n_local, nnz_local, d));
+  if ((!y && n_local > 0) || !classes || !counts || n_fits < 1 || !params || !coef_out || !intercept_out || !kp_out ||
+      !n_iter_out)
+    return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_logreg_fit_csr: NULL argument or n_fits < 1");
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  B2K_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  B2K_TRY(check_no_empty_partition(ctx, "b2k_logreg_fit_csr", n_local, s));
+  return b2k_logreg_fit_csr_impl(ctx, B2kCsr{indptr, indices, values, n_local, nnz_local, d}, y, classes, counts,
+                                 n_classes, n_fits, params, coef_out, intercept_out, kp_out, n_iter_out, s);
+}
+
+extern "C" int b2k_logreg_predict_csr(b2k_ctx* ctx, const int64_t* indptr, const int32_t* indices, const float* values,
+                                      int64_t n, int64_t nnz, int64_t d, int kp, const double* W, const double* b,
+                                      const double* class_values, double* raw_out, double* prob_out, double* pred_out,
+                                      uintptr_t stream) {
+  if (!ctx) return b2k_fail(nullptr, B2K_ERR_INVALID, "b2k_logreg_predict_csr: ctx is NULL");
+  B2K_TRY(check_csr(ctx, "b2k_logreg_predict_csr", indptr, indices, values, n, nnz, d));
+  if (!W || !b || !class_values || ((!raw_out || !prob_out || !pred_out) && n > 0) || kp < 1)
+    return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_logreg_predict_csr: bad W/b/outputs/kp");
+  B2K_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  return b2k_logreg_predict_csr_impl(ctx, B2kCsr{indptr, indices, values, n, nnz, d}, kp, W, b, class_values, raw_out,
+                                     prob_out, pred_out, reinterpret_cast<cudaStream_t>(stream));
+}
+
+// ------------------------------------------------------------------------------------------------
 // evaluation (b2k_eval.cu)
 // ------------------------------------------------------------------------------------------------
 static bool eval_outputs_ok(int classification, int64_t* label_count_out, int64_t* tp_out, int64_t* fp_out,

@@ -232,7 +232,109 @@ int transpose_dispatch(b2k_ctx* ctx, int dt, const void* src, int64_t rows, int 
   }
   return b2k_fail(ctx, B2K_ERR_INVALID, "ingest: unknown src_dtype");
 }
+// One staged batch of Spark vector rows -> CSR rows: a warp per row; row i's entries go to positions vo[i] - vo[0] of
+// the batch (its values' offsets), a dense row (type 1) gets the column indices 0 .. len - 1.
+template <typename T>
+__global__ void __launch_bounds__(256)
+k_csr_ingest(const int8_t* __restrict__ type, const int32_t* __restrict__ io, const int32_t* __restrict__ iv,
+             const int32_t* __restrict__ vo, const T* __restrict__ vv, int64_t rows, int64_t nnz0,
+             int64_t* __restrict__ indptr, int32_t* __restrict__ indices, float* __restrict__ values) {
+  const int lane = threadIdx.x & 31;
+  const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int64_t nwarp = ((int64_t)gridDim.x * blockDim.x) >> 5;
+  for (int64_t r = warp; r < rows; r += nwarp) {
+    const int64_t p = vo[r] - vo[0], len = vo[r + 1] - vo[r], ip = io[r] - io[0];
+    const bool dense = type[r] == 1;
+    for (int64_t e = lane; e < len; e += 32) {
+      indices[nnz0 + p + e] = dense ? (int32_t)e : iv[ip + e];
+      values[nnz0 + p + e] = to_f32(vv[p + e]);
+    }
+    if (lane == 0) indptr[r + 1] = nnz0 + p + len;
+  }
+}
 }  // namespace
+
+extern "C" int b2k_ingest_csr_append(b2k_ctx* ctx, int64_t* indptr, int32_t* indices, float* values, int64_t n_max,
+                                     int64_t nnz_max, int64_t d, int64_t row0, int64_t nnz0, const int8_t* type,
+                                     const int32_t* size, const int32_t* idx_offsets, const int32_t* idx_values,
+                                     const int32_t* val_offsets, const void* val_values, int val_dtype, int64_t n_b,
+                                     uintptr_t stream, int64_t* nnz_written) {
+  if (!ctx) return b2k_fail(nullptr, B2K_ERR_INVALID, "b2k_ingest_csr_append: ctx is NULL");
+  if (nnz_written) *nnz_written = 0;
+  if (!indptr || !indices || !values || n_b < 0 || row0 < 0 || nnz0 < 0 || row0 + n_b > n_max || d < 1 ||
+      (n_b > 0 && (!type || !size || !idx_offsets || !idx_values || !val_offsets || !val_values)))
+    return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_ingest_csr_append: bad destination/source/d/row range");
+  if (val_dtype != B2K_F32 && val_dtype != B2K_F64)
+    return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_ingest_csr_append: values must be f32 or f64");
+  if (n_b == 0) return B2K_OK;
+  // the row widths, as the dense ingest checks them: a sparse row's size and a dense row's length must be d, and a
+  // sparse row holds as many indices as values
+  for (int64_t i = 0; i < n_b; ++i) {
+    const int64_t nv = (int64_t)val_offsets[i + 1] - val_offsets[i], ni = (int64_t)idx_offsets[i + 1] - idx_offsets[i];
+    if (type[i] != 0 && type[i] != 1)
+      return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_ingest_csr_append: row " + std::to_string(i) + " has vector type " +
+                                                std::to_string((int)type[i]) + " (0 sparse, 1 dense)");
+    const int64_t width = type[i] == 0 ? (int64_t)size[i] : nv;
+    if (width != d)
+      return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_ingest_csr_append: row " + std::to_string(i) + " has size " +
+                                                std::to_string(width) + ", expected " + std::to_string(d));
+    if (type[i] == 0 && ni != nv)
+      return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_ingest_csr_append: row " + std::to_string(i) + " has " +
+                                                std::to_string(ni) + " indices and " + std::to_string(nv) + " values");
+  }
+  const int64_t nnz_b = (int64_t)val_offsets[n_b] - val_offsets[0];
+  if (nnz0 + nnz_b > nnz_max) return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_ingest_csr_append: nnz_max exceeded");
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  B2K_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  B2K_TRY(ensure_staging(ctx));
+  const size_t es = dtype_size(val_dtype);
+  // rows [r, r1) per staging slot: type | index offsets | value offsets | indices | values, each 16-byte aligned
+  auto al = [](size_t b) { return (b + 15) & ~(size_t)15; };
+  auto bytes = [&](int64_t r, int64_t r1) {
+    const int64_t ni = (int64_t)idx_offsets[r1] - idx_offsets[r], nv = (int64_t)val_offsets[r1] - val_offsets[r];
+    return al(r1 - r) + 2 * al(4 * (size_t)(r1 - r + 1)) + al(4 * (size_t)ni) + al(es * (size_t)nv);
+  };
+  for (int64_t r = 0; r < n_b;) {
+    int64_t r1 = n_b;
+    while (r1 > r + 1 && bytes(r, r1) > STAGE_BYTES) r1 = r + (r1 - r) / 2;
+    if (bytes(r, r1) > STAGE_BYTES)
+      return b2k_fail(ctx, B2K_ERR_UNSUPPORTED, "b2k_ingest_csr_append: one row exceeds the staging buffer");
+    const int64_t rows = r1 - r;
+    const int64_t ni = (int64_t)idx_offsets[r1] - idx_offsets[r], nv = (int64_t)val_offsets[r1] - val_offsets[r];
+    const int b = ctx->stage_next;
+    ctx->stage_next ^= 1;
+    B2K_CUDA_OK(ctx, cudaEventSynchronize(ctx->stage_evt[b]));   // the previous use of this slot has drained
+    char* pin = static_cast<char*>(ctx->pinned[b]);
+    char* dev = static_cast<char*>(ctx->dev_stage[b]);
+    size_t off = 0;
+    const size_t o_type = off; memcpy(pin + off, type + r, rows); off += al(rows);
+    const size_t o_io = off; memcpy(pin + off, idx_offsets + r, 4 * (rows + 1)); off += al(4 * (rows + 1));
+    const size_t o_vo = off; memcpy(pin + off, val_offsets + r, 4 * (rows + 1)); off += al(4 * (rows + 1));
+    const size_t o_iv = off; copy_pool(ctx)->copy(pin + off, idx_values + idx_offsets[r], 4 * (size_t)ni); off += al(4 * ni);
+    const size_t o_vv = off;
+    copy_pool(ctx)->copy(pin + off, static_cast<const char*>(val_values) + es * (size_t)val_offsets[r], es * (size_t)nv);
+    off += al(es * nv);
+    B2K_CUDA_OK(ctx, cudaMemcpyAsync(dev, pin, off, cudaMemcpyHostToDevice, s));
+    const int64_t at = nnz0 + (int64_t)val_offsets[r] - val_offsets[0];
+    const unsigned grid = (unsigned)std::max<int64_t>(1, std::min<int64_t>((rows + 7) / 8, 16 * ctx->sm_count));
+    auto tp = reinterpret_cast<const int8_t*>(dev + o_type);
+    auto io = reinterpret_cast<const int32_t*>(dev + o_io);
+    auto vo = reinterpret_cast<const int32_t*>(dev + o_vo);
+    auto iv = reinterpret_cast<const int32_t*>(dev + o_iv);
+    if (val_dtype == B2K_F64)
+      k_csr_ingest<double><<<grid, 256, 0, s>>>(tp, io, iv, vo, reinterpret_cast<const double*>(dev + o_vv), rows, at,
+                                                indptr + row0 + r, indices, values);
+    else
+      k_csr_ingest<float><<<grid, 256, 0, s>>>(tp, io, iv, vo, reinterpret_cast<const float*>(dev + o_vv), rows, at,
+                                               indptr + row0 + r, indices, values);
+    B2K_CUDA_OK(ctx, cudaGetLastError());
+    ctx->stats.kernel_launches++;
+    B2K_CUDA_OK(ctx, cudaEventRecord(ctx->stage_evt[b], s));
+    r = r1;
+  }
+  if (nnz_written) *nnz_written = nnz_b;
+  return B2K_OK;
+}
 
 extern "C" int b2k_ingest_append(b2k_ctx* ctx, float* dst, int64_t n_max, int d, int64_t row0, const void* values,
                                  const int32_t* offsets, int64_t n_b, int src_dtype, int layout,

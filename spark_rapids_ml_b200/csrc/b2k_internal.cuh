@@ -4,6 +4,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <functional>
 #include <memory>
 #include <string>
 #include <vector>
@@ -468,6 +469,38 @@ int b2k_logreg_fit_impl(b2k_ctx* ctx, const float* X, const float* y, int64_t n,
 int b2k_logreg_predict_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, int kp, const double* W, const double* b,
                             const double* class_values, double* raw_out, double* prob_out, double* pred_out,
                             cudaStream_t s);
+// The parts of a fit that do not depend on the data layout, shared by the dense and the CSR fits.  An evaluation at
+// (W [kp][d], b [kp]) returns out [kp (d + 1) + 2] = allreduced [sum r x | sum r per class (at k (d + 1) + d) | sum loss
+// | n], the layout of b2k_logreg_eval's pass.
+using B2kLogregEval = std::function<int(int kp, const double* W, const double* b, double* out)>;
+int b2k_logreg_check_params(b2k_ctx* ctx, int n_classes, int n_fits, const b2k_logreg_params* prm);
+std::vector<int> b2k_logreg_class_map(const double* classes, int n_classes);
+// Per setting: the solver frame, penalty weights, prior log-odds start, L-BFGS / OWL-QN through `eval`, W = V / sigma and
+// MLlib's centring; ssq [d] = the global sum of (x - mu)^2 per feature over n_total rows.
+int b2k_logreg_fit_settings(b2k_ctx* ctx, int d, int64_t n_total, const std::vector<double>& ssq, const double* classes,
+                            const int64_t* counts, int n_classes, int n_fits, const b2k_logreg_params* prm,
+                            const B2kLogregEval& eval, double* coef_out, double* intercept_out, int* kp_out,
+                            int* n_iter_out);
+
+// sparse logistic regression — b2k_logreg_sparse.cu.  A rank's rows in CSR: indptr [n + 1] int64 (indptr[0] = 0), indices
+// [nnz] int32, values [nnz] f32.
+constexpr int64_t B2K_LOGREG_CSR_MAX_PARAMS = (int64_t)1 << 25;   // cap on kp (d + 1): the host L-BFGS state
+constexpr size_t B2K_LOGREG_CSR_R_BYTES = (size_t)256 << 20;      // cap on one row chunk's residuals R [rows][kp] fp64
+struct B2kCsr {
+  const int64_t* indptr;
+  const int32_t* indices;
+  const float* values;
+  int64_t n, nnz, d;
+};
+int b2k_logreg_eval_csr_impl(b2k_ctx* ctx, const B2kCsr& X, const float* y, const double* classes, int n_classes, int kp,
+                             const double* W, const double* b, double* loss_out, double* grad_out, int64_t* n_total_out,
+                             cudaStream_t s);
+int b2k_logreg_fit_csr_impl(b2k_ctx* ctx, const B2kCsr& X, const float* y, const double* classes, const int64_t* counts,
+                            int n_classes, int n_fits, const b2k_logreg_params* prm, double* coef_out,
+                            double* intercept_out, int* kp_out, int* n_iter_out, cudaStream_t s);
+int b2k_logreg_predict_csr_impl(b2k_ctx* ctx, const B2kCsr& X, int kp, const double* W, const double* b,
+                                const double* class_values, double* raw_out, double* prob_out, double* pred_out,
+                                cudaStream_t s);
 
 // ------------------------------------------------------------------------------------------------
 // evaluation — b2k_eval.cu (the C ABI entry points in b2k_api.cu check their arguments, then call these)

@@ -101,31 +101,6 @@ __global__ void k_logreg_labels_fold(const double* __restrict__ part, int spans,
 }
 
 // ------------------------------------------------------------------------------------------------
-// per-row loss and residuals (shared by both evaluation paths): m [kp] margins in, r [kp] = p - onehot(c) out
-// ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ double row_loss_residual(double* m, int kp, int c) {
-  if (kp == 1) {
-    const double x = m[0], yy = c == 1 ? 1.0 : 0.0;
-    const double e = exp(-fabs(x));
-    const double p = x >= 0.0 ? 1.0 / (1.0 + e) : e / (1.0 + e);
-    m[0] = p - yy;
-    return fmax(x, 0.0) + log1p(e) - yy * x;
-  }
-  double mx = m[0];
-  for (int k = 1; k < kp; ++k) mx = fmax(mx, m[k]);
-  double s = 0.0;
-  for (int k = 0; k < kp; ++k) s += exp(m[k] - mx);
-  const double lse = mx + log(s);
-  const double loss = lse - (c >= 0 ? m[c] : 0.0);
-  for (int k = 0; k < kp; ++k) m[k] = exp(m[k] - lse) - (k == c ? 1.0 : 0.0);
-  return loss;
-}
-
-__device__ __forceinline__ int class_of(float v, const int* __restrict__ cmap) {
-  return (v >= 0.f && v < (float)MAXC && v == floorf(v)) ? cmap[(int)v] : -1;
-}
-
-// ------------------------------------------------------------------------------------------------
 // fused evaluation pass
 // ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ void cp_async4(float* smem, const float* gmem) {
@@ -277,7 +252,7 @@ __global__ void __launch_bounds__(LR_THREADS, KB == 1 ? 3 : 2) k_logreg_eval(Eva
           for (int sl = 0; sl < fs.fs_n; ++sl) m += mp_s[((size_t)sl * tr + tid) * kp + k];
           rr[k] = m;
         }
-        const double l = row_loss_residual(rr, kp, class_of(a.y[t0 + tid], a.cmap));
+        const double l = b2k_row_loss_residual(rr, kp, b2k_class_of(a.y[t0 + tid], a.cmap, MAXC));
         ls_s[tid] += l;
         for (int k = 0; k < kp; ++k) ib_s[(size_t)tid * kp + k] += rr[k];
       }
@@ -383,7 +358,7 @@ k_logreg_rows(const float* __restrict__ X, int64_t n, int d, int kp, const doubl
     }
     if (sub != 0 || !valid) continue;
     if (TRAIN) {
-      loss[row] = row_loss_residual(mrow, kp, class_of(y[row], cmap));
+      loss[row] = b2k_row_loss_residual(mrow, kp, b2k_class_of(y[row], cmap, MAXC));
     } else if (kp == 1) {
       const double m = mrow[1];
       const double p1 = b2k_sigmoid(m);
@@ -884,7 +859,9 @@ int eval_device(b2k_ctx* ctx, const EvalCall& e, const double* W, const double* 
   return B2K_OK;
 }
 
-std::vector<int> class_map(const double* classes, int n_classes) {
+}  // namespace
+
+std::vector<int> b2k_logreg_class_map(const double* classes, int n_classes) {
   std::vector<int> m(MAXC, -1);
   for (int i = 0; i < n_classes; ++i) {
     const double c = classes[i];
@@ -892,8 +869,6 @@ std::vector<int> class_map(const double* classes, int n_classes) {
   }
   return m;
 }
-
-}  // namespace
 
 int b2k_logreg_eval_impl(b2k_ctx* ctx, const float* X, const float* y, int64_t n, int d, const double* classes,
                          int n_classes, int kp, const double* W, const double* b, double* loss_out, double* grad_out,
@@ -906,7 +881,7 @@ int b2k_logreg_eval_impl(b2k_ctx* ctx, const float* X, const float* y, int64_t n
   if (kp != 1 && kp != n_classes)
     return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_logreg_eval: margins per row must be 1 or the class count " +
                                               std::to_string(n_classes) + ", got " + std::to_string(kp));
-  const std::vector<int> cm = class_map(classes, n_classes);
+  const std::vector<int> cm = b2k_logreg_class_map(classes, n_classes);
   EvalCall e{X, y, n, d, kp, &cm};
   const int M = kp * (d + 1) + 1;
   std::vector<double> out((size_t)M + 1);
@@ -919,16 +894,8 @@ int b2k_logreg_eval_impl(b2k_ctx* ctx, const float* X, const float* y, int64_t n
   return B2K_OK;
 }
 
-int b2k_logreg_fit_impl(b2k_ctx* ctx, const float* X, const float* y, int64_t n, int d, const double* classes,
-                        const int64_t* counts, int n_classes, int n_fits, const b2k_logreg_params* prm,
-                        double* coef_out, double* intercept_out, int* kp_out, int* n_iter_out, cudaStream_t s) {
-  using clk = std::chrono::steady_clock;
-  const auto t_begin = clk::now();
-  if (d > B2K_LOGREG_MAX_D)
-    return b2k_fail(ctx, B2K_ERR_UNSUPPORTED, "logistic regression supports d <= " + std::to_string(B2K_LOGREG_MAX_D) +
-                                                  ", got d = " + std::to_string(d));
-  if (n_classes < 1 || n_classes > MAXC) return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_logreg_fit: bad class count");
-  const int K = n_classes;
+int b2k_logreg_check_params(b2k_ctx* ctx, int K, int n_fits, const b2k_logreg_params* prm) {
+  if (K < 1 || K > MAXC) return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_logreg_fit: bad class count");
   for (int f = 0; f < n_fits; ++f) {   // the driver-side checks, repeated so a direct caller gets them too
     const b2k_logreg_params& p = prm[f];
     if (p.max_iter < 0) return b2k_fail(ctx, B2K_ERR_INVALID, "maxIter given invalid value " + std::to_string(p.max_iter));
@@ -941,11 +908,14 @@ int b2k_logreg_fit_impl(b2k_ctx* ctx, const float* X, const float* y, int64_t n,
       return b2k_fail(ctx, B2K_ERR_INVALID, "Binomial family only supports 1 or 2 outcome classes but found " +
                                                 std::to_string(K) + ".");
   }
-  int64_t n_total = 0;
-  std::vector<double> mu, ssq;
-  B2K_TRY(b2k_colstats_impl(ctx, "logistic regression", X, n, d, &n_total, &mu, &ssq, s));
-  if (!finite_all(mu.data(), d) || !finite_all(ssq.data(), d))
-    return b2k_fail(ctx, B2K_ERR_INVALID, "logistic regression: the features hold a NaN or an infinity");
+  return B2K_OK;
+}
+
+int b2k_logreg_fit_settings(b2k_ctx* ctx, int d, int64_t n_total, const std::vector<double>& ssq, const double* classes,
+                            const int64_t* counts, int n_classes, int n_fits, const b2k_logreg_params* prm,
+                            const B2kLogregEval& eval, double* coef_out, double* intercept_out, int* kp_out,
+                            int* n_iter_out) {
+  const int K = n_classes;
   if (K == 1) {   // one label value: as the reference, no optimisation (after the moments pass, so that bad
                   // features are still reported)
     if (classes[0] != 0.0 && classes[0] != 1.0)
@@ -961,7 +931,6 @@ int b2k_logreg_fit_impl(b2k_ctx* ctx, const float* X, const float* y, int64_t n,
   // sample standard deviations, as MLlib's summarizer (n - 1; 0 for a single row)
   std::vector<double> sigma(d);
   for (int j = 0; j < d; ++j) sigma[j] = n_total > 1 ? std::sqrt(std::max(ssq[j], 0.0) / (double)(n_total - 1)) : 0.0;
-  const std::vector<int> cm = class_map(classes, K);
   for (int f = 0; f < n_fits; ++f) {
     const b2k_logreg_params& p = prm[f];
     const bool multi = p.family == 2 || (p.family == 0 && K > 2);
@@ -991,9 +960,7 @@ int b2k_logreg_fit_impl(b2k_ctx* ctx, const float* X, const float* y, int64_t n,
       }
     }
     struct Fn {
-      b2k_ctx* ctx;
-      EvalCall e;
-      cudaStream_t s;
+      const B2kLogregEval* eval;
       int d, kp;
       bool fi;
       double l2;
@@ -1001,7 +968,7 @@ int b2k_logreg_fit_impl(b2k_ctx* ctx, const float* X, const float* y, int64_t n,
       const std::vector<double>* pen;
       std::vector<double> W, b, out;
       int rc;
-    } F{ctx, EvalCall{X, y, n, d, kp, &cm}, s, d, kp, fi, l2, &inv, &pen,
+    } F{&eval, d, kp, fi, l2, &inv, &pen,
         std::vector<double>(nv), std::vector<double>(kp, 0.0), std::vector<double>((size_t)kp * (d + 1) + 2), B2K_OK};
     auto cb = [](void* user, int, const double* th, double* fval, double* grad) -> int {
       Fn& q = *static_cast<Fn*>(user);
@@ -1009,7 +976,7 @@ int b2k_logreg_fit_impl(b2k_ctx* ctx, const float* X, const float* y, int64_t n,
       for (int k = 0; k < kp; ++k)
         for (int j = 0; j < d; ++j) q.W[(size_t)k * d + j] = th[(size_t)k * d + j] * (*q.inv)[j];
       for (int k = 0; k < kp; ++k) q.b[k] = q.fi ? th[nv + k] : 0.0;
-      q.rc = eval_device(q.ctx, q.e, q.W.data(), q.b.data(), q.out.data(), q.s);
+      q.rc = (*q.eval)(kp, q.W.data(), q.b.data(), q.out.data());
       if (q.rc != B2K_OK) return q.rc;
       const int M = kp * (d + 1) + 1;
       const double nt = q.out[M];
@@ -1060,6 +1027,29 @@ int b2k_logreg_fit_impl(b2k_ctx* ctx, const float* X, const float* y, int64_t n,
     n_iter_out[f] = iters;
     ctx->stats.last_n_iter = iters;
   }
+  return B2K_OK;
+}
+
+int b2k_logreg_fit_impl(b2k_ctx* ctx, const float* X, const float* y, int64_t n, int d, const double* classes,
+                        const int64_t* counts, int n_classes, int n_fits, const b2k_logreg_params* prm,
+                        double* coef_out, double* intercept_out, int* kp_out, int* n_iter_out, cudaStream_t s) {
+  using clk = std::chrono::steady_clock;
+  const auto t_begin = clk::now();
+  if (d > B2K_LOGREG_MAX_D)
+    return b2k_fail(ctx, B2K_ERR_UNSUPPORTED, "logistic regression supports d <= " + std::to_string(B2K_LOGREG_MAX_D) +
+                                                  ", got d = " + std::to_string(d));
+  B2K_TRY(b2k_logreg_check_params(ctx, n_classes, n_fits, prm));
+  int64_t n_total = 0;
+  std::vector<double> mu, ssq;
+  B2K_TRY(b2k_colstats_impl(ctx, "logistic regression", X, n, d, &n_total, &mu, &ssq, s));
+  if (!finite_all(mu.data(), d) || !finite_all(ssq.data(), d))
+    return b2k_fail(ctx, B2K_ERR_INVALID, "logistic regression: the features hold a NaN or an infinity");
+  const std::vector<int> cm = b2k_logreg_class_map(classes, n_classes);
+  const B2kLogregEval eval = [&](int kp, const double* W, const double* b, double* out) {
+    return eval_device(ctx, EvalCall{X, y, n, d, kp, &cm}, W, b, out, s);
+  };
+  B2K_TRY(b2k_logreg_fit_settings(ctx, d, n_total, ssq, classes, counts, n_classes, n_fits, prm, eval, coef_out,
+                                  intercept_out, kp_out, n_iter_out));
   if (ctx->time_kernels)
     ctx->stats.last_loop_ms = std::chrono::duration<double, std::milli>(clk::now() - t_begin).count();
   return B2K_OK;

@@ -1,5 +1,5 @@
-// Per-row prediction code shared by the predict kernels (k_linreg_predict, k_logreg_rows, k_rf_predict) and the
-// multi-model evaluation pass (b2k_eval.cu).  One definition keeps a model's per-row prediction bit-identical in both:
+// Per-row prediction code shared by the predict kernels (k_linreg_predict, k_logreg_rows, k_csr_rows, k_rf_predict) and
+// the multi-model evaluation pass (b2k_eval.cu).  One definition keeps a model's per-row prediction bit-identical in both:
 // the same lane split, the same fp64 FMA order and xor butterfly, the same tree walk and __dadd_rn order.
 #pragma once
 #include <cuda_runtime.h>
@@ -89,6 +89,47 @@ __device__ __forceinline__ void b2k_logistic_lanes(const LD& ld, int d, int kp, 
       }
     }
   }
+}
+
+// Sparse rows (CSR): lane `sub` of the row's L lanes accumulates entries p0 + sub + L i in order in fp64 for the classes
+// k0 .. k0 + RC - 1 (< kp), the weight of class k and feature j at W[k ldk + j ldj] (gathered through L2).
+template <int RC>
+__device__ __forceinline__ void b2k_csr_lanes(const int32_t* __restrict__ idx, const float* __restrict__ val, int64_t p0,
+                                              int64_t p1, int kp, int k0, const double* __restrict__ W, int64_t ldk,
+                                              int64_t ldj, int sub, int L, double (&acc)[RC]) {
+  for (int64_t e = p0 + sub; e < p1; e += L) {
+    const int64_t j = __ldg(idx + e);
+    const double v = (double)__ldg(val + e);
+#pragma unroll
+    for (int q = 0; q < RC; ++q) {
+      const int k = k0 + q;
+      if (k < kp) acc[q] = fma(v, __ldg(W + k * ldk + j * ldj), acc[q]);
+    }
+  }
+}
+
+// Training: m [kp] margins in, r [kp] = p - onehot(c) out (c = -1: no class); returns the row's loss.
+__device__ __forceinline__ double b2k_row_loss_residual(double* m, int kp, int c) {
+  if (kp == 1) {
+    const double x = m[0], yy = c == 1 ? 1.0 : 0.0;
+    const double e = exp(-fabs(x));
+    const double p = x >= 0.0 ? 1.0 / (1.0 + e) : e / (1.0 + e);
+    m[0] = p - yy;
+    return fmax(x, 0.0) + log1p(e) - yy * x;
+  }
+  double mx = m[0];
+  for (int k = 1; k < kp; ++k) mx = fmax(mx, m[k]);
+  double s = 0.0;
+  for (int k = 0; k < kp; ++k) s += exp(m[k] - mx);
+  const double lse = mx + log(s);
+  const double loss = lse - (c >= 0 ? m[c] : 0.0);
+  for (int k = 0; k < kp; ++k) m[k] = exp(m[k] - lse) - (k == c ? 1.0 : 0.0);
+  return loss;
+}
+
+// The class index of label v: cmap [maxc] maps an integral label in [0, maxc) to its class, -1 = none.
+__device__ __forceinline__ int b2k_class_of(float v, const int* __restrict__ cmap, int maxc) {
+  return (v >= 0.f && v < (float)maxc && v == floorf(v)) ? cmap[(int)v] : -1;
 }
 
 // Binomial: the probability of class 1 at margin m.

@@ -174,6 +174,8 @@ class CrossValidator(_CrossValidatorParams):
                                           "fit a local frame")
         self._check()
         est, eva = self.getEstimator(), self.getEvaluator()
+        if hasattr(est, "_check_tuning_input"):   # input the single-pass evaluation cannot read, refused before any fit
+            est._check_tuning_input(dataset)
         maps = list(self.getEstimatorParamMaps())
         k = self.getNumFolds()
         parts = int(est.num_workers) if getattr(est, "num_workers", None) else dataset.getNumPartitions()

@@ -98,6 +98,115 @@ def arrow_list_column_buffers(col: pd.Series, d: Optional[int] = None) -> Option
     return None
 
 
+VECTOR_FIELDS = ("type", "size", "indices", "values")
+
+
+def is_vector_struct(t: pa.DataType) -> bool:
+    """Whether an Arrow type is Spark's VectorUDT SQL layout: struct<type: tinyint, size: int, indices: array<int>,
+    values: array<double>> (type 0 a sparse row, 1 a dense row whose size and indices are null)."""
+    return pa.types.is_struct(t) and tuple(t.field(i).name for i in range(t.num_fields)) == VECTOR_FIELDS
+
+
+def _arrow_array(col: Any) -> pa.Array:
+    arr = col.array._pa_array if hasattr(col.array, "_pa_array") else pa.chunked_array(col.array)
+    if isinstance(arr, pa.ChunkedArray):
+        arr = arr.chunk(0) if arr.num_chunks == 1 else arr.combine_chunks()   # single chunk: stay zero-copy
+    return arr
+
+
+def arrow_vector_column_buffers(col: Any) -> Tuple[np.ndarray, ...]:
+    """The child buffers of an Arrow-backed vector struct column, without copying the index and value buffers:
+    (type int8 [n], size int32 [n], index offsets int32 [n + 1], indices int32, value offsets int32 [n + 1], values)."""
+    arr = _arrow_array(col)
+    if not is_vector_struct(arr.type):
+        raise ValueError(f"expected a vector struct column, got {arr.type}")
+    if arr.null_count:
+        raise ValueError("null feature rows are not supported")
+    t, size, idx, val = arr.flatten()   # flatten applies the struct's offset (zero-copy slices)
+    if t.null_count:
+        raise ValueError("a vector row has a null type")
+    return (t.to_numpy(zero_copy_only=False).astype(np.int8, copy=False),
+            size.fill_null(0).to_numpy(zero_copy_only=False).astype(np.int32, copy=False),
+            idx.offsets.to_numpy(zero_copy_only=True), idx.values.to_numpy(zero_copy_only=True),
+            val.offsets.to_numpy(zero_copy_only=True), val.values.to_numpy(zero_copy_only=True))
+
+
+def densify_vector_column(arr: pa.Array, d: int) -> pa.Array:
+    """A vector struct array as a list<float> column of width d (the dense path's input)."""
+    if arr.null_count:
+        raise ValueError("null feature rows are not supported")
+    t, size, idx, val = arr.flatten()
+    types = t.to_numpy(zero_copy_only=False)
+    n = len(arr)
+    out = np.zeros((n, d), dtype=np.float32)
+    vo, vv = val.offsets.to_numpy(), val.values.to_numpy(zero_copy_only=False)
+    io, iv = idx.offsets.to_numpy(), idx.values.to_numpy(zero_copy_only=False)
+    sizes = size.fill_null(d).to_numpy(zero_copy_only=False)
+    lens = np.diff(vo)
+    if np.any((types == 0) & (sizes != d)) or np.any((types == 1) & (lens != d)):
+        raise ValueError(f"feature vectors have different sizes: expected {d}")
+    rows = np.repeat(np.arange(n), lens)
+    vals = vv[vo[0]:vo[-1]]
+    pos = np.arange(vals.size) - np.repeat(vo[:-1] - vo[0], lens)   # position within the row
+    cols = np.where(np.repeat(types == 1, lens), pos, 0)
+    sp = np.repeat(types == 0, lens)
+    if sp.any():
+        if np.any(np.diff(io)[types == 0] != lens[types == 0]):
+            raise ValueError("a sparse vector holds different numbers of indices and values")
+        ip = np.repeat(io[:-1], lens) + pos
+        cols = np.where(sp, iv[np.where(sp, ip, 0)] if iv.size else 0, cols)
+    if np.any((cols < 0) | (cols >= d)):
+        raise ValueError(f"a vector index is out of bounds for vectors of size {d}")
+    out[rows, cols] = vals
+    offsets = pa.array(np.arange(n + 1, dtype=np.int32) * np.int32(d))
+    return pa.ListArray.from_arrays(offsets, pa.array(out.reshape(-1)))
+
+
+class DeviceCsrAppender:
+    """Growing device CSR (indptr int64 [n + 1], indices int32 [nnz], values float32 [nnz]) fed batch by batch from a
+    vector struct column through b2k_ingest_csr_append; grown geometrically, on the device."""
+
+    def __init__(self, ctx: Any, d: int, first_rows: int = 1 << 16, first_nnz: int = 1 << 20):
+        import torch
+
+        self._torch = torch
+        self.ctx, self.d = ctx, d
+        self.n = self.nnz = 0
+        self.indptr = torch.zeros(max(1, first_rows) + 1, dtype=torch.int64, device=ctx.device)
+        self.indices = torch.empty(max(1, first_nnz), dtype=torch.int32, device=ctx.device)
+        self.values = torch.empty(max(1, first_nnz), dtype=torch.float32, device=ctx.device)
+
+    def _grow(self, name: str, need: int) -> None:
+        old = getattr(self, name)
+        if need <= old.shape[0]:
+            return
+        new = self._torch.empty(max(need, 2 * old.shape[0]), dtype=old.dtype, device=old.device)
+        new[: old.shape[0]] = old
+        setattr(self, name, new)
+
+    def append_column(self, col: Any) -> int:
+        """One batch's vector struct column (Arrow-backed pandas Series) -> rows of the CSR; returns its row count."""
+        bufs = arrow_vector_column_buffers(col)
+        n_b = int(bufs[0].shape[0])
+        if n_b == 0:
+            return 0
+        nnz_b = int(bufs[4][-1]) - int(bufs[4][0])
+        self._grow("indptr", self.n + n_b + 1)
+        self._grow("indices", self.nnz + nnz_b)
+        self._grow("values", self.nnz + nnz_b)
+        self.ctx.ingest_csr(self.indptr, self.indices, self.values, self.d, self.n, self.nnz, *bufs)
+        self.n += n_b
+        self.nnz += nnz_b
+        return n_b
+
+    @property
+    def rows(self) -> int:
+        return self.n
+
+    def finish(self) -> Tuple[Any, Any, Any]:
+        return self.indptr[: self.n + 1], self.indices[: self.nnz], self.values[: self.nnz]
+
+
 class DeviceRowAppender:
     """Growing device matrix [n, d] f32 fed batch by batch through b2k_ingest_append (replaces core.py:907-941
     + clustering.py:388-393).  Capacity grows geometrically by segments; segments are concatenated on the device
