@@ -31,14 +31,13 @@ model fitted either way; CrossValidator and _transformEvaluate of such a frame r
 """
 from __future__ import annotations
 
-from typing import Any, Callable, Dict, Iterator, List, Optional, Sequence, Tuple, Union
+from typing import Any, Callable, Dict, List, Optional, Sequence, Tuple, Union
 
 import numpy as np
 import pyarrow as pa
 
-from .core import FitInputType, _CumlEstimator, _CumlModelWithPredictionCol, _DeviceModel, alias, param_alias
+from .core import FitInputType, _CumlModelWithPredictionCol, _DeviceModel, _TunedEstimator, alias, param_alias
 from .params import HasFeaturesCol, HasFeaturesCols, HasLabelCol, HasPredictionCol, P, _CumlClass, _CumlParams
-from .regression import _ModelIterator
 from .tree import _RandomForestEstimator, _RandomForestModel
 from .sparkshim import LocalDataFrame, Param, Row, TypeConverters, keyword_only
 from .utils import densify_vector_column, is_vector_struct
@@ -194,20 +193,6 @@ class _LogisticRegressionCumlParams(_CumlParams, _LogisticRegressionParams, HasF
         return self._set_params(thresholds=value)
 
 
-# Params a fitMultiple map may change while every map is still fitted from one ingest, label pass and moments pass
-_SOLVER_PARAMS = frozenset(("regParam", "elasticNetParam", "maxIter", "tol", "fitIntercept", "standardization",
-                            "family"))
-
-
-def _fit_settings(est: "_LogisticRegressionCumlParams") -> Dict[str, Any]:
-    family = est.getFamily().lower()
-    if family not in ("auto", "binomial", "multinomial"):
-        raise ValueError(f"family given invalid value {est.getFamily()}")
-    return {"reg": float(est.getRegParam()), "l1_ratio": float(est.getElasticNetParam()), "tol": float(est.getTol()),
-            "max_iter": int(est.getMaxIter()), "fit_intercept": bool(est.getFitIntercept()),
-            "standardization": bool(est.getStandardization()), "family": family}
-
-
 def _check_settings(s: Dict[str, Any]) -> None:
     """The errors b2k_logreg_fit would return, raised on the driver before any task starts."""
     if s["max_iter"] < 0:
@@ -220,7 +205,7 @@ def _check_settings(s: Dict[str, Any]) -> None:
         raise ValueError(f"tol given invalid value {s['tol']!r}")
 
 
-class LogisticRegression(LogisticRegressionClass, _CumlEstimator, _LogisticRegressionCumlParams):
+class LogisticRegression(LogisticRegressionClass, _TunedEstimator, _LogisticRegressionCumlParams):
     """Logistic regression on H100: binomial or multinomial, with no penalty, L2, L1 or the elastic net, with or without
     an intercept and standardization.  One barrier task per GPU holds its partition on the device; the label pass and
     a column-moments pass run once, then every L-BFGS / OWL-QN step evaluates the loss and gradient in one fused fp64
@@ -255,7 +240,19 @@ class LogisticRegression(LogisticRegressionClass, _CumlEstimator, _LogisticRegre
         if self._input_kwargs.get("num_workers", None) is None:
             self._input_kwargs.pop("num_workers", None)
         self._set_params(**self._input_kwargs)
-        self._fit_grid: Optional[List[Dict[str, Any]]] = None
+
+    # every map is fitted from one ingest, one label pass and one moments pass, then optimised on its own
+    _single_pass_params = frozenset(("regParam", "elasticNetParam", "maxIter", "tol", "fitIntercept",
+                                     "standardization", "family"))
+
+    def _settings(self) -> Dict[str, Any]:
+        family = self.getFamily().lower()
+        if family not in ("auto", "binomial", "multinomial"):
+            raise ValueError(f"family given invalid value {self.getFamily()}")
+        return {"reg": float(self.getRegParam()), "l1_ratio": float(self.getElasticNetParam()),
+                "tol": float(self.getTol()), "max_iter": int(self.getMaxIter()),
+                "fit_intercept": bool(self.getFitIntercept()), "standardization": bool(self.getStandardization()),
+                "family": family}
 
     def _set_cuml_reg_params(self) -> "LogisticRegression":
         penalty, C, l1_ratio = self._reg_params_value_mapping(self.getRegParam(), self.getElasticNetParam())
@@ -296,28 +293,18 @@ class LogisticRegression(LogisticRegressionClass, _CumlEstimator, _LogisticRegre
 
     def _validate_parameters(self) -> None:
         super()._validate_parameters()
-        _check_settings(_fit_settings(self))
+        _check_settings(self._settings())
 
     def _fit_label_col(self) -> Optional[str]:
         return self.getLabelCol()
 
-    def _pre_process_data(self, dataset: LocalDataFrame) -> Tuple[LocalDataFrame, Optional[List[str]], int, str]:
-        """The feature columns as for every estimator, plus the label cast to float32 as alias.label."""
-        label = self.getLabelCol()
-        if label not in dataset.columns:
-            raise ValueError(f"label column '{label}' not found in {dataset.columns}")
-        vec = _vector_column(dataset, self.getFeaturesCol())
-        if vec is not None:
-            df, dimension, ftype = self._pre_process_vectors(dataset, vec)
-            multi_col_names = None
-        else:
-            df, multi_col_names, dimension, ftype = super()._pre_process_data(dataset)
-        df = df.with_appended_column(alias.label, [[b.column(label).cast(pa.float32()) for b in p] for p in dataset._parts])
-        return df, multi_col_names, dimension, ftype
-
-    def _pre_process_vectors(self, dataset: LocalDataFrame, col: str) -> Tuple[LocalDataFrame, int, str]:
+    def _pre_process_features(self, dataset: LocalDataFrame) -> Tuple[LocalDataFrame, Optional[List[str]], int, str]:
         """A vector struct column: kept as vectors for the CSR path ("csr") when enable_sparse_data_optim is None and
-        the first row is sparse, else densified to array<float> (the reference's rule, core.py:507-521)."""
+        the first row is sparse, else densified to array<float> (the reference's rule, core.py:507-521).  Other feature
+        columns as for every estimator."""
+        col = _vector_column(dataset, self.getFeaturesCol())
+        if col is None:
+            return super()._pre_process_features(dataset)
         df = dataset.select(col).withColumnRenamed(col, alias.data)
         first = df.first()
         if first is None:
@@ -328,10 +315,10 @@ class LogisticRegression(LogisticRegressionClass, _CumlEstimator, _LogisticRegre
         sparse = v["type"] == 0
         dimension = int(v["size"]) if sparse else len(v["values"])
         if getattr(self, "_sparse_data_optim", None) is None and sparse:
-            return df, dimension, "csr"
+            return df, None, dimension, "csr"
         parts = [[pa.RecordBatch.from_arrays([densify_vector_column(b.column(0), dimension)], names=[alias.data])
                   for b in p] for p in df._parts]
-        return df._derive(parts, pa.schema([pa.field(alias.data, pa.list_(pa.float32()))])), dimension, "float"
+        return df._derive(parts, pa.schema([pa.field(alias.data, pa.list_(pa.float32()))])), None, dimension, "float"
 
     def _check_tuning_input(self, dataset: Any) -> None:
         """CrossValidator's single-pass evaluation reads dense rows: a vector struct frame is refused before any fit."""
@@ -341,7 +328,7 @@ class LogisticRegression(LogisticRegressionClass, _CumlEstimator, _LogisticRegre
 
     def _get_cuml_fit_func(self, dataset: Any, extra_params: Optional[List[Dict[str, Any]]] = None
                            ) -> Callable[[FitInputType, Dict[str, Any]], Dict[str, Any]]:
-        grid = self._fit_grid if self._fit_grid is not None else [_fit_settings(self)]
+        grid = self._fit_grid or [self._settings()]
 
         def _cuml_fit(dfs: FitInputType, params: Dict[str, Any]) -> Dict[str, Any]:
             # stands in for LogisticRegressionMG(handle, ...).fit(...) per param map, the rescaling and the intercept
@@ -384,27 +371,10 @@ class LogisticRegression(LogisticRegressionClass, _CumlEstimator, _LogisticRegre
                                        classes_=list(r["classes_"]), n_cols=int(r["n_cols"]), dtype=str(r["dtype"]),
                                        num_iters=int(r["num_iters"]))
 
-    def _enable_fit_multiple_in_single_pass(self) -> bool:
-        return True
-
     def _supportsTransformEvaluate(self, evaluator: Any) -> bool:
         from .core import _supports_transform_evaluate
 
         return _supports_transform_evaluate(True, evaluator)
-
-    def fitMultiple(self, dataset: Any, paramMaps: Sequence[Dict[Any, Any]]) -> Iterator[Tuple[int, Any]]:
-        """(index, model) per param map, in map order.  When every map changes only fit params (regParam,
-        elasticNetParam, maxIter, tol, fitIntercept, standardization, family), one ingest, one label pass and one
-        moments pass serve all maps, each then optimised on its own; otherwise each map is one fit."""
-        if paramMaps and all(p.name in _SOLVER_PARAMS for pm in paramMaps for p in pm):
-            est = self.copy()
-            est._fit_grid = [_fit_settings(self.copy(pm)) for pm in paramMaps]
-            for s in est._fit_grid:
-                _check_settings(s)
-            if est._use_cpu_fallback():
-                raise ValueError("a Spark Param without GPU support is set and spark_rapids_ml_b200 has no CPU fallback")
-            return _ModelIterator(est._fit_internal(dataset, list(paramMaps)))
-        return _ModelIterator([self.copy(pm)._fit(dataset) for pm in paramMaps])
 
 
 class LogisticRegressionModel(LogisticRegressionClass, _CumlModelWithPredictionCol, _LogisticRegressionCumlParams):
@@ -500,18 +470,7 @@ class LogisticRegressionModel(LogisticRegressionClass, _CumlModelWithPredictionC
         raise NotImplementedError("LogisticRegressionModel.cpu() builds a JVM pyspark.ml model; no JVM/pyspark in this "
                                   "build")
 
-    @classmethod
-    def _combine(cls, models: List["LogisticRegressionModel"]) -> "LogisticRegressionModel":
-        """One model holding several fits' coefficients (reference classification.py:1557-1572)."""
-        assert len(models) > 0 and all(isinstance(m, cls) for m in models)
-        first = models[0]
-        attrs = dict(first._get_model_attributes() or {})
-        attrs["coef_"] = [m.coef_ for m in models]
-        attrs["intercept_"] = [m.intercept_ for m in models]
-        out = cls(**attrs)
-        first._copyValues(out)
-        first._copy_cuml_params(out)
-        return out
+    _combined_attrs = ("coef_", "intercept_")
 
     def _out_schema(self, input_schema: Any = None) -> str:
         return "double"

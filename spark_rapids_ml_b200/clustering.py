@@ -21,13 +21,13 @@ raises NotImplementedError.
 from __future__ import annotations
 
 import functools
-from typing import Any, Callable, Dict, Iterator, List, Optional, Sequence, Tuple, Union
+from typing import Any, Callable, Dict, List, Optional, Sequence, Tuple, Union
 
 import numpy as np
 import pyarrow as pa
 
-from .core import (FitInputType, _CumlCaller, _CumlEstimator, _CumlModelWithPredictionCol, _DeviceModel, alias,
-                   param_alias)
+from .core import (FitInputType, _CumlCaller, _CumlEstimator, _CumlModelWithPredictionCol, _DeviceModel,
+                   _TunedEstimator, alias, param_alias)
 from .params import HasFeaturesCol, HasFeaturesCols, HasIDCol, HasPredictionCol, P, _CumlClass, _CumlParams, _KMeansParams
 from .sparkshim import HAVE_PYSPARK, Param, Row, TypeConverters, keyword_only
 from .utils import get_logger
@@ -114,7 +114,7 @@ class _KMeansCumlParams(_CumlParams, _KMeansParams, HasFeaturesCols):
         return self
 
 
-class KMeans(KMeansClass, _CumlEstimator, _KMeansCumlParams):
+class KMeans(KMeansClass, _TunedEstimator, _KMeansCumlParams):
     """KMeans on H100: one barrier task per GPU; each iteration is ONE fused pass over the device-resident
     partition (TMA -> wgmma 3xTF32 distance tile -> argmin, then per-cluster partial sums) followed by one NCCL
     allreduce of the [k*d sums | k counts] buffer.  Parameters as in the reference (clustering.py:197-236):
@@ -135,7 +135,6 @@ class KMeans(KMeansClass, _CumlEstimator, _KMeansCumlParams):
                  seed: Optional[int] = None, num_workers: Optional[int] = None,
                  verbose: Union[int, bool] = False, **kwargs: Any) -> None:
         super().__init__()
-        self._fit_grid: Optional[List[Dict[str, Any]]] = None
         self._handle_param_spark_confs()   # session-wide defaults for arguments not passed (clustering.py:315)
         # if the user does not override it, n_init = 1 to match Spark behaviour (clustering.py:316-319)
         if "n_init" not in self._input_kwargs:
@@ -167,6 +166,12 @@ class KMeans(KMeansClass, _CumlEstimator, _KMeansCumlParams):
 
     def setWeightCol(self, value: str) -> "KMeans":
         raise ValueError("'weightCol' is not supported by cuML.")
+
+    # every map is fitted in turn on the same device matrix
+    _single_pass_params = frozenset(("k", "maxIter", "tol", "seed", "initMode"))
+
+    def _settings(self) -> Dict[str, Any]:
+        return dict(self.cuml_params)
 
     def _fit_array_order(self) -> str:
         return "C"
@@ -222,27 +227,6 @@ class KMeans(KMeansClass, _CumlEstimator, _KMeansCumlParams):
     def _supportsTransformEvaluate(self, evaluator: Any) -> bool:
         """CrossValidator scores KMeans models with a ClusteringEvaluator's silhouette, either distance measure."""
         return _supports_silhouette(evaluator)
-
-    def fitMultiple(self, dataset: Any, paramMaps: Sequence[Dict[Any, Any]]) -> Iterator[Tuple[int, Any]]:
-        """(index, model) per param map, in map order.  When every map changes only k, maxIter, tol, seed or
-        initMode, one ingest serves all maps: one barrier task per GPU fits each map in turn on the same device matrix,
-        and each model equals est.copy(map).fit(dataset).  Otherwise each map is one fit."""
-        from .regression import _ModelIterator
-
-        maps = list(paramMaps)
-        if not _kmeans_grid_shares_ingest(maps):
-            return _ModelIterator([self.copy(pm)._fit(dataset) for pm in maps])
-        copies = [self.copy(pm) for pm in maps]
-        for c in copies:
-            c._validate_parameters()
-        est = self.copy()
-        est._fit_grid = [dict(c.cuml_params) for c in copies]
-        if est._use_cpu_fallback():
-            raise ValueError("a Spark Param without GPU support is set and spark_rapids_ml_b200 has no CPU fallback")
-        models = est._fit_internal(dataset, maps)
-        for m, c in zip(models, copies):
-            c._copy_cuml_params(m)
-        return _ModelIterator(models)
 
     def _out_schema(self) -> Any:
         # reference: clustering.py:458-468
@@ -308,15 +292,7 @@ class KMeansModel(KMeansClass, _CumlModelWithPredictionCol, _KMeansCumlParams):
         c = self.cluster_centers_
         return [c] if len(c) == 0 or not isinstance(c[0][0], (list, tuple)) else list(c)  # type: ignore[list-item]
 
-    @classmethod
-    def _combine(cls, models: List["KMeansModel"]) -> "KMeansModel":
-        """One model holding several fits' centre sets, for _transformEvaluate."""
-        assert len(models) > 0 and all(isinstance(m, cls) for m in models)
-        first = models[0]
-        out = cls(cluster_centers_=[m.cluster_centers_ for m in models], n_cols=first.n_cols, dtype=first.dtype)
-        first._copyValues(out)
-        first._copy_cuml_params(out)
-        return out
+    _combined_attrs = ("cluster_centers_",)
 
     def _transformEvaluate(self, dataset: Any, evaluator: Any, params: Optional[Dict[Any, Any]] = None) -> List[float]:
         """The silhouette of every model of this (combined) model on a local frame, with the worker count and
@@ -366,12 +342,9 @@ def _supports_silhouette(evaluator: Any) -> bool:
         return False
 
 
-_GRID_FIT_PARAMS = frozenset({"k", "maxIter", "tol", "seed", "initMode"})
-
-
 def _kmeans_grid_shares_ingest(paramMaps: Sequence[Dict[Any, Any]]) -> bool:
     """Whether KMeans.fitMultiple fits these maps from one ingest: every map changes only per-fit params."""
-    return bool(paramMaps) and all(p.name in _GRID_FIT_PARAMS for pm in paramMaps for p in pm)
+    return KMeans._shares_ingest(paramMaps)
 
 
 # ---- DBSCAN (reference: clustering.py:607-1186) ----

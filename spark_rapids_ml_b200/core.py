@@ -22,6 +22,7 @@ from __future__ import annotations
 
 import json
 import os
+import threading
 import uuid
 from abc import abstractmethod
 from collections import namedtuple
@@ -312,7 +313,19 @@ class _CumlCaller(_CumlParams, _CumlCommon):
             raise ValueError(f"tol given invalid value {cp['tol']}")
 
     def _pre_process_data(self, dataset: LocalDataFrame) -> Tuple[LocalDataFrame, Optional[List[str]], int, str]:
-        """-> (selected/cast dataframe, multi_col_names, dimension, feature dtype)."""
+        """-> (selected/cast dataframe, multi_col_names, dimension, feature dtype).  The frame holds the features of
+        _pre_process_features and, when _fit_label_col() names one, the label cast to float32 as alias.label."""
+        label = self._fit_label_col()
+        if label is not None and label not in dataset.columns:
+            raise ValueError(f"label column '{label}' not found in {dataset.columns}")
+        df, multi_col_names, dimension, ftype = self._pre_process_features(dataset)
+        if label is not None:
+            df = df.with_appended_column(alias.label,
+                                         [[b.column(label).cast(pa.float32()) for b in p] for p in dataset._parts])
+        return df, multi_col_names, dimension, ftype
+
+    def _pre_process_features(self, dataset: LocalDataFrame) -> Tuple[LocalDataFrame, Optional[List[str]], int, str]:
+        """The feature columns selected and cast -> (dataframe, multi_col_names, dimension, feature dtype)."""
         input_col, input_cols = self._get_input_columns()
         types = dict(dataset.dtypes)
         if input_col is not None:
@@ -508,8 +521,8 @@ class _CumlEstimator(EstimatorBase, _CumlCaller):
             return est._fit(dataset)
 
         def fitMultiple(self, dataset: LocalDataFrame, paramMaps: Sequence[Dict[Any, Any]]) -> Iterator[Tuple[int, "_CumlModel"]]:
-            """pyspark.ml.Estimator.fitMultiple: (index, model) per param map, one fit each — what the reference falls back
-            to for KMeans (`_enable_fit_multiple_in_single_pass` is False there, core.py:1172-1228)."""
+            """pyspark.ml.Estimator.fitMultiple: (index, model) per param map, one fit each (reference
+            core.py:1172-1228); _TunedEstimator replaces it for the estimators CrossValidator tunes."""
             for index, pm in enumerate(paramMaps):
                 yield index, self.copy(pm)._fit(dataset)
 
@@ -544,6 +557,60 @@ class _CumlEstimator(EstimatorBase, _CumlCaller):
     @classmethod
     def load(cls, path: str) -> "_CumlEstimator":
         return cls.read().load(path)
+
+
+class _ModelIterator:
+    """(index, model) pairs in map order; safe to share between the threads of pyspark's tuning loops."""
+
+    def __init__(self, models: List[Any]) -> None:
+        self._it = iter(enumerate(models))
+        self._lock = threading.Lock()
+
+    def __iter__(self) -> "_ModelIterator":
+        return self
+
+    def __next__(self) -> Tuple[int, Any]:
+        with self._lock:
+            return next(self._it)
+
+
+class _TunedEstimator(_CumlEstimator):
+    """An estimator whose fitMultiple fits a grid of param maps from one ingest when every map changes only
+    `_single_pass_params`.  The fit function then runs once per task over `_fit_grid`, one `_settings()` per map,
+    and returns one model row per map in map order."""
+
+    _single_pass_params: frozenset = frozenset()
+    _fit_grid: Optional[List[Dict[str, Any]]] = None
+
+    @abstractmethod
+    def _settings(self) -> Dict[str, Any]:
+        """What the fit function needs of one map, read from a copy of the estimator that carries the map."""
+        raise NotImplementedError
+
+    @classmethod
+    def _shares_ingest(cls, paramMaps: Sequence[Dict[Any, Any]]) -> bool:
+        """Whether fitMultiple fits these maps from one ingest: there are maps and each changes only
+        `_single_pass_params`."""
+        return bool(paramMaps) and all(p.name in cls._single_pass_params for pm in paramMaps for p in pm)
+
+    def fitMultiple(self, dataset: Any, paramMaps: Sequence[Dict[Any, Any]]) -> Iterator[Tuple[int, Any]]:
+        """(index, model) per param map, in map order; each model equals self.copy(map).fit(dataset), its cuml params
+        included.  When the maps share one ingest (_shares_ingest) a single fit serves them all; otherwise each map is
+        one fit."""
+        maps = list(paramMaps)
+        if not self._shares_ingest(maps):
+            return _ModelIterator([self.copy(pm)._fit(dataset) for pm in maps])
+        copies = [self.copy(pm) for pm in maps]
+        for c in copies:
+            c._validate_parameters()
+        est = self.copy()
+        est._fit_grid = [c._settings() for c in copies]
+        if est._use_cpu_fallback():
+            raise ValueError("a Spark Param without GPU support is set and spark_rapids_ml_b200 has no CPU fallback")
+        models = est._fit_internal(dataset, maps)
+        for m, c in zip(models, copies):
+            c._copy_cuml_params(m)
+        return _ModelIterator(models)
 
 
 TRANSFORM_GROUP_ROWS = 1 << 20    # rows per device pass of transform and evaluation ...
@@ -910,6 +977,23 @@ class _CumlModel(ModelBase, _CumlParams, _CumlCommon):
     if not HAVE_PYSPARK:   # pyspark.ml.Transformer.transform(dataset, params) -> self._transform(dataset) otherwise
         def transform(self, dataset: LocalDataFrame) -> LocalDataFrame:
             return self._transform(dataset)
+
+    # the model attributes that _combine turns into one list entry per model
+    _combined_attrs: Tuple[str, ...] = ()
+
+    @classmethod
+    def _combine(cls, models: List["_CumlModel"]) -> "_CumlModel":
+        """One model holding every model's `_combined_attrs`, for the single-pass evaluation (reference
+        classification.py:1557-1572); its other attributes and its params are the first model's."""
+        assert len(models) > 0 and all(isinstance(m, cls) for m in models)
+        first = models[0]
+        attrs = dict(first._get_model_attributes() or {})
+        for name in cls._combined_attrs:
+            attrs[name] = [m._get_model_attributes()[name] for m in models]
+        out = cls(**attrs)
+        first._copyValues(out)
+        first._copy_cuml_params(out)
+        return out
 
     def _transformEvaluate(self, dataset: Any, evaluator: Any, params: Optional[Dict[Any, Any]] = None) -> List[float]:
         """The evaluator's metric for every model of this (combined) model on a local frame, one device pass per

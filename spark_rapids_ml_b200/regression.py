@@ -23,15 +23,13 @@ evaluate() and summary raise NotImplementedError; loss="huber", solver="l-bfgs" 
 from __future__ import annotations
 
 import functools
-import threading
-from typing import Any, Callable, Dict, Iterator, List, Optional, Sequence, Tuple, Union
+from typing import Any, Callable, Dict, List, Optional, Tuple, Union
 
 import numpy as np
-import pyarrow as pa
 
-from .core import FitInputType, _CumlEstimator, _CumlModelWithPredictionCol, _DeviceModel, alias, param_alias
+from .core import FitInputType, _CumlModelWithPredictionCol, _DeviceModel, _TunedEstimator, param_alias
 from .params import HasFeaturesCol, HasFeaturesCols, HasLabelCol, HasPredictionCol, P, _CumlClass, _CumlParams
-from .sparkshim import LocalDataFrame, Param, Row, TypeConverters, keyword_only
+from .sparkshim import Param, Row, TypeConverters, keyword_only
 
 
 class LinearRegressionClass(_CumlClass):
@@ -152,32 +150,7 @@ class _LinearRegressionCumlParams(_CumlParams, _LinearRegressionParams, HasFeatu
         return self._set_params(predictionCol=value)
 
 
-# Params a fitMultiple map may change while every map is still solved from one pass over the data
-_SOLVER_PARAMS = frozenset(("regParam", "elasticNetParam", "maxIter", "tol", "fitIntercept", "standardization"))
-
-
-def _solver_settings(cuml_params: Dict[str, Any]) -> Dict[str, Any]:
-    return {"reg": float(cuml_params["alpha"]), "l1_ratio": float(cuml_params["l1_ratio"]),
-            "fit_intercept": bool(cuml_params["fit_intercept"]), "standardization": bool(cuml_params["normalize"]),
-            "max_iter": int(cuml_params["max_iter"]), "tol": float(cuml_params["tol"])}
-
-
-class _ModelIterator:
-    """(index, model) pairs in map order; safe to share between the threads of pyspark's tuning loops."""
-
-    def __init__(self, models: List[Any]) -> None:
-        self._it = iter(enumerate(models))
-        self._lock = threading.Lock()
-
-    def __iter__(self) -> "_ModelIterator":
-        return self
-
-    def __next__(self) -> Tuple[int, Any]:
-        with self._lock:
-            return next(self._it)
-
-
-class LinearRegression(LinearRegressionClass, _CumlEstimator, _LinearRegressionCumlParams):
+class LinearRegression(LinearRegressionClass, _TunedEstimator, _LinearRegressionCumlParams):
     """Linear regression on H100 under the squared loss: OLS (regParam = 0), ridge (elasticNetParam = 0), lasso
     (elasticNetParam = 1) and the elastic net in between, with or without an intercept and standardization.  One barrier
     task per GPU runs one pass over the device-resident partition (column sums, then a wgmma Gram pass and a fused
@@ -207,7 +180,16 @@ class LinearRegression(LinearRegressionClass, _CumlEstimator, _LinearRegressionC
         if self._input_kwargs.get("num_workers", None) is None:
             self._input_kwargs.pop("num_workers", None)
         self._set_params(**self._input_kwargs)
-        self._solver_grid: Optional[List[Dict[str, Any]]] = None
+
+    # every map is solved from one moments pass over the data
+    _single_pass_params = frozenset(("regParam", "elasticNetParam", "maxIter", "tol", "fitIntercept",
+                                     "standardization"))
+
+    def _settings(self) -> Dict[str, Any]:
+        cp = self.cuml_params
+        return {"reg": float(cp["alpha"]), "l1_ratio": float(cp["l1_ratio"]),
+                "fit_intercept": bool(cp["fit_intercept"]), "standardization": bool(cp["normalize"]),
+                "max_iter": int(cp["max_iter"]), "tol": float(cp["tol"])}
 
     def setMaxIter(self, value: int) -> "LinearRegression":
         return self._set_params(maxIter=value)
@@ -238,23 +220,14 @@ class LinearRegression(LinearRegressionClass, _CumlEstimator, _LinearRegressionC
 
     def _validate_parameters(self) -> None:
         super()._validate_parameters()
-        _check_solver_settings(_solver_settings(self.cuml_params))
+        _check_solver_settings(self._settings())
 
     def _fit_label_col(self) -> Optional[str]:
         return self.getLabelCol()
 
-    def _pre_process_data(self, dataset: LocalDataFrame) -> Tuple[LocalDataFrame, Optional[List[str]], int, str]:
-        """The feature columns as for every estimator, plus the label cast to float32 as alias.label."""
-        label = self.getLabelCol()
-        if label not in dataset.columns:
-            raise ValueError(f"label column '{label}' not found in {dataset.columns}")
-        df, multi_col_names, dimension, ftype = super()._pre_process_data(dataset)
-        df = df.with_appended_column(alias.label, [[b.column(label).cast(pa.float32()) for b in p] for p in dataset._parts])
-        return df, multi_col_names, dimension, ftype
-
     def _get_cuml_fit_func(self, dataset: Any, extra_params: Optional[List[Dict[str, Any]]] = None
                            ) -> Callable[[FitInputType, Dict[str, Any]], Dict[str, Any]]:
-        grid = self._solver_grid if self._solver_grid is not None else [_solver_settings(self.cuml_params)]
+        grid = self._fit_grid or [self._settings()]
 
         def _cuml_fit(dfs: FitInputType, params: Dict[str, Any]) -> Dict[str, Any]:
             # stands in for LinearRegressionMG / RidgeMG / CDMG(handle, ...).fit(...) and the coefficient rescaling —
@@ -285,27 +258,10 @@ class LinearRegression(LinearRegressionClass, _CumlEstimator, _LinearRegressionC
         return LinearRegressionModel(coef_=list(r["coef_"]), intercept_=float(r["intercept_"]), n_cols=int(r["n_cols"]),
                                      dtype=str(r["dtype"]))
 
-    def _enable_fit_multiple_in_single_pass(self) -> bool:
-        return True
-
     def _supportsTransformEvaluate(self, evaluator: Any) -> bool:
         from .core import _supports_transform_evaluate
 
         return _supports_transform_evaluate(False, evaluator)
-
-    def fitMultiple(self, dataset: Any, paramMaps: Sequence[Dict[Any, Any]]) -> Iterator[Tuple[int, Any]]:
-        """(index, model) per param map, in map order.  When every map changes only solver params (regParam,
-        elasticNetParam, maxIter, tol, fitIntercept, standardization), one pass over the data serves all maps;
-        otherwise each map is one fit."""
-        if paramMaps and all(p.name in _SOLVER_PARAMS for pm in paramMaps for p in pm):
-            est = self.copy()
-            est._solver_grid = [_solver_settings(self.copy(pm).cuml_params) for pm in paramMaps]
-            for s in est._solver_grid:
-                _check_solver_settings(s)
-            if est._use_cpu_fallback():
-                raise ValueError("a Spark Param without GPU support is set and spark_rapids_ml_b200 has no CPU fallback")
-            return _ModelIterator(est._fit_internal(dataset, list(paramMaps)))
-        return _ModelIterator([self.copy(pm)._fit(dataset) for pm in paramMaps])
 
 
 def _check_solver_settings(s: Dict[str, Any]) -> None:
@@ -365,19 +321,7 @@ class LinearRegressionModel(LinearRegressionClass, _CumlModelWithPredictionCol, 
     def _out_schema(self, input_schema: Any = None) -> str:
         return "double"
 
-    @classmethod
-    def _combine(cls, models: List["LinearRegressionModel"]) -> "LinearRegressionModel":
-        """One model holding several fits' coefficients, for the single-pass evaluation (reference
-        classification.py:1557-1572 does this for logistic regression)."""
-        assert len(models) > 0 and all(isinstance(m, cls) for m in models)
-        first = models[0]
-        attrs = dict(first._get_model_attributes() or {})
-        attrs["coef_"] = [list(m.coef_) for m in models]
-        attrs["intercept_"] = [float(m.intercept_) for m in models]
-        out = cls(**attrs)
-        first._copyValues(out)
-        first._copy_cuml_params(out)
-        return out
+    _combined_attrs = ("coef_", "intercept_")
 
     def _models(self) -> List[Tuple[List[float], float]]:
         if isinstance(self.intercept_, (list, tuple)):

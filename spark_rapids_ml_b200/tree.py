@@ -18,15 +18,14 @@ from __future__ import annotations
 
 import json
 import math
-from typing import Any, Callable, Dict, Iterator, List, Optional, Sequence, Tuple, Union
+from typing import Any, Callable, Dict, List, Optional, Tuple, Union
 
 import numpy as np
-import pyarrow as pa
 
-from .core import (FitInputType, _CumlEstimator, _CumlModelWithPredictionCol, _DeviceModel, _no_spark_transform, alias,
+from .core import (FitInputType, _CumlModelWithPredictionCol, _DeviceModel, _TunedEstimator, _no_spark_transform,
                    param_alias)
 from .params import HasFeaturesCol, HasFeaturesCols, HasLabelCol, HasPredictionCol, P, _CumlClass, _CumlParams
-from .sparkshim import LocalDataFrame, Param, Row, TypeConverters
+from .sparkshim import Param, Row, TypeConverters
 
 MAX_DEPTH = 16          # b2k_rf_fit's limit
 MAX_BINS = (2, 256)     # bins are uint8
@@ -211,12 +210,7 @@ def features_per_node(strategy: str, d: int, n_trees: int, classification: bool)
     raise ValueError(f"featureSubsetStrategy given invalid value {strategy}")
 
 
-# Params a fitMultiple map may change while every map is still fitted from one ingest
-_FOREST_PARAMS = frozenset(("maxDepth", "maxBins", "minInstancesPerNode", "minInfoGain", "impurity", "numTrees",
-                            "featureSubsetStrategy", "bootstrap", "seed"))
-
-
-class _RandomForestEstimator(_RandomForestClass, _CumlEstimator, _RandomForestCumlParams):
+class _RandomForestEstimator(_RandomForestClass, _TunedEstimator, _RandomForestCumlParams):
     """The shared estimator: one barrier task per GPU ingests its partition; b2k_rf_fit grows every tree over all
     partitions' rows."""
 
@@ -233,7 +227,10 @@ class _RandomForestEstimator(_RandomForestClass, _CumlEstimator, _RandomForestCu
         self._set_params(**kwargs)
         if "n_streams" not in kwargs:
             self._set_cuml_value("n_streams", 1)
-        self._fit_grid: Optional[List[Dict[str, Any]]] = None
+
+    # every map is fitted from one ingest, with its own label pass and histogram passes
+    _single_pass_params = frozenset(("maxDepth", "maxBins", "minInstancesPerNode", "minInfoGain", "impurity",
+                                     "numTrees", "featureSubsetStrategy", "bootstrap", "seed"))
 
     def _is_classification(self) -> bool:
         raise NotImplementedError
@@ -291,18 +288,9 @@ class _RandomForestEstimator(_RandomForestClass, _CumlEstimator, _RandomForestCu
     def _fit_label_col(self) -> Optional[str]:
         return self.getLabelCol()
 
-    def _pre_process_data(self, dataset: LocalDataFrame) -> Tuple[LocalDataFrame, Optional[List[str]], int, str]:
-        """The feature columns as for every estimator, plus the label cast to float32 as alias.label."""
-        label = self.getLabelCol()
-        if label not in dataset.columns:
-            raise ValueError(f"label column '{label}' not found in {dataset.columns}")
-        df, multi_col_names, dimension, ftype = super()._pre_process_data(dataset)
-        df = df.with_appended_column(alias.label, [[b.column(label).cast(pa.float32()) for b in p] for p in dataset._parts])
-        return df, multi_col_names, dimension, ftype
-
     def _get_cuml_fit_func(self, dataset: Any, extra_params: Optional[List[Dict[str, Any]]] = None
                            ) -> Callable[[FitInputType, Dict[str, Any]], Dict[str, Any]]:
-        grid = self._fit_grid if self._fit_grid is not None else [self._settings()]
+        grid = self._fit_grid or [self._settings()]
         classification = self._is_classification()
 
         def _rf_fit(dfs: FitInputType, params: Dict[str, Any]) -> Dict[str, Any]:
@@ -336,9 +324,6 @@ class _RandomForestEstimator(_RandomForestClass, _CumlEstimator, _RandomForestCu
     def _require_nccl_ucx(self) -> Tuple[bool, bool]:
         return (True, False)
 
-    def _enable_fit_multiple_in_single_pass(self) -> bool:
-        return True
-
     def _supportsTransformEvaluate(self, evaluator: Any) -> bool:
         from .core import _supports_transform_evaluate
 
@@ -353,21 +338,6 @@ class _RandomForestEstimator(_RandomForestClass, _CumlEstimator, _RandomForestCu
         if self._is_classification():
             kw["num_classes"] = int(r["num_classes"])
         return self._model_class()(**kw)
-
-    def fitMultiple(self, dataset: Any, paramMaps: Sequence[Dict[Any, Any]]) -> Iterator[Tuple[int, Any]]:
-        """(index, model) per param map, in map order.  When every map changes only forest params, one ingest serves all
-        maps (each runs its own label pass and histogram passes); otherwise each map is one fit."""
-        from .regression import _ModelIterator
-
-        if paramMaps and all(p.name in _FOREST_PARAMS for pm in paramMaps for p in pm):
-            est = self.copy()
-            est._fit_grid = [self.copy(pm)._settings() for pm in paramMaps]
-            for s in est._fit_grid:
-                _check_settings(s)
-            if est._use_cpu_fallback():
-                raise ValueError("a Spark Param without GPU support is set and spark_rapids_ml_b200 has no CPU fallback")
-            return _ModelIterator(est._fit_internal(dataset, list(paramMaps)))
-        return _ModelIterator([self.copy(pm)._fit(dataset) for pm in paramMaps])
 
 
 def _check_settings(s: Dict[str, Any]) -> None:
@@ -533,16 +503,7 @@ class _RandomForestModel(_RandomForestClass, _CumlModelWithPredictionCol, _Rando
             return vals
         return DenseVector(list(vals))
 
-    @classmethod
-    def _combine(cls, models: List[Any]) -> Any:
-        assert len(models) > 0 and all(isinstance(m, cls) for m in models)
-        first = models[0]
-        attrs = dict(first._get_model_attributes() or {})
-        attrs["model_json"] = [m._model_json for m in models]
-        out = cls(**attrs)
-        first._copyValues(out)
-        first._copy_cuml_params(out)
-        return out
+    _combined_attrs = ("model_json",)
 
     def _out_schema(self, input_schema: Any = None) -> str:
         return "double"

@@ -21,7 +21,7 @@ import numpy as np
 import pyarrow as pa
 
 from .core import (FitInputType, _CumlEstimator, _CumlModelWithColumns, _DeviceModel, _save_metadata, _load_metadata,
-                   _reset_uid, _set_params_from_metadata, alias, param_alias)
+                   _reset_uid, _set_params_from_metadata, param_alias)
 from .params import HasFeaturesCol, HasFeaturesCols, HasLabelCol, HasOutputCol, P, _CumlClass, _CumlParams
 from .sparkshim import HAVE_PYSPARK, Param, TypeConverters, keyword_only
 from .utils import get_logger
@@ -270,16 +270,6 @@ class UMAP(UMAPClass, _CumlEstimator, _UMAPCumlParams):
 
     def _fit_label_col(self) -> Optional[str]:
         return self.getOrDefault("labelCol") if self.isDefined(self.labelCol) and self.isSet(self.labelCol) else None
-
-    def _pre_process_data(self, dataset: Any) -> Tuple[Any, Optional[List[str]], int, str]:
-        df, multi_col_names, dimension, ftype = super()._pre_process_data(dataset)
-        label = self._fit_label_col()
-        if label is not None:
-            if label not in dataset.columns:
-                raise ValueError(f"label column '{label}' not found in {dataset.columns}")
-            df = df.with_appended_column(alias.label,
-                                         [[b.column(label).cast(pa.float32()) for b in p] for p in dataset._parts])
-        return df, multi_col_names, dimension, ftype
 
     @property
     def num_workers(self) -> int:

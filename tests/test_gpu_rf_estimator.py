@@ -72,7 +72,8 @@ def test_regressor_end_to_end_and_fit_multiple(tmp_path):
     models = dict(est.fitMultiple(df, maps))
     for i, pm in enumerate(maps):
         single = est.copy(pm)
-        assert models[i]._model_json == single.fit(df)._model_json
+        one = single.fit(df)
+        assert models[i]._model_json == one._model_json and models[i].cuml_params == one.cuml_params
         ref = _oracle(X, y, single, False)
         rows = models[i].transform(df).collect()
         np.testing.assert_array_equal(np.array([r["prediction"] for r in rows]), ro.predict(X, ref, False)[2])

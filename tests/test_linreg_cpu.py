@@ -346,6 +346,7 @@ res["single_pass_moments_calls"] = len(CALLS_MOMENTS)
 singles = [lr.copy(pm).fit(df) for pm in maps]
 res["same_as_single_fits"] = all(models[i].coef_ == s.coef_ and models[i].intercept_ == s.intercept_
                                  and models[i].getRegParam() == s.getRegParam() for i, s in enumerate(singles))
+res["same_cuml_params"] = [models[i].cuml_params == s.cuml_params for i, s in enumerate(singles)]
 del CALLS_MOMENTS[:]
 models = dict(lr.fitMultiple(df, [{lr.labelCol: "target"}, {lr.maxIter: 3}]))
 res["fallback_moments_calls"] = len(CALLS_MOMENTS)
@@ -371,6 +372,7 @@ def test_local_frames_carry_the_label_and_fit_multiple_takes_one_pass_with_core_
     assert res["coef_err"] < 1e-9 and res["b_err"] < 1e-9, res
     assert res["pred_err"] < 1e-9 and res["pred_is_double"] == "double", res
     assert res["single_pass_moments_calls"] == 1 and res["same_as_single_fits"], res
+    assert all(res["same_cuml_params"]), res
     assert res["fallback_moments_calls"] == 2, res
     assert "label column 'nope' not found" in res["missing_label"], res
 

@@ -340,6 +340,7 @@ res["single_pass_calls"] = dict(CALLS)
 singles = [lr.copy(pm).fit(df) for pm in maps]
 res["same_as_single_fits"] = all(models[i].coef_ == s.coef_ and models[i].intercept_ == s.intercept_
                                  and models[i].getRegParam() == s.getRegParam() for i, s in enumerate(singles))
+res["same_cuml_params"] = [models[i].cuml_params == s.cuml_params for i, s in enumerate(singles)]
 try:
     LogisticRegression(labelCol="nope").fit(df)
 except ValueError as e:
@@ -365,6 +366,7 @@ def test_estimator_end_to_end_on_local_frames_with_core_context_stub():
     assert res["multi"][0] == 3 and res["multi"][1] == 3 and res["multi"][2] == [0.0, 1.0, 2.0], res
     assert set(res["multi_pred"]) <= {0.0, 1.0, 2.0}, res
     assert res["single_pass_calls"] == {"labels": 1, "fit": 1} and res["same_as_single_fits"], res
+    assert all(res["same_cuml_params"]), res
     assert "label column 'nope' not found" in res["missing_label"], res
 
 
