@@ -49,6 +49,8 @@
  *   b2k_silhouette              none: the reference has no clustering evaluator (its DBSCAN benchmark collects the
  *                               frame and calls scikit-learn's silhouette_score); stands in for Spark's
  *                               pyspark.ml.evaluation.ClusteringEvaluator (metricName "silhouette")
+ *   b2k_gmm_fit / _predict      none: the reference has no Gaussian mixture; stands in for Spark's
+ *                               pyspark.ml.clustering.GaussianMixture (fit and GaussianMixtureModel.transform)
  *   b2k_silhouette_multi        none: the reference tunes KMeans with pyspark's CrossValidator, scoring each model on
  *                               the CPU; here one device pass scores every model of a param grid
  *
@@ -836,6 +838,49 @@ int b2k_umap_graph(b2k_ctx* ctx, int64_t* knn_idx, float* knn_dist, double* rho,
  * component gets a NaN row. */
 int b2k_umap_transform(b2k_ctx* ctx, const float* X_train, const float* embedding, int64_t n_train, int d, const float* Q,
                        int64_t nq, const b2k_umap_params* params, float* out, uintptr_t stream);
+
+/* ---- Gaussian mixtures (full covariances, EM) ----
+ * Stands in for pyspark.ml.clustering.GaussianMixture (the reference has no Gaussian mixture).  Model: weights w_k,
+ * means mu_k, covariances Sigma_k, fp64.  Densities follow Spark's MultivariateGaussian, so a singular covariance is
+ * legal: Sigma_k = U diag(lambda) U^T, tol = EPS max(lambda) d with EPS = 2.220446e-16, P_k = diag(lambda_j > tol ?
+ * lambda_j^-1/2 : 0) U^T and log pdf_k(x) = -(d log 2 pi + sum_{lambda_j > tol} log lambda_j) / 2 - ||P_k (x - mu_k)||^2
+ * / 2; a covariance with no eigenvalue above tol is an error.
+ *
+ * b2k_gmm_fit (collective): X device f32 [n_local, d].  E-step per row: p_ik = w_k pdf_k(x_i) + EPS (MLlib's EM),
+ * r_ik = p_ik / sum_j p_ij, LL = sum_i log sum_j p_ij over all rows of all ranks.  M-step: N_k = sum_i r_ik,
+ * w_k = N_k / n, mu_k = sum r_ik x_i / N_k, Sigma_k = sum r_ik (x_i - mu_k)(x_i - mu_k)^T / N_k; the device sums are
+ * taken about c = fl32(column means) and the host removes c in fp64.  One f64 allreduce per iteration.  Stops when
+ * iter == max_iter or |LL - LL_prev| <= tol; *log_likelihood_out = the LL of the last E-step (-inf when max_iter = 0).
+ * init_mode B2K_INIT_ARRAY: the start is init_weights [k], init_means [k][d], init_covs [k][d][d] (host f64);
+ * B2K_INIT_RANDOM: weights 1/k, and component i takes the mean and the biased per-feature variance (a diagonal
+ * covariance) of global rows g_{5i} .. g_{5i+4}, g_j = splitmix64(seed ^ splitmix64(j)) mod n_total, the global row
+ * order being rank 0's rows, then rank 1's, and so on (splitmix64: z += 0x9e3779b97f4a7c15, z = (z ^ z >> 30)
+ * 0xbf58476d1ce4e5b9, z = (z ^ z >> 27) 0x94d049bb133111eb, z ^ z >> 31).  Outputs (host): weights_out [k], means_out
+ * [k][d], covs_out [k][d][d], *n_iter_out, cluster_sizes_out [k] = argmax counts of b2k_gmm_predict with the final
+ * model over all ranks.  E pass on wgmma (3xTF32) for d % 4 == 0, 4 <= d <= 128, k <= 64 and a 16-byte aligned X,
+ * else on a generic fp64 SIMT pass; option "kernel_path" = B2K_PATH_GENERIC forces the generic pass, B2K_PATH_FUSED
+ * fails with B2K_ERR_UNSUPPORTED where wgmma cannot run (decided on every rank together).  The weighted Gram pass of the
+ * M-step runs on wgmma (3xTF32, fp64 partials) for d % 4 == 0 and a 16-byte aligned X, else on an fp64 SIMT pass, and
+ * kernel_path = B2K_PATH_GENERIC forces that pass too; the moments pass is fp64 SIMT.  Errors, decided on allgathered or
+ * allreduced values so that every rank fails together (B2K_ERR_INVALID unless noted): an empty partition on any rank;
+ * a NaN or an infinity in X; k < 2; k > n_total; d < 1; max_iter < 0; tol < 0; a covariance with no eigenvalue above
+ * tol; d > 256, k > 256 or k d^2 > 2^24, more than 2^31 - 256 rows on a rank (B2K_ERR_UNSUPPORTED).  Synchronises `stream`.  Bitwise reproducible for the
+ * same input, rank count and device.  Stats: last_path = the E pass that ran; last_n_iter; with option "time_kernels"
+ * != 0, last_fused_ms = the E passes, last_reduce_ms = the M passes, last_allreduce_ms = the allreduces (device times,
+ * summed over the iterations), last_finalize_ms = the host updates (the eigendecompositions and the model uploads
+ * included) and last_loop_ms = the whole call (host clock). */
+#define B2K_GMM_MAX_D 256
+#define B2K_GMM_MAX_K 256
+int b2k_gmm_fit(b2k_ctx* ctx, const float* X, int64_t n_local, int d, int k, int init_mode, const double* init_weights,
+                const double* init_means, const double* init_covs, int max_iter, double tol, uint64_t seed,
+                double* weights_out, double* means_out, double* covs_out, double* log_likelihood_out, int* n_iter_out,
+                int64_t* cluster_sizes_out, uintptr_t stream);
+/* Local (no collective): per row of X [n, d] the probabilities prob_out [n][k] (device f64, r_ik of the E-step above)
+ * and labels_out [n] (device int32, the first argmax), with the model weights [k], means [k][d], covs [k][d][d] (host
+ * f64).  Rows are read about fl32(sum_k w_k mu_k), so a row's result depends on that row and the model alone.  Same
+ * passes, bounds and errors as b2k_gmm_fit's E-step.  Synchronises `stream`. */
+int b2k_gmm_predict(b2k_ctx* ctx, const float* X, int64_t n, int d, int k, const double* weights, const double* means,
+                    const double* covs, double* prob_out, int32_t* labels_out, uintptr_t stream);
 
 #ifdef __cplusplus
 }

@@ -82,6 +82,8 @@ EXPORTED_SYMBOLS = (
     "b2k_umap_transform",
     "b2k_silhouette",
     "b2k_silhouette_multi",
+    "b2k_gmm_fit",
+    "b2k_gmm_predict",
 )
 
 EVAL_KINDS = {"identity": 0, "logistic": 1, "softmax": 2}
@@ -270,6 +272,9 @@ def load_library() -> ctypes.CDLL:
     L.b2k_umap_transform.argtypes = [vp, vp, vp, i64, i32, vp, i64, ctypes.POINTER(UmapParams), vp, ctypes.c_size_t]
     L.b2k_silhouette.argtypes = [vp, vp, i64, i32, vp, i32, ctypes.POINTER(f64), ctypes.c_size_t]
     L.b2k_silhouette_multi.argtypes = [vp, vp, i64, i32, i32, vp, i32, vp, ctypes.c_size_t]
+    L.b2k_gmm_fit.argtypes = [vp, vp, i64, i32, i32, i32, vp, vp, vp, i32, f64, u64, vp, vp, vp, ctypes.POINTER(f64),
+                              ctypes.POINTER(i32), vp, ctypes.c_size_t]
+    L.b2k_gmm_predict.argtypes = [vp, vp, i64, i32, i32, vp, vp, vp, vp, vp, ctypes.c_size_t]
     for name in EXPORTED_SYMBOLS:
         if name not in ("b2k_last_error",):
             getattr(L, name).restype = i32
@@ -691,6 +696,56 @@ class Context:
                                                    out.data_ptr(), self._stream()))
         t.cuda.current_stream(self.device).synchronize()  # w (possibly a temporary) must outlive the kernel
         return out
+
+    # -- Gaussian mixtures ------------------------------------------------------------------
+    def gmm_fit(self, X: Any, k: int, *, init: Optional[Tuple[Any, Any, Any]] = None, max_iter: int = 100,
+                tol: float = 0.01, seed: int = 0) -> Dict[str, Any]:
+        """GaussianMixture.fit (b2k_gmm_fit, collective when a communicator is initialised).  init = None draws the
+        start from `seed`, or (weights [k], means [k, d], covariances [k, d, d]) starts from those values.  Returns host
+        float64 arrays weights [k], means [k, d], covs [k, d, d], int64 cluster_sizes [k], and log_likelihood, n_iter."""
+        n, d = self._check_X(X)
+        kk = max(int(k), 0)
+        if init is None:
+            mode, iw, im, ic = INIT_RANDOM, None, None, None
+        else:
+            iw = np.ascontiguousarray(init[0], dtype=np.float64).reshape(-1)
+            im = np.ascontiguousarray(init[1], dtype=np.float64)
+            ic = np.ascontiguousarray(init[2], dtype=np.float64)
+            if iw.shape != (kk,) or im.shape != (kk, d) or ic.shape != (kk, d, d):
+                raise ValueError(f"init must be (weights [{kk}], means [{kk}, {d}], covariances [{kk}, {d}, {d}])")
+            mode = INIT_ARRAY
+        w = np.zeros(kk, dtype=np.float64)
+        mu = np.zeros((kk, d), dtype=np.float64)
+        cov = np.zeros((kk, d, d), dtype=np.float64)
+        sizes = np.zeros(kk, dtype=np.int64)
+        ll = ctypes.c_double(0.0)
+        n_iter = ctypes.c_int(0)
+        ptr = lambda a: a.ctypes.data if a is not None else None   # noqa: E731
+        with self._torch.cuda.device(self.device):
+            self._check(self._L.b2k_gmm_fit(
+                self._h, X.data_ptr(), n, d, int(k), mode, ptr(iw), ptr(im), ptr(ic), int(max_iter), float(tol),
+                int(seed) & 0xFFFFFFFFFFFFFFFF, w.ctypes.data, mu.ctypes.data, cov.ctypes.data, ctypes.byref(ll),
+                ctypes.byref(n_iter), sizes.ctypes.data, self._stream()))
+        return {"weights": w, "means": mu, "covs": cov, "cluster_sizes": sizes, "log_likelihood": float(ll.value),
+                "n_iter": int(n_iter.value)}
+
+    def gmm_predict(self, X: Any, weights: Any, means: Any, covs: Any) -> Tuple[Any, Any]:
+        """Per row of X: the float64 probabilities [n, k] and the int32 argmax [n] of a Gaussian mixture (CUDA
+        tensors)."""
+        t = self._torch
+        n, d = self._check_X(X)
+        w = np.ascontiguousarray(weights, dtype=np.float64).reshape(-1)
+        k = int(w.shape[0])
+        mu = np.ascontiguousarray(means, dtype=np.float64)
+        cov = np.ascontiguousarray(covs, dtype=np.float64)
+        if mu.shape != (k, d) or cov.shape != (k, d, d):
+            raise ValueError(f"means must be [{k}, {d}] and covariances [{k}, {d}, {d}]")
+        prob = t.empty((n, k), dtype=t.float64, device=self.device)
+        labels = t.empty((n,), dtype=t.int32, device=self.device)
+        with t.cuda.device(self.device):
+            self._check(self._L.b2k_gmm_predict(self._h, X.data_ptr(), n, d, k, w.ctypes.data, mu.ctypes.data,
+                                                cov.ctypes.data, prob.data_ptr(), labels.data_ptr(), self._stream()))
+        return prob, labels
 
     # -- logistic regression ----------------------------------------------------------------
     def _check_y(self, y: Any, n: int) -> None:

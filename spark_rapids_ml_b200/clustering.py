@@ -570,3 +570,261 @@ class DBSCANModel(DBSCANClass, _CumlModelWithPredictionCol, _CumlCaller, _DBSCAN
                 arrs.append(pa.array(got[np.searchsorted(got_ids, ids)], type=pa.int32()))
             out_parts.append(arrs)
         return dataset.with_appended_column(self._get_prediction_name(), out_parts)
+
+
+# ---- GaussianMixture (pyspark.ml.clustering.GaussianMixture; the reference has no Gaussian mixture) ----
+class GaussianMixtureClass(_CumlClass):
+    @classmethod
+    def _param_mapping(cls) -> Dict[str, Optional[str]]:
+        # None = unsupported, "" = accepted and ignored
+        return {"k": "n_components", "maxIter": "max_iter", "tol": "tol", "seed": "random_state",
+                "aggregationDepth": "", "weightCol": None}
+
+    def _get_cuml_params_default(self) -> Dict[str, Any]:
+        return {"n_components": 2, "max_iter": 100, "tol": 0.01, "random_state": None, "verbose": False}
+
+    def _pyspark_class(self) -> Optional[type]:
+        return None  # pyspark.ml.clustering.GaussianMixture when pyspark is installed
+
+
+class _GaussianMixtureCumlParams(_CumlParams, HasFeaturesCol, HasFeaturesCols, HasPredictionCol):
+    """Shared Spark Params of GaussianMixture and GaussianMixtureModel (Spark's defaults: k=2, maxIter=100, tol=0.01,
+    probabilityCol='probability', aggregationDepth=2)."""
+
+    k = Param("parent", "k", "Number of independent Gaussians in the mixture model. Must be > 1.", TypeConverters.toInt)
+    maxIter = Param("parent", "maxIter", "max number of iterations (>= 0).", TypeConverters.toInt)
+    tol = Param("parent", "tol", "the convergence tolerance for iterative algorithms (>= 0).", TypeConverters.toFloat)
+    seed = Param("parent", "seed", "random seed.", TypeConverters.toInt)
+    probabilityCol = Param("parent", "probabilityCol", "Column name for predicted class conditional probabilities.",
+                           TypeConverters.toString)
+    aggregationDepth = Param("parent", "aggregationDepth", "suggested depth for treeAggregate (>= 2).",
+                             TypeConverters.toInt)
+    weightCol = Param("parent", "weightCol", "weight column name.", TypeConverters.toString)
+
+    def __init__(self) -> None:
+        super().__init__()
+        self._setDefault(k=2, maxIter=100, tol=0.01, probabilityCol="probability", aggregationDepth=2)
+        # the KMeans rule: a 32-bit signed seed from the class name
+        self._setDefault(seed=hash(type(self).__name__) & 0x07FFFFFFF)
+
+    def getK(self) -> int:
+        return self.getOrDefault(self.k)
+
+    def getMaxIter(self) -> int:
+        return self.getOrDefault(self.maxIter)
+
+    def getTol(self) -> float:
+        return self.getOrDefault(self.tol)
+
+    def getSeed(self) -> int:
+        return self.getOrDefault(self.seed)
+
+    def getProbabilityCol(self) -> str:
+        return self.getOrDefault(self.probabilityCol)
+
+    def getAggregationDepth(self) -> int:
+        return self.getOrDefault(self.aggregationDepth)
+
+    def getFeaturesCol(self) -> Union[str, List[str]]:  # type: ignore[override]
+        if self.isDefined(self.featuresCols):
+            return self.getFeaturesCols()
+        if self.isDefined(self.featuresCol):
+            return self.getOrDefault("featuresCol")
+        raise RuntimeError("featuresCol is not set")
+
+    def setFeaturesCol(self: P, value: Union[str, List[str]]) -> P:
+        if isinstance(value, str):
+            self._set_params(featuresCol=value)
+        else:
+            self._set_params(featuresCols=value)
+        return self
+
+    def setFeaturesCols(self: P, value: List[str]) -> P:
+        return self._set_params(featuresCols=value)
+
+    def setPredictionCol(self: P, value: str) -> P:
+        return self._set_params(predictionCol=value)
+
+    def setProbabilityCol(self: P, value: str) -> P:
+        return self._set_params(probabilityCol=value)
+
+
+class GaussianMixture(GaussianMixtureClass, _CumlEstimator, _GaussianMixtureCumlParams):
+    """Gaussian mixture models (full covariances) by EM on H100, Spark's pyspark.ml.clustering.GaussianMixture.  One
+    barrier task per GPU holds its partition on the device; each iteration is one E pass (the whitened quadratic forms
+    of every row and component, on wgmma 3xTF32 where the shape allows), a moments pass and a weighted Gram pass in
+    fp64, one NCCL allreduce and an fp64 update with one eigendecomposition per component on the host.  Parameters:
+    k (2), maxIter (100), tol (0.01, on the total log-likelihood), seed, featuresCol (str for an array column, list of
+    str for scalar columns), predictionCol, probabilityCol ("probability"), aggregationDepth (accepted, unused),
+    num_workers, verbose.  weightCol is not supported.
+
+    The start is Spark's rule (weights 1/k, the mean and diagonal variance of 5 sampled rows per component) with the
+    rows drawn by the library's own seeded generator, so it differs from Spark's for the same seed.
+
+    >>> from spark_rapids_ml_b200.clustering import GaussianMixture
+    >>> model = GaussianMixture(k=2, seed=1).fit(df)
+    >>> model.weights, model.summary.logLikelihood
+    """
+
+    @keyword_only
+    def __init__(self, *, featuresCol: Union[str, List[str]] = "features", predictionCol: str = "prediction",
+                 k: int = 2, probabilityCol: str = "probability", tol: float = 0.01, maxIter: int = 100,
+                 seed: Optional[int] = None, aggregationDepth: int = 2, weightCol: Optional[str] = None,
+                 num_workers: Optional[int] = None, verbose: Union[int, bool] = False, **kwargs: Any) -> None:
+        super().__init__()
+        self._handle_param_spark_confs()
+        self._input_kwargs.pop("kwargs", None)
+        self._input_kwargs.update(kwargs)
+        for name in ("seed", "num_workers", "weightCol"):
+            if self._input_kwargs.get(name, None) is None:
+                self._input_kwargs.pop(name, None)
+        if "weightCol" in self._input_kwargs:
+            raise ValueError("'weightCol' is not supported by GaussianMixture on the GPU.")
+        self._set_params(**self._input_kwargs)
+
+    def setK(self, value: int) -> "GaussianMixture":
+        return self._set_params(k=value)
+
+    def setMaxIter(self, value: int) -> "GaussianMixture":
+        return self._set_params(maxIter=value)
+
+    def setTol(self, value: float) -> "GaussianMixture":
+        return self._set_params(tol=value)
+
+    def setSeed(self, value: int) -> "GaussianMixture":
+        return self._set_params(seed=value)
+
+    def setAggregationDepth(self, value: int) -> "GaussianMixture":
+        return self._set_params(aggregationDepth=value)
+
+    def setWeightCol(self, value: str) -> "GaussianMixture":
+        raise ValueError("'weightCol' is not supported by GaussianMixture on the GPU.")
+
+    def _validate_parameters(self) -> None:
+        super()._validate_parameters()
+        k, max_iter, tol = self.getK(), self.getMaxIter(), self.getTol()
+        if isinstance(k, bool) or not isinstance(k, int) or k < 2:
+            raise ValueError(f"k given invalid value {k} (must be > 1)")
+        if max_iter < 0:
+            raise ValueError(f"maxIter given invalid value {max_iter} (must be >= 0)")
+        if not tol >= 0:
+            raise ValueError(f"tol given invalid value {tol} (must be >= 0)")
+
+    def _fit_array_order(self) -> str:
+        return "C"
+
+    def _get_cuml_fit_func(self, dataset: Any, extra_params: Optional[List[Dict[str, Any]]] = None
+                           ) -> Callable[[FitInputType, Dict[str, Any]], Dict[str, Any]]:
+        cls = self.__class__
+
+        def _cuml_fit(dfs: FitInputType, params: Dict[str, Any]) -> Dict[str, Any]:
+            ctx = params[param_alias.handle]
+            init = params[param_alias.cuml_init]
+            if len(dfs) != 1:
+                raise RuntimeError("the worker scaffold hands the fit function ONE device matrix per partition")
+            seed = init.get("random_state")
+            out = ctx.gmm_fit(dfs[0][0], int(init["n_components"]), max_iter=int(init["max_iter"]),
+                              tol=float(init["tol"]), seed=int(seed) if seed is not None else 0)
+            get_logger(cls).info(f"iterations: {out['n_iter']}, log-likelihood: {out['log_likelihood']}")
+            return {"weights_": [out["weights"].tolist()], "means_": [out["means"].tolist()],
+                    "covs_": [out["covs"].tolist()], "cluster_sizes_": [out["cluster_sizes"].tolist()],
+                    "log_likelihood_": [out["log_likelihood"]], "num_iters": [out["n_iter"]],
+                    "n_cols": [params[param_alias.num_cols]], "dtype": ["float32"]}
+
+        return _cuml_fit
+
+    def _out_schema(self) -> Any:
+        return ("weights_ array<double>, means_ array<array<double>>, covs_ array<array<array<double>>>, "
+                "cluster_sizes_ array<long>, log_likelihood_ double, num_iters int, n_cols int, dtype string")
+
+    def _create_pyspark_model(self, result: Row) -> "GaussianMixtureModel":
+        r = result.asDict()
+        return GaussianMixtureModel(
+            weights_=[float(v) for v in r["weights_"]], means_=[[float(v) for v in m] for m in r["means_"]],
+            covs_=[[[float(v) for v in row] for row in c] for c in r["covs_"]],
+            cluster_sizes_=[int(v) for v in r["cluster_sizes_"]], log_likelihood_=float(r["log_likelihood_"]),
+            num_iters=int(r["num_iters"]), n_cols=int(r["n_cols"]), dtype=str(r["dtype"]))
+
+
+class GaussianMixtureSummary:
+    """The training summary Spark's GaussianMixtureModel.summary holds: k, numIter, logLikelihood, clusterSizes."""
+
+    def __init__(self, k: int, num_iter: int, log_likelihood: float, cluster_sizes: List[int]) -> None:
+        self.k = k
+        self.numIter = num_iter
+        self.logLikelihood = log_likelihood
+        self.clusterSizes = cluster_sizes
+
+
+class GaussianMixtureModel(GaussianMixtureClass, _CumlModelWithPredictionCol, _GaussianMixtureCumlParams):
+    """transform() appends predictionCol (int, the most probable component, the lower one on a tie) and probabilityCol
+    (a double vector of the k component probabilities)."""
+
+    def __init__(self, weights_: List[float], means_: List[List[float]], covs_: List[List[List[float]]],
+                 cluster_sizes_: List[int], log_likelihood_: float, num_iters: int, n_cols: int, dtype: str) -> None:
+        super().__init__(n_cols=n_cols, dtype=dtype, weights_=weights_, means_=means_, covs_=covs_,
+                         cluster_sizes_=cluster_sizes_, log_likelihood_=log_likelihood_, num_iters=num_iters)
+        self.weights_ = weights_
+        self.means_ = means_
+        self.covs_ = covs_
+        self.cluster_sizes_ = cluster_sizes_
+        self.log_likelihood_ = log_likelihood_
+        self.num_iters = num_iters
+        self._set_params(k=len(weights_))
+
+    @property
+    def weights(self) -> List[float]:
+        return list(self.weights_)
+
+    @property
+    def gaussiansDF(self) -> Any:
+        """A local frame with one row per component: mean (a double vector) and cov (a [d, d] double matrix)."""
+        from .sparkshim import get_session
+
+        table = pa.table({
+            "mean": pa.array([list(m) for m in self.means_], type=pa.list_(pa.float64())),
+            "cov": pa.array([[list(r) for r in c] for c in self.covs_], type=pa.list_(pa.list_(pa.float64()))),
+        })
+        return get_session().createDataFrame(table)
+
+    @property
+    def hasSummary(self) -> bool:
+        return True
+
+    @property
+    def summary(self) -> GaussianMixtureSummary:
+        return GaussianMixtureSummary(len(self.weights_), int(self.num_iters), float(self.log_likelihood_),
+                                      list(self.cluster_sizes_))
+
+    def predict(self, value: Any) -> int:
+        raise NotImplementedError("GaussianMixtureModel.predict() of a single vector is not supported; use transform()")
+
+    def predictProbability(self, value: Any) -> Any:
+        raise NotImplementedError("GaussianMixtureModel.predictProbability() of a single vector is not supported; use "
+                                  "transform()")
+
+    def cpu(self) -> Any:
+        raise NotImplementedError("GaussianMixtureModel.cpu() builds a JVM pyspark.ml model; no JVM/pyspark in this "
+                                  "build")
+
+    def _out_schema(self, input_schema: Any = None) -> str:
+        return "int"
+
+    def _transform_outputs(self) -> List[Tuple[str, str]]:
+        return [(self.getOrDefault("predictionCol"), "int"), (self.getProbabilityCol(), "array<double>")]
+
+    def _transform_array_order(self) -> str:
+        return "C"
+
+    def _get_cuml_transform_func(self, dataset: Any, eval_metric_info: Any = None
+                                 ) -> Tuple[Callable, Callable, Optional[Callable]]:
+        w = np.asarray(self.weights_, dtype=np.float64)
+        mu = np.asarray(self.means_, dtype=np.float64)
+        cov = np.asarray(self.covs_, dtype=np.float64)
+
+        def _predict(m: Any, X: Any) -> Tuple[Any, Any]:
+            prob, labels = m.ctx.gmm_predict(X, w, mu, cov)
+            return labels, prob
+
+        k = len(self.weights_)
+        return _DeviceModel, self._grouped_transform(_predict, 4 * int(self.n_cols) + 8 * k + 4), None

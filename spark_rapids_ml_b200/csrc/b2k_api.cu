@@ -1343,3 +1343,112 @@ extern "C" int b2k_umap_transform(b2k_ctx* ctx, const float* X_train, const floa
   return b2k_umap_transform_impl(ctx, X_train, embedding, n_train, d, Q, nq, *params, out,
                                  reinterpret_cast<cudaStream_t>(stream));
 }
+
+// ------------------------------------------------------------------------------------------------
+// Gaussian mixtures (b2k_gmm.cu)
+// ------------------------------------------------------------------------------------------------
+namespace {
+uint64_t gmm_splitmix64(uint64_t z) {
+  z += 0x9e3779b97f4a7c15ull;
+  z = (z ^ (z >> 30)) * 0xbf58476d1ce4e5b9ull;
+  z = (z ^ (z >> 27)) * 0x94d049bb133111ebull;
+  return z ^ (z >> 31);
+}
+
+// Spark's start (GaussianMixture.scala: weights 1/k, the mean of 5 sampled rows and the diagonal of their biased
+// variance), with the rows drawn by a counter-based rule over the global row order, so that the start depends on
+// neither the rank count nor the split of the rows.
+constexpr int GMM_INIT_ROWS = 5;
+int gmm_random_init(b2k_ctx* ctx, const float* X, int64_t n_local, int d, int k, uint64_t seed, const Rows& rows,
+                    std::vector<double>* w, std::vector<double>* mu, std::vector<double>* cov, cudaStream_t s) {
+  const int m = k * GMM_INIT_ROWS;
+  std::vector<int64_t> draw(m);
+  for (int j = 0; j < m; ++j) draw[j] = (int64_t)(gmm_splitmix64(seed ^ gmm_splitmix64((uint64_t)j)) % (uint64_t)rows.total);
+  std::vector<int64_t> gidx(draw);
+  std::sort(gidx.begin(), gidx.end());
+  gidx.erase(std::unique(gidx.begin(), gidx.end()), gidx.end());
+  DevBuf b_out, b_idx;
+  float* out = nullptr;
+  int64_t* idx = nullptr;
+  B2K_TRY(dalloc(ctx, b_out, gidx.size() * d, s, &out));
+  B2K_TRY(dalloc(ctx, b_idx, gidx.size(), s, &idx));
+  B2K_TRY(fetch_global_rows(ctx, X, n_local, d, rows, gidx, out, idx, s));
+  std::vector<float> h(gidx.size() * d);
+  B2K_CUDA_OK(ctx, cudaMemcpyAsync(h.data(), out, h.size() * 4, cudaMemcpyDeviceToHost, s));
+  B2K_CUDA_OK(ctx, cudaStreamSynchronize(s));
+  w->assign(k, 1.0 / k);
+  mu->assign((size_t)k * d, 0.0);
+  cov->assign((size_t)k * d * d, 0.0);
+  for (int i = 0; i < k; ++i) {
+    const float* v[GMM_INIT_ROWS];
+    for (int t = 0; t < GMM_INIT_ROWS; ++t)
+      v[t] = h.data() + (size_t)(std::lower_bound(gidx.begin(), gidx.end(), draw[i * GMM_INIT_ROWS + t]) - gidx.begin()) * d;
+    for (int f = 0; f < d; ++f) {
+      double a = 0.0;
+      for (int t = 0; t < GMM_INIT_ROWS; ++t) a += (double)v[t][f];
+      a /= GMM_INIT_ROWS;
+      double q = 0.0;
+      for (int t = 0; t < GMM_INIT_ROWS; ++t) q += ((double)v[t][f] - a) * ((double)v[t][f] - a);
+      (*mu)[(size_t)i * d + f] = a;
+      (*cov)[((size_t)i * d + f) * d + f] = q / GMM_INIT_ROWS;
+    }
+  }
+  return B2K_OK;
+}
+}  // namespace
+
+extern "C" int b2k_gmm_fit(b2k_ctx* ctx, const float* X, int64_t n_local, int d, int k, int init_mode,
+                           const double* init_weights, const double* init_means, const double* init_covs, int max_iter,
+                           double tol, uint64_t seed, double* weights_out, double* means_out, double* covs_out,
+                           double* log_likelihood_out, int* n_iter_out, int64_t* cluster_sizes_out, uintptr_t stream) {
+  if (!ctx) return b2k_fail(nullptr, B2K_ERR_INVALID, "b2k_gmm_fit: ctx is NULL");
+  // an empty partition may come with no buffer: the collective check below reports it on every rank
+  if ((!X && n_local > 0) || n_local < 0 || !weights_out || !means_out || !covs_out || !log_likelihood_out ||
+      !n_iter_out || !cluster_sizes_out)
+    return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_gmm_fit: bad X/n/outputs");
+  if (d < 1) return b2k_fail(ctx, B2K_ERR_INVALID, "Gaussian mixture: d must be >= 1, got " + std::to_string(d));
+  if (k < 2) return b2k_fail(ctx, B2K_ERR_INVALID, "Gaussian mixture: k must be > 1, got " + std::to_string(k));
+  if (max_iter < 0)
+    return b2k_fail(ctx, B2K_ERR_INVALID, "Gaussian mixture: maxIter must be >= 0, got " + std::to_string(max_iter));
+  if (!(tol >= 0.0)) return b2k_fail(ctx, B2K_ERR_INVALID, "Gaussian mixture: tol must be >= 0");
+  if (init_mode != B2K_INIT_ARRAY && init_mode != B2K_INIT_RANDOM)
+    return b2k_fail(ctx, B2K_ERR_INVALID, "Gaussian mixture: init_mode must be B2K_INIT_ARRAY or B2K_INIT_RANDOM");
+  if (init_mode == B2K_INIT_ARRAY && (!init_weights || !init_means || !init_covs))
+    return b2k_fail(ctx, B2K_ERR_INVALID, "Gaussian mixture: B2K_INIT_ARRAY needs init_weights/init_means/init_covs");
+  if (d > B2K_GMM_MAX_D || k > B2K_GMM_MAX_K || (int64_t)k * d * d > ((int64_t)1 << 24))
+    return b2k_fail(ctx, B2K_ERR_UNSUPPORTED, "Gaussian mixture supports d <= 256, k <= 256 and k d^2 <= 2^24, got d = " +
+                                                  std::to_string(d) + ", k = " + std::to_string(k));
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  B2K_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  Rows rows;
+  B2K_TRY(gather_sizes(ctx, n_local, &rows, s));
+  for (int r = 0; r < ctx->nranks; ++r)
+    if (rows.sizes[r] == 0)
+      return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_gmm_fit: empty partition (rank " + std::to_string(r) +
+                                                " has n_local == 0)");
+  if (k > rows.total)
+    return b2k_fail(ctx, B2K_ERR_INVALID, "Gaussian mixture: k = " + std::to_string(k) + " exceeds the " +
+                                              std::to_string(rows.total) + " rows");
+  std::vector<double> w, mu, cov;
+  if (init_mode == B2K_INIT_ARRAY) {
+    w.assign(init_weights, init_weights + k);
+    mu.assign(init_means, init_means + (size_t)k * d);
+    cov.assign(init_covs, init_covs + (size_t)k * d * d);
+  } else {
+    B2K_TRY(gmm_random_init(ctx, X, n_local, d, k, seed, rows, &w, &mu, &cov, s));
+  }
+  return b2k_gmm_fit_impl(ctx, X, n_local, d, k, std::move(w), std::move(mu), std::move(cov), max_iter, tol,
+                          weights_out, means_out, covs_out, log_likelihood_out, n_iter_out, cluster_sizes_out, s);
+}
+
+extern "C" int b2k_gmm_predict(b2k_ctx* ctx, const float* X, int64_t n, int d, int k, const double* weights,
+                               const double* means, const double* covs, double* prob_out, int32_t* labels_out,
+                               uintptr_t stream) {
+  if (!ctx) return b2k_fail(nullptr, B2K_ERR_INVALID, "b2k_gmm_predict: ctx is NULL");
+  if (n < 0 || d < 1 || k < 1 || !weights || !means || !covs || (n > 0 && (!X || !prob_out || !labels_out)))
+    return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_gmm_predict: bad X/model/outputs/n/d/k");
+  if (n == 0) return B2K_OK;
+  B2K_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  return b2k_gmm_predict_impl(ctx, X, n, d, k, weights, means, covs, prob_out, labels_out,
+                              reinterpret_cast<cudaStream_t>(stream));
+}

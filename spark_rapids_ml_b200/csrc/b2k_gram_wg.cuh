@@ -1,5 +1,12 @@
 // Gram matrix of the centred data on wgmma (sm_90a, 3xTF32): G = sum_rows (x - mu)^T (x - mu), the upper block triangle
-// of 128 x 128 feature blocks.  Included inside the anonymous namespace of b2k_pca.cu after b2k_ptx.cuh.
+// of 128 x 128 feature blocks.  Included inside the anonymous namespace of b2k_pca.cu (k_gram_wg) and of b2k_gmm.cu
+// (k_gmm_gram_wg) after b2k_ptx.cuh; each defines its kernel over gram_wg_body.
+//
+// Weighted variant (W = true, Gaussian mixtures): G_c = sum_rows r_rc (x - mu)^T (x - mu) for each component c of a
+// row weight table r [n][K] (fp64).  Each row's centred fp32 value is multiplied by fl32(sqrt(fl32(r_rc))) before the
+// split, in both operands, so the product carries r_rc.  The grid is a multiple of K * ntile: CTA b owns component
+// (b % (K ntile)) / ntile and tile b % ntile, so the K ntile CTAs of one p read the same row range at the same time and
+// it is fetched from HBM about once per pass.  W = false is the unweighted pass above, unchanged.
 //
 // Work: tile t = (I, J), I <= J, is the product of feature block I (wgmma M, 64 per consumer warpgroup) and feature block
 // J (wgmma N = 128); the contraction runs over rows.  The grid is a multiple of the tile count: CTA b owns tile
@@ -58,8 +65,13 @@ __device__ __forceinline__ void gw_tile_ij(int t, int nblk, int* I, int* J) {
   *J = i + t;
 }
 
-__global__ void __launch_bounds__(GW_NTHREADS, 1)
-k_gram_wg(const __grid_constant__ CUtensorMap mapX, const GramArgs args) {
+struct GramWeights {
+  const double* r;   // [n][K] row weights (W = true), else unused
+  int K;
+};
+
+template <bool W>
+__device__ __forceinline__ void gram_wg_body(const CUtensorMap& mapX, const GramArgs args, const GramWeights wt) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // the runtime aligns dynamic shared memory to 16 B only: the host asks for 1 KB more and the kernel aligns itself
   uint8_t* sm = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -69,9 +81,11 @@ k_gram_wg(const __grid_constant__ CUtensorMap mapX, const GramArgs args) {
   auto xempty = [&](int s) -> uint32_t { return bars + 8u * (uint32_t)(GW_SX + s); };
   float* mu_s = reinterpret_cast<float*>(sm + GW_OFF_MU);   // [0, 128): block I, [128, 256): block J
 
+  const int units = W ? args.ntile * wt.K : args.ntile;   // CTAs that read the same row range
   const int t = (int)blockIdx.x % args.ntile;
-  const int p0 = (int)blockIdx.x / args.ntile;
-  const int P = (int)gridDim.x / args.ntile;
+  const int comp = W ? ((int)blockIdx.x % units) / args.ntile : 0;
+  const int p0 = (int)blockIdx.x / units;
+  const int P = (int)gridDim.x / units;
   int I, J;
   gw_tile_ij(t, args.nblk, &I, &J);
   const bool diag = I == J;
@@ -121,7 +135,9 @@ k_gram_wg(const __grid_constant__ CUtensorMap mapX, const GramArgs args) {
   const int g = warp >> 2, tid = threadIdx.x;   // tid < 256
   // centre, split and transpose one block of the chunk into K-major (hi, lo) operands; a warp handles 32 consecutive
   // features of one group of 4 rows: conflict-free reads, 16-byte stores
-  auto stage = [&](const uint8_t* xb, const float* mub, int nvalid, uint32_t dhi, uint32_t dlo, int kv) {
+  // wrow: W = true, the chunk's first row of the weight table at this CTA's component
+  auto stage = [&](const uint8_t* xb, const float* mub, int nvalid, uint32_t dhi, uint32_t dlo, int kv,
+                   const double* wrow) {
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       const int it = tid + 256 * j;
@@ -132,7 +148,8 @@ k_gram_wg(const __grid_constant__ CUtensorMap mapX, const GramArgs args) {
         const int k = 4 * k4 + i;
         const float raw = *reinterpret_cast<const float*>(
             xb + (nf >> 5) * GW_BOX + k * 128 + ((((nf & 31) >> 2) ^ (k & 7)) << 4) + (nf & 3) * 4);
-        const float v = (k < kv && nf < nvalid) ? raw - mub[nf] : 0.f;
+        float v = (k < kv && nf < nvalid) ? raw - mub[nf] : 0.f;
+        if constexpr (W) v *= k < kv ? sqrtf((float)__ldg(wrow + (int64_t)k * wt.K)) : 0.f;
         hi[i] = rn_tf32_bits(v);
         lo[i] = rn_tf32_bits(v - __uint_as_float(hi[i]));
       }
@@ -163,12 +180,13 @@ k_gram_wg(const __grid_constant__ CUtensorMap mapX, const GramArgs args) {
       const uint32_t bl = bh + (uint32_t)GW_BBYTES;
       const uint32_t ah = diag ? bh : bl + (uint32_t)GW_BBYTES;
       const uint32_t al = diag ? bl : ah + (uint32_t)GW_BBYTES;
+      const double* wrow = W ? wt.r + (row0 + (int64_t)c * GW_KC) * wt.K + comp : nullptr;
       mbar_wait_nocall(xfull(xs), (uint32_t)((q / GW_SX) & 1));
       if (diag) {
-        stage(xI, mu_s, args.d - I * GW_BLK, bh, bl, kv);
+        stage(xI, mu_s, args.d - I * GW_BLK, bh, bl, kv, wrow);
       } else {
-        stage(xI + GW_XHALF, mu_s + GW_BLK, args.d - J * GW_BLK, bh, bl, kv);
-        stage(xI, mu_s, args.d - I * GW_BLK, ah, al, kv);
+        stage(xI + GW_XHALF, mu_s + GW_BLK, args.d - J * GW_BLK, bh, bl, kv, wrow);
+        stage(xI, mu_s, args.d - I * GW_BLK, ah, al, kv, wrow);
       }
       asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // operand writes -> visible to wgmma
       asm volatile("bar.sync 1, 256;" ::: "memory");

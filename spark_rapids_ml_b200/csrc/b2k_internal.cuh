@@ -503,6 +503,18 @@ int b2k_logreg_predict_csr_impl(b2k_ctx* ctx, const B2kCsr& X, int kp, const dou
                                 cudaStream_t s);
 
 // ------------------------------------------------------------------------------------------------
+// Gaussian mixtures — b2k_gmm.cu (the C ABI entry points in b2k_api.cu check their arguments, check the partitions and
+// draw the random start, then call these).  w [k], mu [k][d], cov [k][d][d]: the starting model, fp64.
+// ------------------------------------------------------------------------------------------------
+int b2k_gmm_fit_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, int k, std::vector<double> w,
+                     std::vector<double> mu, std::vector<double> cov, int max_iter, double tol, double* weights_out,
+                     double* means_out, double* covs_out, double* log_likelihood_out, int* n_iter_out,
+                     int64_t* cluster_sizes_out, cudaStream_t s);
+int b2k_gmm_predict_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, int k, const double* weights,
+                         const double* means, const double* covs, double* prob_out, int32_t* labels_out,
+                         cudaStream_t s);
+
+// ------------------------------------------------------------------------------------------------
 // evaluation — b2k_eval.cu (the C ABI entry points in b2k_api.cu check their arguments, then call these)
 // ------------------------------------------------------------------------------------------------
 int b2k_eval_linear_impl(b2k_ctx* ctx, const float* X, const float* y, int64_t n, int d, int m, const int32_t* kind,

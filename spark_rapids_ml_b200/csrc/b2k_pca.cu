@@ -25,6 +25,11 @@ namespace {
 #include "b2k_ptx.cuh"
 #include "b2k_gram_wg.cuh"
 
+__global__ void __launch_bounds__(GW_NTHREADS, 1)
+k_gram_wg(const __grid_constant__ CUtensorMap mapX, const GramArgs args) {
+  gram_wg_body<false>(mapX, args, GramWeights{nullptr, 1});
+}
+
 constexpr int CS_TX = 32, CS_TY = 8;   // column-sum CTA: 32 columns x 8 row lanes
 
 __global__ void __launch_bounds__(CS_TX * CS_TY)
