@@ -51,6 +51,9 @@
  *                               pyspark.ml.evaluation.ClusteringEvaluator (metricName "silhouette")
  *   b2k_gmm_fit / _predict      none: the reference has no Gaussian mixture; stands in for Spark's
  *                               pyspark.ml.clustering.GaussianMixture (fit and GaussianMixtureModel.transform)
+ *   b2k_bkm_fit / _predict      none: the reference has no bisecting k-means; stands in for Spark's
+ *                               pyspark.ml.clustering.BisectingKMeans (fit and BisectingKMeansModel.transform /
+ *                               computeCost)
  *   b2k_silhouette_multi        none: the reference tunes KMeans with pyspark's CrossValidator, scoring each model on
  *                               the CPU; here one device pass scores every model of a param grid
  *
@@ -881,6 +884,61 @@ int b2k_gmm_fit(b2k_ctx* ctx, const float* X, int64_t n_local, int d, int k, int
  * passes, bounds and errors as b2k_gmm_fit's E-step.  Synchronises `stream`. */
 int b2k_gmm_predict(b2k_ctx* ctx, const float* X, int64_t n, int d, int k, const double* weights, const double* means,
                     const double* covs, double* prob_out, int32_t* labels_out, uintptr_t stream);
+
+/* ---- bisecting k-means (euclidean) ----
+ * Stands in for pyspark.ml.clustering.BisectingKMeans (the reference has no bisecting k-means), whose rules are restated
+ * here so that no Spark source is needed.
+ *
+ * Nodes: the root is 1, the children of i are 2i (left) and 2i + 1 (right).  A node's summary is its row count n, its
+ * centre (the fp64 mean of its rows) and its cost (the sum of squared distances of its rows to that centre).
+ * minSize = ceil(min_divisible) when min_divisible >= 1, else ceil(min_divisible n_total).
+ * Levels: level 1 starts with the root as the only active node and need = k - 1.  While there are active nodes,
+ * need > 0 and level < 63: a node is divisible when n >= minSize and cost > EPS n (EPS = 2.220446049250313e-16); when
+ * more than `need` nodes are divisible the `need` largest by n divide, ties to the lower index (Spark breaks ties in
+ * hash-map order, which is not reproduced); when none is, every active node becomes a leaf and the loop ends.
+ * Split start: a node i with centre c starts its children at c - l u and c + l u, l = 1e-4 ||c||_2, u_j =
+ * (splitmix64(splitmix64(seed ^ splitmix64(i)) + j) >> 11) 2^-53 (splitmix64 as for b2k_gmm_fit), so the start
+ * depends on neither the order of the splits nor the rank count.  Spark draws from java.util.Random(seed) in map order:
+ * the start differs from Spark's for the same seed (deliberate).
+ * Iterations: max_iter per level.  Each reassigns every row of every dividing node to the nearer of that node's live
+ * children (fp64 sums of (x_j - c_j)^2 from the fp32 row, ties to the left) and recomputes the children's summaries; a
+ * child left with no rows drops out for the rest of the level.  The device sums are taken about the parent's centre p:
+ * S1 = sum (x - p), S2 = sum ||x - p||^2, centre = p + S1 / n, cost = max(S2 - ||S1||^2 / n, 0) in fp64 (Spark forms
+ * sumSq - n ||c||^2, equal in exact arithmetic but cancelling on offset data: a deliberate difference).  The root's
+ * summary comes from the fp64 column means and centred squares.
+ * Level end: every row of a dividing node is reassigned once more with the final centres (the assignment the next level
+ * starts from); the stored child summaries stay those of the last iteration (Spark's order).  The children with rows
+ * become the active nodes; every other node is inactive; need drops by the number of nodes divided, even when a child
+ * came out empty, so the model can have fewer than k leaves (also when k > n_total, which is legal).
+ * Leaves are numbered 0, 1, ... in depth-first order, left first.  Predict: from the root, move to the nearer existing
+ * child (the fp64 rule above, ties left) until a leaf; a node with one child passes to it.
+ *
+ * b2k_bkm_fit (collective): X device f32 [n_local, d].  Outputs (host): *n_nodes_out; per node in depth-first order
+ * (at most 2k - 1) node_index_out, node_centers_out [n_nodes][d] (fp64), node_size_out, node_cost_out;
+ * *training_cost_out = the sum of the leaf costs; cluster_sizes_out [k] = per leaf the rows b2k_bkm_predict sends
+ * there over all ranks, zero past the leaf count; level_ms_out [B2K_BKM_MAX_LEVELS] (or NULL) = each level's device time
+ * with option "time_kernels".  Errors, decided on allgathered or allreduced values so that every rank fails together
+ * (B2K_ERR_INVALID unless noted): an empty partition on any rank; a NaN or an infinity in X; k < 2; max_iter < 1;
+ * min_divisible <= 0 (or not finite); d < 1; d > B2K_BKM_MAX_D, k > B2K_BKM_MAX_K, k d > 2^24 or more than 2^31 - 1
+ * rows on a rank (B2K_ERR_UNSUPPORTED).  Synchronises `stream`.  No atomics: bitwise reproducible for the same input,
+ * rank count and device (option "grid_limit", which caps the split pass's CTAs, does not change the result).  Stats:
+ * last_n_iter = the levels run; with option "time_kernels" != 0, last_fused_ms = the split passes, last_reduce_ms =
+ * the fold, centre and partition passes, last_allreduce_ms = the allreduces (device times, CUDA events),
+ * last_finalize_ms = the host's level decisions and last_loop_ms = the whole call (host clock). */
+#define B2K_BKM_MAX_D 4096
+#define B2K_BKM_MAX_K 65536
+#define B2K_BKM_MAX_LEVELS 62
+int b2k_bkm_fit(b2k_ctx* ctx, const float* X, int64_t n_local, int d, int k, int max_iter, double min_divisible,
+                uint64_t seed, int* n_nodes_out, int64_t* node_index_out, double* node_centers_out,
+                int64_t* node_size_out, double* node_cost_out, double* training_cost_out, int64_t* cluster_sizes_out,
+                double* level_ms_out, uintptr_t stream);
+/* Local (no collective): per row of X [n, d] the leaf reached by descent (labels_out, device int32) and, when cost_out
+ * is not NULL, the squared distance to that leaf's centre (device f64), for the tree of n_nodes nodes node_index [n_nodes]
+ * with centres node_centers [n_nodes][d] (host, any order; the indices must be distinct, include 1 and every non-root's
+ * parent).  Errors: a bad node list or a non-finite centre (B2K_ERR_INVALID); d > B2K_BKM_MAX_D or more than
+ * 2 B2K_BKM_MAX_K - 1 nodes (B2K_ERR_UNSUPPORTED).  Synchronises `stream`. */
+int b2k_bkm_predict(b2k_ctx* ctx, const float* X, int64_t n, int d, int n_nodes, const int64_t* node_index,
+                    const double* node_centers, int32_t* labels_out, double* cost_out, uintptr_t stream);
 
 #ifdef __cplusplus
 }

@@ -84,7 +84,11 @@ EXPORTED_SYMBOLS = (
     "b2k_silhouette_multi",
     "b2k_gmm_fit",
     "b2k_gmm_predict",
+    "b2k_bkm_fit",
+    "b2k_bkm_predict",
 )
+
+BKM_MAX_LEVELS = 62   # B2K_BKM_MAX_LEVELS
 
 EVAL_KINDS = {"identity": 0, "logistic": 1, "softmax": 2}
 BINARY_METRICS = {"areaUnderROC": 0, "areaUnderPR": 1}
@@ -275,6 +279,9 @@ def load_library() -> ctypes.CDLL:
     L.b2k_gmm_fit.argtypes = [vp, vp, i64, i32, i32, i32, vp, vp, vp, i32, f64, u64, vp, vp, vp, ctypes.POINTER(f64),
                               ctypes.POINTER(i32), vp, ctypes.c_size_t]
     L.b2k_gmm_predict.argtypes = [vp, vp, i64, i32, i32, vp, vp, vp, vp, vp, ctypes.c_size_t]
+    L.b2k_bkm_fit.argtypes = [vp, vp, i64, i32, i32, i32, f64, u64, ctypes.POINTER(i32), vp, vp, vp, vp,
+                              ctypes.POINTER(f64), vp, vp, ctypes.c_size_t]
+    L.b2k_bkm_predict.argtypes = [vp, vp, i64, i32, i32, vp, vp, vp, vp, ctypes.c_size_t]
     for name in EXPORTED_SYMBOLS:
         if name not in ("b2k_last_error",):
             getattr(L, name).restype = i32
@@ -746,6 +753,56 @@ class Context:
             self._check(self._L.b2k_gmm_predict(self._h, X.data_ptr(), n, d, k, w.ctypes.data, mu.ctypes.data,
                                                 cov.ctypes.data, prob.data_ptr(), labels.data_ptr(), self._stream()))
         return prob, labels
+
+    # -- bisecting k-means -------------------------------------------------------------------
+    def bkm_fit(self, X: Any, k: int, *, max_iter: int = 20, min_divisible: float = 1.0, seed: int = 0
+                ) -> Dict[str, Any]:
+        """BisectingKMeans.fit (b2k_bkm_fit, collective when a communicator is initialised).  Returns the tree in
+        depth-first order as host arrays node_index int64 [m], centers float64 [m, d], sizes int64 [m], costs float64
+        [m]; training_cost; cluster_sizes int64 [leaves]; n_levels; level_ms float64 [n_levels] (zeros unless option
+        time_kernels is set)."""
+        n, d = self._check_X(X)
+        kk = max(int(k), 1)
+        m = 2 * kk - 1
+        idx = np.zeros(m, dtype=np.int64)
+        cen = np.zeros((m, max(d, 1)), dtype=np.float64)
+        sizes = np.zeros(m, dtype=np.int64)
+        costs = np.zeros(m, dtype=np.float64)
+        csz = np.zeros(kk, dtype=np.int64)
+        lms = np.zeros(BKM_MAX_LEVELS, dtype=np.float64)
+        nn = ctypes.c_int(0)
+        tc = ctypes.c_double(0.0)
+        with self._torch.cuda.device(self.device):
+            self._check(self._L.b2k_bkm_fit(
+                self._h, X.data_ptr(), n, d, int(k), int(max_iter), float(min_divisible), int(seed) & 0xFFFFFFFFFFFFFFFF,
+                ctypes.byref(nn), idx.ctypes.data, cen.ctypes.data, sizes.ctypes.data, costs.ctypes.data,
+                ctypes.byref(tc), csz.ctypes.data, lms.ctypes.data, self._stream()))
+        nn = int(nn.value)
+        idx, cen = idx[:nn], cen.reshape(-1)[: nn * d].reshape(nn, d)
+        ids = set(idx.tolist())
+        n_leaves = sum(1 for i in ids if 2 * i not in ids and 2 * i + 1 not in ids)
+        levels = int(self.stats()["last_n_iter"])
+        return {"node_index": idx, "centers": cen, "sizes": sizes[:nn], "costs": costs[:nn],
+                "training_cost": float(tc.value), "cluster_sizes": csz[:n_leaves], "n_levels": levels,
+                "level_ms": lms[:levels]}
+
+    def bkm_predict(self, X: Any, node_index: Any, node_centers: Any, *, with_cost: bool = False
+                    ) -> Tuple[Any, Optional[Any]]:
+        """Per row of X the int32 leaf (depth-first number) reached by descent and, with with_cost, the float64
+        squared distance to that leaf's centre (CUDA tensors; the cost is None otherwise)."""
+        t = self._torch
+        n, d = self._check_X(X)
+        idx = np.ascontiguousarray(node_index, dtype=np.int64).reshape(-1)
+        cen = np.ascontiguousarray(node_centers, dtype=np.float64)
+        if cen.shape != (idx.shape[0], d):
+            raise ValueError(f"node_centers must be [{idx.shape[0]}, {d}]")
+        labels = t.empty((n,), dtype=t.int32, device=self.device)
+        cost = t.empty((n,), dtype=t.float64, device=self.device) if with_cost else None
+        with t.cuda.device(self.device):
+            self._check(self._L.b2k_bkm_predict(self._h, X.data_ptr(), n, d, int(idx.shape[0]), idx.ctypes.data,
+                                                cen.ctypes.data, labels.data_ptr(),
+                                                cost.data_ptr() if cost is not None else None, self._stream()))
+        return labels, cost
 
     # -- logistic regression ----------------------------------------------------------------
     def _check_y(self, y: Any, n: int) -> None:

@@ -12,6 +12,7 @@ Same names, argument meaning and error behaviour as the reference:
   reference hands to pyspark's CrossValidator (GPU fits, CPU silhouette); here every fold's grid fits from one ingest
   and its models are scored in one device silhouette pass (b2k_silhouette_multi)
   DBSCANClass, _DBSCANCumlParams, DBSCAN (lazy fit), DBSCANModel.transform             clustering.py:607-1186
+  GaussianMixture / BisectingKMeans: Spark's estimators of those names, which the reference lacks
 
 Differences that are deliberate: no CPU fallback (cpu() / single-vector predict need a JVM and raise), and the
 fit function receives a DEVICE matrix from the worker scaffold instead of host arrays to concatenate.  DBSCAN: every
@@ -828,3 +829,289 @@ class GaussianMixtureModel(GaussianMixtureClass, _CumlModelWithPredictionCol, _G
 
         k = len(self.weights_)
         return _DeviceModel, self._grouped_transform(_predict, 4 * int(self.n_cols) + 8 * k + 4), None
+
+
+# ---- BisectingKMeans (pyspark.ml.clustering.BisectingKMeans; the reference has no bisecting k-means) ----
+class BisectingKMeansClass(_CumlClass):
+    @classmethod
+    def _param_mapping(cls) -> Dict[str, Optional[str]]:
+        # None = unsupported, "" = accepted and ignored (distanceMeasure: only "euclidean", checked by the params)
+        return {"k": "n_clusters", "maxIter": "max_iter", "seed": "random_state",
+                "minDivisibleClusterSize": "min_divisible_cluster_size", "distanceMeasure": "", "weightCol": None}
+
+    def _get_cuml_params_default(self) -> Dict[str, Any]:
+        return {"n_clusters": 4, "max_iter": 20, "random_state": None, "min_divisible_cluster_size": 1.0,
+                "verbose": False}
+
+    def _pyspark_class(self) -> Optional[type]:
+        return None  # pyspark.ml.clustering.BisectingKMeans when pyspark is installed
+
+
+def _check_bkm_distance(value: Any) -> None:
+    if value != "euclidean":
+        raise ValueError(f"distanceMeasure {value!r} is not supported by BisectingKMeans on the GPU: use 'euclidean'")
+
+
+class _BisectingKMeansCumlParams(_CumlParams, HasFeaturesCol, HasFeaturesCols, HasPredictionCol):
+    """Shared Spark Params of BisectingKMeans and BisectingKMeansModel (Spark's defaults: k=4, maxIter=20,
+    minDivisibleClusterSize=1.0, distanceMeasure='euclidean')."""
+
+    k = Param("parent", "k", "The desired number of leaf clusters. Must be > 1.", TypeConverters.toInt)
+    maxIter = Param("parent", "maxIter", "max number of iterations (>= 0).", TypeConverters.toInt)
+    seed = Param("parent", "seed", "random seed.", TypeConverters.toInt)
+    minDivisibleClusterSize = Param("parent", "minDivisibleClusterSize",
+                                    "The minimum number of points (if >= 1.0) or the minimum proportion of points "
+                                    "(if < 1.0) of a divisible cluster.", TypeConverters.toFloat)
+    distanceMeasure = Param("parent", "distanceMeasure", "the distance measure. Supported options: 'euclidean'.",
+                            TypeConverters.toString)
+    weightCol = Param("parent", "weightCol", "weight column name.", TypeConverters.toString)
+
+    def __init__(self) -> None:
+        super().__init__()
+        self._setDefault(k=4, maxIter=20, minDivisibleClusterSize=1.0, distanceMeasure="euclidean")
+        # the KMeans rule: a 32-bit signed seed from the class name
+        self._setDefault(seed=hash(type(self).__name__) & 0x07FFFFFFF)
+
+    def getK(self) -> int:
+        return self.getOrDefault(self.k)
+
+    def getMaxIter(self) -> int:
+        return self.getOrDefault(self.maxIter)
+
+    def getSeed(self) -> int:
+        return self.getOrDefault(self.seed)
+
+    def getMinDivisibleClusterSize(self) -> float:
+        return self.getOrDefault(self.minDivisibleClusterSize)
+
+    def getDistanceMeasure(self) -> str:
+        return self.getOrDefault(self.distanceMeasure)
+
+    def getFeaturesCol(self) -> Union[str, List[str]]:  # type: ignore[override]
+        if self.isDefined(self.featuresCols):
+            return self.getFeaturesCols()
+        if self.isDefined(self.featuresCol):
+            return self.getOrDefault("featuresCol")
+        raise RuntimeError("featuresCol is not set")
+
+    def setFeaturesCol(self: P, value: Union[str, List[str]]) -> P:
+        if isinstance(value, str):
+            self._set_params(featuresCol=value)
+        else:
+            self._set_params(featuresCols=value)
+        return self
+
+    def setFeaturesCols(self: P, value: List[str]) -> P:
+        return self._set_params(featuresCols=value)
+
+    def setPredictionCol(self: P, value: str) -> P:
+        return self._set_params(predictionCol=value)
+
+
+class BisectingKMeans(BisectingKMeansClass, _CumlEstimator, _BisectingKMeansCumlParams):
+    """Bisecting k-means on H100, Spark's pyspark.ml.clustering.BisectingKMeans (euclidean).  One barrier task per GPU
+    holds its partition on the device.  Level by level, the largest divisible clusters are split in two: each
+    iteration is one device pass over the rows of the clusters being split (every row against its cluster's two
+    children, fp64 sums folded in a fixed order), one NCCL allreduce and the new children; the host decides the next
+    level once per level.  Parameters: k (4), maxIter (20, iterations per level), seed, minDivisibleClusterSize (1.0:
+    a count when >= 1, else a fraction of the rows), distanceMeasure ("euclidean" only), featuresCol (str for an array
+    column, list of str for scalar columns), predictionCol, num_workers, verbose.  weightCol is not supported.
+
+    A split starts from the library's own seeded generator, so the tree differs from Spark's for the same seed; ties
+    between equally large divisible clusters go to the lower node index.
+
+    >>> from spark_rapids_ml_b200.clustering import BisectingKMeans
+    >>> model = BisectingKMeans(k=8, seed=1).fit(df)
+    >>> model.clusterCenters(), model.summary.trainingCost
+    """
+
+    @keyword_only
+    def __init__(self, *, featuresCol: Union[str, List[str]] = "features", predictionCol: str = "prediction",
+                 maxIter: int = 20, seed: Optional[int] = None, k: int = 4, minDivisibleClusterSize: float = 1.0,
+                 distanceMeasure: str = "euclidean", weightCol: Optional[str] = None,
+                 num_workers: Optional[int] = None, verbose: Union[int, bool] = False, **kwargs: Any) -> None:
+        super().__init__()
+        self._handle_param_spark_confs()
+        self._input_kwargs.pop("kwargs", None)
+        self._input_kwargs.update(kwargs)
+        for name in ("seed", "num_workers", "weightCol"):
+            if self._input_kwargs.get(name, None) is None:
+                self._input_kwargs.pop(name, None)
+        if "weightCol" in self._input_kwargs:
+            raise ValueError("'weightCol' is not supported by BisectingKMeans on the GPU.")
+        if "distanceMeasure" in self._input_kwargs:
+            _check_bkm_distance(self._input_kwargs["distanceMeasure"])
+        self._set_params(**self._input_kwargs)
+
+    def setK(self, value: int) -> "BisectingKMeans":
+        return self._set_params(k=value)
+
+    def setMaxIter(self, value: int) -> "BisectingKMeans":
+        return self._set_params(maxIter=value)
+
+    def setSeed(self, value: int) -> "BisectingKMeans":
+        return self._set_params(seed=value)
+
+    def setMinDivisibleClusterSize(self, value: float) -> "BisectingKMeans":
+        return self._set_params(minDivisibleClusterSize=value)
+
+    def setDistanceMeasure(self, value: str) -> "BisectingKMeans":
+        _check_bkm_distance(value)
+        return self._set_params(distanceMeasure=value)
+
+    def setWeightCol(self, value: str) -> "BisectingKMeans":
+        raise ValueError("'weightCol' is not supported by BisectingKMeans on the GPU.")
+
+    def _validate_parameters(self) -> None:
+        super()._validate_parameters()
+        k, max_iter, mdcs = self.getK(), self.getMaxIter(), self.getMinDivisibleClusterSize()
+        if isinstance(k, bool) or not isinstance(k, int) or k < 2:
+            raise ValueError(f"k given invalid value {k} (must be > 1)")
+        if max_iter < 1:
+            raise ValueError(f"maxIter given invalid value {max_iter} (must be >= 1)")
+        if not mdcs > 0:
+            raise ValueError(f"minDivisibleClusterSize given invalid value {mdcs} (must be > 0)")
+        _check_bkm_distance(self.getDistanceMeasure())
+
+    def _fit_array_order(self) -> str:
+        return "C"
+
+    def _get_cuml_fit_func(self, dataset: Any, extra_params: Optional[List[Dict[str, Any]]] = None
+                           ) -> Callable[[FitInputType, Dict[str, Any]], Dict[str, Any]]:
+        cls = self.__class__
+
+        def _cuml_fit(dfs: FitInputType, params: Dict[str, Any]) -> Dict[str, Any]:
+            ctx = params[param_alias.handle]
+            init = params[param_alias.cuml_init]
+            if len(dfs) != 1:
+                raise RuntimeError("the worker scaffold hands the fit function ONE device matrix per partition")
+            seed = init.get("random_state")
+            out = ctx.bkm_fit(dfs[0][0], int(init["n_clusters"]), max_iter=int(init["max_iter"]),
+                              min_divisible=float(init["min_divisible_cluster_size"]),
+                              seed=int(seed) if seed is not None else 0)
+            get_logger(cls).info(f"levels: {out['n_levels']}, nodes: {len(out['node_index'])}, "
+                                 f"training cost: {out['training_cost']}")
+            return {"node_index_": [out["node_index"].tolist()], "node_centers_": [out["centers"].tolist()],
+                    "node_sizes_": [out["sizes"].tolist()], "node_costs_": [out["costs"].tolist()],
+                    "cluster_sizes_": [out["cluster_sizes"].tolist()], "training_cost_": [out["training_cost"]],
+                    "num_iters": [int(init["max_iter"])], "n_cols": [params[param_alias.num_cols]],
+                    "dtype": ["float32"]}
+
+        return _cuml_fit
+
+    def _out_schema(self) -> Any:
+        return ("node_index_ array<long>, node_centers_ array<array<double>>, node_sizes_ array<long>, "
+                "node_costs_ array<double>, cluster_sizes_ array<long>, training_cost_ double, num_iters int, "
+                "n_cols int, dtype string")
+
+    def _create_pyspark_model(self, result: Row) -> "BisectingKMeansModel":
+        r = result.asDict()
+        return BisectingKMeansModel(
+            node_index_=[int(v) for v in r["node_index_"]],
+            node_centers_=[[float(v) for v in c] for c in r["node_centers_"]],
+            node_sizes_=[int(v) for v in r["node_sizes_"]], node_costs_=[float(v) for v in r["node_costs_"]],
+            cluster_sizes_=[int(v) for v in r["cluster_sizes_"]], training_cost_=float(r["training_cost_"]),
+            num_iters=int(r["num_iters"]), n_cols=int(r["n_cols"]), dtype=str(r["dtype"]))
+
+
+class BisectingKMeansSummary:
+    """The training summary Spark's BisectingKMeansModel.summary holds: k (the leaf count), numIter, clusterSizes and
+    trainingCost."""
+
+    def __init__(self, k: int, num_iter: int, cluster_sizes: List[int], training_cost: float) -> None:
+        self.k = k
+        self.numIter = num_iter
+        self.clusterSizes = cluster_sizes
+        self.trainingCost = training_cost
+
+
+class BisectingKMeansModel(BisectingKMeansClass, _CumlModelWithPredictionCol, _BisectingKMeansCumlParams):
+    """The cluster tree: node indices (root 1, children 2i and 2i + 1), centres, sizes and costs in depth-first order.
+    transform() appends predictionCol (int): the leaf reached by descending from the root to the nearer child, leaves
+    numbered in depth-first order as clusterCenters() lists them."""
+
+    def __init__(self, node_index_: List[int], node_centers_: List[List[float]], node_sizes_: List[int],
+                 node_costs_: List[float], cluster_sizes_: List[int], training_cost_: float, num_iters: int,
+                 n_cols: int, dtype: str) -> None:
+        super().__init__(n_cols=n_cols, dtype=dtype, node_index_=node_index_, node_centers_=node_centers_,
+                         node_sizes_=node_sizes_, node_costs_=node_costs_, cluster_sizes_=cluster_sizes_,
+                         training_cost_=training_cost_, num_iters=num_iters)
+        self.node_index_ = node_index_
+        self.node_centers_ = node_centers_
+        self.node_sizes_ = node_sizes_
+        self.node_costs_ = node_costs_
+        self.cluster_sizes_ = cluster_sizes_
+        self.training_cost_ = training_cost_
+        self.num_iters = num_iters
+        self._set_params(k=len(self._leaves()))
+
+    def _leaves(self) -> List[int]:
+        ids = set(self.node_index_)
+        return [j for j, i in enumerate(self.node_index_) if 2 * i not in ids and 2 * i + 1 not in ids]
+
+    def clusterCenters(self) -> List[np.ndarray]:
+        return [np.asarray(self.node_centers_[j], dtype=np.float64) for j in self._leaves()]
+
+    @property
+    def hasSummary(self) -> bool:
+        return True
+
+    @property
+    def summary(self) -> BisectingKMeansSummary:
+        return BisectingKMeansSummary(len(self._leaves()), int(self.num_iters), list(self.cluster_sizes_),
+                                      float(self.training_cost_))
+
+    def computeCost(self, dataset: Any) -> float:
+        """The sum of squared distances of the rows of `dataset` to the centres of the leaves they are predicted to."""
+        from .core import _CumlCommon, _GroupedTransform, _iter_transform, _select_features
+        from .sparkshim import BarrierTaskContext
+        from .sparkshim.sql import _batches_to_pdf_iter
+
+        if HAVE_PYSPARK:
+            from . import spark_binding
+
+            if spark_binding.is_spark_dataframe(dataset):
+                raise NotImplementedError("BisectingKMeansModel.computeCost of a pyspark DataFrame is not supported "
+                                          "yet; use a local frame")
+        idx = np.asarray(self.node_index_, dtype=np.int64)
+        cen = np.asarray(self.node_centers_, dtype=np.float64)
+        transform = _GroupedTransform(lambda m, X: (m.ctx.bkm_predict(X, idx, cen, with_cost=True)[1],),
+                                      int(self.n_cols), 4 * int(self.n_cols) + 12, ["double"])
+        input_col, input_cols = self._get_input_columns()
+        total, model = 0.0, None
+        for pid, part in enumerate(dataset._parts):
+            if part and model is None:
+                model = _DeviceModel(_CumlCommon._set_gpu_device(BarrierTaskContext(pid, len(dataset._parts)), True,
+                                                                 True))
+            frames = _batches_to_pdf_iter(_select_features(part, input_col, input_cols), dataset.arrow_backed_pandas)
+            for (c,) in _iter_transform(transform, model, frames):
+                total += float(np.sum(c, dtype=np.float64))
+        if model is not None:
+            model.close()
+        return total
+
+    def predict(self, value: Any) -> int:
+        raise NotImplementedError("BisectingKMeansModel.predict() of a single vector is not supported; use transform()")
+
+    def cpu(self) -> Any:
+        raise NotImplementedError("BisectingKMeansModel.cpu() builds a JVM pyspark.ml model; no JVM/pyspark in this "
+                                  "build")
+
+    def _out_schema(self, input_schema: Any = None) -> str:
+        return "int"
+
+    def _transform_outputs(self) -> List[Tuple[str, str]]:
+        return [(self.getOrDefault("predictionCol"), "int")]
+
+    def _transform_array_order(self) -> str:
+        return "C"
+
+    def _get_cuml_transform_func(self, dataset: Any, eval_metric_info: Any = None
+                                 ) -> Tuple[Callable, Callable, Optional[Callable]]:
+        idx = np.asarray(self.node_index_, dtype=np.int64)
+        cen = np.asarray(self.node_centers_, dtype=np.float64)
+
+        def _predict(m: Any, X: Any) -> Tuple[Any]:
+            return (m.ctx.bkm_predict(X, idx, cen)[0],)
+
+        return _DeviceModel, self._grouped_transform(_predict, 4 * int(self.n_cols) + 4), None

@@ -1348,12 +1348,6 @@ extern "C" int b2k_umap_transform(b2k_ctx* ctx, const float* X_train, const floa
 // Gaussian mixtures (b2k_gmm.cu)
 // ------------------------------------------------------------------------------------------------
 namespace {
-uint64_t gmm_splitmix64(uint64_t z) {
-  z += 0x9e3779b97f4a7c15ull;
-  z = (z ^ (z >> 30)) * 0xbf58476d1ce4e5b9ull;
-  z = (z ^ (z >> 27)) * 0x94d049bb133111ebull;
-  return z ^ (z >> 31);
-}
 
 // Spark's start (GaussianMixture.scala: weights 1/k, the mean of 5 sampled rows and the diagonal of their biased
 // variance), with the rows drawn by a counter-based rule over the global row order, so that the start depends on
@@ -1363,7 +1357,7 @@ int gmm_random_init(b2k_ctx* ctx, const float* X, int64_t n_local, int d, int k,
                     std::vector<double>* w, std::vector<double>* mu, std::vector<double>* cov, cudaStream_t s) {
   const int m = k * GMM_INIT_ROWS;
   std::vector<int64_t> draw(m);
-  for (int j = 0; j < m; ++j) draw[j] = (int64_t)(gmm_splitmix64(seed ^ gmm_splitmix64((uint64_t)j)) % (uint64_t)rows.total);
+  for (int j = 0; j < m; ++j) draw[j] = (int64_t)(b2k_splitmix64(seed ^ b2k_splitmix64((uint64_t)j)) % (uint64_t)rows.total);
   std::vector<int64_t> gidx(draw);
   std::sort(gidx.begin(), gidx.end());
   gidx.erase(std::unique(gidx.begin(), gidx.end()), gidx.end());
@@ -1450,5 +1444,42 @@ extern "C" int b2k_gmm_predict(b2k_ctx* ctx, const float* X, int64_t n, int d, i
   if (n == 0) return B2K_OK;
   B2K_CUDA_OK(ctx, cudaSetDevice(ctx->device));
   return b2k_gmm_predict_impl(ctx, X, n, d, k, weights, means, covs, prob_out, labels_out,
+                              reinterpret_cast<cudaStream_t>(stream));
+}
+
+// ------------------------------------------------------------------------------------------------
+// bisecting k-means (b2k_bisect.cu)
+// ------------------------------------------------------------------------------------------------
+extern "C" int b2k_bkm_fit(b2k_ctx* ctx, const float* X, int64_t n_local, int d, int k, int max_iter,
+                           double min_divisible, uint64_t seed, int* n_nodes_out, int64_t* node_index_out,
+                           double* node_centers_out, int64_t* node_size_out, double* node_cost_out,
+                           double* training_cost_out, int64_t* cluster_sizes_out, double* level_ms_out,
+                           uintptr_t stream) {
+  if (!ctx) return b2k_fail(nullptr, B2K_ERR_INVALID, "b2k_bkm_fit: ctx is NULL");
+  // an empty partition may come with no buffer: the collective check below reports it on every rank
+  if ((!X && n_local > 0) || n_local < 0 || !n_nodes_out || !node_index_out || !node_centers_out || !node_size_out ||
+      !node_cost_out || !training_cost_out || !cluster_sizes_out)
+    return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_bkm_fit: bad X/n/outputs");
+  if (d < 1) return b2k_fail(ctx, B2K_ERR_INVALID, "bisecting k-means: d must be >= 1, got " + std::to_string(d));
+  if (k < 2) return b2k_fail(ctx, B2K_ERR_INVALID, "bisecting k-means: k must be > 1, got " + std::to_string(k));
+  if (max_iter < 1)
+    return b2k_fail(ctx, B2K_ERR_INVALID, "bisecting k-means: maxIter must be >= 1, got " + std::to_string(max_iter));
+  if (!(min_divisible > 0.0) || !std::isfinite(min_divisible))
+    return b2k_fail(ctx, B2K_ERR_INVALID, "bisecting k-means: minDivisibleClusterSize must be > 0");
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  B2K_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  B2K_TRY(check_no_empty_partition(ctx, "b2k_bkm_fit", n_local, s));
+  return b2k_bkm_fit_impl(ctx, X, n_local, d, k, max_iter, min_divisible, seed, n_nodes_out, node_index_out,
+                          node_centers_out, node_size_out, node_cost_out, training_cost_out, cluster_sizes_out,
+                          level_ms_out, s);
+}
+
+extern "C" int b2k_bkm_predict(b2k_ctx* ctx, const float* X, int64_t n, int d, int n_nodes, const int64_t* node_index,
+                               const double* node_centers, int32_t* labels_out, double* cost_out, uintptr_t stream) {
+  if (!ctx) return b2k_fail(nullptr, B2K_ERR_INVALID, "b2k_bkm_predict: ctx is NULL");
+  if (n < 0 || d < 1 || n_nodes < 1 || !node_index || !node_centers || (n > 0 && (!X || !labels_out)))
+    return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_bkm_predict: bad X/nodes/outputs/n/d");
+  B2K_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  return b2k_bkm_predict_impl(ctx, X, n, d, n_nodes, node_index, node_centers, labels_out, cost_out,
                               reinterpret_cast<cudaStream_t>(stream));
 }

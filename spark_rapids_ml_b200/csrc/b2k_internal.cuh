@@ -91,6 +91,15 @@ struct b2k_ctx {
   b2k_stats stats{};
 };
 
+// The library's counter-based generator (host): Gaussian mixtures draw their start rows from it, bisecting k-means its
+// split starts.
+inline uint64_t b2k_splitmix64(uint64_t z) {
+  z += 0x9e3779b97f4a7c15ull;
+  z = (z ^ (z >> 30)) * 0xbf58476d1ce4e5b9ull;
+  z = (z ^ (z >> 27)) * 0x94d049bb133111ebull;
+  return z ^ (z >> 31);
+}
+
 // ------------------------------------------------------------------------------------------------
 // error helpers
 // ------------------------------------------------------------------------------------------------
@@ -513,6 +522,17 @@ int b2k_gmm_fit_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, int k, std:
 int b2k_gmm_predict_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, int k, const double* weights,
                          const double* means, const double* covs, double* prob_out, int32_t* labels_out,
                          cudaStream_t s);
+
+// ------------------------------------------------------------------------------------------------
+// bisecting k-means — b2k_bisect.cu (the C ABI entry points in b2k_api.cu check their arguments and the partitions, then
+// call these)
+// ------------------------------------------------------------------------------------------------
+int b2k_bkm_fit_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, int k, int max_iter, double min_divisible,
+                     uint64_t seed, int* n_nodes_out, int64_t* node_index_out, double* node_centers_out,
+                     int64_t* node_size_out, double* node_cost_out, double* training_cost_out,
+                     int64_t* cluster_sizes_out, double* level_ms_out, cudaStream_t s);
+int b2k_bkm_predict_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, int n_nodes, const int64_t* node_index,
+                         const double* node_centers, int32_t* labels_out, double* cost_out, cudaStream_t s);
 
 // ------------------------------------------------------------------------------------------------
 // evaluation — b2k_eval.cu (the C ABI entry points in b2k_api.cu check their arguments, then call these)
