@@ -54,6 +54,8 @@
  *   b2k_bkm_fit / _predict      none: the reference has no bisecting k-means; stands in for Spark's
  *                               pyspark.ml.clustering.BisectingKMeans (fit and BisectingKMeansModel.transform /
  *                               computeCost)
+ *   b2k_mlp_eval / _fit /       none: the reference has no multilayer perceptron; stands in for Spark's
+ *     _predict                  pyspark.ml.classification.MultilayerPerceptronClassifier (fit and the model's transform)
  *   b2k_silhouette_multi        none: the reference tunes KMeans with pyspark's CrossValidator, scoring each model on
  *                               the CPU; here one device pass scores every model of a param grid
  *
@@ -939,6 +941,69 @@ int b2k_bkm_fit(b2k_ctx* ctx, const float* X, int64_t n_local, int d, int k, int
  * 2 B2K_BKM_MAX_K - 1 nodes (B2K_ERR_UNSUPPORTED).  Synchronises `stream`. */
 int b2k_bkm_predict(b2k_ctx* ctx, const float* X, int64_t n, int d, int n_nodes, const int64_t* node_index,
                     const double* node_centers, int32_t* labels_out, double* cost_out, uintptr_t stream);
+
+/* ---- multilayer perceptron classification ----
+ * Stands in for pyspark.ml.classification.MultilayerPerceptronClassifier (the reference has none); its rules are restated
+ * here so that no Spark source is needed.
+ *
+ * Topology: layers [n_layers] = [d, h_1, ..., h_{L-1}, C], n_layers >= 2, every entry >= 1 (B2K_ERR_INVALID) and at most
+ * B2K_MLP_MAX_WIDTH (B2K_ERR_UNSUPPORTED); layers[0] must equal d, C = layers[L] is the class count.  Every layer is
+ * affine, z_l = W_l a_{l-1} + b_l (a_0 = x); hidden layers apply the sigmoid a_l = 1 / (1 + exp(-z_l)); the last layer's
+ * z_L goes to the softmax with cross-entropy loss.
+ * Weights (Spark's flat layout, fp64): for l = 1 .. L in order, W_l (numOut x numIn, column-major: element (o, i) at
+ * offset i numOut + o), then its numOut biases; P = sum_l numOut_l (numIn_l + 1) values in all.  So a Spark model's
+ * weights can be used as they are.
+ * Objective: F(w) = (1/n) sum_rows -log softmax(z_L)_y, the log-sum-exp with the row maximum removed; no regularisation.
+ * Gradient: delta_L = p - onehot(y), delta_l = (W_{l+1}^T delta_{l+1}) (.) a_l (1 - a_l), dW_l = (1/n) sum delta_l
+ * a_{l-1}^T, db_l = (1/n) sum delta_l.
+ * Labels: integers in [0, C), checked by b2k_logreg_labels' pass and rules ("Labels MUST be Integers, but got v", ...)
+ * plus a max label < C check, decided on gathered values: every rank fails together.  Spark truncates a fractional
+ * label; rejecting it is a deliberate difference.
+ * Loss weighting: Spark averages the loss within blockSize blocks and then across blocks; here the average is over
+ * rows, so blockSize has no effect (deliberate).
+ *
+ * Device passes: the rows run in chunks whose fp32 (wgmma) or fp64 (generic) activations take at most 32 MB (rows per
+ * chunk: the largest multiple of 4096 within 2^25 / (8 + es sum_{l >= 1} ceil4(layers[l])), es = 4 or 8, at least 4096).
+ * The products run on wgmma (3xTF32: fp32-accurate products, fp32 activations and deltas) when d % 4 == 0 and X is
+ * 16-byte aligned on every rank (the wgmma envelope, decided on an allreduced flag; any widths up to B2K_MLP_MAX_WIDTH),
+ * else on a generic fp64 SIMT path (fp64 products, activations and sums); option "kernel_path" = B2K_PATH_GENERIC
+ * forces the generic path, B2K_PATH_FUSED fails with B2K_ERR_UNSUPPORTED outside the envelope.  The gradient sums are
+ * formed per fixed 512-row unit of a rank's rows (in fp32 on the wgmma path: 32-row chunks added in round-to-nearest
+ * fp32; in fp64 on the generic path), and the units are folded in order in fp64: no atomics, bitwise reproducible for
+ * the same input, rank count and device, whatever option "grid_limit" (a cap on the CTAs of every pass) is.  Across
+ * rank counts the unit boundaries move with the shards: the generic path's gradient agrees with one rank's to about
+ * 1e-12 of |grad F|, the wgmma path's to about 1e-6 of |grad F| (the fp32 unit sums); F agrees to about 1e-12 on both
+ * (its per-row losses are fp64 and row-local).
+ *
+ * b2k_mlp_eval (collective): X device f32 [n_local, d], y device f32 [n_local], weights host f64 [P].  Outputs (host):
+ * *f_out = F, grad_out [P] = its gradient in the flat layout, *n_total_out (may be NULL).  One label pass, one f64
+ * allreduce; synchronises `stream`.  Errors (B2K_ERR_INVALID unless noted, every rank together): an empty partition on
+ * any rank; a NaN or an infinity in X; a non-finite weight; the layer and label rules; kernel_path=2 outside the envelope
+ * (B2K_ERR_UNSUPPORTED).  Stats: last_path; with option "time_kernels", last_fused_ms = the device passes.
+ *
+ * b2k_mlp_fit (collective): solver B2K_MLP_LBFGS: b2k_logreg_minimize's L-BFGS (l1 = NULL) with max_iter and tol;
+ * B2K_MLP_GD: MLlib's full-batch GradientDescent with SimpleUpdater, w_t = w_{t-1} - (step_size / sqrt(t)) grad F(w_{t-1}),
+ * t = 1 .. max_iter, stopping early when ||w_t - w_{t-1}|| < tol max(||w_t||, 1).  The start is initial_weights [P] when
+ * not NULL, else weight j of layer l is (u_j 4.8 - 2.4) / sqrt(numIn_l), u_j = (splitmix64(seed ^ splitmix64(j)) >> 11)
+ * 2^-53 (splitmix64 as for b2k_gmm_fit), so it depends on neither the rank count nor the partitioning.  Spark draws
+ * from XORShiftRandom: the start differs from Spark's for the same seed (deliberate).  Outputs (host): weights_out [P];
+ * history_out [max_iter + 1] = F at each accepted iterate (L-BFGS: the start, then each iteration; GD: the point of each
+ * step, before its update, as MLlib records it); *n_iter_out = the entries written.  Errors: those of b2k_mlp_eval;
+ * max_iter < 0; tol < 0; step_size <= 0 (GD); an unknown solver.  Stats: last_n_iter; with "time_kernels",
+ * last_fused_ms = the device passes of every evaluation and last_loop_ms = the whole call (host clock).
+ *
+ * b2k_mlp_predict (local, asynchronous on `stream`; the weights are copied before it returns): per row of X [n, d]
+ * raw_out [n][C] = z_L, prob_out [n][C] = softmax(z_L), pred_out [n] = the first argmax of z_L (device f64).  Same
+ * paths; errors: the layer rules, a non-finite weight, kernel_path=2 outside the envelope. */
+#define B2K_MLP_MAX_WIDTH 1024
+typedef enum b2k_mlp_solver { B2K_MLP_LBFGS = 0, B2K_MLP_GD = 1 } b2k_mlp_solver;
+int b2k_mlp_eval(b2k_ctx* ctx, const float* X, const float* y, int64_t n_local, const int32_t* layers, int n_layers,
+                 const double* weights, double* f_out, double* grad_out, int64_t* n_total_out, uintptr_t stream);
+int b2k_mlp_fit(b2k_ctx* ctx, const float* X, const float* y, int64_t n_local, const int32_t* layers, int n_layers,
+                int solver, int max_iter, double tol, double step_size, uint64_t seed, const double* initial_weights,
+                double* weights_out, double* history_out, int* n_iter_out, uintptr_t stream);
+int b2k_mlp_predict(b2k_ctx* ctx, const float* X, int64_t n, const int32_t* layers, int n_layers, const double* weights,
+                    double* raw_out, double* prob_out, double* pred_out, uintptr_t stream);
 
 #ifdef __cplusplus
 }

@@ -86,7 +86,12 @@ EXPORTED_SYMBOLS = (
     "b2k_gmm_predict",
     "b2k_bkm_fit",
     "b2k_bkm_predict",
+    "b2k_mlp_eval",
+    "b2k_mlp_fit",
+    "b2k_mlp_predict",
 )
+
+MLP_SOLVERS = {"l-bfgs": 0, "gd": 1}   # b2k_mlp_solver
 
 BKM_MAX_LEVELS = 62   # B2K_BKM_MAX_LEVELS
 
@@ -282,6 +287,11 @@ def load_library() -> ctypes.CDLL:
     L.b2k_bkm_fit.argtypes = [vp, vp, i64, i32, i32, i32, f64, u64, ctypes.POINTER(i32), vp, vp, vp, vp,
                               ctypes.POINTER(f64), vp, vp, ctypes.c_size_t]
     L.b2k_bkm_predict.argtypes = [vp, vp, i64, i32, i32, vp, vp, vp, vp, ctypes.c_size_t]
+    L.b2k_mlp_eval.argtypes = [vp, vp, vp, i64, vp, i32, vp, ctypes.POINTER(f64), vp, ctypes.POINTER(i64),
+                               ctypes.c_size_t]
+    L.b2k_mlp_fit.argtypes = [vp, vp, vp, i64, vp, i32, i32, i32, f64, f64, u64, vp, vp, vp, ctypes.POINTER(i32),
+                              ctypes.c_size_t]
+    L.b2k_mlp_predict.argtypes = [vp, vp, i64, vp, i32, vp, vp, vp, vp, ctypes.c_size_t]
     for name in EXPORTED_SYMBOLS:
         if name not in ("b2k_last_error",):
             getattr(L, name).restype = i32
@@ -803,6 +813,74 @@ class Context:
                                                 cen.ctypes.data, labels.data_ptr(),
                                                 cost.data_ptr() if cost is not None else None, self._stream()))
         return labels, cost
+
+    # -- multilayer perceptron ----------------------------------------------------------------
+    @staticmethod
+    def _mlp_layers(layers: Sequence[int], d: int) -> Tuple[np.ndarray, int]:
+        lay = np.ascontiguousarray([int(v) for v in layers], dtype=np.int32)
+        if lay.size >= 1 and int(lay[0]) != d:
+            raise ValueError(f"layers[0] = {int(lay[0])} must equal the feature count {d}")
+        P = sum(int(lay[i]) * (int(lay[i - 1]) + 1) for i in range(1, lay.size))
+        return lay, P
+
+    def mlp_eval(self, X: Any, y: Any, layers: Sequence[int], weights: Any) -> Tuple[float, np.ndarray, int]:
+        """One loss-and-gradient evaluation (collective): F(w) and its gradient [P] in Spark's flat layout, n_total."""
+        n, d = self._check_X(X)
+        self._check_y(y, n)
+        lay, P = self._mlp_layers(layers, d)
+        w = np.ascontiguousarray(weights, dtype=np.float64).reshape(-1)
+        if w.shape != (P,):
+            raise ValueError(f"weights must be [{P}]")
+        f = ctypes.c_double(0.0)
+        g = np.zeros(P, dtype=np.float64)
+        nt = ctypes.c_int64(0)
+        with self._torch.cuda.device(self.device):
+            self._check(self._L.b2k_mlp_eval(self._h, X.data_ptr(), y.data_ptr(), n, lay.ctypes.data, int(lay.size),
+                                             w.ctypes.data, ctypes.byref(f), g.ctypes.data, ctypes.byref(nt),
+                                             self._stream()))
+        return float(f.value), g, int(nt.value)
+
+    def mlp_fit(self, X: Any, y: Any, layers: Sequence[int], *, solver: str = "l-bfgs", max_iter: int = 100,
+                tol: float = 1e-6, step_size: float = 0.03, seed: int = 0, initial_weights: Any = None
+                ) -> Dict[str, Any]:
+        """MultilayerPerceptronClassifier.fit (b2k_mlp_fit, collective) -> weights [P], objective_history, n_iter."""
+        n, d = self._check_X(X)
+        self._check_y(y, n)
+        lay, P = self._mlp_layers(layers, d)
+        if solver not in MLP_SOLVERS:
+            raise ValueError(f"solver must be one of {sorted(MLP_SOLVERS)}, got {solver!r}")
+        w0 = None
+        if initial_weights is not None:
+            w0 = np.ascontiguousarray(initial_weights, dtype=np.float64).reshape(-1)
+            if w0.shape != (P,):
+                raise ValueError(f"initialWeights must have {P} values, got {w0.size}")
+        w = np.zeros(P, dtype=np.float64)
+        hist = np.zeros(max(int(max_iter), 0) + 1, dtype=np.float64)
+        it = ctypes.c_int(0)
+        with self._torch.cuda.device(self.device):
+            self._check(self._L.b2k_mlp_fit(
+                self._h, X.data_ptr(), y.data_ptr(), n, lay.ctypes.data, int(lay.size), MLP_SOLVERS[solver],
+                int(max_iter), float(tol), float(step_size), int(seed) & 0xFFFFFFFFFFFFFFFF,
+                w0.ctypes.data if w0 is not None else None, w.ctypes.data, hist.ctypes.data, ctypes.byref(it),
+                self._stream()))
+        return {"weights": w, "objective_history": hist[: it.value].copy(), "n_iter": int(it.value)}
+
+    def mlp_predict(self, X: Any, layers: Sequence[int], weights: Any) -> Tuple[Any, Any, Any]:
+        """rawPrediction [n, C], probability [n, C] and prediction [n] as float64 CUDA tensors."""
+        t = self._torch
+        n, d = self._check_X(X)
+        lay, P = self._mlp_layers(layers, d)
+        w = np.ascontiguousarray(weights, dtype=np.float64).reshape(-1)
+        if w.shape != (P,):
+            raise ValueError(f"weights must be [{P}]")
+        C = int(lay[-1]) if lay.size else 0
+        raw = t.empty((n, C), dtype=t.float64, device=self.device)
+        prob = t.empty((n, C), dtype=t.float64, device=self.device)
+        pred = t.empty((n,), dtype=t.float64, device=self.device)
+        with t.cuda.device(self.device):
+            self._check(self._L.b2k_mlp_predict(self._h, X.data_ptr(), n, lay.ctypes.data, int(lay.size), w.ctypes.data,
+                                                raw.data_ptr(), prob.data_ptr(), pred.data_ptr(), self._stream()))
+        return raw, prob, pred
 
     # -- logistic regression ----------------------------------------------------------------
     def _check_y(self, y: Any, n: int) -> None:

@@ -36,11 +36,12 @@ from typing import Any, Callable, Dict, List, Optional, Sequence, Tuple, Union
 import numpy as np
 import pyarrow as pa
 
-from .core import FitInputType, _CumlModelWithPredictionCol, _DeviceModel, _TunedEstimator, alias, param_alias
+from .core import (FitInputType, _CumlEstimator, _CumlModelWithPredictionCol, _DeviceModel, _TunedEstimator, alias,
+                   param_alias)
 from .params import HasFeaturesCol, HasFeaturesCols, HasLabelCol, HasPredictionCol, P, _CumlClass, _CumlParams
 from .tree import _RandomForestEstimator, _RandomForestModel
-from .sparkshim import LocalDataFrame, Param, Row, TypeConverters, keyword_only
-from .utils import densify_vector_column, is_vector_struct
+from .sparkshim import HAVE_PYSPARK, LocalDataFrame, Param, Row, TypeConverters, keyword_only
+from .utils import densify_vector_column, get_logger, is_vector_struct
 
 
 class LogisticRegressionClass(_CumlClass):
@@ -654,3 +655,348 @@ class RandomForestClassificationModel(_RandomForestModel):
 
     def evaluate(self, dataset: Any) -> Any:
         raise NotImplementedError("RandomForestClassificationModel.evaluate() is not supported in this build")
+
+
+# ---- MultilayerPerceptronClassifier (pyspark.ml.classification; the reference has no multilayer perceptron) ----
+class MultilayerPerceptronClassifierClass(_CumlClass):
+    @classmethod
+    def _param_mapping(cls) -> Dict[str, Optional[str]]:
+        # None = unsupported, "" = accepted and ignored
+        return {"layers": "layers", "maxIter": "max_iter", "tol": "tol", "seed": "random_state", "blockSize": "",
+                "solver": "solver", "stepSize": "step_size", "initialWeights": "initial_weights", "thresholds": None}
+
+    def _get_cuml_params_default(self) -> Dict[str, Any]:
+        return {"layers": None, "max_iter": 100, "tol": 1e-6, "random_state": None, "solver": "l-bfgs",
+                "step_size": 0.03, "initial_weights": None, "verbose": False}
+
+    def _pyspark_class(self) -> Optional[type]:
+        return None  # pyspark.ml.classification.MultilayerPerceptronClassifier when pyspark is installed
+
+
+def _to_int_list(v: Any) -> List[int]:
+    return [int(x) for x in v]
+
+
+def _to_float_list(v: Any) -> List[float]:
+    return [float(x) for x in np.asarray(v, dtype=np.float64).reshape(-1)]
+
+
+class _MultilayerPerceptronCumlParams(_CumlParams, HasFeaturesCol, HasFeaturesCols, HasLabelCol, HasPredictionCol):
+    """Shared Spark Params of MultilayerPerceptronClassifier and its model (Spark's defaults: maxIter=100, tol=1e-6,
+    blockSize=128, solver='l-bfgs', stepSize=0.03, rawPredictionCol='rawPrediction', probabilityCol='probability')."""
+
+    layers = Param("parent", "layers", "Sizes of layers from input layer to output layer.", _to_int_list)
+    maxIter = Param("parent", "maxIter", "max number of iterations (>= 0).", TypeConverters.toInt)
+    tol = Param("parent", "tol", "the convergence tolerance for iterative algorithms (>= 0).", TypeConverters.toFloat)
+    seed = Param("parent", "seed", "random seed.", TypeConverters.toInt)
+    blockSize = Param("parent", "blockSize", "block size for stacking input data in matrices (accepted; the loss is "
+                      "averaged over rows).", TypeConverters.toInt)
+    solver = Param("parent", "solver", "The solver algorithm for optimization. Supported options: l-bfgs, gd.",
+                   TypeConverters.toString)
+    stepSize = Param("parent", "stepSize", "Step size to be used for each iteration of optimization (> 0).",
+                     TypeConverters.toFloat)
+    initialWeights = Param("parent", "initialWeights", "The initial weights of the model.", _to_float_list)
+    rawPredictionCol = Param("parent", "rawPredictionCol", "raw prediction (a.k.a. confidence) column name.",
+                             TypeConverters.toString)
+    probabilityCol = Param("parent", "probabilityCol", "Column name for predicted class conditional probabilities.",
+                           TypeConverters.toString)
+    thresholds = Param("parent", "thresholds", "Thresholds in multi-class classification (not supported).",
+                       _to_float_list)
+
+    def __init__(self) -> None:
+        super().__init__()
+        self._setDefault(maxIter=100, tol=1e-6, blockSize=128, solver="l-bfgs", stepSize=0.03, labelCol="label",
+                         predictionCol="prediction", rawPredictionCol="rawPrediction", probabilityCol="probability")
+        # the KMeans rule: a 32-bit signed seed from the class name
+        self._setDefault(seed=hash(type(self).__name__) & 0x07FFFFFFF)
+
+    def getLayers(self) -> List[int]:
+        return list(self.getOrDefault(self.layers))
+
+    def getMaxIter(self) -> int:
+        return self.getOrDefault(self.maxIter)
+
+    def getTol(self) -> float:
+        return self.getOrDefault(self.tol)
+
+    def getSeed(self) -> int:
+        return self.getOrDefault(self.seed)
+
+    def getBlockSize(self) -> int:
+        return self.getOrDefault(self.blockSize)
+
+    def getSolver(self) -> str:
+        return self.getOrDefault(self.solver)
+
+    def getStepSize(self) -> float:
+        return self.getOrDefault(self.stepSize)
+
+    def getInitialWeights(self) -> Optional[List[float]]:
+        return list(self.getOrDefault(self.initialWeights)) if self.isDefined(self.initialWeights) else None
+
+    def getRawPredictionCol(self) -> str:
+        return self.getOrDefault(self.rawPredictionCol)
+
+    def getProbabilityCol(self) -> str:
+        return self.getOrDefault(self.probabilityCol)
+
+    def getFeaturesCol(self) -> Union[str, List[str]]:  # type: ignore[override]
+        if self.isDefined(self.featuresCols):
+            return self.getFeaturesCols()
+        if self.isDefined(self.featuresCol):
+            return self.getOrDefault("featuresCol")
+        raise RuntimeError("featuresCol is not set")
+
+    def setFeaturesCol(self: P, value: Union[str, List[str]]) -> P:
+        if isinstance(value, str):
+            self._set_params(featuresCol=value)
+        else:
+            self._set_params(featuresCols=value)
+        return self
+
+    def setFeaturesCols(self: P, value: List[str]) -> P:
+        return self._set_params(featuresCols=value)
+
+    def setLabelCol(self: P, value: str) -> P:
+        return self._set_params(labelCol=value)
+
+    def setPredictionCol(self: P, value: str) -> P:
+        return self._set_params(predictionCol=value)
+
+    def setRawPredictionCol(self: P, value: str) -> P:
+        return self._set_params(rawPredictionCol=value)
+
+    def setProbabilityCol(self: P, value: str) -> P:
+        return self._set_params(probabilityCol=value)
+
+    def setThresholds(self: P, value: List[float]) -> P:
+        raise ValueError("'thresholds' is not supported by MultilayerPerceptronClassifier on the GPU.")
+
+
+def _mlp_n_weights(layers: Sequence[int]) -> int:
+    return sum(int(layers[i]) * (int(layers[i - 1]) + 1) for i in range(1, len(layers)))
+
+
+def _refuse_pyspark(dataset: Any, who: str) -> None:
+    if HAVE_PYSPARK:
+        from . import spark_binding
+
+        if spark_binding.is_spark_dataframe(dataset):
+            raise NotImplementedError(f"{who} of a pyspark DataFrame is not supported yet; use a local frame")
+
+
+class MultilayerPerceptronClassifier(MultilayerPerceptronClassifierClass, _CumlEstimator,
+                                     _MultilayerPerceptronCumlParams):
+    """Multilayer perceptron classification on H100, Spark's pyspark.ml.classification.MultilayerPerceptronClassifier:
+    sigmoid hidden layers, a softmax output layer and the cross-entropy loss, trained by L-BFGS (default) or full-batch
+    gradient descent.  Every solver step is one evaluation of the loss and its gradient over the device-resident rows
+    (the layer products and the gradient sums on wgmma 3xTF32 when d % 4 == 0, else in fp64) and one NCCL allreduce.
+    Parameters: layers (required: [numFeatures, hidden..., numClasses]), maxIter (100), tol (1e-6), seed, blockSize
+    (128; accepted, no effect: the loss is averaged over rows, not within blocks), solver ("l-bfgs" | "gd"), stepSize
+    (0.03, gd only), initialWeights (Spark's flat layout), featuresCol / featuresCols, labelCol, predictionCol,
+    rawPredictionCol, probabilityCol, num_workers, verbose.
+
+    Deliberate differences from Spark: without initialWeights the start comes from the library's seeded generator, not
+    XORShiftRandom; a fractional label is an error (Spark truncates it).  thresholds, sparse input, a pyspark DataFrame
+    and CrossValidator / fitMultiple in one pass are not supported.
+
+    >>> from spark_rapids_ml_b200.classification import MultilayerPerceptronClassifier
+    >>> model = MultilayerPerceptronClassifier(layers=[4, 8, 3], seed=1).fit(df)
+    >>> model.transform(df)
+    """
+
+    @keyword_only
+    def __init__(self, *, featuresCol: Union[str, List[str]] = "features", labelCol: str = "label",
+                 predictionCol: str = "prediction", maxIter: int = 100, tol: float = 1e-6, seed: Optional[int] = None,
+                 layers: Optional[List[int]] = None, blockSize: int = 128, stepSize: float = 0.03,
+                 solver: str = "l-bfgs", initialWeights: Optional[Any] = None, probabilityCol: str = "probability",
+                 rawPredictionCol: str = "rawPrediction", thresholds: Optional[List[float]] = None,
+                 num_workers: Optional[int] = None, verbose: Union[int, bool] = False, **kwargs: Any) -> None:
+        super().__init__()
+        self._handle_param_spark_confs()
+        self._input_kwargs.pop("kwargs", None)
+        self._input_kwargs.update(kwargs)
+        for name in ("seed", "num_workers", "layers", "initialWeights", "thresholds"):
+            if self._input_kwargs.get(name, None) is None:
+                self._input_kwargs.pop(name, None)
+        if "thresholds" in self._input_kwargs:
+            raise ValueError("'thresholds' is not supported by MultilayerPerceptronClassifier on the GPU.")
+        if "initialWeights" in self._input_kwargs:
+            self._input_kwargs["initialWeights"] = [float(v) for v in np.asarray(self._input_kwargs["initialWeights"],
+                                                                                 dtype=np.float64).reshape(-1)]
+        self._set_params(**self._input_kwargs)
+
+    def setLayers(self, value: List[int]) -> "MultilayerPerceptronClassifier":
+        return self._set_params(layers=value)
+
+    def setMaxIter(self, value: int) -> "MultilayerPerceptronClassifier":
+        return self._set_params(maxIter=value)
+
+    def setTol(self, value: float) -> "MultilayerPerceptronClassifier":
+        return self._set_params(tol=value)
+
+    def setSeed(self, value: int) -> "MultilayerPerceptronClassifier":
+        return self._set_params(seed=value)
+
+    def setBlockSize(self, value: int) -> "MultilayerPerceptronClassifier":
+        return self._set_params(blockSize=value)
+
+    def setSolver(self, value: str) -> "MultilayerPerceptronClassifier":
+        return self._set_params(solver=value)
+
+    def setStepSize(self, value: float) -> "MultilayerPerceptronClassifier":
+        return self._set_params(stepSize=value)
+
+    def setInitialWeights(self, value: Any) -> "MultilayerPerceptronClassifier":
+        return self._set_params(initialWeights=[float(v) for v in np.asarray(value, dtype=np.float64).reshape(-1)])
+
+    def _validate_parameters(self) -> None:
+        super()._validate_parameters()
+        if not self.isDefined(self.layers):
+            raise ValueError("layers must be set: [numFeatures, hidden layer sizes..., numClasses]")
+        layers = self.getLayers()
+        if len(layers) < 2:
+            raise ValueError(f"layers given invalid value {layers} (must have at least 2 entries)")
+        if any(v < 1 for v in layers):
+            raise ValueError(f"layers given invalid value {layers} (every entry must be > 0)")
+        if self.getMaxIter() < 0:
+            raise ValueError(f"maxIter given invalid value {self.getMaxIter()}")
+        if not self.getTol() >= 0:
+            raise ValueError(f"tol given invalid value {self.getTol()}")
+        if self.getBlockSize() < 1:
+            raise ValueError(f"blockSize given invalid value {self.getBlockSize()}")
+        if self.getSolver() not in ("l-bfgs", "gd"):
+            raise ValueError(f"solver given invalid value {self.getSolver()} (supported: l-bfgs, gd)")
+        if not self.getStepSize() > 0:
+            raise ValueError(f"stepSize given invalid value {self.getStepSize()}")
+        w0 = self.getInitialWeights()
+        if w0 is not None and len(w0) != _mlp_n_weights(layers):
+            raise ValueError(f"initialWeights has {len(w0)} values; layers {layers} need {_mlp_n_weights(layers)}")
+
+    def _fit_label_col(self) -> Optional[str]:
+        return self.getLabelCol()
+
+    def _fit_array_order(self) -> str:
+        return "C"
+
+    def _fit(self, dataset: Any) -> "MultilayerPerceptronClassificationModel":
+        _refuse_pyspark(dataset, "MultilayerPerceptronClassifier.fit")
+        if isinstance(dataset, LocalDataFrame) and _vector_column(dataset, self.getFeaturesCol()) is not None:
+            raise NotImplementedError("MultilayerPerceptronClassifier on sparse input (a vector struct features column) "
+                                      "is not supported")
+        self._validate_parameters()
+        return super()._fit(dataset)  # type: ignore[return-value]
+
+    def _get_cuml_fit_func(self, dataset: Any, extra_params: Optional[List[Dict[str, Any]]] = None
+                           ) -> Callable[[FitInputType, Dict[str, Any]], Dict[str, Any]]:
+        cls = self.__class__
+        layers = self.getLayers()
+        w0 = self.getInitialWeights()
+
+        def _cuml_fit(dfs: FitInputType, params: Dict[str, Any]) -> Dict[str, Any]:
+            ctx = params[param_alias.handle]
+            init = params[param_alias.cuml_init]
+            if len(dfs) != 1:
+                raise RuntimeError("the worker scaffold hands the fit function ONE device matrix per partition")
+            X, y, _ = dfs[0]
+            d = params[param_alias.num_cols]
+            if layers[0] != d:
+                raise ValueError(f"layers[0] = {layers[0]} must equal the number of features {d}")
+            seed = init.get("random_state")
+            out = ctx.mlp_fit(X, y, layers, solver=str(init["solver"]), max_iter=int(init["max_iter"]),
+                              tol=float(init["tol"]), step_size=float(init["step_size"]),
+                              seed=int(seed) if seed is not None else 0, initial_weights=w0)
+            get_logger(cls).info(f"iterations: {out['n_iter']}, loss: {out['objective_history'][-1:]}")
+            return {"weights_": [out["weights"].tolist()], "layers_": [list(layers)],
+                    "objective_history_": [out["objective_history"].tolist()],
+                    "n_cols": [d], "dtype": ["float32"]}
+
+        return _cuml_fit
+
+    def _out_schema(self) -> Any:
+        return "weights_ array<double>, layers_ array<int>, objective_history_ array<double>, n_cols int, dtype string"
+
+    def _create_pyspark_model(self, result: Row) -> "MultilayerPerceptronClassificationModel":
+        r = result.asDict()
+        return MultilayerPerceptronClassificationModel(
+            weights_=[float(v) for v in r["weights_"]], layers_=[int(v) for v in r["layers_"]],
+            objective_history_=[float(v) for v in r["objective_history_"]], n_cols=int(r["n_cols"]),
+            dtype=str(r["dtype"]))
+
+
+class MultilayerPerceptronClassificationTrainingSummary:
+    """The training summary Spark's MultilayerPerceptronClassificationModel.summary() holds: objectiveHistory (F at
+    each accepted iterate) and totalIterations (its length, as Spark reports it)."""
+
+    def __init__(self, objective_history: List[float]) -> None:
+        self.objectiveHistory = list(objective_history)
+        self.totalIterations = len(objective_history)
+
+
+class MultilayerPerceptronClassificationModel(MultilayerPerceptronClassifierClass, _CumlModelWithPredictionCol,
+                                              _MultilayerPerceptronCumlParams):
+    """transform() appends rawPredictionCol (the last layer's affine output, a double vector), probabilityCol (its
+    softmax) and predictionCol (the index of the largest raw value, the lower one on a tie, a double)."""
+
+    def __init__(self, weights_: List[float], layers_: List[int], objective_history_: List[float], n_cols: int,
+                 dtype: str) -> None:
+        super().__init__(n_cols=n_cols, dtype=dtype, weights_=weights_, layers_=layers_,
+                         objective_history_=objective_history_)
+        self.weights_ = weights_
+        self.layers_ = layers_
+        self.objective_history_ = objective_history_
+        self._set_params(layers=list(layers_))
+
+    @property
+    def weights(self) -> Any:
+        return _dense(self.weights_)
+
+    @property
+    def numFeatures(self) -> int:
+        return int(self.layers_[0])
+
+    @property
+    def numClasses(self) -> int:
+        return int(self.layers_[-1])
+
+    @property
+    def hasSummary(self) -> bool:
+        return True
+
+    def summary(self) -> MultilayerPerceptronClassificationTrainingSummary:
+        return MultilayerPerceptronClassificationTrainingSummary(self.objective_history_)
+
+    def predict(self, value: Any) -> float:
+        raise NotImplementedError("MultilayerPerceptronClassificationModel.predict() of a single vector is not "
+                                  "supported; use transform()")
+
+    def predictRaw(self, value: Any) -> Any:
+        raise NotImplementedError("MultilayerPerceptronClassificationModel.predictRaw() of a single vector is not "
+                                  "supported; use transform()")
+
+    def predictProbability(self, value: Any) -> Any:
+        raise NotImplementedError("MultilayerPerceptronClassificationModel.predictProbability() of a single vector is "
+                                  "not supported; use transform()")
+
+    def cpu(self) -> Any:
+        raise NotImplementedError("MultilayerPerceptronClassificationModel.cpu() builds a JVM pyspark.ml model; no "
+                                  "JVM/pyspark in this build")
+
+    def _transform_array_order(self) -> str:
+        return "C"
+
+    def _transform_outputs(self) -> List[Tuple[str, str]]:
+        return [(self.getRawPredictionCol(), "array<double>"), (self.getProbabilityCol(), "array<double>"),
+                (self.getOrDefault("predictionCol"), "double")]
+
+    def _get_cuml_transform_func(self, dataset: Any, eval_metric_info: Any = None
+                                 ) -> Tuple[Callable, Callable, Optional[Callable]]:
+        _refuse_pyspark(dataset, "MultilayerPerceptronClassificationModel.transform")
+        if isinstance(dataset, LocalDataFrame) and _vector_column(dataset, self.getFeaturesCol()) is not None:
+            raise NotImplementedError("MultilayerPerceptronClassificationModel.transform of sparse input (a vector "
+                                      "struct features column) is not supported")
+        layers = list(self.layers_)
+        w = np.asarray(self.weights_, dtype=np.float64)
+        C = layers[-1]
+        return _DeviceModel, self._grouped_transform(lambda m, X: m.ctx.mlp_predict(X, layers, w),
+                                                     4 * int(self.n_cols) + 8 * (2 * C + 1)), None

@@ -1483,3 +1483,53 @@ extern "C" int b2k_bkm_predict(b2k_ctx* ctx, const float* X, int64_t n, int d, i
   return b2k_bkm_predict_impl(ctx, X, n, d, n_nodes, node_index, node_centers, labels_out, cost_out,
                               reinterpret_cast<cudaStream_t>(stream));
 }
+
+// ------------------------------------------------------------------------------------------------
+// multilayer perceptron (b2k_mlp.cu)
+// ------------------------------------------------------------------------------------------------
+extern "C" int b2k_mlp_eval(b2k_ctx* ctx, const float* X, const float* y, int64_t n_local, const int32_t* layers,
+                            int n_layers, const double* weights, double* f_out, double* grad_out, int64_t* n_total_out,
+                            uintptr_t stream) {
+  if (!ctx) return b2k_fail(nullptr, B2K_ERR_INVALID, "b2k_mlp_eval: ctx is NULL");
+  // an empty partition may come with no buffer: the collective check below reports it on every rank
+  if (((!X || !y) && n_local > 0) || n_local < 0 || !weights || !f_out || !grad_out)
+    return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_mlp_eval: bad X/y/n/weights/outputs");
+  B2K_TRY(b2k_mlp_check_layers(ctx, layers, n_layers, layers && n_layers > 0 ? layers[0] : 0));
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  B2K_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  B2K_TRY(check_no_empty_partition(ctx, "b2k_mlp_eval", n_local, s));
+  return b2k_mlp_eval_impl(ctx, X, y, n_local, layers, n_layers, weights, f_out, grad_out, n_total_out, s);
+}
+
+extern "C" int b2k_mlp_fit(b2k_ctx* ctx, const float* X, const float* y, int64_t n_local, const int32_t* layers,
+                           int n_layers, int solver, int max_iter, double tol, double step_size, uint64_t seed,
+                           const double* initial_weights, double* weights_out, double* history_out, int* n_iter_out,
+                           uintptr_t stream) {
+  if (!ctx) return b2k_fail(nullptr, B2K_ERR_INVALID, "b2k_mlp_fit: ctx is NULL");
+  if (((!X || !y) && n_local > 0) || n_local < 0 || !weights_out || !history_out || !n_iter_out)
+    return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_mlp_fit: bad X/y/n/outputs");
+  B2K_TRY(b2k_mlp_check_layers(ctx, layers, n_layers, layers && n_layers > 0 ? layers[0] : 0));
+  if (solver != B2K_MLP_LBFGS && solver != B2K_MLP_GD)
+    return b2k_fail(ctx, B2K_ERR_INVALID, "multilayer perceptron: solver must be l-bfgs or gd");
+  if (max_iter < 0) return b2k_fail(ctx, B2K_ERR_INVALID, "maxIter given invalid value " + std::to_string(max_iter));
+  if (!(tol >= 0.0)) return b2k_fail(ctx, B2K_ERR_INVALID, "multilayer perceptron: tol must be >= 0");
+  if (solver == B2K_MLP_GD && !(step_size > 0.0 && std::isfinite(step_size)))
+    return b2k_fail(ctx, B2K_ERR_INVALID, "multilayer perceptron: stepSize must be > 0");
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  B2K_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  B2K_TRY(check_no_empty_partition(ctx, "b2k_mlp_fit", n_local, s));
+  return b2k_mlp_fit_impl(ctx, X, y, n_local, layers, n_layers, solver, max_iter, tol, step_size, seed, initial_weights,
+                          weights_out, history_out, n_iter_out, s);
+}
+
+extern "C" int b2k_mlp_predict(b2k_ctx* ctx, const float* X, int64_t n, const int32_t* layers, int n_layers,
+                               const double* weights, double* raw_out, double* prob_out, double* pred_out,
+                               uintptr_t stream) {
+  if (!ctx) return b2k_fail(nullptr, B2K_ERR_INVALID, "b2k_mlp_predict: ctx is NULL");
+  if (n < 0 || !weights || (n > 0 && (!X || !raw_out || !prob_out || !pred_out)))
+    return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_mlp_predict: bad X/n/weights/outputs");
+  B2K_TRY(b2k_mlp_check_layers(ctx, layers, n_layers, layers && n_layers > 0 ? layers[0] : 0));
+  B2K_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  return b2k_mlp_predict_impl(ctx, X, n, layers, n_layers, weights, raw_out, prob_out, pred_out,
+                              reinterpret_cast<cudaStream_t>(stream));
+}

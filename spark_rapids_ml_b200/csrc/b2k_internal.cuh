@@ -470,8 +470,10 @@ int b2k_logreg_labels_impl(b2k_ctx* ctx, const float* y, int64_t n, double* clas
 int b2k_logreg_eval_impl(b2k_ctx* ctx, const float* X, const float* y, int64_t n, int d, const double* classes,
                          int n_classes, int kp, const double* W, const double* b, double* loss_out, double* grad_out,
                          int64_t* n_total_out, cudaStream_t s);
+// f_hist (may be NULL): F at the start and at each accepted iterate
 int b2k_logreg_minimize_impl(b2k_logreg_objective fn, void* user, int n, double* x_io, const double* l1, int max_iter,
-                             double tol, int* n_iter_out, int* n_eval_out, double* f_out);
+                             double tol, int* n_iter_out, int* n_eval_out, double* f_out,
+                             std::vector<double>* f_hist = nullptr);
 int b2k_logreg_fit_impl(b2k_ctx* ctx, const float* X, const float* y, int64_t n, int d, const double* classes,
                         const int64_t* counts, int n_classes, int n_fits, const b2k_logreg_params* prm,
                         double* coef_out, double* intercept_out, int* kp_out, int* n_iter_out, cudaStream_t s);
@@ -533,6 +535,21 @@ int b2k_bkm_fit_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, int k, int 
                      int64_t* cluster_sizes_out, double* level_ms_out, cudaStream_t s);
 int b2k_bkm_predict_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, int n_nodes, const int64_t* node_index,
                          const double* node_centers, int32_t* labels_out, double* cost_out, cudaStream_t s);
+
+// ------------------------------------------------------------------------------------------------
+// multilayer perceptron — b2k_mlp.cu (the C ABI entry points in b2k_api.cu check their arguments and the partitions,
+// then call these; layers are checked by b2k_mlp_check_layers)
+// ------------------------------------------------------------------------------------------------
+int b2k_mlp_check_layers(b2k_ctx* ctx, const int* layers, int n_layers, int d);
+int64_t b2k_mlp_n_weights(const int* layers, int n_layers);
+int b2k_mlp_eval_impl(b2k_ctx* ctx, const float* X, const float* y, int64_t n, const int* layers, int n_layers,
+                      const double* weights, double* f_out, double* grad_out, int64_t* n_total_out, cudaStream_t s);
+int b2k_mlp_fit_impl(b2k_ctx* ctx, const float* X, const float* y, int64_t n, const int* layers, int n_layers,
+                     int solver, int max_iter, double tol, double step_size, uint64_t seed,
+                     const double* initial_weights, double* weights_out, double* history_out, int* n_iter_out,
+                     cudaStream_t s);
+int b2k_mlp_predict_impl(b2k_ctx* ctx, const float* X, int64_t n, const int* layers, int n_layers,
+                         const double* weights, double* raw_out, double* prob_out, double* pred_out, cudaStream_t s);
 
 // ------------------------------------------------------------------------------------------------
 // evaluation — b2k_eval.cu (the C ABI entry points in b2k_api.cu check their arguments, then call these)

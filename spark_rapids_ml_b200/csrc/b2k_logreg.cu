@@ -526,7 +526,7 @@ double interpolate(double a, double fa, double da, double b, double fb, double d
 }  // namespace
 
 int b2k_logreg_minimize_impl(b2k_logreg_objective fn, void* user, int n, double* x_io, const double* l1, int max_iter,
-                             double tol, int* n_iter_out, int* n_eval_out, double* f_out) {
+                             double tol, int* n_iter_out, int* n_eval_out, double* f_out, std::vector<double>* f_hist) {
   auto fail = [](int code, const std::string& msg) { return b2k_fail(nullptr, code, msg); };
   if (!fn || !x_io || n < 1) return fail(B2K_ERR_INVALID, "b2k_logreg_minimize: NULL objective / x or n < 1");
   if (max_iter < 0) return fail(B2K_ERR_INVALID, "maxIter given invalid value " + std::to_string(max_iter));
@@ -544,6 +544,7 @@ int b2k_logreg_minimize_impl(b2k_logreg_objective fn, void* user, int n, double*
   double F = f + obj.l1_term(x);   // Breeze's adjusted value
   obj.pseudo_grad(x, g, &pg);
   const double F0 = F;
+  if (f_hist) f_hist->assign(1, F);
   std::vector<std::vector<double>> S, Y;   // curvature pairs, oldest first
   std::vector<double> fhist{INFINITY};
   int iter = 0;
@@ -684,6 +685,7 @@ int b2k_logreg_minimize_impl(b2k_logreg_objective fn, void* user, int n, double*
     F = owl ? Fn : f;
     obj.pseudo_grad(x, g, &pg);
     ++iter;
+    if (f_hist) f_hist->push_back(F);
     fhist.push_back(F);
     if ((int)fhist.size() > FVAL_MEMORY) fhist.erase(fhist.begin());
   }
