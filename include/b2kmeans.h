@@ -56,6 +56,8 @@
  *                               computeCost)
  *   b2k_mlp_eval / _fit /       none: the reference has no multilayer perceptron; stands in for Spark's
  *     _predict                  pyspark.ml.classification.MultilayerPerceptronClassifier (fit and the model's transform)
+ *   b2k_als_fit / _predict /    none: the reference has no recommender; stands in for Spark's
+ *     _recommend                pyspark.ml.recommendation.ALS (fit, ALSModel.transform and the recommendFor* calls)
  *   b2k_silhouette_multi        none: the reference tunes KMeans with pyspark's CrossValidator, scoring each model on
  *                               the CPU; here one device pass scores every model of a param grid
  *
@@ -1004,6 +1006,77 @@ int b2k_mlp_fit(b2k_ctx* ctx, const float* X, const float* y, int64_t n_local, c
                 double* weights_out, double* history_out, int* n_iter_out, uintptr_t stream);
 int b2k_mlp_predict(b2k_ctx* ctx, const float* X, int64_t n, const int32_t* layers, int n_layers, const double* weights,
                     double* raw_out, double* prob_out, double* pred_out, uintptr_t stream);
+
+/* ---- ALS (alternating least squares collaborative filtering) ----
+ * Stands in for pyspark.ml.recommendation.ALS (the reference has none); its rules are restated here so that no Spark
+ * source is needed.
+ *
+ * Input: per rank, n_local (user, item, rating) triples.  users / items are device f64 [n_local] (any numeric column,
+ * cast): each value must be integral and inside int32, else B2K_ERR_INVALID with Spark's message ("ALS only supports
+ * values in Integer range and without fractional part for column user. Value v was either out of Integer range or
+ * contained a fractional part that could not be converted.").  ratings is device f32 [n_local], or NULL for every rating
+ * 1.0; a non-finite rating is B2K_ERR_INVALID.  Duplicate (user, item) pairs are all kept, each a separate rating.  The
+ * sizes and the first bad value of every rank are allgathered first, so every error fails on every rank.  A rank may
+ * hold no ratings; the whole dataset may not be empty.
+ * Indexing: users are the sorted distinct user ids over all ranks (dense index u), items likewise (dense index i).
+ * Start: without init_user_factors, user u's factor is x_j = fl32(v_j / sqrt(sum_j v_j^2)) (the sum in fp64, in j order),
+ * v_j = fl32(sqrt(-2 ln u1) cos(2 pi u2)) for j < rank, where h = splitmix64(splitmix64(splitmix64(seed) ^ id) ^ j)
+ * (id the raw user id as uint32, splitmix64 as for b2k_gmm_fit), u1 = ((h >> 11) + 1) 2^-53, u2 = (splitmix64(h) >> 11)
+ * 2^-53.  Spark draws from XORShiftRandom per block: the start differs from Spark's for the same seed (deliberate), and
+ * depends on neither the rank count nor the partitioning.  The item factors need no start.
+ * Iteration (max_iter >= 0 times, Spark's order): solve every item from the user factors, then every user from the item
+ * factors.  For destination d over its ratings (s, r), with source factors y_s:
+ *   explicit: A = sum y_s y_s^T, b = sum r y_s, n = #ratings;
+ *   implicit: c1 = alpha |r|, A = Y^T Y + sum c1 y_s y_s^T, b = sum_{r > 0} (1 + c1) y_s, n = #{r > 0}, Y^T Y the Gram of
+ *   every source factor;
+ *   then (A + reg_param n I) x = b by Cholesky, accumulated and solved in fp64 from the fp32 factors, x stored as fp32.
+ *   A system that is not positive definite (reg_param = 0 with fewer ratings than rank, say) fails on every rank
+ *   (B2K_ERR_INVALID), as Spark's solver fails.  With max_iter = 0 the item factors are zero.
+ * Distribution: rank q owns users [U q / R, U (q + 1) / R) and items likewise.  The ratings travel by chunked allgathers
+ * (2^22 per rank per round); each rank keeps those of its users sorted by (user, item, global row) and of its items by
+ * (item, user, global row), global row = the rank's offset + local row.  Per rank the fit holds: the n_local triples
+ * (12 B each, freed after the redistribution), both full factor tables ((U + I) rank 4 B), its own ratings twice (12 B
+ * each, plus 24 B each and the sort buffers while it sorts them), one round's buffers (R 2^22 x 88 B at most) and at most
+ * 1 GB of fp64 unit partials (more only when one destination needs more).  Each half-step every rank holds the whole
+ * source table, forms Y^T Y over all of it (no allreduce: the result does not depend on the rank count), solves the
+ * destinations it owns and allgathers them.  No pass uses atomics: the factors are bitwise identical for the same input
+ * on any rank count and any option "grid_limit" (a cap on the CTAs of the normal-equation and solve passes).
+ * Device passes: the normal-equation pass runs over units of at most 512 ratings of one destination; each unit sums the
+ * upper triangle of A, b and n in fp64 FMA (the fp32 products are exact in fp64, so only the order of the additions
+ * matters, and it is the rating order), a long destination spanning several units that the solve pass folds in unit
+ * order; Y^T Y comes from the local generic Gram pass; the solve pass runs one CTA per destination on [A | b] in shared
+ * memory.  1 <= rank <= B2K_ALS_MAX_RANK, else B2K_ERR_UNSUPPORTED.
+ *
+ * b2k_als_fit (collective): outputs on the device, sized by the caller: user_ids_out [user_cap] i32, user_factors_out
+ * [user_cap][rank] f32, item_ids_out [item_cap], item_factors_out [item_cap][rank]; *n_users_out = U and *n_items_out = I
+ * (host), set also when a cap is too small (then B2K_ERR_INVALID on every rank, so a caller can size and call again).
+ * init_user_factors (host f32 [init_n_users][rank], in sorted user-id order; NULL: the seeded start) must have
+ * init_n_users == U.  Errors also: max_iter < 0, reg_param < 0 or not finite, alpha < 0 or not finite (implicit).
+ * Synchronises `stream`.  Stats: last_n_iter; with option "time_kernels": last_fused_ms, last_finalize_ms,
+ * last_allreduce_ms and last_reduce_ms = the mean device time per half-step of the normal-equation pass, the solve pass,
+ * the factor allgather and the Y^T Y pass; last_probe_ms = the setup (check, id maps, redistribution, sorts) and
+ * last_loop_ms = the whole call (host clock).
+ *
+ * b2k_als_predict (local, asynchronous on `stream`): out [n] f32 = for each (users[j], items[j]) (device f64) the fp32
+ * dot product s = fl32(s + fl32(u_k v_k)) in k order of the user's and the item's factors, looked up in the sorted id
+ * maps (device i32 [n_users] / [n_items] with their factor tables); NaN when either id is unknown, fractional or outside
+ * int32.
+ *
+ * b2k_als_recommend (local, asynchronous): for each query row q of Q [nq][rank] (device f32), the n best rows of T
+ * [nt][rank] by the same dot product, score descending, the lower row first on a tie: idx_out [nq][n] i32 (-1 past nt)
+ * and score_out [nq][n] f32 (NaN past nt).  1 <= n <= B2K_ALS_MAX_N. */
+#define B2K_ALS_MAX_RANK 128
+#define B2K_ALS_MAX_N 1024
+int b2k_als_fit(b2k_ctx* ctx, const double* users, const double* items, const float* ratings, int64_t n_local,
+                int rank, int max_iter, double reg_param, int implicit_prefs, double alpha, uint64_t seed,
+                const float* init_user_factors, int64_t init_n_users, int64_t user_cap, int64_t item_cap,
+                int32_t* user_ids_out, float* user_factors_out, int32_t* item_ids_out, float* item_factors_out,
+                int64_t* n_users_out, int64_t* n_items_out, uintptr_t stream);
+int b2k_als_predict(b2k_ctx* ctx, const double* users, const double* items, int64_t n, int rank,
+                    const int32_t* user_ids, const float* user_factors, int64_t n_users, const int32_t* item_ids,
+                    const float* item_factors, int64_t n_items, float* out, uintptr_t stream);
+int b2k_als_recommend(b2k_ctx* ctx, const float* Q, int64_t nq, const float* T, int64_t nt, int rank, int n,
+                      int32_t* idx_out, float* score_out, uintptr_t stream);
 
 #ifdef __cplusplus
 }

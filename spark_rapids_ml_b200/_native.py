@@ -89,7 +89,13 @@ EXPORTED_SYMBOLS = (
     "b2k_mlp_eval",
     "b2k_mlp_fit",
     "b2k_mlp_predict",
+    "b2k_als_fit",
+    "b2k_als_predict",
+    "b2k_als_recommend",
 )
+
+ALS_MAX_RANK = 128   # B2K_ALS_MAX_RANK
+ALS_MAX_N = 1024     # B2K_ALS_MAX_N
 
 MLP_SOLVERS = {"l-bfgs": 0, "gd": 1}   # b2k_mlp_solver
 
@@ -292,6 +298,10 @@ def load_library() -> ctypes.CDLL:
     L.b2k_mlp_fit.argtypes = [vp, vp, vp, i64, vp, i32, i32, i32, f64, f64, u64, vp, vp, vp, ctypes.POINTER(i32),
                               ctypes.c_size_t]
     L.b2k_mlp_predict.argtypes = [vp, vp, i64, vp, i32, vp, vp, vp, vp, ctypes.c_size_t]
+    L.b2k_als_fit.argtypes = [vp, vp, vp, vp, i64, i32, i32, f64, i32, f64, u64, vp, i64, i64, i64, vp, vp, vp, vp,
+                              ctypes.POINTER(i64), ctypes.POINTER(i64), ctypes.c_size_t]
+    L.b2k_als_predict.argtypes = [vp, vp, vp, i64, i32, vp, vp, i64, vp, vp, i64, vp, ctypes.c_size_t]
+    L.b2k_als_recommend.argtypes = [vp, vp, i64, vp, i64, i32, i32, vp, vp, ctypes.c_size_t]
     for name in EXPORTED_SYMBOLS:
         if name not in ("b2k_last_error",):
             getattr(L, name).restype = i32
@@ -881,6 +891,84 @@ class Context:
             self._check(self._L.b2k_mlp_predict(self._h, X.data_ptr(), n, lay.ctypes.data, int(lay.size), w.ctypes.data,
                                                 raw.data_ptr(), prob.data_ptr(), pred.data_ptr(), self._stream()))
         return raw, prob, pred
+
+    # -- ALS ------------------------------------------------------------------------------------
+    def _als_col(self, v: Any, n: int, dtype: Any, name: str) -> Any:
+        t = self._torch
+        if not (isinstance(v, t.Tensor) and v.is_cuda and v.dtype == dtype and v.dim() == 1 and v.is_contiguous()
+                and v.shape[0] == n):
+            raise ValueError(f"{name} must be a contiguous 1-D {dtype} CUDA tensor of {n} values")
+        return v
+
+    def als_fit(self, users: Any, items: Any, ratings: Any, *, rank: int = 10, max_iter: int = 10,
+                reg_param: float = 0.1, implicit_prefs: bool = False, alpha: float = 1.0, seed: int = 0,
+                init_user_factors: Any = None) -> Dict[str, Any]:
+        """ALS.fit (b2k_als_fit, collective): users / items float64 and ratings float32 (or None: every rating 1.0)
+        CUDA tensors of this rank's triples -> user_ids [U] int32, user_factors [U, rank] float32, item_ids [I],
+        item_factors [I, rank] (CUDA tensors, sorted by id).  init_user_factors: [U, rank] float32 in user-id order."""
+        t = self._torch
+        n = int(users.shape[0]) if users is not None else 0
+        self._als_col(users, n, t.float64, "users")
+        self._als_col(items, n, t.float64, "items")
+        if ratings is not None:
+            self._als_col(ratings, n, t.float32, "ratings")
+        w0, nw = None, 0
+        if init_user_factors is not None:
+            w0 = np.ascontiguousarray(init_user_factors, dtype=np.float32)
+            if w0.ndim != 2 or w0.shape[1] != int(rank):
+                raise ValueError(f"init_user_factors must be [n_users, {rank}]")
+            nw = int(w0.shape[0])
+        nu, ni = ctypes.c_int64(0), ctypes.c_int64(0)
+        cap_u = cap_i = max(min(n, 1 << 20), nw, 1)
+        for _ in range(2):   # a cap too small fails on every rank with the sizes set: every rank calls again with them
+            uid = t.empty(max(cap_u, 1), dtype=t.int32, device=self.device)
+            uf = t.empty((max(cap_u, 1), int(rank)), dtype=t.float32, device=self.device)
+            iid = t.empty(max(cap_i, 1), dtype=t.int32, device=self.device)
+            itf = t.empty((max(cap_i, 1), int(rank)), dtype=t.float32, device=self.device)
+            with t.cuda.device(self.device):
+                rc = self._L.b2k_als_fit(
+                    self._h, users.data_ptr() if n else None, items.data_ptr() if n else None,
+                    ratings.data_ptr() if (ratings is not None and n) else None, n, int(rank), int(max_iter),
+                    float(reg_param), int(bool(implicit_prefs)), float(alpha), int(seed) & 0xFFFFFFFFFFFFFFFF,
+                    w0.ctypes.data if w0 is not None else None, nw, cap_u, cap_i, uid.data_ptr(), uf.data_ptr(),
+                    iid.data_ptr(), itf.data_ptr(), ctypes.byref(nu), ctypes.byref(ni), self._stream())
+            if rc != B2K_OK and (self._L.b2k_last_error(self._h) or b"").startswith(b"ALS: the outputs hold fewer"):
+                cap_u, cap_i = max(cap_u, nu.value), max(cap_i, ni.value)
+                continue
+            self._check(rc)
+            break
+        U, I = int(nu.value), int(ni.value)
+        return {"user_ids": uid[:U], "user_factors": uf[:U], "item_ids": iid[:I], "item_factors": itf[:I]}
+
+    def als_predict(self, users: Any, items: Any, user_ids: Any, user_factors: Any, item_ids: Any,
+                    item_factors: Any) -> Any:
+        """ALSModel.transform's prediction (b2k_als_predict): float32 [n], NaN for an unknown id."""
+        t = self._torch
+        n = int(users.shape[0])
+        self._als_col(users, n, t.float64, "users")
+        self._als_col(items, n, t.float64, "items")
+        rank = int(user_factors.shape[1])
+        out = t.empty(n, dtype=t.float32, device=self.device)
+        with t.cuda.device(self.device):
+            self._check(self._L.b2k_als_predict(self._h, users.data_ptr(), items.data_ptr(), n, rank,
+                                                user_ids.data_ptr(), user_factors.data_ptr(), int(user_ids.shape[0]),
+                                                item_ids.data_ptr(), item_factors.data_ptr(), int(item_ids.shape[0]),
+                                                out.data_ptr(), self._stream()))
+        return out
+
+    def als_recommend(self, Q: Any, T: Any, n: int) -> Tuple[Any, Any]:
+        """The n best rows of T [nt, rank] for each row of Q [nq, rank] (b2k_als_recommend): row indices [nq, n] int32
+        (-1 past nt) and scores [nq, n] float32, score descending, the lower row first on a tie."""
+        t = self._torch
+        nq, rank = int(Q.shape[0]), int(Q.shape[1])
+        nt = int(T.shape[0])
+        idx = t.empty((nq, int(n)), dtype=t.int32, device=self.device)
+        sc = t.empty((nq, int(n)), dtype=t.float32, device=self.device)
+        with t.cuda.device(self.device):
+            self._check(self._L.b2k_als_recommend(self._h, Q.data_ptr() if nq else None, nq,
+                                                  T.data_ptr() if nt else None, nt, rank, int(n), idx.data_ptr(),
+                                                  sc.data_ptr(), self._stream()))
+        return idx, sc
 
     # -- logistic regression ----------------------------------------------------------------
     def _check_y(self, y: Any, n: int) -> None:

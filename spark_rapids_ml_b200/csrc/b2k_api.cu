@@ -1533,3 +1533,61 @@ extern "C" int b2k_mlp_predict(b2k_ctx* ctx, const float* X, int64_t n, const in
   return b2k_mlp_predict_impl(ctx, X, n, layers, n_layers, weights, raw_out, prob_out, pred_out,
                               reinterpret_cast<cudaStream_t>(stream));
 }
+
+// ------------------------------------------------------------------------------------------------
+// ALS (b2k_als.cu)
+// ------------------------------------------------------------------------------------------------
+extern "C" int b2k_als_fit(b2k_ctx* ctx, const double* users, const double* items, const float* ratings,
+                           int64_t n_local, int rank, int max_iter, double reg_param, int implicit_prefs, double alpha,
+                           uint64_t seed, const float* init_user_factors, int64_t init_n_users, int64_t user_cap,
+                           int64_t item_cap, int32_t* user_ids_out, float* user_factors_out, int32_t* item_ids_out,
+                           float* item_factors_out, int64_t* n_users_out, int64_t* n_items_out, uintptr_t stream) {
+  if (!ctx) return b2k_fail(nullptr, B2K_ERR_INVALID, "b2k_als_fit: ctx is NULL");
+  if (n_local < 0 || ((!users || !items) && n_local > 0) || !n_users_out || !n_items_out || user_cap < 0 ||
+      item_cap < 0 || ((!user_ids_out || !user_factors_out) && user_cap > 0) ||
+      ((!item_ids_out || !item_factors_out) && item_cap > 0))
+    return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_als_fit: bad users/items/n/outputs");
+  if (rank < 1) return b2k_fail(ctx, B2K_ERR_INVALID, "ALS: rank must be >= 1, got " + std::to_string(rank));
+  if (rank > B2K_ALS_MAX_RANK)
+    return b2k_fail(ctx, B2K_ERR_UNSUPPORTED, "ALS supports rank <= " + std::to_string(B2K_ALS_MAX_RANK) + ", got " +
+                                                  std::to_string(rank));
+  if (max_iter < 0) return b2k_fail(ctx, B2K_ERR_INVALID, "maxIter given invalid value " + std::to_string(max_iter));
+  if (!(reg_param >= 0.0) || !std::isfinite(reg_param))
+    return b2k_fail(ctx, B2K_ERR_INVALID, "regParam given invalid value " + std::to_string(reg_param));
+  if (implicit_prefs && (!(alpha >= 0.0) || !std::isfinite(alpha)))
+    return b2k_fail(ctx, B2K_ERR_INVALID, "alpha given invalid value " + std::to_string(alpha));
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  B2K_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  return b2k_als_fit_impl(ctx, users, items, ratings, n_local, rank, max_iter, reg_param, implicit_prefs, alpha, seed,
+                          init_user_factors, init_n_users, user_cap, item_cap, user_ids_out, user_factors_out,
+                          item_ids_out, item_factors_out, n_users_out, n_items_out, s);
+}
+
+extern "C" int b2k_als_predict(b2k_ctx* ctx, const double* users, const double* items, int64_t n, int rank,
+                               const int32_t* user_ids, const float* user_factors, int64_t n_users,
+                               const int32_t* item_ids, const float* item_factors, int64_t n_items, float* out,
+                               uintptr_t stream) {
+  if (!ctx) return b2k_fail(nullptr, B2K_ERR_INVALID, "b2k_als_predict: ctx is NULL");
+  if (n < 0 || n_users < 0 || n_items < 0 || (n > 0 && (!users || !items || !out)) ||
+      (n_users > 0 && (!user_ids || !user_factors)) || (n_items > 0 && (!item_ids || !item_factors)))
+    return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_als_predict: bad ids/factors/n/out");
+  if (rank < 1 || rank > B2K_ALS_MAX_RANK)
+    return b2k_fail(ctx, rank < 1 ? B2K_ERR_INVALID : B2K_ERR_UNSUPPORTED, "b2k_als_predict: bad rank");
+  B2K_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  return b2k_als_predict_impl(ctx, users, items, n, rank, user_ids, user_factors, n_users, item_ids, item_factors,
+                              n_items, out, reinterpret_cast<cudaStream_t>(stream));
+}
+
+extern "C" int b2k_als_recommend(b2k_ctx* ctx, const float* Q, int64_t nq, const float* T, int64_t nt, int rank, int n,
+                                 int32_t* idx_out, float* score_out, uintptr_t stream) {
+  if (!ctx) return b2k_fail(nullptr, B2K_ERR_INVALID, "b2k_als_recommend: ctx is NULL");
+  if (nq < 0 || nt < 0 || nt > INT32_MAX || (nq > 0 && (!Q || !idx_out || !score_out)) || (nt > 0 && !T))
+    return b2k_fail(ctx, B2K_ERR_INVALID, "b2k_als_recommend: bad Q/T/n/outputs");
+  if (n < 1 || n > B2K_ALS_MAX_N)
+    return b2k_fail(ctx, B2K_ERR_UNSUPPORTED, "ALS recommendations support 1 <= numItems/numUsers <= " +
+                                                  std::to_string(B2K_ALS_MAX_N) + ", got " + std::to_string(n));
+  if (rank < 1 || rank > B2K_ALS_MAX_RANK)
+    return b2k_fail(ctx, rank < 1 ? B2K_ERR_INVALID : B2K_ERR_UNSUPPORTED, "b2k_als_recommend: bad rank");
+  B2K_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+  return b2k_als_recommend_impl(ctx, Q, nq, T, nt, rank, n, idx_out, score_out, reinterpret_cast<cudaStream_t>(stream));
+}

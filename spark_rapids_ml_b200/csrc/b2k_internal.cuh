@@ -91,9 +91,9 @@ struct b2k_ctx {
   b2k_stats stats{};
 };
 
-// The library's counter-based generator (host): Gaussian mixtures draw their start rows from it, bisecting k-means its
-// split starts.
-inline uint64_t b2k_splitmix64(uint64_t z) {
+// The library's counter-based generator (host and device): Gaussian mixtures draw their start rows from it, bisecting
+// k-means its split starts, ALS its start factors.
+__host__ __device__ inline uint64_t b2k_splitmix64(uint64_t z) {
   z += 0x9e3779b97f4a7c15ull;
   z = (z ^ (z >> 30)) * 0xbf58476d1ce4e5b9ull;
   z = (z ^ (z >> 27)) * 0x94d049bb133111ebull;
@@ -314,6 +314,9 @@ int b2k_pca_finalize_impl(b2k_ctx* ctx, const double* cov, int d, int64_t n_tota
                           double* evr_out, double* sv_out);
 int b2k_pca_transform_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, const float* C, int k, float* Y,
                            cudaStream_t s);
+// G [d][d] (device) = X^T X in fp64 over this rank's rows only (no collective): the generic Gram pass with a zero mean,
+// its row spans a function of (n, d) alone.  Uses ctx->scratch.
+int b2k_gram_local_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, double* G, cudaStream_t s);
 
 // ------------------------------------------------------------------------------------------------
 // exact k-NN — b2k_knn.cu (the C ABI entry point in b2k_api.cu checks its arguments, then calls this)
@@ -550,6 +553,20 @@ int b2k_mlp_fit_impl(b2k_ctx* ctx, const float* X, const float* y, int64_t n, co
                      cudaStream_t s);
 int b2k_mlp_predict_impl(b2k_ctx* ctx, const float* X, int64_t n, const int* layers, int n_layers,
                          const double* weights, double* raw_out, double* prob_out, double* pred_out, cudaStream_t s);
+
+// ------------------------------------------------------------------------------------------------
+// ALS — b2k_als.cu (the C ABI entry points in b2k_api.cu check their arguments, then call these)
+// ------------------------------------------------------------------------------------------------
+int b2k_als_fit_impl(b2k_ctx* ctx, const double* users, const double* items, const float* ratings, int64_t n,
+                     int rank, int max_iter, double reg_param, int implicit_prefs, double alpha, uint64_t seed,
+                     const float* init_user_factors, int64_t init_n_users, int64_t user_cap, int64_t item_cap,
+                     int32_t* user_ids_out, float* user_factors_out, int32_t* item_ids_out, float* item_factors_out,
+                     int64_t* n_users_out, int64_t* n_items_out, cudaStream_t s);
+int b2k_als_predict_impl(b2k_ctx* ctx, const double* users, const double* items, int64_t n, int rank,
+                         const int32_t* user_ids, const float* user_factors, int64_t n_users, const int32_t* item_ids,
+                         const float* item_factors, int64_t n_items, float* out, cudaStream_t s);
+int b2k_als_recommend_impl(b2k_ctx* ctx, const float* Q, int64_t nq, const float* T, int64_t nt, int rank, int n,
+                           int32_t* idx_out, float* score_out, cudaStream_t s);
 
 // ------------------------------------------------------------------------------------------------
 // evaluation — b2k_eval.cu (the C ABI entry points in b2k_api.cu check their arguments, then call these)

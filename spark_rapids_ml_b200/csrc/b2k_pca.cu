@@ -632,3 +632,30 @@ int b2k_pca_transform_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, const
   ctx->stats.kernel_launches++;
   return B2K_OK;
 }
+
+int b2k_gram_local_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, double* G, cudaStream_t s) {
+  // the generic pass's span count, as b2k_moments_impl plans it: a function of (n, d) only
+  const size_t dd = (size_t)d * d;
+  const int S = (int)std::max<int64_t>(1, std::min<int64_t>({64, (int64_t)((64u << 20) / (dd * 8)), (n + GG_T - 1) / GG_T}));
+  const int64_t gspan = std::max<int64_t>(1, (n + S - 1) / S);
+  double* part;
+  float* zero;
+  B2K_TRY(b2k_scratch_layout(ctx, "b2k_gram_local", [&](B2kLayout& L) -> int {
+    part = L.take<double>((size_t)S * dd);
+    zero = L.take<float>((size_t)d);
+    return B2K_OK;
+  }));
+  B2K_CUDA_OK(ctx, cudaMemsetAsync(zero, 0, (size_t)d * 4, s));
+  const int nb = (d + GG_T - 1) / GG_T;
+  if (n > 0) {
+    k_gram_generic<<<dim3(nb * (nb + 1) / 2, S), 256, 0, s>>>(X, n, d, zero, gspan, part);
+    B2K_CUDA_OK(ctx, cudaGetLastError());
+    ctx->stats.kernel_launches++;
+  } else {
+    B2K_CUDA_OK(ctx, cudaMemsetAsync(part, 0, (size_t)S * dd * 8, s));
+  }
+  k_gram_fold_generic<<<(int)((dd + 255) / 256), 256, 0, s>>>(part, S, d, G);
+  B2K_CUDA_OK(ctx, cudaGetLastError());
+  ctx->stats.kernel_launches++;
+  return B2K_OK;
+}
