@@ -295,7 +295,7 @@ __global__ void __launch_bounds__(ALS_SOLVE_NT) k_als_solve(const double* __rest
         } else if (j <= i) {
           const size_t off = (size_t)tile_index(j >> 2, i >> 2, nb) * 16 + (j & 3) * 4 + (i & 3);
           for (int64_t u = u0; u < u1; ++u) s += part[u * PS + off];
-          if (YtY) s += YtY[(size_t)i * rank + j];
+          if (YtY) s += YtY[j * (2 * rank - j + 1) / 2 + (i - j)];   // (j, i) of the packed upper triangle
         }
         A[e] = s;
       } else {
@@ -937,7 +937,7 @@ int b2k_als_fit_impl(b2k_ctx* ctx, const double* users, const double* items, con
   int32_t* sbad;
   B2K_TRY(dalloc(ctx, uf_b, (size_t)U * rank, s, &UF));
   B2K_TRY(dalloc(ctx, if_b, (size_t)I * rank, s, &IF));
-  B2K_TRY(dalloc(ctx, ytY_b, (size_t)rank * rank, s, &YtY));
+  B2K_TRY(dalloc(ctx, ytY_b, (size_t)rank * (rank + 1) / 2, s, &YtY));
   B2K_TRY(dalloc(ctx, bad_b2, (size_t)std::max<int64_t>(1, std::max(US.nd, IS.nd)), s, &sbad));
   B2K_TRY(dalloc(ctx, nbad_b, 1, s, &nbad));
   if (R > 1) B2K_TRY(dalloc(ctx, g_b, (size_t)R * ((std::max(U, I) + R - 1) / R + 1) * rank, s, &gbuf));

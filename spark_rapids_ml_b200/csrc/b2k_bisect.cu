@@ -349,26 +349,6 @@ k_bkm_predict(const float* __restrict__ X, int64_t n, int d, const double* __res
   }
 }
 
-// part[span][j] = rows of the span in leaf j (thread j counts, every thread reads each label)
-__global__ void __launch_bounds__(256) k_bkm_sizes(const int32_t* __restrict__ labels, int64_t n, int nl,
-                                                   int64_t span_rows, double* __restrict__ part) {
-  const int64_t r0 = (int64_t)blockIdx.x * span_rows;
-  const int64_t r1 = min(n, r0 + span_rows);
-  for (int j = threadIdx.x; j < nl; j += blockDim.x) {
-    int64_t c = 0;
-    for (int64_t row = r0; row < r1; ++row) c += labels[row] == j;
-    part[(size_t)blockIdx.x * nl + j] = (double)c;
-  }
-}
-
-__global__ void k_bkm_sizes_fold(const double* __restrict__ part, int spans, int nl, double* __restrict__ out) {
-  const int j = blockIdx.x * blockDim.x + threadIdx.x;
-  if (j >= nl) return;
-  double t = 0.0;
-  for (int s = 0; s < spans; ++s) t += part[(size_t)s * nl + j];
-  out[j] = t;
-}
-
 // ---------------------------------------------------------------------------------------------------------------------
 // host
 // ---------------------------------------------------------------------------------------------------------------------
@@ -552,8 +532,7 @@ int b2k_bkm_fit_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, int k, int 
   BkmUnit* units;
   double *parent, *child, *summ, *buf, *part, *spart;
   BkmTreeDev tree{};
-  int cspans = (int)std::min<int64_t>(8 * ctx->sm_count, std::max<int64_t>(1, (n + 63) / 64));
-  const int64_t cspan_rows = std::max<int64_t>(1, (n + cspans - 1) / cspans);
+  const int cspans = b2k_row_spans(ctx, n, 1).spans;   // of b2k_launch_label_counts
   B2K_TRY(b2k_scratch_layout(ctx, "b2k_bkm_fit", [&](B2kLayout& L) -> int {
     perm[0] = L.take<int32_t>((size_t)n);
     perm[1] = L.take<int32_t>((size_t)n);
@@ -774,11 +753,7 @@ int b2k_bkm_fit_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, int k, int 
   B2K_TRY(bkm_tree_upload(ctx, tree, nn, d, hc.data(), kid, leaf, s));
   B2K_TRY(bkm_predict_launch(ctx, tree, X, n, d, labels, nullptr, s));
   double* sizes = spart + (size_t)cspans * k;
-  k_bkm_sizes<<<cspans, 256, 0, s>>>(labels, n, nleaves, cspan_rows, spart);
-  B2K_CUDA_OK(ctx, cudaGetLastError());
-  k_bkm_sizes_fold<<<(nleaves + 255) / 256, 256, 0, s>>>(spart, cspans, nleaves, sizes);
-  B2K_CUDA_OK(ctx, cudaGetLastError());
-  ctx->stats.kernel_launches += 2;
+  B2K_TRY(b2k_launch_label_counts(ctx, labels, n, nleaves, spart, sizes, s));
   B2K_TRY(b2k_comm_allreduce_f64(ctx, sizes, (size_t)nleaves, s));
   std::vector<double> hsz(nleaves);
   B2K_CUDA_OK(ctx, cudaMemcpyAsync(hsz.data(), sizes, (size_t)nleaves * 8, cudaMemcpyDeviceToHost, s));

@@ -8,6 +8,8 @@
 // empty cluster keeps its centroid, convergence on sum_j||dc_j||^2 < tol (SURVEY.md §8a a-6..a-9).
 #include <float.h>
 
+#include <algorithm>
+
 #include "b2k_internal.cuh"
 
 #define B2K_EARLY_EXIT(st) \
@@ -427,6 +429,52 @@ int b2k_launch_fold_f64(b2k_ctx* ctx, const double* in, int m, double* out, cuda
   ctx->stats.kernel_launches++;
   B2K_CUDA_OK(ctx, cudaGetLastError());
   return B2K_OK;
+}
+
+B2kRowSpans b2k_row_spans(const b2k_ctx* ctx, int64_t n, int ncb) {
+  const int64_t spans_max = std::max<int64_t>(1, (n + 63) / 64);
+  const int spans = (int)std::min<int64_t>(std::max(1, (8 * ctx->sm_count + ncb - 1) / ncb), spans_max);
+  return {spans, std::max<int64_t>(1, (n + spans - 1) / spans)};
+}
+
+__global__ void k_fold_spans(const double* __restrict__ part, int spans, int m, int64_t n_tail, double* __restrict__ out) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c < m) {
+    double t = 0.0;
+    for (int s = 0; s < spans; ++s) t += part[(size_t)s * m + c];
+    out[c] = t;
+  } else if (c == m && n_tail >= 0) {
+    out[m] = (double)n_tail;
+  }
+}
+
+int b2k_launch_fold_spans(b2k_ctx* ctx, const double* part, int spans, int m, double* out, cudaStream_t s,
+                          int64_t n_tail) {
+  k_fold_spans<<<(m + 1 + 255) / 256, 256, 0, s>>>(part, spans, m, n_tail, out);
+  ctx->stats.kernel_launches++;
+  B2K_CUDA_OK(ctx, cudaGetLastError());
+  return B2K_OK;
+}
+
+// part[span][j] = rows of the span with label j (thread j counts, every thread reads each label)
+__global__ void __launch_bounds__(256) k_label_counts(const int32_t* __restrict__ labels, int64_t n, int m,
+                                                      int64_t span_rows, double* __restrict__ part) {
+  const int64_t r0 = (int64_t)blockIdx.x * span_rows;
+  const int64_t r1 = min(n, r0 + span_rows);
+  for (int j = threadIdx.x; j < m; j += blockDim.x) {
+    int64_t c = 0;
+    for (int64_t row = r0; row < r1; ++row) c += labels[row] == j;
+    part[(size_t)blockIdx.x * m + j] = (double)c;
+  }
+}
+
+int b2k_launch_label_counts(b2k_ctx* ctx, const int32_t* labels, int64_t n, int m, double* part, double* out,
+                            cudaStream_t s) {
+  const B2kRowSpans sp = b2k_row_spans(ctx, n, 1);
+  k_label_counts<<<sp.spans, 256, 0, s>>>(labels, n, m, sp.span_rows, part);
+  ctx->stats.kernel_launches++;
+  B2K_CUDA_OK(ctx, cudaGetLastError());
+  return b2k_launch_fold_spans(ctx, part, sp.spans, m, out, s);
 }
 
 int b2k_launch_sum_f32_to_f64(b2k_ctx* ctx, const float* v, int64_t n, double* out, double* block_scratch,

@@ -13,16 +13,15 @@
 //              are the hi / lo planes of P_k, one 128-row block per component.  The epilogue forms
 //              sum_j (D_ij - b_kj)^2 in fp64 per quad and keeps it in shared memory until the row's last component.
 //              generic (k_gmm_e_generic, SIMT): every shape; P_k (x - c) in fp64 from the exact fp64 differences.
-//   M passes N_k and sum r_ik (x_i - c) (k_gmm_mom, fp64), and S_k = sum r_ik (x_i - c)(x_i - c)^T, the upper block
-//            triangle per component:
-//              wgmma (k_gmm_gram_wg, the weighted variant of b2k_gram_wg.cuh, 3xTF32): d % 4 == 0, X 16-byte aligned;
-//              x - c rounded once to fp32 and scaled by fl32(sqrt(r_ik)) at the split; grid over (component, tile)
-//              so that a row range is read from HBM about once; fp64 partials per CTA folded in CTA order.
-//              generic (k_gmm_gram, SIMT): every shape; fp64 products of the exact differences.
+//   M passes N_k and sum r_ik (x_i - c) (k_gmm_mom, fp64, folded in span order), and S_k = sum r_ik (x_i - c)(x_i - c)^T
+//            by the weighted pass of b2k_gram.cu, its upper triangle per component:
+//              wgmma (3xTF32): d % 4 == 0, X 16-byte aligned; x - c rounded once to fp32 and scaled by fl32(sqrt(r_ik))
+//              at the split; grid over (component, tile) so that a row range is read from HBM about once.
+//              generic (SIMT): every shape; fp64 products of the exact differences.
 //            Every partial is folded in a fixed order.
-//   host     one f64 allreduce per iteration of [LL | N | s | upper triangles of S]; then w_k = N_k / n,
-//            mu_k = c + s_k / N_k, Sigma_k = S_k / N_k - (s_k / N_k)(s_k / N_k)^T and one eigendecomposition per
-//            component, identically on every rank.
+//   host     one f64 allreduce per iteration of [LL | [k][d + 1] (s_k, then N_k) | upper triangles of S];
+//            then w_k = N_k / n, mu_k = c + s_k / N_k, Sigma_k = S_k / N_k - (s_k / N_k)(s_k / N_k)^T and one
+//            eigendecomposition per component, identically on every rank.
 // No atomics: two calls on the same input, rank count and device give the same bits.
 #include <algorithm>
 #include <chrono>
@@ -36,7 +35,6 @@
 namespace {
 #include "b2k_ptx.cuh"
 #include "b2k_pair_wg.cuh"
-#include "b2k_gram_wg.cuh"
 
 constexpr double GMM_EPS = 2.220446049250313e-16;   // MLlib's EPSILON
 constexpr double GMM_LOG_2PI = 1.8378770664093453;
@@ -276,128 +274,6 @@ k_gmm_mom(const float* __restrict__ X, const double* __restrict__ r, int64_t n, 
     for (int y = 0; y < MO_TY; ++y) t += red[y][jj][threadIdx.x];
     part[(size_t)blockIdx.x * m + (size_t)(j0 + jj) * (d + 1) + f] = t;
   }
-}
-
-// spans in order -> N [k], s [k][d] of the allreduce buffer
-__global__ void k_gmm_mom_fold(const double* __restrict__ part, int spans, int d, int k, double* __restrict__ N,
-                               double* __restrict__ S1) {
-  const int m = k * (d + 1);
-  const int o = blockIdx.x * blockDim.x + threadIdx.x;
-  if (o >= m) return;
-  double t = 0.0;
-  for (int s = 0; s < spans; ++s) t += part[(size_t)s * m + o];
-  const int j = o / (d + 1), f = o - j * (d + 1);
-  if (f < d) S1[(size_t)j * d + f] = t;
-  else N[j] = t;
-}
-
-// ---- weighted Gram, generic: 32 x 32 tiles of the upper block triangle x component (blockIdx.x, tile fastest, so the
-// CTAs of one row span run together and read it from L2) x row span (blockIdx.y); thread (tx, ty) forms entries (ty + 16 a, tx + 16 b) of sum r (x - c)(x - c)^T in fp64 ----
-constexpr int GG_T = 32;
-__global__ void __launch_bounds__(256)
-k_gmm_gram(const float* __restrict__ X, const double* __restrict__ r, int64_t n, int d, int k,
-           const float* __restrict__ c32, int64_t span_rows, double* __restrict__ part) {
-  __shared__ double xi[GG_T][GG_T + 1], xj[GG_T][GG_T + 1];
-  __shared__ double wr[GG_T];
-  const int nb = (d + GG_T - 1) / GG_T, ntri = nb * (nb + 1) / 2;
-  int t = (int)blockIdx.x % ntri, I = 0;
-  while (t >= nb - I) {
-    t -= nb - I;
-    ++I;
-  }
-  const int J = I + t, comp = (int)blockIdx.x / ntri;
-  const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
-  const int64_t r0 = (int64_t)blockIdx.y * span_rows;
-  const int64_t r1 = min(n, r0 + span_rows);
-  double acc[2][2] = {{0.0, 0.0}, {0.0, 0.0}};
-  for (int64_t rb = r0; rb < r1; rb += GG_T) {
-    for (int e = threadIdx.x; e < GG_T * GG_T; e += 256) {
-      const int rr = e / GG_T, cc = e % GG_T;
-      const int64_t row = rb + rr;
-      const int ci = I * GG_T + cc, cj = J * GG_T + cc;
-      xi[rr][cc] = (row < r1 && ci < d) ? (double)X[row * d + ci] - (double)c32[ci] : 0.0;
-      xj[rr][cc] = (row < r1 && cj < d) ? (double)X[row * d + cj] - (double)c32[cj] : 0.0;
-    }
-    if (threadIdx.x < GG_T) wr[threadIdx.x] = rb + threadIdx.x < r1 ? r[(rb + threadIdx.x) * k + comp] : 0.0;
-    __syncthreads();
-#pragma unroll 4
-    for (int rr = 0; rr < GG_T; ++rr) {
-      const double w = wr[rr];
-      const double a0 = w * xi[rr][ty], a1 = w * xi[rr][ty + 16];
-      const double b0 = xj[rr][tx], b1 = xj[rr][tx + 16];
-      acc[0][0] = fma(a0, b0, acc[0][0]);
-      acc[0][1] = fma(a0, b1, acc[0][1]);
-      acc[1][0] = fma(a1, b0, acc[1][0]);
-      acc[1][1] = fma(a1, b1, acc[1][1]);
-    }
-    __syncthreads();
-  }
-  double* o = part + ((size_t)blockIdx.y * k + comp) * d * d;
-#pragma unroll
-  for (int p = 0; p < 2; ++p)
-#pragma unroll
-    for (int q = 0; q < 2; ++q) {
-      const int gi = I * GG_T + ty + 16 * p, gj = J * GG_T + tx + 16 * q;
-      if (gi < d && gj < d) o[(size_t)gi * d + gj] = acc[p][q];
-    }
-}
-
-// spans in order -> the upper triangles [k][d (d + 1) / 2] (row-major, i <= j) of the allreduce buffer
-__global__ void k_gmm_gram_fold(const double* __restrict__ part, int S, int d, int k, double* __restrict__ tri) {
-  const int64_t dd = (int64_t)d * d;
-  const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= (int64_t)k * dd) return;
-  const int comp = (int)(idx / dd);
-  const int gi = (int)((idx % dd) / d), gj = (int)(idx % d);
-  if (gi > gj) return;
-  double s = 0.0;
-  for (int sp = 0; sp < S; ++sp) s += part[((size_t)sp * k + comp) * dd + gi * d + gj];
-  const int64_t T = (int64_t)d * (d + 1) / 2;
-  tri[comp * T + (int64_t)gi * d - (int64_t)gi * (gi - 1) / 2 + (gj - gi)] = s;
-}
-
-// ---- weighted Gram, wgmma: the W = true instance of b2k_gram_wg.cuh ----
-__global__ void __launch_bounds__(GW_NTHREADS, 1)
-k_gmm_gram_wg(const __grid_constant__ CUtensorMap mapX, const GramArgs args, const GramWeights wt) {
-  gram_wg_body<true>(mapX, args, wt);
-}
-
-// CTA b = (p K + comp) ntile + t: the P partials of (comp, tile (I, J)) in CTA order -> the upper triangles
-__global__ void k_gmm_gram_fold_wg(const double* __restrict__ part, int P, int ntile, int nblk, int d, int k,
-                                   double* __restrict__ tri) {
-  const int64_t dd = (int64_t)d * d;
-  const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= (int64_t)k * dd) return;
-  const int comp = (int)(idx / dd);
-  const int gi = (int)((idx % dd) / d), gj = (int)(idx % d);
-  if (gi > gj) return;
-  const int I = gi / GW_BLK, J = gj / GW_BLK;
-  const int t = I * nblk - I * (I - 1) / 2 + (J - I);
-  const size_t e = (size_t)(gi % GW_BLK) * GW_BLK + (gj % GW_BLK);
-  double s = 0.0;
-  for (int p = 0; p < P; ++p) s += part[(((size_t)p * k + comp) * ntile + t) * GW_BLK * GW_BLK + e];
-  const int64_t T = (int64_t)d * (d + 1) / 2;
-  tri[comp * T + (int64_t)gi * d - (int64_t)gi * (gi - 1) / 2 + (gj - gi)] = s;
-}
-
-// ---- cluster sizes: part[span][j] = rows of the span with label j (thread j counts, every thread reads each label) ----
-__global__ void __launch_bounds__(256) k_gmm_count(const int32_t* __restrict__ labels, int64_t n, int k,
-                                                   int64_t span_rows, double* __restrict__ part) {
-  const int64_t r0 = (int64_t)blockIdx.x * span_rows;
-  const int64_t r1 = min(n, r0 + span_rows);
-  for (int j = threadIdx.x; j < k; j += blockDim.x) {
-    int64_t c = 0;
-    for (int64_t row = r0; row < r1; ++row) c += labels[row] == j;
-    part[(size_t)blockIdx.x * k + j] = (double)c;
-  }
-}
-
-__global__ void k_gmm_count_fold(const double* __restrict__ part, int spans, int k, double* __restrict__ out) {
-  const int j = blockIdx.x * blockDim.x + threadIdx.x;
-  if (j >= k) return;
-  double t = 0.0;
-  for (int s = 0; s < spans; ++s) t += part[(size_t)s * k + j];
-  out[j] = t;
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -646,24 +522,11 @@ int b2k_gmm_fit_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, int k, std:
   B2K_TRY(gmm_e_plan(ctx, who, X, n, d, k, &e));
   const int m1 = k * (d + 1);
   const int ncb = (d + 1 + MO_TX - 1) / MO_TX * ((k + MO_JG - 1) / MO_JG);   // column blocks x component groups
-  const int64_t nspan_max = std::max<int64_t>(1, (n + 63) / 64);
-  const int spans = (int)std::min<int64_t>(std::max(1, (8 * ctx->sm_count + ncb - 1) / ncb), nspan_max);
-  const int64_t span_rows = std::max<int64_t>(1, (n + spans - 1) / spans);
+  const B2kRowSpans ms = b2k_row_spans(ctx, n, ncb);
   const size_t dd = (size_t)d * d, T = (size_t)d * (d + 1) / 2;
-  const int S = (int)std::max<int64_t>(1, std::min<int64_t>({64, (int64_t)((256u << 20) / ((size_t)k * dd * 8)),
-                                                             (n + GG_T - 1) / GG_T}));
-  const int64_t gspan = std::max<int64_t>(1, (n + S - 1) / S);
-  // the wgmma Gram pass runs under the Gram pass's shape conditions (d % 4 == 0, 16-byte aligned X)
-  const bool gram_wg = d % 4 == 0 && (reinterpret_cast<uintptr_t>(X) & 15u) == 0 && ctx->kernel_path != B2K_PATH_GENERIC;
-  const int nblk = (d + GW_BLK - 1) / GW_BLK, ntile = nblk * (nblk + 1) / 2;
-  const int nrange = (int)std::max<int64_t>(1, (n + GW_RANGE - 1) / GW_RANGE);
-  int gsm = ctx->sm_count;
-  if (ctx->grid_limit > 0 && ctx->grid_limit < gsm) gsm = ctx->grid_limit;
-  const int GP = std::max(1, std::min(gsm / (ntile * k), nrange));   // CTAs per (component, tile)
-  const int ggrid = GP * ntile * k;
-  const int cspans = (int)std::min<int64_t>(8 * ctx->sm_count, nspan_max);
-  const int64_t cspan_rows = std::max<int64_t>(1, (n + cspans - 1) / cspans);
-  const size_t nbuf = 1 + (size_t)k + (size_t)k * d + (size_t)k * T;
+  const B2kGramPlan gp = b2k_gram_plan(ctx, X, n, d, k, ctx->kernel_path != B2K_PATH_GENERIC, (size_t)256 << 20);
+  const int cspans = b2k_row_spans(ctx, n, 1).spans;   // of b2k_launch_label_counts
+  const size_t nbuf = 1 + (size_t)m1 + gp.out_len;      // [LL | moments [k][d + 1] | upper triangles [k][T]]
   double *r, *mpart, *gpart, *buf, *cpart;
   float* cpad;
   int32_t* labels;
@@ -671,33 +534,20 @@ int b2k_gmm_fit_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, int k, std:
     gmm_e_take(L, e, d, k);
     r = L.take<double>((size_t)n * k);
     labels = L.take<int32_t>((size_t)n);
-    mpart = L.take<double>((size_t)spans * m1);
-    gpart = gram_wg ? L.take<double>((size_t)ggrid * GW_BLK * GW_BLK, 1024) : L.take<double>((size_t)S * k * dd);
-    cpad = gram_wg ? L.take<float>((size_t)nblk * GW_BLK) : nullptr;
+    mpart = L.take<double>((size_t)ms.spans * m1);
+    gpart = L.take<double>(gp.part_len, 1024);
+    cpad = L.take<float>(gp.mu_len);
     buf = L.take<double>(nbuf);
     cpart = L.take<double>((size_t)cspans * k);
     return B2K_OK;
   }));
-  double* Nd = buf + 1;
-  double* S1 = Nd + k;
-  double* tri = S1 + (size_t)k * d;
-  CUtensorMap gmap;
-  GramArgs ga{};
-  if (gram_wg) {
-    std::vector<float> cp((size_t)nblk * GW_BLK, 0.f);
+  double* mom = buf + 1;
+  double* tri = mom + m1;
+  {
+    std::vector<float> cp(gp.mu_len, 0.f);
     std::copy(c32.begin(), c32.end(), cp.begin());
     B2K_CUDA_OK(ctx, cudaMemcpyAsync(cpad, cp.data(), cp.size() * 4, cudaMemcpyHostToDevice, s));
     B2K_CUDA_OK(ctx, cudaStreamSynchronize(s));   // cp dies at scope end
-    B2K_TRY(b2k_encode_2d(ctx, &gmap, X, (uint64_t)d, (uint64_t)n, (uint64_t)d * 4, 32, GW_KC,
-                          CU_TENSOR_MAP_L2_PROMOTION_L2_256B));
-    B2K_CUDA_OK(ctx, cudaFuncSetAttribute(k_gmm_gram_wg, cudaFuncAttributeMaxDynamicSharedMemorySize, GW_SMEM + 1024));
-    ga.n = n;
-    ga.d = d;
-    ga.nblk = nblk;
-    ga.ntile = ntile;
-    ga.nrange = nrange;
-    ga.mu = cpad;
-    ga.part = gpart;
   }
 
   B2kTimer tm(ctx->time_kernels != 0);
@@ -705,7 +555,6 @@ int b2k_gmm_fit_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, int k, std:
   std::vector<double> hb(nbuf), cd(c32.begin(), c32.end());
   double ll = -INFINITY, llp;
   int iter = 0;
-  const int nb = (d + GG_T - 1) / GG_T;
   while (iter < max_iter) {
     const auto t_load = clk::now();
     B2K_TRY(gmm_e_load(ctx, who, e, d, k, c32, w.data(), mu.data(), cov.data(), s));
@@ -713,25 +562,17 @@ int b2k_gmm_fit_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, int k, std:
     tm.mark(0, s);
     B2K_TRY(gmm_e_launch(ctx, e, X, n, d, k, r, nullptr, buf, s));
     tm.mark(1, s);
-    k_gmm_mom<<<dim3(spans, ncb), dim3(MO_TX, MO_TY), 0, s>>>(X, r, n, d, k, e.c32, span_rows, mpart);
+    k_gmm_mom<<<dim3(ms.spans, ncb), dim3(MO_TX, MO_TY), 0, s>>>(X, r, n, d, k, e.c32, ms.span_rows, mpart);
     B2K_CUDA_OK(ctx, cudaGetLastError());
-    k_gmm_mom_fold<<<(m1 + 255) / 256, 256, 0, s>>>(mpart, spans, d, k, Nd, S1);
-    B2K_CUDA_OK(ctx, cudaGetLastError());
-    const unsigned fold_blocks = (unsigned)(((int64_t)k * dd + 255) / 256);
-    if (gram_wg) {
-      k_gmm_gram_wg<<<ggrid, GW_NTHREADS, GW_SMEM + 1024, s>>>(gmap, ga, GramWeights{r, k});
-      B2K_CUDA_OK(ctx, cudaGetLastError());
-      k_gmm_gram_fold_wg<<<fold_blocks, 256, 0, s>>>(gpart, GP, ntile, nblk, d, k, tri);
+    B2K_TRY(b2k_launch_fold_spans(ctx, mpart, ms.spans, m1, mom, s));
+    B2K_TRY(b2k_gram_launch(ctx, gp, X, cpad, r, gpart, tri, s));
+    if (gp.wg) {
       ctx->stats.fused_tc_launches++;
       ctx->stats.generic_launches++;
     } else {
-      k_gmm_gram<<<dim3(nb * (nb + 1) / 2 * k, S), 256, 0, s>>>(X, r, n, d, k, e.c32, gspan, gpart);
-      B2K_CUDA_OK(ctx, cudaGetLastError());
-      k_gmm_gram_fold<<<fold_blocks, 256, 0, s>>>(gpart, S, d, k, tri);
       ctx->stats.generic_launches += 2;
     }
-    B2K_CUDA_OK(ctx, cudaGetLastError());
-    ctx->stats.kernel_launches += 4;
+    ctx->stats.kernel_launches += 3;
     tm.mark(2, s);
     B2K_TRY(b2k_comm_allreduce_f64(ctx, buf, nbuf, s));
     tm.mark(3, s);
@@ -746,15 +587,14 @@ int b2k_gmm_fit_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, int k, std:
     // ---- M step (fp64, identical on every rank) ----
     llp = ll;
     ll = hb[0];
-    const double* hN = hb.data() + 1;
-    const double* hS1 = hN + k;
-    const double* htri = hS1 + (size_t)k * d;
+    const double* hmom = hb.data() + 1;   // [k][d + 1]: sum r (x - c) per feature, then N_j
+    const double* htri = hmom + m1;
     std::vector<double> m(d);
     for (int j = 0; j < k; ++j) {
-      const double Nj = hN[j];
+      const double Nj = hmom[(size_t)j * (d + 1) + d];
       w[j] = Nj / (double)n_total;
       for (int f = 0; f < d; ++f) {
-        m[f] = hS1[(size_t)j * d + f] / Nj;
+        m[f] = hmom[(size_t)j * (d + 1) + f] / Nj;
         mu[(size_t)j * d + f] = cd[f] + m[f];
       }
       const double* tj = htri + (size_t)j * T;
@@ -771,12 +611,8 @@ int b2k_gmm_fit_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, int k, std:
   // ---- cluster sizes: the predict pass of the final model, allreduced ----
   const std::vector<float> cpred = gmm_model_shift(k, d, w.data(), mu.data());
   B2K_TRY(gmm_e_load(ctx, who, e, d, k, cpred, w.data(), mu.data(), cov.data(), s));
-  B2K_TRY(gmm_e_launch(ctx, e, X, n, d, k, r, labels, buf + 1 + k, s));
-  k_gmm_count<<<cspans, 256, 0, s>>>(labels, n, k, cspan_rows, cpart);
-  B2K_CUDA_OK(ctx, cudaGetLastError());
-  k_gmm_count_fold<<<(k + 255) / 256, 256, 0, s>>>(cpart, cspans, k, buf);
-  B2K_CUDA_OK(ctx, cudaGetLastError());
-  ctx->stats.kernel_launches += 2;
+  B2K_TRY(gmm_e_launch(ctx, e, X, n, d, k, r, labels, buf + k, s));   // its log-likelihood lands past the counts
+  B2K_TRY(b2k_launch_label_counts(ctx, labels, n, k, cpart, buf, s));
   B2K_TRY(b2k_comm_allreduce_f64(ctx, buf, (size_t)k, s));
   std::vector<double> hc(k);
   B2K_CUDA_OK(ctx, cudaMemcpyAsync(hc.data(), buf, (size_t)k * 8, cudaMemcpyDeviceToHost, s));

@@ -205,6 +205,22 @@ int b2k_launch_finalize(b2k_ctx* ctx, const double* R, float* C, int k, int d, d
 int b2k_launch_sum_f32_to_f64(b2k_ctx* ctx, const float* v, int64_t n, double* out /*1*/,
                               double* block_scratch, int nblocks, cudaStream_t s);
 int b2k_launch_fold_f64(b2k_ctx* ctx, const double* in, int m, double* out /*1*/, cudaStream_t s);
+// The row spans of the fp64 column passes (per-span partials, folded in span order): with ncb column blocks per span,
+// spans = min(max(1, ceil(8 SMs / ncb)), max(1, ceil(n / 64))) and span_rows = max(1, ceil(n / spans)).  A function of
+// (n, ncb) and the device alone, so every call on the same shape adds in the same order.
+struct B2kRowSpans {
+  int spans;
+  int64_t span_rows;
+};
+B2kRowSpans b2k_row_spans(const b2k_ctx* ctx, int64_t n, int ncb);
+// out[c] = sum over s = 0 .. spans - 1 of part[s m + c], in span order from 0.0 (c < m); with n_tail >= 0 also
+// out[m] = n_tail (a row count that an allreduce then turns into the global one)
+int b2k_launch_fold_spans(b2k_ctx* ctx, const double* part, int spans, int m, double* out, cudaStream_t s,
+                          int64_t n_tail = -1);
+// out [m] (fp64) = the rows of labels [n] with each label value 0 .. m - 1, per row span of b2k_row_spans(n, 1) into
+// part [spans][m], folded in span order
+int b2k_launch_label_counts(b2k_ctx* ctx, const int32_t* labels, int64_t n, int m, double* part, double* out,
+                            cudaStream_t s);
 int b2k_launch_gather_rows(b2k_ctx* ctx, const float* X, int d, const int64_t* rows_local, int m,
                            float* out, int64_t out_row0, cudaStream_t s);
 // chunked assign: md_acc/lab_acc <- (md, lab + base) where md < md_acc
@@ -314,9 +330,35 @@ int b2k_pca_finalize_impl(b2k_ctx* ctx, const double* cov, int d, int64_t n_tota
                           double* evr_out, double* sv_out);
 int b2k_pca_transform_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, const float* C, int k, float* Y,
                            cudaStream_t s);
-// G [d][d] (device) = X^T X in fp64 over this rank's rows only (no collective): the generic Gram pass with a zero mean,
-// its row spans a function of (n, d) alone.  Uses ctx->scratch.
+// G [d (d + 1) / 2] (device, the packed upper triangle of b2k_gram.cu) = X^T X in fp64 over this rank's rows only (no
+// collective): the generic Gram pass with a zero mean, its row spans a function of (n, d) alone.  Uses ctx->scratch.
 int b2k_gram_local_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, double* G, cudaStream_t s);
+
+// ------------------------------------------------------------------------------------------------
+// Gram passes — b2k_gram.cu: G_c = sum_rows r_rc (x - mu)(x - mu)^T in fp64 for k components, as packed upper triangles
+// [k][d (d + 1) / 2] (row-major, i <= j).  Unweighted (r NULL, k = 1): x - mu in fp32; weighted (r [n][k] fp64): x - mu
+// in fp64 (generic) or rounded once to fp32 and scaled by fl32(sqrt(r)) (wgmma).
+// ------------------------------------------------------------------------------------------------
+bool b2k_gram_wg_ok(const float* X, int d);   // the wgmma pass takes the shape: d % 4 == 0, X 16-byte aligned
+struct B2kGramPlan {
+  bool wg = false;      // the wgmma pass (else the generic one)
+  int64_t n = 0;
+  int d = 0, k = 1;
+  int grid = 0;         // wgmma: CTAs; generic: CTAs per row span (tiles x k)
+  int spans = 0;        // wgmma: CTAs per (component, tile); generic: row spans
+  size_t part_len = 0;  // fp64 partials
+  size_t mu_len = 0;    // fp32 mean the pass reads (zero past d)
+  size_t out_len = 0;   // k d (d + 1) / 2
+};
+// the pass for (n, d, k): wgmma when allow_wg and b2k_gram_wg_ok; the generic row spans keep their partials within
+// part_bytes (at most 64 spans), so that they depend on (n, d, k) alone
+B2kGramPlan b2k_gram_plan(const b2k_ctx* ctx, const float* X, int64_t n, int d, int k, bool allow_wg, size_t part_bytes);
+// the pass and its fold into tri [out_len]; mu [mu_len], part [part_len].  n == 0: zero partials, folded.  Counts no
+// launches: the callers keep their own stats.
+int b2k_gram_launch(b2k_ctx* ctx, const B2kGramPlan& p, const float* X, const float* mu, const double* r, double* part,
+                    double* tri, cudaStream_t s);
+// G [d][d] (device) <- one packed upper triangle, mirrored; counts no launch
+int b2k_launch_gram_unpack(b2k_ctx* ctx, const double* tri, int d, double* G, cudaStream_t s);
 
 // ------------------------------------------------------------------------------------------------
 // exact k-NN — b2k_knn.cu (the C ABI entry point in b2k_api.cu checks its arguments, then calls this)

@@ -2,8 +2,9 @@
 //
 //   moments  b2k_moments_impl (b2k_pca.cu) runs PCA's column-sum and Gram passes on X, k_colsum on y as an [n, 1]
 //            matrix, and k_xty below: sum (x - mu32)(y - muy32) and sum (y - muy32)^2, centred, multiplied and summed in
-//            fp64 (the fp32 differences are exact there), per-CTA partials over fixed row spans folded in span order.  One f64 allreduce of the d * d + d + 1
-//            moments; the host then removes the offsets of (mu32, muy32) from the fp64 means exactly.
+//            fp64 (the fp32 differences are exact there), per-CTA partials over fixed row spans folded in span order.
+//            One f64 allreduce of the d (d + 1) / 2 + d + 1 moments (the Gram's upper triangle, X^T y, y^T y); the
+//            host then removes the offsets of (mu32, muy32) from the fp64 means exactly.
 //   solve    host, fp64, from the moments alone: Cholesky (minimum norm through b2k_sym_eig when a pivot is negligible)
 //            for OLS / ridge, cyclic coordinate descent on the covariance for the elastic net.
 //   predict  k_linreg_predict: b + sum_j x_j w_j in fp64, in an order fixed by d alone.
@@ -51,14 +52,6 @@ k_xty(const float* __restrict__ X, const float* __restrict__ y, int64_t n, int d
     for (int q = 0; q < XT_TY; ++q) t += red[q][threadIdx.x];
     part[(size_t)blockIdx.x * (d + 1) + c] = t;
   }
-}
-
-__global__ void k_xty_fold(const double* __restrict__ part, int spans, int m, double* __restrict__ out) {
-  const int c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c >= m) return;
-  double t = 0.0;
-  for (int s = 0; s < spans; ++s) t += part[(size_t)s * m + c];
-  out[c] = t;
 }
 
 // out[r] = b + sum_j x_rj w_j.  A group of L lanes (L a power of two, L = 32 from d = 100 on) owns one row: lane l
@@ -157,9 +150,7 @@ bool solve_spd_or_min_norm(std::vector<double> A, int d, double ridge, const std
 }  // namespace
 
 int b2k_xty_spans(const b2k_ctx* ctx, int64_t n, int d) {
-  const int ncb = (d + 1 + XT_TX - 1) / XT_TX;
-  const int64_t nspan_max = std::max<int64_t>(1, (n + 63) / 64);
-  return (int)std::min<int64_t>(std::max(1, (8 * ctx->sm_count + ncb - 1) / ncb), nspan_max);
+  return b2k_row_spans(ctx, n, (d + 1 + XT_TX - 1) / XT_TX).spans;
 }
 
 int b2k_launch_xty(b2k_ctx* ctx, const float* X, const float* y, int64_t n, int d, const float* mu32, float muy32,
@@ -173,10 +164,7 @@ int b2k_launch_xty(b2k_ctx* ctx, const float* X, const float* y, int64_t n, int 
   } else {
     B2K_CUDA_OK(ctx, cudaMemsetAsync(part, 0, (size_t)spans * m * 8, s));
   }
-  k_xty_fold<<<(m + 255) / 256, 256, 0, s>>>(part, spans, m, out);
-  B2K_CUDA_OK(ctx, cudaGetLastError());
-  ctx->stats.kernel_launches++;
-  return B2K_OK;
+  return b2k_launch_fold_spans(ctx, part, spans, m, out, s);
 }
 
 int b2k_linreg_moments_impl(b2k_ctx* ctx, const float* X, const float* y, int64_t n, int d, int64_t* n_total_out,

@@ -304,19 +304,6 @@ __global__ void __launch_bounds__(LR_THREADS, KB == 1 ? 3 : 2) k_logreg_eval(Eva
   }
 }
 
-// out [m + 1]: the partials folded in order, then n
-__global__ void k_logreg_fold(const double* __restrict__ part, int P, int m, int64_t n, double* __restrict__ out) {
-  const int c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c > m) return;
-  if (c == m) {
-    out[m] = (double)n;
-    return;
-  }
-  double t = 0.0;
-  for (int s = 0; s < P; ++s) t += part[(size_t)s * m + c];
-  out[c] = t;
-}
-
 // ------------------------------------------------------------------------------------------------
 // generic rows kernel (evaluation path and transform)
 // ------------------------------------------------------------------------------------------------
@@ -850,9 +837,7 @@ int eval_device(b2k_ctx* ctx, const EvalCall& e, const double* W, const double* 
     }
   }
   tm.mark(1, s);
-  k_logreg_fold<<<(M + 1 + 255) / 256, 256, 0, s>>>(part, P, M, n, out);
-  B2K_CUDA_OK(ctx, cudaGetLastError());
-  ctx->stats.kernel_launches++;
+  B2K_TRY(b2k_launch_fold_spans(ctx, part, P, M, out, s, n));   // out [M + 1]: the partials in order, then n
   B2K_TRY(b2k_comm_allreduce_f64(ctx, out, (size_t)M + 1, s));
   B2K_CUDA_OK(ctx, cudaMemcpyAsync(out_host, out, ((size_t)M + 1) * 8, cudaMemcpyDeviceToHost, s));
   B2K_CUDA_OK(ctx, cudaStreamSynchronize(s));

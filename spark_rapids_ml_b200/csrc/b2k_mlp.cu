@@ -16,7 +16,7 @@
 //          unit).
 //          Per 32-wide K chunk the operands are loaded from global memory, split x = hi + lo (both round-to-nearest
 //          tf32) and written K-major, 128-byte swizzled; D += lo.hi + hi.lo + hi.hi from a zero accumulator, added in
-//          round-to-nearest fp32 into a second accumulator (3xTF32, the discipline of b2k_gram_wg.cuh).  Activations and
+//          round-to-nearest fp32 into a second accumulator (3xTF32, the discipline of b2k_gram.cu).  Activations and
 //          deltas are fp32 in the chunk buffers; the weights are uploaded as fp32 in the orientation each product reads
 //          K-contiguous (forward: W_l as [numOut][numIn]; backward: Spark's layout, [numIn][numOut]).
 //   simt   k_mlp_simt<TA, TB>: one thread per output, fp64 products and sums; activations and deltas fp64.

@@ -1,13 +1,12 @@
 // PCA (sm_90a): the covariance passes, the projection kernel of transform and the host eigen step.
 //
-//   pass 1  k_colsum: fp64 column sums, per-CTA partials over fixed row spans, folded in span order (k_colsum_fold) into
-//           [d sums | n]; one f64 allreduce of d + 1 values; the host forms mu = sum / n_total in fp64.
-//   pass 2  the Gram matrix G = sum (x - mu32)(x - mu32)^T of the data centred on mu32 = fl32(mu):
-//             wgmma path (b2k_gram_wg.cuh, 3xTF32): d % 4 == 0, d <= B2K_PCA_MAX_D, X 16-byte aligned;
-//             generic path (k_gram_generic, SIMT, products and sums in fp64): every d <= B2K_PCA_MAX_D;
-//           per-CTA fp64 partials folded in a fixed order and mirrored (upper triangle -> both), one f64 allreduce of
-//           d * d values.  The host then removes the offset of mu32 from mu exactly:
-//           cov = (G - n (mu - mu32)(mu - mu32)^T) / (n - 1).
+//   pass 1  k_colsum: fp64 column sums, per-CTA partials over the row spans of b2k_row_spans, folded in span order
+//           (b2k_launch_fold_spans) into [d sums | n]; one f64 allreduce of d + 1 values; the host forms
+//           mu = sum / n_total in fp64.
+//   pass 2  the Gram matrix G = sum (x - mu32)(x - mu32)^T of the data centred on mu32 = fl32(mu), by the unweighted pass
+//           of b2k_gram.cu (wgmma, 3xTF32, for d % 4 == 0 and a 16-byte aligned X; generic SIMT in fp64 for every d):
+//           its upper triangle, d (d + 1) / 2 values, in one f64 allreduce, then unpacked to [d][d] on the device.  The host
+//           then removes the offset of mu32 from mu exactly: cov = (G - n (mu - mu32)(mu - mu32)^T) / (n - 1).
 //   eigen   b2k_pca_finalize_impl (host, fp64): Householder tridiagonalisation + implicit-shift QL, descending order,
 //           sign convention, ratios, singular values.
 //   transform  k_project: Y = X C^T, fp32 (SIMT; the components stay in shared memory).
@@ -22,13 +21,6 @@
 #include "b2k_internal.cuh"
 
 namespace {
-#include "b2k_ptx.cuh"
-#include "b2k_gram_wg.cuh"
-
-__global__ void __launch_bounds__(GW_NTHREADS, 1)
-k_gram_wg(const __grid_constant__ CUtensorMap mapX, const GramArgs args) {
-  gram_wg_body<false>(mapX, args, GramWeights{nullptr, 1});
-}
 
 constexpr int CS_TX = 32, CS_TY = 8;   // column-sum CTA: 32 columns x 8 row lanes
 
@@ -76,90 +68,6 @@ k_colsq(const float* __restrict__ X, int64_t n, int d, const float* __restrict__
     for (int y = 0; y < CS_TY; ++y) t += red[y][threadIdx.x];
     part[(size_t)blockIdx.x * d + c] = t;
   }
-}
-
-// sums[c] = sum over spans in order; sums[d] = n (the allreduce turns it into n_total)
-__global__ void k_colsum_fold(const double* __restrict__ part, int nspan, int d, int64_t n, double* __restrict__ sums) {
-  const int c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c < d) {
-    double t = 0.0;
-    for (int s = 0; s < nspan; ++s) t += part[(size_t)s * d + c];
-    sums[c] = t;
-  } else if (c == d) {
-    sums[d] = (double)n;
-  }
-}
-
-// wgmma path: G[i][j] = G[j][i] = sum over the P CTAs of tile (i / 128, j / 128), in CTA order, for i <= j
-__global__ void k_gram_fold_wg(const double* __restrict__ part, int P, int ntile, int nblk, int d, double* __restrict__ G) {
-  const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= (int64_t)d * d) return;
-  const int gi = (int)(idx / d), gj = (int)(idx % d);
-  if (gi > gj) return;
-  const int I = gi / GW_BLK, J = gj / GW_BLK;
-  const int t = I * nblk - I * (I - 1) / 2 + (J - I);
-  const size_t e = (size_t)(gi % GW_BLK) * GW_BLK + (gj % GW_BLK);
-  double s = 0.0;
-  for (int p = 0; p < P; ++p) s += part[((size_t)p * ntile + t) * GW_BLK * GW_BLK + e];
-  G[(size_t)gi * d + gj] = s;
-  G[(size_t)gj * d + gi] = s;
-}
-
-// generic path: 32 x 32 tiles of the upper block triangle (blockIdx.x) over row span blockIdx.y; thread (tx, ty) forms
-// entries (ty + 16 a, tx + 16 b) of the tile in fp64 from the fp32 centred values
-constexpr int GG_T = 32;
-__global__ void __launch_bounds__(256)
-k_gram_generic(const float* __restrict__ X, int64_t n, int d, const float* __restrict__ mu, int64_t span_rows,
-               double* __restrict__ part) {
-  __shared__ float xi[GG_T][GG_T + 1], xj[GG_T][GG_T + 1];
-  const int nb = (d + GG_T - 1) / GG_T;
-  int t = blockIdx.x, I = 0;
-  while (t >= nb - I) {
-    t -= nb - I;
-    ++I;
-  }
-  const int J = I + t;
-  const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
-  const int64_t r0 = (int64_t)blockIdx.y * span_rows;
-  const int64_t r1 = min(n, r0 + span_rows);
-  double acc[2][2] = {{0.0, 0.0}, {0.0, 0.0}};
-  for (int64_t rb = r0; rb < r1; rb += GG_T) {
-    for (int e = threadIdx.x; e < GG_T * GG_T; e += 256) {
-      const int rr = e / GG_T, cc = e % GG_T;
-      const int64_t row = rb + rr;
-      const int ci = I * GG_T + cc, cj = J * GG_T + cc;
-      xi[rr][cc] = (row < r1 && ci < d) ? X[row * d + ci] - mu[ci] : 0.f;
-      xj[rr][cc] = (row < r1 && cj < d) ? X[row * d + cj] - mu[cj] : 0.f;
-    }
-    __syncthreads();
-#pragma unroll 8
-    for (int rr = 0; rr < GG_T; ++rr) {
-      const double a0 = xi[rr][ty], a1 = xi[rr][ty + 16];
-      const double b0 = xj[rr][tx], b1 = xj[rr][tx + 16];
-      acc[0][0] = fma(a0, b0, acc[0][0]);
-      acc[0][1] = fma(a0, b1, acc[0][1]);
-      acc[1][0] = fma(a1, b0, acc[1][0]);
-      acc[1][1] = fma(a1, b1, acc[1][1]);
-    }
-    __syncthreads();
-  }
-  double* o = part + (size_t)blockIdx.y * d * d;
-  for (int a = 0; a < 2; ++a)
-    for (int b = 0; b < 2; ++b) {
-      const int gi = I * GG_T + ty + 16 * a, gj = J * GG_T + tx + 16 * b;
-      if (gi < d && gj < d) o[(size_t)gi * d + gj] = acc[a][b];
-    }
-}
-
-__global__ void k_gram_fold_generic(const double* __restrict__ part, int S, int d, double* __restrict__ G) {
-  const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= (int64_t)d * d) return;
-  const int gi = (int)(idx / d), gj = (int)(idx % d);
-  if (gi > gj) return;
-  double s = 0.0;
-  for (int sp = 0; sp < S; ++sp) s += part[(size_t)sp * d * d + idx];
-  G[(size_t)gi * d + gj] = s;
-  G[(size_t)gj * d + gi] = s;
 }
 
 // Y[n][k] = X[n][d] . C[k][d]^T.  CTA: PJ_ROWS rows (one per thread) x PJ_KT components (blockIdx.y); the CTA's
@@ -375,42 +283,30 @@ int b2k_pca_finalize_impl(b2k_ctx* ctx, const double* cov, int d, int64_t n_tota
 
 int b2k_moments_impl(b2k_ctx* ctx, const char* who, const float* X, const float* y, int64_t n, int d, int64_t min_rows,
                      B2kMoments* m, cudaStream_t s) {
-  const bool wg_ok = d % 4 == 0 && (reinterpret_cast<uintptr_t>(X) & 15u) == 0;
-  if (ctx->kernel_path == B2K_PATH_FUSED && !wg_ok)
+  if (ctx->kernel_path == B2K_PATH_FUSED && !b2k_gram_wg_ok(X, d))
     return b2k_fail(ctx, B2K_ERR_UNSUPPORTED, "kernel_path=2 requested but the wgmma Gram pass needs d % 4 == 0 and a "
                                               "16-byte aligned X (d = " + std::to_string(d) + ")");
-  const bool wg = wg_ok && ctx->kernel_path != B2K_PATH_GENERIC;
   B2kTimer tm(ctx->time_kernels != 0);
 
   // ---- plan and scratch ----
   const int ncb = (d + CS_TX - 1) / CS_TX;
-  const int64_t nspan_max = std::max<int64_t>(1, (n + 63) / 64);
-  const int nspan = (int)std::min<int64_t>(std::max(1, (8 * ctx->sm_count + ncb - 1) / ncb), nspan_max);
-  const int64_t span_rows = std::max<int64_t>(1, (n + nspan - 1) / nspan);
-  const int yspan = (int)std::min<int64_t>(8 * ctx->sm_count, nspan_max);   // the label: one column block
-  const int64_t yspan_rows = std::max<int64_t>(1, (n + yspan - 1) / yspan);
+  const B2kRowSpans xs = b2k_row_spans(ctx, n, ncb);
+  const B2kRowSpans ys = b2k_row_spans(ctx, n, 1);   // the label: one column block
   const int xty_spans = y ? b2k_xty_spans(ctx, n, d) : 0;
-  const int nblk = (d + GW_BLK - 1) / GW_BLK, ntile = nblk * (nblk + 1) / 2;
-  const int nrange = (int)std::max<int64_t>(1, (n + GW_RANGE - 1) / GW_RANGE);
-  int sm = ctx->sm_count;
-  if (ctx->grid_limit > 0 && ctx->grid_limit < sm) sm = ctx->grid_limit;
-  const int P = std::max(1, std::min(sm / ntile, nrange));   // CTAs per tile
-  // generic: row spans of the fp64 partials, at most 64 MB of them
-  const size_t dd = (size_t)d * d;
-  const int S = (int)std::max<int64_t>(1, std::min<int64_t>({64, (int64_t)((64u << 20) / (dd * 8)), (n + GG_T - 1) / GG_T}));
-  const int64_t gspan = std::max<int64_t>(1, (n + S - 1) / S);
-  const size_t part_len = wg ? (size_t)P * ntile * GW_BLK * GW_BLK : (size_t)S * dd;   // fp64 partials
-  const size_t nsum = (size_t)d + (y ? 2 : 1), nmom = dd + (y ? (size_t)d + 1 : 0);
-  double *colp, *sums, *G, *part, *ycolp = nullptr, *xtyp = nullptr;
+  const B2kGramPlan gp = b2k_gram_plan(ctx, X, n, d, 1, ctx->kernel_path != B2K_PATH_GENERIC, (size_t)64 << 20);
+  const size_t T = gp.out_len, dd = (size_t)d * d;
+  const size_t nsum = (size_t)d + (y ? 2 : 1), nmom = T + (y ? (size_t)d + 1 : 0);
+  double *colp, *sums, *G, *Gfull, *part, *ycolp = nullptr, *xtyp = nullptr;
   float* mu32_dev;
   B2K_TRY(b2k_scratch_layout(ctx, who, [&](B2kLayout& L) -> int {
-    colp = L.take<double>((size_t)nspan * d);
+    colp = L.take<double>((size_t)xs.spans * d);
     sums = L.take<double>(nsum);
-    mu32_dev = L.take<float>((size_t)nblk * GW_BLK);
-    G = L.take<double>(nmom);   // [d][d] Gram (+ [d] X^T y, [1] y^T y)
-    part = L.take<double>(part_len, 1024);
+    mu32_dev = L.take<float>(gp.mu_len);
+    G = L.take<double>(nmom);   // [d (d + 1) / 2] upper triangle of the Gram (+ [d] X^T y, [1] y^T y)
+    Gfull = L.take<double>(dd);
+    part = L.take<double>(gp.part_len, 1024);
     if (y) {
-      ycolp = L.take<double>((size_t)yspan);
+      ycolp = L.take<double>((size_t)ys.spans);
       xtyp = L.take<double>((size_t)xty_spans * (d + 1));
     }
     return B2K_OK;
@@ -419,26 +315,20 @@ int b2k_moments_impl(b2k_ctx* ctx, const char* who, const float* X, const float*
   // ---- pass 1: column sums, allreduce of [d sums | n] (with a label: [d sums | label sum | n]) ----
   tm.mark(0, s);
   if (n > 0) {
-    k_colsum<<<dim3(nspan, ncb), dim3(CS_TX, CS_TY), 0, s>>>(X, n, d, span_rows, colp);
+    k_colsum<<<dim3(xs.spans, ncb), dim3(CS_TX, CS_TY), 0, s>>>(X, n, d, xs.span_rows, colp);
     B2K_CUDA_OK(ctx, cudaGetLastError());
     ctx->stats.kernel_launches++;
     if (y) {
-      k_colsum<<<dim3(yspan, 1), dim3(CS_TX, CS_TY), 0, s>>>(y, n, 1, yspan_rows, ycolp);
+      k_colsum<<<dim3(ys.spans, 1), dim3(CS_TX, CS_TY), 0, s>>>(y, n, 1, ys.span_rows, ycolp);
       B2K_CUDA_OK(ctx, cudaGetLastError());
       ctx->stats.kernel_launches++;
     }
   } else {
-    B2K_CUDA_OK(ctx, cudaMemsetAsync(colp, 0, (size_t)nspan * d * 8, s));
-    if (y) B2K_CUDA_OK(ctx, cudaMemsetAsync(ycolp, 0, (size_t)yspan * 8, s));
+    B2K_CUDA_OK(ctx, cudaMemsetAsync(colp, 0, (size_t)xs.spans * d * 8, s));
+    if (y) B2K_CUDA_OK(ctx, cudaMemsetAsync(ycolp, 0, (size_t)ys.spans * 8, s));
   }
-  k_colsum_fold<<<(d + 1 + 255) / 256, 256, 0, s>>>(colp, nspan, d, n, sums);
-  B2K_CUDA_OK(ctx, cudaGetLastError());
-  ctx->stats.kernel_launches++;
-  if (y) {   // sums[d] <- label sum, sums[d + 1] <- n
-    k_colsum_fold<<<1, 32, 0, s>>>(ycolp, yspan, 1, n, sums + d);
-    B2K_CUDA_OK(ctx, cudaGetLastError());
-    ctx->stats.kernel_launches++;
-  }
+  B2K_TRY(b2k_launch_fold_spans(ctx, colp, xs.spans, d, sums, s, n));
+  if (y) B2K_TRY(b2k_launch_fold_spans(ctx, ycolp, ys.spans, 1, sums + d, s, n));   // label sum, n
   tm.mark(1, s);
   B2K_TRY(b2k_comm_allreduce_f64(ctx, sums, nsum, s));
   tm.mark(2, s);
@@ -453,7 +343,7 @@ int b2k_moments_impl(b2k_ctx* ctx, const char* who, const float* X, const float*
   m->n_total = n_total;
   m->mu.assign(dm, 0.0);
   m->delta.assign(dm, 0.0);
-  std::vector<float> mu32((size_t)nblk * GW_BLK, 0.f);
+  std::vector<float> mu32(gp.mu_len, 0.f);
   float muy32 = 0.f;
   for (int c = 0; c < dm; ++c) {
     m->mu[c] = hs[c] / (double)n_total;
@@ -466,50 +356,20 @@ int b2k_moments_impl(b2k_ctx* ctx, const char* who, const float* X, const float*
 
   // ---- pass 2: Gram matrix of the data centred on mu32 (and X^T y), allreduce ----
   tm.mark(3, s);
-  const int fold_blocks = (int)((dd + 255) / 256);
-  if (wg) {
-    if (n > 0) {
-      CUtensorMap map;
-      B2K_TRY(b2k_encode_2d(ctx, &map, X, (uint64_t)d, (uint64_t)n, (uint64_t)d * 4, 32, GW_KC,
-                            CU_TENSOR_MAP_L2_PROMOTION_L2_256B));
-      GramArgs ga;
-      ga.n = n;
-      ga.d = d;
-      ga.nblk = nblk;
-      ga.ntile = ntile;
-      ga.nrange = nrange;
-      ga.mu = mu32_dev;
-      ga.part = part;
-      B2K_CUDA_OK(ctx, cudaFuncSetAttribute(k_gram_wg, cudaFuncAttributeMaxDynamicSharedMemorySize, GW_SMEM + 1024));
-      k_gram_wg<<<P * ntile, GW_NTHREADS, GW_SMEM + 1024, s>>>(map, ga);
-      B2K_CUDA_OK(ctx, cudaGetLastError());
-      ctx->stats.kernel_launches++;
-    } else {
-      B2K_CUDA_OK(ctx, cudaMemsetAsync(part, 0, part_len * 8, s));
-    }
-    k_gram_fold_wg<<<fold_blocks, 256, 0, s>>>(part, P, ntile, nblk, d, G);
-  } else {
-    const int nb = (d + GG_T - 1) / GG_T;
-    if (n > 0) {
-      k_gram_generic<<<dim3(nb * (nb + 1) / 2, S), 256, 0, s>>>(X, n, d, mu32_dev, gspan, part);
-      B2K_CUDA_OK(ctx, cudaGetLastError());
-      ctx->stats.kernel_launches++;
-      ctx->stats.generic_launches++;
-    } else {
-      B2K_CUDA_OK(ctx, cudaMemsetAsync(part, 0, part_len * 8, s));
-    }
-    k_gram_fold_generic<<<fold_blocks, 256, 0, s>>>(part, S, d, G);
-  }
-  B2K_CUDA_OK(ctx, cudaGetLastError());
-  ctx->stats.kernel_launches++;
-  ctx->stats.last_path = wg ? B2K_PATH_FUSED : B2K_PATH_GENERIC;
+  B2K_TRY(b2k_gram_launch(ctx, gp, X, mu32_dev, nullptr, part, G, s));
+  ctx->stats.kernel_launches += n > 0 ? 2 : 1;
+  if (n > 0 && !gp.wg) ctx->stats.generic_launches++;
+  ctx->stats.last_path = gp.wg ? B2K_PATH_FUSED : B2K_PATH_GENERIC;
   tm.mark(4, s);
-  if (y) B2K_TRY(b2k_launch_xty(ctx, X, y, n, d, mu32_dev, muy32, xty_spans, xtyp, G + dd, s));
+  if (y) B2K_TRY(b2k_launch_xty(ctx, X, y, n, d, mu32_dev, muy32, xty_spans, xtyp, G + T, s));
   tm.mark(6, s);
   B2K_TRY(b2k_comm_allreduce_f64(ctx, G, nmom, s));
   tm.mark(5, s);
-  m->G.resize(nmom);
-  B2K_CUDA_OK(ctx, cudaMemcpyAsync(m->G.data(), G, nmom * 8, cudaMemcpyDeviceToHost, s));
+  // the triangle unpacked to [d][d] on the device, then the label's moments
+  B2K_TRY(b2k_launch_gram_unpack(ctx, G, d, Gfull, s));
+  m->G.resize(dd + (nmom - T));
+  B2K_CUDA_OK(ctx, cudaMemcpyAsync(m->G.data(), Gfull, dd * 8, cudaMemcpyDeviceToHost, s));
+  if (y) B2K_CUDA_OK(ctx, cudaMemcpyAsync(m->G.data() + dd, G + T, (nmom - T) * 8, cudaMemcpyDeviceToHost, s));
   B2K_CUDA_OK(ctx, cudaStreamSynchronize(s));
   if (tm.on) {
     ctx->stats.last_reduce_ms = tm.ms(0, 1);
@@ -523,13 +383,11 @@ int b2k_moments_impl(b2k_ctx* ctx, const char* who, const float* X, const float*
 int b2k_colstats_impl(b2k_ctx* ctx, const char* who, const float* X, int64_t n, int d, int64_t* n_total,
                       std::vector<double>* mu, std::vector<double>* ssq, cudaStream_t s) {
   const int ncb = (d + CS_TX - 1) / CS_TX;
-  const int64_t nspan_max = std::max<int64_t>(1, (n + 63) / 64);
-  const int nspan = (int)std::min<int64_t>(std::max(1, (8 * ctx->sm_count + ncb - 1) / ncb), nspan_max);
-  const int64_t span_rows = std::max<int64_t>(1, (n + nspan - 1) / nspan);
+  const B2kRowSpans xs = b2k_row_spans(ctx, n, ncb);
   double *colp, *sums, *sq;
   float* mu32_dev;
   B2K_TRY(b2k_scratch_layout(ctx, who, [&](B2kLayout& L) -> int {
-    colp = L.take<double>((size_t)nspan * d);
+    colp = L.take<double>((size_t)xs.spans * d);
     sums = L.take<double>((size_t)d + 1);
     sq = L.take<double>((size_t)d + 1);
     mu32_dev = L.take<float>((size_t)d);
@@ -537,15 +395,13 @@ int b2k_colstats_impl(b2k_ctx* ctx, const char* who, const float* X, int64_t n, 
   }));
   // sums and n, allreduced; then the centred squares on mu32
   if (n > 0) {
-    k_colsum<<<dim3(nspan, ncb), dim3(CS_TX, CS_TY), 0, s>>>(X, n, d, span_rows, colp);
+    k_colsum<<<dim3(xs.spans, ncb), dim3(CS_TX, CS_TY), 0, s>>>(X, n, d, xs.span_rows, colp);
     B2K_CUDA_OK(ctx, cudaGetLastError());
     ctx->stats.kernel_launches++;
   } else {
-    B2K_CUDA_OK(ctx, cudaMemsetAsync(colp, 0, (size_t)nspan * d * 8, s));
+    B2K_CUDA_OK(ctx, cudaMemsetAsync(colp, 0, (size_t)xs.spans * d * 8, s));
   }
-  k_colsum_fold<<<(d + 1 + 255) / 256, 256, 0, s>>>(colp, nspan, d, n, sums);
-  B2K_CUDA_OK(ctx, cudaGetLastError());
-  ctx->stats.kernel_launches++;
+  B2K_TRY(b2k_launch_fold_spans(ctx, colp, xs.spans, d, sums, s, n));
   B2K_TRY(b2k_comm_allreduce_f64(ctx, sums, (size_t)d + 1, s));
   std::vector<double> hs((size_t)d + 1);
   B2K_CUDA_OK(ctx, cudaMemcpyAsync(hs.data(), sums, hs.size() * 8, cudaMemcpyDeviceToHost, s));
@@ -560,13 +416,11 @@ int b2k_colstats_impl(b2k_ctx* ctx, const char* who, const float* X, int64_t n, 
   }
   B2K_CUDA_OK(ctx, cudaMemcpyAsync(mu32_dev, mu32.data(), (size_t)d * 4, cudaMemcpyHostToDevice, s));
   if (n > 0) {
-    k_colsq<<<dim3(nspan, ncb), dim3(CS_TX, CS_TY), 0, s>>>(X, n, d, mu32_dev, span_rows, colp);
+    k_colsq<<<dim3(xs.spans, ncb), dim3(CS_TX, CS_TY), 0, s>>>(X, n, d, mu32_dev, xs.span_rows, colp);
     B2K_CUDA_OK(ctx, cudaGetLastError());
     ctx->stats.kernel_launches++;
   }
-  k_colsum_fold<<<(d + 1 + 255) / 256, 256, 0, s>>>(colp, nspan, d, 0, sq);
-  B2K_CUDA_OK(ctx, cudaGetLastError());
-  ctx->stats.kernel_launches++;
+  B2K_TRY(b2k_launch_fold_spans(ctx, colp, xs.spans, d, sq, s));
   B2K_TRY(b2k_comm_allreduce_f64(ctx, sq, (size_t)d, s));
   ssq->assign(d, 0.0);
   B2K_CUDA_OK(ctx, cudaMemcpyAsync(ssq->data(), sq, (size_t)d * 8, cudaMemcpyDeviceToHost, s));
@@ -634,28 +488,16 @@ int b2k_pca_transform_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, const
 }
 
 int b2k_gram_local_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, double* G, cudaStream_t s) {
-  // the generic pass's span count, as b2k_moments_impl plans it: a function of (n, d) only
-  const size_t dd = (size_t)d * d;
-  const int S = (int)std::max<int64_t>(1, std::min<int64_t>({64, (int64_t)((64u << 20) / (dd * 8)), (n + GG_T - 1) / GG_T}));
-  const int64_t gspan = std::max<int64_t>(1, (n + S - 1) / S);
+  const B2kGramPlan gp = b2k_gram_plan(ctx, X, n, d, 1, false, (size_t)64 << 20);   // as b2k_moments_impl's generic pass
   double* part;
   float* zero;
   B2K_TRY(b2k_scratch_layout(ctx, "b2k_gram_local", [&](B2kLayout& L) -> int {
-    part = L.take<double>((size_t)S * dd);
-    zero = L.take<float>((size_t)d);
+    part = L.take<double>(gp.part_len);
+    zero = L.take<float>(gp.mu_len);
     return B2K_OK;
   }));
-  B2K_CUDA_OK(ctx, cudaMemsetAsync(zero, 0, (size_t)d * 4, s));
-  const int nb = (d + GG_T - 1) / GG_T;
-  if (n > 0) {
-    k_gram_generic<<<dim3(nb * (nb + 1) / 2, S), 256, 0, s>>>(X, n, d, zero, gspan, part);
-    B2K_CUDA_OK(ctx, cudaGetLastError());
-    ctx->stats.kernel_launches++;
-  } else {
-    B2K_CUDA_OK(ctx, cudaMemsetAsync(part, 0, (size_t)S * dd * 8, s));
-  }
-  k_gram_fold_generic<<<(int)((dd + 255) / 256), 256, 0, s>>>(part, S, d, G);
-  B2K_CUDA_OK(ctx, cudaGetLastError());
-  ctx->stats.kernel_launches++;
+  B2K_CUDA_OK(ctx, cudaMemsetAsync(zero, 0, gp.mu_len * 4, s));
+  B2K_TRY(b2k_gram_launch(ctx, gp, X, zero, nullptr, part, G, s));
+  ctx->stats.kernel_launches += n > 0 ? 2 : 1;
   return B2K_OK;
 }
