@@ -13,15 +13,19 @@
 //              are the hi / lo planes of P_k, one 128-row block per component.  The epilogue forms
 //              sum_j (D_ij - b_kj)^2 in fp64 per quad and keeps it in shared memory until the row's last component.
 //              generic (k_gmm_e_generic, SIMT): every shape; P_k (x - c) in fp64 from the exact fp64 differences.
-//   M passes N_k and sum r_ik (x_i - c) (k_gmm_mom, fp64, folded in span order), and S_k = sum r_ik (x_i - c)(x_i - c)^T
-//            by the weighted pass of b2k_gram.cu, its upper triangle per component:
-//              wgmma (3xTF32): d % 4 == 0, X 16-byte aligned; x - c rounded once to fp32 and scaled by fl32(sqrt(r_ik))
-//              at the split; grid over (component, tile) so that a row range is read from HBM about once.
+//   M pass 1 N_k and s_k = sum r_ik (x_i - c) (k_gmm_mom, fp64, folded in span order); one f64 allreduce of
+//            [LL | [k][d + 1] (s_k, then N_k)]; the host forms w_k = N_k / n, mu_k = c + s_k / N_k and the centre
+//            c_k = fl32(mu_k) of each component, identically on every rank.
+//   M pass 2 T_k = sum (r_ik / N_k)(x_i - c_k)(x_i - c_k)^T by the weighted pass of b2k_gram.cu, its upper triangle per
+//            component, the weight r_ik / N_k formed in fp64 on the device:
+//              wgmma (3xTF32): d % 4 == 0, X 16-byte aligned; x - c_k rounded once to fp32 and scaled by
+//              fl32(sqrt(r_ik / N_k)) at the split; grid over (component, tile) so that a row range is read from HBM
+//              about once.
 //              generic (SIMT): every shape; fp64 products of the exact differences.
-//            Every partial is folded in a fixed order.
-//   host     one f64 allreduce per iteration of [LL | [k][d + 1] (s_k, then N_k) | upper triangles of S];
-//            then w_k = N_k / n, mu_k = c + s_k / N_k, Sigma_k = S_k / N_k - (s_k / N_k)(s_k / N_k)^T and one
-//            eigendecomposition per component, identically on every rank.
+//            Every partial is folded in a fixed order.  One f64 allreduce of the triangles; then
+//            Sigma_k = T_k - (mu_k - c_k)(mu_k - c_k)^T and one eigendecomposition per component on every rank.
+//            Centring each component at its own mean keeps the wgmma pass's error relative to that component's spread,
+//            and the weights r / N_k sum to 1, so a component whose r lie below FLT_MIN still has its covariance.
 // No atomics: two calls on the same input, rank count and device give the same bits.
 #include <algorithm>
 #include <chrono>
@@ -527,8 +531,9 @@ int b2k_gmm_fit_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, int k, std:
   const B2kGramPlan gp = b2k_gram_plan(ctx, X, n, d, k, ctx->kernel_path != B2K_PATH_GENERIC, (size_t)256 << 20);
   const int cspans = b2k_row_spans(ctx, n, 1).spans;   // of b2k_launch_label_counts
   const size_t nbuf = 1 + (size_t)m1 + gp.out_len;      // [LL | moments [k][d + 1] | upper triangles [k][T]]
-  double *r, *mpart, *gpart, *buf, *cpart;
-  float* cpad;
+  const size_t cstride = gp.mu_len / k;                  // of the Gram pass's centres [k][cstride]
+  double *r, *mpart, *gpart, *buf, *cpart, *ginv;
+  float* gcen;
   int32_t* labels;
   B2K_TRY(b2k_scratch_layout(ctx, "b2k_gmm_fit", [&](B2kLayout& L) -> int {
     gmm_e_take(L, e, d, k);
@@ -536,23 +541,20 @@ int b2k_gmm_fit_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, int k, std:
     labels = L.take<int32_t>((size_t)n);
     mpart = L.take<double>((size_t)ms.spans * m1);
     gpart = L.take<double>(gp.part_len, 1024);
-    cpad = L.take<float>(gp.mu_len);
+    gcen = L.take<float>(gp.mu_len);
+    ginv = L.take<double>((size_t)k);
     buf = L.take<double>(nbuf);
     cpart = L.take<double>((size_t)cspans * k);
     return B2K_OK;
   }));
   double* mom = buf + 1;
   double* tri = mom + m1;
-  {
-    std::vector<float> cp(gp.mu_len, 0.f);
-    std::copy(c32.begin(), c32.end(), cp.begin());
-    B2K_CUDA_OK(ctx, cudaMemcpyAsync(cpad, cp.data(), cp.size() * 4, cudaMemcpyHostToDevice, s));
-    B2K_CUDA_OK(ctx, cudaStreamSynchronize(s));   // cp dies at scope end
-  }
 
   B2kTimer tm(ctx->time_kernels != 0);
   double e_ms = 0.0, m_ms = 0.0, ar_ms = 0.0, host_ms = 0.0;
   std::vector<double> hb(nbuf), cd(c32.begin(), c32.end());
+  std::vector<double> hinv(k), dm((size_t)k * d);   // 1 / N_k; mu_k - c_k
+  std::vector<float> ck(gp.mu_len, 0.f);            // c_k = fl32(mu_k), zero past d
   double ll = -INFINITY, llp;
   int iter = 0;
   while (iter < max_iter) {
@@ -565,7 +567,32 @@ int b2k_gmm_fit_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, int k, std:
     k_gmm_mom<<<dim3(ms.spans, ncb), dim3(MO_TX, MO_TY), 0, s>>>(X, r, n, d, k, e.c32, ms.span_rows, mpart);
     B2K_CUDA_OK(ctx, cudaGetLastError());
     B2K_TRY(b2k_launch_fold_spans(ctx, mpart, ms.spans, m1, mom, s));
-    B2K_TRY(b2k_gram_launch(ctx, gp, X, cpad, r, gpart, tri, s));
+    tm.mark(2, s);
+    B2K_TRY(b2k_comm_allreduce_f64(ctx, buf, 1 + (size_t)m1, s));
+    tm.mark(3, s);
+    B2K_CUDA_OK(ctx, cudaMemcpyAsync(hb.data(), buf, (1 + (size_t)m1) * 8, cudaMemcpyDeviceToHost, s));
+    B2K_CUDA_OK(ctx, cudaStreamSynchronize(s));
+    // ---- M step, weights and means (fp64, identical on every rank), and the centres of the Gram pass ----
+    auto t_host = clk::now();
+    llp = ll;
+    ll = hb[0];
+    const double* hmom = hb.data() + 1;   // [k][d + 1]: sum r (x - c) per feature, then N_j
+    for (int j = 0; j < k; ++j) {
+      const double Nj = hmom[(size_t)j * (d + 1) + d];
+      w[j] = Nj / (double)n_total;
+      hinv[j] = 1.0 / Nj;
+      for (int f = 0; f < d; ++f) {
+        const double mf = cd[f] + hmom[(size_t)j * (d + 1) + f] / Nj;
+        mu[(size_t)j * d + f] = mf;
+        ck[(size_t)j * cstride + f] = (float)mf;
+        dm[(size_t)j * d + f] = mf - (double)(float)mf;
+      }
+    }
+    B2K_CUDA_OK(ctx, cudaMemcpyAsync(gcen, ck.data(), ck.size() * 4, cudaMemcpyHostToDevice, s));
+    B2K_CUDA_OK(ctx, cudaMemcpyAsync(ginv, hinv.data(), (size_t)k * 8, cudaMemcpyHostToDevice, s));
+    host_ms += std::chrono::duration<double, std::milli>(clk::now() - t_host).count();
+    tm.mark(4, s);
+    B2K_TRY(b2k_gram_launch(ctx, gp, X, gcen, r, ginv, gpart, tri, s));
     if (gp.wg) {
       ctx->stats.fused_tc_launches++;
       ctx->stats.generic_launches++;
@@ -573,35 +600,26 @@ int b2k_gmm_fit_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, int k, std:
       ctx->stats.generic_launches += 2;
     }
     ctx->stats.kernel_launches += 3;
-    tm.mark(2, s);
-    B2K_TRY(b2k_comm_allreduce_f64(ctx, buf, nbuf, s));
-    tm.mark(3, s);
-    B2K_CUDA_OK(ctx, cudaMemcpyAsync(hb.data(), buf, nbuf * 8, cudaMemcpyDeviceToHost, s));
-    B2K_CUDA_OK(ctx, cudaStreamSynchronize(s));
-    const auto t_host = clk::now();
+    tm.mark(5, s);
+    B2K_TRY(b2k_comm_allreduce_f64(ctx, tri, gp.out_len, s));
+    tm.mark(6, s);
+    B2K_CUDA_OK(ctx, cudaMemcpyAsync(hb.data() + 1 + m1, tri, gp.out_len * 8, cudaMemcpyDeviceToHost, s));
+    B2K_CUDA_OK(ctx, cudaStreamSynchronize(s));   // also keeps ck and hinv alive until their copies are done
+    t_host = clk::now();
     if (tm.on) {
       e_ms += tm.ms(0, 1);
-      m_ms += tm.ms(1, 2);
-      ar_ms += tm.ms(2, 3);
+      m_ms += tm.ms(1, 2) + tm.ms(4, 5);
+      ar_ms += tm.ms(2, 3) + tm.ms(5, 6);
     }
-    // ---- M step (fp64, identical on every rank) ----
-    llp = ll;
-    ll = hb[0];
-    const double* hmom = hb.data() + 1;   // [k][d + 1]: sum r (x - c) per feature, then N_j
+    // ---- M step, covariances: Sigma_k = T_k - (mu_k - c_k)(mu_k - c_k)^T ----
     const double* htri = hmom + m1;
-    std::vector<double> m(d);
     for (int j = 0; j < k; ++j) {
-      const double Nj = hmom[(size_t)j * (d + 1) + d];
-      w[j] = Nj / (double)n_total;
-      for (int f = 0; f < d; ++f) {
-        m[f] = hmom[(size_t)j * (d + 1) + f] / Nj;
-        mu[(size_t)j * d + f] = cd[f] + m[f];
-      }
       const double* tj = htri + (size_t)j * T;
+      const double* m = dm.data() + (size_t)j * d;
       double* cj = cov.data() + (size_t)j * dd;
       size_t t = 0;
       for (int a = 0; a < d; ++a)
-        for (int b = a; b < d; ++b, ++t) cj[(size_t)a * d + b] = cj[(size_t)b * d + a] = tj[t] / Nj - m[a] * m[b];
+        for (int b = a; b < d; ++b, ++t) cj[(size_t)a * d + b] = cj[(size_t)b * d + a] = tj[t] - m[a] * m[b];
     }
     ++iter;
     host_ms += std::chrono::duration<double, std::milli>(clk::now() - t_host).count();

@@ -1,14 +1,15 @@
-// The fp64 Gram passes (sm_90a): G_c = sum_rows r_rc (x - mu)(x - mu)^T for k components c, as packed upper triangles
-// [k][d (d + 1) / 2] (row-major, i <= j).  PCA and linear regression (b2k_moments_impl) and ALS's Y^T Y
-// (b2k_gram_local_impl) run the unweighted pass (W = false, k = 1); Gaussian mixtures the weighted one (W = true: r [n][k]
-// fp64 row weights).
+// The fp64 Gram passes (sm_90a): G_c = sum_rows f_c r_rc (x - mu_c)(x - mu_c)^T for k components c, as packed upper
+// triangles [k][d (d + 1) / 2] (row-major, i <= j).  PCA and linear regression (b2k_moments_impl) and ALS's Y^T Y
+// (b2k_gram_local_impl) run the unweighted pass (W = false, k = 1, r = f = 1); Gaussian mixtures the weighted one
+// (W = true: r [n][k] fp64 row weights, f [k] fp64 factors, each component about its own centre mu_c).
 //
 //   wgmma   k_gram_wg<W> (3xTF32): d % 4 == 0, X 16-byte aligned.  Per-CTA fp64 partials of one 128 x 128 tile,
 //           folded in CTA order (k_gram_fold_wg).
 //   generic k_gram_generic<W> (SIMT, fp64 products and sums): every d.  Per-row-span fp64 partials of every 32 x 32 tile,
 //           folded in span order (k_gram_fold_generic).
 //   Numerics.  W = false centres in fp32 (x - mu as a float; exact for data near mu); W = true centres in fp64 (the
-//   generic pass) or rounds x - mu once to fp32 and scales it by fl32(sqrt(fl32(r))) at the split (the wgmma pass).
+//   generic pass) or rounds x - mu_c once to fp32 and scales it by fl32(sqrt(fl32(f_c r))) at the split (the wgmma
+//   pass), f_c r formed in fp64.
 // Every output is a fixed function of (n, d, k, grid): no atomics, bitwise reproducible.
 #include <algorithm>
 #include <type_traits>
@@ -21,8 +22,10 @@ namespace {
 // ---------------------------------------------------------------------------------------------------------------------
 // wgmma pass: the upper block triangle of 128 x 128 feature blocks.
 //
-// Weighted variant (W = true): G_c for each component c of r [n][K].  Each row's centred fp32 value is multiplied by
-// fl32(sqrt(fl32(r_rc))) before the split, in both operands, so the product carries r_rc.  The grid is a multiple of
+// Weighted variant (W = true): G_c for each component c of r [n][K], about the component's own centre mu_c.  Each row's
+// centred fp32 value is multiplied by fl32(sqrt(fl32(f_c r_rc))) before the split, in both operands, so the product
+// carries f_c r_rc.  The caller picks f_c = 1 / N_c: the weights of a component then sum to 1, so a component whose r
+// all lie below FLT_MIN keeps its weights in fp32, and G_c is its covariance about mu_c.  The grid is a multiple of
 // K * ntile: CTA b owns component (b % (K ntile)) / ntile and tile b % ntile, so the K ntile CTAs of one p read the same
 // row range at the same time and it is fetched from HBM about once per pass.
 //
@@ -70,12 +73,13 @@ struct GramArgs {
   int nblk;          // feature blocks, ceil(d / 128)
   int ntile;         // nblk (nblk + 1) / 2
   int nrange;        // ceil(n / GW_RANGE)
-  const float* mu;   // [nblk * 128] fp32 mean, 0 past d
+  const float* mu;   // [K][nblk * 128] fp32 centre per component (K = 1 unless W), 0 past d
   double* part;      // [grid][128][128] fp64 sums of the CTA's tile (rows of block I, columns of block J)
 };
 
 struct GramWeights {
-  const double* r;   // [n][K] row weights (W = true), else unused
+  const double* r;       // [n][K] row weights (W = true), else unused
+  const double* scale;   // [K] per-component factors of r (W = true), else unused
   int K;
 };
 
@@ -117,8 +121,9 @@ k_gram_wg(const __grid_constant__ CUtensorMap mapX, const GramArgs args, const G
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
+  const float* mu_c = args.mu + (size_t)comp * args.nblk * GW_BLK;
   for (int i = threadIdx.x; i < 2 * GW_BLK; i += GW_NTHREADS)
-    mu_s[i] = args.mu[(i < GW_BLK ? I : J) * GW_BLK + (i & (GW_BLK - 1))];
+    mu_s[i] = mu_c[(i < GW_BLK ? I : J) * GW_BLK + (i & (GW_BLK - 1))];
   __syncthreads();
 
   const int warp = threadIdx.x >> 5;
@@ -155,7 +160,8 @@ k_gram_wg(const __grid_constant__ CUtensorMap mapX, const GramArgs args, const G
   const int g = warp >> 2, tid = threadIdx.x;   // tid < 256
   // centre, split and transpose one block of the chunk into K-major (hi, lo) operands; a warp handles 32 consecutive
   // features of one group of 4 rows: conflict-free reads, 16-byte stores
-  // wrow: W = true, the chunk's first row of the weight table at this CTA's component
+  // wrow: W = true, the chunk's first row of the weight table at this CTA's component, scaled by wsc in fp64
+  const double wsc = W ? __ldg(wt.scale + comp) : 1.0;
   auto stage = [&](const uint8_t* xb, const float* mub, int nvalid, uint32_t dhi, uint32_t dlo, int kv,
                    const double* wrow) {
 #pragma unroll
@@ -169,7 +175,7 @@ k_gram_wg(const __grid_constant__ CUtensorMap mapX, const GramArgs args, const G
         const float raw = *reinterpret_cast<const float*>(
             xb + (nf >> 5) * GW_BOX + k * 128 + ((((nf & 31) >> 2) ^ (k & 7)) << 4) + (nf & 3) * 4);
         float v = (k < kv && nf < nvalid) ? raw - mub[nf] : 0.f;
-        if constexpr (W) v *= k < kv ? sqrtf((float)__ldg(wrow + (int64_t)k * wt.K)) : 0.f;
+        if constexpr (W) v *= k < kv ? sqrtf((float)(__ldg(wrow + (int64_t)k * wt.K) * wsc)) : 0.f;
         hi[i] = rn_tf32_bits(v);
         lo[i] = rn_tf32_bits(v - __uint_as_float(hi[i]));
       }
@@ -270,12 +276,14 @@ __global__ void k_gram_fold_wg(const double* __restrict__ part, int P, int ntile
 
 // ---- generic pass: 32 x 32 tiles of the upper block triangle x component (blockIdx.x, tile fastest, so the CTAs of one
 // row span run together and read it from L2) x row span (blockIdx.y); thread (tx, ty) forms entries (ty + 16 a,
-// tx + 16 b) of the tile in fp64.  W = false stages x - mu in fp32, W = true in fp64 with the row weights r [n][k]. ----
+// tx + 16 b) of the tile in fp64.  W = false stages x - mu in fp32, W = true x - mu_comp (mu [k][d]) in fp64 with the
+// row weights r [n][k] times scale [k]. ----
 constexpr int GG_T = 32;
 template <bool W>
 __global__ void __launch_bounds__(256)
 k_gram_generic(const float* __restrict__ X, const double* __restrict__ r, int64_t n, int d, int k,
-               const float* __restrict__ mu, int64_t span_rows, double* __restrict__ part) {
+               const float* __restrict__ mu, int64_t span_rows, double* __restrict__ part,
+               const double* __restrict__ scale) {
   using T = typename std::conditional<W, double, float>::type;
   __shared__ T xi[GG_T][GG_T + 1], xj[GG_T][GG_T + 1];
   __shared__ double wr[W ? GG_T : 1];
@@ -296,14 +304,15 @@ k_gram_generic(const float* __restrict__ X, const double* __restrict__ r, int64_
       const int64_t row = rb + rr;
       const int ci = I * GG_T + cc, cj = J * GG_T + cc;
       if constexpr (W) {
-        xi[rr][cc] = (row < r1 && ci < d) ? (double)X[row * d + ci] - (double)mu[ci] : 0.0;
-        xj[rr][cc] = (row < r1 && cj < d) ? (double)X[row * d + cj] - (double)mu[cj] : 0.0;
+        xi[rr][cc] = (row < r1 && ci < d) ? (double)X[row * d + ci] - (double)mu[(size_t)comp * d + ci] : 0.0;
+        xj[rr][cc] = (row < r1 && cj < d) ? (double)X[row * d + cj] - (double)mu[(size_t)comp * d + cj] : 0.0;
       } else {
         xi[rr][cc] = (row < r1 && ci < d) ? X[row * d + ci] - mu[ci] : 0.f;
         xj[rr][cc] = (row < r1 && cj < d) ? X[row * d + cj] - mu[cj] : 0.f;
       }
     }
-    if (W && threadIdx.x < GG_T) wr[threadIdx.x] = rb + threadIdx.x < r1 ? r[(rb + threadIdx.x) * k + comp] : 0.0;
+    if (W && threadIdx.x < GG_T)
+      wr[threadIdx.x] = rb + threadIdx.x < r1 ? r[(rb + threadIdx.x) * k + comp] * scale[comp] : 0.0;
     __syncthreads();
 #pragma unroll(W ? 4 : 8)
     for (int rr = 0; rr < GG_T; ++rr) {
@@ -377,7 +386,7 @@ B2kGramPlan b2k_gram_plan(const b2k_ctx* ctx, const float* X, int64_t n, int d, 
     p.spans = std::max(1, std::min(sm / (ntile * k), nrange));   // CTAs per (component, tile)
     p.grid = p.spans * ntile * k;
     p.part_len = (size_t)p.grid * GW_BLK * GW_BLK;
-    p.mu_len = (size_t)nblk * GW_BLK;
+    p.mu_len = (size_t)k * nblk * GW_BLK;
   } else {
     // row spans of the fp64 partials, at most part_bytes of them: a function of (n, d, k) alone
     p.spans = (int)std::max<int64_t>(
@@ -385,13 +394,13 @@ B2kGramPlan b2k_gram_plan(const b2k_ctx* ctx, const float* X, int64_t n, int d, 
     const int nb = (d + GG_T - 1) / GG_T;
     p.grid = nb * (nb + 1) / 2 * k;
     p.part_len = (size_t)p.spans * k * dd;
-    p.mu_len = (size_t)d;
+    p.mu_len = (size_t)k * d;
   }
   return p;
 }
 
-int b2k_gram_launch(b2k_ctx* ctx, const B2kGramPlan& p, const float* X, const float* mu, const double* r, double* part,
-                    double* tri, cudaStream_t s) {
+int b2k_gram_launch(b2k_ctx* ctx, const B2kGramPlan& p, const float* X, const float* mu, const double* r,
+                    const double* r_scale, double* part, double* tri, cudaStream_t s) {
   const int64_t n = p.n;
   const int d = p.d, k = p.k;
   const bool W = r != nullptr;
@@ -406,7 +415,7 @@ int b2k_gram_launch(b2k_ctx* ctx, const B2kGramPlan& p, const float* X, const fl
       const GramArgs ga{n, d, nblk, ntile, (int)std::max<int64_t>(1, (n + GW_RANGE - 1) / GW_RANGE), mu, part};
       auto kern = W ? k_gram_wg<true> : k_gram_wg<false>;
       B2K_CUDA_OK(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, GW_SMEM + 1024));
-      kern<<<p.grid, GW_NTHREADS, GW_SMEM + 1024, s>>>(map, ga, GramWeights{r, k});
+      kern<<<p.grid, GW_NTHREADS, GW_SMEM + 1024, s>>>(map, ga, GramWeights{r, r_scale, k});
       B2K_CUDA_OK(ctx, cudaGetLastError());
     }
     k_gram_fold_wg<<<fold_blocks, 256, 0, s>>>(part, p.spans, ntile, nblk, d, k, tri);
@@ -414,7 +423,7 @@ int b2k_gram_launch(b2k_ctx* ctx, const B2kGramPlan& p, const float* X, const fl
     if (n > 0) {
       const int64_t span_rows = std::max<int64_t>(1, (n + p.spans - 1) / p.spans);
       auto kern = W ? k_gram_generic<true> : k_gram_generic<false>;
-      kern<<<dim3(p.grid, p.spans), 256, 0, s>>>(X, r, n, d, k, mu, span_rows, part);
+      kern<<<dim3(p.grid, p.spans), 256, 0, s>>>(X, r, n, d, k, mu, span_rows, part, r_scale);
       B2K_CUDA_OK(ctx, cudaGetLastError());
     }
     k_gram_fold_generic<<<fold_blocks, 256, 0, s>>>(part, p.spans, d, k, tri);

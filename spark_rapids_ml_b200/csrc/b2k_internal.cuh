@@ -335,9 +335,10 @@ int b2k_pca_transform_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, const
 int b2k_gram_local_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, double* G, cudaStream_t s);
 
 // ------------------------------------------------------------------------------------------------
-// Gram passes — b2k_gram.cu: G_c = sum_rows r_rc (x - mu)(x - mu)^T in fp64 for k components, as packed upper triangles
-// [k][d (d + 1) / 2] (row-major, i <= j).  Unweighted (r NULL, k = 1): x - mu in fp32; weighted (r [n][k] fp64): x - mu
-// in fp64 (generic) or rounded once to fp32 and scaled by fl32(sqrt(r)) (wgmma).
+// Gram passes — b2k_gram.cu: G_c = sum_rows f_c r_rc (x - mu_c)(x - mu_c)^T in fp64 for k components, as packed upper
+// triangles [k][d (d + 1) / 2] (row-major, i <= j).  Unweighted (r NULL, k = 1): x - mu in fp32; weighted (r [n][k],
+// f [k] fp64, mu_c the component's own centre): x - mu_c in fp64 (generic) or rounded once to fp32 and scaled by
+// fl32(sqrt(f_c r)) (wgmma).
 // ------------------------------------------------------------------------------------------------
 bool b2k_gram_wg_ok(const float* X, int d);   // the wgmma pass takes the shape: d % 4 == 0, X 16-byte aligned
 struct B2kGramPlan {
@@ -347,16 +348,16 @@ struct B2kGramPlan {
   int grid = 0;         // wgmma: CTAs; generic: CTAs per row span (tiles x k)
   int spans = 0;        // wgmma: CTAs per (component, tile); generic: row spans
   size_t part_len = 0;  // fp64 partials
-  size_t mu_len = 0;    // fp32 mean the pass reads (zero past d)
+  size_t mu_len = 0;    // fp32 centres the pass reads, k of them at a stride of mu_len / k (zero past d)
   size_t out_len = 0;   // k d (d + 1) / 2
 };
 // the pass for (n, d, k): wgmma when allow_wg and b2k_gram_wg_ok; the generic row spans keep their partials within
 // part_bytes (at most 64 spans), so that they depend on (n, d, k) alone
 B2kGramPlan b2k_gram_plan(const b2k_ctx* ctx, const float* X, int64_t n, int d, int k, bool allow_wg, size_t part_bytes);
-// the pass and its fold into tri [out_len]; mu [mu_len], part [part_len].  n == 0: zero partials, folded.  Counts no
-// launches: the callers keep their own stats.
-int b2k_gram_launch(b2k_ctx* ctx, const B2kGramPlan& p, const float* X, const float* mu, const double* r, double* part,
-                    double* tri, cudaStream_t s);
+// the pass and its fold into tri [out_len]; mu [mu_len], part [part_len], r [n][k] and r_scale [k] (both NULL for the
+// unweighted pass).  n == 0: zero partials, folded.  Counts no launches: the callers keep their own stats.
+int b2k_gram_launch(b2k_ctx* ctx, const B2kGramPlan& p, const float* X, const float* mu, const double* r,
+                    const double* r_scale, double* part, double* tri, cudaStream_t s);
 // G [d][d] (device) <- one packed upper triangle, mirrored; counts no launch
 int b2k_launch_gram_unpack(b2k_ctx* ctx, const double* tri, int d, double* G, cudaStream_t s);
 

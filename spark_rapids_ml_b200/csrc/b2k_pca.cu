@@ -356,7 +356,7 @@ int b2k_moments_impl(b2k_ctx* ctx, const char* who, const float* X, const float*
 
   // ---- pass 2: Gram matrix of the data centred on mu32 (and X^T y), allreduce ----
   tm.mark(3, s);
-  B2K_TRY(b2k_gram_launch(ctx, gp, X, mu32_dev, nullptr, part, G, s));
+  B2K_TRY(b2k_gram_launch(ctx, gp, X, mu32_dev, nullptr, nullptr, part, G, s));
   ctx->stats.kernel_launches += n > 0 ? 2 : 1;
   if (n > 0 && !gp.wg) ctx->stats.generic_launches++;
   ctx->stats.last_path = gp.wg ? B2K_PATH_FUSED : B2K_PATH_GENERIC;
@@ -497,7 +497,7 @@ int b2k_gram_local_impl(b2k_ctx* ctx, const float* X, int64_t n, int d, double* 
     return B2K_OK;
   }));
   B2K_CUDA_OK(ctx, cudaMemsetAsync(zero, 0, gp.mu_len * 4, s));
-  B2K_TRY(b2k_gram_launch(ctx, gp, X, zero, nullptr, part, G, s));
+  B2K_TRY(b2k_gram_launch(ctx, gp, X, zero, nullptr, nullptr, part, G, s));
   ctx->stats.kernel_launches += n > 0 ? 2 : 1;
   return B2K_OK;
 }

@@ -27,6 +27,18 @@ def data(d, k, seed, n=3000):
     return (means[z] + rng.normal(size=(n, d))).astype(np.float32)
 
 
+def dead_component(n=3 * 4096 + 5, seed=4):
+    """Tight rows (sigma = 0.05, d = 132) of two live components and an injected third one 50 units from every row, whose
+    responsibilities lie far below FLT_MIN: (X, (weights, means, covariances))."""
+    d, s = 132, 0.05
+    rng = np.random.default_rng(seed)
+    e = np.eye(d)
+    live = np.stack([e[0], -e[0]])
+    X = (live[np.arange(n) % 2] + s * rng.normal(size=(n, d))).astype(np.float32)
+    init = (np.array([0.45, 0.45, 0.1]), np.stack([e[0], -e[0], 50.0 * e[1]]), np.stack([np.eye(d) * s * s] * 3))
+    return X, init
+
+
 def shard_sizes(R, n):
     return [n * 6 // 10, n - n * 6 // 10] if R == 2 else [n * 5 // 10, n * 2 // 10, n - n * 7 // 10]
 
@@ -44,6 +56,13 @@ def _cases(R):
             return {"start": start, "fit": out}
 
         cases[name] = (parts, {"X": X}, f)
+    if R == 2:
+        # one M step, so both of its allreduces run on every rank of an uneven split.  (A second one is not defined:
+        # the step gathers the support-less component onto a few rows, and its density then overflows an fp64.)
+        X, init = dead_component()
+        parts = [{"X": a} for a in rc.split(X, shard_sizes(R, len(X)))]
+        cases["dead"] = (parts, {"X": X},
+                         lambda ctx, a: {"fit": ctx.gmm_fit(a["X"], 3, init=init, max_iter=1, tol=0.0)})
     X = data(4, 2, seed=1)
     empty = [{"X": a} for a in rc.split(X, [len(X), 0] if R == 2 else [len(X) - 10, 0, 10])]
     cases["empty"] = (empty, None, lambda ctx, a: {"fit": ctx.gmm_fit(a["X"], 2, max_iter=2)})

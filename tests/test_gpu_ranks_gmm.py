@@ -1,6 +1,7 @@
 """b2k_gmm_fit at R = 2 and 3 ranks on one GPU through the in-process NCCL stand-in (child: tests/_ranks_child_gmm.py):
 the seeded start is bitwise the one-rank start, the fit agrees with the one-rank fit within the E pass's tolerance and
-is the same on every rank; an empty partition fails on every rank with one message."""
+is the same on every rank; a component with no support fits on every rank of an uneven split; an empty partition fails
+on every rank with one message."""
 import os
 import pickle
 import subprocess
@@ -58,6 +59,30 @@ def test_start_bitwise_and_fit_within_tolerance(R, name, d, k, path):
     np.testing.assert_allclose(f["covs"], s["covs"], atol=10 * atol)
     assert abs(f["log_likelihood"] - s["log_likelihood"]) <= atol * abs(s["log_likelihood"])
     assert f["cluster_sizes"].sum() == 3000
+
+
+def test_dead_component_at_two_ranks():
+    # the E pass is the generic one (d = 132) and reads each row alone, so the ranks and the one-rank run differ only in
+    # the order of the fp64 sums and in the wgmma Gram's row ranges: each covariance is within 1e-5 of its component's
+    # spread (tests/test_gpu_gram.py) on both sides
+    c = _run(2)["dead"]
+    assert "harness_error" not in c, c.get("harness_error")
+    assert c["errs"] == [None, None], c["errs"]
+    f = c["outs"][0]["fit"]
+    for o in c["outs"]:
+        for key in ("weights", "means", "covs", "cluster_sizes"):
+            np.testing.assert_array_equal(o["fit"][key], f[key])
+    s = c["single"]["fit"]
+    assert f["n_iter"] == s["n_iter"] == 1
+    np.testing.assert_allclose(f["weights"], s["weights"], rtol=1e-9, atol=0)
+    np.testing.assert_allclose(f["means"], s["means"], rtol=0, atol=1e-9)
+    for j in range(3):
+        spread = np.diag(s["covs"][j]).max()
+        assert np.abs(f["covs"][j] - s["covs"][j]).max() <= 2e-5 * spread, j
+    lam = np.linalg.eigvalsh(f["covs"][2])
+    assert lam.max() > 0 and lam.min() >= -1e-6 * lam.max(), (lam.min(), lam.max())   # PSD within the Gram's bound
+    assert f["weights"][2] < 1e-80
+    assert f["cluster_sizes"].sum() == 3 * 4096 + 5
 
 
 @pytest.mark.parametrize("R", [2, 3])
