@@ -1,7 +1,8 @@
 """ctypes binding of libb2kmeans.so (the C ABI declared in include/b2kmeans.h).
 
-PyTorch tensors are used only as device-memory containers: every call hands raw ``data_ptr()``
-addresses and the current CUDA stream to the library.  There is NO fallback: if the shared library
+PyTorch tensors are used only as device-memory containers: every call hands raw addresses and the
+current CUDA stream to the library, which trusts them, so Context takes every device address through
+Context._dev after checking the tensor behind it.  There is NO fallback: if the shared library
 is missing or no CUDA device is present, the compute entry points raise.
 """
 from __future__ import annotations
@@ -119,6 +120,24 @@ class B2KError(RuntimeError):
         self.code = code
 
 
+def _u64(seed: int) -> int:
+    """A seed as the library's uint64_t (a negative seed wraps as in C)."""
+    return int(seed) & 0xFFFFFFFFFFFFFFFF
+
+
+def _dims(shape: Sequence[Optional[int]]) -> str:
+    return "[" + ", ".join("*" if s is None else str(s) for s in shape) + "]"
+
+
+def _host(a: Any, dtype: Any, shape: Sequence[Optional[int]], name: str) -> np.ndarray:
+    """a as a C-contiguous host array of dtype, once its shape is checked against `shape` (None: any extent).  The
+    caller keeps the array alive while the library reads it through .ctypes.data."""
+    arr = np.ascontiguousarray(a, dtype=dtype)
+    if arr.ndim != len(shape) or any(s is not None and e != s for e, s in zip(arr.shape, shape)):
+        raise ValueError(f"{name} must be a {arr.dtype} array {_dims(shape)}, got shape {list(arr.shape)}")
+    return arr
+
+
 class LogregParams(ctypes.Structure):
     _fields_ = [
         ("reg", ctypes.c_double),
@@ -174,8 +193,7 @@ def umap_params(n_neighbors: int = 15, n_components: int = 2, n_epochs: int = 20
     """b2k_umap_params from keyword values (n_epochs resolved by the caller)."""
     return UmapParams(int(n_neighbors), int(n_components), int(n_epochs), UMAP_INIT_CODES[init],
                       int(negative_sample_rate), 0, float(local_connectivity), float(set_op_mix_ratio),
-                      float(learning_rate), float(repulsion_strength), float(a), float(b),
-                      int(seed) & 0xFFFFFFFFFFFFFFFF)
+                      float(learning_rate), float(repulsion_strength), float(a), float(b), _u64(seed))
 
 
 class Stats(ctypes.Structure):
@@ -343,11 +361,9 @@ def linreg_solve(mean: np.ndarray, moments: np.ndarray, n_total: int, reg: float
     """b2k_linreg_solve (host only): the fit from the outputs of Context.linreg_moments -> (coef [d] float64,
     intercept, coordinate-descent sweeps)."""
     L = load_library()
-    mean = np.ascontiguousarray(mean, dtype=np.float64)
-    moments = np.ascontiguousarray(moments, dtype=np.float64)
+    mean = _host(mean, np.float64, (None,), "mean")
     d = int(mean.shape[0]) - 1
-    if mean.ndim != 1 or moments.shape != (d + 1, d + 1):
-        raise ValueError("mean must be [d + 1] and moments [d + 1, d + 1]")
+    moments = _host(moments, np.float64, (d + 1, d + 1), "moments")
     coef = np.zeros(max(d, 0), dtype=np.float64)
     b = ctypes.c_double(0.0)
     it = ctypes.c_int(0)
@@ -366,9 +382,7 @@ def logreg_minimize(fun: Any, x0: np.ndarray, l1: Optional[np.ndarray] = None, m
     L = load_library()
     x = np.array(x0, dtype=np.float64, copy=True)
     n = int(x.shape[0])
-    l1a = None if l1 is None else np.ascontiguousarray(l1, dtype=np.float64)
-    if l1a is not None and l1a.shape != (n,):
-        raise ValueError(f"l1 must be [{n}]")
+    l1a = None if l1 is None else _host(l1, np.float64, (n,), "l1")
     err: list = []
 
     def _cb(_user: Any, m: int, xp: Any, fp: Any, gp: Any) -> int:
@@ -422,6 +436,40 @@ class Context:
     def _stream(self) -> int:
         return _stream_handle(self._torch, self.device)
 
+    def _invoke(self, fn: str, *args: Any, after: Tuple[Any, ...] = ()) -> int:
+        """The status of the stream-ordered entry point fn(ctx, *args, stream, *after), called on this context's device
+        with its current stream."""
+        with self._torch.cuda.device(self.device):
+            return getattr(self._L, fn)(self._h, *args, self._stream(), *after)
+
+    def _call(self, fn: str, *args: Any, after: Tuple[Any, ...] = ()) -> None:
+        self._check(self._invoke(fn, *args, after=after))
+
+    def _dev(self, x: Any, dtype: Any, shape: Sequence[Optional[int]], name: str, optional: bool = False
+             ) -> Optional[int]:
+        """The device address of x, once x is checked to be a contiguous `dtype` tensor of `shape` (None: any extent)
+        on this context's device; None when optional and x is None.  The library trusts every address it receives, so
+        no tensor reaches it any other way."""
+        if x is None and optional:
+            return None
+        t = self._torch
+        if not (isinstance(x, t.Tensor) and x.device == self.device and x.dtype == dtype and x.is_contiguous()
+                and x.dim() == len(shape) and all(s is None or e == s for e, s in zip(x.shape, shape))):
+            got = (f"{'' if x.is_contiguous() else 'a non-contiguous '}{x.dtype} {list(x.shape)} on {x.device}"
+                   if isinstance(x, t.Tensor) else type(x).__name__)
+            raise ValueError(f"{name} must be a contiguous {dtype} tensor {_dims(shape)} on {self.device}, got {got}")
+        return x.data_ptr()
+
+    def _empty(self, shape: Sequence[int], dtype: Any) -> Tuple[Any, int]:
+        """A new output tensor on this device and its address."""
+        x = self._torch.empty(tuple(shape), dtype=dtype, device=self.device)
+        return x, self._dev(x, dtype, shape, "output")
+
+    def _check_X(self, X: Any, name: str = "X") -> Tuple[int, int, int]:
+        """(address, n, d) of the float32 rows X [n, d]."""
+        p = self._dev(X, self._torch.float32, (None, None), name)
+        return p, int(X.shape[0]), int(X.shape[1])
+
     def close(self) -> None:
         if getattr(self, "_h", None) is not None and self._h:
             self._L.b2k_ctx_destroy(self._h)
@@ -459,7 +507,8 @@ class Context:
 
     # -- comm -------------------------------------------------------------------------------
     def comm_init(self, nranks: int, rank: int, uid: bytes) -> None:
-        assert len(uid) == UNIQUE_ID_BYTES
+        if len(uid) != UNIQUE_ID_BYTES:
+            raise ValueError(f"uid must hold the {UNIQUE_ID_BYTES} bytes of comm_unique_id(), got {len(uid)}")
         self._check(self._L.b2k_comm_init(self._h, int(nranks), int(rank), uid))
         self.nranks, self.rank = int(nranks), int(rank)
 
@@ -478,9 +527,11 @@ class Context:
         code = _DTYPE_CODES.get(values.dtype)
         if code is None:
             raise TypeError(f"unsupported source dtype {values.dtype}")
-        assert values.flags.c_contiguous
+        if not values.flags.c_contiguous:
+            raise ValueError("values must be a C-contiguous host array")
+        dp = self._dev(dst, self._torch.float32, (None, int(d)), "dst")
         if offsets is not None:
-            offsets = np.ascontiguousarray(offsets, dtype=np.int32)
+            offsets = _host(offsets, np.int32, (None,), "offsets")
             n_b = offsets.shape[0] - 1
         else:
             n_b = int(n_rows) if n_rows is not None else values.size // d
@@ -490,20 +541,22 @@ class Context:
                 raise ValueError(f"feature batch holds {values.size} values for {n_b} rows of width {d}: "
                                  "row width differs from the expected dimension")
         wrote = ctypes.c_int64(0)
-        self._check(self._L.b2k_ingest_append(
-            self._h, dst.data_ptr(), int(dst.shape[0]), int(d), int(row0), values.ctypes.data,
-            offsets.ctypes.data if offsets is not None else None, int(n_b), code, LAYOUT_ROWS,
-            self._stream(), ctypes.byref(wrote)))
+        self._call("b2k_ingest_append", dp, int(dst.shape[0]), int(d), int(row0), values.ctypes.data,
+                   offsets.ctypes.data if offsets is not None else None, int(n_b), code, LAYOUT_ROWS,
+                   after=(ctypes.byref(wrote),))
         return int(wrote.value)
 
     def ingest_pinned_tensor(self, dst: Any, row0: int, src: Any) -> int:
         """Append a (pinned) host torch tensor [n_b, d] f32."""
-        assert src.dtype == self._torch.float32 and src.is_contiguous()
+        t = self._torch
+        if not (isinstance(src, t.Tensor) and src.device.type == "cpu" and src.dtype == t.float32 and src.dim() == 2
+                and src.is_contiguous()):
+            raise ValueError("src must be a contiguous float32 host tensor [n_b, d]")
         n_b, d = int(src.shape[0]), int(src.shape[1])
+        dp = self._dev(dst, t.float32, (None, d), "dst")
         wrote = ctypes.c_int64(0)
-        self._check(self._L.b2k_ingest_append(
-            self._h, dst.data_ptr(), int(dst.shape[0]), d, int(row0), src.data_ptr(), None, n_b, 0,
-            LAYOUT_ROWS, self._stream(), ctypes.byref(wrote)))
+        self._call("b2k_ingest_append", dp, int(dst.shape[0]), d, int(row0), src.data_ptr(), None, n_b, 0, LAYOUT_ROWS,
+                   after=(ctypes.byref(wrote),))
         return int(wrote.value)
 
     def ingest_columns(self, dst: Any, row0: int, columns: Sequence[np.ndarray]) -> int:
@@ -516,114 +569,86 @@ class Context:
         n_b = int(columns[0].shape[0])
         cols = [np.ascontiguousarray(c) for c in columns]
         for c in cols:
-            if c.dtype != dt or c.shape[0] != n_b:
+            if c.dtype != dt or c.shape != (n_b,):
                 raise ValueError("columns must share dtype and length")
+        dp = self._dev(dst, self._torch.float32, (None, d), "dst")
         ptrs = (ctypes.c_void_p * d)(*[c.ctypes.data for c in cols])
         wrote = ctypes.c_int64(0)
-        self._check(self._L.b2k_ingest_append(
-            self._h, dst.data_ptr(), int(dst.shape[0]), d, int(row0), ctypes.addressof(ptrs), None, n_b,
-            code, LAYOUT_COLUMNS, self._stream(), ctypes.byref(wrote)))
+        self._call("b2k_ingest_append", dp, int(dst.shape[0]), d, int(row0), ctypes.addressof(ptrs), None, n_b, code,
+                   LAYOUT_COLUMNS, after=(ctypes.byref(wrote),))
         self._torch.cuda.current_stream(self.device).synchronize()  # cols/ptrs must outlive the staging copies
         return int(wrote.value)
 
     # -- compute ----------------------------------------------------------------------------
-    def _check_X(self, X: Any) -> Tuple[int, int]:
-        t = self._torch
-        if not (X.is_cuda and X.dtype == t.float32 and X.dim() == 2 and X.is_contiguous()):
-            raise ValueError("X must be a contiguous float32 CUDA tensor [n, d]")
-        if X.device.index != self.device_index:
-            raise ValueError("X lives on a different device than this context")
-        return int(X.shape[0]), int(X.shape[1])
-
     def kmeans_fit(self, X: Any, k: int, *, init: Any = "scalable-k-means++", max_iter: int = 300,
                    tol: float = 1e-4, seed: int = 0, oversampling_factor: float = 2.0, n_init: int = 1,
                    compute_inertia: bool = True) -> Dict[str, Any]:
         """KMeansMG(**cuml_init).fit(X) equivalent.  Returns dict(cluster_centers_ [k,d] cuda tensor,
         n_iter_, inertia_)."""
         t = self._torch
-        n, d = self._check_X(X)
-        init_ptr = None
+        Xp, n, d = self._check_X(X)
         if isinstance(init, str):
             mode = {"scalable-k-means++": INIT_KMEANS_PARALLEL, "k-means||": INIT_KMEANS_PARALLEL,
                     "random": INIT_RANDOM}.get(init)
             if mode is None:
                 raise ValueError(f"unknown init {init!r}")
-            keep = None
+            init_p = None
         else:
             keep = t.as_tensor(init, dtype=t.float32, device=self.device).contiguous()
-            if tuple(keep.shape) != (k, d):
-                raise ValueError(f"init array must have shape ({k}, {d})")
+            init_p = self._dev(keep, t.float32, (int(k), d), "init")
             mode = INIT_ARRAY
-            init_ptr = keep.data_ptr()
-        centers = t.empty((k, d), dtype=t.float32, device=self.device)
+        centers, cp = self._empty((int(k), d), t.float32)
         n_iter = ctypes.c_int(0)
         inertia = ctypes.c_double(0.0)
-        with t.cuda.device(self.device):
-            self._check(self._L.b2k_kmeans_fit(
-                self._h, X.data_ptr(), n, d, int(k), mode, init_ptr, int(max_iter), float(tol),
-                int(seed) & 0xFFFFFFFFFFFFFFFF, float(oversampling_factor), int(n_init), centers.data_ptr(),
-                ctypes.byref(n_iter), ctypes.byref(inertia) if compute_inertia else None, self._stream()))
-        del keep
+        self._call("b2k_kmeans_fit", Xp, n, d, int(k), mode, init_p, int(max_iter), float(tol), _u64(seed),
+                   float(oversampling_factor), int(n_init), cp, ctypes.byref(n_iter),
+                   ctypes.byref(inertia) if compute_inertia else None)
         return {"cluster_centers_": centers, "n_iter_": int(n_iter.value),
                 "inertia_": float(inertia.value) if compute_inertia else None}
 
     def kmeans_lloyd(self, X: Any, centers: Any, max_iter: int, tol: float) -> Tuple[int, float]:
         """Lloyd loop in place on `centers` (cuda f32 [k,d]); returns (n_iter, last shift)."""
-        t = self._torch
-        n, d = self._check_X(X)
-        if not (centers.is_cuda and centers.dtype == t.float32 and centers.is_contiguous()
-                and centers.shape[1] == d):
-            raise ValueError("centers must be a contiguous float32 CUDA tensor [k, d]")
+        Xp, n, d = self._check_X(X)
+        cp = self._dev(centers, self._torch.float32, (None, d), "centers")
         n_iter = ctypes.c_int(0)
         shift = ctypes.c_double(0.0)
-        with t.cuda.device(self.device):
-            self._check(self._L.b2k_kmeans_lloyd(
-                self._h, X.data_ptr(), n, d, int(centers.shape[0]), centers.data_ptr(), int(max_iter),
-                float(tol), ctypes.byref(n_iter), ctypes.byref(shift), self._stream()))
+        self._call("b2k_kmeans_lloyd", Xp, n, d, int(centers.shape[0]), cp, int(max_iter), float(tol),
+                   ctypes.byref(n_iter), ctypes.byref(shift))
         return int(n_iter.value), float(shift.value)
 
     def kmeans_assign(self, X: Any, centers: Any, want_mindist: bool = False) -> Tuple[Any, Any]:
         """KMeans.predict equivalent: int32 labels (and optionally squared min distances)."""
         t = self._torch
-        n, d = self._check_X(X)
+        Xp, n, d = self._check_X(X)
         C = t.as_tensor(centers, dtype=t.float32, device=self.device).contiguous()
-        if C.dim() != 2 or C.shape[1] != d:
-            raise ValueError("centers must be [k, d]")
-        labels = t.empty((n,), dtype=t.int32, device=self.device)
-        md = t.empty((n,), dtype=t.float32, device=self.device) if want_mindist else None
-        with t.cuda.device(self.device):
-            self._check(self._L.b2k_kmeans_assign(
-                self._h, X.data_ptr(), n, d, C.data_ptr(), int(C.shape[0]), labels.data_ptr(),
-                md.data_ptr() if md is not None else None, self._stream()))
+        cp = self._dev(C, t.float32, (None, d), "centers")
+        labels, lp = self._empty((n,), t.int32)
+        md, mp = self._empty((n,), t.float32) if want_mindist else (None, None)
+        self._call("b2k_kmeans_assign", Xp, n, d, cp, int(C.shape[0]), lp, mp)
         t.cuda.current_stream(self.device).synchronize()  # C (a temporary) must outlive the kernels
         return labels, md
 
     def pca_fit(self, X: Any, k: int) -> Dict[str, np.ndarray]:
         """PCAMG(n_components=k).fit(X) equivalent (collective when a communicator is initialised).  Returns host float64
         arrays: mean_ [d], components_ [k, d], explained_variance_ratio_ [k], singular_values_ [k]."""
-        n, d = self._check_X(X)
+        Xp, n, d = self._check_X(X)
         kk = max(int(k), 0)
         mean = np.zeros(d, dtype=np.float64)
         comp = np.zeros((kk, d), dtype=np.float64)
         evr = np.zeros(kk, dtype=np.float64)
         sv = np.zeros(kk, dtype=np.float64)
-        with self._torch.cuda.device(self.device):
-            self._check(self._L.b2k_pca_fit(self._h, X.data_ptr(), n, d, int(k), mean.ctypes.data, comp.ctypes.data,
-                                            evr.ctypes.data, sv.ctypes.data, self._stream()))
+        self._call("b2k_pca_fit", Xp, n, d, int(k), mean.ctypes.data, comp.ctypes.data, evr.ctypes.data, sv.ctypes.data)
         return {"mean_": mean, "components_": comp, "explained_variance_ratio_": evr, "singular_values_": sv}
 
     def pca_transform(self, X: Any, components: Any) -> Any:
         """PCAModel.transform equivalent: X [n, d] . components^T -> float32 CUDA tensor [n, k] (no mean subtracted)."""
         t = self._torch
-        n, d = self._check_X(X)
+        Xp, n, d = self._check_X(X)
         C = t.as_tensor(components, dtype=t.float32, device=self.device).contiguous()
-        if C.dim() != 2 or C.shape[1] != d:
-            raise ValueError(f"components must be [k, {d}]")
+        cp = self._dev(C, t.float32, (None, d), "components")
         k = int(C.shape[0])
-        out = t.empty((n, k), dtype=t.float32, device=self.device)
-        with t.cuda.device(self.device):
-            self._check(self._L.b2k_pca_transform(self._h, X.data_ptr(), n, d, C.data_ptr(), k, out.data_ptr(),
-                                                  self._stream()))
+        out, op = self._empty((n, k), t.float32)
+        self._call("b2k_pca_transform", Xp, n, d, cp, k, op)
         t.cuda.current_stream(self.device).synchronize()  # C (possibly a temporary) must outlive the kernel
         return out
 
@@ -633,21 +658,15 @@ class Context:
         (either may have 0 rows), item_ids an int64 CUDA tensor [n_items] or None (ids = global rows).  Returns CUDA
         tensors distances float32 [n_q, k] (Euclidean, ascending) and indices int64 [n_q, k] (ids)."""
         t = self._torch
-        n, d = self._check_X(items)
-        nq, dq = self._check_X(queries)
+        ip, n, d = self._check_X(items, "items")
+        qp, nq, dq = self._check_X(queries, "queries")
         if dq != d:
             raise ValueError(f"queries have {dq} features, items {d}")
-        if item_ids is not None:
-            if not (item_ids.is_cuda and item_ids.dtype == t.int64 and item_ids.is_contiguous()
-                    and tuple(item_ids.shape) == (n,)):
-                raise ValueError("item_ids must be a contiguous int64 CUDA tensor [n_items]")
+        idp = self._dev(item_ids, t.int64, (n,), "item_ids", optional=True)
         kk = max(int(k), 0)
-        dist = t.empty((nq, kk), dtype=t.float32, device=self.device)
-        idx = t.empty((nq, kk), dtype=t.int64, device=self.device)
-        with t.cuda.device(self.device):
-            self._check(self._L.b2k_knn_search(
-                self._h, items.data_ptr(), n, item_ids.data_ptr() if item_ids is not None else None,
-                queries.data_ptr(), nq, d, int(k), dist.data_ptr(), idx.data_ptr(), self._stream()))
+        dist, dp = self._empty((nq, kk), t.float32)
+        idx, xp = self._empty((nq, kk), t.int64)
+        self._call("b2k_knn_search", ip, n, idp, qp, nq, d, int(k), dp, xp)
         return dist, idx
 
     IVF_METRICS = {"euclidean": 0, "l2": 0, "sqeuclidean": 1}
@@ -661,66 +680,51 @@ class Context:
         indices, centers) as CUDA tensors, plus (item lists int32 [n_items], probes int32 [n_q, min(nprobe, nlist)])
         with return_lists."""
         t = self._torch
-        n, d = self._check_X(items)
-        nq, dq = self._check_X(queries)
+        ip, n, d = self._check_X(items, "items")
+        qp, nq, dq = self._check_X(queries, "queries")
         if dq != d:
             raise ValueError(f"queries have {dq} features, items {d}")
         if metric not in self.IVF_METRICS:
             raise ValueError(f"metric {metric!r} is not supported by IVF-Flat (supported: {sorted(self.IVF_METRICS)})")
-        if item_ids is not None:
-            if not (item_ids.is_cuda and item_ids.dtype == t.int64 and item_ids.is_contiguous()
-                    and tuple(item_ids.shape) == (n,)):
-                raise ValueError("item_ids must be a contiguous int64 CUDA tensor [n_items]")
-        nl = max(int(nlist), 1)
+        idp = self._dev(item_ids, t.int64, (n,), "item_ids", optional=True)
         train = centers is None
-        if train:
-            C = t.empty((nl, d), dtype=t.float32, device=self.device)
-        else:
-            if not (centers.is_cuda and centers.dtype == t.float32 and centers.is_contiguous()
-                    and tuple(centers.shape) == (int(nlist), d)):
-                raise ValueError(f"centers must be a contiguous float32 CUDA tensor [{nlist}, {d}]")
-            C = centers.clone()
+        self._dev(centers, t.float32, (int(nlist), d), "centers", optional=True)
+        nl = max(int(nlist), 1)
         kk = max(int(k), 0)
         npr = max(min(int(nprobe), nl), 0)
-        dist = t.empty((nq, kk), dtype=t.float32, device=self.device)
-        idx = t.empty((nq, kk), dtype=t.int64, device=self.device)
-        lists = t.empty((n,), dtype=t.int32, device=self.device) if return_lists else None
-        probes = t.empty((nq, npr), dtype=t.int32, device=self.device) if return_lists else None
-        ptr = lambda x: x.data_ptr() if x is not None else None   # noqa: E731
-        with t.cuda.device(self.device):
-            self._check(self._L.b2k_ivf_search(
-                self._h, items.data_ptr(), n, ptr(item_ids), queries.data_ptr(), nq, d, int(k), int(nlist), int(nprobe),
-                int(n_iters), float(train_fraction), self.IVF_METRICS[metric], int(train), C.data_ptr(), ptr(lists),
-                ptr(probes), dist.data_ptr(), idx.data_ptr(), self._stream()))
+        if train:
+            C, Cp = self._empty((nl, d), t.float32)
+        else:
+            C = centers.clone()
+            Cp = self._dev(C, t.float32, (int(nlist), d), "centers")
+        dist, dp = self._empty((nq, kk), t.float32)
+        idx, xp = self._empty((nq, kk), t.int64)
+        lists, lp = self._empty((n,), t.int32) if return_lists else (None, None)
+        probes, pp = self._empty((nq, npr), t.int32) if return_lists else (None, None)
+        self._call("b2k_ivf_search", ip, n, idp, qp, nq, d, int(k), int(nlist), int(nprobe), int(n_iters),
+                   float(train_fraction), self.IVF_METRICS[metric], int(train), Cp, lp, pp, dp, xp)
         return (dist, idx, C, lists, probes) if return_lists else (dist, idx, C)
 
     def linreg_moments(self, X: Any, y: Any) -> Tuple[int, np.ndarray, np.ndarray]:
         """The passes over the data of a linear regression fit (collective when a communicator is initialised): X [n, d]
         and y [n] float32 CUDA tensors -> (n_total, mean [d + 1], centred moments [d + 1, d + 1] of [X | y]), host
         float64."""
-        t = self._torch
-        n, d = self._check_X(X)
-        if not (y.is_cuda and y.dtype == t.float32 and y.is_contiguous() and tuple(y.shape) == (n,)):
-            raise ValueError(f"y must be a contiguous float32 CUDA tensor [{n}]")
+        Xp, n, d = self._check_X(X)
+        yp = self._dev(y, self._torch.float32, (n,), "y")
         n_total = ctypes.c_int64(0)
         mean = np.zeros(d + 1, dtype=np.float64)
         mom = np.zeros((d + 1, d + 1), dtype=np.float64)
-        with t.cuda.device(self.device):
-            self._check(self._L.b2k_linreg_moments(self._h, X.data_ptr(), y.data_ptr(), n, d, ctypes.byref(n_total),
-                                                   mean.ctypes.data, mom.ctypes.data, self._stream()))
+        self._call("b2k_linreg_moments", Xp, yp, n, d, ctypes.byref(n_total), mean.ctypes.data, mom.ctypes.data)
         return int(n_total.value), mean, mom
 
     def linreg_predict(self, X: Any, coef: Any, intercept: float) -> Any:
         """intercept + X . coef, accumulated in fp64 -> float64 CUDA tensor [n]."""
         t = self._torch
-        n, d = self._check_X(X)
+        Xp, n, d = self._check_X(X)
         w = t.as_tensor(coef, dtype=t.float64, device=self.device).contiguous()
-        if tuple(w.shape) != (d,):
-            raise ValueError(f"coef must be [{d}]")
-        out = t.empty((n,), dtype=t.float64, device=self.device)
-        with t.cuda.device(self.device):
-            self._check(self._L.b2k_linreg_predict(self._h, X.data_ptr(), n, d, w.data_ptr(), float(intercept),
-                                                   out.data_ptr(), self._stream()))
+        wp = self._dev(w, t.float64, (d,), "coef")
+        out, op = self._empty((n,), t.float64)
+        self._call("b2k_linreg_predict", Xp, n, d, wp, float(intercept), op)
         t.cuda.current_stream(self.device).synchronize()  # w (possibly a temporary) must outlive the kernel
         return out
 
@@ -730,29 +734,23 @@ class Context:
         """GaussianMixture.fit (b2k_gmm_fit, collective when a communicator is initialised).  init = None draws the
         start from `seed`, or (weights [k], means [k, d], covariances [k, d, d]) starts from those values.  Returns host
         float64 arrays weights [k], means [k, d], covs [k, d, d], int64 cluster_sizes [k], and log_likelihood, n_iter."""
-        n, d = self._check_X(X)
+        Xp, n, d = self._check_X(X)
         kk = max(int(k), 0)
-        if init is None:
-            mode, iw, im, ic = INIT_RANDOM, None, None, None
-        else:
-            iw = np.ascontiguousarray(init[0], dtype=np.float64).reshape(-1)
-            im = np.ascontiguousarray(init[1], dtype=np.float64)
-            ic = np.ascontiguousarray(init[2], dtype=np.float64)
-            if iw.shape != (kk,) or im.shape != (kk, d) or ic.shape != (kk, d, d):
-                raise ValueError(f"init must be (weights [{kk}], means [{kk}, {d}], covariances [{kk}, {d}, {d}])")
-            mode = INIT_ARRAY
+        init_p: List[Optional[int]] = [None, None, None]
+        if init is not None:
+            iw = _host(np.ravel(init[0]), np.float64, (kk,), "init weights")
+            im = _host(init[1], np.float64, (kk, d), "init means")
+            ic = _host(init[2], np.float64, (kk, d, d), "init covariances")
+            init_p = [iw.ctypes.data, im.ctypes.data, ic.ctypes.data]
         w = np.zeros(kk, dtype=np.float64)
         mu = np.zeros((kk, d), dtype=np.float64)
         cov = np.zeros((kk, d, d), dtype=np.float64)
         sizes = np.zeros(kk, dtype=np.int64)
         ll = ctypes.c_double(0.0)
         n_iter = ctypes.c_int(0)
-        ptr = lambda a: a.ctypes.data if a is not None else None   # noqa: E731
-        with self._torch.cuda.device(self.device):
-            self._check(self._L.b2k_gmm_fit(
-                self._h, X.data_ptr(), n, d, int(k), mode, ptr(iw), ptr(im), ptr(ic), int(max_iter), float(tol),
-                int(seed) & 0xFFFFFFFFFFFFFFFF, w.ctypes.data, mu.ctypes.data, cov.ctypes.data, ctypes.byref(ll),
-                ctypes.byref(n_iter), sizes.ctypes.data, self._stream()))
+        self._call("b2k_gmm_fit", Xp, n, d, int(k), INIT_RANDOM if init is None else INIT_ARRAY, *init_p, int(max_iter),
+                   float(tol), _u64(seed), w.ctypes.data, mu.ctypes.data, cov.ctypes.data, ctypes.byref(ll),
+                   ctypes.byref(n_iter), sizes.ctypes.data)
         return {"weights": w, "means": mu, "covs": cov, "cluster_sizes": sizes, "log_likelihood": float(ll.value),
                 "n_iter": int(n_iter.value)}
 
@@ -760,18 +758,14 @@ class Context:
         """Per row of X: the float64 probabilities [n, k] and the int32 argmax [n] of a Gaussian mixture (CUDA
         tensors)."""
         t = self._torch
-        n, d = self._check_X(X)
-        w = np.ascontiguousarray(weights, dtype=np.float64).reshape(-1)
+        Xp, n, d = self._check_X(X)
+        w = _host(np.ravel(weights), np.float64, (None,), "weights")
         k = int(w.shape[0])
-        mu = np.ascontiguousarray(means, dtype=np.float64)
-        cov = np.ascontiguousarray(covs, dtype=np.float64)
-        if mu.shape != (k, d) or cov.shape != (k, d, d):
-            raise ValueError(f"means must be [{k}, {d}] and covariances [{k}, {d}, {d}]")
-        prob = t.empty((n, k), dtype=t.float64, device=self.device)
-        labels = t.empty((n,), dtype=t.int32, device=self.device)
-        with t.cuda.device(self.device):
-            self._check(self._L.b2k_gmm_predict(self._h, X.data_ptr(), n, d, k, w.ctypes.data, mu.ctypes.data,
-                                                cov.ctypes.data, prob.data_ptr(), labels.data_ptr(), self._stream()))
+        mu = _host(means, np.float64, (k, d), "means")
+        cov = _host(covs, np.float64, (k, d, d), "covs")
+        prob, pp = self._empty((n, k), t.float64)
+        labels, lp = self._empty((n,), t.int32)
+        self._call("b2k_gmm_predict", Xp, n, d, k, w.ctypes.data, mu.ctypes.data, cov.ctypes.data, pp, lp)
         return prob, labels
 
     # -- bisecting k-means -------------------------------------------------------------------
@@ -781,7 +775,7 @@ class Context:
         depth-first order as host arrays node_index int64 [m], centers float64 [m, d], sizes int64 [m], costs float64
         [m]; training_cost; cluster_sizes int64 [leaves]; n_levels; level_ms float64 [n_levels] (zeros unless option
         time_kernels is set)."""
-        n, d = self._check_X(X)
+        Xp, n, d = self._check_X(X)
         kk = max(int(k), 1)
         m = 2 * kk - 1
         idx = np.zeros(m, dtype=np.int64)
@@ -792,11 +786,9 @@ class Context:
         lms = np.zeros(BKM_MAX_LEVELS, dtype=np.float64)
         nn = ctypes.c_int(0)
         tc = ctypes.c_double(0.0)
-        with self._torch.cuda.device(self.device):
-            self._check(self._L.b2k_bkm_fit(
-                self._h, X.data_ptr(), n, d, int(k), int(max_iter), float(min_divisible), int(seed) & 0xFFFFFFFFFFFFFFFF,
-                ctypes.byref(nn), idx.ctypes.data, cen.ctypes.data, sizes.ctypes.data, costs.ctypes.data,
-                ctypes.byref(tc), csz.ctypes.data, lms.ctypes.data, self._stream()))
+        self._call("b2k_bkm_fit", Xp, n, d, int(k), int(max_iter), float(min_divisible), _u64(seed), ctypes.byref(nn),
+                   idx.ctypes.data, cen.ctypes.data, sizes.ctypes.data, costs.ctypes.data, ctypes.byref(tc),
+                   csz.ctypes.data, lms.ctypes.data)
         nn = int(nn.value)
         idx, cen = idx[:nn], cen.reshape(-1)[: nn * d].reshape(nn, d)
         ids = set(idx.tolist())
@@ -811,17 +803,12 @@ class Context:
         """Per row of X the int32 leaf (depth-first number) reached by descent and, with with_cost, the float64
         squared distance to that leaf's centre (CUDA tensors; the cost is None otherwise)."""
         t = self._torch
-        n, d = self._check_X(X)
-        idx = np.ascontiguousarray(node_index, dtype=np.int64).reshape(-1)
-        cen = np.ascontiguousarray(node_centers, dtype=np.float64)
-        if cen.shape != (idx.shape[0], d):
-            raise ValueError(f"node_centers must be [{idx.shape[0]}, {d}]")
-        labels = t.empty((n,), dtype=t.int32, device=self.device)
-        cost = t.empty((n,), dtype=t.float64, device=self.device) if with_cost else None
-        with t.cuda.device(self.device):
-            self._check(self._L.b2k_bkm_predict(self._h, X.data_ptr(), n, d, int(idx.shape[0]), idx.ctypes.data,
-                                                cen.ctypes.data, labels.data_ptr(),
-                                                cost.data_ptr() if cost is not None else None, self._stream()))
+        Xp, n, d = self._check_X(X)
+        idx = _host(np.ravel(node_index), np.int64, (None,), "node_index")
+        cen = _host(node_centers, np.float64, (idx.shape[0], d), "node_centers")
+        labels, lp = self._empty((n,), t.int32)
+        cost, cp = self._empty((n,), t.float64) if with_cost else (None, None)
+        self._call("b2k_bkm_predict", Xp, n, d, int(idx.shape[0]), idx.ctypes.data, cen.ctypes.data, lp, cp)
         return labels, cost
 
     # -- multilayer perceptron ----------------------------------------------------------------
@@ -835,71 +822,49 @@ class Context:
 
     def mlp_eval(self, X: Any, y: Any, layers: Sequence[int], weights: Any) -> Tuple[float, np.ndarray, int]:
         """One loss-and-gradient evaluation (collective): F(w) and its gradient [P] in Spark's flat layout, n_total."""
-        n, d = self._check_X(X)
-        self._check_y(y, n)
+        Xp, n, d = self._check_X(X)
+        yp = self._dev(y, self._torch.float32, (n,), "y")
         lay, P = self._mlp_layers(layers, d)
-        w = np.ascontiguousarray(weights, dtype=np.float64).reshape(-1)
-        if w.shape != (P,):
-            raise ValueError(f"weights must be [{P}]")
+        w = _host(np.ravel(weights), np.float64, (P,), "weights")
         f = ctypes.c_double(0.0)
         g = np.zeros(P, dtype=np.float64)
         nt = ctypes.c_int64(0)
-        with self._torch.cuda.device(self.device):
-            self._check(self._L.b2k_mlp_eval(self._h, X.data_ptr(), y.data_ptr(), n, lay.ctypes.data, int(lay.size),
-                                             w.ctypes.data, ctypes.byref(f), g.ctypes.data, ctypes.byref(nt),
-                                             self._stream()))
+        self._call("b2k_mlp_eval", Xp, yp, n, lay.ctypes.data, int(lay.size), w.ctypes.data, ctypes.byref(f),
+                   g.ctypes.data, ctypes.byref(nt))
         return float(f.value), g, int(nt.value)
 
     def mlp_fit(self, X: Any, y: Any, layers: Sequence[int], *, solver: str = "l-bfgs", max_iter: int = 100,
                 tol: float = 1e-6, step_size: float = 0.03, seed: int = 0, initial_weights: Any = None
                 ) -> Dict[str, Any]:
         """MultilayerPerceptronClassifier.fit (b2k_mlp_fit, collective) -> weights [P], objective_history, n_iter."""
-        n, d = self._check_X(X)
-        self._check_y(y, n)
+        Xp, n, d = self._check_X(X)
+        yp = self._dev(y, self._torch.float32, (n,), "y")
         lay, P = self._mlp_layers(layers, d)
         if solver not in MLP_SOLVERS:
             raise ValueError(f"solver must be one of {sorted(MLP_SOLVERS)}, got {solver!r}")
-        w0 = None
-        if initial_weights is not None:
-            w0 = np.ascontiguousarray(initial_weights, dtype=np.float64).reshape(-1)
-            if w0.shape != (P,):
-                raise ValueError(f"initialWeights must have {P} values, got {w0.size}")
+        w0 = None if initial_weights is None else _host(np.ravel(initial_weights), np.float64, (P,), "initialWeights")
         w = np.zeros(P, dtype=np.float64)
         hist = np.zeros(max(int(max_iter), 0) + 1, dtype=np.float64)
         it = ctypes.c_int(0)
-        with self._torch.cuda.device(self.device):
-            self._check(self._L.b2k_mlp_fit(
-                self._h, X.data_ptr(), y.data_ptr(), n, lay.ctypes.data, int(lay.size), MLP_SOLVERS[solver],
-                int(max_iter), float(tol), float(step_size), int(seed) & 0xFFFFFFFFFFFFFFFF,
-                w0.ctypes.data if w0 is not None else None, w.ctypes.data, hist.ctypes.data, ctypes.byref(it),
-                self._stream()))
+        self._call("b2k_mlp_fit", Xp, yp, n, lay.ctypes.data, int(lay.size), MLP_SOLVERS[solver], int(max_iter),
+                   float(tol), float(step_size), _u64(seed), w0.ctypes.data if w0 is not None else None, w.ctypes.data,
+                   hist.ctypes.data, ctypes.byref(it))
         return {"weights": w, "objective_history": hist[: it.value].copy(), "n_iter": int(it.value)}
 
     def mlp_predict(self, X: Any, layers: Sequence[int], weights: Any) -> Tuple[Any, Any, Any]:
         """rawPrediction [n, C], probability [n, C] and prediction [n] as float64 CUDA tensors."""
         t = self._torch
-        n, d = self._check_X(X)
+        Xp, n, d = self._check_X(X)
         lay, P = self._mlp_layers(layers, d)
-        w = np.ascontiguousarray(weights, dtype=np.float64).reshape(-1)
-        if w.shape != (P,):
-            raise ValueError(f"weights must be [{P}]")
+        w = _host(np.ravel(weights), np.float64, (P,), "weights")
         C = int(lay[-1]) if lay.size else 0
-        raw = t.empty((n, C), dtype=t.float64, device=self.device)
-        prob = t.empty((n, C), dtype=t.float64, device=self.device)
-        pred = t.empty((n,), dtype=t.float64, device=self.device)
-        with t.cuda.device(self.device):
-            self._check(self._L.b2k_mlp_predict(self._h, X.data_ptr(), n, lay.ctypes.data, int(lay.size), w.ctypes.data,
-                                                raw.data_ptr(), prob.data_ptr(), pred.data_ptr(), self._stream()))
+        raw, rp = self._empty((n, C), t.float64)
+        prob, pp = self._empty((n, C), t.float64)
+        pred, dp = self._empty((n,), t.float64)
+        self._call("b2k_mlp_predict", Xp, n, lay.ctypes.data, int(lay.size), w.ctypes.data, rp, pp, dp)
         return raw, prob, pred
 
     # -- ALS ------------------------------------------------------------------------------------
-    def _als_col(self, v: Any, n: int, dtype: Any, name: str) -> Any:
-        t = self._torch
-        if not (isinstance(v, t.Tensor) and v.is_cuda and v.dtype == dtype and v.dim() == 1 and v.is_contiguous()
-                and v.shape[0] == n):
-            raise ValueError(f"{name} must be a contiguous 1-D {dtype} CUDA tensor of {n} values")
-        return v
-
     def als_fit(self, users: Any, items: Any, ratings: Any, *, rank: int = 10, max_iter: int = 10,
                 reg_param: float = 0.1, implicit_prefs: bool = False, alpha: float = 1.0, seed: int = 0,
                 init_user_factors: Any = None) -> Dict[str, Any]:
@@ -907,31 +872,25 @@ class Context:
         CUDA tensors of this rank's triples -> user_ids [U] int32, user_factors [U, rank] float32, item_ids [I],
         item_factors [I, rank] (CUDA tensors, sorted by id).  init_user_factors: [U, rank] float32 in user-id order."""
         t = self._torch
-        n = int(users.shape[0]) if users is not None else 0
-        self._als_col(users, n, t.float64, "users")
-        self._als_col(items, n, t.float64, "items")
-        if ratings is not None:
-            self._als_col(ratings, n, t.float32, "ratings")
+        up = self._dev(users, t.float64, (None,), "users")
+        n = int(users.shape[0])
+        ip = self._dev(items, t.float64, (n,), "items")
+        rp = self._dev(ratings, t.float32, (n,), "ratings", optional=True)
         w0, nw = None, 0
         if init_user_factors is not None:
-            w0 = np.ascontiguousarray(init_user_factors, dtype=np.float32)
-            if w0.ndim != 2 or w0.shape[1] != int(rank):
-                raise ValueError(f"init_user_factors must be [n_users, {rank}]")
+            w0 = _host(init_user_factors, np.float32, (None, int(rank)), "init_user_factors")
             nw = int(w0.shape[0])
         nu, ni = ctypes.c_int64(0), ctypes.c_int64(0)
         cap_u = cap_i = max(min(n, 1 << 20), nw, 1)
         for _ in range(2):   # a cap too small fails on every rank with the sizes set: every rank calls again with them
-            uid = t.empty(max(cap_u, 1), dtype=t.int32, device=self.device)
-            uf = t.empty((max(cap_u, 1), int(rank)), dtype=t.float32, device=self.device)
-            iid = t.empty(max(cap_i, 1), dtype=t.int32, device=self.device)
-            itf = t.empty((max(cap_i, 1), int(rank)), dtype=t.float32, device=self.device)
-            with t.cuda.device(self.device):
-                rc = self._L.b2k_als_fit(
-                    self._h, users.data_ptr() if n else None, items.data_ptr() if n else None,
-                    ratings.data_ptr() if (ratings is not None and n) else None, n, int(rank), int(max_iter),
-                    float(reg_param), int(bool(implicit_prefs)), float(alpha), int(seed) & 0xFFFFFFFFFFFFFFFF,
-                    w0.ctypes.data if w0 is not None else None, nw, cap_u, cap_i, uid.data_ptr(), uf.data_ptr(),
-                    iid.data_ptr(), itf.data_ptr(), ctypes.byref(nu), ctypes.byref(ni), self._stream())
+            uid, uidp = self._empty((max(cap_u, 1),), t.int32)
+            uf, ufp = self._empty((max(cap_u, 1), int(rank)), t.float32)
+            iid, iidp = self._empty((max(cap_i, 1),), t.int32)
+            itf, itfp = self._empty((max(cap_i, 1), int(rank)), t.float32)
+            rc = self._invoke("b2k_als_fit", up if n else None, ip if n else None, rp if n else None, n, int(rank),
+                              int(max_iter), float(reg_param), int(bool(implicit_prefs)), float(alpha), _u64(seed),
+                              w0.ctypes.data if w0 is not None else None, nw, cap_u, cap_i, uidp, ufp, iidp, itfp,
+                              ctypes.byref(nu), ctypes.byref(ni))
             if rc != B2K_OK and (self._L.b2k_last_error(self._h) or b"").startswith(b"ALS: the outputs hold fewer"):
                 cap_u, cap_i = max(cap_u, nu.value), max(cap_i, ni.value)
                 continue
@@ -944,80 +903,69 @@ class Context:
                     item_factors: Any) -> Any:
         """ALSModel.transform's prediction (b2k_als_predict): float32 [n], NaN for an unknown id."""
         t = self._torch
+        up = self._dev(users, t.float64, (None,), "users")
         n = int(users.shape[0])
-        self._als_col(users, n, t.float64, "users")
-        self._als_col(items, n, t.float64, "items")
+        ip = self._dev(items, t.float64, (n,), "items")
+        uidp = self._dev(user_ids, t.int32, (None,), "user_ids")
+        nu = int(user_ids.shape[0])
+        ufp = self._dev(user_factors, t.float32, (nu, None), "user_factors")
         rank = int(user_factors.shape[1])
-        out = t.empty(n, dtype=t.float32, device=self.device)
-        with t.cuda.device(self.device):
-            self._check(self._L.b2k_als_predict(self._h, users.data_ptr(), items.data_ptr(), n, rank,
-                                                user_ids.data_ptr(), user_factors.data_ptr(), int(user_ids.shape[0]),
-                                                item_ids.data_ptr(), item_factors.data_ptr(), int(item_ids.shape[0]),
-                                                out.data_ptr(), self._stream()))
+        iidp = self._dev(item_ids, t.int32, (None,), "item_ids")
+        ni = int(item_ids.shape[0])
+        ifp = self._dev(item_factors, t.float32, (ni, rank), "item_factors")
+        out, op = self._empty((n,), t.float32)
+        self._call("b2k_als_predict", up, ip, n, rank, uidp, ufp, nu, iidp, ifp, ni, op)
         return out
 
     def als_recommend(self, Q: Any, T: Any, n: int) -> Tuple[Any, Any]:
         """The n best rows of T [nt, rank] for each row of Q [nq, rank] (b2k_als_recommend): row indices [nq, n] int32
         (-1 past nt) and scores [nq, n] float32, score descending, the lower row first on a tie."""
         t = self._torch
+        qp = self._dev(Q, t.float32, (None, None), "Q")
         nq, rank = int(Q.shape[0]), int(Q.shape[1])
+        tp = self._dev(T, t.float32, (None, rank), "T")
         nt = int(T.shape[0])
-        idx = t.empty((nq, int(n)), dtype=t.int32, device=self.device)
-        sc = t.empty((nq, int(n)), dtype=t.float32, device=self.device)
-        with t.cuda.device(self.device):
-            self._check(self._L.b2k_als_recommend(self._h, Q.data_ptr() if nq else None, nq,
-                                                  T.data_ptr() if nt else None, nt, rank, int(n), idx.data_ptr(),
-                                                  sc.data_ptr(), self._stream()))
+        idx, xp = self._empty((nq, int(n)), t.int32)
+        sc, sp = self._empty((nq, int(n)), t.float32)
+        self._call("b2k_als_recommend", qp if nq else None, nq, tp if nt else None, nt, rank, int(n), xp, sp)
         return idx, sc
 
     # -- logistic regression ----------------------------------------------------------------
-    def _check_y(self, y: Any, n: int) -> None:
-        t = self._torch
-        if not (y.is_cuda and y.dtype == t.float32 and y.is_contiguous() and tuple(y.shape) == (n,)):
-            raise ValueError(f"y must be a contiguous float32 CUDA tensor [{n}]")
-
     def logreg_labels(self, y: Any) -> Tuple[np.ndarray, np.ndarray, int]:
         """The label pass (collective): y [n] float32 CUDA tensor -> (classes float64 [K], counts int64 [K], n_total)."""
-        n = int(y.shape[0]) if y.dim() == 1 else -1
-        self._check_y(y, n)
+        yp = self._dev(y, self._torch.float32, (None,), "y")
         cls = np.zeros(1024, dtype=np.float64)
         cnt = np.zeros(1024, dtype=np.int64)
         k, nt = ctypes.c_int(0), ctypes.c_int64(0)
-        with self._torch.cuda.device(self.device):
-            self._check(self._L.b2k_logreg_labels(self._h, y.data_ptr(), n, cls.ctypes.data, cnt.ctypes.data,
-                                                  ctypes.byref(k), ctypes.byref(nt), self._stream()))
+        self._call("b2k_logreg_labels", yp, int(y.shape[0]), cls.ctypes.data, cnt.ctypes.data, ctypes.byref(k),
+                   ctypes.byref(nt))
         return cls[: k.value].copy(), cnt[: k.value].copy(), int(nt.value)
 
-    def logreg_eval(self, X: Any, y: Any, classes: Sequence[float], W: np.ndarray, b: np.ndarray
-                    ) -> Tuple[float, np.ndarray, np.ndarray, int]:
-        """One loss-and-gradient evaluation (collective): (1/n) sum loss and its gradient at W [kp, d], b [kp] (no
-        penalty) -> (loss, dW [kp, d], db [kp], n_total)."""
-        n, d = self._check_X(X)
-        self._check_y(y, n)
-        cls = np.ascontiguousarray(classes, dtype=np.float64)
-        W = np.ascontiguousarray(W, dtype=np.float64)
+    @staticmethod
+    def _logreg_W(W: Any, b: Any, d: int) -> Tuple[np.ndarray, np.ndarray, int]:
+        """Host float64 W [kp, d] and b [kp] of a logistic model, and kp."""
+        W = _host(W, np.float64, (None, d), "W")
         kp = int(W.shape[0])
-        b = np.ascontiguousarray(b, dtype=np.float64)
-        if W.shape != (kp, d) or b.shape != (kp,):
-            raise ValueError(f"W must be [kp, {d}] and b [kp]")
+        return W, _host(b, np.float64, (kp,), "b"), kp
+
+    def _logreg_eval(self, fn: str, data: Sequence[Any], d: int, classes: Sequence[float], W: Any, b: Any
+                     ) -> Tuple[float, np.ndarray, np.ndarray, int]:
+        """logreg_eval through the entry point fn; data: its (checked) arguments before classes."""
+        cls = _host(classes, np.float64, (None,), "classes")
+        W, b, kp = self._logreg_W(W, b, d)
         loss = ctypes.c_double(0.0)
         grad = np.zeros((kp, d + 1), dtype=np.float64)
         nt = ctypes.c_int64(0)
-        with self._torch.cuda.device(self.device):
-            self._check(self._L.b2k_logreg_eval(self._h, X.data_ptr(), y.data_ptr(), n, d, cls.ctypes.data, int(cls.size),
-                                                kp, W.ctypes.data, b.ctypes.data, ctypes.byref(loss), grad.ctypes.data,
-                                                ctypes.byref(nt), self._stream()))
+        self._call(fn, *data, cls.ctypes.data, int(cls.size), kp, W.ctypes.data, b.ctypes.data, ctypes.byref(loss),
+                   grad.ctypes.data, ctypes.byref(nt))
         return float(loss.value), grad[:, :d].copy(), grad[:, d].copy(), int(nt.value)
 
-    def logreg_fit(self, X: Any, y: Any, classes: np.ndarray, counts: np.ndarray, settings: Sequence[Dict[str, Any]]
-                   ) -> List[Tuple[np.ndarray, np.ndarray, int]]:
-        """Fits (collective), one per setting dict (reg, l1_ratio, tol, max_iter, fit_intercept, standardization,
-        family) from one column-moments pass -> [(coef [kp, d], intercept [kp], iterations)]."""
-        n, d = self._check_X(X)
-        self._check_y(y, n)
-        cls = np.ascontiguousarray(classes, dtype=np.float64)
-        cnt = np.ascontiguousarray(counts, dtype=np.int64)
+    def _logreg_fit(self, fn: str, data: Sequence[Any], d: int, classes: np.ndarray, counts: np.ndarray,
+                    settings: Sequence[Dict[str, Any]]) -> List[Tuple[np.ndarray, np.ndarray, int]]:
+        """logreg_fit through the entry point fn; data: its (checked) arguments before classes."""
+        cls = _host(classes, np.float64, (None,), "classes")
         K, m = int(cls.size), len(settings)
+        cnt = _host(counts, np.int64, (K,), "counts")
         prm = (LogregParams * m)(*[LogregParams(float(s["reg"]), float(s["l1_ratio"]), float(s["tol"]),
                                                 int(s["max_iter"]), int(bool(s["fit_intercept"])),
                                                 int(bool(s["standardization"])), FAMILY_CODES[s["family"]])
@@ -1026,37 +974,65 @@ class Context:
         icpt = np.zeros((m, K), dtype=np.float64)
         kp = np.zeros(m, dtype=np.int32)
         it = np.zeros(m, dtype=np.int32)
-        with self._torch.cuda.device(self.device):
-            self._check(self._L.b2k_logreg_fit(self._h, X.data_ptr(), y.data_ptr(), n, d, cls.ctypes.data, cnt.ctypes.data,
-                                               K, m, prm, coef.ctypes.data, icpt.ctypes.data, kp.ctypes.data,
-                                               it.ctypes.data, self._stream()))
+        self._call(fn, *data, cls.ctypes.data, cnt.ctypes.data, K, m, prm, coef.ctypes.data, icpt.ctypes.data,
+                   kp.ctypes.data, it.ctypes.data)
         return [(coef[f, : kp[f]].copy(), icpt[f, : kp[f]].copy(), int(it[f])) for f in range(m)]
+
+    def _logreg_model(self, W: Any, b: Any, class_values: Sequence[float], d: int
+                      ) -> Tuple[int, List[Any], List[Any]]:
+        """nout, the device copies of W [kp, d], b [kp] and class_values [nout] of a logistic model (nout = 2 for a
+        binomial W [1, d]), and the predict entry points' arguments kp, W, b, class values."""
+        t = self._torch
+        W, b, kp = self._logreg_W(W, b, d)
+        nout = 2 if kp == 1 else kp
+        cv = _host(class_values, np.float64, (nout,), "class_values")
+        dev = [t.as_tensor(a, device=self.device) for a in (W, b, cv)]
+        return nout, dev, [kp] + [self._dev(x, t.float64, x.shape, name)
+                                  for x, name in zip(dev, ("W", "b", "class_values"))]
+
+    def logreg_eval(self, X: Any, y: Any, classes: Sequence[float], W: np.ndarray, b: np.ndarray
+                    ) -> Tuple[float, np.ndarray, np.ndarray, int]:
+        """One loss-and-gradient evaluation (collective): (1/n) sum loss and its gradient at W [kp, d], b [kp] (no
+        penalty) -> (loss, dW [kp, d], db [kp], n_total)."""
+        Xp, n, d = self._check_X(X)
+        yp = self._dev(y, self._torch.float32, (n,), "y")
+        return self._logreg_eval("b2k_logreg_eval", (Xp, yp, n, d), d, classes, W, b)
+
+    def logreg_fit(self, X: Any, y: Any, classes: np.ndarray, counts: np.ndarray, settings: Sequence[Dict[str, Any]]
+                   ) -> List[Tuple[np.ndarray, np.ndarray, int]]:
+        """Fits (collective), one per setting dict (reg, l1_ratio, tol, max_iter, fit_intercept, standardization,
+        family) from one column-moments pass -> [(coef [kp, d], intercept [kp], iterations)]."""
+        Xp, n, d = self._check_X(X)
+        yp = self._dev(y, self._torch.float32, (n,), "y")
+        return self._logreg_fit("b2k_logreg_fit", (Xp, yp, n, d), d, classes, counts, settings)
 
     def logreg_predict(self, X: Any, W: Any, b: Any, class_values: Sequence[float]) -> Tuple[Any, Any, Any]:
         """rawPrediction [n, nout], probability [n, nout] and prediction [n] as float64 CUDA tensors (nout = 2 for a
         binomial W [1, d])."""
         t = self._torch
-        n, d = self._check_X(X)
-        Wd = t.as_tensor(np.ascontiguousarray(W, dtype=np.float64), device=self.device).contiguous()
-        bd = t.as_tensor(np.ascontiguousarray(b, dtype=np.float64), device=self.device).contiguous()
-        kp = int(Wd.shape[0])
-        if tuple(Wd.shape) != (kp, d) or tuple(bd.shape) != (kp,):
-            raise ValueError(f"W must be [kp, {d}] and b [kp]")
-        nout = 2 if kp == 1 else kp
-        cv = t.as_tensor(np.ascontiguousarray(class_values, dtype=np.float64), device=self.device).contiguous()
-        if tuple(cv.shape) != (nout,):
-            raise ValueError(f"class_values must be [{nout}]")
-        raw = t.empty((n, nout), dtype=t.float64, device=self.device)
-        prob = t.empty((n, nout), dtype=t.float64, device=self.device)
-        pred = t.empty((n,), dtype=t.float64, device=self.device)
-        with t.cuda.device(self.device):
-            self._check(self._L.b2k_logreg_predict(self._h, X.data_ptr(), n, d, kp, Wd.data_ptr(), bd.data_ptr(),
-                                                   cv.data_ptr(), raw.data_ptr(), prob.data_ptr(), pred.data_ptr(),
-                                                   self._stream()))
+        Xp, n, d = self._check_X(X)
+        nout, (Wd, bd, cv), model = self._logreg_model(W, b, class_values, d)
+        raw, rp = self._empty((n, nout), t.float64)
+        prob, pp = self._empty((n, nout), t.float64)
+        pred, dp = self._empty((n,), t.float64)
+        self._call("b2k_logreg_predict", Xp, n, d, *model, rp, pp, dp)
         t.cuda.current_stream(self.device).synchronize()  # Wd, bd, cv (temporaries) must outlive the kernel
         return raw, prob, pred
 
     # -- sparse logistic regression: rows as a device CSR (indptr int64 [n + 1], indices int32, values float32) --------
+    def _check_csr(self, X: Any, d: int) -> Tuple[List[int], int, int]:
+        """The addresses of the CSR triple X = (indptr [n + 1], indices [nnz], values [nnz]) of width d, n and nnz."""
+        t = self._torch
+        indptr, indices, values = X
+        ptrs = [self._dev(indptr, t.int64, (None,), "indptr"), self._dev(indices, t.int32, (None,), "indices")]
+        nnz = int(indices.shape[0])
+        ptrs.append(self._dev(values, t.float32, (nnz,), "values"))
+        if indptr.shape[0] < 1:
+            raise ValueError("indptr must hold n + 1 >= 1 offsets")
+        if int(d) < 1:
+            raise ValueError("d must be >= 1")
+        return ptrs, int(indptr.shape[0]) - 1, nnz
+
     def ingest_csr(self, indptr: Any, indices: Any, values: Any, d: int, row0: int, nnz0: int, type_: np.ndarray,
                    size: np.ndarray, idx_offsets: np.ndarray, idx_values: np.ndarray, val_offsets: np.ndarray,
                    val_values: np.ndarray) -> int:
@@ -1065,94 +1041,43 @@ class Context:
         code = _DTYPE_CODES.get(val_values.dtype)
         if code not in (0, 1):
             raise TypeError(f"unsupported vector value dtype {val_values.dtype}")
-        arrs = [np.ascontiguousarray(type_, dtype=np.int8), np.ascontiguousarray(size, dtype=np.int32),
-                np.ascontiguousarray(idx_offsets, dtype=np.int32), np.ascontiguousarray(idx_values, dtype=np.int32),
-                np.ascontiguousarray(val_offsets, dtype=np.int32), np.ascontiguousarray(val_values)]
+        ptrs, n_max, nnz_max = self._check_csr((indptr, indices, values), d)
+        tp = _host(type_, np.int8, (None,), "type")
+        n_b = int(tp.shape[0])
+        arrs = [tp, _host(size, np.int32, (n_b,), "size"), _host(idx_offsets, np.int32, (n_b + 1,), "idx_offsets"),
+                _host(idx_values, np.int32, (None,), "idx_values"),
+                _host(val_offsets, np.int32, (n_b + 1,), "val_offsets"),
+                _host(val_values, val_values.dtype, (None,), "val_values")]
         wrote = ctypes.c_int64(0)
-        self._check(self._L.b2k_ingest_csr_append(
-            self._h, indptr.data_ptr(), indices.data_ptr(), values.data_ptr(), int(indptr.shape[0]) - 1,
-            int(indices.shape[0]), int(d), int(row0), int(nnz0), *[a.ctypes.data for a in arrs], code,
-            int(arrs[0].shape[0]), self._stream(), ctypes.byref(wrote)))
+        self._call("b2k_ingest_csr_append", *ptrs, n_max, nnz_max, int(d), int(row0), int(nnz0),
+                   *[a.ctypes.data for a in arrs], code, n_b, after=(ctypes.byref(wrote),))
         return int(wrote.value)
-
-    def _check_csr(self, X: Any, d: int) -> Tuple[int, int]:
-        t = self._torch
-        indptr, indices, values = X
-        ok = (indptr.dtype == t.int64 and indices.dtype == t.int32 and values.dtype == t.float32 and
-              all(a.is_cuda and a.dim() == 1 and a.is_contiguous() and a.device.index == self.device_index
-                  for a in X) and indices.shape == values.shape and indptr.shape[0] >= 1)
-        if not ok:
-            raise ValueError("X must be a CSR triple of contiguous CUDA tensors on this device: indptr int64 [n + 1], "
-                             "indices int32 [nnz], values float32 [nnz]")
-        if int(d) < 1:
-            raise ValueError("d must be >= 1")
-        return int(indptr.shape[0]) - 1, int(indices.shape[0])
 
     def logreg_eval_csr(self, X: Any, d: int, y: Any, classes: Sequence[float], W: np.ndarray, b: np.ndarray
                         ) -> Tuple[float, np.ndarray, np.ndarray, int]:
         """logreg_eval on CSR rows X = (indptr, indices, values) of width d (collective; builds its own CSC)."""
-        n, nnz = self._check_csr(X, d)
-        self._check_y(y, n)
-        cls = np.ascontiguousarray(classes, dtype=np.float64)
-        W = np.ascontiguousarray(W, dtype=np.float64)
-        kp = int(W.shape[0])
-        b = np.ascontiguousarray(b, dtype=np.float64)
-        if W.shape != (kp, d) or b.shape != (kp,):
-            raise ValueError(f"W must be [kp, {d}] and b [kp]")
-        loss = ctypes.c_double(0.0)
-        grad = np.zeros((kp, d + 1), dtype=np.float64)
-        nt = ctypes.c_int64(0)
-        with self._torch.cuda.device(self.device):
-            self._check(self._L.b2k_logreg_eval_csr(self._h, *[a.data_ptr() for a in X], n, nnz, int(d), y.data_ptr(),
-                                                    cls.ctypes.data, int(cls.size), kp, W.ctypes.data, b.ctypes.data,
-                                                    ctypes.byref(loss), grad.ctypes.data, ctypes.byref(nt),
-                                                    self._stream()))
-        return float(loss.value), grad[:, :d].copy(), grad[:, d].copy(), int(nt.value)
+        ptrs, n, nnz = self._check_csr(X, d)
+        yp = self._dev(y, self._torch.float32, (n,), "y")
+        return self._logreg_eval("b2k_logreg_eval_csr", (*ptrs, n, nnz, int(d), yp), int(d), classes, W, b)
 
     def logreg_fit_csr(self, X: Any, d: int, y: Any, classes: np.ndarray, counts: np.ndarray,
                        settings: Sequence[Dict[str, Any]]) -> List[Tuple[np.ndarray, np.ndarray, int]]:
         """logreg_fit on CSR rows X = (indptr, indices, values) of width d: one CSC and one moments pass for every
         setting (collective)."""
-        n, nnz = self._check_csr(X, d)
-        self._check_y(y, n)
-        cls = np.ascontiguousarray(classes, dtype=np.float64)
-        cnt = np.ascontiguousarray(counts, dtype=np.int64)
-        K, m = int(cls.size), len(settings)
-        prm = (LogregParams * m)(*[LogregParams(float(s["reg"]), float(s["l1_ratio"]), float(s["tol"]),
-                                                int(s["max_iter"]), int(bool(s["fit_intercept"])),
-                                                int(bool(s["standardization"])), FAMILY_CODES[s["family"]])
-                                   for s in settings])
-        coef = np.zeros((m, K, d), dtype=np.float64)
-        icpt = np.zeros((m, K), dtype=np.float64)
-        kp = np.zeros(m, dtype=np.int32)
-        it = np.zeros(m, dtype=np.int32)
-        with self._torch.cuda.device(self.device):
-            self._check(self._L.b2k_logreg_fit_csr(self._h, *[a.data_ptr() for a in X], n, nnz, int(d), y.data_ptr(),
-                                                   cls.ctypes.data, cnt.ctypes.data, K, m, prm, coef.ctypes.data,
-                                                   icpt.ctypes.data, kp.ctypes.data, it.ctypes.data, self._stream()))
-        return [(coef[f, : kp[f]].copy(), icpt[f, : kp[f]].copy(), int(it[f])) for f in range(m)]
+        ptrs, n, nnz = self._check_csr(X, d)
+        yp = self._dev(y, self._torch.float32, (n,), "y")
+        return self._logreg_fit("b2k_logreg_fit_csr", (*ptrs, n, nnz, int(d), yp), int(d), classes, counts, settings)
 
     def logreg_predict_csr(self, X: Any, d: int, W: Any, b: Any, class_values: Sequence[float]
                            ) -> Tuple[Any, Any, Any]:
         """logreg_predict on CSR rows X = (indptr, indices, values) of width d."""
         t = self._torch
-        n, nnz = self._check_csr(X, d)
-        Wd = t.as_tensor(np.ascontiguousarray(W, dtype=np.float64), device=self.device).contiguous()
-        bd = t.as_tensor(np.ascontiguousarray(b, dtype=np.float64), device=self.device).contiguous()
-        kp = int(Wd.shape[0])
-        if tuple(Wd.shape) != (kp, d) or tuple(bd.shape) != (kp,):
-            raise ValueError(f"W must be [kp, {d}] and b [kp]")
-        nout = 2 if kp == 1 else kp
-        cv = t.as_tensor(np.ascontiguousarray(class_values, dtype=np.float64), device=self.device).contiguous()
-        if tuple(cv.shape) != (nout,):
-            raise ValueError(f"class_values must be [{nout}]")
-        raw = t.empty((n, nout), dtype=t.float64, device=self.device)
-        prob = t.empty((n, nout), dtype=t.float64, device=self.device)
-        pred = t.empty((n,), dtype=t.float64, device=self.device)
-        with t.cuda.device(self.device):
-            self._check(self._L.b2k_logreg_predict_csr(self._h, *[a.data_ptr() for a in X], n, nnz, int(d), kp,
-                                                       Wd.data_ptr(), bd.data_ptr(), cv.data_ptr(), raw.data_ptr(),
-                                                       prob.data_ptr(), pred.data_ptr(), self._stream()))
+        ptrs, n, nnz = self._check_csr(X, d)
+        nout, (Wd, bd, cv), model = self._logreg_model(W, b, class_values, int(d))
+        raw, rp = self._empty((n, nout), t.float64)
+        prob, pp = self._empty((n, nout), t.float64)
+        pred, dp = self._empty((n,), t.float64)
+        self._call("b2k_logreg_predict_csr", *ptrs, n, nnz, int(d), *model, rp, pp, dp)
         t.cuda.current_stream(self.device).synchronize()  # Wd, bd, cv (temporaries) must outlive the kernel
         return raw, prob, pred
 
@@ -1162,16 +1087,14 @@ class Context:
         have 0 rows) -> (labels int32 [n], core flags bool [n], both CUDA tensors for this rank's rows, and the number of
         clusters).  metric is "euclidean" or "cosine"."""
         t = self._torch
-        n, d = self._check_X(X)
+        Xp, n, d = self._check_X(X)
         if metric not in METRIC_CODES:
             raise ValueError(f"metric must be one of {sorted(METRIC_CODES)}, got {metric!r}")
-        labels = t.empty((n,), dtype=t.int32, device=self.device)
-        core = t.empty((n,), dtype=t.uint8, device=self.device)
+        labels, lp = self._empty((n,), t.int32)
+        core, cp = self._empty((n,), t.uint8)
         ncl = ctypes.c_int64(0)
-        with t.cuda.device(self.device):
-            self._check(self._L.b2k_dbscan_fit(self._h, X.data_ptr(), n, d, float(eps), int(min_samples),
-                                               METRIC_CODES[metric], labels.data_ptr(), core.data_ptr(),
-                                               ctypes.byref(ncl), self._stream()))
+        self._call("b2k_dbscan_fit", Xp, n, d, float(eps), int(min_samples), METRIC_CODES[metric], lp, cp,
+                   ctypes.byref(ncl))
         return labels, core.bool(), int(ncl.value)
 
     # -- silhouette -------------------------------------------------------------------------
@@ -1179,20 +1102,12 @@ class Context:
         """b2k_silhouette over all ranks' rows (collective when a communicator is initialised): X [n, d] float32 and
         cluster_ids [n] int64 CUDA tensors (n may be 0) -> Spark's silhouette, the same value on every rank.
         distance_measure is "squaredEuclidean" or "cosine"."""
-        t = self._torch
-        n, d = self._check_X(X)
+        Xp, n, d = self._check_X(X)
         if distance_measure not in SILHOUETTE_METRICS:
             raise ValueError(f"distance_measure must be one of {sorted(SILHOUETTE_METRICS)}, got {distance_measure!r}")
-        if not (cluster_ids.is_cuda and cluster_ids.dtype == t.int64 and cluster_ids.dim() == 1 and
-                cluster_ids.is_contiguous() and int(cluster_ids.shape[0]) == n):
-            raise ValueError("cluster_ids must be a contiguous int64 CUDA tensor [n]")
-        if cluster_ids.device.index != self.device_index:
-            raise ValueError("cluster_ids lives on a different device than this context")
+        ip = self._dev(cluster_ids, self._torch.int64, (n,), "cluster_ids")
         out = ctypes.c_double(0.0)
-        with t.cuda.device(self.device):
-            self._check(self._L.b2k_silhouette(self._h, X.data_ptr(), n, d, cluster_ids.data_ptr(),
-                                               SILHOUETTE_METRICS[distance_measure], ctypes.byref(out),
-                                               self._stream()))
+        self._call("b2k_silhouette", Xp, n, d, ip, SILHOUETTE_METRICS[distance_measure], ctypes.byref(out))
         return float(out.value)
 
     def silhouette_multi(self, X: Any, ids_list: Sequence[Any], distance_measure: str = "squaredEuclidean") -> List[float]:
@@ -1200,25 +1115,17 @@ class Context:
         is initialised).  X [n, d] float32 and each of ids_list [n] int64 CUDA tensors -> one value per clustering,
         each with the bits Context.silhouette returns for it; one device pass over X serves the models whose shifts
         agree."""
-        t = self._torch
-        n, d = self._check_X(X)
+        Xp, n, d = self._check_X(X)
         if distance_measure not in SILHOUETTE_METRICS:
             raise ValueError(f"distance_measure must be one of {sorted(SILHOUETTE_METRICS)}, got {distance_measure!r}")
         ids_list = list(ids_list)
         if not ids_list:
             raise ValueError("ids_list must hold at least one cluster-id tensor")
-        for ids in ids_list:
-            if not (ids.is_cuda and ids.dtype == t.int64 and ids.dim() == 1 and ids.is_contiguous() and
-                    int(ids.shape[0]) == n):
-                raise ValueError("every cluster-id tensor must be a contiguous int64 CUDA tensor [n]")
-            if ids.device.index != self.device_index:
-                raise ValueError("cluster ids live on a different device than this context")
         M = len(ids_list)
-        ptrs = (ctypes.c_void_p * M)(*[ids.data_ptr() for ids in ids_list])
+        ptrs = (ctypes.c_void_p * M)(*[self._dev(ids, self._torch.int64, (n,), f"ids_list[{j}]")
+                                       for j, ids in enumerate(ids_list)])
         out = (ctypes.c_double * M)()
-        with t.cuda.device(self.device):
-            self._check(self._L.b2k_silhouette_multi(self._h, X.data_ptr(), n, d, M, ptrs,
-                                                     SILHOUETTE_METRICS[distance_measure], out, self._stream()))
+        self._call("b2k_silhouette_multi", Xp, n, d, M, ptrs, SILHOUETTE_METRICS[distance_measure], out)
         return [float(v) for v in out]
 
     # -- random forests ---------------------------------------------------------------------
@@ -1231,21 +1138,19 @@ class Context:
         tree_offsets int64 [T + 1], feature int32 [N] (-1 for a leaf), threshold float32 [N], children int32 [N, 2],
         gain float64 [N], count int64 [N], value float64 [N, V], and n_values V, level_ms [max_depth + 1] (with option
         time_kernels), level_updates [max_depth + 1]."""
-        n, d = self._check_X(X)
-        self._check_y(y, n)
+        Xp, n, d = self._check_X(X)
+        yp = self._dev(y, self._torch.float32, (n,), "y")
         if impurity not in IMPURITY_CODES:
             raise ValueError(f"impurity must be one of {sorted(IMPURITY_CODES)}, got {impurity!r}")
         prm = RfParams(int(n_trees), int(max_depth), int(max_bins), int(min_instances),
                        int(d if features_per_node is None else features_per_node), int(bool(bootstrap)),
-                       IMPURITY_CODES[impurity], 0, float(min_info_gain), int(seed) & 0xFFFFFFFFFFFFFFFF)
+                       IMPURITY_CODES[impurity], 0, float(min_info_gain), _u64(seed))
         nv, nn = ctypes.c_int(0), ctypes.c_int64(0)
         L = max(int(max_depth), 0) + 1
         lms = np.zeros(L, dtype=np.float64)
         lup = np.zeros(L, dtype=np.int64)
-        with self._torch.cuda.device(self.device):
-            self._check(self._L.b2k_rf_fit(self._h, X.data_ptr(), y.data_ptr(), n, d, ctypes.byref(prm),
-                                           ctypes.byref(nv), ctypes.byref(nn), lms.ctypes.data, lup.ctypes.data,
-                                           self._stream()))
+        self._call("b2k_rf_fit", Xp, yp, n, d, ctypes.byref(prm), ctypes.byref(nv), ctypes.byref(nn), lms.ctypes.data,
+                   lup.ctypes.data)
         V, N, T = int(nv.value), int(nn.value), int(n_trees)
         out = {"tree_offsets": np.zeros(T + 1, dtype=np.int64), "feature": np.zeros(N, dtype=np.int32),
                "threshold": np.zeros(N, dtype=np.float32), "children": np.zeros((N, 2), dtype=np.int32),
@@ -1262,25 +1167,17 @@ class Context:
         [n, V], probability [n, V] and prediction [n] (classification; prediction = the class index), or (None, None,
         prediction [n]) for regression."""
         t = self._torch
-        n, d = self._check_X(X)
-        off = np.ascontiguousarray(forest["tree_offsets"], dtype=np.int64)
-        T = int(off.size) - 1
-        value = np.ascontiguousarray(forest["value"], dtype=np.float64)
-        V = int(value.shape[1])
-        dev = {key: t.as_tensor(np.ascontiguousarray(forest[key], dtype=dt), device=self.device)
-               for key, dt in (("feature", np.int32), ("threshold", np.float32), ("children", np.int32))}
-        offd = t.as_tensor(off, device=self.device)
-        vald = t.as_tensor(value, device=self.device)
-        raw = t.empty((n, V), dtype=t.float64, device=self.device) if classification else None
-        prob = t.empty((n, V), dtype=t.float64, device=self.device) if classification else None
-        pred = t.empty((n,), dtype=t.float64, device=self.device)
-        with t.cuda.device(self.device):
-            self._check(self._L.b2k_rf_predict(self._h, X.data_ptr(), n, d, T, offd.data_ptr(),
-                                               dev["feature"].data_ptr(), dev["threshold"].data_ptr(),
-                                               dev["children"].data_ptr(), vald.data_ptr(), V, int(bool(classification)),
-                                               raw.data_ptr() if raw is not None else None,
-                                               prob.data_ptr() if prob is not None else None, pred.data_ptr(),
-                                               self._stream()))
+        Xp, n, d = self._check_X(X)
+        host = {key: np.ascontiguousarray(forest[key], dtype=dt) for key, dt in
+                (("tree_offsets", np.int64), ("feature", np.int32), ("threshold", np.float32), ("children", np.int32),
+                 ("value", np.float64))}
+        T, V = int(host["tree_offsets"].size) - 1, int(host["value"].shape[1])
+        dev = {key: t.as_tensor(a, device=self.device) for key, a in host.items()}
+        ptrs = [self._dev(x, x.dtype, x.shape, key) for key, x in dev.items()]
+        raw, rp = self._empty((n, V), t.float64) if classification else (None, None)
+        prob, pp = self._empty((n, V), t.float64) if classification else (None, None)
+        pred, dp = self._empty((n,), t.float64)
+        self._call("b2k_rf_predict", Xp, n, d, T, *ptrs, V, int(bool(classification)), rp, pp, dp)
         return raw, prob, pred
 
     # -- evaluation -------------------------------------------------------------------------
@@ -1302,8 +1199,8 @@ class Context:
         class_values [2 or K'].  Returns host arrays: classification {n, label_count [C], tp [M, C], fp [M, C],
         loss [M]} (C = 1 + the largest label or class value), regression {n, reg [M, 3, 5]} (columns label,
         label - prediction, prediction; stats count, mean, m2n, m2, l1)."""
-        n, d = self._check_X(X)
-        self._check_y(y, n)
+        Xp, n, d = self._check_X(X)
+        yp = self._dev(y, self._torch.float32, (n,), "y")
         m = len(models)
         kinds, rows, W, b = self._linear_table(models, d)
         classification = bool(kinds[0] != 0)
@@ -1311,27 +1208,22 @@ class Context:
                                                    for md in models])) if classification else np.zeros(1))
         C = self._eval_classes(y, n, int(cv.max()) + 1 if classification and cv.size else 0) if classification else 0
         out = self._eval_out(m, C, classification)
-        with self._torch.cuda.device(self.device):
-            self._check(self._L.b2k_eval_linear(
-                self._h, X.data_ptr(), y.data_ptr(), n, d, m, kinds.ctypes.data, rows.ctypes.data, W.ctypes.data,
-                b.ctypes.data, cv.ctypes.data, C, float(eps), *self._eval_ptrs(out, classification), self._stream()))
+        self._call("b2k_eval_linear", Xp, yp, n, d, m, kinds.ctypes.data, rows.ctypes.data, W.ctypes.data,
+                   b.ctypes.data, cv.ctypes.data, C, float(eps), *self._eval_ptrs(out, classification))
         return self._eval_result(out, n, C, classification)
 
     def eval_forest(self, X: Any, y: Any, forests: Sequence[Dict[str, Any]], classification: bool,
                     eps: float = 1e-15) -> Dict[str, Any]:
         """b2k_eval_forest: M forests (each laid out as rf_fit's output) scored on (X, y) in one read of X.  Returns
         what eval_linear returns."""
-        n, d = self._check_X(X)
-        self._check_y(y, n)
+        Xp, n, d = self._check_X(X)
+        yp = self._dev(y, self._torch.float32, (n,), "y")
         m = len(forests)
         nt, nv, *arrays = self._forest_table(forests)
         C = self._eval_classes(y, n, int(nv.max())) if classification else 0
         out = self._eval_out(m, C, classification)
-        with self._torch.cuda.device(self.device):
-            self._check(self._L.b2k_eval_forest(
-                self._h, X.data_ptr(), y.data_ptr(), n, d, m, int(bool(classification)), nt.ctypes.data,
-                nv.ctypes.data, *[a.ctypes.data for a in arrays], C, float(eps), *self._eval_ptrs(out, classification),
-                self._stream()))
+        self._call("b2k_eval_forest", Xp, yp, n, d, m, int(bool(classification)), nt.ctypes.data, nv.ctypes.data,
+                   *[a.ctypes.data for a in arrays], C, float(eps), *self._eval_ptrs(out, classification))
         return self._eval_result(out, n, C, classification)
 
     @staticmethod
@@ -1373,52 +1265,47 @@ class Context:
         return (t.empty((int(n_models), int(n)), dtype=t.float64, device=self.device),
                 t.empty((int(n),), dtype=t.uint8, device=self.device))
 
-    def _check_binary_out(self, scores: Any, pos: Any, m: int, row0: int, n: int) -> None:
+    def _binary_out(self, scores: Any, pos: Any, m: Optional[int], row0: int, n: int) -> Tuple[int, int, int]:
+        """The addresses of column row0 of scores [m, N] float64 and of pos[row0] in pos [N] uint8, and N, once rows
+        [row0, row0 + n) are checked to lie inside both."""
         t = self._torch
-        if not (scores.is_cuda and scores.dtype == t.float64 and scores.dim() == 2 and scores.is_contiguous()
-                and scores.shape[0] == m and pos.is_cuda and pos.dtype == t.uint8 and pos.is_contiguous()
-                and pos.shape == (scores.shape[1],) and 0 <= row0 and row0 + n <= scores.shape[1]):
-            raise ValueError(f"scores must be a contiguous float64 CUDA tensor [{m}, N] and pos uint8 [N], N >= "
-                             f"row0 + n = {row0 + n}")
+        sp = self._dev(scores, t.float64, (m, None), "scores")
+        N = int(scores.shape[1])
+        pp = self._dev(pos, t.uint8, (N,), "pos")
+        if not (0 <= row0 and row0 + n <= N):
+            raise ValueError(f"scores and pos must hold rows [{row0}, {row0 + n}), and hold {N}")
+        return sp + 8 * row0, pp + row0, N
 
     def binary_scores_linear(self, X: Any, y: Any, models: Sequence[Dict[str, Any]], scores: Any, pos: Any,
                              row0: int = 0) -> None:
         """b2k_eval_linear_scores: scores[i, row0 + r] = rawPrediction[r][1] of logistic model i (kind "logistic" or
         "softmax", as eval_linear takes them) on (X [n, d], y [n]), pos[row0 + r] = y[r] > 0.5; one read of X."""
-        n, d = self._check_X(X)
-        self._check_y(y, n)
+        Xp, n, d = self._check_X(X)
+        yp = self._dev(y, self._torch.float32, (n,), "y")
         m = len(models)
-        self._check_binary_out(scores, pos, m, row0, n)
+        sp, pp, N = self._binary_out(scores, pos, m, row0, n)
         kinds, rows, W, b = self._linear_table(models, d)
-        with self._torch.cuda.device(self.device):
-            self._check(self._L.b2k_eval_linear_scores(
-                self._h, X.data_ptr(), y.data_ptr(), n, d, m, kinds.ctypes.data, rows.ctypes.data, W.ctypes.data,
-                b.ctypes.data, scores.data_ptr() + 8 * row0, scores.shape[1], pos.data_ptr() + row0, self._stream()))
+        self._call("b2k_eval_linear_scores", Xp, yp, n, d, m, kinds.ctypes.data, rows.ctypes.data, W.ctypes.data,
+                   b.ctypes.data, sp, N, pp)
 
     def binary_scores_forest(self, X: Any, y: Any, forests: Sequence[Dict[str, Any]], scores: Any, pos: Any,
                              row0: int = 0) -> None:
         """b2k_eval_forest_scores: as binary_scores_linear for classification forests (rf_fit's layout, >= 2 values)."""
-        n, d = self._check_X(X)
-        self._check_y(y, n)
+        Xp, n, d = self._check_X(X)
+        yp = self._dev(y, self._torch.float32, (n,), "y")
         m = len(forests)
-        self._check_binary_out(scores, pos, m, row0, n)
+        sp, pp, N = self._binary_out(scores, pos, m, row0, n)
         nt, nv, *arrays = self._forest_table(forests)
-        with self._torch.cuda.device(self.device):
-            self._check(self._L.b2k_eval_forest_scores(
-                self._h, X.data_ptr(), y.data_ptr(), n, d, m, nt.ctypes.data, nv.ctypes.data,
-                *[a.ctypes.data for a in arrays], scores.data_ptr() + 8 * row0, scores.shape[1],
-                pos.data_ptr() + row0, self._stream()))
+        self._call("b2k_eval_forest_scores", Xp, yp, n, d, m, nt.ctypes.data, nv.ctypes.data,
+                   *[a.ctypes.data for a in arrays], sp, N, pp)
 
     def eval_binary(self, scores: Any, pos: Any, num_bins: int, metric: str) -> np.ndarray:
         """b2k_eval_binary: areaUnderROC or areaUnderPR of each row of scores [M, n] with the label bits pos [n]
         (Spark's BinaryClassificationMetrics with numBins, the whole list of distinct scores as one partition)."""
+        sp, pp, N = self._binary_out(scores, pos, None, 0, 0)
         m = int(scores.shape[0])
-        self._check_binary_out(scores, pos, m, 0, 0)
         out = np.zeros(m, dtype=np.float64)
-        with self._torch.cuda.device(self.device):
-            self._check(self._L.b2k_eval_binary(self._h, scores.data_ptr(), pos.data_ptr(), scores.shape[1], m,
-                                                int(num_bins), BINARY_METRICS[metric], out.ctypes.data,
-                                                self._stream()))
+        self._call("b2k_eval_binary", sp, pp, N, m, int(num_bins), BINARY_METRICS[metric], out.ctypes.data)
         return out
 
     def _eval_classes(self, y: Any, n: int, c_models: int) -> int:
@@ -1443,19 +1330,15 @@ class Context:
         init a float32 [n, C] start (params.init must then be 2).  Returns (embedding float32 CUDA tensor [n, C],
         info dict: n, k, nnz, epochs, init_used, ritz_residual, max_weight)."""
         t = self._torch
-        n, d = self._check_X(X)
+        Xp, n, d = self._check_X(X)
         C = int(params.n_components)
-        emb = t.empty((n, max(C, 1)), dtype=t.float32, device=self.device)
-        if init is not None:
-            emb.copy_(t.as_tensor(init, dtype=t.float32, device=self.device).reshape(n, C))
-        if labels is not None and not (labels.is_cuda and labels.dtype == t.int32 and labels.is_contiguous()
-                                       and tuple(labels.shape) == (n,)):
-            raise ValueError(f"labels must be a contiguous int32 CUDA tensor [{n}]")
+        lp = self._dev(labels, t.int32, (n,), "labels", optional=True)
+        start = None if init is None else t.as_tensor(init, dtype=t.float32, device=self.device).reshape(n, C)
+        emb, ep = self._empty((n, max(C, 1)), t.float32)
+        if start is not None:
+            emb.copy_(start)
         info = np.zeros(8, dtype=np.float64)
-        with t.cuda.device(self.device):
-            self._check(self._L.b2k_umap_fit(self._h, X.data_ptr(), n, d,
-                                             labels.data_ptr() if labels is not None else None, ctypes.byref(params),
-                                             emb.data_ptr(), info.ctypes.data, self._stream()))
+        self._call("b2k_umap_fit", Xp, n, d, lp, ctypes.byref(params), ep, info.ctypes.data)
         keys = ("n", "k", "nnz", "epochs", "init_used", "ritz_residual", "n_components", "max_weight")
         out = {key: (float(v) if key in ("ritz_residual", "max_weight") else int(v)) for key, v in zip(keys, info)}
         return emb, out
@@ -1477,16 +1360,12 @@ class Context:
         """b2k_umap_transform: Q [nq, d] against the model (X_train [n, d], embedding [n, C], float32 CUDA tensors) ->
         float32 CUDA tensor [nq, C]; params.n_epochs is the transform's epoch count."""
         t = self._torch
-        n, d = self._check_X(X_train)
-        nq, dq = self._check_X(Q)
+        Xp, n, d = self._check_X(X_train, "X_train")
+        qp, nq, dq = self._check_X(Q, "Q")
         C = int(params.n_components)
         if dq != d:
-            raise ValueError(f"queries have {dq} features, the model {d}")
-        if tuple(embedding.shape) != (n, C) or not embedding.is_contiguous() or embedding.dtype != t.float32:
-            raise ValueError(f"embedding must be a contiguous float32 CUDA tensor [{n}, {C}]")
-        out = t.empty((nq, C), dtype=t.float32, device=self.device)
-        with t.cuda.device(self.device):
-            self._check(self._L.b2k_umap_transform(self._h, X_train.data_ptr(), embedding.data_ptr(), n, d,
-                                                   Q.data_ptr(), nq, ctypes.byref(params), out.data_ptr(),
-                                                   self._stream()))
+            raise ValueError(f"Q has {dq} features, the model {d}")
+        ep = self._dev(embedding, t.float32, (n, C), "embedding")
+        out, op = self._empty((nq, C), t.float32)
+        self._call("b2k_umap_transform", Xp, ep, n, d, qp, nq, ctypes.byref(params), op)
         return out
