@@ -523,7 +523,10 @@ class Context:
     # -- ingest -----------------------------------------------------------------------------
     def ingest_rows(self, dst: Any, row0: int, values: np.ndarray, d: int,
                     offsets: Optional[np.ndarray] = None, n_rows: Optional[int] = None) -> int:
-        """Append a contiguous [n_b, d] host value buffer (Arrow list child buffer) at dst[row0:]."""
+        """Append a contiguous [n_b, d] host value buffer (Arrow list child buffer) at dst[row0:].  Row i is
+        values[offsets[i]:offsets[i + 1]] when offsets are given (a sliced list array starts past 0).  A page-locked
+        `values` is read by the device asynchronously: it must stay unchanged until the current stream has passed
+        this call."""
         code = _DTYPE_CODES.get(values.dtype)
         if code is None:
             raise TypeError(f"unsupported source dtype {values.dtype}")
@@ -532,6 +535,11 @@ class Context:
         dp = self._dev(dst, self._torch.float32, (None, int(d)), "dst")
         if offsets is not None:
             offsets = _host(offsets, np.int32, (None,), "offsets")
+            # the library reads values[offsets[0]:offsets[-1]] and checks only each row's width against d
+            if offsets.shape[0] < 1 or offsets[0] < 0 or offsets[-1] > values.size:
+                ends = offsets[[0, -1]].tolist() if offsets.size else "none"
+                raise ValueError(f"offsets must be n_b + 1 >= 1 positions within the {values.size} values, "
+                                 f"got first and last {ends}")
             n_b = offsets.shape[0] - 1
         else:
             n_b = int(n_rows) if n_rows is not None else values.size // d
@@ -547,7 +555,8 @@ class Context:
         return int(wrote.value)
 
     def ingest_pinned_tensor(self, dst: Any, row0: int, src: Any) -> int:
-        """Append a (pinned) host torch tensor [n_b, d] f32."""
+        """Append a (pinned) host torch tensor [n_b, d] f32.  A pinned `src` is copied to dst by the device
+        asynchronously, with no staging copy: it must stay unchanged until the current stream has passed this call."""
         t = self._torch
         if not (isinstance(src, t.Tensor) and src.device.type == "cpu" and src.dtype == t.float32 and src.dim() == 2
                 and src.is_contiguous()):

@@ -80,6 +80,22 @@ class _CumlCommon:
         return gpu_id
 
 
+def _feature_columns(arrays: Sequence[Any]) -> List[np.ndarray]:
+    """Scalar feature columns as the library ingests them.  Columns that share one of its source dtypes go over as
+    they are, and the device converts them to float32.  Any other set (mixed dtypes, unsigned, boolean) is converted
+    on the host column by column: each column's astype(float32) rounds every value once from that column's own type,
+    exactly as the device would, so the matrix equals ingesting each column alone.  A common type first would not:
+    int64 -> float64 -> float32 rounds twice, and int64 -> int8 or float64 -> int64 truncates."""
+    from ._native import _DTYPE_CODES
+
+    cols = [np.ascontiguousarray(a) for a in arrays]
+    dt = cols[0].dtype
+    if dt in _DTYPE_CODES and all(c.dtype == dt for c in cols):
+        return cols
+    with np.errstate(over="ignore"):   # beyond float32's range is +-inf, as on the device
+        return [np.ascontiguousarray(c, dtype=np.float32) for c in cols]
+
+
 def _features_from_pdf(pdf: pd.DataFrame, multi_col_names: Optional[List[str]], appender: DeviceRowAppender,
                        logger: Any) -> int:
     """One Arrow batch -> rows of the device matrix.  Fast path: the Arrow child buffer, zero-copy.
@@ -88,16 +104,7 @@ def _features_from_pdf(pdf: pd.DataFrame, multi_col_names: Optional[List[str]], 
     if n_b == 0:
         return 0
     if multi_col_names:
-        cols = []
-        for c in multi_col_names:
-            a = pdf[c].to_numpy()
-            if a.dtype == np.float64 or a.dtype == np.float32 or a.dtype.kind == "i":
-                cols.append(np.ascontiguousarray(a))
-            else:
-                cols.append(np.ascontiguousarray(a, dtype=np.float32))
-        dt = cols[0].dtype
-        cols = [c if c.dtype == dt else c.astype(dt) for c in cols]
-        appender.append_columns(cols)
+        appender.append_columns(_feature_columns([pdf[c].to_numpy() for c in multi_col_names]))
         return n_b
     col = pdf[alias.data]
     bufs = arrow_list_column_buffers(col, appender.d)
@@ -133,9 +140,7 @@ def _append_transform_features(app: DeviceRowAppender, df: Union[pd.DataFrame, n
     elif isinstance(df, pd.DataFrame):
         if len(df.columns) != n_cols:
             raise ValueError(f"{len(df.columns)} feature columns do not match the model's {n_cols}")
-        cols = [np.ascontiguousarray(df[c].to_numpy()) for c in df.columns]
-        dt = cols[0].dtype
-        app.append_columns([c if c.dtype == dt else c.astype(dt) for c in cols])
+        app.append_columns(_feature_columns([df[c].to_numpy() for c in df.columns]))
     else:
         arr = np.ascontiguousarray(df, dtype=np.float32)
         if arr.ndim != 2 or arr.shape[1] != n_cols:

@@ -280,6 +280,18 @@ def test_bad_tensor_is_rejected_before_the_library(ctx, method, name, fault):
     assert ctx._invoke.calls == [] and ctx.direct == []
 
 
+@pytest.mark.parametrize("offsets", [[], [-D, 0], [-1, D - 1], [D, 3 * D], [0, D, 2 * D, 3 * D]])
+def test_ingest_rows_keeps_offsets_within_values(ctx, offsets):
+    """The library reads values[offsets[0]:offsets[-1]] and checks only that each row is d wide: offsets that start
+    before the buffer or end past it would make it read host memory outside the buffer."""
+    values = np.zeros(2 * D, np.float32)
+    with pytest.raises(ValueError, match="^offsets"):
+        ctx.ingest_rows(f32(8, D), 0, values, D, offsets=np.array(offsets, np.int32))
+    assert ctx._invoke.calls == []
+    ctx.ingest_rows(f32(8, D), 0, values, D, offsets=np.array([D, 2 * D], np.int32))   # a sliced list: one row
+    assert ctx._invoke.calls == ["b2k_ingest_append"]
+
+
 def test_comm_init_checks_the_unique_id_length(ctx):
     with pytest.raises(ValueError, match="^uid"):
         ctx.comm_init(2, 0, b"x" * (_native.UNIQUE_ID_BYTES - 1))
